@@ -3,6 +3,7 @@
 pairs/sec on 3DMatch-size clouds).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--pairs B] [--config C]
+                    [--dump-outputs DIR]
 
 One "step" = one pass of the hot path (pyramid -> KPConv encoder -> cross-encoder -> regressor ->
 Kabsch) over one batch of B synthetic 3DMatch-shaped pairs per GPU.  Default workload: BASELINE
@@ -11,6 +12,8 @@ config 2 (one ~20k-point pair, batch 1, 1 GPU).  N>1 (torchrun): every rank runs
 
 Prints ONE JSON line on rank 0 (see the keys in `main`).  Timing: CUDA events per step on the
 launching stream, W >= 3 warm-up steps, L2 flushed between timed steps, max over ranks.
+--dump-outputs DIR writes the output dict of the last timed step (rank 0) as DIR/<name>.npy: inputs and
+weights are seeded, so two builds of the project can be compared output for output.
 """
 from __future__ import annotations
 
@@ -31,6 +34,7 @@ import torch  # noqa: E402
 
 WEIGHT_SEED = 2024
 POOL = 8          # distinct synthetic pairs rotated through the steps
+DUMP_BYTES = 64 << 20
 _T0 = time.time()
 
 
@@ -48,7 +52,7 @@ def cpu_threads():
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
-    ap.add_argument('--steps', type=int, default=200)
+    ap.add_argument('--steps', type=int, default=200, help='timed steps (>= 1)')
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
     ap.add_argument('--config', type=int, default=2, help='BASELINE.json config id (2..5)')
@@ -56,11 +60,38 @@ def parse():
     ap.add_argument('--cpu-baseline', type=int, default=1, help='time the CPU port beside the GPU run (N=1 only)')
     ap.add_argument('--checks', type=int, default=1, help='report pose error vs the oracle on one pair')
     ap.add_argument('--attention', default='fp32', choices=['fp32', 'tf32_tc', 'bf16_tc'],
-                    help="fp32: parity kernel (default, pose within 1e-4); bf16_tc: tcgen05 tensor-core core")
+                    help="fp32: parity kernel (default, pose within 1e-4); tf32_tc / bf16_tc: wgmma tensor-core cores")
     ap.add_argument('--inflight', type=int, default=10,
                     help='independent pairs in flight per GPU (CUDA-graph executors on private streams); 1 = serial')
     ap.add_argument('--graph', type=int, default=1, help='1: CUDA-graph executor (GraphedRegTR); 0: eager forward')
-    return ap.parse_args()
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step as DIR/<name>.npy (at most 64 MB)')
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be >= 1')
+    return args
+
+
+def dump_outputs(out, path):
+    """The output dict of one forward as <name>.npy files: tensors under their key, per-pair lists as <key>_<i>;
+    float64 for integer and float64 arrays, float32 otherwise.  An array larger than its share of DUMP_BYTES is
+    replaced by a fixed, seeded sample along its longest axis (the indices go to <name>_sample_idx.npy)."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {}
+    for key in sorted(out.keys()):
+        v = out[key]
+        for name, t in ([(key, v)] if torch.is_tensor(v) else [(f'{key}_{i}', x) for i, x in enumerate(v)]):
+            a = t.detach().cpu().numpy()
+            arrays[name] = a.astype(np.float32 if a.dtype in (np.float32, np.float16, np.bool_) else np.float64)
+    share = DUMP_BYTES // (2 * max(len(arrays), 1))
+    for name, a in arrays.items():
+        if a.nbytes > share:
+            ax = int(np.argmax(a.shape))
+            keep = max(1, share * a.shape[ax] // a.nbytes)
+            idx = np.sort(np.random.default_rng(0).choice(a.shape[ax], size=keep, replace=False))
+            a = np.take(a, idx, axis=ax)
+            np.save(os.path.join(path, f'{name}_sample_idx.npy'), idx.astype(np.float64))
+        np.save(os.path.join(path, f'{name}.npy'), a)
 
 
 def pairs_per_gpu(args):
@@ -220,7 +251,8 @@ def run_reference(args, rank, world):
 
 
 def peak_table():
-    """Roofline denominators: measured (MEASURED_PEAKS.json, driver-written) or the profiling guide's fallback."""
+    """Roofline denominators: measured (MEASURED_PEAKS.json beside this file, when present) or NVIDIA's data sheet
+    for the H100 SXM (700 W; a card with a lower power limit reaches less)."""
     path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     try:
         d = json.load(open(path))
@@ -228,22 +260,8 @@ def peak_table():
                     bf16_tflops_sustained=float(d.get('bf16_tflops_sustained', d['bf16_tflops'])),
                     source='measured (MEASURED_PEAKS.json)')
     except Exception:
-        return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0,
-                    source='fallback (B200_PROFILING.md: 6.65 TB/s, 1.59 PFLOP/s)')
-
-
-def ncu_traffic(kernel_key, pairs):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of a kernel family (for `whole_forward`: per replay),
-    read at run time from the committed ncu summary (profiles/r02_ncu_traffic.json, written by
-    scripts/ncu_summary.py from one `ncu --set full` capture of a graph replay of this workload at the same number of
-    pairs per forward); None when no capture at this batch size is committed.  kpconv_gather: the aggregation kernels
-    only -- the [Nq, 15 Cin] intermediate they write is read back by the contraction GEMM, which the capture lists
-    under gemm_tf32x3."""
-    try:
-        d = json.load(open(os.path.join(ROOT, 'profiles', 'r02_ncu_traffic.json')))
-        return d[str(pairs)][kernel_key]['dram_bytes_per_launch']
-    except Exception:
-        return None
+        return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0,
+                    source='data sheet (H100 SXM: 3.35 TB/s HBM3, 989 TFLOP/s dense BF16)')
 
 
 def measure_stages(model, batch_at, resident, flush, W, B, reps=20):
@@ -322,13 +340,12 @@ def measure_rooflines(model, batch_at, resident, flush, W, K, B, ms_per_step):
                   kernel='KPConv neighbour gather + kernel-point influence + aggregation (one launch per KPConv, each '
                          'timed alone right after an L2 flush); bytes = SURVEY 8d algorithmic bytes of the KPConv op',
                   achieved=ach, peak=pk['hbm_gbs'], unit='GB/s', frac=ach / pk['hbm_gbs'],
-                  traffic=ncu_traffic('kpconv_gather', B), traffic_unit='bytes/launch (committed ncu capture)',
                   peak_source=pk['source'], launches=len(ktr), algorithmic_bytes_per_step=step_bytes,
                   algorithmic_bytes_per_launch=step_bytes / max(len(ktr), 1), ms_per_step=gather_ms,
                   ms_per_step_l2_warm=warm_ms, frac_l2_warm=step_bytes / (warm_ms * 1e-3) / 1e9 / pk['hbm_gbs'],
                   per_launch=per_launch)
 
-    # ---- dense layers: 3xTF32 tcgen05 GEMM (tensor bound); MMA flops = 2*M*N*K*3
+    # ---- dense layers: 3xTF32 wgmma GEMM (tensor bound); MMA flops = 2*M*N*K*3
     g_ms = g_flops = 0.0
     shapes = {}
     for kind, info, fn in tr:
@@ -347,7 +364,7 @@ def measure_rooflines(model, batch_at, resident, flush, W, K, B, ms_per_step):
                 kernel='k_gemm_tf32x3 (+ split-K reduce): every nn.Linear and the KPConv weight contraction; flops = '
                        '2*M*N*K*3 TF32 MMA flops (3xTF32 split) summed over the launches of one forward, each timed alone '
                        'after an L2 flush',
-                achieved=ach, peak=tf32_peak, unit='TFLOP/s', frac=ach / tf32_peak, traffic=ncu_traffic('gemm_tf32x3', B),
+                achieved=ach, peak=tf32_peak, unit='TFLOP/s', frac=ach / tf32_peak,
                 peak_source=pk['source'] + ': bf16_tflops / 2 (dense TF32)', launches=n_gemm, ms_per_step=g_ms,
                 fp32_equiv_flops_per_step=g_flops, fp32_equiv_tflops=g_flops / (g_ms * 1e-3) / 1e12,
                 top_shapes=[dict(M=k[0], N=k[1], K=k[2], launches=c[0], us=round(c[1] * 1e3, 1),
@@ -368,7 +385,7 @@ def measure_rooflines(model, batch_at, resident, flush, W, K, B, ms_per_step):
         att = dict(name='attention_core', bound='tensor',
                    kernel='attention core (softmax(QK^T)V per head, varlen problems): 4*q*k*E flops per problem, x3 '
                           '(3xTF32 split), self and cross launches of the 6 layers',
-                   achieved=ach, peak=tf32_peak, unit='TFLOP/s', frac=ach / tf32_peak, traffic=ncu_traffic('attention_core', B),
+                   achieved=ach, peak=tf32_peak, unit='TFLOP/s', frac=ach / tf32_peak,
                    peak_source=pk['source'] + ': bf16_tflops / 2 (dense TF32)', launches=n_att, ms_per_step=a_ms,
                    fp32_equiv_flops_per_step=a_flops)
 
@@ -380,8 +397,7 @@ def measure_rooflines(model, batch_at, resident, flush, W, K, B, ms_per_step):
                  kernel='whole forward at the benchmarked throughput: fp32-equivalent algorithmic flops of one step '
                         '(dense layers + attention core + KPConv aggregation/influence) / ms_per_step; the fp32-accurate '
                         'path issues 3 TF32 MMA flops per algorithmic flop',
-                 achieved=3.0 * tf, peak=sus, unit='TFLOP/s', frac=3.0 * tf / sus, traffic=ncu_traffic('whole_forward', B),
-                 traffic_unit='DRAM bytes of one forward (all kernels of a graph replay, committed ncu capture)',
+                 achieved=3.0 * tf, peak=sus, unit='TFLOP/s', frac=3.0 * tf / sus,
                  peak_source=pk['source'] + ': bf16_tflops_sustained / 2 (dense TF32, kernel inside a long step)',
                  fp32_equiv_flops_per_step=total_flops, fp32_equiv_tflops=tf,
                  hbm_algorithmic_bytes_per_step=step_bytes,
@@ -440,16 +456,18 @@ def main():
         ids = [(step * B + j) % n_pool for j in range(B)]
         return {'src_xyz': [src[i][0] for i in ids], 'tgt_xyz': [src[i][1] for i in ids]}, ids
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 50 MB L2
 
     def barrier():
         if world > 1:
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}                                   # output dict of the latest device-resident step
+
     def device_step(step):
         batch, _ = batch_at(step, resident)
-        out = runner(batch)
+        out = last['out'] = runner(batch)
         return gather_poses(out['pose'], B * world) if world > 1 else out['pose']
 
     def e2e_step(step):
@@ -493,7 +511,10 @@ def main():
         host_rec['blocked_on_gpu_ms_per_step'] = 1e3 * waited / K            # of which: waiting in event.synchronize
         host_rec['host_work_ms_per_step'] = 1e3 * (t_cpu - waited) / K       # Python + CUDA API calls
         log(f'submit loop {1e3 * t_cpu / K:.3f} ms/step, of which waiting for the GPU {1e3 * waited / K:.3f}')
-        outs += [o['host_pose'].clone() for o in pipe.drain()]
+        drained = pipe.drain()
+        outs += [o['host_pose'].clone() for o in drained]
+        if drained:
+            last['out'] = drained[-1]           # the newest submission: the run's last step
         pipe.join()
         if world > 1:                           # the run's poses, gathered over the ranks (288 B / pair)
             gather_poses(torch.cat(outs, dim=1).to(dev, non_blocking=True), B * K * world)
@@ -522,6 +543,10 @@ def main():
         barrier()
     launches = ops.LAUNCHES - launches0
     log(f'device-resident: {t_dev_ms / K:.3f} ms/step')
+    if rank == 0 and args.dump_outputs:         # before anything else reuses the executors' static buffers
+        dump_outputs(last['out'], args.dump_outputs)
+        torch.cuda.synchronize()
+        log(f'outputs of step {W + K - 1} written to {args.dump_outputs}')
 
     # ---------------- end-to-end: host buffers in, pose on the host out
     h2d = sum(host[j][0].numel() * 4 + host[j][1].numel() * 4 for j in batch_at(W, host)[1])
@@ -590,8 +615,9 @@ def main():
             dtype='f32', data='synthetic',
             config=dict(workload=workload_name(args, B), pairs_per_gpu_per_step=B,
                         parallelism=f'pair-level data parallel x{world}', l2_flush_between_steps=True,
-                        weights='seeded random init (no pretrained weights offline)', precision_mode='fp32 parity (3xTF32 tcgen05 GEMMs, 3xTF32 mma.sync attention + KPConv aggregation)' if args.attention == 'fp32'
-                        else 'fast (3xTF32 GEMMs, bf16 tcgen05 attention core)',
+                        weights='seeded random init (no pretrained weights offline)', precision_mode={'fp32': 'fp32 parity (3xTF32 wgmma GEMMs, 3xTF32 mma.sync attention + KPConv aggregation)',
+                                        'tf32_tc': 'fp32 parity (3xTF32 wgmma GEMMs and attention core)',
+                                        'bf16_tc': 'fast (3xTF32 GEMMs, bf16 wgmma attention core)'}[args.attention],
                         executor=(f'cuda-graph, {depth} pairs in flight (PipelinedRegTR)' if depth > 1 else
                                   'cuda-graph (GraphedRegTR)') if args.graph else 'eager',
                         timed_region='K steps incl. one 256 MB L2-flush kernel per step' if depth > 1 else

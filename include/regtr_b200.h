@@ -1,5 +1,5 @@
 /*
- * regtr_b200 -- C ABI of the B200-native RegTR correspondence-prediction hot path.
+ * regtr_b200 -- C ABI of the H100-native (sm_90a) RegTR correspondence-prediction hot path.
  *
  * The reference (yewzijian/RegTR) has no FFI layer: its boundary for this path is
  * the nn.Module surface (src/models/regtr.py:104-235) over ATen ops plus two
@@ -159,14 +159,13 @@ int regtr_instnorm_apply(const float* x, const int32_t* offs, int n_clouds, int 
  * used to pre-split weight matrices for regtr_gemm_tf32x3. */
 int regtr_split_tf32(const float* x, long long n, float* hi, float* lo, void* stream);
 
-/* fp32-accurate GEMM on the tcgen05 tensor cores (3xTF32):
+/* fp32-accurate GEMM on the Hopper tensor cores (wgmma, 3xTF32):
  *   C[M,N] = act(A[M,K] @ B[N,K]^T + bias[N] + R[M,N]),  B given pre-split as B_hi / B_lo.
  * Replaces nn.Linear (kpconv_blocks.py:546, regtr.py:36/145, transformers.py:95-101,
  * regtr.py:404-411) and the KPConv weight contraction (kpconv_blocks.py:401-406).
  * Row-major fp32; lda/ldb multiples of 4 and 16-byte aligned bases (TMA); bias / R optional;
  * m_dev (optional device int32): actual row count when M is a capacity; relu != 0 applies ReLU.
- * ws: regtr_gemm_ws_bytes(M,N,K) bytes (deterministic split-K planes for skinny long-K shapes;
- * also limits the tensor cores' truncating fp32 accumulation to short K runs). */
+ * ws: regtr_gemm_ws_bytes(M,N,K) bytes (deterministic split-K planes for skinny long-K shapes). */
 size_t regtr_gemm_ws_bytes(int M, int N, int K);
 int regtr_gemm_tf32x3(const float* A, int lda, const float* B_hi, const float* B_lo, int ldb,
                       float* C, int ldc, const float* bias, const float* R, int ldr,
@@ -235,7 +234,7 @@ int regtr_corr_decode_fwd(const float* Qp, const float* Kp, int ld, const float*
                           const int32_t* k_len, int n_problems, int max_q_len, int n_layers, int n_rows,
                           int D, float scale, void* stream);
 
-/* Tensor-core attention core (bf16 operands, fp32 TMEM accumulation, fp32 softmax): the "fast"
+/* Tensor-core attention core (bf16 operands, fp32 register accumulation, fp32 softmax): the "fast"
  * precision mode of the same nn.MultiheadAttention core (transformers.py:197-226), head_dim 32.
  * Inputs are produced by regtr_gemm_tf32x3_qkv_bf16 (the packed in-projection with a bf16
  * epilogue): QK [n_tokens, 2E] bf16 row-major (q | k), Vt [E, ld_vt] bf16 (v transposed, columns
@@ -248,9 +247,9 @@ int regtr_mha_bf16_tc_fwd(const void* QK, int ld_qk, const void* Vt, int ld_vt, 
                           const int32_t* k_len, int n_problems, int max_q_len, int n_heads, int head_dim,
                           float scale, void* stream);
 
-/* fp32-accurate attention core on the tcgen05 tensor cores (the parity mode of the same nn.MultiheadAttention core,
- * transformers.py:197-226): S = Q K^T and O = P V as 3xTF32 tcgen05.mma with TMA-fed operands, P kept in tensor
- * memory, fp32 softmax.  Inputs from regtr_gemm_tf32x3_qkv_split, the packed in-projection (N = 3E: q | k | v) whose
+/* fp32-accurate attention core on the Hopper tensor cores (the parity mode of the same nn.MultiheadAttention core,
+ * transformers.py:197-226): S = Q K^T and O = P V as 3xTF32 wgmma with TMA-fed operands, P kept in registers,
+ * fp32 softmax.  Inputs from regtr_gemm_tf32x3_qkv_split, the packed in-projection (N = 3E: q | k | v) whose
  * epilogue writes every value as its two TF32 halves: qk4 [n_tokens, 4E] fp32 = [Q_hi | Q_lo | K_hi | K_lo] with q
  * pre-multiplied by qscale (pass softmax_scale * log2(e)); vt2 [2E, ld_vt] fp32 = v transposed, hi rows then lo rows
  * (columns >= the real token count must be finite, e.g. zero).  O [n_tokens, E] fp32.  head_dim must be 32.

@@ -1,4 +1,4 @@
-"""regtr_b200 -- B200-native (sm_100a) implementation of the RegTR correspondence-prediction
+"""regtr_b200 -- H100-native (sm_90a) implementation of the RegTR correspondence-prediction
 hot path behind the reference's nn.Module API.  See DESIGN.md / INTEGRATION.md."""
 from .config import Cfg, get_config, load_config  # noqa: F401
 

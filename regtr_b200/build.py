@@ -2,8 +2,7 @@
 
     python -m regtr_b200.build          (or __graft_entry__.build())
 
-nvcc cross-compiles for sm_100a without a GPU.  The .so is git-ignored but travels to the
-GPU box with the repository snapshot.
+nvcc cross-compiles for sm_90a without a GPU.  The .so is a build product and stays out of git.
 """
 from __future__ import annotations
 
@@ -16,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libregtr_b200.so')
 
-NVCC_FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo',
+NVCC_FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 

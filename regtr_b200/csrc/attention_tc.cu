@@ -1,20 +1,18 @@
-// Variable-length multi-head attention core on the tcgen05 tensor cores (bf16 operands, fp32
-// accumulation in TMEM, fp32 softmax) -- the "fast" precision mode of the MHA core of
-// TransformerCrossEncoderLayer.forward_pre (/root/reference/src/models/transformer/
-// transformers.py:197-226).  head_dim = 32.
+// Variable-length multi-head attention core on the Hopper tensor cores (bf16 operands, fp32 accumulation,
+// fp32 softmax) -- the "fast" precision mode of the MHA core of TransformerCrossEncoderLayer.forward_pre
+// (reference src/models/transformer/transformers.py:197-226).  head_dim = 32.
 //
 // Inputs come from the in-projection GEMM's bf16 epilogue (gemm_tc.cu, mode QKV_BF16):
 //   QK  [N_tokens, 2E] bf16 row-major : columns [0,E) = q, [E,2E) = k          (TMA, SWIZZLE_64B)
 //   Vt  [E, ld_vt]     bf16           : v transposed (one row per head-dim channel, tokens
 //                                        contiguous) so that P*V is a K-major x K-major MMA (TMA, SWIZZLE_128B)
-// CTA = (problem, head, tile of 128 queries); 6 warps:
-//   warp 0     TMA producer (Q once; K / Vt tiles of 64 keys, 2 stages)
-//   warp 1     TMEM allocator + MMA issuer: S = Q K^T (M128 x N64 x K32), O += P V (M128 x N32 x K64)
-//   warps 2-5  softmax: thread t owns query row t == TMEM lane t
-// Two passes over the keys -- pass 1: exact row maximum; pass 2: p = exp2((s - max) * scale*log2e),
-// row sums in registers, P written to shared memory as bf16 in the SWIZZLE_128B K-major layout and
-// consumed by the P V MMA -- so the TMEM accumulator never needs an online-softmax rescale.
-// S is double buffered in TMEM so that Q K^T of tile i+1 overlaps the softmax of tile i.
+// CTA = (problem, head, tile of 128 queries); 9 warps:
+//   warp 8     TMA producer (Q once; K / Vt tiles of 64 keys, 2 stages)
+//   warps 0-7  two consumer warpgroups, queries [0, 64) and [64, 128): S = Q K^T (wgmma m64n64k16, both operands
+//              from shared memory), O += P V (m64n32k16, P from registers: the bf16 A fragment of a 16-key step is
+//              exactly the accumulator layout of the two 8-key column blocks it covers)
+// Two passes over the keys -- pass 1: exact row maximum; pass 2: p = exp2((s - max) * scale*log2e), row sums in
+// registers -- so the accumulator never needs an online-softmax rescale.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -25,26 +23,14 @@ namespace {
 constexpr int HD = 32;          // head dim
 constexpr int BQ = 128;         // queries per CTA
 constexpr int BKEY = 64;        // keys per tile
-constexpr int TMEM_COLS = 256;  // S0 [0,64) S1 [64,128) O [128,160)
+constexpr int THREADS = 288;
 
 constexpr int Q_BYTES = BQ * HD * 2;        // 8 KB   (rows of 64 B)
 constexpr int K_BYTES = BKEY * HD * 2;      // 4 KB
 constexpr int V_BYTES = HD * BKEY * 2;      // 4 KB   (32 rows of 128 B)
-constexpr int P_BYTES = BQ * BKEY * 2;      // 16 KB  (128 rows of 128 B)
-constexpr int SMEM_BYTES = Q_BYTES + 2 * K_BYTES + 2 * V_BYTES + 2 * P_BYTES + 1024 + 256;
+constexpr int SMEM_BYTES = Q_BYTES + 2 * K_BYTES + 2 * V_BYTES + 1024 + 256;
 
-// K-major operand tile with 64-byte rows stored by TMA SWIZZLE_64B: 8-row groups are 512 B apart.
-__device__ __forceinline__ uint64_t umma_desc_sw64_kmajor(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(512 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)4 << 61;         // SWIZZLE_64B
-    return d;
-}
-
-__global__ void __launch_bounds__(192, 2)
+__global__ void __launch_bounds__(THREADS, 2)
 k_mha_bf16_tc(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
               const __grid_constant__ CUtensorMap tmVt, float* __restrict__ O, int ldo, int E,
               const int32_t* __restrict__ q_start, const int32_t* __restrict__ q_len,
@@ -72,37 +58,20 @@ k_mha_bf16_tc(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ C
     unsigned char* sQ = base;
     auto sK = [&](int s) { return base + Q_BYTES + s * K_BYTES; };
     auto sV = [&](int s) { return base + Q_BYTES + 2 * K_BYTES + s * V_BYTES; };
-    auto sP = [&](int b) { return base + Q_BYTES + 2 * K_BYTES + 2 * V_BYTES + b * P_BYTES; };
-    uint64_t* bars = reinterpret_cast<uint64_t*>(base + Q_BYTES + 2 * K_BYTES + 2 * V_BYTES + 2 * P_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(base + Q_BYTES + 2 * K_BYTES + 2 * V_BYTES);
     uint64_t* q_full = bars;            // 1
     uint64_t* kv_full = bars + 1;       // [2] TMA landed
-    uint64_t* kv_empty = bars + 3;      // [2] MMAs that read the stage retired (commit)
-    uint64_t* s_full = bars + 5;        // [2] S = QK^T ready in TMEM (commit)
-    uint64_t* s_empty = bars + 7;       // [2] softmax finished reading S (128 arrivals)
-    uint64_t* p_full = bars + 9;        // [2] P tile written to smem (128 arrivals)
-    uint64_t* p_empty = bars + 11;      // [2] PV MMAs that read P retired (commit)
-    uint64_t* o_full = bars + 13;       // 1
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14);
+    uint64_t* kv_empty = bars + 3;      // [2] every consumer warp's MMAs that read the stage retired (8 arrivals)
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tc::mbar_init(q_full, 1);
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(&kv_full[i], 1); tc::mbar_init(&kv_empty[i], 1);
-            tc::mbar_init(&s_full[i], 1); tc::mbar_init(&s_empty[i], 128);
-            tc::mbar_init(&p_full[i], 128); tc::mbar_init(&p_empty[i], 1);
-        }
-        tc::mbar_init(o_full, 1);
+        for (int i = 0; i < 2; ++i) { tc::mbar_init(&kv_full[i], 1); tc::mbar_init(&kv_empty[i], 8); }
         tc::fence_barrier_init();
         tc::tma_prefetch_desc(&tmQ); tc::tma_prefetch_desc(&tmK); tc::tma_prefetch_desc(&tmVt);
     }
-    if (warp == 1) tc::tmem_alloc<TMEM_COLS>(tmem_slot);
-    tc::fence_before_thread_sync();
     __syncthreads();
-    tc::fence_after_thread_sync();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t tmem_O = tmem + 128;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             tc::mbar_arrive_expect_tx(q_full, Q_BYTES);
             tc::tma_load_2d(sQ, &tmQ, q_full, head * HD, q0);
@@ -117,106 +86,96 @@ k_mha_bf16_tc(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ C
                 if (second) tc::tma_load_2d(sV(s), &tmVt, &kv_full[s], ka + kt * BKEY, head * HD);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = tc::umma_idesc(tc::FMT_BF16, BQ, BKEY);
-            constexpr uint32_t idesc_o = tc::umma_idesc(tc::FMT_BF16, BQ, HD);
-            tc::mbar_wait(q_full, 0);
-            const uint64_t dQ = umma_desc_sw64_kmajor(tc::smem_u32(sQ));
-            auto issue_qk = [&](int it) {
-                const int s = it & 1;
-                const uint32_t ph = (it >> 1) & 1;
-                tc::mbar_wait(&kv_full[s], ph);
-                tc::mbar_wait(&s_empty[s], ph ^ 1);
-                tc::fence_after_thread_sync();
-                const uint64_t dK = umma_desc_sw64_kmajor(tc::smem_u32(sK(s)));
+        return;
+    }
+
+    const int wg = warp >> 2;
+    const int g = lane >> 2, t = lane & 3;
+    const int row0 = wg * 64 + (warp & 3) * 16 + g;             // this thread's query rows: row0 and row0 + 8
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    float o[HD / 2];
 #pragma unroll
-                for (int k = 0; k < HD / 16; ++k)              // UMMA_K = 16 bf16 = 32 bytes
-                    tc::umma_f16(tmem + (uint32_t)(s * BKEY), dQ + (uint64_t)(k * 2), dK + (uint64_t)(k * 2), idesc_s, k != 0);
-                tc::umma_commit(&s_full[s]);
-                if (it < n_kt) tc::umma_commit(&kv_empty[s]);   // pass 1: the stage is free once QK^T retired
-            };
-            issue_qk(0);
-            for (int it = 0; it < n_it; ++it) {
-                if (it + 1 < n_it) issue_qk(it + 1);            // overlaps the softmax of tile `it`
-                if (it >= n_kt) {
-                    const int s = it & 1;
-                    const int j = it - n_kt;                    // P buffer index sequence
-                    const int pb = j & 1;
-                    tc::mbar_wait(&p_full[pb], (j >> 1) & 1);
-                    tc::fence_after_thread_sync();
-                    const uint64_t dP = tc::umma_desc_sw128_kmajor(tc::smem_u32(sP(pb)));
-                    const uint64_t dV = tc::umma_desc_sw128_kmajor(tc::smem_u32(sV(s)));
+    for (int j = 0; j < HD / 2; ++j) o[j] = 0.f;
+    tc::mbar_wait(q_full, 0);
+    const uint64_t dQ = tc::gmma_desc_sw64(tc::smem_u32(sQ + wg * 64 * 64));
+    float sc[BKEY / 2];
+    for (int it = 0; it < n_kt; ++it) {                           // pass 1
+        const int s = it & 1;
+        const int jlo = max(0, k0 - (ka + it * BKEY));          // keys [jlo, jhi) of this tile belong to the problem
+        const int jhi = min(BKEY, k0 + kl - (ka + it * BKEY));
+        tc::mbar_wait(&kv_full[s], (it >> 1) & 1);
+        const uint64_t dK = tc::gmma_desc_sw64(tc::smem_u32(sK(s)));
+        tc::wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < BKEY / 16; ++k)
-                        tc::umma_f16(tmem_O, dP + (uint64_t)(k * 2), dV + (uint64_t)(k * 2), idesc_o, (j | k) != 0);
-                    tc::umma_commit(&p_empty[pb]);
-                    tc::umma_commit(&kv_empty[s]);
-                }
-            }
-            tc::umma_commit(o_full);
-        }
-    } else {
-        const int q = warp & 3;                                // TMEM lane quarter of this warp
-        const int row = q * 32 + lane;                         // query row within the tile
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-        float m = -INFINITY, l = 0.f;
-        for (int it = 0; it < n_it; ++it) {
-            const int s = it & 1;
-            const uint32_t ph = (it >> 1) & 1;
-            const int kt = it < n_kt ? it : it - n_kt;
-            const int jlo = max(0, k0 - (ka + kt * BKEY));      // keys [jlo, jhi) of this tile belong to the problem
-            const int jhi = min(BKEY, k0 + kl - (ka + kt * BKEY));
-            tc::mbar_wait(&s_full[s], ph);
-            tc::fence_after_thread_sync();
-            float v[BKEY];
-            tc::tmem_ld_32x32(tmem + lane_addr + (uint32_t)(s * BKEY), v);
-            tc::tmem_ld_32x32(tmem + lane_addr + (uint32_t)(s * BKEY + 32), v + 32);
-            tc::fence_before_thread_sync();
-            tc::mbar_arrive(&s_empty[s]);                       // S buffer may be overwritten
-            if (it < n_kt) {
+        for (int k = 0; k < HD / 16; ++k)                         // k-step = 16 bf16 = 32 bytes
+            tc::wgmma_bf16_ss_n64(sc, dQ + (uint64_t)(2 * k), dK + (uint64_t)(2 * k), k != 0);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&kv_empty[s]);
 #pragma unroll
-                for (int j = 0; j < BKEY; ++j) if (j >= jlo && j < jhi) m = fmaxf(m, v[j]);
-            } else {
-                const int jt = it - n_kt, pb = jt & 1;
-                tc::mbar_wait(&p_empty[pb], ((jt >> 1) & 1) ^ 1);
-                const float mm = m * scale_log2e;
-                uint32_t packed[BKEY / 2];
-#pragma unroll
-                for (int j = 0; j < BKEY; j += 2) {
-                    const float p0 = (j >= jlo && j < jhi) ? exp2f(fmaf(v[j], scale_log2e, -mm)) : 0.f;
-                    const float p1 = (j + 1 >= jlo && j + 1 < jhi) ? exp2f(fmaf(v[j + 1], scale_log2e, -mm)) : 0.f;
-                    const __nv_bfloat162 b = __floats2bfloat162_rn(p0, p1);
-                    // the row sum uses the SAME rounded values the tensor core multiplies with V
-                    l += __low2float(b) + __high2float(b);
-                    packed[j >> 1] = *reinterpret_cast<const uint32_t*>(&b);
-                }
-                // row `row` of the P tile: 128 bytes = 8 chunks of 16 B, chunk c stored at c ^ (row & 7)
-                unsigned char* prow = sP(pb) + (row >> 3) * 1024 + (row & 7) * 128;
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const uint4 val = make_uint4(packed[4 * c], packed[4 * c + 1], packed[4 * c + 2], packed[4 * c + 3]);
-                    *reinterpret_cast<uint4*>(prow + ((c ^ (row & 7)) << 4)) = val;
-                }
-                tc::fence_proxy_async_smem();
-                tc::mbar_arrive(&p_full[pb]);
-            }
-        }
-        tc::mbar_wait(o_full, 0);
-        tc::fence_after_thread_sync();
-        float o[HD];
-        tc::tmem_ld_32x32(tmem_O + lane_addr, o);
-        if (qt * BQ + row < ql) {
-            const float inv = l > 0.f ? 1.f / l : 0.f;
-            float4* dst = reinterpret_cast<float4*>(O + (size_t)(q0 + row) * ldo + head * HD);
-#pragma unroll
-            for (int j = 0; j < HD / 4; ++j)
-                dst[j] = make_float4(o[4 * j] * inv, o[4 * j + 1] * inv, o[4 * j + 2] * inv, o[4 * j + 3] * inv);
+        for (int i = 0; i < BKEY / 2; ++i) {
+            const int j = 8 * (i >> 2) + 2 * t + (i & 1);
+            if (j >= jlo && j < jhi) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], sc[i]);
         }
     }
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc<TMEM_COLS>(tmem);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {                                 // row maximum over the quad that shares the row
+        m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 1));
+        m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 2));
+    }
+    const float mm[2] = {m[0] * scale_log2e, m[1] * scale_log2e};
+    for (int it = n_kt; it < n_it; ++it) {                        // pass 2
+        const int s = it & 1;
+        const int kt = it - n_kt;
+        const int jlo = max(0, k0 - (ka + kt * BKEY));
+        const int jhi = min(BKEY, k0 + kl - (ka + kt * BKEY));
+        tc::mbar_wait(&kv_full[s], (it >> 1) & 1);
+        const uint64_t dK = tc::gmma_desc_sw64(tc::smem_u32(sK(s)));
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < HD / 16; ++k)
+            tc::wgmma_bf16_ss_n64(sc, dQ + (uint64_t)(2 * k), dK + (uint64_t)(2 * k), k != 0);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        uint32_t pa[BKEY / 16][4];                                // A fragments of the four 16-key steps
+#pragma unroll
+        for (int i = 0; i < BKEY / 2; i += 2) {
+            const int j = 8 * (i >> 2) + 2 * t, r = (i >> 1) & 1;
+            const float p0 = (j >= jlo && j < jhi) ? exp2f(fmaf(sc[i], scale_log2e, -mm[r])) : 0.f;
+            const float p1 = (j + 1 >= jlo && j + 1 < jhi) ? exp2f(fmaf(sc[i + 1], scale_log2e, -mm[r])) : 0.f;
+            const __nv_bfloat162 b = __floats2bfloat162_rn(p0, p1);
+            // the row sum uses the SAME rounded values the tensor core multiplies with V
+            l[r] += __low2float(b) + __high2float(b);
+            pa[i >> 3][(i >> 1) & 3] = *reinterpret_cast<const uint32_t*>(&b);
+        }
+        float ot[HD / 2];
+        const uint64_t dV = tc::gmma_desc_sw128(tc::smem_u32(sV(s)));
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BKEY / 16; ++k) tc::wgmma_bf16_n32(ot, pa[k], dV + (uint64_t)(2 * k), k != 0);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&kv_empty[s]);
+#pragma unroll
+        for (int j = 0; j < HD / 2; ++j) o[j] += ot[j];
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+        l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int row = row0 + 8 * r;
+        if (qt * BQ + row >= ql) continue;
+        const float inv = l[r] > 0.f ? 1.f / l[r] : 0.f;
+        float* dst = O + (size_t)(q0 + row) * ldo + head * HD;
+#pragma unroll
+        for (int j = 0; j < HD / 8; ++j)
+            *reinterpret_cast<float2*>(dst + 8 * j + 2 * t) = make_float2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
+    }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -273,7 +232,7 @@ extern "C" int regtr_mha_bf16_tc_fwd(const void* QK, int ld_qk, const void* Vt, 
         attr_set = true;
     }
     dim3 grid(regtr_cdiv(max_q_len, BQ), n_heads, n_problems);
-    k_mha_bf16_tc<<<grid, 192, SMEM_BYTES, st>>>(tQ, tK, tV, O, ldo, E, q_start, q_len, k_start, k_len,
+    k_mha_bf16_tc<<<grid, THREADS, SMEM_BYTES, st>>>(tQ, tK, tV, O, ldo, E, q_start, q_len, k_start, k_len,
                                                  scale * 1.4426950408889634f);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;

@@ -1,27 +1,23 @@
-// fp32-accurate variable-length multi-head attention core on the tcgen05 tensor cores (3xTF32 split, fp32
-// accumulation in TMEM, fp32 softmax): the parity-mode MHA core of TransformerCrossEncoderLayer.forward_pre
-// (/root/reference/src/models/transformer/transformers.py:197-226) with both contractions -- S = Q K^T and
-// O = P V -- fed by TMA and issued as tcgen05.mma.kind::tf32.  head_dim = 32.
+// fp32-accurate variable-length multi-head attention core on the Hopper tensor cores (3xTF32 split, fp32
+// accumulation, fp32 softmax): the parity-mode MHA core of TransformerCrossEncoderLayer.forward_pre
+// (reference src/models/transformer/transformers.py:197-226) with both contractions -- S = Q K^T and
+// O = P V -- fed by TMA and issued as wgmma.m64nNk8 tf32.  head_dim = 32.
 //
 // Inputs come from the in-projection GEMM's split epilogue (gemm_tc.cu, regtr_gemm_tf32x3_qkv_split):
 //   qk4 [N_tokens, 4E] fp32 : [Q_hi | Q_lo | K_hi | K_lo], q pre-scaled by scale * log2(e); x = hi + lo with both
 //                             halves exactly representable in TF32                       (TMA, SWIZZLE_128B)
 //   vt2 [2E, ld_vt]    fp32 : v TRANSPOSED (rows = channels, hi then lo; tokens contiguous), so that P V is a
 //                             K-major x K-major MMA                                       (TMA, SWIZZLE_128B)
-// CTA = (problem, head, tile of 128 queries); 6 warps:
-//   warp 0     TMA producer (Q_hi / Q_lo once; per 64-key tile K_hi [+ K_lo, Vt_hi, Vt_lo in pass 2], 2 stages)
-//   warp 1     TMEM allocator + MMA issuer
-//   warps 2-5  softmax: thread t owns query row t == TMEM lane t
+// CTA = (problem, head, tile of 128 queries); 9 warps:
+//   warp 8     TMA producer (Q_hi / Q_lo once; per 64-key tile K_hi [+ K_lo, Vt_hi, Vt_lo in pass 2], 2 stages)
+//   warps 0-7  two consumer warpgroups, queries [0, 64) and [64, 128) of the tile; S and O live in registers
 // Two passes over the keys:
 //   pass 1  S ~ Q_hi K_hi^T (one TF32 MMA per k-step: the row maximum only stabilises the exponentials, any
 //           value within a few per cent of it serves) -> row maximum m;
 //   pass 2  S = Q_lo K_hi^T + Q_hi K_lo^T + Q_hi K_hi^T (fp32-accurate), p = exp2(s - m), row sums in registers,
-//           p split into (hi, lo) TF32 halves and stored with tcgen05.st into TENSOR MEMORY -- P_hi over the S
-//           columns it came from, P_lo beside them -- where the P V MMAs read it as their A operand
-//           (O += P_lo V_hi + P_hi V_lo + P_hi V_hi).  P never touches shared memory, the accumulator is never
-//           rescaled.
-// S is double buffered in TMEM so that Q K^T of tile i+1 overlaps the softmax of tile i; 224 TMEM columns and
-// 97 KB of shared memory per CTA: two CTAs per SM.
+//           p moved from the accumulator layout into the A-fragment layout with quad shuffles and split into
+//           (hi, lo) TF32 halves there: O_tile = P_lo V_hi + P_hi V_lo + P_hi V_hi, added to the running O with
+//           round-to-nearest fp32 adds.  P never touches shared memory, the accumulator is never rescaled.
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -30,8 +26,7 @@ namespace {
 constexpr int HD = 32;          // head dim (floats: one 128-byte swizzle row)
 constexpr int BQ = 128;         // queries per CTA
 constexpr int BKEY = 64;        // keys per tile
-constexpr int TMEM_COLS = 256;  // S0 / P_hi0 [0,64)  S1 / P_hi1 [64,128)  P_lo [128,192)  O even tiles [192,224)  O odd tiles [224,256)
-constexpr uint32_t COL_PLO = 128, COL_O = 192;
+constexpr int THREADS = 288;
 
 constexpr int Q_BYTES = BQ * HD * 4;        // 16 KB per half (hi / lo)
 constexpr int K_BYTES = BKEY * HD * 4;      // 8 KB per half
@@ -43,7 +38,7 @@ constexpr uint32_t HI_MASK = 0xFFFFE000u;
 __device__ __forceinline__ uint32_t tf32_rn(float x) { return (__float_as_uint(x) + 0x1000u) & HI_MASK; }
 __device__ __forceinline__ float fast_exp2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
-__global__ void __launch_bounds__(192, 2)
+__global__ void __launch_bounds__(THREADS, 1)
 k_mha_tf32_tc(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
               const __grid_constant__ CUtensorMap tmVt, float* __restrict__ O, int ldo, int E,
               const int32_t* __restrict__ q_start, const int32_t* __restrict__ q_len,
@@ -87,32 +82,17 @@ k_mha_tf32_tc(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ C
     uint64_t* bars = reinterpret_cast<uint64_t*>(base + 2 * Q_BYTES + 2 * STAGE_BYTES);
     uint64_t* q_full = bars;            // 1
     uint64_t* kv_full = bars + 1;       // [2] TMA landed
-    uint64_t* kv_empty = bars + 3;      // [2] MMAs that read the stage retired (commit)
-    uint64_t* s_full = bars + 5;        // [2] S = QK^T ready in TMEM (commit)
-    uint64_t* s_empty = bars + 7;       // [2] pass 1: softmax finished reading S (4 warp arrivals)
-    uint64_t* p_full = bars + 9;        // [2] P halves stored to TMEM (4 warp arrivals)
-    uint64_t* pv_done = bars + 11;      // [2] PV MMAs of the tile retired (commit): S/P_hi buffer and P_lo reusable
-    uint64_t* o_full = bars + 13;       // 1
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14);
+    uint64_t* kv_empty = bars + 3;      // [2] every consumer warp's MMAs that read the stage retired (8 arrivals)
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tc::mbar_init(q_full, 1);
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(&kv_full[i], 1); tc::mbar_init(&kv_empty[i], 1);
-            tc::mbar_init(&s_full[i], 1); tc::mbar_init(&s_empty[i], 4);
-            tc::mbar_init(&p_full[i], 4); tc::mbar_init(&pv_done[i], 1);
-        }
-        tc::mbar_init(o_full, 1);
+        for (int i = 0; i < 2; ++i) { tc::mbar_init(&kv_full[i], 1); tc::mbar_init(&kv_empty[i], 8); }
         tc::fence_barrier_init();
         tc::tma_prefetch_desc(&tmQ); tc::tma_prefetch_desc(&tmK); tc::tma_prefetch_desc(&tmVt);
     }
-    if (warp == 1) tc::tmem_alloc<TMEM_COLS>(tmem_slot);
-    tc::fence_before_thread_sync();
     __syncthreads();
-    tc::fence_after_thread_sync();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             tc::mbar_arrive_expect_tx(q_full, 2 * Q_BYTES);
             tc::tma_load_2d(sQhi, &tmQ, q_full, head * HD, q0);
@@ -137,152 +117,121 @@ k_mha_tf32_tc(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ C
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = tc::umma_idesc(tc::FMT_TF32, BQ, BKEY);
-            constexpr uint32_t idesc_o = tc::umma_idesc(tc::FMT_TF32, BQ, HD);
-            tc::mbar_wait(q_full, 0);
-            const uint64_t dQhi = tc::umma_desc_sw128_kmajor(tc::smem_u32(sQhi));
-            const uint64_t dQlo = tc::umma_desc_sw128_kmajor(tc::smem_u32(sQlo));
-            auto issue_qk = [&](int it) {
-                const int s = it & 1;
-                const uint32_t ph = (it >> 1) & 1;
-                tc::mbar_wait(&kv_full[s], ph);
-                // S[s] was last used by iteration it - 2: read by the softmax (pass 1) or, as P_hi, by its PV MMAs (pass 2)
-                if (it >= 2) {
-                    if (it - 2 < n_kt) tc::mbar_wait(&s_empty[s], ((it - 2) >> 1) & 1);
-                    else tc::mbar_wait(&pv_done[s], ((it - 2 - n_kt) >> 1) & 1);
-                }
-                tc::fence_after_thread_sync();
-                const uint64_t dKhi = tc::umma_desc_sw128_kmajor(tc::smem_u32(sKhi(s)));
-                const uint32_t acc = tmem + (uint32_t)(s * BKEY);
-                if (it < n_kt) {
+        return;
+    }
+
+    const int wg = warp >> 2;
+    const int g = lane >> 2, t = lane & 3;
+    const int row0 = wg * 64 + (warp & 3) * 16 + g;             // this thread's query rows: row0 and row0 + 8
+    const int src_a = (lane & ~3) | (t >> 1), src_b = src_a + 2; // quad lanes holding columns t and t + 4
+    const bool odd = t & 1;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    float o[HD / 2];
 #pragma unroll
-                    for (int k = 0; k < HD / 8; ++k)               // UMMA_K = 8 tf32 = 32 bytes
-                        tc::umma_tf32(acc, dQhi + (uint64_t)(2 * k), dKhi + (uint64_t)(2 * k), idesc_s, k != 0);
-                    tc::umma_commit(&s_full[s]);
-                    tc::umma_commit(&kv_empty[s]);              // pass 1: the stage is free once QK^T retired
-                } else {
-                    const uint64_t dKlo = tc::umma_desc_sw128_kmajor(tc::smem_u32(sKlo(s)));
+    for (int j = 0; j < HD / 2; ++j) o[j] = 0.f;
+    tc::mbar_wait(q_full, 0);
+    const uint64_t dQhi = tc::gmma_desc_sw128(tc::smem_u32(sQhi + wg * 64 * 128));
+    const uint64_t dQlo = tc::gmma_desc_sw128(tc::smem_u32(sQlo + wg * 64 * 128));
+    float sc[BKEY / 2];
+    for (int it = 0; it < n_kt; ++it) {                           // pass 1
+        const int s = it & 1;
+        const int jlo = max(0, k0 - (ka + it * BKEY));          // keys [jlo, jhi) of this tile belong to the problem
+        const int jhi = min(BKEY, k0 + kl - (ka + it * BKEY));
+        tc::mbar_wait(&kv_full[s], (it >> 1) & 1);
+        const uint64_t dKhi = tc::gmma_desc_sw128(tc::smem_u32(sKhi(s)));
+        tc::wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < HD / 8; ++k) {
-                        const uint64_t adv = (uint64_t)(2 * k);
-                        tc::umma_tf32(acc, dQlo + adv, dKhi + adv, idesc_s, k != 0);       // small terms first
-                        tc::umma_tf32(acc, dQhi + adv, dKlo + adv, idesc_s, 1);
-                        tc::umma_tf32(acc, dQhi + adv, dKhi + adv, idesc_s, 1);
-                    }
-                    tc::umma_commit(&s_full[s]);
-                }
-            };
-            issue_qk(0);
-            for (int it = 0; it < n_it; ++it) {
-                if (it + 1 < n_it) issue_qk(it + 1);            // overlaps the softmax of tile `it`
-                if (it >= n_kt) {
-                    const int s = it & 1;
-                    const int j = it - n_kt;                    // pass-2 tile index; its S / P_hi buffer is s
-                    tc::mbar_wait(&p_full[s], (j >> 1) & 1);
-                    tc::fence_after_thread_sync();
-                    const uint32_t p_hi = tmem + (uint32_t)(s * BKEY), p_lo = tmem + COL_PLO;
+        for (int k = 0; k < HD / 8; ++k)                          // k-step = 8 tf32 = 32 bytes
+            tc::wgmma_tf32_ss_n64(sc, dQhi + (uint64_t)(2 * k), dKhi + (uint64_t)(2 * k), k != 0);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&kv_empty[s]);
 #pragma unroll
-                    for (int k = 0; k < BKEY / 8; ++k) {
-                        const int h = k >> 2;
-                        const uint64_t adv = (uint64_t)(2 * (k & 3));
-                        const uint64_t dVhi = tc::umma_desc_sw128_kmajor(tc::smem_u32(sVhi(s, h))) + adv;
-                        const uint64_t dVlo = tc::umma_desc_sw128_kmajor(tc::smem_u32(sVlo(s, h))) + adv;
-                        // two output accumulators (even / odd key tiles), added in the epilogue: the tensor core
-                        // truncates when it accumulates, and the bias grows with the length of the chain
-                        const uint32_t o_acc = tmem + COL_O + (uint32_t)(32 * (j & 1));
-                        tc::umma_tf32_ts(o_acc, p_lo + 8 * k, dVhi, idesc_o, ((j >> 1) | k) != 0);
-                        tc::umma_tf32_ts(o_acc, p_hi + 8 * k, dVlo, idesc_o, 1);
-                        tc::umma_tf32_ts(o_acc, p_hi + 8 * k, dVhi, idesc_o, 1);
-                    }
-                    tc::umma_commit(&pv_done[s]);
-                    tc::umma_commit(&kv_empty[s]);
-                }
-            }
-            tc::umma_commit(o_full);
-        }
-    } else {
-        const int q = warp & 3;                                // TMEM lane quarter of this warp
-        const int row = q * 32 + lane;                         // query row within the tile
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-        float m = -INFINITY, l = 0.f;
-        for (int it = 0; it < n_it; ++it) {
-            const int s = it & 1;
-            const uint32_t ph = (it >> 1) & 1;
-            const int kt = it < n_kt ? it : it - n_kt;
-            const int jlo = max(0, k0 - (ka + kt * BKEY));      // keys [jlo, jhi) of this tile belong to the problem
-            const int jhi = min(BKEY, k0 + kl - (ka + kt * BKEY));
-            tc::mbar_wait(&s_full[s], ph);
-            tc::fence_after_thread_sync();
-            float v[BKEY];
-            tc::tmem_ld_32x32(tmem + lane_addr + (uint32_t)(s * BKEY), v);
-            tc::tmem_ld_32x32(tmem + lane_addr + (uint32_t)(s * BKEY + 32), v + 32);
-            if (it < n_kt) {
-                tc::fence_before_thread_sync();
-                __syncwarp();
-                if (lane == 0) tc::mbar_arrive(&s_empty[s]);    // S buffer may be overwritten
-#pragma unroll
-                for (int j = 0; j < BKEY; ++j) if (j >= jlo && j < jhi) m = fmaxf(m, v[j]);
-            } else {
-                const int jt = it - n_kt;
-                const uint32_t dst_hi = tmem + lane_addr + (uint32_t)(s * BKEY), dst_lo = tmem + lane_addr + COL_PLO;
-                // sweep 1: p = exp2(s - m) (kept in v[]), row sum, P_hi over the S columns this thread just read --
-                // no hazard with the PV MMAs of the previous tile, which read the OTHER S / P_hi buffer
-#pragma unroll
-                for (int c = 0; c < BKEY / 16; ++c) {
-                    uint32_t hi[16];
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) {
-                        const int j = 16 * c + e;
-                        const float p = (j >= jlo && j < jhi) ? fast_exp2(v[j] - m) : 0.f;
-                        l += p;
-                        v[j] = p;
-                        hi[e] = tf32_rn(p);
-                    }
-                    tc::tmem_st_32x16(dst_hi + 16 * c, hi);
-                }
-                // P_lo is single buffered: the PV MMAs of the previous pass-2 tile must have retired before it is
-                // overwritten (the exponentials above ran while they executed)
-                if (jt >= 1) tc::mbar_wait(&pv_done[s ^ 1], ((jt - 1) >> 1) & 1);
-                tc::fence_after_thread_sync();
-#pragma unroll
-                for (int c = 0; c < BKEY / 16; ++c) {
-                    uint32_t lo[16];
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) {
-                        const float p = v[16 * c + e];
-                        lo[e] = tf32_rn(p - __uint_as_float(tf32_rn(p)));
-                    }
-                    tc::tmem_st_32x16(dst_lo + 16 * c, lo);
-                }
-                tc::tmem_st_wait();
-                tc::fence_before_thread_sync();
-                __syncwarp();
-                if (lane == 0) tc::mbar_arrive(&p_full[s]);
-            }
-        }
-        tc::mbar_wait(o_full, 0);
-        tc::fence_after_thread_sync();
-        float o[HD];
-        tc::tmem_ld_32x32(tmem + lane_addr + COL_O, o);
-        if (n_kt > 1) {                                          // odd tiles' accumulator (never written otherwise)
-            float o1[HD];
-            tc::tmem_ld_32x32(tmem + lane_addr + COL_O + 32, o1);
-#pragma unroll
-            for (int j = 0; j < HD; ++j) o[j] += o1[j];
-        }
-        if (qt * BQ + row < ql) {
-            const float inv = l > 0.f ? 1.f / l : 0.f;
-            float4* dst = reinterpret_cast<float4*>(O + (size_t)(q0 + row) * ldo + head * HD);
-#pragma unroll
-            for (int j = 0; j < HD / 4; ++j)
-                dst[j] = make_float4(o[4 * j] * inv, o[4 * j + 1] * inv, o[4 * j + 2] * inv, o[4 * j + 3] * inv);
+        for (int i = 0; i < BKEY / 2; ++i) {
+            const int j = 8 * (i >> 2) + 2 * t + (i & 1);
+            if (j >= jlo && j < jhi) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], sc[i]);
         }
     }
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc<TMEM_COLS>(tmem);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {                                 // row maximum over the quad that shares the row
+        m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 1));
+        m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 2));
+    }
+    for (int it = n_kt; it < n_it; ++it) {                        // pass 2
+        const int s = it & 1;
+        const int kt = it - n_kt;
+        const int jlo = max(0, k0 - (ka + kt * BKEY));
+        const int jhi = min(BKEY, k0 + kl - (ka + kt * BKEY));
+        tc::mbar_wait(&kv_full[s], (it >> 1) & 1);
+        const uint64_t dKhi = tc::gmma_desc_sw128(tc::smem_u32(sKhi(s)));
+        const uint64_t dKlo = tc::gmma_desc_sw128(tc::smem_u32(sKlo(s)));
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < HD / 8; ++k) {
+            const uint64_t adv = (uint64_t)(2 * k);
+            tc::wgmma_tf32_ss_n64(sc, dQlo + adv, dKhi + adv, k != 0);      // small terms first
+            tc::wgmma_tf32_ss_n64(sc, dQhi + adv, dKlo + adv, 1);
+            tc::wgmma_tf32_ss_n64(sc, dQhi + adv, dKhi + adv, 1);
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < BKEY / 2; ++i) {
+            const int j = 8 * (i >> 2) + 2 * t + (i & 1);
+            const float p = (j >= jlo && j < jhi) ? fast_exp2(sc[i] - m[(i >> 1) & 1]) : 0.f;
+            l[(i >> 1) & 1] += p;
+            sc[i] = p;
+        }
+        // accumulator layout (row g: columns 8j + 2t, +1) -> A fragments of k-step j (row g: columns t, t + 4)
+        uint32_t phi[BKEY / 8][4], plo[BKEY / 8][4];
+#pragma unroll
+        for (int j = 0; j < BKEY / 8; ++j)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const float e0 = sc[4 * j + 2 * r], e1 = sc[4 * j + 2 * r + 1];
+                const float xa0 = __shfl_sync(0xffffffffu, e0, src_a), xa1 = __shfl_sync(0xffffffffu, e1, src_a);
+                const float xb0 = __shfl_sync(0xffffffffu, e0, src_b), xb1 = __shfl_sync(0xffffffffu, e1, src_b);
+                const float pa = odd ? xa1 : xa0, pb = odd ? xb1 : xb0;
+                phi[j][r] = tf32_rn(pa);
+                plo[j][r] = tf32_rn(pa - __uint_as_float(phi[j][r]));
+                phi[j][2 + r] = tf32_rn(pb);
+                plo[j][2 + r] = tf32_rn(pb - __uint_as_float(phi[j][2 + r]));
+            }
+        float ot[HD / 2];
+        tc::wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < BKEY / 8; ++j) {
+            const int h = j >> 2;
+            const uint64_t adv = (uint64_t)(2 * (j & 3));
+            const uint64_t dVhi = tc::gmma_desc_sw128(tc::smem_u32(sVhi(s, h))) + adv;
+            const uint64_t dVlo = tc::gmma_desc_sw128(tc::smem_u32(sVlo(s, h))) + adv;
+            tc::wgmma_tf32_n32(ot, plo[j], dVhi, j != 0);
+            tc::wgmma_tf32_n32(ot, phi[j], dVlo, 1);
+            tc::wgmma_tf32_n32(ot, phi[j], dVhi, 1);
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&kv_empty[s]);
+#pragma unroll
+        for (int j = 0; j < HD / 2; ++j) o[j] += ot[j];
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+        l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int row = row0 + 8 * r;
+        if (qt * BQ + row >= ql) continue;
+        const float inv = l[r] > 0.f ? 1.f / l[r] : 0.f;
+        float* dst = O + (size_t)(q0 + row) * ldo + head * HD;
+#pragma unroll
+        for (int j = 0; j < HD / 8; ++j)
+            *reinterpret_cast<float2*>(dst + 8 * j + 2 * t) = make_float2(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
+    }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -339,7 +288,7 @@ extern "C" int regtr_mha_tf32_tc_fwd(const float* qk4, int ld4, const float* vt2
         attr_set = true;
     }
     const dim3 grid = tile_base ? dim3(max_tiles, n_heads, 1) : dim3(regtr_cdiv(max_q_len, BQ), n_heads, n_problems);
-    k_mha_tf32_tc<<<grid, 192, SMEM_BYTES, st>>>(tQ, tK, tV, O, ldo, E, q_start, q_len, k_start, k_len, tile_base,
+    k_mha_tf32_tc<<<grid, THREADS, SMEM_BYTES, st>>>(tQ, tK, tV, O, ldo, E, q_start, q_len, k_start, k_len, tile_base,
                                                  n_problems);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;

@@ -1,11 +1,11 @@
-// Shared helpers for the regtr_b200 CUDA kernels (sm_100a only).
+// Shared helpers for the regtr_b200 CUDA kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/regtr_b200.h"
 
-#define REGTR_NUM_SMS 148
+#define REGTR_NUM_SMS 132
 
 #define REGTR_CHECK_LAUNCH()                                         \
     do {                                                             \

@@ -1,4 +1,4 @@
-// fp32-accurate dense GEMM on the 5th-generation tensor cores (tcgen05, 3xTF32 split).
+// fp32-accurate dense GEMM on the Hopper tensor cores (wgmma, 3xTF32 split).
 //
 //   C[M,N] = act( A[M,K] @ B[N,K]^T + bias[N] + R[M,N] )        (all row-major fp32)
 //
@@ -6,16 +6,9 @@
 // blocks kpconv_blocks.py:546-561, feat_proj regtr.py:145, attention in/out projections and FFN
 // transformers.py:197-238, regressor MLP regtr.py:413-443) and the KPConv weight contraction
 // (kpconv_blocks.py:401-406) while keeping the fp32 parity tolerance: a single TF32 pass moves
-// the pose by 4e-3 (measured, DESIGN.md), so every operand is split x = hi + lo with both halves
-// exactly representable in TF32 and the product is accumulated as hi*hi + hi*lo + lo*hi in fp32
-// TMEM accumulators (dropped term lo*lo ~ 2^-22 relative).
-//
-// Structure (one 128 x BN output tile per CTA, 6 warps):
-//   warp 0     TMA producer: A tile (fp32), B_hi tile, B_lo tile per 32-wide k-block (SWIZZLE_128B)
-//   warp 1     TMEM allocator + MMA issuer: 4 k-steps x 3 tcgen05.mma.kind::tf32 per stage, A operand from TMEM
-//   warps 2-5  converters (thread = tile row = TMEM lane): split A into TF32 (hi, lo) in registers and store both
-//              halves to tensor memory with tcgen05.st; then the epilogue: TMEM -> registers -> bias / residual /
-//              ReLU -> global (+ optional InstanceNorm partial sums, + the attention in-projection's split outputs)
+// the pose by 4e-3 (DESIGN.md), so every operand is split x = hi + lo with both halves exactly
+// representable in TF32 and the product is accumulated as hi*hi + hi*lo + lo*hi in fp32
+// (dropped term lo*lo ~ 2^-22 relative).  Kernel structure: see k_gemm_tf32x3_wg.
 // B (weights) is split once on the host side of the ABI (regtr_split_tf32) and cached.
 #include <cuda_bf16.h>
 
@@ -35,7 +28,7 @@ struct QkvOut {
     __nv_bfloat16* vt;
     int ld_vt;
     int split;
-    // fp32 split epilogue for the tcgen05 3xTF32 attention core (attention_tf32_tc.cu): columns [0,E) = q (scaled by
+    // fp32 split epilogue for the 3xTF32 tensor-core attention core (attention_tf32_tc.cu): columns [0,E) = q (scaled by
     // qscale), [E,2E) = k, [2E,3E) = v; every value is written as its two TF32 halves:
     //   qk4 [M, 4E] = [Q_hi | Q_lo | K_hi | K_lo],  vt2 [2E, ld_vtf] = v transposed (hi rows, then lo rows)
     float* qk4;
@@ -125,175 +118,163 @@ __global__ void k_split_tf32(const float* __restrict__ x, long long n, float* __
     lo[i] = tf32_hi(v - h);
 }
 
-// ---- A operand through TENSOR MEMORY ---------------------------------------------------------------------
-// Round 1 split A in shared memory (converter warps read the TMA tile and wrote hi + lo back: 48 KB per k-block;
-// the tensor core then read A_hi twice and A_lo once: another 48 KB), independent of the tile width -- at
-// N = 32/64 that, not the MMA, was the k-block time (measured here: 184 -> 127 us at M = 304000, N = 32, K = 480).
-// Now the converter warps read the TMA tile once (thread = tile row, the TMEM lane it
-// owns), split in registers and store hi | lo with tcgen05.st into a double-buffered 2 x (32 + 32)-column
-// TMEM region; the MMAs take A from TMEM ([a_tmem] operand form) and only B from shared memory.  Shared
-// memory traffic per k-block drops from 96 KB + 3 B to 32 KB + 3 B, and the issuer never waits on a
-// shared-memory round trip.  lo = x - hi is exact in fp32 and is rounded to nearest TF32 as well (the tensor
-// core would otherwise truncate it: a one-sided 2^-21 bias that adds up linearly along K and moved the
-// ill-conditioned random-weight pose by 1e-4).
-template <int BN, int NACC, int ST> struct CfgT {
+// ---- Hopper warpgroup MMA ----------------------------------------------------------------------------------------
+// A CTA walks output tiles blockIdx.x, + gridDim.x, ... (one tile per CTA for launches of up to REGTR_NUM_SMS tiles):
+//   warp 8      TMA producer: A tile (fp32), B_hi tile, B_lo tile per 32-wide k-block (SWIZZLE_128B), STAGES deep;
+//               its stage / phase counters run across tiles, so the next tile's loads fly under the epilogue
+//   warps 0-7   two consumer warpgroups, rows [0, 64) and [64, 128) of the tile: each thread reads its tf32
+//               A fragments from the swizzled stage, splits them into (hi, lo) in registers and issues
+//               wgmma.m64nBNk8 with A from registers and B_hi / B_lo through shared-memory descriptors
+// Every k-block is accumulated by the tensor core into a fresh register block (lo*hi + hi*lo + hi*hi, small terms
+// first) that is then added to the running fp32 sum with round-to-nearest adds: the tensor core's own accumulation
+// truncates, so its chains stay 12 MMAs long whatever K is.  lo = x - hi is exact in fp32 and rounded to nearest
+// TF32 as well (a truncated lo is a one-sided 2^-21 bias that adds up linearly along K).
+// The epilogue stages the tile through shared memory of its own: thread = tile row, 32 columns at a time, as
+// bias / residual / ReLU -> global (+ optional InstanceNorm partial sums, + the attention in-projection's outputs).
+constexpr int CONSUMER_THREADS = 256;
+constexpr int GEMM_THREADS = CONSUMER_THREADS + 32;
+
+template <int BN, int ST> struct CfgT {
     static constexpr int STAGES = ST;
     static constexpr int A_BYTES = BM * BK * 4;          // 16 KB (fp32 tile as loaded by TMA)
     static constexpr int B_BYTES = BN * BK * 4;
     static constexpr int STAGE_BYTES = A_BYTES + 2 * B_BYTES;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-    static constexpr int ACC_COLS = NACC * BN;           // interleaved accumulators (see Cfg)
-    static constexpr int A_COLS = 2 * 2 * BK;            // 2 buffers x (hi | lo) x 32 columns
-    static constexpr int NEED = ACC_COLS + A_COLS;
-    static constexpr int TMEM_COLS = NEED <= 128 ? 128 : (NEED <= 256 ? 256 : 512);
-    static constexpr int MIN_CTAS = (TMEM_COLS <= 256 && SMEM <= 113 * 1024) ? 2 : 1;
+    static constexpr int LDT = BN + 4;                   // epilogue tile pitch (floats): row reads conflict-free
+    static constexpr int TILE_BYTES = BM * LDT * 4;
+    static constexpr int SMEM = STAGES * STAGE_BYTES + TILE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int MIN_CTAS = SMEM <= 113 * 1024 ? 2 : 1;
 };
 
-template <int BN, int NACC, int ST>
-__global__ void __launch_bounds__(192, CfgT<BN, NACC, ST>::MIN_CTAS)
-k_gemm_tf32x3_ts(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_THREADS) : "memory"); }
+
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (BN == 128) tc::wgmma_tf32_n128(d, a, bdesc, accumulate);
+    else if constexpr (BN == 64) tc::wgmma_tf32_n64(d, a, bdesc, accumulate);
+    else tc::wgmma_tf32_n32(d, a, bdesc, accumulate);
+}
+
+template <int BN, int ST>
+__global__ void __launch_bounds__(GEMM_THREADS, CfgT<BN, ST>::MIN_CTAS)
+k_gemm_tf32x3_wg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
                  const __grid_constant__ CUtensorMap tmBlo, float* __restrict__ C, int ldc,
                  const float* __restrict__ bias, const float* __restrict__ R, int ldr, int M, int N, int K,
                  const int32_t* __restrict__ m_dev, int relu, int kb_per_split, size_t split_stride, QkvOut qkv,
                  float2* __restrict__ part) {
-    using P = CfgT<BN, NACC, ST>;
+    using P = CfgT<BN, ST>;
     extern __shared__ unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
     if (m_dev) M = min(M, *m_dev);
-    if (m0 >= M) return;                                   // capacity padding tile (uniform exit)
+    const int tiles_n = (N + BN - 1) / BN;
+    const int n_tiles = ((M + BM - 1) / BM) * tiles_n;       // tiles that hold real rows
+    if ((int)blockIdx.x >= n_tiles) return;                  // capacity padding (uniform exit)
 
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     auto stage_A = [&](int s) { return base + s * P::STAGE_BYTES; };
     auto stage_Bhi = [&](int s) { return base + s * P::STAGE_BYTES + P::A_BYTES; };
     auto stage_Blo = [&](int s) { return base + s * P::STAGE_BYTES + P::A_BYTES + P::B_BYTES; };
-    uint64_t* bars = reinterpret_cast<uint64_t*>(base + P::STAGES * P::STAGE_BYTES);
-    uint64_t* full = bars;                    // TMA bytes landed                      (count 1 + tx)
-    uint64_t* empty = bars + P::STAGES;       // MMAs of the stage retired             (count 1, tcgen05.commit)
-    uint64_t* aready = bars + 2 * P::STAGES;  // A buffer b holds the split tile       (count 4: one per converter warp)
-    uint64_t* afree = aready + 2;             // MMAs reading A buffer b retired       (count 1, tcgen05.commit)
-    uint64_t* tmem_full = afree + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
+    float* ctile = reinterpret_cast<float*>(base + P::STAGES * P::STAGE_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(base + P::STAGES * P::STAGE_BYTES + P::TILE_BYTES);
+    uint64_t* full = bars;                    // TMA bytes landed                        (count 1 + tx)
+    uint64_t* empty = bars + P::STAGES;       // every consumer warp is done with stage  (count 8)
 
     const int nkb_total = (K + BK - 1) / BK;
     const int kb0 = blockIdx.z * kb_per_split;
     const int nkb = min(kb_per_split, nkb_total - kb0);
-    const int n_pre = min(nkb, P::STAGES);                 // k-blocks whose loads start before the set-up barrier
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < P::STAGES; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { tc::mbar_init(&aready[b], 4); tc::mbar_init(&afree[b], 1); }
-        tc::mbar_init(tmem_full, 1);
+    if (warp == 8 && lane == 0) {
+        for (int s = 0; s < P::STAGES; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], CONSUMER_THREADS / 32); }
         tc::fence_barrier_init();
-        // the first loads do not need tensor memory: they fly while warp 1 allocates it
-        for (int kb = 0; kb < n_pre; ++kb) {
-            tc::mbar_arrive_expect_tx(&full[kb], P::A_BYTES + 2 * P::B_BYTES);
-            tc::tma_load_2d(stage_A(kb), &tmA, &full[kb], (kb0 + kb) * BK, m0);
-            tc::tma_load_2d(stage_Bhi(kb), &tmBhi, &full[kb], (kb0 + kb) * BK, n0);
-            tc::tma_load_2d(stage_Blo(kb), &tmBlo, &full[kb], (kb0 + kb) * BK, n0);
-        }
+        tc::tma_prefetch_desc(&tmA); tc::tma_prefetch_desc(&tmBhi); tc::tma_prefetch_desc(&tmBlo);
     }
-    if (warp == 1) tc::tmem_alloc<P::TMEM_COLS>(tmem_slot);
-    tc::fence_before_thread_sync();
     __syncthreads();
-    tc::fence_after_thread_sync();
-    const uint32_t tmem_d = *tmem_slot;
-    const uint32_t tmem_a = tmem_d + (uint32_t)P::ACC_COLS;
     C += (size_t)blockIdx.z * split_stride;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
-            for (int kb = n_pre; kb < nkb; ++kb) {
-                const int s = kb % P::STAGES;
-                const uint32_t ph = (kb / P::STAGES) & 1;
-                tc::mbar_wait(&empty[s], ph ^ 1);
-                tc::mbar_arrive_expect_tx(&full[s], P::A_BYTES + 2 * P::B_BYTES);
-                tc::tma_load_2d(stage_A(s), &tmA, &full[s], (kb0 + kb) * BK, m0);
-                tc::tma_load_2d(stage_Bhi(s), &tmBhi, &full[s], (kb0 + kb) * BK, n0);
-                tc::tma_load_2d(stage_Blo(s), &tmBlo, &full[s], (kb0 + kb) * BK, n0);
+            int it = 0;                                         // k-block counter across tiles
+            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+                const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
+                for (int kb = 0; kb < nkb; ++kb, ++it) {
+                    const int s = it % P::STAGES;
+                    const uint32_t ph = (it / P::STAGES) & 1;
+                    tc::mbar_wait(&empty[s], ph ^ 1);
+                    tc::mbar_arrive_expect_tx(&full[s], P::A_BYTES + 2 * P::B_BYTES);
+                    tc::tma_load_2d(stage_A(s), &tmA, &full[s], (kb0 + kb) * BK, m0);
+                    tc::tma_load_2d(stage_Bhi(s), &tmBhi, &full[s], (kb0 + kb) * BK, n0);
+                    tc::tma_load_2d(stage_Blo(s), &tmBlo, &full[s], (kb0 + kb) * BK, n0);
+                }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = tc::umma_idesc(tc::FMT_TF32, BM, BN);
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % P::STAGES, ab = kb & 1;
-                const uint32_t ph = (kb / P::STAGES) & 1, aph = (kb >> 1) & 1;
-                tc::mbar_wait(&full[s], ph);               // B tiles of the stage (this thread's own acquire)
-                tc::mbar_wait(&aready[ab], aph);           // A split into TMEM buffer ab
-                tc::fence_after_thread_sync();
-                const uint64_t dBhi = tc::umma_desc_sw128_kmajor(tc::smem_u32(stage_Bhi(s)));
-                const uint64_t dBlo = tc::umma_desc_sw128_kmajor(tc::smem_u32(stage_Blo(s)));
-                const uint32_t a_hi = tmem_a + (uint32_t)(ab * 2 * BK), a_lo = a_hi + BK;
+        return;
+    }
+
+    const int g = lane >> 2, t = lane & 3;
+    const int fr = (warp >> 2) * 64 + (warp & 3) * 16 + g;   // this thread's fragment rows: fr and fr + 8
+    const int q = warp & 3;                                  // epilogue: rows 32q .. 32q + 31 (thread = row)
+    const int r = q * 32 + lane;
+    int it = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
+        float acc[BN / 2], blk[BN / 2];
 #pragma unroll
-                for (int k = 0; k < BK / 8; ++k) {             // UMMA_K = 8 tf32
-                    const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                    const uint32_t acc = tmem_d + (uint32_t)((k % NACC) * BN);
-                    const uint32_t first = (kb == 0 && k < NACC) ? 0u : 1u;
-                    tc::umma_tf32_ts(acc, a_lo + 8 * k, dBhi + adv, idesc, first);   // small terms first
-                    tc::umma_tf32_ts(acc, a_hi + 8 * k, dBlo + adv, idesc, 1);
-                    tc::umma_tf32_ts(acc, a_hi + 8 * k, dBhi + adv, idesc, 1);
+        for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+            const int s = it % P::STAGES;
+            tc::mbar_wait(&full[s], (it / P::STAGES) & 1);
+            // SWIZZLE_128B tile: 16-byte chunk c of row x sits at chunk (c ^ (x & 7)) of its 128-byte row
+            const unsigned char* sa = stage_A(s);
+            uint32_t ahi[BK / 8][4], alo[BK / 8][4];
+#pragma unroll
+            for (int k = 0; k < BK / 8; ++k)
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int x = fr + (i & 1) * 8, chunk = 2 * k + (i >> 1);
+                    const float f = *reinterpret_cast<const float*>(sa + x * 128 + ((chunk ^ (x & 7)) << 4) + 4 * t);
+                    const uint32_t h = (__float_as_uint(f) + 0x1000u) & HI_MASK;             // RN (ties away) to TF32
+                    ahi[k][i] = h;
+                    alo[k][i] = (__float_as_uint(f - __uint_as_float(h)) + 0x1000u) & HI_MASK;   // RN: unbiased
                 }
-                tc::umma_commit(&empty[s]);                // smem stage reusable
-                tc::umma_commit(&afree[ab]);               // TMEM A buffer reusable
+            const uint64_t dBhi = tc::gmma_desc_sw128(tc::smem_u32(stage_Bhi(s)));
+            const uint64_t dBlo = tc::gmma_desc_sw128(tc::smem_u32(stage_Blo(s)));
+            tc::wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 8; ++k) {                     // k-step = 8 tf32 = 32 bytes of the swizzled row
+                const uint64_t adv = (uint64_t)(2 * k);
+                wgmma_tf32<BN>(blk, alo[k], dBhi + adv, k != 0);   // small terms first
+                wgmma_tf32<BN>(blk, ahi[k], dBlo + adv, 1);
+                wgmma_tf32<BN>(blk, ahi[k], dBhi + adv, 1);
             }
-            tc::umma_commit(tmem_full);
-        }
-    } else {
-        // ---- converter warps: thread = tile row = TMEM lane 32 * (warp % 4) + lane
-        const int q = warp & 3;
-        const int r = q * 32 + lane;
-        const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-        for (int kb = 0; kb < nkb; ++kb) {
-            const int s = kb % P::STAGES, ab = kb & 1;
-            const uint32_t ph = (kb / P::STAGES) & 1, aph = (kb >> 1) & 1;
-            tc::mbar_wait(&full[s], ph);
-            tc::mbar_wait(&afree[ab], aph ^ 1);            // the MMAs of this buffer's previous use have retired
-            tc::fence_after_thread_sync();
-            // SWIZZLE_128B tile: 16-byte chunk c of row r sits at chunk (c ^ (r & 7)) of its 128-byte row
-            const unsigned char* rowp = stage_A(s) + r * 128;
-            const uint32_t dst = tmem_a + lane_sel + (uint32_t)(ab * 2 * BK);
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                uint32_t hi[16], lo[16];
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    const float4 v = *reinterpret_cast<const float4*>(rowp + (((half * 4 + c) ^ (r & 7)) << 4));
-                    const float f[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const uint32_t h = (__float_as_uint(f[e]) + 0x1000u) & HI_MASK;   // RN (ties away) to TF32
-                        hi[4 * c + e] = h;
-                        lo[4 * c + e] = (__float_as_uint(f[e] - __uint_as_float(h)) + 0x1000u) & HI_MASK;   // RN: unbiased
-                    }
-                }
-                tc::tmem_st_32x16(dst + 16 * half, hi);
-                tc::tmem_st_32x16(dst + BK + 16 * half, lo);
-            }
-            tc::tmem_st_wait();
-            tc::fence_before_thread_sync();
+            tc::wgmma_commit();
+            tc::wgmma_wait<0>();
             __syncwarp();
-            if (lane == 0) tc::mbar_arrive(&aready[ab]);
+            if (lane == 0) tc::mbar_arrive(&empty[s]);            // A read into registers, B read by the MMAs
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) acc[j] += blk[j];
         }
-        // ---- epilogue: this warp owns TMEM lanes 32*(warp%4) .. +31 = output rows
-        tc::mbar_wait(tmem_full, 0);
-        tc::fence_after_thread_sync();
-        const int row = m0 + q * 32 + lane;
+        // ---- epilogue of this tile: fragments -> shared tile -> thread-per-row chunks of 32 columns
+        consumer_sync();                                           // the previous tile's epilogue is done reading
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            *reinterpret_cast<float2*>(ctile + fr * P::LDT + 8 * j + 2 * t) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(ctile + (fr + 8) * P::LDT + 8 * j + 2 * t) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        consumer_sync();
+        const int row = m0 + r;
         const bool row_ok = row < M;
         float* crow = C + (size_t)row * ldc;
         const float* rrow = (R && row_ok) ? R + (size_t)row * ldr : nullptr;
+        const int row_base = m0 + q * 32;
 #pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-            float v[32];
-            tc::tmem_ld_32x32(tmem_d + lane_sel + (uint32_t)c0, v);
-#pragma unroll
-            for (int a = 1; a < NACC; ++a) {
-                float u[32];
-                tc::tmem_ld_32x32(tmem_d + lane_sel + (uint32_t)(a * BN + c0), u);
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] += u[j];
-            }
+        for (int c0 = 32 * (warp >> 2); c0 < BN; c0 += 64) {
             const int col0 = n0 + c0;
             if (col0 >= N) continue;                           // warp-uniform
+            const float* tq = ctile + q * 32 * P::LDT + c0;    // this warp's 32 x 32 block
+            float v[32];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const float4 o = *reinterpret_cast<const float4*>(tq + lane * P::LDT + 4 * j);
+                v[4 * j] = o.x; v[4 * j + 1] = o.y; v[4 * j + 2] = o.z; v[4 * j + 3] = o.w;
+            }
             if (qkv.qk) {                                      // bf16 epilogue (N % 32 == 0 guaranteed by the host)
                 if (!row_ok) continue;
                 if (bias) {
@@ -318,14 +299,7 @@ k_gemm_tf32x3_ts(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 continue;
             }
             if (qkv.qk4) {                                     // fp32 split epilogue (N = 3E, E % 32 == 0)
-                // through shared memory (the pipeline stages are idle now): q / k leave as 128-byte row segments
-                // per 8 lanes, v transposed with lane = token
-                float* tile = reinterpret_cast<float*>(base) + q * (32 * 36);
-#pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    *reinterpret_cast<float4*>(tile + lane * 36 + 4 * j) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                __syncwarp();
-                const int row_base = m0 + q * 32;
+                // q / k leave as 128-byte row segments per 8 lanes, v transposed with lane = token
                 const int sec = col0 / qkv.E, cin = col0 - sec * qkv.E;
                 if (sec < 2) {
                     const int cq = lane & 7, rsub = lane >> 3;
@@ -335,7 +309,7 @@ k_gemm_tf32x3_ts(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
                     for (int it = 0; it < 8; ++it) {
                         const int rr = it * 4 + rsub, rg = row_base + rr;
-                        const float4 o = *reinterpret_cast<const float4*>(tile + rr * 36 + 4 * cq);
+                        const float4 o = *reinterpret_cast<const float4*>(tq + rr * P::LDT + 4 * cq);
                         const float f[4] = {(o.x + b4.x) * sc, (o.y + b4.y) * sc, (o.z + b4.z) * sc, (o.w + b4.w) * sc};
                         float h[4], l[4];
 #pragma unroll
@@ -353,7 +327,7 @@ k_gemm_tf32x3_ts(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     const int rg = row_base + lane;
 #pragma unroll 4
                     for (int j = 0; j < 32; ++j) {
-                        const float f = tile[lane * 36 + j] + (bias ? bias[col0 + j] : 0.f);
+                        const float f = tq[lane * P::LDT + j] + (bias ? bias[col0 + j] : 0.f);
                         const float h = __uint_as_float((__float_as_uint(f) + 0x1000u) & HI_MASK);
                         const float l = __uint_as_float((__float_as_uint(f - h) + 0x1000u) & HI_MASK);
                         if (rg < M) {
@@ -362,25 +336,18 @@ k_gemm_tf32x3_ts(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                         }
                     }
                 }
-                __syncwarp();
                 continue;
             }
             if (col0 + 32 <= N && (ldc & 3) == 0 && (!R || (ldr & 3) == 0)) {
-                // through shared memory (the pipeline stages are idle now): the thread-per-row accumulators leave as
-                // 128-byte row segments, 4 rows per warp instruction -- 4 memory wavefronts instead of 32 per store,
-                // and the residual is read the same way
-                float* tile = reinterpret_cast<float*>(base) + q * (32 * 36);
-#pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    *reinterpret_cast<float4*>(tile + lane * 36 + 4 * j) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                __syncwarp();
-                const int cq = lane & 7, rsub = lane >> 3, row_base = m0 + q * 32;
+                // the block's rows leave as 128-byte row segments, 4 rows per warp instruction -- 4 memory wavefronts
+                // instead of 32 per store, and the residual is read the same way
+                const int cq = lane & 7, rsub = lane >> 3;
                 float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (bias) b4 = *reinterpret_cast<const float4*>(bias + col0 + 4 * cq);
 #pragma unroll
                 for (int it = 0; it < 8; ++it) {
                     const int rr = it * 4 + rsub, rg = row_base + rr;
-                    float4 o = *reinterpret_cast<const float4*>(tile + rr * 36 + 4 * cq);
+                    float4 o = *reinterpret_cast<const float4*>(tq + rr * P::LDT + 4 * cq);
                     if (rg < M) {
                         o.x += b4.x; o.y += b4.y; o.z += b4.z; o.w += b4.w;
                         if (R) {
@@ -391,7 +358,6 @@ k_gemm_tf32x3_ts(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                         *reinterpret_cast<float4*>(C + (size_t)rg * ldc + col0 + 4 * cq) = o;
                     }
                 }
-                __syncwarp();                                  // the tile is rewritten by the next 32-column chunk
             } else {
 #pragma unroll
                 for (int j = 0; j < 32; ++j) {
@@ -415,217 +381,6 @@ k_gemm_tf32x3_ts(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
         }
     }
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc<P::TMEM_COLS>(tmem_d);
-}
-
-// ---- persistent variant (every launch of more than 37 tiles) ------------------------------------------------------
-// One-tile CTAs pay the set-up (barriers, tensor-memory allocation, descriptor fetch) and a full TMA round trip per
-// tile; with K = 32..128 that is most of the ~11 us a tile takes (ncu: converter warps wait on TMA 24 % of samples).
-// Here a CTA walks tiles blockIdx.x, + gridDim.x, ...: the barriers' stage / phase counters run across tiles, the TMA
-// warp loads the next tile while the converter warps run the epilogue of the current one, the MMA warp waits for the
-// accumulator to be drained (tmem_empty) before it starts the next tile.  Plain epilogue (bias / residual / ReLU) and
-// the InstanceNorm partials only; no split-K.  The epilogue stages 16 rows at a time through its own 9 KB of shared
-// memory (the pipeline stages are busy with the next tile).
-template <int BN, int NACC, int ST> struct CfgP : CfgT<BN, NACC, ST> {
-    static constexpr int EPI_BYTES = 4 * 16 * 36 * 4;
-    static constexpr int SMEM = CfgT<BN, NACC, ST>::SMEM + EPI_BYTES;
-};
-
-template <int BN, int NACC, int ST>
-__global__ void __launch_bounds__(192, 2)
-k_gemm_tf32x3_persist(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
-                      const __grid_constant__ CUtensorMap tmBlo, float* __restrict__ C, int ldc,
-                      const float* __restrict__ bias, const float* __restrict__ R, int ldr, int M, int N, int K,
-                      const int32_t* __restrict__ m_dev, int relu, float2* __restrict__ part) {
-    using P = CfgP<BN, NACC, ST>;
-    static_assert(P::TMEM_COLS <= 256 && P::SMEM <= 113 * 1024, "two CTAs per SM");
-    extern __shared__ unsigned char smem_raw[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (m_dev) M = min(M, *m_dev);
-    const int tiles_n = (N + BN - 1) / BN;
-    const int n_tiles = ((M + BM - 1) / BM) * tiles_n;       // tiles that hold real rows
-    if ((int)blockIdx.x >= n_tiles) return;                  // uniform exit
-
-    unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    auto stage_A = [&](int s) { return base + s * P::STAGE_BYTES; };
-    auto stage_Bhi = [&](int s) { return base + s * P::STAGE_BYTES + P::A_BYTES; };
-    auto stage_Blo = [&](int s) { return base + s * P::STAGE_BYTES + P::A_BYTES + P::B_BYTES; };
-    float* epi = reinterpret_cast<float*>(base + P::STAGES * P::STAGE_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(base + P::STAGES * P::STAGE_BYTES + P::EPI_BYTES);
-    uint64_t* full = bars;
-    uint64_t* empty = bars + P::STAGES;
-    uint64_t* aready = bars + 2 * P::STAGES;
-    uint64_t* afree = aready + 2;
-    uint64_t* tmem_full = afree + 2;
-    uint64_t* tmem_empty = tmem_full + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 1);
-
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < P::STAGES; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { tc::mbar_init(&aready[b], 4); tc::mbar_init(&afree[b], 1); }
-        tc::mbar_init(tmem_full, 1);
-        tc::mbar_init(tmem_empty, 4);
-        tc::fence_barrier_init();
-        tc::tma_prefetch_desc(&tmA); tc::tma_prefetch_desc(&tmBhi); tc::tma_prefetch_desc(&tmBlo);
-    }
-    if (warp == 1) tc::tmem_alloc<P::TMEM_COLS>(tmem_slot);
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    tc::fence_after_thread_sync();
-    const uint32_t tmem_d = *tmem_slot;
-    const uint32_t tmem_a = tmem_d + (uint32_t)P::ACC_COLS;
-    const int nkb = (K + BK - 1) / BK;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int it = 0;                                         // k-block counter across tiles
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
-                for (int kb = 0; kb < nkb; ++kb, ++it) {
-                    const int s = it % P::STAGES;
-                    const uint32_t ph = (it / P::STAGES) & 1;
-                    tc::mbar_wait(&empty[s], ph ^ 1);
-                    tc::mbar_arrive_expect_tx(&full[s], P::A_BYTES + 2 * P::B_BYTES);
-                    tc::tma_load_2d(stage_A(s), &tmA, &full[s], kb * BK, m0);
-                    tc::tma_load_2d(stage_Bhi(s), &tmBhi, &full[s], kb * BK, n0);
-                    tc::tma_load_2d(stage_Blo(s), &tmBlo, &full[s], kb * BK, n0);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = tc::umma_idesc(tc::FMT_TF32, BM, BN);
-            int it = 0, tcount = 0;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-                if (tcount > 0) {                               // the epilogue of the previous tile has drained the accumulator
-                    tc::mbar_wait(tmem_empty, (tcount - 1) & 1);
-                    tc::fence_after_thread_sync();
-                }
-                for (int kb = 0; kb < nkb; ++kb, ++it) {
-                    const int s = it % P::STAGES, ab = it & 1;
-                    const uint32_t ph = (it / P::STAGES) & 1, aph = (it >> 1) & 1;
-                    tc::mbar_wait(&full[s], ph);
-                    tc::mbar_wait(&aready[ab], aph);
-                    tc::fence_after_thread_sync();
-                    const uint64_t dBhi = tc::umma_desc_sw128_kmajor(tc::smem_u32(stage_Bhi(s)));
-                    const uint64_t dBlo = tc::umma_desc_sw128_kmajor(tc::smem_u32(stage_Blo(s)));
-                    const uint32_t a_hi = tmem_a + (uint32_t)(ab * 2 * BK), a_lo = a_hi + BK;
-#pragma unroll
-                    for (int k = 0; k < BK / 8; ++k) {
-                        const uint64_t adv = (uint64_t)((k * 32) >> 4);
-                        const uint32_t acc = tmem_d + (uint32_t)((k % NACC) * BN);
-                        const uint32_t first = (kb == 0 && k < NACC) ? 0u : 1u;
-                        tc::umma_tf32_ts(acc, a_lo + 8 * k, dBhi + adv, idesc, first);
-                        tc::umma_tf32_ts(acc, a_hi + 8 * k, dBlo + adv, idesc, 1);
-                        tc::umma_tf32_ts(acc, a_hi + 8 * k, dBhi + adv, idesc, 1);
-                    }
-                    tc::umma_commit(&empty[s]);
-                    tc::umma_commit(&afree[ab]);
-                }
-                tc::umma_commit(tmem_full);
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int r = q * 32 + lane;
-        const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-        float* tile_s = epi + q * (16 * 36);
-        int it = 0, tcount = 0;
-        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-            const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
-            for (int kb = 0; kb < nkb; ++kb, ++it) {
-                const int s = it % P::STAGES, ab = it & 1;
-                const uint32_t ph = (it / P::STAGES) & 1, aph = (it >> 1) & 1;
-                tc::mbar_wait(&full[s], ph);
-                tc::mbar_wait(&afree[ab], aph ^ 1);
-                tc::fence_after_thread_sync();
-                const unsigned char* rowp = stage_A(s) + r * 128;
-                const uint32_t dst = tmem_a + lane_sel + (uint32_t)(ab * 2 * BK);
-#pragma unroll
-                for (int half = 0; half < 2; ++half) {
-                    uint32_t hi[16], lo[16];
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        const float4 v = *reinterpret_cast<const float4*>(rowp + (((half * 4 + c) ^ (r & 7)) << 4));
-                        const float f[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const uint32_t h = (__float_as_uint(f[e]) + 0x1000u) & HI_MASK;
-                            hi[4 * c + e] = h;
-                            lo[4 * c + e] = (__float_as_uint(f[e] - __uint_as_float(h)) + 0x1000u) & HI_MASK;
-                        }
-                    }
-                    tc::tmem_st_32x16(dst + 16 * half, hi);
-                    tc::tmem_st_32x16(dst + BK + 16 * half, lo);
-                }
-                tc::tmem_st_wait();
-                tc::fence_before_thread_sync();
-                __syncwarp();
-                if (lane == 0) tc::mbar_arrive(&aready[ab]);
-            }
-            // ---- epilogue of this tile
-            tc::mbar_wait(tmem_full, tcount & 1);
-            tc::fence_after_thread_sync();
-            const int row_base = m0 + q * 32;
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += 32) {
-                float v[32];
-                tc::tmem_ld_32x32(tmem_d + lane_sel + (uint32_t)c0, v);
-#pragma unroll
-                for (int a = 1; a < NACC; ++a) {
-                    float u[32];
-                    tc::tmem_ld_32x32(tmem_d + lane_sel + (uint32_t)(a * BN + c0), u);
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] += u[j];
-                }
-                const int col0 = n0 + c0;
-                if (col0 >= N) continue;                           // warp-uniform (N % 32 == 0 on this path)
-                const int cq = lane & 7, rsub = lane >> 3;
-                float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (bias) b4 = *reinterpret_cast<const float4*>(bias + col0 + 4 * cq);
-#pragma unroll
-                for (int half = 0; half < 2; ++half) {             // 16 rows at a time through shared memory
-                    if ((lane >> 4) == half) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            *reinterpret_cast<float4*>(tile_s + (lane & 15) * 36 + 4 * j) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    }
-                    __syncwarp();
-#pragma unroll
-                    for (int i4 = 0; i4 < 4; ++i4) {
-                        const int rr = i4 * 4 + rsub, rg = row_base + 16 * half + rr;
-                        float4 o = *reinterpret_cast<const float4*>(tile_s + rr * 36 + 4 * cq);
-                        if (rg < M) {
-                            o.x += b4.x; o.y += b4.y; o.z += b4.z; o.w += b4.w;
-                            if (R) {
-                                const float4 rv = *reinterpret_cast<const float4*>(R + (size_t)rg * ldr + col0 + 4 * cq);
-                                o.x += rv.x; o.y += rv.y; o.z += rv.z; o.w += rv.w;
-                            }
-                            if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                            *reinterpret_cast<float4*>(C + (size_t)rg * ldc + col0 + 4 * cq) = o;
-                        }
-                    }
-                    __syncwarp();
-                }
-                if (part) {
-                    float sq[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) sq[j] = v[j] * v[j];
-                    const float s1 = warp_transpose_sum(v, lane);
-                    const float s2 = warp_transpose_sum(sq, lane);
-                    part[(size_t)((m0 >> 5) + q) * N + col0 + lane] = make_float2(s1, s2);
-                }
-            }
-            tc::fence_before_thread_sync();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(tmem_empty);            // the accumulator may be overwritten
-        }
-    }
-    tc::fence_before_thread_sync();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc<P::TMEM_COLS>(tmem_d);
 }
 
 // C = act(sum_z P[z] + bias + R): deterministic split-K reduction (fixed order), 4 columns / thread
@@ -682,16 +437,14 @@ __global__ void k_gemm_ffma(const float* __restrict__ A, int lda, const float* _
     }
 }
 
-// split count: only for skinny problems (few output tiles) with a long K.  Two reasons to split: fill the machine
-// (ceil(148 / tiles)), and keep the accumulation runs short -- the tensor core adds into its fp32 accumulator with
-// truncation, so a split covers at most 16 k-blocks (K = 512) and the planes are summed with round-to-nearest
-// adds by the reduction kernel (measured on the ill-conditioned random-weight ModelNet pose: 1.2e-4 with 30-60
-// k-block runs, below 1e-4 with <= 16).
+// split count: only for skinny problems (few output tiles) with a long K, to fill the machine
+// (ceil(REGTR_NUM_SMS / tiles) planes, each of at least 8 k-blocks); the planes are summed in a fixed order by the
+// reduction kernel.  At most 16 k-blocks (K = 512) per plane keeps the split's partial sums short as well.
 int choose_splits(int M, int N, int K, int bn) {
     const int tiles = regtr_cdiv(M, BM) * regtr_cdiv(N, bn);
     const int nkb = regtr_cdiv(K, BK);
-    if (tiles >= 74 || nkb < 16 || (N & 3)) return 1;
-    int s = regtr_cdiv(148, tiles);
+    if (tiles >= REGTR_NUM_SMS / 2 || nkb < 16 || (N & 3)) return 1;
+    int s = regtr_cdiv(REGTR_NUM_SMS, tiles);
     if (s > nkb / 8) s = nkb / 8;
     if (s > 8) s = 8;
     const int s_acc = regtr_cdiv(nkb, 16);
@@ -701,10 +454,9 @@ int choose_splits(int M, int N, int K, int bn) {
 }
 
 // Widest tile that covers N: the pipeline keeps several independent pairs in flight, so the machine is
-// filled by OTHER forwards and what counts is the total CTA time (A is streamed / split once per
-// N-tile): measured 632 -> 696 pairs/s against a "fill 148 SMs per launch" heuristic.
+// filled by OTHER forwards and what counts is the total CTA time (A is streamed / split once per N-tile).
 int choose_bn(int M, int N) {
-    (void)M;        // (BN = 64 for M <= 2048 was measured: attention stage 1.00 -> 0.84 ms serial, throughput 1217 -> 1185)
+    (void)M;
     return N > 64 ? 128 : (N > 32 ? 64 : 32);
 }
 
@@ -738,62 +490,44 @@ bool make_map(CUtensorMap* m, const float* ptr, int rows, int cols, int ld, int 
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int BN, int NACC, int ST>
-int launch_gemm_ts(const float* A, int lda, const float* Bhi, const float* Blo, int ldb, float* C, int ldc,
-                   const float* bias, const float* R, int ldr, int M, int N, int K, const int32_t* m_dev, int relu,
-                   int splits, float* ws, cudaStream_t st, QkvOut qkv = NO_QKV, float2* part = nullptr) {
-    using P = CfgT<BN, NACC, ST>;
+template <int BN, int ST>
+int launch_gemm(const float* A, int lda, const float* Bhi, const float* Blo, int ldb, float* C, int ldc,
+                const float* bias, const float* R, int ldr, int M, int N, int K, const int32_t* m_dev, int relu,
+                int splits, float* ws, cudaStream_t st, QkvOut qkv = NO_QKV, float2* part = nullptr) {
+    using P = CfgT<BN, ST>;
     CUtensorMap tA, tBh, tBl;
     if (!make_map(&tA, A, M, K, lda, BM) || !make_map(&tBh, Bhi, N, K, ldb, BN) || !make_map(&tBl, Blo, N, K, ldb, BN))
         return REGTR_ERR_ARG;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(k_gemm_tf32x3_ts<BN, NACC, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::SMEM);
+        cudaError_t e = cudaFuncSetAttribute(k_gemm_tf32x3_wg<BN, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::SMEM);
         if (e != cudaSuccess) return -(1000 + (int)e);
         attr_set = true;
     }
     const int nkb = regtr_cdiv(K, BK);
+    const int tiles = regtr_cdiv(M, BM) * regtr_cdiv(N, BN);
     if (splits <= 1) {
-        dim3 grid(regtr_cdiv(M, BM), regtr_cdiv(N, BN), 1);
-        k_gemm_tf32x3_ts<BN, NACC, ST><<<grid, 192, P::SMEM, st>>>(tA, tBh, tBl, C, ldc, bias, R, ldr, M, N, K, m_dev, relu,
-                                                                   nkb, 0, qkv, part);
+        // Launches of several waves walk their tiles with fewer CTAs: ~4 tiles per CTA, between half and twice the SM
+        // count, so that one set-up serves several tiles and the other forwards' kernels still find free SMs.
+        int grid = tiles;
+        if (tiles > REGTR_NUM_SMS / 4) {
+            grid = tiles / 4;
+            grid = grid < REGTR_NUM_SMS / 2 ? REGTR_NUM_SMS / 2 : (grid > 2 * REGTR_NUM_SMS ? 2 * REGTR_NUM_SMS : grid);
+            if (grid > tiles) grid = tiles;
+        }
+        k_gemm_tf32x3_wg<BN, ST><<<grid, GEMM_THREADS, P::SMEM, st>>>(tA, tBh, tBl, C, ldc, bias, R, ldr, M, N, K, m_dev,
+                                                                      relu, nkb, 0, qkv, part);
         REGTR_CHECK_LAUNCH();
         return REGTR_OK;
     }
     const int per = regtr_cdiv(nkb, splits);
     const int z = regtr_cdiv(nkb, per);                     // every plane gets >= 1 k-block
     const size_t stride = (size_t)M * N;
-    dim3 grid(regtr_cdiv(M, BM), regtr_cdiv(N, BN), z);
-    k_gemm_tf32x3_ts<BN, NACC, ST><<<grid, 192, P::SMEM, st>>>(tA, tBh, tBl, ws, N, nullptr, nullptr, 0, M, N, K, m_dev, 0,
-                                                               per, stride, NO_QKV, nullptr);
+    k_gemm_tf32x3_wg<BN, ST><<<dim3(tiles, 1, z), GEMM_THREADS, P::SMEM, st>>>(tA, tBh, tBl, ws, N, nullptr, nullptr, 0, M, N,
+                                                                               K, m_dev, 0, per, stride, NO_QKV, nullptr);
     REGTR_CHECK_LAUNCH();
     k_splitk_reduce<<<regtr_cdiv((long long)M * (N / 4), 256), 256, 0, st>>>(ws, z, stride, C, ldc, bias, R, ldr, M, N,
                                                                             m_dev, relu);
-    REGTR_CHECK_LAUNCH();
-    return REGTR_OK;
-}
-
-template <int BN, int NACC, int ST>
-int launch_gemm_persist(const float* A, int lda, const float* Bhi, const float* Blo, int ldb, float* C, int ldc,
-                        const float* bias, const float* R, int ldr, int M, int N, int K, const int32_t* m_dev, int relu,
-                        cudaStream_t st, float2* part) {
-    using P = CfgP<BN, NACC, ST>;
-    CUtensorMap tA, tBh, tBl;
-    if (!make_map(&tA, A, M, K, lda, BM) || !make_map(&tBh, Bhi, N, K, ldb, BN) || !make_map(&tBl, Blo, N, K, ldb, BN))
-        return REGTR_ERR_ARG;
-    static bool attr_set = false;
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(k_gemm_tf32x3_persist<BN, NACC, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::SMEM);
-        if (e != cudaSuccess) return -(1000 + (int)e);
-        attr_set = true;
-    }
-    const int tiles = regtr_cdiv(M, BM) * regtr_cdiv(N, BN);
-    // At least ~4 tiles per CTA, between 74 CTAs (half the SMs: small launches amortise their set-up and leave room for
-    // the other forwards' kernels -- swept 6..296: 1 pair/step 1226 -> 1281 pairs/s, 8 pairs/step 1617 -> 1650) and 296.
-    int grid = tiles / 4;
-    grid = grid < REGTR_NUM_SMS / 2 ? REGTR_NUM_SMS / 2 : (grid > 2 * REGTR_NUM_SMS ? 2 * REGTR_NUM_SMS : grid);
-    if (grid > tiles) grid = tiles;
-    k_gemm_tf32x3_persist<BN, NACC, ST><<<grid, 192, P::SMEM, st>>>(tA, tBh, tBl, C, ldc, bias, R, ldr, M, N, K, m_dev, relu, part);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
 }
@@ -827,9 +561,6 @@ static int gemm_dispatch(const float* A, int lda, const float* B_hi, const float
     // TMA: 16-byte aligned bases and row pitches
     if ((lda & 3) || (ldb & 3) || ((uintptr_t)A & 15) || ((uintptr_t)B_hi & 15) || ((uintptr_t)B_lo & 15))
         return REGTR_ERR_UNSUPPORTED;
-    // Tile width: the widest BN that still yields >= ~1 wave of CTAs (148 SMs); short-K problems
-    // take 2 pipeline stages so that two CTAs fit one SM (their fixed prologue/epilogue overlap);
-    // skinny long-K problems are split along K (deterministic two-pass reduction).
     {
         const char* impl = getenv("REGTR_GEMM_IMPL");
         if (impl && impl[0] == 'f') {
@@ -844,33 +575,11 @@ static int gemm_dispatch(const float* A, int lda, const float* B_hi, const float
     int splits = choose_splits(M, N, K, bn);
     if (used_splits) *used_splits = splits;
     if (splits > 1 && (!ws || ws_bytes < regtr_gemm_ws_bytes(M, N, K))) return REGTR_ERR_WORKSPACE;
-    // accumulation runs per TMEM accumulator: k-blocks per split / NACC (the tensor core adds with truncation)
-    const int nkb_split = regtr_cdiv(regtr_cdiv(K, BK), splits);
-    // several waves of short tiles: the persistent kernel (one set-up per CTA, loads of the next tile under the epilogue)
-    {
-        static const int persist_on = [] { const char* e = getenv("REGTR_GEMM_PERSIST"); return e ? atoi(e) : 1; }();
-        const int tiles = regtr_cdiv(M, BM) * regtr_cdiv(N, bn);
-        if (persist_on && splits == 1 && tiles > REGTR_NUM_SMS / 4 && (bn != 128 || nkb_split <= 16) && (N & 31) == 0 && (ldc & 3) == 0 &&
-            (!R || (ldr & 3) == 0)) {
-            if (bn == 128) return launch_gemm_persist<128, 1, 2>(A, lda, B_hi, B_lo, ldb, C, ldc, bias, R, ldr, M, N, K, m_dev, relu, st, part);
-            if (bn == 64) return launch_gemm_persist<64, 2, 3>(A, lda, B_hi, B_lo, ldb, C, ldc, bias, R, ldr, M, N, K, m_dev, relu, st, part);
-            return launch_gemm_persist<32, 4, 4>(A, lda, B_hi, B_lo, ldb, C, ldc, bias, R, ldr, M, N, K, m_dev, relu, st, part);
-        }
-    }
-#define REGTR_TS_CASE(BN_, NACC_, ST_)                                                                                 \
-    return launch_gemm_ts<BN_, NACC_, ST_>(A, lda, B_hi, B_lo, ldb, C, ldc, bias, R, ldr, M, N, K, m_dev, relu, splits, \
-                                           (float*)ws, st, NO_QKV, splits > 1 ? nullptr : part)
-    // 2 co-resident CTAs per SM (2-4 stages of <= 48 KB, <= 256 TMEM columns) overlap one CTA's load latency and
-    // epilogue with the other's MMAs -- also across the independent forwards of the multi-stream executor; only long
-    // accumulation runs take the 4-stage variant with two interleaved accumulators.  (Deeper single-CTA-per-SM
-    // variants with 3-4 accumulators were measured: 2x more accurate at K = 960, but 1.3-2x slower per launch.)
-    // (4- and 6-stage single-CTA-per-SM variants for launches of <= 148 CTAs were measured too: the serial forward gets
-    // 4 % shorter, the multi-stream throughput 3 % lower -- a CTA that owns the SM's shared memory keeps the other
-    // forwards' CTAs out.)
-    if (bn == 128) { if (nkb_split <= 16) REGTR_TS_CASE(128, 1, 2); REGTR_TS_CASE(128, 2, 4); }
-    if (bn == 64) REGTR_TS_CASE(64, 2, 3);
-    REGTR_TS_CASE(32, 4, 4);
-#undef REGTR_TS_CASE
+    float2* p = splits > 1 ? nullptr : part;
+    // Stages: as deep as keeps the epilogue tile beside them; the 32-wide tile takes 3 so that two CTAs share an SM.
+    if (bn == 128) return launch_gemm<128, 3>(A, lda, B_hi, B_lo, ldb, C, ldc, bias, R, ldr, M, N, K, m_dev, relu, splits, (float*)ws, st, NO_QKV, p);
+    if (bn == 64) return launch_gemm<64, 4>(A, lda, B_hi, B_lo, ldb, C, ldc, bias, R, ldr, M, N, K, m_dev, relu, splits, (float*)ws, st, NO_QKV, p);
+    return launch_gemm<32, 3>(A, lda, B_hi, B_lo, ldb, C, ldc, bias, R, ldr, M, N, K, m_dev, relu, splits, (float*)ws, st, NO_QKV, p);
 }
 
 int regtr_gemm_tf32x3(const float* A, int lda, const float* B_hi, const float* B_lo, int ldb, float* C, int ldc,
@@ -916,13 +625,9 @@ int regtr_gemm_tf32x3_qkv_bf16(const float* A, int lda, const float* B_hi, const
     q.qk = (__nv_bfloat16*)qk_out; q.ld_qk = ld_qk; q.vt = (__nv_bfloat16*)vt_out; q.ld_vt = ld_vt; q.split = split;
     float* dummy = reinterpret_cast<float*>(qk_out);      // C is never written in this mode
     const int bn = choose_bn(M, N);
-#define REGTR_TSQ_CASE(BN_, NACC_, ST_)                                                                                 \
-    return launch_gemm_ts<BN_, NACC_, ST_>(A, lda, B_hi, B_lo, ldb, dummy, 0, bias, nullptr, 0, M, N, K, m_dev, 0, 1, \
-                                           nullptr, st, q)
-    if (bn == 128) { if (K <= 512) REGTR_TSQ_CASE(128, 1, 2); REGTR_TSQ_CASE(128, 2, 4); }
-    if (bn == 64) REGTR_TSQ_CASE(64, 2, 3);
-    REGTR_TSQ_CASE(32, 4, 4);
-#undef REGTR_TSQ_CASE
+    if (bn == 128) return launch_gemm<128, 3>(A, lda, B_hi, B_lo, ldb, dummy, 0, bias, nullptr, 0, M, N, K, m_dev, 0, 1, nullptr, st, q);
+    if (bn == 64) return launch_gemm<64, 4>(A, lda, B_hi, B_lo, ldb, dummy, 0, bias, nullptr, 0, M, N, K, m_dev, 0, 1, nullptr, st, q);
+    return launch_gemm<32, 3>(A, lda, B_hi, B_lo, ldb, dummy, 0, bias, nullptr, 0, M, N, K, m_dev, 0, 1, nullptr, st, q);
 }
 
 // In-projection of the attention block with the fp32 split epilogue consumed by regtr_mha_tf32_tc_fwd (see QkvOut).
@@ -938,9 +643,7 @@ int regtr_gemm_tf32x3_qkv_split(const float* A, int lda, const float* B_hi, cons
         return REGTR_ERR_UNSUPPORTED;
     QkvOut q = NO_QKV;
     q.qk4 = qk4; q.ld4 = ld4; q.vt2 = vt2; q.ld_vtf = ld_vt; q.E = E; q.qscale = qscale;
-    if (regtr_cdiv(K, BK) > 16)
-        return launch_gemm_ts<128, 2, 4>(A, lda, B_hi, B_lo, ldb, qk4, 0, bias, nullptr, 0, M, N, K, m_dev, 0, 1, nullptr, st, q);
-    return launch_gemm_ts<128, 1, 2>(A, lda, B_hi, B_lo, ldb, qk4, 0, bias, nullptr, 0, M, N, K, m_dev, 0, 1, nullptr, st, q);
+    return launch_gemm<128, 3>(A, lda, B_hi, B_lo, ldb, qk4, 0, bias, nullptr, 0, M, N, K, m_dev, 0, 1, nullptr, st, q);
 }
 
 }  // extern "C"

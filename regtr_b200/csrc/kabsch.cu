@@ -213,7 +213,7 @@ int regtr_status_clear(uint32_t* status, void* stream_) {
 int regtr_version(void) { return 1; }
 
 const char* regtr_build_info(void) {
-    return "regtr_b200 ABI 1; nvcc " __DATE__ "; -gencode arch=compute_100a,code=sm_100a -lineinfo";
+    return "regtr_b200 ABI 1; nvcc " __DATE__ "; -gencode arch=compute_90a,code=sm_90a -lineinfo";
 }
 
 }  // extern "C"

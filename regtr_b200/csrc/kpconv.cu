@@ -33,11 +33,11 @@ __global__ void k_row_flags(const float* __restrict__ x, int n, int C, uint8_t* 
 // defined (zero) contents only inside the tile that straddles n; the rest of the capacity is left untouched.
 __device__ __forceinline__ int pad_band_end(int n) { return (n + 127) & ~127; }
 
-// ---- packed fp32x2 FMA (sm_100: one instruction, two FMAs)
-typedef unsigned long long f2;
-__device__ __forceinline__ f2 f2_dup(float x) { f2 r; asm("mov.b64 %0, {%1, %1};" : "=l"(r) : "f"(x)); return r; }
-__device__ __forceinline__ f2 f2_fma(f2 a, f2 b, f2 c) { f2 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ void f2_unpack(f2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
+// ---- fp32 pairs: kernel points (2j, 2j+1) side by side, one round-to-nearest FMA each
+typedef float2 f2;
+__device__ __forceinline__ f2 f2_dup(float x) { return make_float2(x, x); }
+__device__ __forceinline__ f2 f2_fma(f2 a, f2 b, f2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ void f2_unpack(f2 v, float& lo, float& hi) { lo = v.x; hi = v.y; }
 
 // Phase 1 (lanes own neighbours): compact the valid (non-shadow) neighbours of one query into
 // shared memory as (relative position, id) and count those whose feature row sums to > 0.
@@ -128,7 +128,7 @@ k_kpconv_agg(const float* __restrict__ q, const float* __restrict__ s, const int
 #pragma unroll
     for (int j = 0; j < 8; ++j)
 #pragma unroll
-        for (int v = 0; v < VEC; ++v) acc[j][v] = 0ull;
+        for (int v = 0; v < VEC; ++v) acc[j][v] = make_float2(0.f, 0.f);
 
     const int n_pad = (n_valid + 3) & ~3;          // UNROLL divides 4; padded slots carry zero influences
     for (int k0 = 0; k0 < n_pad; k0 += UNROLL) {
@@ -151,9 +151,10 @@ k_kpconv_agg(const float* __restrict__ q, const float* __restrict__ s, const int
         }
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
-            const ulonglong2* wr = reinterpret_cast<const ulonglong2*>(w_s + (k0 + u) * KPP);
-            const ulonglong2 a = wr[0], b = wr[1], c = wr[2], d = wr[3];
-            const f2 w2[8] = {a.x, a.y, b.x, b.y, c.x, c.y, d.x, d.y};
+            const float4* wr = reinterpret_cast<const float4*>(w_s + (k0 + u) * KPP);
+            const float4 a = wr[0], b = wr[1], c = wr[2], d = wr[3];
+            const f2 w2[8] = {make_float2(a.x, a.y), make_float2(a.z, a.w), make_float2(b.x, b.y), make_float2(b.z, b.w),
+                              make_float2(c.x, c.y), make_float2(c.z, c.w), make_float2(d.x, d.y), make_float2(d.z, d.w)};
 #pragma unroll
             for (int v = 0; v < VEC; ++v) {
                 const f2 xx = f2_dup(xv[u][v]);
@@ -908,7 +909,7 @@ int regtr_kpconv_fwd(const float* q, const float* s, const int32_t* idx, const f
         REGTR_CHECK_LAUNCH();
         return REGTR_OK;
     }
-    // out[Nq,Cout] = wf[Nq,15*Cin] @ W[15*Cin,Cout] on the library's own 3xTF32 tcgen05 GEMM: split + transpose
+    // out[Nq,Cout] = wf[Nq,15*Cin] @ W[15*Cin,Cout] on the library's own 3xTF32 wgmma GEMM: split + transpose
     // W into the workspace tail, then regtr_gemm_tf32x3 (the Python front end caches the split instead)
     const int KD = KP * Cin;
     if (KD % 4) return REGTR_ERR_UNSUPPORTED;

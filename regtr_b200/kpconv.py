@@ -1,4 +1,4 @@
-"""KPConv backbone on the B200 kernels: pyramid pre-processor, KPConv op, blocks, encoder.
+"""KPConv backbone on the H100 kernels: pyramid pre-processor, KPConv op, blocks, encoder.
 
 Host-side mirror of the reference modules (same class names, constructor arguments,
 forward signatures and state_dict keys) for the parts of

@@ -1,7 +1,7 @@
 """Torch-tensor front end of the C ABI (one function per entry point of include/regtr_b200.h).
 
 PyTorch is used for device memory and streams only; every operation below runs a
-hand-written sm_100a kernel from libregtr_b200.so on the current CUDA stream.
+hand-written sm_90a kernel from libregtr_b200.so on the current CUDA stream.
 Tensors must live on a CUDA device; there is no CPU fallback.
 """
 from __future__ import annotations
@@ -333,7 +333,7 @@ def split_weight(w: torch.Tensor, transpose: bool = False):
 
 
 def gemm(a, b_hi, b_lo, bias=None, residual=None, relu=False, m_dev=None, out=None):
-    """act(a @ B^T + bias + residual) with B = b_hi + b_lo ([N,K] row-major), 3xTF32 tcgen05 kernel."""
+    """act(a @ B^T + bias + residual) with B = b_hi + b_lo ([N,K] row-major), 3xTF32 wgmma kernel."""
     L = _lib.load()
     if not a.is_cuda or a.dtype != torch.float32 or a.dim() != 2 or a.stride(1) != 1:
         raise ValueError('gemm: A must be a CUDA fp32 matrix with unit column stride')
@@ -385,7 +385,7 @@ def linear_instats(x, weight, offs, n_clouds: int, eps: float = 1e-5, m_dev=None
 
 
 def linear(x, weight, bias=None, residual=None, relu=False, m_dev=None):
-    """nn.Linear forward (x @ weight^T + bias) (+ residual, + ReLU) on the 3xTF32 tcgen05 GEMM of this
+    """nn.Linear forward (x @ weight^T + bias) (+ residual, + ReLU) on the 3xTF32 wgmma GEMM of this
     library.  The TMA row pitch needs K % 4 == 0 and 16-byte aligned rows; anything else raises (callers
     with an odd K zero-pad it, see PositionEmbeddingLearned) -- there is no library fallback."""
     if x.shape[1] % 4 or x.stride(0) % 4 or x.data_ptr() % 16:
@@ -493,7 +493,7 @@ def mha_varlen(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_heads:
 
 def mha_bf16_tc(x, in_w, in_b, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int, m_dev=None):
     """Attention block core in the fast precision mode: packed in-projection (3xTF32 GEMM, bf16
-    epilogue) + tcgen05 bf16 attention.  x (N,E) fp32 (already LN + pos); returns O (N,E) fp32."""
+    epilogue) + wgmma bf16 attention.  x (N,E) fp32 (already LN + pos); returns O (N,E) fp32."""
     L = _lib.load()
     _chk(x, torch.float32, 'x', 2)
     N, E = x.shape
@@ -514,8 +514,8 @@ def mha_bf16_tc(x, in_w, in_b, q_start, q_len, k_start, k_len, max_q_len: int, n
 
 
 def mha_tf32_tc(x, in_w, in_b, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int, m_dev=None, tiles=None):
-    """Attention block core, fp32-accurate, on the tcgen05 tensor cores: packed in-projection (3xTF32 GEMM whose
-    epilogue writes q / k / v^T as TF32 (hi, lo) halves) + the TMA-fed 3xTF32 attention kernel (P in tensor memory).
+    """Attention block core, fp32-accurate, on the Hopper tensor cores: packed in-projection (3xTF32 GEMM whose
+    epilogue writes q / k / v^T as TF32 (hi, lo) halves) + the TMA-fed 3xTF32 attention kernel (P in registers).
     x (N,E) fp32 (already LN + pos); returns O (N,E) fp32."""
     L = _lib.load()
     _chk(x, torch.float32, 'x', 2)

@@ -1,4 +1,4 @@
-"""RegTR forward on the B200 kernels -- the drop-in boundary.
+"""RegTR forward on the H100 kernels -- the drop-in boundary.
 
 `RegTR(cfg)` keeps the reference's constructor, sub-module names, state_dict layout
 (168 keys for the 3DMatch config, loadable with strict=True) and
@@ -11,7 +11,7 @@
        side effect batch['kpconv_meta'] (regtr.py:118).
 
 What differs from the reference is *how*: packed tokens instead of padded ones, one host
-sync for the pyramid sizes, hand-written sm_100a kernels for the neighbour search, the
+sync for the pyramid sizes, hand-written sm_90a kernels for the neighbour search, the
 KPConv gather/aggregation, normalisations, attention core and Kabsch, and a fused
 correspondence-assembly + sigmoid + Kabsch kernel (regtr.py:185-203 in one launch).
 Training (`compute_loss`, autograd through the custom kernels) is a "next" row.

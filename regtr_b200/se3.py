@@ -1,4 +1,4 @@
-"""Rigid-transform solve on the B200 kernel.
+"""Rigid-transform solve on the H100 kernel.
 
 `compute_rigid_transform(a, b, weights)` keeps the reference signature and semantics
 (/root/reference/src/utils/se3_torch.py:108-154): `a`, `b` ([*,] N, 3), `weights` ([*,] N)

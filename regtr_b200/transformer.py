@@ -1,4 +1,4 @@
-"""Stacked self/cross attention over the down-sampled point features, on the B200 kernels.
+"""Stacked self/cross attention over the down-sampled point features, on the H100 kernels.
 
 Host-side mirror of /root/reference/src/models/transformer/{transformers.py,
 position_embedding.py} for the branches both configs select: pre-norm
@@ -119,7 +119,7 @@ class AttentionPlan:
         self.xk_start, self.xk_len = table[2, :n2], table[3, :n2]
         self.max_len = int(max_len)
         self.n_dev = n_dev
-        # (device tile table, host bound of the total) for the 64-query (mma.sync) and 128-query (tcgen05) cores
+        # (device tile table, host bound of the total) for the 64-query (mma.sync) and 128-query (wgmma) cores
         self.tiles64 = (table[4], int(max_tiles[0]))
         self.tiles128 = (table[5], int(max_tiles[1]))
 
@@ -137,7 +137,7 @@ class TransformerCrossEncoderLayer(nn.Module):
                  attention_type='dot_prod', attention_impl='fp32'):
         super().__init__()
         if attention_impl not in ('fp32', 'tf32_tc', 'bf16_tc'):
-            raise ValueError("attention_impl: 'tf32_tc' (tcgen05 3xTF32, fp32-accurate), 'fp32' (mma.sync 3xTF32) or 'bf16_tc'")
+            raise ValueError("attention_impl: 'tf32_tc' (wgmma 3xTF32, fp32-accurate), 'fp32' (mma.sync 3xTF32) or 'bf16_tc'")
         self.attention_impl = attention_impl
         if attention_type != 'dot_prod':
             raise NotImplementedError
@@ -162,11 +162,11 @@ class TransformerCrossEncoderLayer(nn.Module):
         W, b = mha.in_proj_weight, mha.in_proj_bias
         ks, kl = (plan.xk_start, plan.xk_len) if cross else (plan.q_start, plan.q_len)
         if self.attention_impl == 'bf16_tc' and val_has_pos:
-            # fast mode: in-projection with a bf16 epilogue + tcgen05 attention core (TMA-fed, TMEM accumulators)
+            # fast mode: in-projection with a bf16 epilogue + wgmma attention core (TMA-fed, register accumulators)
             return ops.mha_bf16_tc(x2p, W, b, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead,
                                    m_dev=plan.n_dev)
         if self.attention_impl == 'tf32_tc' and val_has_pos:
-            # parity mode on the Blackwell path: split-epilogue in-projection + TMA-fed tcgen05 3xTF32 attention core
+            # parity mode on the tensor cores: split-epilogue in-projection + TMA-fed wgmma 3xTF32 attention core
             return ops.mha_tf32_tc(x2p, W, b, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead,
                                    m_dev=plan.n_dev, tiles=plan.tiles128)
         nd = plan.n_dev

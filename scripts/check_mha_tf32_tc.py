@@ -1,4 +1,4 @@
-"""tcgen05 3xTF32 attention block vs float64 and vs the mma.sync core (error + time)."""
+"""wgmma 3xTF32 attention block vs float64 and vs the mma.sync core (error + time)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -30,8 +30,8 @@ for lens in ([410, 339], [130, 7, 300, 129], [64, 64], [410, 380, 395, 402, 350,
             w = torch.softmax(q @ k.transpose(1, 2) / 32 ** 0.5, -1)
             ref[st[c]:st[c + 1]] = (w @ v).transpose(0, 1).reshape(-1, E)
         e_tc = float((got.double() - ref).abs().max()); e_mma = float((want.double() - ref).abs().max())
-        print(f'lens {lens[:4]}.. n={n} {name}: tcgen05 err {e_tc:.2e}  mma.sync err {e_mma:.2e}  finite {bool(torch.isfinite(got).all())}')
-    # timing (graph-free, back to back; includes the in-projection for the tcgen05 path)
+        print(f'lens {lens[:4]}.. n={n} {name}: wgmma err {e_tc:.2e}  mma.sync err {e_mma:.2e}  finite {bool(torch.isfinite(got).all())}')
+    # timing (graph-free, back to back; includes the in-projection for the wgmma path)
     e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
     for _ in range(3):
         ops.mha_tf32_tc(x, W, b, plan.q_start, plan.q_len, plan.xk_start, plan.xk_len, plan.max_len, H)
@@ -43,4 +43,4 @@ for lens in ([410, 339], [130, 7, 300, 129], [64, 64], [410, 380, 395, 402, 350,
         qkv = ops.linear(x, W, b)
         ops.mha_varlen(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], plan.q_start, plan.q_len, plan.xk_start, plan.xk_len, plan.max_len, H)
     e[2].record(); torch.cuda.synchronize()
-    print(f'   block time (in-proj + core): tcgen05 {e[0].elapsed_time(e[1]) / 20 * 1e3:.1f} us, mma.sync {e[1].elapsed_time(e[2]) / 20 * 1e3:.1f} us')
+    print(f'   block time (in-proj + core): wgmma {e[0].elapsed_time(e[1]) / 20 * 1e3:.1f} us, mma.sync {e[1].elapsed_time(e[2]) / 20 * 1e3:.1f} us')

@@ -1,4 +1,4 @@
-"""3DMatch / 3DLoMatch registration recall of a checkpoint on the B200 path (the reference's `test.py`):
+"""3DMatch / 3DLoMatch registration recall of a checkpoint on the CUDA path (the reference's `test.py`):
 
     python scripts/eval_3dmatch.py --root <data/indoor> --info <test_3DMatch_info.pkl> \
         --gt <datasets/3dmatch/benchmarks/3DMatch> --ckpt <model.pth> --out logs/3DMatch

@@ -395,6 +395,29 @@ def grad_fixture():
     print('grad: parameters with a gradient', n, 'total loss', float(fx['loss_total']))
 
 
+def data_fixture():
+    """What the reference's collate_pair (src/data_loaders/collate_functions.py) and sequence helpers
+    (src/utils/seq_manipulation.py) return on the seeded inputs of tests/test_data.py."""
+    import importlib.util
+    import pathlib
+    import tempfile
+    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    import test_data as T
+
+    def load(rel):
+        spec = importlib.util.spec_from_file_location(os.path.basename(rel)[:-3], os.path.join(ref_bridge.REF_SRC, rel))
+        mod = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(mod)
+        return mod
+    collate, seq = load('data_loaders/collate_functions.py'), load('utils/seq_manipulation.py')
+    with tempfile.TemporaryDirectory() as d:
+        ds, _ = T._make_dataset(pathlib.Path(d))
+        fx = T.encode_collate(collate.collate_pair([ds[i] for i in T.COLLATE_ITEMS]))
+    fx.update(T.encode_seq(seq, *T.seq_inputs()))
+    np.savez_compressed(os.path.join(OUT, 'data.npz'), **fx)
+    print('data', len(fx), 'arrays')
+
+
 if __name__ == '__main__':
     torch.manual_seed(0)
     np.random.seed(0)
@@ -409,6 +432,9 @@ if __name__ == '__main__':
     if len(sys.argv) > 1 and sys.argv[1] == 'grad':
         grad_fixture()
         sys.exit(0)
+    if len(sys.argv) > 1 and sys.argv[1] == 'data':
+        data_fixture()
+        sys.exit(0)
     eval_fixtures()
     loss_fixture()
     grad_fixture()
@@ -416,6 +442,7 @@ if __name__ == '__main__':
     for case in FORWARD_CASES:
         forward_fixture(case)
     benchmark_fixture()
+    data_fixture()
     for case in REAL_CASES:
         real_fixture(case)
     for f in sorted(os.listdir(OUT)):

@@ -1,16 +1,18 @@
 """CPU tests of the input pipeline (SURVEY.md 8f N2, regtr_b200/data.py): file formats of the reference's
-3DMatch loader, collate layout, size bucketing, read-ahead stream."""
+3DMatch loader, collate layout, size bucketing, read-ahead stream.  What the reference's own functions return
+on the same inputs is stored in tests/golden/data.npz (tests/golden/make_golden.py)."""
+import json
 import os
 import pickle
-import sys
 
 import numpy as np
 import pytest
 import torch
 
+from conftest import GOLDEN, load_golden
 from regtr_b200 import data as D
 
-REF = '/root/reference'
+COLLATE_ITEMS = (4, 0, 7)
 
 
 def _make_dataset(tmp_path, n_pairs=11, seed=0):
@@ -43,40 +45,87 @@ def test_dataset_items_and_collate(tmp_path):
     assert b['overlap_p'].shape == (3,) and b['idx'] == [0, 1, 2]
 
 
+def encode_collate(batch):
+    """A collated batch as flat arrays: 'collate/<key>' for a tensor, 'collate/<key>/<i>' for list entries, plus
+    the key list and which keys are lists."""
+    fx = {'collate/__keys__': np.array(sorted(batch)),
+          'collate/__lists__': np.array(sorted(k for k, v in batch.items() if isinstance(v, list)))}
+    for k, v in batch.items():
+        for name, x in ([(f'collate/{k}', v)] if torch.is_tensor(v) else
+                        [(f'collate/{k}/{i}', x) for i, x in enumerate(v)]):
+            fx[name] = x.numpy() if torch.is_tensor(x) else np.array(x)
+    return fx
+
+
+def seq_inputs():
+    rng = np.random.default_rng(2)
+    seqs = [torch.from_numpy(rng.normal(size=(n, 5)).astype(np.float32)) for n in (7, 3, 11, 1)]
+    six = torch.from_numpy(rng.normal(size=(6, 11, 4, 5)).astype(np.float32))
+    return seqs, six
+
+
+def encode_seq(S, seqs, six):
+    """Outputs of pad_sequence / unpad_sequences / split_src_tgt of module S on the inputs above, as flat arrays."""
+    fx = {}
+    lens = [len(x) for x in seqs]
+    for name, kw in (('plain', dict()), ('mask_lens', dict(require_padding_mask=True, require_lens=True))):
+        padded, mask, plens = S.pad_sequence(seqs, **kw)
+        fx[f'seq/pad_{name}'] = padded.numpy()
+        fx[f'seq/pad_{name}_mask'] = np.zeros(0, bool) if mask is None else mask.numpy()
+        fx[f'seq/pad_{name}_lens'] = np.array(-1 if plens is None else plens)
+    for b, x in enumerate(S.unpad_sequences(six, lens)):
+        fx[f'seq/unpad_{b}'] = x.numpy()
+    src, tgt = S.split_src_tgt(torch.cat(seqs), lens)
+    for side, xs in (('src', src), ('tgt', tgt)):
+        for i, x in enumerate(xs):
+            fx[f'seq/split_{side}_{i}'] = x.numpy()
+    return fx
+
+
+def assert_same_arrays(got, want, prefix):
+    want = {k: v for k, v in want.items() if k.startswith(prefix)}
+    assert set(got) == set(want)
+    for k, v in want.items():
+        assert got[k].dtype == v.dtype and got[k].shape == v.shape and np.array_equal(got[k], v), k
+
+
 def test_collate_matches_reference_function(tmp_path):
-    if not os.path.isdir(REF):
-        pytest.skip('reference not present on this machine')
-    import importlib.util                       # the file only imports torch; its package __init__ needs h5py
-    spec = importlib.util.spec_from_file_location('ref_collate_functions',
-                                                  os.path.join(REF, 'src', 'data_loaders', 'collate_functions.py'))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    ref_collate = mod.collate_pair
+    """collate_pair vs what the reference's collate_functions.collate_pair returned on the same items."""
     ds, _ = _make_dataset(tmp_path)
-    items = [ds[i] for i in (4, 0, 7)]
-    a, b = D.collate_pair(items), ref_collate(items)
-    assert set(a) == set(b)
-    for k in a:
-        if torch.is_tensor(a[k]):
-            assert torch.equal(a[k], b[k])
-        else:
-            assert len(a[k]) == len(b[k]) and all(
-                (torch.equal(x, y) if torch.is_tensor(x) else x == y) for x, y in zip(a[k], b[k]))
+    got = encode_collate(D.collate_pair([ds[i] for i in COLLATE_ITEMS]))
+    assert_same_arrays(got, load_golden('data'), 'collate/')
 
 
-def test_reads_the_reference_sample_pairs():
-    """The 3DMatch pairs shipped with the reference (data/indoor, demo.py) through the real benchmark pickle."""
-    root, info = os.path.join(REF, 'data', 'indoor'), os.path.join(REF, 'src', 'datasets', '3dmatch', 'test_3DMatch_info.pkl')
-    if not (os.path.isdir(root) and os.path.isfile(info)):
-        pytest.skip('reference data not present on this machine')
-    ds = D.ThreeDMatchPairs(root, info)
-    assert len(ds) == 1623
-    have = [i for i in range(len(ds)) if all(os.path.isfile(os.path.join(root, ds.infos[k][i])) for k in ('src', 'tgt'))]
-    assert have, 'no complete pair among the shipped sample clouds'
-    it = ds[have[0]]
-    raw = torch.load(os.path.join(root, it['src_path']), weights_only=False)
-    assert raw.dtype == np.float64 and torch.equal(it['src_xyz'], torch.from_numpy(raw).float())
-    assert 5000 < it['src_xyz'].shape[0] < 60000 and it['pose'].shape == (3, 4)
+def test_reads_the_reference_sample_pairs(tmp_path):
+    """The reference's two shipped 3DMatch benchmark pairs (data/indoor, demo.py) through a benchmark pickle with
+    their real rows, the clouds stored as the dataset stores them (float64 .pth under test/<scene>/)."""
+    rows = json.load(open(os.path.join(GOLDEN, 'real', 'test_3DMatch_info_rows.json')))
+    infos = dict(rot=[], trans=[], src=[], tgt=[], overlap=[])
+    raws = {}
+    for r in rows:
+        inp = np.load(os.path.join(GOLDEN, 'real', r['fixture'] + '_input.npz'))
+        for rel in (r['src'], r['tgt']):
+            which = 'src_xyz' if os.path.basename(rel) == os.path.basename(str(inp['src_file'])) else 'tgt_xyz'
+            os.makedirs(tmp_path / 'indoor' / os.path.dirname(rel), exist_ok=True)
+            raws[rel] = inp[which].astype(np.float64)
+            torch.save(raws[rel], tmp_path / 'indoor' / rel)
+        for k in ('rot', 'trans'):
+            infos[k].append(np.array(r[k]))
+        for k in ('src', 'tgt', 'overlap'):
+            infos[k].append(r[k])
+    with open(tmp_path / 'info.pkl', 'wb') as f:
+        pickle.dump(infos, f)
+    root = str(tmp_path / 'indoor')
+    ds = D.ThreeDMatchPairs(root, str(tmp_path / 'info.pkl'))
+    assert len(ds) == len(rows) == 2
+    for i, r in enumerate(rows):
+        it = ds[i]
+        raw = torch.load(os.path.join(root, it['src_path']), weights_only=False)
+        assert raw.dtype == np.float64 and np.array_equal(raw, raws[r['src']])
+        assert torch.equal(it['src_xyz'], torch.from_numpy(raw).float())
+        assert 5000 < it['src_xyz'].shape[0] < 60000 and it['pose'].shape == (3, 4)
+        np.testing.assert_allclose(it['pose'][:, :3].numpy(), np.array(r['rot']), atol=1e-6)
+        np.testing.assert_allclose(it['pose'][:, 3:].numpy(), np.array(r['trans']), atol=1e-6)
 
 
 def test_bucket_order_is_a_partition_grouped_by_capacity():
@@ -105,11 +154,9 @@ def test_pair_stream_order_and_errors(tmp_path):
 
 
 def test_sequence_helpers_match_reference():
-    """regtr_b200.seq vs utils/seq_manipulation.py (imported when the reference is present), plus a padded
-    round trip."""
+    """regtr_b200.seq vs what utils/seq_manipulation.py returned on the same inputs, plus a padded round trip."""
     from regtr_b200 import seq as S
-    rng = np.random.default_rng(2)
-    seqs = [torch.from_numpy(rng.normal(size=(n, 5)).astype(np.float32)) for n in (7, 3, 11, 1)]
+    seqs, six = seq_inputs()
     padded, mask, lens = S.pad_sequence(seqs, require_padding_mask=True, require_lens=True)
     assert padded.shape == (11, 4, 5) and mask.shape == (4, 11) and lens == [7, 3, 11, 1]
     assert mask[1, 3:].all() and not mask[1, :3].any() and not mask[2].any()
@@ -118,20 +165,7 @@ def test_sequence_helpers_match_reference():
     stacked = torch.cat(seqs)
     src, tgt = S.split_src_tgt(stacked, torch.tensor(lens))
     assert len(src) == 2 and torch.equal(tgt[1], seqs[3])
-    if os.path.isdir(REF):
-        import importlib.util
-        spec = importlib.util.spec_from_file_location('ref_seq', os.path.join(REF, 'src', 'utils', 'seq_manipulation.py'))
-        R = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(R)
-        for kw in (dict(), dict(require_padding_mask=True, require_lens=True)):
-            a, b = S.pad_sequence(seqs, **kw), R.pad_sequence(seqs, **kw)
-            assert torch.equal(a[0], b[0]) and (a[1] is None) == (b[1] is None) and a[2] == b[2]
-            if a[1] is not None:
-                assert torch.equal(a[1], b[1])
-        six = torch.from_numpy(rng.normal(size=(6, 11, 4, 5)).astype(np.float32))
-        assert all(torch.equal(x, y) for x, y in zip(S.unpad_sequences(six, lens), R.unpad_sequences(six, lens)))
-        a, b = S.split_src_tgt(stacked, lens), R.split_src_tgt(stacked, lens)
-        assert all(torch.equal(x, y) for x, y in zip(a[0] + a[1], b[0] + b[1]))
+    assert_same_arrays(encode_seq(S, seqs, six), load_golden('data'), 'seq/')
 
 
 def test_compute_overlap_properties(tmp_path):

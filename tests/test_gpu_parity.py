@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA product, called through the C ABI, against
+"""GPU parity tests (run on an H100): the CUDA product, called through the C ABI, against
 (a) the golden fixtures produced by the unmodified reference and (b) the CPU oracle on the same
 seeded inputs.  Integer / index results must be bit-exact; float tolerances are stated per test
 (SURVEY.md 8c: features <= 1e-4 * max|ref|, correspondences <= 1e-5 m ... pose <= 1e-4)."""
@@ -429,7 +429,7 @@ def test_graphed_executor_matches_eager_and_survives_overflow():
 
 
 def test_tcgen05_attention_core_vs_fp32_kernel():
-    """bf16 tcgen05 attention (TMA-fed, TMEM accumulators) vs the fp32 parity kernel on ragged self and
+    """bf16 wgmma attention (TMA-fed, register accumulators) vs the fp32 parity kernel on ragged self and
     cross problems (unaligned key ranges, partial tiles, a 7-token cloud).  Tolerance of the fast mode:
     3e-2 * max|ref| (bf16 operands, SURVEY 8c)."""
     from regtr_b200 import ops
@@ -742,12 +742,12 @@ def N_(t):
 
 @pytest.mark.parametrize('N,K', [(32, 64), (32, 480), (64, 960), (128, 32), (128, 64), (256, 64)])
 def test_gemm_persistent_tiles_vs_float64(N, K):
-    """Launches of several waves take the persistent kernel (tile loop per CTA, barrier phases running across tiles,
-    accumulator hand-over between MMA and epilogue): bias / residual / ReLU, a device-side row count that ends inside
+    """Launches of several waves walk their tiles persistently (tile loop per CTA, barrier phases running across
+    tiles, the next tile's loads in flight under the epilogue): bias / residual / ReLU, a device-side row count that ends inside
     a tile, InstanceNorm partials of two clouds, all against float64; repeated calls bit-identical."""
     from regtr_b200 import ops
     rng = np.random.default_rng(N * 1000 + K)
-    cap, M = 46000, 44321                                      # 360 row tiles > 2 x 148; the last real tile is partial
+    cap, M = 46000, 44321                                      # 360 row tiles > 2 x 132 SMs; the last real tile is partial
     a = np.zeros((cap, K), dtype=np.float32)
     a[:M] = rng.normal(size=(M, K)) * 0.9 + 0.2
     a[M:] = 7e2
@@ -834,7 +834,7 @@ def test_benchmark_loop_on_real_sample_pairs_through_graph_executor(tmp_path):
         assert np.allclose(traj[0, 3], [0, 0, 0, 1])
 
 
-# ------------------------------------------------- fp32-accurate tcgen05 attention core (3xTF32, TMA-fed, P in TMEM)
+# ------------------------------------------------- fp32-accurate wgmma attention core (3xTF32, TMA-fed, P in registers)
 
 @pytest.mark.parametrize('lens', [[410, 339], [130, 7, 300, 129], [64, 64], [1, 200, 65, 3]])
 def test_tf32_tcgen05_attention_block_vs_float64(lens):
@@ -875,8 +875,8 @@ def test_tf32_tcgen05_attention_block_vs_float64(lens):
 
 
 def test_forward_with_tf32_tcgen05_attention_vs_reference_golden():
-    """Full forward with attention_impl='tf32_tc' (both MHA contractions on tcgen05, fed by TMA) against the
-    unmodified reference: features 1e-4, pose 1e-4 -- the parity mode on the Blackwell path."""
+    """Full forward with attention_impl='tf32_tc' (both MHA contractions on wgmma, fed by TMA) against the
+    unmodified reference: features 1e-4, pose 1e-4 -- the parity mode on the tensor cores."""
     case = 'fwd_3dmatch_small_b2'
     cfg, sd, src, tgt = make_case(case)
     cfg.attention_impl = 'tf32_tc'
