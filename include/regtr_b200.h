@@ -263,6 +263,51 @@ int regtr_mha_tf32_tc_fwd(const float* qk4, int ld4, const float* vt2, int ld_vt
                           int max_tiles, int n_heads, int head_dim, void* stream);
 /* (tile_base / max_tiles as for regtr_mha_varlen_fwd, with 128-query tiles.) */
 
+/* Training forward of the regtr_mha_varlen_fwd core (the default 3xTF32 mma.sync kernel): same O, bit for bit, plus
+ * lse [n_tokens, n_heads] = log2(sum_k exp2(s_qk)) of the base-2 scores s = (q * scale * log2 e) . k -- what
+ * regtr_mha_varlen_bwd recomputes the softmax from (-inf for a query whose key range is empty).  No tile table. */
+int regtr_mha_varlen_fwd_lse(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                             float* O, int ldo, float* lse, const int32_t* q_start, const int32_t* q_len,
+                             const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
+                             int n_heads, int head_dim, float scale, void* stream);
+
+/* ---- backward (training) ---------------------------------------------------------- */
+
+/* Backward of the attention core over the same problem tables: given O and lse from regtr_mha_varlen_fwd_lse and
+ * dO, writes dQ (rows of every query range), dK and dV (rows of every key range; 0 for a key range whose problem
+ * has no queries).  Each key row must belong to the key range of exactly one problem (true of the self and of the
+ * cross table of regtr_attention_plan); dQ / dK / dV may be column slices of one packed [n_rows, 3E] buffer.
+ * n_rows: rows of Q / lse (an upper bound of every query row index + 1); max_k_len: host bound of k_len[].
+ * Deterministic (no atomics): one pass owns the query rows, a second one the key rows.
+ * ws: regtr_mha_varlen_bwd_ws_bytes(n_rows, n_heads) bytes (rowsum(dO * O) per query and head). */
+size_t regtr_mha_varlen_bwd_ws_bytes(int n_rows, int n_heads);
+int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                         const float* O, int ldo, const float* dO, int lddo, const float* lse,
+                         float* dQ, int lddq, float* dK, int lddk, float* dV, int lddv,
+                         const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
+                         const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len,
+                         int n_heads, int head_dim, float scale, void* ws, size_t ws_bytes, void* stream);
+
+/* Backward of regtr_layernorm_pos: dy and dy_pos (either may be NULL; they add) are the gradients of y and y_pos,
+ * dres (optional) a gradient of x arriving through a residual connection, added to dx.  Mean and rstd are
+ * recomputed from x.  dgamma / dbeta (E) from per-block column partials summed in a fixed order.  E % 32 == 0,
+ * E <= 256.  ws: regtr_layernorm_bwd_ws_bytes(n, E) bytes. */
+size_t regtr_layernorm_bwd_ws_bytes(int n, int E);
+int regtr_layernorm_bwd(const float* x, const float* gamma, const float* dy, const float* dy_pos, const float* dres,
+                        int n, int E, float eps, float* dx, float* dgamma, float* dbeta,
+                        void* ws, size_t ws_bytes, void* stream);
+
+/* ReLU backward: out = dh * (h > 0), h the ReLU's output (n elements; out may alias dh). */
+int regtr_relu_bwd(const float* dh, const float* h, long long n, float* out, void* stream);
+
+/* Weight gradient of a dense layer Y = X W^T + b:  dW[N,K] = dY^T X,  db[N] = sum_rows dY (db optional),
+ * 3xTF32 on regtr_gemm_tf32x3 (the reduction over the M rows uses its deterministic split-K).  X (M,K) and
+ * dY (M,N) row-major with leading dimensions ldx / ldy.  ws: regtr_linear_wgrad_ws_bytes(M, N, K) bytes,
+ * 256-byte aligned (transposed, TF32-split operands and the product). */
+size_t regtr_linear_wgrad_ws_bytes(int M, int N, int K);
+int regtr_linear_wgrad(const float* X, int ldx, const float* dY, int ldy, int M, int N, int K,
+                       float* dW, float* db, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- pose ------------------------------------------------------------------------- */
 
 /* Weighted Kabsch.  Replaces compute_rigid_transform (utils/se3_torch.py:108-154):

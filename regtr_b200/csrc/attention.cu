@@ -154,7 +154,7 @@ __global__ void __launch_bounds__(128)
 k_mha_tf32x3(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp, int ldk, const float* __restrict__ Vp,
              int ldv, float* __restrict__ O, int ldo, const int32_t* __restrict__ q_start,
              const int32_t* __restrict__ q_len, const int32_t* __restrict__ k_start, const int32_t* __restrict__ k_len,
-             const int32_t* __restrict__ tile_base, int n_prob, float scale) {
+             const int32_t* __restrict__ tile_base, int n_prob, float scale, float* __restrict__ lse) {
     __shared__ __align__(16) float sKh[MK][MLD], sKl[MK][MLD], sVh[MK][MLD], sVl[MK][MLD];
     int prob = blockIdx.z, tile = blockIdx.x;
     const int head = blockIdx.y;
@@ -288,6 +288,11 @@ k_mha_tf32x3(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
     const float i0 = l0 > 0.f ? 1.f / l0 : 0.f, i1 = l1 > 0.f ? 1.f / l1 : 0.f;
+    if (lse && t == 0) {                         // base-2 log-sum-exp of the scaled scores (-inf: empty key range)
+        const int nh = gridDim.y;
+        if (r0 < ql) lse[(size_t)(q0 + r0) * nh + head] = m0 + log2f(l0);
+        if (r1 < ql) lse[(size_t)(q0 + r1) * nh + head] = m1 + log2f(l1);
+    }
     // C fragment: (r0, 8j+2t), (r0, 8j+2t+1), (r1, 8j+2t), (r1, 8j+2t+1)
     if (r0 < ql) {
         float* dst = O + (size_t)(q0 + r0) * ldo + col + 2 * t;
@@ -427,24 +432,23 @@ extern "C" int regtr_attention_plan(const int32_t* offs, int B, int32_t* plan, v
     return REGTR_OK;
 }
 
-extern "C" int regtr_mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
-                                    float* O, int ldo, const int32_t* q_start, const int32_t* q_len,
-                                    const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
-                                    const int32_t* tile_base, int max_tiles, int n_heads, int head_dim, float scale,
-                                    void* stream_) {
-    cudaStream_t st = (cudaStream_t)stream_;
+static int mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, float* O, int ldo,
+                          const int32_t* q_start, const int32_t* q_len, const int32_t* k_start, const int32_t* k_len,
+                          int n_problems, int max_q_len, const int32_t* tile_base, int max_tiles, int n_heads,
+                          int head_dim, float scale, float* lse, cudaStream_t st) {
     if (n_problems < 0 || max_q_len < 0 || n_heads <= 0 || max_tiles < 0) return REGTR_ERR_ARG;
     if (head_dim != HD) return REGTR_ERR_UNSUPPORTED;
     if (n_problems == 0 || max_q_len == 0 || (tile_base && max_tiles == 0)) return REGTR_OK;
     if (!Q || !K || !V || !O || !q_start || !q_len || !k_start || !k_len) return REGTR_ERR_ARG;
     if ((ldq | ldk | ldv) % 4 != 0 || n_problems > 65535 || n_heads > 65535) return REGTR_ERR_ARG;
     const char* impl = getenv("REGTR_MHA_IMPL");           // "ffma": CUDA-core kernel (A/B measurements)
-    if (!(impl && impl[0] == 'f') && (ldo % 2) == 0) {
+    if (lse || (!(impl && impl[0] == 'f') && (ldo % 2) == 0)) {
+        if (ldo % 2) return REGTR_ERR_UNSUPPORTED;
         // with the tile table: linear 64-query tile index (max_tiles = host bound of the total); else one grid
         // column per problem sized by the longest sequence
         const dim3 grid = tile_base ? dim3(max_tiles, n_heads, 1) : dim3(regtr_cdiv(max_q_len, MQ), n_heads, n_problems);
         k_mha_tf32x3<<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, tile_base,
-                                          n_problems, scale * 1.4426950408889634f);
+                                          n_problems, scale * 1.4426950408889634f, lse);
         REGTR_CHECK_LAUNCH();
         return REGTR_OK;
     }
@@ -454,6 +458,26 @@ extern "C" int regtr_mha_varlen_fwd(const float* Q, int ldq, const float* K, int
                                             scale * 1.4426950408889634f);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
+}
+
+extern "C" int regtr_mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                                    float* O, int ldo, const int32_t* q_start, const int32_t* q_len,
+                                    const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
+                                    const int32_t* tile_base, int max_tiles, int n_heads, int head_dim, float scale,
+                                    void* stream_) {
+    return mha_varlen_fwd(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, n_problems, max_q_len,
+                          tile_base, max_tiles, n_heads, head_dim, scale, nullptr, (cudaStream_t)stream_);
+}
+
+// Training forward: the same 3xTF32 core, which also stores the per-(row, head) base-2 log-sum-exp that the backward
+// recomputes the softmax from.
+extern "C" int regtr_mha_varlen_fwd_lse(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                                        float* O, int ldo, float* lse, const int32_t* q_start, const int32_t* q_len,
+                                        const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
+                                        int n_heads, int head_dim, float scale, void* stream_) {
+    if (!lse) return REGTR_ERR_ARG;
+    return mha_varlen_fwd(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, n_problems, max_q_len,
+                          nullptr, 0, n_heads, head_dim, scale, lse, (cudaStream_t)stream_);
 }
 
 extern "C" int regtr_corr_decode_fwd(const float* Qp, const float* Kp, int ld, const float* xyz, float* out,

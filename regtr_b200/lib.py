@@ -64,6 +64,15 @@ SIGNATURES = {
     'regtr_mha_bf16_tc_fwd': (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     'regtr_gemm_tf32x3_qkv_split': (_I, [_P, _I, _P, _P, _I, _P, _I, _I, _I, _I, _F, _P, _I, _P, _I, _P, _P]),
     'regtr_mha_tf32_tc_fwd': (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _P, _P, _P, _I, _I, _P, _I, _I, _I, _P]),
+    'regtr_mha_varlen_fwd_lse': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
+    'regtr_mha_varlen_bwd_ws_bytes': (_Z, [_I, _I]),
+    'regtr_mha_varlen_bwd': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _I, _P, _I, _P, _I,
+                                  _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P, _Z, _P]),
+    'regtr_layernorm_bwd_ws_bytes': (_Z, [_I, _I]),
+    'regtr_layernorm_bwd': (_I, [_P, _P, _P, _P, _P, _I, _I, _F, _P, _P, _P, _P, _Z, _P]),
+    'regtr_relu_bwd': (_I, [_P, _P, _c.c_longlong, _P, _P]),
+    'regtr_linear_wgrad_ws_bytes': (_Z, [_I, _I, _I]),
+    'regtr_linear_wgrad': (_I, [_P, _I, _P, _I, _I, _I, _I, _P, _P, _P, _Z, _P]),
     'regtr_kabsch_fwd': (_I, [_P, _P, _P, _P, _I, _P, _P]),
     'regtr_pose_from_corr': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),

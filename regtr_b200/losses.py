@@ -1,12 +1,13 @@
 """Loss values of a forward pass (SURVEY.md 8f N1/N3: `test_step` reports them, `training_step` needs them).
 
-Forward-only mirror of
+Mirror of
   * `RegTR.compute_loss` (/root/reference/src/models/regtr.py:237-294) and its `weight_dict` (regtr.py:89-93),
   * `compute_overlaps` (/root/reference/src/models/backbone_kpconv/kpconv.py:540-566),
   * `CorrCriterion` (/root/reference/src/models/losses/corr_loss.py:9-40),
   * `InfoNCELossFull` (/root/reference/src/models/losses/feature_loss.py:246-314).
 Plain torch ops on whatever device the predictions live on: this is bookkeeping around the hot path, not part
-of it.  Gradients do not flow into the CUDA kernels yet (N3)."""
+of it.  Differentiable: on outputs of `RegTR.forward_train` the gradient flows on into the library's backward
+kernels (everything after the KPConv encoder)."""
 from __future__ import annotations
 
 from typing import Dict, List

@@ -384,10 +384,23 @@ def linear_instats(x, weight, offs, n_clouds: int, eps: float = 1e-5, m_dev=None
     return gemm_instats(x, hi, lo, offs, n_clouds, eps, m_dev=m_dev)
 
 
+def _wants_grad(*ts):
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
+
+
 def linear(x, weight, bias=None, residual=None, relu=False, m_dev=None):
     """nn.Linear forward (x @ weight^T + bias) (+ residual, + ReLU) on the 3xTF32 wgmma GEMM of this
     library.  The TMA row pitch needs K % 4 == 0 and 16-byte aligned rows; anything else raises (callers
-    with an odd K zero-pad it, see PositionEmbeddingLearned) -- there is no library fallback."""
+    with an odd K zero-pad it, see PositionEmbeddingLearned) -- there is no library fallback.
+    Differentiable (_LinearFn) when grad mode is on and an input requires grad (exact shapes only)."""
+    if _wants_grad(x, weight, bias, residual):
+        if m_dev is not None:
+            raise ValueError('linear: the backward needs exact shapes (no m_dev)')
+        return _LinearFn.apply(x, weight, bias, residual, bool(relu))
+    return _linear_fwd(x, weight, bias, residual, relu, m_dev)
+
+
+def _linear_fwd(x, weight, bias=None, residual=None, relu=False, m_dev=None):
     if x.shape[1] % 4 or x.stride(0) % 4 or x.data_ptr() % 16:
         raise _lib.RegtrLibError(f'linear: K={x.shape[1]}, row stride {x.stride(0)}: rows must be 16-byte '
                                  'aligned multiples of 4 floats (zero-pad K); no cuBLAS fallback')
@@ -426,8 +439,22 @@ def pos_embed_sine(xyz, d_model: int = 256, temperature: float = 10000.0, scale:
     return out
 
 
-def layernorm_pos(x, gamma, beta, pos=None, eps: float = 1e-5, want_plain=True, want_pos=True, n_dev=None):
-    """-> (LN(x), LN(x)+pos); either may be skipped.  n_dev: device row count when x is capacity-shaped."""
+def layernorm_pos(x, gamma, beta, pos=None, eps: float = 1e-5, want_plain=True, want_pos=True, n_dev=None,
+                  skip=False):
+    """-> (LN(x), LN(x)+pos); either may be skipped.  n_dev: device row count when x is capacity-shaped.
+    Differentiable (_LayerNormPosFn) when grad mode is on and an input requires grad.  skip=True (training path)
+    also returns x itself as a third output, for the residual connection that adds x back: its gradient then reaches
+    the LayerNorm backward as `dres` and is added there, so x has one consumer in the autograd graph."""
+    if _wants_grad(x, gamma, beta):
+        if n_dev is not None:
+            raise ValueError('layernorm_pos: the backward needs exact shapes (no n_dev)')
+        outs = _LayerNormPosFn.apply(x, gamma, beta, pos, float(eps), bool(want_plain), bool(want_pos), bool(skip))
+        return outs if skip else outs[:2]
+    outs = _layernorm_pos_fwd(x, gamma, beta, pos, eps, want_plain, want_pos, n_dev)
+    return outs + (x,) if skip else outs
+
+
+def _layernorm_pos_fwd(x, gamma, beta, pos=None, eps: float = 1e-5, want_plain=True, want_pos=True, n_dev=None):
     L = _lib.load()
     _chk(x, torch.float32, 'x', 2)
     n, E = x.shape
@@ -545,6 +572,166 @@ def mha_tf32_tc(x, in_w, in_b, q_start, q_len, k_start, k_len, max_q_len: int, n
                                        _stream()), 'regtr_mha_tf32_tc_fwd')
     _count(2)
     return out
+
+
+def mha_varlen_lse(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int):
+    """Training forward of `mha_varlen` (the default 3xTF32 core): -> (O (N,E), lse (N, n_heads)), lse the base-2
+    log-sum-exp of the scaled scores that `mha_varlen_bwd` recomputes the softmax from."""
+    L = _lib.load()
+    for t, nm in ((q, 'q'), (k, 'k'), (v, 'v')):
+        if not t.is_cuda or t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1:
+            raise ValueError(f'mha_varlen: {nm} must be a CUDA fp32 matrix with unit column stride')
+    E = q.shape[1]
+    dh = E // n_heads
+    out = torch.empty((q.shape[0], E), dtype=torch.float32, device=q.device)
+    lse = torch.empty((q.shape[0], n_heads), dtype=torch.float32, device=q.device)
+    _lib.check(L.regtr_mha_varlen_fwd_lse(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(out),
+                                          out.stride(0), _p(lse), _p(q_start), _p(q_len), _p(k_start), _p(k_len),
+                                          q_start.numel(), int(max_q_len), n_heads, dh, 1.0 / math.sqrt(dh), _stream()),
+               'regtr_mha_varlen_fwd_lse')
+    _count(1)
+    return out, lse
+
+
+def mha_varlen_bwd(q, k, v, o, lse, d_o, dq, dk, dv, q_start, q_len, k_start, k_len, max_q_len: int, max_k_len: int,
+                   n_heads: int):
+    """Backward of the attention core: writes dq / dk / dv (views of the caller's buffers, e.g. column slices of one
+    packed [N, 3E] gradient).  Every key row must lie in the key range of exactly one problem."""
+    L = _lib.load()
+    _chk(d_o, torch.float32, 'dO', 2)
+    E = q.shape[1]
+    dh = E // n_heads
+    n_rows = q.shape[0]
+    ws = workspace(L.regtr_mha_varlen_bwd_ws_bytes(n_rows, n_heads), q.device, 'mha_bwd')
+    _lib.check(L.regtr_mha_varlen_bwd(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(o), o.stride(0),
+                                      _p(d_o), d_o.stride(0), _p(lse), _p(dq), dq.stride(0), _p(dk), dk.stride(0),
+                                      _p(dv), dv.stride(0), _p(q_start), _p(q_len), _p(k_start), _p(k_len),
+                                      q_start.numel(), n_rows, int(max_q_len), int(max_k_len), n_heads, dh,
+                                      1.0 / math.sqrt(dh), _p(ws), ws.numel(), _stream()), 'regtr_mha_varlen_bwd')
+    _count(2)
+
+
+def mha_packed(qkv, q_start, q_len, k_start, k_len, max_len: int, n_heads: int):
+    """Attention core over a packed in-projection output qkv (N, 3E) = [q | k | v]; differentiable with respect to
+    qkv (one packed (N, 3E) gradient, written by the backward kernels directly) when grad mode is on."""
+    E = qkv.shape[1] // 3
+    if _wants_grad(qkv):
+        return _MHAPackedFn.apply(qkv, q_start, q_len, k_start, k_len, int(max_len), int(n_heads))
+    return mha_varlen(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], q_start, q_len, k_start, k_len, max_len, n_heads)
+
+
+def layernorm_bwd(x, gamma, dy, dy_pos, dres, eps: float):
+    """-> (dx, dgamma, dbeta) of regtr_layernorm_pos; dy / dy_pos / dres may be None."""
+    L = _lib.load()
+    _chk(x, torch.float32, 'x', 2)
+    n, E = x.shape
+    for t, nm in ((dy, 'dy'), (dy_pos, 'dy_pos'), (dres, 'dres')):
+        if t is not None:
+            _chk(t, torch.float32, nm, 2)
+    dx = torch.empty_like(x)
+    dg = torch.empty_like(gamma)
+    db = torch.empty_like(gamma)
+    ws = workspace(L.regtr_layernorm_bwd_ws_bytes(n, E), x.device, 'ln_bwd')
+    _lib.check(L.regtr_layernorm_bwd(_p(x), _p(gamma), _p(dy), _p(dy_pos), _p(dres), n, E, float(eps), _p(dx), _p(dg),
+                                     _p(db), _p(ws), ws.numel(), _stream()), 'regtr_layernorm_bwd')
+    _count(2)
+    return dx, dg, db
+
+
+def relu_bwd(dh, h):
+    L = _lib.load()
+    out = torch.empty_like(dh)
+    _lib.check(L.regtr_relu_bwd(_p(dh), _p(h), dh.numel(), _p(out), _stream()), 'regtr_relu_bwd')
+    _count(1)
+    return out
+
+
+def linear_dgrad(dy, weight):
+    """dX = dY @ W on the 3xTF32 GEMM with the transposed pre-split weight.  N_out % 4 != 0 (the 3- and 1-wide heads) zero-pads dY and W^T to the TMA row pitch."""
+    N = weight.shape[0]
+    hi, lo = split_weight(weight, transpose=True)            # (K, N)
+    pad = (-N) % 4
+    if pad:
+        dy = torch.nn.functional.pad(dy, (0, pad))
+        hi, lo = torch.nn.functional.pad(hi, (0, pad)), torch.nn.functional.pad(lo, (0, pad))
+    return gemm(dy, hi, lo)
+
+
+def linear_wgrad(x, dy, want_bias: bool):
+    """-> (dW (N,K), db (N) or None): dW = dY^T X, db = sum_rows dY (regtr_linear_wgrad)."""
+    L = _lib.load()
+    M, K = x.shape
+    N = dy.shape[1]
+    dw = torch.empty((N, K), dtype=torch.float32, device=x.device)
+    db = torch.empty(N, dtype=torch.float32, device=x.device) if want_bias else None
+    ws = workspace(L.regtr_linear_wgrad_ws_bytes(M, N, K), x.device, 'wgrad')
+    _lib.check(L.regtr_linear_wgrad(_p(x), x.stride(0), _p(dy), dy.stride(0), M, N, K, _p(dw), _p(db), _p(ws),
+                                    ws.numel(), _stream()), 'regtr_linear_wgrad')
+    _count(4 + (L.regtr_gemm_ws_bytes(N, (K + 4) // 4 * 4, (M + 3) // 4 * 4) > 256))
+    return dw, db
+
+
+class _LinearFn(torch.autograd.Function):
+    """act(x W^T + b + residual); backward on regtr_relu_bwd, the 3xTF32 GEMM (dX) and regtr_linear_wgrad."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual, relu):
+        out = _linear_fwd(x, weight, bias, residual, relu)
+        ctx.save_for_backward(x, out if relu else None)
+        ctx.weight, ctx.relu, ctx.has_bias = weight, relu, bias is not None   # the parameter itself: split cache
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x, out = ctx.saved_tensors
+        g = g.contiguous()
+        if ctx.relu:
+            g = relu_bwd(g, out)
+        need = ctx.needs_input_grad
+        dx = linear_dgrad(g, ctx.weight) if need[0] else None
+        dw = db = None
+        if need[1] or need[2]:
+            dw, db = linear_wgrad(x, g, ctx.has_bias and need[2])
+        return dx, (dw if need[1] else None), db, (g if need[3] else None), None
+
+
+class _LayerNormPosFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, gamma, beta, pos, eps, want_plain, want_pos, skip):
+        ctx.set_materialize_grads(False)
+        y, yp = _layernorm_pos_fwd(x, gamma, beta, pos, eps, want_plain, want_pos)
+        ctx.save_for_backward(x, gamma)
+        ctx.eps = eps
+        return y, yp, (x if skip else None)
+
+    @staticmethod
+    def backward(ctx, dy, dyp, dres):
+        x, gamma = ctx.saved_tensors
+        c = lambda t: None if t is None else t.contiguous()
+        dx, dg, db = layernorm_bwd(x, gamma, c(dy), c(dyp), c(dres), ctx.eps)
+        need = ctx.needs_input_grad
+        return (dx if need[0] else None), (dg if need[1] else None), (db if need[2] else None), \
+            None, None, None, None, None
+
+
+class _MHAPackedFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, qkv, q_start, q_len, k_start, k_len, max_len, n_heads):
+        E = qkv.shape[1] // 3
+        o, lse = mha_varlen_lse(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], q_start, q_len, k_start, k_len, max_len,
+                                n_heads)
+        ctx.save_for_backward(qkv, o, lse, q_start, q_len, k_start, k_len)
+        ctx.max_len, ctx.n_heads = max_len, n_heads
+        return o
+
+    @staticmethod
+    def backward(ctx, g):
+        qkv, o, lse, qs, ql, ks, kl = ctx.saved_tensors
+        E = qkv.shape[1] // 3
+        d = torch.zeros_like(qkv)            # rows outside every problem keep a zero gradient
+        mha_varlen_bwd(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], o, lse, g.contiguous(), d[:, :E], d[:, E:2 * E],
+                       d[:, 2 * E:], qs, ql, ks, kl, ctx.max_len, ctx.max_len, ctx.n_heads)
+        return d, None, None, None, None, None, None
 
 
 # --------------------------------------------------------------------------- pose

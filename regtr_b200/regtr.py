@@ -14,7 +14,9 @@ What differs from the reference is *how*: packed tokens instead of padded ones, 
 sync for the pyramid sizes, hand-written sm_90a kernels for the neighbour search, the
 KPConv gather/aggregation, normalisations, attention core and Kabsch, and a fused
 correspondence-assembly + sigmoid + Kabsch kernel (regtr.py:185-203 in one launch).
-Training (`compute_loss`, autograd through the custom kernels) is a "next" row.
+`forward_train(batch)` is the differentiable variant for fine-tuning everything after the KPConv encoder (the
+encoder runs without grad and must be frozen); `compute_loss` of its outputs is differentiable, and the backward
+runs on the library's backward kernels (attention, LayerNorm, dense layers).  The encoder backward is not built yet.
 """
 from __future__ import annotations
 
@@ -182,12 +184,65 @@ class RegTR(nn.Module):
         }
 
     def compute_loss(self, pred, batch):
-        """Loss VALUES of a forward (regtr.py:237-294: overlap BCE, InfoNCE feature losses, L1 correspondence
-        loss, weighted total) as `test_step` reports them; forward-only -- gradients do not flow into the CUDA
-        kernels yet (SURVEY.md 8f N3).  Needs batch['pose'], ['src_overlap'], ['tgt_overlap'], ['kpconv_meta']."""
+        """Losses of a forward (regtr.py:237-294: overlap BCE, InfoNCE feature losses, L1 correspondence loss,
+        weighted total).  For outputs of `forward_train` (which carry autograd history) `total` is differentiable;
+        for outputs of `forward` the values are computed without grad, as `test_step` reports them.
+        Needs batch['pose'], ['src_overlap'], ['tgt_overlap'], ['kpconv_meta']."""
         from . import losses
+        if torch.is_grad_enabled() and pred['src_feat'][0].requires_grad:
+            return losses.compute_loss(self, pred, batch)
         with torch.no_grad():
             return losses.compute_loss(self, pred, batch)
+
+    def _check_trainable(self):
+        """forward_train covers the branches both reference configs select; anything else raises."""
+        cfg = self.cfg
+        if any(p.requires_grad for p in self.kpf_encoder.parameters()):
+            raise ValueError('forward_train: the KPConv encoder has no backward yet; freeze it first with '
+                             'model.kpf_encoder.requires_grad_(False)')
+        unsupported = []
+        if not cfg.pre_norm:
+            unsupported.append('pre_norm=False')
+        if not cfg.get('direct_regress_coor', False):
+            unsupported.append('direct_regress_coor=False (CorrespondenceDecoder)')
+        if cfg.get('pos_emb_type', 'sine') != 'sine':
+            unsupported.append(f"pos_emb_type={cfg['pos_emb_type']!r}")
+        if not (cfg.sa_val_has_pos_emb and cfg.ca_val_has_pos_emb):
+            unsupported.append('sa/ca_val_has_pos_emb=False')
+        if cfg.get('attention_impl', 'fp32') != 'fp32':
+            unsupported.append(f"attention_impl={cfg['attention_impl']!r}")
+        if unsupported:
+            raise NotImplementedError('forward_train: no backward for ' + ', '.join(unsupported))
+
+    def _stage_attention_train(self, feats_un, xyz_c, offs_c, B: int, plan: AttentionPlan):
+        """Differentiable stages after the encoder: feature projection, cross-encoder, correspondence heads.
+        The position embedding and the pose carry no gradient (the reference loss does not use the pose)."""
+        cfg = self.cfg
+        both_un = ops.linear(feats_un, self.feat_proj.weight, self.feat_proj.bias)             # regtr.py:145
+        with torch.no_grad():
+            pe = self.pos_embed(xyz_c)
+        cond = self.transformer_encoder.forward_train_packed(
+            both_un, pe if cfg.transformer_encoder_has_pos_emb else None, plan)
+        corr, logit = self.correspondence_decoder.forward_packed(cond, xyz_c, pe, plan)
+        with torch.no_grad():
+            pose = ops.pose_from_corr(xyz_c, corr.detach().contiguous(), logit.detach()[..., 0].contiguous(), offs_c, B)
+        return dict(both_un=both_un, xyz_c=xyz_c, cond=cond, corr=corr, logit=logit, pose=pose)
+
+    def forward_train(self, batch):
+        """`forward` with autograd: same output dict, whose src/tgt_feat(_un), *_kp_warped and *_overlap carry
+        history back to every parameter after the KPConv encoder.  The pyramid and the encoder run without grad
+        (freeze the encoder: model.kpf_encoder.requires_grad_(False)).  Exact shapes, eager only."""
+        self._check_trainable()
+        B = len(batch['src_xyz'])
+        with torch.no_grad():
+            meta = self.preprocessor(list(batch['src_xyz']) + list(batch['tgt_xyz']), lazy_upsamples=True)
+            batch['kpconv_meta'] = meta
+            pts = meta['_points']
+            feats_un, _ = self.kpf_encoder(torch.ones_like(pts[0][:, 0:1]), meta)             # regtr.py:122-136
+        lens_c = meta['_lens'][-1]
+        plan = AttentionPlan(lens_c, pts[-1].device)
+        core = self._stage_attention_train(feats_un, pts[-1], meta['_offs'][-1], B, plan)
+        return self._assemble(core, lens_c, B)
 
     @torch.no_grad()
     def forward(self, batch):

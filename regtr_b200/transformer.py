@@ -204,6 +204,24 @@ class TransformerCrossEncoderLayer(nn.Module):
         return x
 
 
+    def forward_train_packed(self, x, pos, plan: AttentionPlan):
+        """Differentiable pre-norm layer (exact shapes) for the branches both reference configs select: pre-norm,
+        values carrying the position embedding, the default 3xTF32 attention core.  Same math as `forward_packed`;
+        every LayerNorm also hands x on to the residual add that follows it (layernorm_pos(skip=True)), so the
+        residual gradient is added inside the LayerNorm backward."""
+        has_pos = pos is not None
+        for mha, norm, cross in ((self.self_attn, self.norm1, False), (self.multihead_attn, self.norm2, True)):
+            y, yp, x = ops.layernorm_pos(x, norm.weight, norm.bias, pos, norm.eps, want_plain=not has_pos,
+                                         want_pos=has_pos, skip=True)
+            qkv = ops.linear(yp if has_pos else y, mha.in_proj_weight, mha.in_proj_bias)
+            ks, kl = (plan.xk_start, plan.xk_len) if cross else (plan.q_start, plan.q_len)
+            o = ops.mha_packed(qkv, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead)
+            x = ops.linear(o, mha.out_proj.weight, mha.out_proj.bias, residual=x)
+        x2, _, x = ops.layernorm_pos(x, self.norm3.weight, self.norm3.bias, None, self.norm3.eps,
+                                     want_plain=True, want_pos=False, skip=True)
+        h = ops.linear(x2, self.linear1.weight, self.linear1.bias, relu=True)
+        return ops.linear(h, self.linear2.weight, self.linear2.bias, residual=x)
+
     def forward_post_packed(self, x, pos, plan: AttentionPlan):
         """Post-norm layer (transformers.py:121-181): attention on x (+pos), then LayerNorm(x + update)."""
         has_pos = pos is not None
@@ -246,6 +264,16 @@ class TransformerCrossEncoder(nn.Module):
                 outs.append(self._final(x, plan.n_dev))
         if not self.return_intermediate:
             outs.append(self._final(x, plan.n_dev))
+        return torch.stack(outs)
+
+    def forward_train_packed(self, x, pos, plan: AttentionPlan):
+        """Differentiable `forward_packed` (pre-norm layers with a final norm, return_intermediate): -> (L, N, E).
+        The final norm of each intermediate output passes x on to the next layer (skip=True)."""
+        outs = []
+        for layer in self.layers:
+            x = layer.forward_train_packed(x, pos, plan)
+            y, _, x = ops.layernorm_pos(x, self.norm.weight, self.norm.bias, None, self.norm.eps, True, False, skip=True)
+            outs.append(y)
         return torch.stack(outs)
 
     def _final(self, x, n_dev=None):
