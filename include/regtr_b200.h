@@ -308,6 +308,56 @@ size_t regtr_linear_wgrad_ws_bytes(int M, int N, int K);
 int regtr_linear_wgrad(const float* X, int ldx, const float* dY, int ldy, int M, int N, int K,
                        float* dW, float* db, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- backward of the KPConv encoder (training with the encoder) --------------------- */
+
+/* Transpose of a neighbour list: the incoming edges of every support row as CSR.  idx (Nq,K) i32 with shadow
+ * index Ns (any entry outside [0, Ns) is a shadow slot and is left out) -> row_start (Ns+1) i32 and
+ * edges (Nq*K capacity) i32 = edge ids q*K + k, ascending inside each row (rows in support order).  The edge
+ * order does not depend on scheduling.  The gather-scatter of the KPConv (kpconv_blocks.py:388-391) and of
+ * max_pool (kpconv_blocks.py:138-141) read their lists through it in the backward, so that every support row
+ * sums its gradient contributions itself: no floating-point atomics.
+ * ws: regtr_neighbor_csr_ws_bytes(Ns) bytes (per-row counters, contents irrelevant on entry). */
+size_t regtr_neighbor_csr_ws_bytes(int Ns);
+int regtr_neighbor_csr(const int32_t* idx, int Nq, int K, int Ns, int32_t* row_start, int32_t* edges,
+                       void* ws, size_t ws_bytes, void* stream);
+
+/* Input gradient of the rigid KPConv (kpconv_blocks.py:388-412) given dwf = dOut W^T (Nq, 15*Cin), the
+ * gradient of the aggregated features (compute it with regtr_gemm_tf32x3 and W viewed as (15*Cin, Cout)):
+ *   dx[s] = sum_{(q,k): idx[q,k]=s} (1/cnt_q) sum_p h(q,k,p) dwf[q,p,:]
+ * h is recomputed exactly as regtr_kpconv_aggregate computes it; cnt_q = max(1, #valid neighbours whose
+ * feature row sums to > 0) carries no gradient.  flags (Ns bytes, optional): the forward's row flags (as
+ * regtr_kpconv_aggregate's rowflag_ws); NULL recomputes them from x.  row_start / edges: regtr_neighbor_csr of
+ * idx.  dx (Ns, Cin), every row written (0 for supports no query references).  Cin <= 256, K <= 128.
+ * ws: regtr_kpconv_bwd_input_ws_bytes(Nq, K, Cin) bytes: one (1/cnt_q) h^T dwf[q] row per edge, then summed
+ * per support in CSR order (2 * nnz * Cin * 4 bytes of traffic). */
+size_t regtr_kpconv_bwd_input_ws_bytes(int Nq, int K, int Cin);
+int regtr_kpconv_bwd_input(const float* q, const float* s, const int32_t* idx, const float* x,
+                           const uint8_t* flags, const float* kp, int Nq, int Ns, int K, int Cin, float extent,
+                           const float* dwf, const int32_t* row_start, const int32_t* edges, float* dx,
+                           void* ws, size_t ws_bytes, void* stream);
+
+/* Backward of regtr_max_pool (kpconv_blocks.py:127-143): the gradient of out[q,c] goes to the first maximal
+ * entry in neighbour order (torch.max(dim)'s tie rule); the zero shadow row is a candidate and gradient routed
+ * to it is dropped.  x (Ns,C) the pooled input, idx (Nq,K) i32, dout (Nq,C), row_start / edges its
+ * regtr_neighbor_csr -> dx (Ns,C), every row written.  K <= 255.
+ * ws: regtr_max_pool_bwd_ws_bytes(Nq, C) bytes (the arg-max slot per output entry). */
+size_t regtr_max_pool_bwd_ws_bytes(int Nq, int C);
+int regtr_max_pool_bwd(const float* x, const int32_t* idx, int Nq, int Ns, int K, int C, const float* dout,
+                       const int32_t* row_start, const int32_t* edges, float* dx, void* ws, size_t ws_bytes,
+                       void* stream);
+
+/* Backward of regtr_instnorm_act / regtr_instnorm_apply, out = act(norm(x) + res)
+ * (kpconv_blocks.py:497-519, 546-561, 646, 741).  g (n,C) the gradient of out; out is read for the LeakyReLU
+ * mask (g' = g * (out > 0 ? 1 : slope)) and may be NULL when slope < 0 (no activation).
+ *   dx = rstd (g' - mean_cloud(g') - xh mean_cloud(g' xh)),  xh = (x - mean) rstd;   dres = g' (optional).
+ * mean / rstd are recomputed from x in fp64 (fixed 128-row chunks inside each cloud, added in order), so the
+ * result does not depend on which forward entry produced the statistics.  A one-point cloud gets dx = 0; rows
+ * beyond offs[n_clouds] get zeros.  C % 4 == 0.  ws: regtr_instnorm_bwd_ws_bytes(n, n_clouds, C) bytes. */
+size_t regtr_instnorm_bwd_ws_bytes(int n, int n_clouds, int C);
+int regtr_instnorm_bwd(const float* g, const float* x, const float* out, const int32_t* offs, int n_clouds,
+                       int n, int C, float eps, float slope, float* dx, float* dres,
+                       void* ws, size_t ws_bytes, void* stream);
+
 /* ---- pose ------------------------------------------------------------------------- */
 
 /* Weighted Kabsch.  Replaces compute_rigid_transform (utils/se3_torch.py:108-154):

@@ -304,7 +304,8 @@ class BatchNormBlock(nn.Module):
         return F.leaky_relu(y, slope) if slope >= 0 else y
 
     def apply(self, x, stats, offs, n_clouds, res=None, slope=-1.0, want_flags=False):
-        """Normalise with statistics that the producing GEMM accumulated in its epilogue."""
+        """Normalise with statistics that the producing GEMM accumulated in its epilogue (differentiable in x and
+        res: the backward recomputes the statistics from x)."""
         return ops.instnorm_apply(x, offs, n_clouds, stats, res=res, slope=slope, want_flags=want_flags)
 
     def forward(self, x, stack_lengths):
@@ -321,14 +322,21 @@ class UnaryBlock(nn.Module):
         self.mlp = nn.Linear(in_dim, out_dim, bias=False)
         self.batch_norm = BatchNormBlock(out_dim, use_bn, bn_momentum)
 
-    def fuse(self, x, offs, n_clouds, res=None, final_slope=None, m_dev=None, want_flags=False):
+    def fuse(self, x, offs, n_clouds, res=None, final_slope=None, m_dev=None, want_flags=False, skip=False):
+        """skip=True also returns x, as the last element, for the block's shortcut branch: in training its gradient
+        is then added in this layer's dX GEMM (ops.linear_instats) instead of by autograd."""
         slope = final_slope if final_slope is not None else (-1.0 if self.no_relu else 0.1)
         if self.use_bn and self.out_dim % 32 == 0 and EPILOGUE_STATS:
             # Linear with the InstanceNorm statistics accumulated in the GEMM epilogue, then the apply pass
-            y, stats = ops.linear_instats(x, self.mlp.weight, offs, n_clouds, m_dev=m_dev)
-            return self.batch_norm.apply(y, stats, offs, n_clouds, res=res, slope=slope, want_flags=want_flags)
-        return self.batch_norm.fuse(ops.linear(x, self.mlp.weight, m_dev=m_dev), offs, n_clouds, res=res,
-                                    slope=slope, want_flags=want_flags)
+            y, stats, *xs = ops.linear_instats(x, self.mlp.weight, offs, n_clouds, m_dev=m_dev, skip=skip)
+            out = self.batch_norm.apply(y, stats, offs, n_clouds, res=res, slope=slope, want_flags=want_flags)
+        else:
+            xs = [x]
+            out = self.batch_norm.fuse(ops.linear(x, self.mlp.weight, m_dev=m_dev), offs, n_clouds, res=res,
+                                       slope=slope, want_flags=want_flags)
+        if not skip:
+            return out
+        return (*out, xs[0]) if want_flags else (out, xs[0])
 
     def forward(self, x, stack_lengths=None):
         offs = ops.make_offsets(stack_lengths, x.device)
@@ -393,8 +401,9 @@ class ResnetBottleneckBlock(nn.Module):
         q, s, idx, offs_pre, offs_post, nq_dev, ns_dev, nc = _block_io(self, batch)
         flags = None
         if isinstance(self.unary1, UnaryBlock) and self.use_bn:
-            # the normalisation pass also emits the KPConv's "row sums to > 0" neighbour-count flags
-            x, flags = self.unary1.fuse(features, offs_pre, nc, m_dev=ns_dev, want_flags=True)
+            # the normalisation pass also emits the KPConv's "row sums to > 0" neighbour-count flags; `features`
+            # continues as unary1's skip output, so that the shortcut's gradient joins unary1's dX in one GEMM
+            x, flags, features = self.unary1.fuse(features, offs_pre, nc, m_dev=ns_dev, want_flags=True, skip=True)
         else:
             x = self.unary1.fuse(features, offs_pre, nc, m_dev=ns_dev) if isinstance(self.unary1, UnaryBlock) \
                 else features

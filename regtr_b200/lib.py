@@ -73,6 +73,14 @@ SIGNATURES = {
     'regtr_relu_bwd': (_I, [_P, _P, _c.c_longlong, _P, _P]),
     'regtr_linear_wgrad_ws_bytes': (_Z, [_I, _I, _I]),
     'regtr_linear_wgrad': (_I, [_P, _I, _P, _I, _I, _I, _I, _P, _P, _P, _Z, _P]),
+    'regtr_neighbor_csr_ws_bytes': (_Z, [_I]),
+    'regtr_neighbor_csr': (_I, [_P, _I, _I, _I, _P, _P, _P, _Z, _P]),
+    'regtr_kpconv_bwd_input_ws_bytes': (_Z, [_I, _I, _I]),
+    'regtr_kpconv_bwd_input': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P, _P, _P, _P, _P, _Z, _P]),
+    'regtr_max_pool_bwd_ws_bytes': (_Z, [_I, _I]),
+    'regtr_max_pool_bwd': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _Z, _P]),
+    'regtr_instnorm_bwd_ws_bytes': (_Z, [_I, _I, _I]),
+    'regtr_instnorm_bwd': (_I, [_P, _P, _P, _P, _I, _I, _I, _F, _F, _P, _P, _P, _Z, _P]),
     'regtr_kabsch_fwd': (_I, [_P, _P, _P, _P, _I, _P, _P]),
     'regtr_pose_from_corr': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),

@@ -191,7 +191,19 @@ def kpconv(q_pts, s_pts, idx32, x, weights, kernel_points, extent: float, out=No
            row_flags=None, instats=None):
     """KPConv.forward (rigid / linear / sum).  idx32 (Nq,K) int32, x (Ns,Cin) -> (Nq,Cout).
     nq_dev / ns_dev: optional 1-element int32 device tensors with the actual counts when the
-    leading dimensions are capacities."""
+    leading dimensions are capacities.
+    Differentiable with respect to x and weights (_KPConvFn) when grad mode is on and either requires grad (exact
+    shapes only); kernel_points and the coordinates carry no gradient."""
+    if _wants_grad(x, weights):
+        if out is not None or nq_dev is not None or ns_dev is not None:
+            raise ValueError('kpconv: the backward needs exact shapes (no out / nq_dev / ns_dev)')
+        out, stats = _KPConvFn.apply(x, weights, q_pts, s_pts, idx32, kernel_points, float(extent), row_flags, instats)
+        return out if instats is None else (out, stats)
+    return _kpconv_fwd(q_pts, s_pts, idx32, x, weights, kernel_points, extent, out, nq_dev, ns_dev, row_flags, instats)
+
+
+def _kpconv_fwd(q_pts, s_pts, idx32, x, weights, kernel_points, extent: float, out=None, nq_dev=None, ns_dev=None,
+                row_flags=None, instats=None):
     L = _lib.load()
     _chk(q_pts, torch.float32, 'q_pts', 2); _chk(s_pts, torch.float32, 's_pts', 2)
     _chk(idx32, torch.int32, 'neighb_inds', 2); _chk(x, torch.float32, 'x', 2)
@@ -260,6 +272,16 @@ def kpconv_aggregate(q_pts, s_pts, idx32, x, kernel_points, extent: float, wf=No
 
 
 def max_pool(x, idx32, ns_dev=None):
+    """max over the K gathered rows with a zero shadow row.  Differentiable (_MaxPoolFn) when grad mode is on and x
+    requires grad (exact shapes only)."""
+    if _wants_grad(x):
+        if ns_dev is not None:
+            raise ValueError('max_pool: the backward needs exact shapes (no ns_dev)')
+        return _MaxPoolFn.apply(x, idx32)
+    return _max_pool_fwd(x, idx32, ns_dev)
+
+
+def _max_pool_fwd(x, idx32, ns_dev=None):
     L = _lib.load()
     _chk(x, torch.float32, 'x', 2); _chk(idx32, torch.int32, 'inds', 2)
     Nq, K = idx32.shape
@@ -273,7 +295,18 @@ def max_pool(x, idx32, ns_dev=None):
 def instnorm_act(x, offs, n_clouds: int, res=None, slope: float = -1.0, eps: float = 1e-5, out=None,
                  want_flags: bool = False):
     """out = act(InstanceNorm_per_cloud(x) + res); slope < 0 -> no activation.
-    want_flags: also return the per-row `sum > 0` flags the consuming KPConv needs (uint8, n rows)."""
+    want_flags: also return the per-row `sum > 0` flags the consuming KPConv needs (uint8, n rows).
+    Differentiable with respect to x and res (_InstNormFn) when grad mode is on and either requires grad."""
+    if _wants_grad(x, res):
+        if out is not None:
+            raise ValueError('instnorm_act: no out= on the differentiable path')
+        y, flags = _InstNormFn.apply(x, res, None, offs, n_clouds, float(slope), float(eps), bool(want_flags))
+        return (y, flags) if want_flags else y
+    return _instnorm_act_fwd(x, offs, n_clouds, res, slope, eps, out, want_flags)
+
+
+def _instnorm_act_fwd(x, offs, n_clouds: int, res=None, slope: float = -1.0, eps: float = 1e-5, out=None,
+                      want_flags: bool = False):
     L = _lib.load()
     _chk(x, torch.float32, 'x', 2); _chk(offs, torch.int32, 'offs', 1)
     n, C = x.shape
@@ -293,9 +326,22 @@ def instnorm_act(x, offs, n_clouds: int, res=None, slope: float = -1.0, eps: flo
     return (out, flags) if want_flags else out
 
 
-def instnorm_apply(x, offs, n_clouds: int, stats, res=None, slope: float = -1.0, out=None, want_flags: bool = False):
+def instnorm_apply(x, offs, n_clouds: int, stats, res=None, slope: float = -1.0, out=None, want_flags: bool = False,
+                   eps: float = 1e-5):
     """Apply pass of the per-cloud InstanceNorm with statistics from `gemm_instats`:
-    out = act((x - mean) * rstd + res)."""
+    out = act((x - mean) * rstd + res).  Differentiable with respect to x and res (_InstNormFn) when grad mode is on
+    and either requires grad: the statistics are functions of x, and the backward recomputes them from x (`eps` must
+    be the one they were computed with)."""
+    if _wants_grad(x, res):
+        if out is not None:
+            raise ValueError('instnorm_apply: no out= on the differentiable path')
+        y, flags = _InstNormFn.apply(x, res, stats, offs, n_clouds, float(slope), float(eps), bool(want_flags))
+        return (y, flags) if want_flags else y
+    return _instnorm_apply_fwd(x, offs, n_clouds, stats, res, slope, out, want_flags)
+
+
+def _instnorm_apply_fwd(x, offs, n_clouds: int, stats, res=None, slope: float = -1.0, out=None,
+                        want_flags: bool = False):
     L = _lib.load()
     _chk(x, torch.float32, 'x', 2); _chk(offs, torch.int32, 'offs', 1); _chk(stats, torch.float32, 'stats', 3)
     n, C = x.shape
@@ -376,8 +422,21 @@ def gemm_instats(a, b_hi, b_lo, offs, n_clouds: int, eps: float = 1e-5, m_dev=No
     return out, stats
 
 
-def linear_instats(x, weight, offs, n_clouds: int, eps: float = 1e-5, m_dev=None):
-    """nn.Linear(bias=False) followed by InstanceNorm statistics (UnaryBlock, kpconv_blocks.py:546-561)."""
+def linear_instats(x, weight, offs, n_clouds: int, eps: float = 1e-5, m_dev=None, skip: bool = False):
+    """nn.Linear(bias=False) followed by InstanceNorm statistics (UnaryBlock, kpconv_blocks.py:546-561).
+    Differentiable with respect to x and weight (_LinearInstatsFn) when grad mode is on and either requires grad.
+    skip=True also returns x itself as a third output, for the block's shortcut branch: its gradient then reaches the
+    dX GEMM as a residual and is added in the epilogue, so x has one consumer in the autograd graph."""
+    if _wants_grad(x, weight):
+        if m_dev is not None:
+            raise ValueError('linear_instats: the backward needs exact shapes (no m_dev)')
+        y, stats, xs = _LinearInstatsFn.apply(x, weight, offs, n_clouds, float(eps), bool(skip))
+        return (y, stats, xs) if skip else (y, stats)
+    y, stats = _linear_instats_fwd(x, weight, offs, n_clouds, eps, m_dev)
+    return (y, stats, x) if skip else (y, stats)
+
+
+def _linear_instats_fwd(x, weight, offs, n_clouds: int, eps: float = 1e-5, m_dev=None):
     if x.shape[1] % 4 or x.stride(0) % 4 or x.data_ptr() % 16:
         raise _lib.RegtrLibError(f'linear: K={x.shape[1]}: rows must be 16-byte aligned multiples of 4 floats')
     hi, lo = split_weight(weight)
@@ -646,15 +705,15 @@ def relu_bwd(dh, h):
     return out
 
 
-def linear_dgrad(dy, weight):
-    """dX = dY @ W on the 3xTF32 GEMM with the transposed pre-split weight.  N_out % 4 != 0 (the 3- and 1-wide heads) zero-pads dY and W^T to the TMA row pitch."""
+def linear_dgrad(dy, weight, residual=None):
+    """dX = dY @ W (+ residual, added in the epilogue) on the 3xTF32 GEMM with the transposed pre-split weight.  N_out % 4 != 0 (the 3- and 1-wide heads) zero-pads dY and W^T to the TMA row pitch."""
     N = weight.shape[0]
     hi, lo = split_weight(weight, transpose=True)            # (K, N)
     pad = (-N) % 4
     if pad:
         dy = torch.nn.functional.pad(dy, (0, pad))
         hi, lo = torch.nn.functional.pad(hi, (0, pad)), torch.nn.functional.pad(lo, (0, pad))
-    return gemm(dy, hi, lo)
+    return gemm(dy, hi, lo, residual=residual)
 
 
 def linear_wgrad(x, dy, want_bias: bool):
@@ -732,6 +791,196 @@ class _MHAPackedFn(torch.autograd.Function):
         mha_varlen_bwd(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], o, lse, g.contiguous(), d[:, :E], d[:, E:2 * E],
                        d[:, 2 * E:], qs, ql, ks, kl, ctx.max_len, ctx.max_len, ctx.n_heads)
         return d, None, None, None, None, None, None
+
+
+# ------------------------------------------------------------------ encoder backward
+
+def neighbor_csr(idx32, Ns: int):
+    """Incoming-edge CSR of a neighbour list (regtr_neighbor_csr) -> (row_start (Ns+1), edges (Nq*K)) int32.
+    Cached on the index tensor itself, so the blocks that share a list in one training step (every block of a level
+    shares its conv list; a strided block's KPConv and max-pool share its pool list) build it once."""
+    L = _lib.load()
+    _chk(idx32, torch.int32, 'neighb_inds', 2)
+    cache = idx32.__dict__.setdefault('_regtr_csr', {})
+    key = (int(Ns), idx32._version)
+    hit = cache.get(key)
+    if hit is not None:
+        return hit
+    Nq, K = idx32.shape
+    row_start = torch.empty(Ns + 1, dtype=torch.int32, device=idx32.device)
+    edges = torch.empty(max(Nq * K, 1), dtype=torch.int32, device=idx32.device)
+    ws = workspace(L.regtr_neighbor_csr_ws_bytes(Ns), idx32.device, 'csr')
+    _lib.check(L.regtr_neighbor_csr(_p(idx32), Nq, K, Ns, _p(row_start), _p(edges), _p(ws), ws.numel(), _stream()),
+               'regtr_neighbor_csr')
+    _count(5)
+    cache.clear()
+    cache[key] = (row_start, edges)
+    return row_start, edges
+
+
+def kpconv_bwd_input(q_pts, s_pts, idx32, x, flags, kernel_points, extent: float, dwf, csr):
+    """dx (Ns, Cin) of the KPConv from dwf = dOut W^T (Nq, 15 Cin); flags: the forward's row flags or None."""
+    L = _lib.load()
+    Nq, K = idx32.shape
+    Ns, Cin = x.shape
+    _chk(dwf, torch.float32, 'dwf', 2)
+    dx = torch.empty_like(x)
+    ws = workspace(L.regtr_kpconv_bwd_input_ws_bytes(Nq, K, Cin), x.device, 'kpconv_bwd')
+    _lib.check(L.regtr_kpconv_bwd_input(_p(q_pts), _p(s_pts), _p(idx32), _p(x), _p(flags), _p(kernel_points), Nq, Ns,
+                                        K, Cin, float(extent), _p(dwf), _p(csr[0]), _p(csr[1]), _p(dx), _p(ws),
+                                        ws.numel(), _stream()), 'regtr_kpconv_bwd_input')
+    _count(2)
+    return dx
+
+
+def max_pool_bwd(x, idx32, dout, csr):
+    L = _lib.load()
+    Nq, K = idx32.shape
+    Ns, C = x.shape
+    _chk(dout, torch.float32, 'dout', 2)
+    dx = torch.empty_like(x)
+    ws = workspace(L.regtr_max_pool_bwd_ws_bytes(Nq, C), x.device, 'maxpool_bwd')
+    _lib.check(L.regtr_max_pool_bwd(_p(x), _p(idx32), Nq, Ns, K, C, _p(dout), _p(csr[0]), _p(csr[1]), _p(dx), _p(ws),
+                                    ws.numel(), _stream()), 'regtr_max_pool_bwd')
+    _count(2)
+    return dx
+
+
+def instnorm_bwd(g, x, out, offs, n_clouds: int, slope: float, eps: float = 1e-5, want_dres: bool = False):
+    """-> (dx, dres or None) of out = act(InstanceNorm_per_cloud(x) + res) (regtr_instnorm_bwd)."""
+    L = _lib.load()
+    _chk(g, torch.float32, 'g', 2); _chk(x, torch.float32, 'x', 2); _chk(offs, torch.int32, 'offs', 1)
+    n, C = x.shape
+    dx = torch.empty_like(x)
+    dres = torch.empty_like(x) if want_dres else None
+    ws = workspace(L.regtr_instnorm_bwd_ws_bytes(n, n_clouds, C), x.device, 'instnorm_bwd')
+    _lib.check(L.regtr_instnorm_bwd(_p(g), _p(x), _p(out if slope >= 0 else None), _p(offs), n_clouds, n, C,
+                                    float(eps), float(slope), _p(dx), _p(dres), _p(ws), ws.numel(), _stream()),
+               'regtr_instnorm_bwd')
+    _count(3)
+    return dx, dres
+
+
+def _kpconv_wf(q_pts, s_pts, idx32, x, kernel_points, extent: float, row_flags):
+    """Recompute the forward's aggregated features wf (Nq, 15 Cin) for the weight gradient; -> (wf, row flags used by
+    the count, or None for Cin = 1, whose aggregation counts from x itself)."""
+    L = _lib.load()
+    Nq, K = idx32.shape
+    Ns, Cin = x.shape
+    wf = torch.empty((Nq, 15 * Cin), dtype=torch.float32, device=x.device)
+    flags = row_flags
+    if flags is None:       # computed by the aggregation (Cin > 1); Cin = 1 never touches it
+        flags = torch.empty(max(Ns, 1) if Cin > 1 else 1, dtype=torch.uint8, device=x.device)
+    _lib.check(L.regtr_kpconv_aggregate(_p(q_pts), _p(s_pts), _p(idx32), _p(x), _p(kernel_points), Nq, Ns, None, None,
+                                        K, Cin, float(extent), _p(wf), _p(flags), 1 if row_flags is not None else 0,
+                                        _stream()), 'regtr_kpconv_aggregate')
+    _count(1 if (row_flags is not None or Cin == 1) else 2)
+    return wf, (flags if Cin > 1 else None)
+
+
+class _KPConvFn(torch.autograd.Function):
+    """KPConv forward (the fused C1 kernel, or the aggregation + contraction GEMM with optional statistics epilogue).
+    Backward: wf recomputed by regtr_kpconv_aggregate, dW = wf^T dOut (regtr_linear_wgrad), dwf = dOut W^T (3xTF32
+    GEMM), dx by regtr_kpconv_bwd_input through the list's CSR."""
+
+    @staticmethod
+    def forward(ctx, x, weights, q_pts, s_pts, idx32, kernel_points, extent, row_flags, instats):
+        ctx.set_materialize_grads(False)
+        r = _kpconv_fwd(q_pts, s_pts, idx32, x, weights, kernel_points, extent, row_flags=row_flags, instats=instats)
+        out, stats = r if instats is not None else (r, None)
+        ctx.save_for_backward(x, q_pts, s_pts, kernel_points, row_flags)
+        ctx.idx, ctx.weights, ctx.extent = idx32, weights, extent     # idx: the CSR cache lives on this object
+        if stats is not None:
+            ctx.mark_non_differentiable(stats)
+        return out, stats
+
+    @staticmethod
+    def backward(ctx, g, _gstats):
+        x, q_pts, s_pts, kp, row_flags = ctx.saved_tensors
+        need_x, need_w = ctx.needs_input_grad[:2]
+        dx = dw = None
+        if g is None:
+            return (None,) * 9
+        g = g.contiguous()
+        Ns, Cin = x.shape
+        Cout = ctx.weights.shape[2]
+        flags = row_flags
+        if need_w:
+            wf, flags = _kpconv_wf(q_pts, s_pts, ctx.idx, x, kp, ctx.extent, row_flags)
+            dw = linear_wgrad(g, wf, False)[0].view(15, Cin, Cout)       # (15 Cin, Cout) = wf^T dOut
+        if need_x:
+            hi, lo = split_weight(ctx.weights.view(15 * Cin, Cout))
+            dwf = gemm(g, hi, lo)
+            dx = kpconv_bwd_input(q_pts, s_pts, ctx.idx, x, flags, kp, ctx.extent, dwf, neighbor_csr(ctx.idx, Ns))
+        return dx, dw, None, None, None, None, None, None, None
+
+
+class _MaxPoolFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, idx32):
+        ctx.save_for_backward(x)
+        ctx.idx = idx32
+        return _max_pool_fwd(x, idx32)
+
+    @staticmethod
+    def backward(ctx, g):
+        x, = ctx.saved_tensors
+        return max_pool_bwd(x, ctx.idx, g.contiguous(), neighbor_csr(ctx.idx, x.shape[0])), None
+
+
+class _InstNormFn(torch.autograd.Function):
+    """act(InstanceNorm_per_cloud(x) + res); statistics from the producing GEMM's epilogue (stats) or computed here.
+    Backward on regtr_instnorm_bwd (statistics recomputed from x)."""
+
+    @staticmethod
+    def forward(ctx, x, res, stats, offs, n_clouds, slope, eps, want_flags):
+        ctx.set_materialize_grads(False)
+        if stats is None:
+            y, flags = _instnorm_act_fwd(x, offs, n_clouds, res=res, slope=slope, eps=eps, want_flags=True) \
+                if want_flags else (_instnorm_act_fwd(x, offs, n_clouds, res=res, slope=slope, eps=eps), None)
+        else:
+            y, flags = _instnorm_apply_fwd(x, offs, n_clouds, stats, res=res, slope=slope, want_flags=True) \
+                if want_flags else (_instnorm_apply_fwd(x, offs, n_clouds, stats, res=res, slope=slope), None)
+        ctx.save_for_backward(x, y if slope >= 0 else None, offs)
+        ctx.n_clouds, ctx.slope, ctx.eps = n_clouds, slope, eps
+        if flags is not None:
+            ctx.mark_non_differentiable(flags)
+        return y, flags
+
+    @staticmethod
+    def backward(ctx, g, _gflags):
+        if g is None:
+            return (None,) * 8
+        x, y, offs = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        dx, dres = instnorm_bwd(g.contiguous(), x, y, offs, ctx.n_clouds, ctx.slope, ctx.eps, want_dres=need[1])
+        return (dx if need[0] else None), dres, None, None, None, None, None, None
+
+
+class _LinearInstatsFn(torch.autograd.Function):
+    """x W^T plus the per-cloud InstanceNorm statistics of the result (non-differentiable: _InstNormFn's backward
+    differentiates through them).  Backward: dX on the 3xTF32 GEMM (+ the shortcut gradient of the skip output in its
+    epilogue), dW on regtr_linear_wgrad."""
+
+    @staticmethod
+    def forward(ctx, x, weight, offs, n_clouds, eps, skip):
+        ctx.set_materialize_grads(False)
+        y, stats = _linear_instats_fwd(x, weight, offs, n_clouds, eps)
+        ctx.save_for_backward(x)
+        ctx.weight = weight
+        ctx.mark_non_differentiable(stats)
+        return y, stats, (x if skip else None)
+
+    @staticmethod
+    def backward(ctx, g, _gstats, gskip):
+        x, = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        if g is None:
+            return gskip, None, None, None, None, None
+        g = g.contiguous()
+        dx = linear_dgrad(g, ctx.weight, residual=None if gskip is None else gskip.contiguous()) if need[0] else None
+        dw = linear_wgrad(x, g, False)[0] if need[1] else None
+        return dx, dw, None, None, None, None
 
 
 # --------------------------------------------------------------------------- pose

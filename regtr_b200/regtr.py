@@ -15,11 +15,13 @@ sync for the pyramid sizes, hand-written sm_90a kernels for the neighbour search
 KPConv gather/aggregation, normalisations, attention core and Kabsch, and a fused
 correspondence-assembly + sigmoid + Kabsch kernel (regtr.py:185-203 in one launch).
 `forward_train(batch)` is the differentiable variant for fine-tuning everything after the KPConv encoder (the
-encoder runs without grad and must be frozen); `compute_loss` of its outputs is differentiable, and the backward
-runs on the library's backward kernels (attention, LayerNorm, dense layers).  The encoder backward is not built yet.
+encoder runs without grad and must be frozen); `forward_train(batch, train_encoder=True)` trains the encoder as well.
+`compute_loss` of its outputs is differentiable, and the backward runs on the library's backward kernels (attention,
+LayerNorm, dense layers, and for the encoder KPConv, max-pool and per-cloud InstanceNorm).
 """
 from __future__ import annotations
 
+import contextlib
 import logging
 import time
 import weakref
@@ -194,12 +196,19 @@ class RegTR(nn.Module):
         with torch.no_grad():
             return losses.compute_loss(self, pred, batch)
 
-    def _check_trainable(self):
+    def _check_trainable(self, train_encoder: bool = False):
         """forward_train covers the branches both reference configs select; anything else raises."""
         cfg = self.cfg
-        if any(p.requires_grad for p in self.kpf_encoder.parameters()):
-            raise ValueError('forward_train: the KPConv encoder has no backward yet; freeze it first with '
-                             'model.kpf_encoder.requires_grad_(False)')
+        if not train_encoder and any(p.requires_grad for p in self.kpf_encoder.parameters()):
+            raise ValueError('forward_train: the KPConv encoder has parameters that require grad; pass '
+                             'train_encoder=True to train it, or freeze it with model.kpf_encoder.requires_grad_(False)')
+        if train_encoder:
+            if not cfg.use_batch_norm:
+                raise NotImplementedError('forward_train(train_encoder=True): no backward for use_batch_norm=False')
+            for name, p in self.kpf_encoder.named_parameters():
+                if name.endswith('kernel_points') and p.requires_grad:
+                    raise NotImplementedError(f'forward_train(train_encoder=True): kpf_encoder.{name} requires grad, but '
+                                              'the kernel disposition is fixed (no gradient through the influences)')
         unsupported = []
         if not cfg.pre_norm:
             unsupported.append('pre_norm=False')
@@ -228,16 +237,21 @@ class RegTR(nn.Module):
             pose = ops.pose_from_corr(xyz_c, corr.detach().contiguous(), logit.detach()[..., 0].contiguous(), offs_c, B)
         return dict(both_un=both_un, xyz_c=xyz_c, cond=cond, corr=corr, logit=logit, pose=pose)
 
-    def forward_train(self, batch):
+    def forward_train(self, batch, train_encoder: bool = False):
         """`forward` with autograd: same output dict, whose src/tgt_feat(_un), *_kp_warped and *_overlap carry
-        history back to every parameter after the KPConv encoder.  The pyramid and the encoder run without grad
-        (freeze the encoder: model.kpf_encoder.requires_grad_(False)).  Exact shapes, eager only."""
-        self._check_trainable()
+        history back to every parameter after the KPConv encoder.  The pyramid always runs without grad.
+        train_encoder=False: the encoder runs without grad and must be frozen
+        (model.kpf_encoder.requires_grad_(False)).  train_encoder=True: the encoder runs under autograd too, on the
+        encoder backward kernels, and every encoder parameter that requires grad receives one (kernel_points must
+        stay frozen, as in the reference); its output is bit-identical to the inference encoder's.
+        Exact shapes, eager only."""
+        self._check_trainable(train_encoder)
         B = len(batch['src_xyz'])
         with torch.no_grad():
             meta = self.preprocessor(list(batch['src_xyz']) + list(batch['tgt_xyz']), lazy_upsamples=True)
             batch['kpconv_meta'] = meta
-            pts = meta['_points']
+        pts = meta['_points']
+        with contextlib.nullcontext() if train_encoder else torch.no_grad():
             feats_un, _ = self.kpf_encoder(torch.ones_like(pts[0][:, 0:1]), meta)             # regtr.py:122-136
         lens_c = meta['_lens'][-1]
         plan = AttentionPlan(lens_c, pts[-1].device)

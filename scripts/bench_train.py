@@ -1,7 +1,8 @@
 """Time training steps of the fine-tuning path: RegTR.forward_train + compute_loss + backward() with the KPConv
-encoder frozen (gradients of every parameter after the encoder; no optimiser step).
+encoder frozen (gradients of every parameter after the encoder), or with --train-encoder the full training step
+(forward_train(batch, train_encoder=True): gradients of every parameter except the kernel points).  No optimiser step.
 
-    python scripts/bench_train.py [--config 2|3] [--pairs B] [--steps K] [--warmup W]
+    python scripts/bench_train.py [--config 2|3] [--pairs B] [--steps K] [--warmup W] [--train-encoder]
 
 Same workload as bench.py: seeded random weights, the synthetic 3DMatch-shaped pairs of the chosen BASELINE config
 (config 2: 1 pair per step, config 3: 8), the attention_impl='fp32' core.  CUDA events around the forward + loss
@@ -45,6 +46,7 @@ def main():
     ap.add_argument('--pairs', type=int, default=None, help='pairs per step (default: 1 for config 2, 8 for 3)')
     ap.add_argument('--steps', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=3)
+    ap.add_argument('--train-encoder', action='store_true', help='train the KPConv encoder too (full training step)')
     args = ap.parse_args()
     if args.steps < 1:
         ap.error('--steps must be >= 1')
@@ -55,7 +57,8 @@ def main():
     cfg = get_config('3dmatch')
     model = RegTR(cfg).to(dev)
     model.load_state_dict(random_state_dict(cfg, WEIGHT_SEED), strict=True)
-    model.kpf_encoder.requires_grad_(False)
+    if not args.train_encoder:
+        model.kpf_encoder.requires_grad_(False)
     n_pool = max(POOL, B)
     b = make_batch(2, n_pool)
     pool = [(torch.from_numpy(s).to(dev), torch.from_numpy(t).to(dev)) for s, t in zip(b['src_xyz'], b['tgt_xyz'])]
@@ -71,7 +74,7 @@ def main():
         model.zero_grad(set_to_none=True)
         if evs:
             evs[0].record()
-        total = model.compute_loss(model.forward_train(batch), batch)['total']
+        total = model.compute_loss(model.forward_train(batch, train_encoder=args.train_encoder), batch)['total']
         if evs:
             evs[1].record()
         total.backward()
@@ -92,7 +95,9 @@ def main():
     bwd = sum(e[1].elapsed_time(e[2]) for e in timed)
     name, power = card()
     print(json.dumps(dict(
-        metric='training steps/s of forward_train + compute_loss + backward (KPConv encoder frozen)',
+        metric='training steps/s of forward_train + compute_loss + backward ' +
+               ('(KPConv encoder trained)' if args.train_encoder else '(KPConv encoder frozen)'),
+        train_encoder=args.train_encoder,
         workload=f'BASELINE config {args.config}: synthetic 3DMatch-like pairs, ~20k pts/cloud, {B} pair(s)/step',
         steps=args.steps, warmup=args.warmup, train_pairs_per_s=B * args.steps / ((fwd + bwd) * 1e-3),
         train_ms_per_step=(fwd + bwd) / args.steps, train_forward_ms_per_step=fwd / args.steps,

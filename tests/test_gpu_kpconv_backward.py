@@ -1,0 +1,435 @@
+"""GPU tests of the KPConv-encoder backward (neighbour-list transpose, KPConv, max-pool, per-cloud InstanceNorm) and of
+RegTR.forward_train(train_encoder=True): op by op against float64 torch autograd of the CPU oracle's math, bit-for-bit
+determinism, and every parameter gradient, encoder included, against the unmodified reference's own backward
+(tests/golden/grad.npz) and against the CPU oracle's autograd."""
+import os
+import sys
+import types
+
+import numpy as np
+import pytest
+import torch
+
+from conftest import FORWARD_CASES, load_golden, make_case
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden'))
+import eval_inputs as ei  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+
+DEV = 'cuda:0'
+
+
+def _rel(got, want):
+    """max |got - want| / max |want|"""
+    want = want.double()
+    return float((got.double().cpu() - want).abs().max() / want.abs().max().clamp_min(1e-30))
+
+
+# ------------------------------------------------------------------------------------------ neighbour-list transpose
+
+def _csr_numpy(idx, Ns):
+    flat = idx.reshape(-1)
+    rows = [np.nonzero(flat == s)[0] for s in range(Ns)]          # ascending edge ids
+    row_start = np.concatenate([[0], np.cumsum([len(r) for r in rows])]).astype(np.int32)
+    edges = np.concatenate(rows).astype(np.int32) if rows else np.zeros(0, np.int32)
+    return row_start, edges
+
+
+@pytest.mark.parametrize('Nq,K,Ns', [(300, 20, 500), (1, 7, 3), (0, 40, 11), (257, 64, 90), (50, 40, 0)])
+def test_neighbor_csr_equals_numpy_inverse(Nq, K, Ns):
+    """Shadow padding (== Ns, and a negative id), supports no query references (the top quarter and an 'empty cloud'
+    range in the middle), all-shadow rows, an empty query set and an empty support set."""
+    from regtr_b200 import ops
+    rng = np.random.default_rng(Nq * 31 + K)
+    hi = max(Ns * 3 // 4, 1)
+    idx = rng.integers(0, hi, size=(Nq, K)).astype(np.int32)
+    if Ns > 8:
+        gap = (Ns // 4, Ns // 4 + Ns // 8)                         # a contiguous unreferenced range
+        idx[(idx >= gap[0]) & (idx < gap[1])] = Ns
+    idx[rng.random((Nq, K)) < 0.3] = Ns
+    if Nq > 3:
+        idx[3] = Ns
+        idx[0, 0] = -1
+    if Ns == 0:
+        idx[:] = 0                                                 # every id is a shadow slot
+    t = torch.from_numpy(idx).to(DEV)
+    rs, ed = ops.neighbor_csr(t, Ns)
+    want_rs, want_ed = _csr_numpy(np.where((idx >= 0) & (idx < Ns), idx, -1), Ns)
+    assert np.array_equal(rs.cpu().numpy(), want_rs)
+    nnz = int(want_rs[-1])
+    assert np.array_equal(ed.cpu().numpy()[:nnz], want_ed)
+    t2 = t.clone()                                                 # a fresh object: no cache hit
+    rs2, ed2 = ops.neighbor_csr(t2, Ns)
+    assert torch.equal(rs, rs2) and torch.equal(ed[:nnz], ed2[:nnz])
+    assert ops.neighbor_csr(t, Ns)[0] is rs                        # cached on the list for the step
+
+
+# ---------------------------------------------------------------------------------------------------------- KPConv
+
+_PYR = {}
+
+
+def _pyramid():
+    """A two-cloud 3DMatch pyramid from PreprocessorGPU (clouds of different sizes)."""
+    if 'meta' not in _PYR:
+        from regtr_b200.config import get_config
+        from regtr_b200.kpconv import PreprocessorGPU
+        from regtr_b200.synthetic import make_3dmatch_pair
+        cfg = get_config('3dmatch')
+        p = make_3dmatch_pair(21, 1500)
+        clouds = [torch.from_numpy(p['src_xyz']).to(DEV), torch.from_numpy(p['tgt_xyz']).to(DEV)]
+        _PYR['meta'] = PreprocessorGPU(cfg)(clouds)
+        _PYR['cfg'] = cfg
+    return _PYR['cfg'], _PYR['meta']
+
+
+def _kp_case(kind, Cin, seed):
+    from regtr_b200.config import pyramid_plan
+    from regtr_b200.weights import kernel_disposition
+    cfg, meta = _pyramid()
+    levels, _, _ = pyramid_plan(cfg)
+    r = levels[0]['radius']
+    if kind == 'conv':
+        q, s, idx = meta['points'][0], meta['points'][0], meta['neighbors'][0]
+    else:
+        q, s, idx = meta['points'][1], meta['points'][0], meta['pools'][0]
+    idx = idx.to(torch.int32).clone()
+    Ns = s.shape[0]
+    idx[:5] = Ns                                                   # queries whose neighbours are all shadow
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(Ns, Cin, generator=g) + 0.1                    # about half the rows sum to <= 0
+    if Cin == 1:
+        x = torch.where(torch.rand(Ns, 1, generator=g) < 0.3, -x.abs(), x)
+    Cout = 64
+    w = torch.randn(15, Cin, Cout, generator=g) / np.sqrt(15 * Cin)
+    kp = torch.from_numpy(kernel_disposition(r, 15))
+    extent = r * cfg.KP_extent / cfg.conv_radius
+    gout = torch.randn(q.shape[0], Cout, generator=g)
+    return q.contiguous(), s.contiguous(), idx, x, w, kp, extent, gout
+
+
+@pytest.mark.parametrize('mode', ['flags', 'noflags', 'x_only'])
+@pytest.mark.parametrize('kind', ['conv', 'pool'])
+@pytest.mark.parametrize('Cin', [1, 32, 64, 128, 256])
+def test_kpconv_backward_matches_float64(Cin, kind, mode):
+    """dx and dW of ops.kpconv against float64 autograd of oracle.regtr_oracle.kpconv.  mode: the forward's row flags
+    passed in (as the normalisation pass emits them) | computed by the aggregation | dx alone (weights frozen: the
+    count is recomputed from x inside the backward kernel)."""
+    from oracle import regtr_oracle as O
+    from regtr_b200 import ops
+    q, s, idx, x, w, kp, extent, gout = _kp_case(kind, Cin, Cin * 10 + len(kind))
+
+    def run():
+        xs = x.to(DEV).requires_grad_(True)
+        ws = w.to(DEV).requires_grad_(mode != 'x_only')
+        flags = (x.double().sum(1) > 0).to(torch.uint8).to(DEV) if mode == 'flags' else None
+        out = ops.kpconv(q, s, idx, xs, ws, kp.to(DEV), extent, row_flags=flags)
+        out.backward(gout.to(DEV))
+        return out.detach(), xs.grad, ws.grad
+
+    out, dx, dw = run()
+    out2, dx2, dw2 = run()
+    with torch.no_grad():                                          # the differentiable forward is the inference one
+        out_inf = ops.kpconv(q, s, idx, x.to(DEV), w.to(DEV), kp.to(DEV), extent)
+    assert torch.equal(out, out_inf)
+    assert torch.equal(dx, dx2) and (dw is None or torch.equal(dw, dw2))
+    xr, wr = x.double().requires_grad_(True), w.double().requires_grad_(True)
+    yr = O.kpconv(q.cpu().double(), s.cpu().double(), idx.cpu().long(), xr, wr, kp.double(), extent)
+    yr.backward(gout.double())
+    errs = dict(out=_rel(out, yr.detach()), dx=_rel(dx, xr.grad))
+    if mode != 'x_only':
+        errs['dW'] = _rel(dw, wr.grad)
+    else:
+        assert dw is None
+    print(Cin, kind, mode, errs)
+    assert max(errs.values()) <= 1e-4, errs
+
+
+# ---------------------------------------------------------------------------------------------------- InstanceNorm
+
+@pytest.mark.parametrize('slope', [-1.0, 0.1])
+@pytest.mark.parametrize('with_res', [False, True])
+@pytest.mark.parametrize('C', [32, 256, 1028])
+def test_instnorm_backward_matches_float64(C, with_res, slope):
+    """Uneven clouds including sizes 1 and 0 (and one spanning several 128-row chunks)."""
+    from oracle import regtr_oracle as O
+    from regtr_b200 import ops
+    lens = [5, 1, 0, 300, 1, 77, 0, 129]
+    n = sum(lens)
+    g = torch.Generator().manual_seed(C + with_res)
+    x = torch.randn(n, C, generator=g) * 3 + 1.5
+    res = torch.randn(n, C, generator=g) if with_res else None
+    gy = torch.randn(n, C, generator=g)
+    offs = ops.make_offsets(lens, DEV)
+
+    def run():
+        xs = x.to(DEV).requires_grad_(True)
+        rs = res.to(DEV).requires_grad_(True) if with_res else None
+        y = ops.instnorm_act(xs, offs, len(lens), res=rs, slope=slope)
+        y.backward(gy.to(DEV))
+        return y.detach(), xs.grad, (rs.grad if with_res else None)
+
+    y, dx, dr = run()
+    y2, dx2, dr2 = run()
+    assert torch.equal(dx, dx2) and (dr is None or torch.equal(dr, dr2))
+    xr = x.double().requires_grad_(True)
+    rr = res.double().requires_grad_(True) if with_res else None
+    yr = O.instance_norm(xr, lens) + (rr if with_res else 0)
+    if slope >= 0:
+        yr = torch.nn.functional.leaky_relu(yr, slope)
+    yr.backward(gy.double())
+    errs = dict(y=_rel(y, yr.detach()), dx=_rel(dx, xr.grad))
+    if with_res:
+        errs['dres'] = _rel(dr, rr.grad)
+    print(C, with_res, slope, errs)
+    assert max(errs.values()) <= 1e-5, errs
+    single = [sum(lens[:i]) for i, l in enumerate(lens) if l == 1]
+    assert float(dx[single].abs().max().cpu()) == 0.0             # one-point clouds: dx = 0
+
+
+def test_instnorm_backward_through_epilogue_statistics():
+    """UnaryBlock's path: linear_instats (statistics from the GEMM epilogue) -> instnorm_apply with residual and
+    LeakyReLU; dx, dW and dres against float64."""
+    from oracle import regtr_oracle as O
+    from regtr_b200 import ops
+    lens = [200, 1, 333]
+    n = sum(lens)
+    g = torch.Generator().manual_seed(5)
+    x, w = torch.randn(n, 64, generator=g), torch.randn(128, 64, generator=g) / 8
+    res, gy = torch.randn(n, 128, generator=g), torch.randn(n, 128, generator=g)
+    offs = ops.make_offsets(lens, DEV)
+    xs, ws, rs = (t.to(DEV).requires_grad_(True) for t in (x, w, res))
+    y, stats = ops.linear_instats(xs, ws, offs, len(lens))
+    out = ops.instnorm_apply(y, offs, len(lens), stats, res=rs, slope=0.1)
+    out.backward(gy.to(DEV))
+    xr, wr, rr = (t.double().requires_grad_(True) for t in (x, w, res))
+    outr = torch.nn.functional.leaky_relu(O.instance_norm(xr @ wr.t(), lens) + rr, 0.1)
+    outr.backward(gy.double())
+    errs = dict(out=_rel(out.detach(), outr.detach()), dx=_rel(xs.grad, xr.grad), dW=_rel(ws.grad, wr.grad),
+                dres=_rel(rs.grad, rr.grad))
+    assert max(errs.values()) <= 1e-5, errs
+
+
+# -------------------------------------------------------------------------------------------------------- max-pool
+
+def test_max_pool_backward_matches_float64():
+    """Ties (values on a coarse grid), all-negative columns where the zero shadow row wins, padded (shadow) slots and
+    all-shadow rows.  The set of (support, channel) entries that receive gradient equals float64 autograd's."""
+    from oracle import regtr_oracle as O
+    from regtr_b200 import ops
+    rng = np.random.default_rng(7)
+    Ns, Nq, K, C = 700, 300, 40, 128
+    x = (rng.integers(-4, 5, size=(Ns, C)) * 0.5).astype(np.float32)          # many ties
+    x[:, :8] = -np.abs(x[:, :8]) - 0.5                                        # all-negative columns
+    idx = rng.integers(0, Ns, size=(Nq, K)).astype(np.int32)
+    idx[:, 30:] = Ns                                                          # padded slots
+    idx[rng.random((Nq, K)) < 0.1] = Ns
+    idx[:4] = Ns                                                              # all-shadow rows
+    idx[10:20, :] = rng.integers(0, Ns, size=(10, K))                         # rows without any shadow slot
+    gout = torch.from_numpy(rng.standard_normal((Nq, C)).astype(np.float32))
+    xt, it = torch.from_numpy(x), torch.from_numpy(idx)
+
+    def run():
+        xs = xt.to(DEV).requires_grad_(True)
+        y = ops.max_pool(xs, it.to(DEV))
+        y.backward(gout.to(DEV))
+        return y.detach(), xs.grad
+
+    y, dx = run()
+    y2, dx2 = run()
+    assert torch.equal(dx, dx2)
+    xr = xt.double().requires_grad_(True)
+    yr = O.max_pool(xr, it.long())
+    yr.backward(gout.double())
+    assert torch.equal(y.cpu().double(), yr.detach())
+    got, want = dx.cpu().double(), xr.grad
+    assert torch.equal(got != 0, want != 0)
+    assert float((got - want).abs().max()) <= 1e-6 * float(want.abs().max())
+
+
+# ------------------------------------------------------------------------------------------------------ whole model
+
+def _model(case, train_encoder=True):
+    from regtr_b200.regtr import RegTR
+    cfg, sd0, src, tgt = make_case(case)
+    sd = ei.loss_state_dict(sd0)
+    model = RegTR(cfg).to(DEV)
+    model.load_state_dict(sd, strict=True)
+    if not train_encoder:
+        model.kpf_encoder.requires_grad_(False)
+    return cfg, sd, model, src, tgt
+
+
+def _pairs(case):
+    from regtr_b200.synthetic import make_3dmatch_pair, make_modelnet_pair
+    return [(make_modelnet_pair if kind == 'modelnet' else make_3dmatch_pair)(*args)
+            for kind, args in FORWARD_CASES[case][2]]
+
+
+def _batch(case, src, tgt):
+    b = {'src_xyz': [torch.from_numpy(s).to(DEV) for s in src], 'tgt_xyz': [torch.from_numpy(t).to(DEV) for t in tgt]}
+    li = ei.loss_inputs(_pairs(case), [len(s) for s in src], [len(t) for t in tgt])
+    b['pose'] = li['pose'].to(DEV)
+    b['src_overlap'] = [m.to(DEV) for m in li['src_overlap']]
+    b['tgt_overlap'] = [m.to(DEV) for m in li['tgt_overlap']]
+    return b
+
+
+def _check_grads(got, want, worst):
+    """test_oracle_grad.py's criteria: norm within 1e-3 relative, 32 sampled entries within 5e-3 of the rms."""
+    for name, g in got.items():
+        w = want[name]
+        g = g.detach().double().reshape(-1).cpu()
+        idx = ei.grad_sample_index(name, g.numel())
+        scale = max(w[0] / np.sqrt(g.numel()), 1e-12)
+        nrm = abs(float(g.norm()) - w[0]) / max(w[0], 1e-30)
+        err = np.abs(g[torch.from_numpy(idx)].numpy() - w[2:]).max() / scale
+        if nrm > worst['norm']:
+            worst.update(norm=nrm, norm_at=name)
+        if err > worst['entry']:
+            worst.update(entry=err, entry_at=name)
+        assert abs(float(g.norm()) - w[0]) <= 1e-3 * w[0] + 1e-9, (name, float(g.norm()), w[0])
+        assert err <= 5e-3, (name, err)
+
+
+def _worst():
+    return dict(norm=0.0, entry=0.0, norm_at=None, entry_at=None)
+
+
+def test_train_encoder_gradients_match_reference_backward():
+    """fwd_modelnet_b1: forward_train(train_encoder=True) -> compute_loss -> backward() against the unmodified
+    reference's d(total)/d(parameter) for all 140 trainable parameters (grad.npz); kernel_points get no gradient."""
+    fx = load_golden('grad')
+    cfg, sd, model, src, tgt = _model('fwd_modelnet_b1')
+    batch = _batch('fwd_modelnet_b1', src, tgt)
+    total = model.compute_loss(model.forward_train(batch, train_encoder=True), batch)['total']
+    np.testing.assert_allclose(float(total.detach()), float(fx['loss_total']), rtol=2e-5)
+    total.backward()
+    params = dict(model.named_parameters())
+    kps = [n for n in params if n.endswith('kernel_points')]
+    assert len(kps) == 6 and all(params[n].grad is None for n in kps)
+    names = [k[2:] for k in fx if k.startswith('g|') and not k.endswith('kernel_points')]
+    assert len(names) == 140 and all(params[n].grad is not None for n in names)
+    worst = _worst()
+    _check_grads({n: params[n].grad for n in names}, {n: fx['g|' + n] for n in names}, worst)
+    print('worst vs reference backward:', worst)
+
+
+@pytest.mark.xfail(strict=True, reason='encoder gradients are up to 1.2e-2 of the rms off the fp32 oracle on sampled '
+                   'entries (criterion 5e-3); tests/diag_grad_accuracy.py and DESIGN.md section 9 give the per-block '
+                   'numbers against float64')
+def test_train_encoder_gradients_match_oracle_3dmatch_b2():
+    """fwd_3dmatch_small_b2 (two pairs of different sizes, four pyramid levels, every Cin path): every parameter
+    gradient, encoder included, against the CPU oracle's autograd."""
+    from oracle import regtr_oracle as O
+    from regtr_b200 import losses as LS
+    case = 'fwd_3dmatch_small_b2'
+    cfg, sd, model, src, tgt = _model(case)
+    sdo = {k: (v.clone().requires_grad_(not k.endswith('kernel_points')) if v.is_floating_point() else v)
+           for k, v in sd.items()}
+    pred_o = O.forward(sdo, cfg, src, tgt)
+    meta_o = pred_o['kpconv_meta']
+    bo = {'kpconv_meta': {k: [torch.as_tensor(np.asarray(v)) for v in meta_o[k]] for k in ('points', 'pools', 'stack_lengths')}}
+    bo.update(ei.loss_inputs(_pairs(case), [len(s) for s in src], [len(t) for t in tgt]))
+    mo = types.SimpleNamespace(cfg=cfg, feature_criterion=types.SimpleNamespace(W=sdo['feature_criterion.W']),
+                               feature_criterion_un=types.SimpleNamespace(W=sdo['feature_criterion_un.W']))
+    total_o = LS.compute_loss(mo, pred_o, bo)['total']
+    total_o.backward()
+    batch = _batch(case, src, tgt)
+    total = model.compute_loss(model.forward_train(batch, train_encoder=True), batch)['total']
+    np.testing.assert_allclose(float(total.detach()), float(total_o.detach()), rtol=2e-5)
+    total.backward()
+    got, want = {}, {}
+    for n, p in model.named_parameters():
+        if n.endswith('kernel_points'):
+            assert p.grad is None
+            continue
+        got[n] = p.grad
+        ref = sdo[n].grad.double().reshape(-1)
+        idx = ei.grad_sample_index(n, ref.numel())
+        want[n] = np.concatenate([[float(ref.norm()), float(ref.sum())], ref[torch.from_numpy(idx)].numpy()])
+    assert sum(n.startswith('kpf_encoder.') for n in got) == 35
+    worst = _worst()
+    _check_grads(got, want, worst)
+    print('worst vs oracle autograd:', worst)
+
+
+@pytest.mark.parametrize('case', ['fwd_modelnet_b1', 'fwd_3dmatch_small_b2'])
+def test_train_encoder_forward_is_bit_identical_to_inference(case):
+    cfg, sd, model, src, tgt = _model(case)
+    pred = model.forward_train(_batch(case, src, tgt), train_encoder=True)
+    with torch.no_grad():
+        ref = model(_batch(case, src, tgt))
+    assert pred['src_feat_un'][0].requires_grad
+    for k in ref:
+        a, b = pred[k], ref[k]
+        for u, v in (zip(a, b) if isinstance(a, (list, tuple)) else [(a, b)]):
+            assert torch.equal(u.detach(), v), k
+
+
+def test_train_encoder_steps_are_deterministic():
+    cfg, sd, model, src, tgt = _model('fwd_3dmatch_small_b1')
+    opt = torch.optim.SGD([p for p in model.parameters() if p.requires_grad], lr=1e-3)
+    runs = []
+    for _ in range(2):
+        model.load_state_dict(sd, strict=True)
+        grads = []
+        for step in range(2):
+            batch = _batch('fwd_3dmatch_small_b1', src, tgt)
+            opt.zero_grad(set_to_none=True)
+            model.compute_loss(model.forward_train(batch, train_encoder=True), batch)['total'].backward()
+            grads.append({n: p.grad.clone() for n, p in model.named_parameters() if p.grad is not None})
+            opt.step()
+        runs.append(grads)
+    for step in range(2):
+        a, b = runs[0][step], runs[1][step]
+        assert a.keys() == b.keys() and sum(n.startswith('kpf_encoder.') for n in a) == 35
+        for n in a:
+            assert torch.equal(a[n], b[n]), (step, n)
+
+
+def test_train_encoder_sgd_steps_reduce_the_loss():
+    """After every optimizer.step() (encoder included) the inference forward equals that of a fresh model loaded with
+    the state_dict, and the loss goes down."""
+    from regtr_b200.regtr import RegTR
+    cfg, sd, model, src, tgt = _model('fwd_modelnet_b1')
+    opt = torch.optim.SGD([p for p in model.parameters() if p.requires_grad], lr=2e-3)
+    losses = []
+    for step in range(4):
+        batch = _batch('fwd_modelnet_b1', src, tgt)
+        opt.zero_grad(set_to_none=True)
+        total = model.compute_loss(model.forward_train(batch, train_encoder=True), batch)['total']
+        losses.append(float(total.detach()))
+        total.backward()
+        opt.step()
+        fresh = RegTR(cfg).to(DEV)
+        fresh.load_state_dict(model.state_dict(), strict=True)
+        a = model(_batch('fwd_modelnet_b1', src, tgt))
+        b = fresh(_batch('fwd_modelnet_b1', src, tgt))
+        for k in ('src_feat_un', 'src_feat', 'tgt_overlap', 'src_kp_warped'):
+            assert torch.equal(a[k][0], b[k][0]), (step, k)
+        assert torch.equal(a['pose'], b['pose']), step
+    print('losses', losses)
+    assert losses[-1] < losses[0]
+
+
+def test_train_encoder_flag_surface():
+    from regtr_b200.config import get_config
+    from regtr_b200.regtr import RegTR
+    cfg, sd, model, src, tgt = _model('fwd_modelnet_b1')
+    with pytest.raises(ValueError, match='requires_grad_'):                  # a live encoder needs the flag
+        model.forward_train(_batch('fwd_modelnet_b1', src, tgt))
+    kp = model.kpf_encoder.encoder_blocks[2].KPConv.kernel_points
+    kp.requires_grad_(True)
+    with pytest.raises(NotImplementedError, match='encoder_blocks.2.KPConv.kernel_points'):
+        model.forward_train(_batch('fwd_modelnet_b1', src, tgt), train_encoder=True)
+    kp.requires_grad_(False)
+    m = RegTR(get_config('modelnet', use_batch_norm=False)).to(DEV)
+    with pytest.raises(NotImplementedError, match='use_batch_norm'):
+        m.forward_train(_batch('fwd_modelnet_b1', src, tgt), train_encoder=True)
+    model.kpf_encoder.requires_grad_(False)                                   # frozen encoder + flag: valid
+    batch = _batch('fwd_modelnet_b1', src, tgt)
+    model.compute_loss(model.forward_train(batch, train_encoder=True), batch)['total'].backward()
+    assert all(p.grad is None for p in model.kpf_encoder.parameters())
+    assert model.feat_proj.weight.grad is not None
