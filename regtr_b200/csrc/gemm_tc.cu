@@ -49,18 +49,21 @@ constexpr QkvOut NO_QKV = {nullptr, 0, nullptr, 0, 0, nullptr, 0, nullptr, 0, 0,
 // into per-(cloud, column) fixed-point accumulators: exact and order-independent, but ~10^4 warps adding to the
 // same few hundred addresses made the level-0 GEMMs 2x slower than the separate statistics kernel they replaced.)
 
-// v[j] of lane l -> lane j receives the sum over the lanes of v_l[j] (fixed butterfly: deterministic)
-__device__ __forceinline__ float warp_transpose_sum(float (&v)[32], int lane) {
+// v[j] of lane l -> lane j receives the sum over the lanes of v_l[j] (fixed butterfly: deterministic).  One template
+// level per butterfly stage, so that every index is a compile-time constant and v stays in registers.
+template <int OFF>
+__device__ __forceinline__ void transpose_sum_step(float (&v)[32], int lane) {
+    const bool up = (lane & OFF) != 0;
 #pragma unroll
-    for (int off = 16; off >= 1; off >>= 1) {
-        const bool up = (lane & off) != 0;
-#pragma unroll
-        for (int i = 0; i < off; ++i) {
-            const float mine = up ? v[i + off] : v[i];
-            const float give = up ? v[i] : v[i + off];
-            v[i] = mine + __shfl_xor_sync(0xffffffffu, give, off);
-        }
+    for (int i = 0; i < OFF; ++i) {
+        const float mine = up ? v[i + OFF] : v[i];
+        const float give = up ? v[i] : v[i + OFF];
+        v[i] = mine + __shfl_xor_sync(0xffffffffu, give, OFF);
     }
+    if constexpr (OFF > 1) transpose_sum_step<OFF / 2>(v, lane);
+}
+__device__ __forceinline__ float warp_transpose_sum(float (&v)[32], int lane) {
+    transpose_sum_step<16>(v, lane);
     return v[0];
 }
 
@@ -124,7 +127,8 @@ __global__ void k_split_tf32(const float* __restrict__ x, long long n, float* __
 //               its stage / phase counters run across tiles, so the next tile's loads fly under the epilogue
 //   warps 0-7   two consumer warpgroups, rows [0, 64) and [64, 128) of the tile: each thread reads its tf32
 //               A fragments from the swizzled stage, splits them into (hi, lo) in registers and issues
-//               wgmma.m64nBNk8 with A from registers and B_hi / B_lo through shared-memory descriptors
+//               wgmma.m64nBNk8 with A from registers and B_hi / B_lo through shared-memory descriptors, one commit
+//               group per k-step, so that a k-step's fragments are split while the previous k-step's MMAs run
 // Every k-block is accumulated by the tensor core into a fresh register block (lo*hi + hi*lo + hi*hi, small terms
 // first) that is then added to the running fp32 sum with round-to-nearest adds: the tensor core's own accumulation
 // truncates, so its chains stay 12 MMAs long whatever K is.  lo = x - hi is exact in fp32 and rounded to nearest
@@ -212,10 +216,13 @@ k_gemm_tf32x3_wg(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int fr = (warp >> 2) * 64 + (warp & 3) * 16 + g;   // this thread's fragment rows: fr and fr + 8
     const int q = warp & 3;                                  // epilogue: rows 32q .. 32q + 31 (thread = row)
     const int r = q * 32 + lane;
+    constexpr int KSTEPS = BK / 8;                           // k-step = 8 tf32 = 32 bytes of the swizzled row
+    constexpr int FSLOTS = 2;                                // A fragment slots (k-steps whose MMAs may be in flight)
     int it = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
         float acc[BN / 2], blk[BN / 2];
+        uint32_t ahi[FSLOTS][4], alo[FSLOTS][4];
 #pragma unroll
         for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
         for (int kb = 0; kb < nkb; ++kb, ++it) {
@@ -223,29 +230,39 @@ k_gemm_tf32x3_wg(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             tc::mbar_wait(&full[s], (it / P::STAGES) & 1);
             // SWIZZLE_128B tile: 16-byte chunk c of row x sits at chunk (c ^ (x & 7)) of its 128-byte row
             const unsigned char* sa = stage_A(s);
-            uint32_t ahi[BK / 8][4], alo[BK / 8][4];
+            const uint64_t dBhi = tc::gmma_desc_sw128(tc::smem_u32(stage_Bhi(s)));
+            const uint64_t dBlo = tc::gmma_desc_sw128(tc::smem_u32(stage_Blo(s)));
+            // One commit group per k-step: its 3 MMAs read the k-step's A fragments from registers, so the tensor
+            // core works on k-step k - 1 while k-step k is loaded and split.  Fragment slot k % FSLOTS is rewritten
+            // once wait<FSLOTS - 1> has retired the group that last read it.
 #pragma unroll
-            for (int k = 0; k < BK / 8; ++k)
+            for (int k = 0; k < KSTEPS; ++k) {
+                uint32_t (&fh)[4] = ahi[k % FSLOTS];
+                uint32_t (&fl)[4] = alo[k % FSLOTS];
+                if (k >= FSLOTS) tc::wgmma_wait<FSLOTS - 1>();
+                tc::fence_operand(fh);
+                tc::fence_operand(fl);
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const int x = fr + (i & 1) * 8, chunk = 2 * k + (i >> 1);
                     const float f = *reinterpret_cast<const float*>(sa + x * 128 + ((chunk ^ (x & 7)) << 4) + 4 * t);
                     const uint32_t h = (__float_as_uint(f) + 0x1000u) & HI_MASK;             // RN (ties away) to TF32
-                    ahi[k][i] = h;
-                    alo[k][i] = (__float_as_uint(f - __uint_as_float(h)) + 0x1000u) & HI_MASK;   // RN: unbiased
+                    fh[i] = h;
+                    fl[i] = (__float_as_uint(f - __uint_as_float(h)) + 0x1000u) & HI_MASK;   // RN: unbiased
                 }
-            const uint64_t dBhi = tc::gmma_desc_sw128(tc::smem_u32(stage_Bhi(s)));
-            const uint64_t dBlo = tc::gmma_desc_sw128(tc::smem_u32(stage_Blo(s)));
-            tc::wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < BK / 8; ++k) {                     // k-step = 8 tf32 = 32 bytes of the swizzled row
+                tc::fence_operand(blk);
+                tc::fence_operand(fh);
+                tc::fence_operand(fl);
+                tc::wgmma_fence();
                 const uint64_t adv = (uint64_t)(2 * k);
-                wgmma_tf32<BN>(blk, alo[k], dBhi + adv, k != 0);   // small terms first
-                wgmma_tf32<BN>(blk, ahi[k], dBlo + adv, 1);
-                wgmma_tf32<BN>(blk, ahi[k], dBhi + adv, 1);
+                wgmma_tf32<BN>(blk, fl, dBhi + adv, k != 0);       // small terms first
+                wgmma_tf32<BN>(blk, fh, dBlo + adv, 1);
+                wgmma_tf32<BN>(blk, fh, dBhi + adv, 1);
+                tc::wgmma_commit();
+                tc::fence_operand(blk);
             }
-            tc::wgmma_commit();
             tc::wgmma_wait<0>();
+            tc::fence_operand(blk);
             __syncwarp();
             if (lane == 0) tc::mbar_arrive(&empty[s]);            // A read into registers, B read by the MMAs
 #pragma unroll

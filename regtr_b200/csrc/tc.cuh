@@ -73,6 +73,20 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
+// Operand fences: an empty volatile asm that "reads and writes" the registers.  Volatile asms keep their order, so
+// the compiler can neither move an access of an accumulator or A fragment across a wgmma issue / wait placed
+// between two fences nor hand those registers to another value while an asynchronous MMA still reads them.
+template <int N>
+__device__ __forceinline__ void fence_operand(float (&r)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i]));
+}
+template <int N>
+__device__ __forceinline__ void fence_operand(uint32_t (&r)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i]));
+}
+
 // D[64 x N] (+)= A[64 x K] * B[N x K]^T; A from registers, B (K-major) through a shared-memory descriptor.
 // Fragments (g = lane / 4, t = lane % 4, rows relative to the 16-row slab of warp w % 4 of the warpgroup):
 //   tf32 A (k8):  a0 (g, t)  a1 (g + 8, t)  a2 (g, t + 4)  a3 (g + 8, t + 4)

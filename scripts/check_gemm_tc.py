@@ -1,7 +1,19 @@
-import sys, os
+# Accuracy of the 3xTF32 wgmma GEMM against float64 at the model's shapes, then per-shape timings.
+#   --save DIR      write every accuracy-case output to DIR/<M>x<N>x<K>.npy
+#   --compare DIR   check that every output is bit-identical to the one saved in DIR (e.g. by an older build)
+import argparse, sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np
 import torch
 from regtr_b200 import ops
+ap = argparse.ArgumentParser()
+ap.add_argument('--save', metavar='DIR')
+ap.add_argument('--compare', metavar='DIR')
+args = ap.parse_args()
+if args.save:
+    os.makedirs(args.save, exist_ok=True)
+# H100 SXM data sheet: dense TF32 tensor rate and HBM3 bandwidth (a power-limited card reaches less)
+PEAK_TF32, PEAK_HBM = 495e12, 3.35e12
 torch.manual_seed(0)
 dev = 'cuda:0'
 ok = True
@@ -27,6 +39,13 @@ for (M, N, K, bias, res, relu) in [(300, 64, 64, False, False, False), (128, 128
     if relu: ref32 = ref32.relu()
     err32 = float((ref32.double() - want).abs().max())
     good = err <= 2e-6 * scale * max(1.0, (K / 64) ** 0.5)
+    name = f'{M}x{N}x{K}.npy'
+    if args.save:
+        np.save(os.path.join(args.save, name), got.cpu().numpy())
+    if args.compare:
+        same = np.array_equal(np.load(os.path.join(args.compare, name)).view(np.uint32), got.cpu().numpy().view(np.uint32))
+        print(f'  {name}: {"bit-identical" if same else "DIFFERS"} to {args.compare}')
+        good &= same
     ok &= good
     print(f'M={M:6d} N={N:5d} K={K:5d} err {err:.3e} (cublas fp32 err {err32:.3e}) scale {scale:.2f} {"OK" if good else "FAIL"}')
 # device-side row count
@@ -54,5 +73,9 @@ for (M, N, K) in [(38061, 128, 64), (38061, 32, 64), (38061, 32, 480), (38061, 1
     for _ in range(20): a @ w.t()
     e2.record(); torch.cuda.synchronize()
     fl = 2 * M * N * K
-    print(f'M={M} N={N} K={K}: tc3x {e0.elapsed_time(e1)/20*1e3:.1f} us ({fl/(e0.elapsed_time(e1)/20*1e-3)/1e12:.1f} TF/s)  cublas fp32 {e1.elapsed_time(e2)/20*1e3:.1f} us')
+    t = e0.elapsed_time(e1) / 20 * 1e-3
+    nbytes = 4 * (M * K + 2 * N * K + M * N)           # algorithmic: A, B_hi, B_lo read once, C written once
+    bound = 'tensor' if 3 * fl / PEAK_TF32 >= nbytes / PEAK_HBM else 'hbm'
+    print(f'M={M} N={N} K={K}: tc3x {t*1e6:.1f} us ({fl/t/1e12:.1f} TF/s fp32-equiv, {3*fl/t/1e12:.1f} TF/s 3xTF32 MMA, '
+          f'{nbytes/t/1e9:.0f} GB/s algorithmic, {bound}-bound)  cublas fp32 {e1.elapsed_time(e2)/20*1e3:.1f} us')
 print('ALL OK' if ok else 'SOME FAILED')
