@@ -26,7 +26,7 @@ def _t(x, dtype):
 
 # ----------------------------------------------------------------------- KPConv
 
-def kpconv(q_pts, s_pts, inds, x, weights, kernel_points, extent, chunk=8192):
+def kpconv(q_pts, s_pts, inds, x, weights, kernel_points, extent, chunk=8192, count=None):
     """Rigid KPConv, linear influence, sum aggregation.
 
     Follows KPConv.forward, /root/reference/src/models/backbone_kpconv/kpconv_blocks.py:
@@ -34,7 +34,8 @@ def kpconv(q_pts, s_pts, inds, x, weights, kernel_points, extent, chunk=8192):
     to the kernel points (325-329), linear influence clamp (368), zero shadow
     feature row (388), gather (391), influence-weighted sum (394), per-kernel-point
     weight contraction and sum (401-406), division by the number of neighbours
-    whose feature row sums to > 0 (409-412).
+    whose feature row sums to > 0 (409-412).  `count` (Nq,) fixes that divisor
+    (see `kpconv_count`).
     """
     dt = x.dtype
     s_aug = torch.cat([s_pts, torch.full_like(s_pts[:1], 1e6)], 0)
@@ -49,9 +50,15 @@ def kpconv(q_pts, s_pts, inds, x, weights, kernel_points, extent, chunk=8192):
         nx = x_aug[idx]                                                # (n,K,Cin)
         wf = infl @ nx                                                 # (n,P,Cin)
         out = torch.einsum('npc,pco->no', wf, weights.to(dt))
-        cnt = (nx.sum(-1) > 0).sum(-1).clamp(min=1)
+        cnt = (nx.sum(-1) > 0).sum(-1).clamp(min=1) if count is None else count[a:a + chunk]
         outs.append(out / cnt[:, None].to(dt))
     return torch.cat(outs, 0) if outs else x.new_zeros((0, weights.shape[-1]))
+
+
+def kpconv_count(inds, x):
+    """kpconv's divisor per query: the number of neighbours whose feature row sums to > 0, at least 1."""
+    pos = torch.cat([x.detach().sum(-1) > 0, torch.zeros(1, dtype=torch.bool)])
+    return pos[inds].sum(-1).clamp(min=1)
 
 
 def instance_norm(x, lens, eps=1e-5):
@@ -68,45 +75,76 @@ def instance_norm(x, lens, eps=1e-5):
     return out
 
 
-def unary(x, w, lens, relu=True):
+def _act(x, slope, decisions=None, site=None):
+    """LeakyReLU(slope), ReLU for slope 0.  With `decisions`, the elements that take the identity branch are the
+    boolean mask decisions[site] (recorded there as x > 0 when absent); the math stays smooth in x."""
+    if decisions is None:
+        return F.relu(x) if slope == 0 else F.leaky_relu(x, slope)
+    mask = decisions.setdefault(site, x.detach() > 0)
+    return torch.where(mask, x, x * slope)
+
+
+def unary(x, w, lens, relu=True, decisions=None, site=None):
     """UnaryBlock: Linear(no bias) -> InstanceNorm -> LeakyReLU(0.1) (kpconv_blocks.py:533-561)."""
     y = instance_norm(x @ w.t(), lens)
-    return F.leaky_relu(y, 0.1) if relu else y
+    return _act(y, 0.1, decisions, site) if relu else y
 
 
-def max_pool(x, inds):
-    """kpconv_blocks.py:127-143: max over the K gathered rows, zero shadow row."""
+def max_pool(x, inds, winner=None):
+    """kpconv_blocks.py:127-143: max over the K gathered rows, zero shadow row.  `winner` (Nq,C) fixes the slot
+    that each output takes (see `max_pool_winner`)."""
     x_aug = torch.cat([x, torch.zeros_like(x[:1])], 0)
-    return x_aug[inds].max(1).values
+    if winner is None:
+        return x_aug[inds].max(1).values
+    return x_aug[inds].gather(1, winner[:, None, :]).squeeze(1)
+
+
+def max_pool_winner(x, inds):
+    """The first slot of each (query, channel) that holds the maximum, (Nq,C) int64."""
+    g = torch.cat([x.detach(), torch.zeros_like(x[:1])], 0)[inds]
+    return (g == g.max(1, keepdim=True).values).to(torch.uint8).argmax(1)
+
+
+def encoder_block(sd, cfg, i, x, meta, dtype=torch.float32, decisions=None, prefix='kpf_encoder.encoder_blocks.'):
+    """Encoder block i: SimpleBlock (kpconv_blocks.py:632-646) or ResnetBottleneckBlock (706-741).
+
+    `decisions` (a dict, optional) fixes the block's branches; every site absent from it is filled in with the
+    choice this evaluation takes, so `{}` records them.  Sites: 'kpconv' the KPConv divisor per query (Nq,);
+    'pool' the max-pool winner slot per (query, channel); 'unary1', 'conv', 'out' the LeakyReLU masks after
+    unary1, after the KPConv's InstanceNorm and at the block output ('out' alone for a SimpleBlock)."""
+    b = pyramid_plan(cfg)[1][i]
+    g = lambda k: sd[f'{prefix}{i}.{k}'].to(dtype)
+    d = decisions
+    lv = b['level']
+    lens = [np.asarray(l) for l in meta['stack_lengths']]
+    if b['strided']:
+        q, s, idx, l_post = (_t(meta['points'][lv + 1], dtype), _t(meta['points'][lv], dtype),
+                             _t(meta['pools'][lv], torch.long), lens[lv + 1])
+    else:
+        s = _t(meta['points'][lv], dtype)
+        q, idx, l_post = s, _t(meta['neighbors'][lv], torch.long), lens[lv]
+    conv = lambda h: kpconv(q, s, idx, h, g('KPConv.weights'), g('KPConv.kernel_points'), b['extent'],
+                            count=None if d is None else d.setdefault('kpconv', kpconv_count(idx, h)))
+    if b['kind'] == 'simple':
+        return _act(instance_norm(conv(x), l_post), 0.1, d, 'out')
+    mid = b['out_dim'] // 4
+    h = unary(x, g('unary1.mlp.weight'), lens[lv], decisions=d, site='unary1') if b['in_dim'] != mid else x
+    h = _act(instance_norm(conv(h), l_post), 0.1, d, 'conv')
+    h = unary(h, g('unary2.mlp.weight'), l_post, relu=False)
+    sc = x
+    if b['strided']:
+        sc = max_pool(x, idx, None if d is None else d.setdefault('pool', max_pool_winner(x, idx)))
+    if b['in_dim'] != b['out_dim']:
+        sc = unary(sc, g('unary_shortcut.mlp.weight'), l_post, relu=False)
+    return _act(h + sc, 0.1, d, 'out')
 
 
 def encoder(sd, cfg, meta, dtype=torch.float32, prefix='kpf_encoder.encoder_blocks.'):
-    """KPFEncoder.forward (kpconv.py:81-88) over SimpleBlock (kpconv_blocks.py:632-646)
-    and ResnetBottleneckBlock (706-741)."""
+    """KPFEncoder.forward (kpconv.py:81-88): the blocks in sequence on a constant input feature."""
     _, blocks, _ = pyramid_plan(cfg)
-    pts = [_t(p, dtype) for p in meta['points']]
-    lens = [np.asarray(l) for l in meta['stack_lengths']]
-    x = torch.ones((pts[0].shape[0], 1), dtype=dtype)                   # regtr.py:122
-    for i, b in enumerate(blocks):
-        g = lambda k: sd[f'{prefix}{i}.{k}'].to(dtype)
-        lv = b['level']
-        if b['strided']:
-            q, s, idx, l_post = pts[lv + 1], pts[lv], _t(meta['pools'][lv], torch.long), lens[lv + 1]
-        else:
-            q, s, idx, l_post = pts[lv], pts[lv], _t(meta['neighbors'][lv], torch.long), lens[lv]
-        if b['kind'] == 'simple':
-            y = kpconv(q, s, idx, x, g('KPConv.weights'), g('KPConv.kernel_points'), b['extent'])
-            x = F.leaky_relu(instance_norm(y, l_post), 0.1)
-            continue
-        mid = b['out_dim'] // 4
-        h = unary(x, g('unary1.mlp.weight'), lens[lv]) if b['in_dim'] != mid else x
-        h = kpconv(q, s, idx, h, g('KPConv.weights'), g('KPConv.kernel_points'), b['extent'])
-        h = F.leaky_relu(instance_norm(h, l_post), 0.1)
-        h = unary(h, g('unary2.mlp.weight'), l_post, relu=False)
-        sc = max_pool(x, idx) if b['strided'] else x
-        if b['in_dim'] != b['out_dim']:
-            sc = unary(sc, g('unary_shortcut.mlp.weight'), l_post, relu=False)
-        x = F.leaky_relu(h + sc, 0.1)
+    x = torch.ones((len(meta['points'][0]), 1), dtype=dtype)           # regtr.py:122
+    for i in range(len(blocks)):
+        x = encoder_block(sd, cfg, i, x, meta, dtype, prefix=prefix)
     return x
 
 
@@ -148,49 +186,58 @@ def mha(q_in, k_in, v_in, in_w, in_b, out_w, out_b, nhead):
     return o @ out_w.t() + out_b
 
 
-def cross_encoder(sd, cfg, src, tgt, src_pe, tgt_pe, prefix='transformer_encoder.'):
-    """TransformerCrossEncoder.forward with return_intermediate and final norm
-    (transformers.py:27-59) over TransformerCrossEncoderLayer.forward_pre (183-244).
-    Operates per pair on un-padded sequences; returns (L,S,E), (L,T,E)."""
+def cross_encoder_layer(sd, cfg, i, src, tgt, sp, tp, decisions=None, prefix='transformer_encoder.'):
+    """TransformerCrossEncoderLayer i: forward_pre (transformers.py:183-244) or, without pre_norm, forward_post
+    (121-181), on one pair of un-padded sequences; sp / tp are the position embeddings the layer adds (zeros when
+    it adds none).  `decisions` (a dict, optional) fixes the feed-forward ReLU masks, sites 'ffn_src' and
+    'ffn_tgt', as in `encoder_block`.  Returns (src, tgt)."""
     E, H = cfg.d_embed, cfg.nhead
     dt = src.dtype
-    g = lambda k: sd[prefix + k].to(dt)
+    p = f'{prefix}layers.{i}.'
+    g = lambda k: sd[p + k].to(dt)
     ln = lambda x, k: F.layer_norm(x, (E,), g(k + '.weight'), g(k + '.bias'), 1e-5)
+    att = lambda m, q, k, v: mha(q, k, v, g(m + '.in_proj_weight'), g(m + '.in_proj_bias'),
+                                 g(m + '.out_proj.weight'), g(m + '.out_proj.bias'), H)
+    ffn = lambda x, site: _act(x @ g('linear1.weight').t() + g('linear1.bias'), 0, decisions, site) \
+        @ g('linear2.weight').t() + g('linear2.bias')
+    if not cfg.pre_norm:
+        swp, twp = src + sp, tgt + tp
+        src = ln(src + att('self_attn', swp, swp, swp if cfg.sa_val_has_pos_emb else src), 'norm1')
+        tgt = ln(tgt + att('self_attn', twp, twp, twp if cfg.sa_val_has_pos_emb else tgt), 'norm1')
+        swp, twp = src + sp, tgt + tp
+        s3 = att('multihead_attn', swp, twp, twp if cfg.ca_val_has_pos_emb else tgt)
+        t3 = att('multihead_attn', twp, swp, swp if cfg.ca_val_has_pos_emb else src)
+        src, tgt = ln(src + s3, 'norm2'), ln(tgt + t3, 'norm2')
+        return ln(src + ffn(src, 'ffn_src'), 'norm3'), ln(tgt + ffn(tgt, 'ffn_tgt'), 'norm3')
+    s2 = ln(src, 'norm1'); s2p = s2 + sp
+    src = src + att('self_attn', s2p, s2p, s2p if cfg.sa_val_has_pos_emb else s2)
+    t2 = ln(tgt, 'norm1'); t2p = t2 + tp
+    tgt = tgt + att('self_attn', t2p, t2p, t2p if cfg.sa_val_has_pos_emb else t2)
+    s2, t2 = ln(src, 'norm2'), ln(tgt, 'norm2')
+    s2p, t2p = s2 + sp, t2 + tp
+    s3 = att('multihead_attn', s2p, t2p, t2p if cfg.ca_val_has_pos_emb else t2)
+    t3 = att('multihead_attn', t2p, s2p, s2p if cfg.ca_val_has_pos_emb else s2)
+    src, tgt = src + s3, tgt + t3
+    return src + ffn(ln(src, 'norm3'), 'ffn_src'), tgt + ffn(ln(tgt, 'norm3'), 'ffn_tgt')
+
+
+def cross_encoder(sd, cfg, src, tgt, src_pe, tgt_pe, prefix='transformer_encoder.'):
+    """TransformerCrossEncoder.forward with return_intermediate and final norm
+    (transformers.py:27-59) over `cross_encoder_layer`.
+    Operates per pair on un-padded sequences; returns (L,S,E), (L,T,E)."""
+    E = cfg.d_embed
+    dt = src.dtype
     use_pe = cfg.transformer_encoder_has_pos_emb
     sp = src_pe if use_pe else torch.zeros_like(src)
     tp = tgt_pe if use_pe else torch.zeros_like(tgt)
+    # no final norm without pre_norm (regtr.py:64)
+    ln = (lambda x: F.layer_norm(x, (E,), sd[prefix + 'norm.weight'].to(dt), sd[prefix + 'norm.bias'].to(dt), 1e-5)) \
+        if cfg.pre_norm else (lambda x: x)
     outs_s, outs_t = [], []
     for i in range(cfg.num_encoder_layers):
-        p = f'layers.{i}.'
-        att = lambda m, q, k, v: mha(q, k, v, g(p + m + '.in_proj_weight'), g(p + m + '.in_proj_bias'),
-                                     g(p + m + '.out_proj.weight'), g(p + m + '.out_proj.bias'), H)
-        ffn = lambda x: F.relu(x @ g(p + 'linear1.weight').t() + g(p + 'linear1.bias')) \
-            @ g(p + 'linear2.weight').t() + g(p + 'linear2.bias')
-        if not cfg.pre_norm:                              # forward_post (transformers.py:121-181)
-            swp, twp = src + sp, tgt + tp
-            src = ln(src + att('self_attn', swp, swp, swp if cfg.sa_val_has_pos_emb else src), p + 'norm1')
-            tgt = ln(tgt + att('self_attn', twp, twp, twp if cfg.sa_val_has_pos_emb else tgt), p + 'norm1')
-            swp, twp = src + sp, tgt + tp
-            s3 = att('multihead_attn', swp, twp, twp if cfg.ca_val_has_pos_emb else tgt)
-            t3 = att('multihead_attn', twp, swp, swp if cfg.ca_val_has_pos_emb else src)
-            src, tgt = ln(src + s3, p + 'norm2'), ln(tgt + t3, p + 'norm2')
-            src, tgt = ln(src + ffn(src), p + 'norm3'), ln(tgt + ffn(tgt), p + 'norm3')
-            outs_s.append(src)                            # no final norm without pre_norm (regtr.py:64)
-            outs_t.append(tgt)
-            continue
-        s2 = ln(src, p + 'norm1'); s2p = s2 + sp
-        src = src + att('self_attn', s2p, s2p, s2p if cfg.sa_val_has_pos_emb else s2)
-        t2 = ln(tgt, p + 'norm1'); t2p = t2 + tp
-        tgt = tgt + att('self_attn', t2p, t2p, t2p if cfg.sa_val_has_pos_emb else t2)
-        s2, t2 = ln(src, p + 'norm2'), ln(tgt, p + 'norm2')
-        s2p, t2p = s2 + sp, t2 + tp
-        s3 = att('multihead_attn', s2p, t2p, t2p if cfg.ca_val_has_pos_emb else t2)
-        t3 = att('multihead_attn', t2p, s2p, s2p if cfg.ca_val_has_pos_emb else s2)
-        src, tgt = src + s3, tgt + t3
-        src = src + ffn(ln(src, p + 'norm3'))
-        tgt = tgt + ffn(ln(tgt, p + 'norm3'))
-        outs_s.append(ln(src, 'norm'))
-        outs_t.append(ln(tgt, 'norm'))
+        src, tgt = cross_encoder_layer(sd, cfg, i, src, tgt, sp, tp, prefix=prefix)
+        outs_s.append(ln(src))
+        outs_t.append(ln(tgt))
     return torch.stack(outs_s), torch.stack(outs_t)
 
 

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from conftest import FORWARD_CASES, load_golden, make_case
+from grad_yardstick import Yardstick
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden'))
 import eval_inputs as ei  # noqa: E402
@@ -52,12 +53,12 @@ def _attention_case(seed=0):
     return qkv, d_o, self_p, cross_p, E, H
 
 
-def _attention_ref(qkv, d_o, problems, E, H):
-    """float64 autograd: (O, lse base 2, dqkv) restricted to the rows the problems cover."""
-    x = qkv.double().cpu().requires_grad_(True)
-    g = d_o.double().cpu()
-    o = torch.zeros(x.shape[0], E, dtype=torch.float64)
-    lse = torch.full((x.shape[0], H), -math.inf, dtype=torch.float64)
+def _attention_ref(qkv, d_o, problems, E, H, dtype=torch.float64):
+    """autograd in `dtype`: (O, lse base 2, dqkv) restricted to the rows the problems cover."""
+    x = qkv.cpu().to(dtype).requires_grad_(True)
+    g = d_o.cpu().to(dtype)
+    o = torch.zeros(x.shape[0], E, dtype=dtype)
+    lse = torch.full((x.shape[0], H), -math.inf, dtype=dtype)
     for qs, ql, ks, kl in problems:
         if ql == 0:
             continue
@@ -75,6 +76,7 @@ def _attention_ref(qkv, d_o, problems, E, H):
 
 @pytest.mark.parametrize('kind', ['self', 'cross'])
 def test_attention_backward_matches_float64(kind):
+    """O and lse within 1e-4·max of float64; dQ, dK, dV under the fp32 yardstick (tests/grad_yardstick.py)."""
     from regtr_b200 import ops
     qkv, d_o, self_p, cross_p, E, H = _attention_case()
     problems = self_p if kind == 'self' else cross_p
@@ -98,11 +100,15 @@ def test_attention_backward_matches_float64(kind):
     errs = {}
     errs['lse'] = float((lg[fin] - lr[fin]).abs().max() / lr[fin].abs().max())
     dc, dr = d.cpu(), d_ref
-    errs['dq'] = _rel(dc[rows, :E], dr[rows, :E])
-    errs['dk'] = _rel(dc[krows, E:2 * E], dr[krows, E:2 * E])
-    errs['dv'] = _rel(dc[krows, 2 * E:], dr[krows, 2 * E:])
     print(kind, errs)
     assert max(errs.values()) <= 1e-4, errs
+    d32 = _attention_ref(qkv, d_o, problems, E, H, torch.float32)[2]
+    ys = Yardstick(f'attention backward, {kind} problems')
+    ys.add('dq', dc[rows, :E], d32[rows, :E], dr[rows, :E])
+    ys.add('dk', dc[krows, E:2 * E], d32[krows, E:2 * E], dr[krows, E:2 * E])
+    ys.add('dv', dc[krows, 2 * E:], d32[krows, 2 * E:], dr[krows, 2 * E:])
+    ys.report()
+    assert not ys.failures(), ys.failures()
     if kind == 'cross':                                  # empty key range -> dQ = 0; no queries -> dK = dV = 0
         e = cross_p[2]
         assert float(dc[e[0]:e[0] + e[1], :E].abs().max()) == 0.0

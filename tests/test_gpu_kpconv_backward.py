@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from conftest import FORWARD_CASES, load_golden, make_case
+from grad_yardstick import Yardstick
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden'))
 import eval_inputs as ei  # noqa: E402
@@ -113,7 +114,8 @@ def _kp_case(kind, Cin, seed):
 @pytest.mark.parametrize('kind', ['conv', 'pool'])
 @pytest.mark.parametrize('Cin', [1, 32, 64, 128, 256])
 def test_kpconv_backward_matches_float64(Cin, kind, mode):
-    """dx and dW of ops.kpconv against float64 autograd of oracle.regtr_oracle.kpconv.  mode: the forward's row flags
+    """dx and dW of ops.kpconv against float64 autograd of oracle.regtr_oracle.kpconv, under the fp32 yardstick (the
+    same oracle in fp32; tests/grad_yardstick.py), the forward within 1e-4·max.  mode: the forward's row flags
     passed in (as the normalisation pass emits them) | computed by the aggregation | dx alone (weights frozen: the
     count is recomputed from x inside the backward kernel)."""
     from oracle import regtr_oracle as O
@@ -134,16 +136,25 @@ def test_kpconv_backward_matches_float64(Cin, kind, mode):
         out_inf = ops.kpconv(q, s, idx, x.to(DEV), w.to(DEV), kp.to(DEV), extent)
     assert torch.equal(out, out_inf)
     assert torch.equal(dx, dx2) and (dw is None or torch.equal(dw, dw2))
-    xr, wr = x.double().requires_grad_(True), w.double().requires_grad_(True)
-    yr = O.kpconv(q.cpu().double(), s.cpu().double(), idx.cpu().long(), xr, wr, kp.double(), extent)
-    yr.backward(gout.double())
-    errs = dict(out=_rel(out, yr.detach()), dx=_rel(dx, xr.grad))
+    count = O.kpconv_count(idx.cpu().long(), x.double())           # the divisor the GPU used, for both oracles
+
+    def oracle(dtype):
+        xr, wr = x.to(dtype).requires_grad_(True), w.to(dtype).requires_grad_(True)
+        yr = O.kpconv(q.cpu().to(dtype), s.cpu().to(dtype), idx.cpu().long(), xr, wr, kp.to(dtype), extent,
+                      count=count)
+        yr.backward(gout.to(dtype))
+        return yr.detach(), xr.grad, wr.grad
+    y64, dx64, dw64 = oracle(torch.float64)
+    _, dx32, dw32 = oracle(torch.float32)
+    assert _rel(out, y64) <= 1e-4
+    ys = Yardstick(f'KPConv Cin={Cin} {kind} {mode}')
+    ys.add('dx', dx, dx32, dx64)
     if mode != 'x_only':
-        errs['dW'] = _rel(dw, wr.grad)
+        ys.add('dW', dw, dw32, dw64)
     else:
         assert dw is None
-    print(Cin, kind, mode, errs)
-    assert max(errs.values()) <= 1e-4, errs
+    ys.report()
+    assert not ys.failures(), ys.failures()
 
 
 # ---------------------------------------------------------------------------------------------------- InstanceNorm
@@ -317,8 +328,10 @@ def test_train_encoder_gradients_match_reference_backward():
 
 
 @pytest.mark.xfail(strict=True, reason='encoder gradients are up to 1.2e-2 of the rms off the fp32 oracle on sampled '
-                   'entries (criterion 5e-3); tests/diag_grad_accuracy.py and DESIGN.md section 9 give the per-block '
-                   'numbers against float64')
+                   'entries (criterion 5e-3).  Not kernel arithmetic: every block and layer backward and the encoder '
+                   'backward fed the float64 d(feats_un) are as close to float64 as the fp32 oracle, with no branch '
+                   'decision flipped (tests/test_gpu_grad_stages.py).  The GPU encoder forward output is 3e-6 off '
+                   'float64, and the stages after it turn that into a 4.8e-4 change of d(feats_un); DESIGN.md section 9')
 def test_train_encoder_gradients_match_oracle_3dmatch_b2():
     """fwd_3dmatch_small_b2 (two pairs of different sizes, four pyramid levels, every Cin path): every parameter
     gradient, encoder included, against the CPU oracle's autograd."""

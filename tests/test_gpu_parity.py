@@ -66,6 +66,12 @@ def test_kpconv_all_channel_paths_vs_oracle(cin, cout, impl, monkeypatch):
     want = O.kpconv(*(torch.from_numpy(a) for a in (q, s)), torch.from_numpy(idx), torch.from_numpy(x),
                     torch.from_numpy(W), torch.from_numpy(kp), 0.05).numpy()
     got = N(ops.kpconv(G(q), G(s), G(idx, torch.int32), G(x), G(W), G(kp), 0.05))
+    # which side a deviation comes from: both against the same math in float64
+    w64 = O.kpconv(*(torch.from_numpy(a).double() for a in (q, s)), torch.from_numpy(idx),
+                   *(torch.from_numpy(a).double() for a in (x, W, kp)), 0.05).numpy()
+    scale = np.abs(w64).max()
+    print(f'kpconv cin={cin} cout={cout} {impl}: vs float64, GPU {np.abs(got - w64).max() / scale:.2e}, '
+          f'fp32 oracle {np.abs(want - w64).max() / scale:.2e}')
     # SURVEY 8c feature tolerance (1e-4 * max|ref|); the kernels measure ~2e-7 here.  Twice in ~20 suite runs the
     # Cin = 1 case came out 5e-5 off on a few entries (not reproduced in isolated processes, sanitizer-clean:
     # DESIGN.md 9), hence not the tighter 2e-5 the other paths would allow.
