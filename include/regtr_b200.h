@@ -358,6 +358,72 @@ int regtr_instnorm_bwd(const float* g, const float* x, const float* out, const i
                        int n, int C, float eps, float slope, float* dx, float* dres,
                        void* ws, size_t ws_bytes, void* stream);
 
+/* ---- optimizer step (training) ---------------------------------------------------- */
+
+/* Multi-tensor launches over a DEVICE table of descriptors: the number of launches does not depend on the number of
+ * tensors.  Each tensor is cut into chunks of REGTR_OPTIM_CHUNK elements; `first` is the exclusive prefix of the
+ * chunk counts ceil(n / REGTR_OPTIM_CHUNK) over the table (the table is sorted by it) and n_chunks the total.
+ * Tensors are contiguous fp32; entries with n == 0 own no chunk. */
+#define REGTR_OPTIM_CHUNK 8192
+
+typedef struct {
+    float* g;             /* gradient (scaled in place by regtr_grad_scale) */
+    long long n;          /* elements */
+    long long first;      /* first chunk */
+} regtr_grad_ref;
+
+/* Total 2-norm of all gradients, as torch.nn.utils.clip_grad_norm_(max_norm, norm_type=2) computes it:
+ * out[0] = sqrt(sum g^2) (sum of squares in fp64: fixed per-chunk order, then the chunk partials in a fixed order;
+ * no atomics), out[1] = min(1, max_norm / (out[0] + 1e-6)) in fp32 with torch's roundings (NaN propagates).
+ * Two launches.  ws: regtr_grad_norm_ws_bytes(n_chunks) bytes (one fp64 partial per chunk). */
+size_t regtr_grad_norm_ws_bytes(int n_chunks);
+int regtr_grad_norm(const regtr_grad_ref* table, int n_tensors, int n_chunks, float max_norm, float* out,
+                    void* ws, size_t ws_bytes, void* stream);
+/* g *= *coef for every gradient of the table (coef: device fp32, e.g. out + 1 of regtr_grad_norm).  One launch. */
+int regtr_grad_scale(const regtr_grad_ref* table, int n_tensors, int n_chunks, const float* coef, void* stream);
+
+#define REGTR_ADAM_FRESH 1u      /* state just created: exp_avg / exp_avg_sq are read as zero (and written) */
+#define REGTR_ADAM_COUPLED 2u    /* Adam weight decay: g += wd * p */
+#define REGTR_ADAM_DECOUPLED 4u  /* AdamW weight decay: p *= decay */
+
+/* One tensor of an Adam / AdamW step.  The host scalars are torch's for this tensor's step t (already incremented),
+ * rounded to fp32 as torch's kernels round them:  decay = 1 - lr * wd,  b1w = 1 - beta1 (the lerp weight),
+ * one_m_b2 = 1 - beta2,  rcp_bc2_sqrt = 1 / fp32(sqrt(1 - beta2^t)) (fp32 division),
+ * neg_step_size = -lr / (1 - beta1^t)  (the bias corrections in double). */
+typedef struct {
+    float* p;             /* parameter */
+    const float* g;       /* gradient */
+    float* m;             /* exp_avg */
+    float* v;             /* exp_avg_sq */
+    long long n;
+    long long first;      /* first chunk */
+    float decay, wd, b1w, b2, one_m_b2, rcp_bc2_sqrt, neg_step_size, eps;
+    uint32_t flags;       /* REGTR_ADAM_* */
+    uint32_t pad;
+} regtr_adam_tensor;
+
+/* Replaces torch.optim.Adam / AdamW.step (foreach=False arithmetic, torch 2.11 _single_tensor_adam):
+ *   p = p * decay (decoupled) or g = g + wd * p (coupled);  m = lerp(m, g, b1w);  v = v * b2 + one_m_b2 * g * g;
+ *   p = p - step_size * m / (sqrt(v) / sqrt(1 - beta2^t) + eps).   One launch. */
+int regtr_adam_step(const regtr_adam_tensor* table, int n_tensors, int n_chunks, void* stream);
+
+/* A 2-D view of a weight whose TF32 halves are cached: out[a, b] = src[a * s0 + b * s1] for a < rows, b < cols,
+ * hi / lo contiguous (rows, cols).  `first`: exclusive prefix of the 32 x 32 tile counts
+ * ceil(rows / 32) * ceil(cols / 32) over the table. */
+typedef struct {
+    const float* src;
+    float* hi;
+    float* lo;
+    long long s0, s1;     /* element strides of the view (a transposed weight has s0 == 1) */
+    long long first;      /* first tile */
+    int rows, cols;
+} regtr_split_view;
+
+/* Re-split updated weights into their existing (hi, lo) buffers with the rounding of regtr_split_tf32 (the result
+ * is bit-identical to a fresh split of the view); transposed views go through a shared-memory tile so that reads
+ * and writes coalesce.  One launch. */
+int regtr_split_refresh(const regtr_split_view* table, int n_views, int n_tiles, void* stream);
+
 /* ---- pose ------------------------------------------------------------------------- */
 
 /* Weighted Kabsch.  Replaces compute_rigid_transform (utils/se3_torch.py:108-154):

@@ -45,14 +45,16 @@ _COMMON = dict(
     aggregation_mode='sum', fixed_kernel_points='center', in_feats_dim=1, in_points_dim=3,
     deform_radius=5.0, KP_extent=2.0, KP_influence='linear', use_batch_norm=True,
     batch_norm_momentum=0.02, modulated=False, num_kernel_points=15,
+    # solver section (conf/*.yaml: `solver:`): read by RegTR.configure_optimizers
+    optimizer='AdamW', base_lr=1e-4, weight_decay=1e-4, grad_clip=0.1, scheduler='step',
 )
 
 
 def regtr_3dmatch() -> Cfg:
-    """Values of src/conf/3dmatch.yaml (kpconv_options 35-55, model 58-80, losses 83-103)."""
+    """Values of src/conf/3dmatch.yaml (solver 17-23, kpconv_options 35-55, model 58-80, losses 83-103)."""
     c = dict(_COMMON)
     c.update(
-        dataset='3dmatch', num_layers=4, neighborhood_limits=[40, 40, 40, 40],
+        dataset='3dmatch', scheduler_param=[205860, 0.5], num_layers=4, neighborhood_limits=[40, 40, 40, 40],
         first_subsampling_dl=0.025, first_feats_dim=128, conv_radius=2.5, overlap_radius=0.0375,
         r_p=0.2, r_n=0.4,
         architecture=['simple', 'resnetb', 'resnetb_strided', 'resnetb', 'resnetb',
@@ -63,10 +65,10 @@ def regtr_3dmatch() -> Cfg:
 
 
 def regtr_modelnet() -> Cfg:
-    """Values of src/conf/modelnet.yaml (kpconv_options 37-58, model 61-83, losses 86-106)."""
+    """Values of src/conf/modelnet.yaml (solver 25-31, kpconv_options 37-58, model 61-83, losses 86-106)."""
     c = dict(_COMMON)
     c.update(
-        dataset='modelnet', num_layers=2, neighborhood_limits=[50, 50],
+        dataset='modelnet', scheduler_param=[127800, 0.5], num_layers=2, neighborhood_limits=[50, 50],
         first_subsampling_dl=0.03, first_feats_dim=512, conv_radius=2.75, overlap_radius=0.04,
         r_p=0.12, r_n=0.24,
         architecture=['simple', 'resnetb', 'resnetb', 'resnetb_strided', 'resnetb', 'resnetb'],

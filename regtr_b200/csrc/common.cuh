@@ -43,6 +43,14 @@ __device__ __forceinline__ void regtr_row_col(unsigned t, unsigned w, int& row, 
     else { row = (int)(t / w); col = (int)(t - (unsigned)row * w); }
 }
 
+// round-to-nearest-even to TF32 precision (10 mantissa bits): the hi half of regtr_split_tf32 (x = hi + lo with
+// lo = regtr_tf32_rne(x - hi)); unbiased, so split errors do not accumulate linearly along K as truncation does
+__device__ __forceinline__ float regtr_tf32_rne(float x) {
+    uint32_t u = __float_as_uint(x);
+    u += 0x0FFFu + ((u >> 13) & 1u);
+    return __uint_as_float(u & 0xFFFFE000u);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -105,13 +105,8 @@ constexpr int BM = 128;
 constexpr int BK = 32;                       // fp32 elements = 128 bytes = one swizzle span
 constexpr uint32_t HI_MASK = 0xFFFFE000u;    // keep sign, exponent and 10 mantissa bits
 
-// round-to-nearest-even to TF32 precision (10 mantissa bits); unbiased, so split errors do not
-// accumulate linearly along K as plain truncation does
-__device__ __forceinline__ float tf32_hi(float x) {
-    uint32_t u = __float_as_uint(x);
-    u += 0x0FFFu + ((u >> 13) & 1u);
-    return __uint_as_float(u & HI_MASK);
-}
+// round-to-nearest-even to TF32 precision (common.cuh; regtr_split_refresh uses the same rounding)
+__device__ __forceinline__ float tf32_hi(float x) { return regtr_tf32_rne(x); }
 
 __global__ void k_split_tf32(const float* __restrict__ x, long long n, float* __restrict__ hi, float* __restrict__ lo) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;

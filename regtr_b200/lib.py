@@ -81,6 +81,11 @@ SIGNATURES = {
     'regtr_max_pool_bwd': (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _Z, _P]),
     'regtr_instnorm_bwd_ws_bytes': (_Z, [_I, _I, _I]),
     'regtr_instnorm_bwd': (_I, [_P, _P, _P, _P, _I, _I, _I, _F, _F, _P, _P, _P, _Z, _P]),
+    'regtr_grad_norm_ws_bytes': (_Z, [_I]),
+    'regtr_grad_norm': (_I, [_P, _I, _I, _F, _P, _P, _Z, _P]),
+    'regtr_grad_scale': (_I, [_P, _I, _I, _P, _P]),
+    'regtr_adam_step': (_I, [_P, _I, _I, _P]),
+    'regtr_split_refresh': (_I, [_P, _I, _I, _P]),
     'regtr_kabsch_fwd': (_I, [_P, _P, _P, _P, _I, _P, _P]),
     'regtr_pose_from_corr': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),

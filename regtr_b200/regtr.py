@@ -196,6 +196,32 @@ class RegTR(nn.Module):
         with torch.no_grad():
             return losses.compute_loss(self, pred, batch)
 
+    def configure_optimizers(self):
+        """The reference's solver (generic_reg_model.py:28-62) over self.parameters(), on the library's optimizer:
+        cfg.optimizer 'AdamW' / 'Adam' (lr cfg.base_lr, weight_decay cfg.weight_decay) and cfg.scheduler 'step'
+        (StepLR(*cfg.scheduler_param)) or 'none' (StepLR(50, 1.0)).  Sets and returns (self.optimizer, self.scheduler).
+        Clip the gradients to cfg.grad_clip with regtr_b200.optim.clip_grad_norm_ before every optimizer.step()."""
+        from . import optim
+        cfg = self.cfg
+        scheduler_type = cfg.get('scheduler', None)
+        if scheduler_type == 'warmup':
+            raise NotImplementedError("configure_optimizers: scheduler 'warmup' (no shipped config selects it)")
+        if scheduler_type not in (None, 'none', 'step'):
+            raise NotImplementedError(f'configure_optimizers: scheduler {scheduler_type!r}')
+        if cfg.optimizer == 'AdamW':
+            self.optimizer = optim.AdamW(self.parameters(), lr=cfg.base_lr, weight_decay=cfg.weight_decay)
+        elif cfg.optimizer == 'Adam':
+            self.optimizer = optim.Adam(self.parameters(), lr=cfg.base_lr, weight_decay=cfg.weight_decay)
+        else:
+            raise NotImplementedError(f'configure_optimizers: optimizer {cfg.optimizer!r}')
+        if scheduler_type == 'step':
+            self.scheduler = torch.optim.lr_scheduler.StepLR(self.optimizer, cfg.scheduler_param[0],
+                                                             cfg.scheduler_param[1])
+        else:
+            self.scheduler = torch.optim.lr_scheduler.StepLR(self.optimizer, 50, 1.0)
+        self.logger.info(f'Using optimizer {self.optimizer} with scheduler {self.scheduler}')
+        return self.optimizer, self.scheduler
+
     def _check_trainable(self, train_encoder: bool = False):
         """forward_train covers the branches both reference configs select; anything else raises."""
         cfg = self.cfg
@@ -289,6 +315,10 @@ class GraphedRegTR:
     replayed back to back with CUDA events in between: `stage_ms()` then reports where a pair's
     latency goes (bench.py).  Every captured graph owns a private scratch namespace (ops.new_namespace):
     no graph ever shares or outlives a buffer another graph writes.
+
+    Training with validation in between: after the library optimizer's step() (regtr_b200.optim.AdamW / Adam) the
+    captured graphs stay valid -- the step rewrites the split weights they read in place.  After a torch optimizer's
+    step the cached splits are dropped and rebuilt elsewhere, so call `invalidate()` before the next call.
     """
 
     STAGES = ('preprocess', 'encoder', 'attention_decoder', 'pose')
@@ -306,7 +336,8 @@ class GraphedRegTR:
         self.fallbacks = 0
         self.wait_s = 0.0               # host time spent blocked in result() waiting for the GPU (diagnostics)
         # the graphs bake in pointers to the split (hi, lo) weights: load_state_dict bumps the model's epoch and
-        # every graph is re-captured on its next use; in-place edits of a parameter need invalidate()
+        # every graph is re-captured on its next use; regtr_b200.optim's step() rewrites the splits in place (the
+        # graphs stay valid); any other in-place edit of a parameter (a torch optimizer's step) needs invalidate()
         self._epoch = getattr(model, '_weights_epoch', 0)
         if not hasattr(model, '_weights_epoch'):
             model._weights_epoch = 0

@@ -1,8 +1,15 @@
 """Time training steps of the fine-tuning path: RegTR.forward_train + compute_loss + backward() with the KPConv
 encoder frozen (gradients of every parameter after the encoder), or with --train-encoder the full training step
-(forward_train(batch, train_encoder=True): gradients of every parameter except the kernel points).  No optimiser step.
+(forward_train(batch, train_encoder=True): gradients of every parameter except the kernel points).
 
     python scripts/bench_train.py [--config 2|3] [--pairs B] [--steps K] [--warmup W] [--train-encoder]
+                                  [--optimizer none|library|torch]
+
+--optimizer none (default) times forward + loss + backward only.  library / torch add the rest of the reference's
+training iteration to every step: clip_grad_norm_(cfg.grad_clip), AdamW.step() and StepLR.step() of
+RegTR.configure_optimizers() (regtr_b200.optim: library kernels) or of torch (torch.optim.AdamW with its default
+foreach path and torch.nn.utils.clip_grad_norm_).  The optimizer's time is reported from CUDA events of its own,
+with the library kernel launches per step (ops.LAUNCHES).
 
 Same workload as bench.py: seeded random weights, the synthetic 3DMatch-shaped pairs of the chosen BASELINE config
 (config 2: 1 pair per step, config 3: 8), the attention_impl='fp32' core.  CUDA events around the forward + loss
@@ -19,6 +26,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
+from regtr_b200 import ops  # noqa: E402
 from regtr_b200.config import get_config  # noqa: E402
 from regtr_b200.regtr import RegTR  # noqa: E402
 from regtr_b200.synthetic import make_batch  # noqa: E402
@@ -47,6 +55,8 @@ def main():
     ap.add_argument('--steps', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--train-encoder', action='store_true', help='train the KPConv encoder too (full training step)')
+    ap.add_argument('--optimizer', default='none', choices=['none', 'library', 'torch'],
+                    help='add clip + AdamW + StepLR on the library kernels or torch\'s to every step')
     args = ap.parse_args()
     if args.steps < 1:
         ap.error('--steps must be >= 1')
@@ -59,6 +69,16 @@ def main():
     model.load_state_dict(random_state_dict(cfg, WEIGHT_SEED), strict=True)
     if not args.train_encoder:
         model.kpf_encoder.requires_grad_(False)
+    opt = sched = clip = None
+    if args.optimizer == 'library':
+        from regtr_b200 import optim
+        opt, sched = model.configure_optimizers()
+        clip = optim.clip_grad_norm_
+    elif args.optimizer == 'torch':
+        opt = torch.optim.AdamW(model.parameters(), lr=cfg.base_lr, weight_decay=cfg.weight_decay)
+        sched = torch.optim.lr_scheduler.StepLR(opt, cfg.scheduler_param[0], cfg.scheduler_param[1])
+        clip = torch.nn.utils.clip_grad_norm_
+    opt_launches = []
     n_pool = max(POOL, B)
     b = make_batch(2, n_pool)
     pool = [(torch.from_numpy(s).to(dev), torch.from_numpy(t).to(dev)) for s, t in zip(b['src_xyz'], b['tgt_xyz'])]
@@ -80,6 +100,14 @@ def main():
         total.backward()
         if evs:
             evs[2].record()
+        if opt is not None:
+            n0 = ops.LAUNCHES
+            clip(model.parameters(), cfg.grad_clip)
+            opt.step()
+            sched.step()
+            if evs:
+                evs[3].record()
+                opt_launches.append(ops.LAUNCHES - n0)
 
     for i in range(args.warmup):
         step(i)
@@ -87,13 +115,19 @@ def main():
     timed = []
     for i in range(args.steps):
         flush.zero_()
-        evs = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        evs = [torch.cuda.Event(enable_timing=True) for _ in range(3 if opt is None else 4)]
         step(args.warmup + i, evs)
         timed.append(evs)
     torch.cuda.synchronize()
     fwd = sum(e[0].elapsed_time(e[1]) for e in timed)
     bwd = sum(e[1].elapsed_time(e[2]) for e in timed)
     name, power = card()
+    extra = {}
+    if opt is not None:
+        ost = sum(e[2].elapsed_time(e[3]) for e in timed)
+        extra = dict(optimizer=args.optimizer, optimizer_ms_per_step=ost / args.steps,
+                     train_ms_per_step_with_optimizer=(fwd + bwd + ost) / args.steps,
+                     optimizer_library_launches_per_step=sum(opt_launches) / args.steps)
     print(json.dumps(dict(
         metric='training steps/s of forward_train + compute_loss + backward ' +
                ('(KPConv encoder trained)' if args.train_encoder else '(KPConv encoder frozen)'),
@@ -102,7 +136,7 @@ def main():
         steps=args.steps, warmup=args.warmup, train_pairs_per_s=B * args.steps / ((fwd + bwd) * 1e-3),
         train_ms_per_step=(fwd + bwd) / args.steps, train_forward_ms_per_step=fwd / args.steps,
         train_backward_ms_per_step=bwd / args.steps, train_backward_share=bwd / (fwd + bwd),
-        gpu=name, power_limit=power)), flush=True)
+        **extra, gpu=name, power_limit=power)), flush=True)
 
 
 if __name__ == '__main__':
