@@ -39,6 +39,7 @@ extern "C" {
 #define REGTR_STATUS_KEY_RANGE 1u /* a voxel / cell coordinate left the 16-bit key range */
 #define REGTR_STATUS_CAPACITY 2u  /* a capacity-bounded output (sub-sampled level) overflowed; results truncated */
 #define REGTR_STATUS_GRID 4u      /* voxel bounding box beyond the dense-grid budget: redo with regtr_grid_subsample_sorted */
+#define REGTR_STATUS_RANGE 8u     /* overlap search: |coordinate| beyond regtr_overlap_coord_bound; neighbours may be missed */
 
 int regtr_version(void);                 /* ABI version, currently 1 */
 const char* regtr_build_info(void);      /* host pointer: arch + compile flags string */
@@ -439,6 +440,51 @@ int regtr_kabsch_fwd(const float* a, const float* b, const float* w, const int32
  * w=[sigmoid(src_logit) ; sigmoid(tgt_logit)]. */
 int regtr_pose_from_corr(const float* kp, const float* corr, const float* logit,
                          const int32_t* offs, int n, int B, int L, float* pose, void* stream);
+
+/* ---- training data (3DMatch) ------------------------------------------------------ */
+
+/* Overlap ground truth of B pairs.  Replaces compute_overlap (utils/pointcloud.py:8-65) on the aligned clouds
+ * (data_loaders/threedmatch.py:79-86).  xyz (n_cap,3) float64 stacked src_0..src_{B-1}, tgt_0..tgt_{B-1} with
+ * offs (2B+1) i32; pose (B,3,4) float64 maps source to target.  The sources are moved by the pose in float64
+ * (((r0 x + r1 y) + r2 z) + t, no contraction); one cell list over the fp32 copy of all 2B clouds (cell `cell`, use
+ * radius * (1 + 1e-3)); per point the NEAREST point of the partner cloud with float64 squared distance strictly below
+ * radius^2, equal distances to the lowest index: nn (n_cap) i32 = its index inside the partner cloud, or -1.
+ * A |coordinate| of an aligned point beyond regtr_overlap_coord_bound(radius, cell) raises REGTR_STATUS_RANGE: past
+ * it the fp32 cell assignment could hide a neighbour.  ws / state: the *_bytes functions below (state ZERO before the
+ * first call; every call leaves it zero). */
+double regtr_overlap_coord_bound(double radius, float cell);
+size_t regtr_overlap_ws_bytes(int n_cap);
+size_t regtr_overlap_state_bytes(int n_cap);
+int regtr_overlap_nn(const double* xyz, const int32_t* offs, int B, int n_cap, const double* pose, double radius,
+                     float cell, int32_t* nn, uint32_t* status, void* ws, size_t ws_bytes, void* state,
+                     size_t state_bytes, void* stream);
+
+/* Per-pair flags of regtr_train_augment */
+#define REGTR_PREP_PERTURB_SRC 1  /* the perturbation moves the source (else the target) */
+#define REGTR_PREP_CENTRE 2       /* rotate about the perturbed cloud's centroid ('small' mode) */
+#define REGTR_PREP_SWAP 4         /* swap source and target */
+#define REGTR_PREP_SHUFFLE 8      /* permute the points (and truncate to max_pts) */
+
+/* The reference's training augmentations (data_loaders/transforms.py:15-149: RigidPerturb -> Jitter ->
+ * ShufflePoints -> RandomSwap) applied to the clouds of regtr_overlap_nn, with its nn as the overlap.
+ * pert (B,3,4) float64: the host-drawn perturbation P; flags (B) i32: REGTR_PREP_*.  Pose: pose P'^-1 (source
+ * perturbed) or P' pose, inverted when swapped, P' = P about the centroid with REGTR_PREP_CENTRE.  Output slot s of
+ * the augmented batch (src_0..src_{B-1}, tgt_0..) holds out_offs[s+1] - out_offs[s] = min(n, max_pts) points (no
+ * truncation without SHUFFLE) of its input cloud: out_xyz[k] = fp32(P' x[perm(k)] + noise * N(0,1)^3) with perm a
+ * keyed bijection (Feistel network, cycle walking) and the normals from Philox4x32-10 keyed by (seed, step, pair,
+ * side, point index); out_mask (out_cap bytes) = nn >= 0 of that point.  out_pose (B,3,4) fp32.
+ * corr (2, corr_cap >= n_src_cap) i32: mutual matches with a nonzero target index whose ends survive the truncation,
+ * in ascending source index, remapped through the permutation (rows swapped for swapped pairs); pair b owns columns
+ * [corr_offs[b], corr_offs[b+1]).  n_src_cap >= offs[B].  ws / state: the *_bytes functions (state ZERO before the
+ * first call; every call leaves it zero). */
+size_t regtr_train_augment_ws_bytes(int n_src_cap, int B);
+size_t regtr_train_augment_state_bytes(int n_src_cap);
+int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
+                        const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
+                        unsigned long long step, double noise, int max_pts, const int32_t* out_offs, int out_cap,
+                        float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
+                        int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
+                        void* stream);
 
 /* ---- status word helpers (device uint32) ------------------------------------------ */
 int regtr_status_clear(uint32_t* status, void* stream);

@@ -8,8 +8,8 @@ Host-side mirror of the inference branch of
   * `collate_pair` (/root/reference/src/data_loaders/collate_functions.py:4-22): variable-size fields stay
     python lists, `pose` is stacked (B,3,4), `overlap_p` becomes a tensor.
 The overlap masks / correspondences the losses need are computed on the fly (`compute_overlap`, the branch the
-reference takes when its precomputed h5 file is missing); the training augmentation transforms are outside
-this round's scope (SURVEY.md 8f N3).
+reference takes when its precomputed h5 file is missing); with `float64=True` the clouds stay float64 for
+`augment.TrainingPrep`, which computes the overlap and the training augmentations on the device.
 
 At >1k pairs/s per GPU the loader is part of the path: `PairStream` reads ahead on worker threads, pins the
 host clouds (so that `GraphedRegTR.submit` can issue asynchronous H2D copies straight into its static
@@ -61,11 +61,16 @@ class ThreeDMatchPairs(torch.utils.data.Dataset):
     idx, src_path, tgt_path, overlap_p}.  `root` holds the `test/<scene>/cloud_bin_<i>.pth` files,
     `info_file` is the benchmark's pickle."""
 
-    def __init__(self, root: str, info_file: str, pin: bool = False, overlap_radius: Optional[float] = None):
+    def __init__(self, root: str, info_file: str, pin: bool = False, overlap_radius: Optional[float] = None,
+                 float64: bool = False):
         """overlap_radius (cfg.overlap_radius, 0.0375 for 3DMatch): also produce the training / loss fields
         `src_overlap`, `tgt_overlap`, `correspondences` like the reference does when the precomputed h5 file is
-        missing (threedmatch.py:79-86)."""
-        self.overlap_radius = overlap_radius
+        missing (threedmatch.py:79-86).
+        float64=True: `src_xyz`, `tgt_xyz` and `pose` stay float64 as stored on disk -- the input of
+        `augment.TrainingPrep`, which computes the overlap on the device (no CPU overlap then)."""
+        if float64 and overlap_radius is not None:
+            raise ValueError('float64=True leaves the overlap to augment.TrainingPrep: pass no overlap_radius')
+        self.overlap_radius, self.float64 = overlap_radius, bool(float64)
         with open(info_file, 'rb') as fid:
             self.infos = pickle.load(fid)
         for k in ('rot', 'trans', 'src', 'tgt', 'overlap'):
@@ -78,13 +83,15 @@ class ThreeDMatchPairs(torch.utils.data.Dataset):
 
     def _cloud(self, rel):
         xyz = torch.load(os.path.join(self.root, rel), weights_only=False)
-        t = torch.from_numpy(np.asarray(xyz)).float()                  # float64 ndarray on disk (threedmatch.py:91)
+        t = torch.from_numpy(np.asarray(xyz))                          # float64 ndarray on disk (threedmatch.py:91)
+        t = t.double() if self.float64 else t.float()
         return t.pin_memory() if self.pin else t
 
     def __getitem__(self, item):
         pose = np.concatenate([self.infos['rot'][item], self.infos['trans'][item]], axis=-1)   # se3_init
+        pose_t = torch.from_numpy(np.asarray(pose, dtype=np.float64))
         out = {'src_xyz': self._cloud(self.infos['src'][item]), 'tgt_xyz': self._cloud(self.infos['tgt'][item]),
-               'pose': torch.from_numpy(pose).float(), 'idx': item,
+               'pose': pose_t if self.float64 else pose_t.float(), 'idx': item,
                'src_path': self.infos['src'][item], 'tgt_path': self.infos['tgt'][item],
                'overlap_p': self.infos['overlap'][item]}
         if self.overlap_radius is not None:

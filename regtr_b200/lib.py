@@ -88,6 +88,14 @@ SIGNATURES = {
     'regtr_split_refresh': (_I, [_P, _I, _I, _P]),
     'regtr_kabsch_fwd': (_I, [_P, _P, _P, _P, _I, _P, _P]),
     'regtr_pose_from_corr': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P]),
+    'regtr_overlap_coord_bound': (_c.c_double, [_c.c_double, _F]),
+    'regtr_overlap_ws_bytes': (_Z, [_I]),
+    'regtr_overlap_state_bytes': (_Z, [_I]),
+    'regtr_overlap_nn': (_I, [_P, _P, _I, _I, _P, _c.c_double, _F, _P, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_train_augment_ws_bytes': (_Z, [_I, _I]),
+    'regtr_train_augment_state_bytes': (_Z, [_I]),
+    'regtr_train_augment': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _c.c_ulonglong, _c.c_ulonglong, _c.c_double, _I,
+                                 _P, _I, _P, _P, _P, _P, _I, _P, _P, _Z, _P, _Z, _P]),
     'regtr_status_clear': (_I, [_P, _P]),
 }
 

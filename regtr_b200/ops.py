@@ -1006,3 +1006,61 @@ def pose_from_corr(kp, corr, logit, offs, B: int):
                'regtr_pose_from_corr')
     _count(1)
     return pose
+
+
+# --------------------------------------------------------------------------- training data
+
+PREP_PERTURB_SRC, PREP_CENTRE, PREP_SWAP, PREP_SHUFFLE = 1, 2, 4, 8     # REGTR_PREP_*
+STATUS_RANGE = 8                                                         # REGTR_STATUS_RANGE
+
+
+def overlap_cell(radius: float) -> float:
+    """Cell size of the overlap search's cell list: radius * (1 + 1e-3), rounded to fp32."""
+    return float(torch.tensor(radius * (1.0 + 1e-3), dtype=torch.float32))
+
+
+def overlap_coord_bound(radius: float) -> float:
+    """Largest |coordinate| (aligned clouds) for which the overlap search is exact (REGTR_STATUS_RANGE beyond)."""
+    return float(_lib.load().regtr_overlap_coord_bound(float(radius), overlap_cell(radius)))
+
+
+def overlap_nn(xyz, offs, B: int, pose, radius: float, status):
+    """Nearest point of the partner cloud within `radius` (float64, strict, lowest index on ties) for every point of
+    the stacked float64 clouds src_0..src_{B-1}, tgt_0..tgt_{B-1}; sources moved by `pose` (B,3,4) float64 first.
+    -> nn (n,) int32: index inside the partner cloud or -1.  No host sync."""
+    L = _lib.load()
+    _chk(xyz, torch.float64, 'xyz', 2); _chk(offs, torch.int32, 'offs', 1); _chk(pose, torch.float64, 'pose', 3)
+    n = xyz.shape[0]
+    nn = torch.empty(max(n, 1), dtype=torch.int32, device=xyz.device)
+    ws = workspace(L.regtr_overlap_ws_bytes(n), xyz.device)
+    state = workspace(L.regtr_overlap_state_bytes(n), xyz.device, 'scan_state', zero=True)
+    _lib.check(L.regtr_overlap_nn(_p(xyz), _p(offs), B, n, _p(pose), float(radius), overlap_cell(radius), _p(nn),
+                                  _p(status), _p(ws), ws.numel(), _p(state), state.numel(), _stream()),
+               'regtr_overlap_nn')
+    _count(6 if n > 0 else 0)
+    return nn[:n]
+
+
+def train_augment(xyz, offs, B: int, n_src: int, pose, nn, pert, flags, seed: int, step: int, noise: float,
+                  max_pts: int, out_offs, out_total: int):
+    """The augmentations of regtr_train_augment on the clouds / overlap of `overlap_nn`.
+    -> (out_xyz (out_total,3) f32, out_mask (out_total,) bool, out_pose (B,3,4) f32, corr (2, n_src) i32,
+        corr_offs (B+1) i32).  No host sync."""
+    L = _lib.load()
+    _chk(xyz, torch.float64, 'xyz', 2); _chk(pose, torch.float64, 'pose', 3); _chk(pert, torch.float64, 'pert', 3)
+    _chk(flags, torch.int32, 'flags', 1); _chk(out_offs, torch.int32, 'out_offs', 1); _chk(nn, torch.int32, 'nn', 1)
+    dev = xyz.device
+    out_xyz = torch.empty((out_total, 3), dtype=torch.float32, device=dev)
+    out_mask = torch.empty(out_total, dtype=torch.bool, device=dev)
+    out_pose = torch.empty((B, 3, 4), dtype=torch.float32, device=dev)
+    corr = torch.empty((2, max(n_src, 1)), dtype=torch.int32, device=dev)
+    corr_offs = torch.empty(B + 1, dtype=torch.int32, device=dev)
+    ws = workspace(L.regtr_train_augment_ws_bytes(n_src, B), dev)
+    state = workspace(L.regtr_train_augment_state_bytes(n_src), dev, 'scan_state', zero=True)
+    _lib.check(L.regtr_train_augment(_p(xyz), _p(offs), B, n_src, _p(pose), _p(nn), _p(pert), _p(flags),
+                                     int(seed) & (2**64 - 1), int(step) & (2**64 - 1), float(noise), int(max_pts),
+                                     _p(out_offs), out_total, _p(out_xyz), _p(out_mask), _p(out_pose), _p(corr),
+                                     corr.shape[1], _p(corr_offs), _p(ws), ws.numel(), _p(state), state.numel(),
+                                     _stream()), 'regtr_train_augment')
+    _count(5 if out_total > 0 else 4)
+    return out_xyz, out_mask, out_pose, corr, corr_offs
