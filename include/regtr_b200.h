@@ -486,6 +486,50 @@ int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src
                         int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
                         void* stream);
 
+/* ---- training-loop bookkeeping ---------------------------------------------------- */
+
+#define REGTR_METER_MAX_KEYS 16
+#define REGTR_METER_MAX_BANKS 4
+
+/* One step's loss scalars into device-resident meter banks (utils/misc.py AverageMeter.update, StatsMeter) and the
+ * trainer's loss_smooth EMA (trainer.py:127-134).  The struct lives in host memory and is passed to the kernel by
+ * value: no descriptor upload.  Every pointer inside is device memory.
+ *   bank b, key k: banks[b][4k .. 4k+3] = (val, sum, sq_sum, count) in fp64; a NaN value is skipped (math.isnan:
+ *   +-inf is accumulated), else val = v, sum += v, sq_sum += v * v, count += 1 with IEEE double roundings (no FMA),
+ *   so the sums equal Python floats fed the same .item() values.  All-zero rows are cleared meters.
+ *   smooth (NULL: no EMA) = [loss_smooth, 1.0 once set], fed by vals[total_key]: the first value is taken as it is;
+ *   afterwards a non-finite value is skipped and its step appended to log, else s = 0.99 s + 0.01 v.
+ *   log (NULL: none) = [n, step_1 .. step_log_cap]: n counts every skipped step, the first log_cap are kept.
+ * One launch. */
+typedef struct {
+    const float* vals[REGTR_METER_MAX_KEYS];  /* 0-d fp32 loss values, one per key */
+    double* banks[REGTR_METER_MAX_BANKS];     /* (n_keys, 4) fp64 each */
+    double* smooth;
+    long long* log;
+    long long step;                           /* recorded in the log */
+    int n_keys, n_banks;
+    int total_key;                            /* index of 'total' in vals, or -1: no EMA */
+    int log_cap;
+} regtr_meter_args;
+int regtr_meter_update(const regtr_meter_args* args, void* stream);
+
+/* Pose errors of one validation batch (utils/se3_torch.py se3_compare, generic_reg_model.py _compute_metrics /
+ * _aggregate_metrics): for layer l < L and pair b < B, in fp64 from the fp32 inputs, with R = Ra Rb^T,
+ *   rot = acos(clamp(0.5 (trace R - 1), -1, 1)) * 180 / pi,   trans = || ta - R tb ||.
+ * rot_hist / trans_hist (L, hist_cap) fp64 get them at columns [offset, offset + B); acc (L, 4) fp64 accumulates
+ * (sum rot, sum trans, n_success, n) pair by pair in order; success = rot < thresh_rot && trans < thresh_trans.
+ * One launch. */
+typedef struct {
+    const float* pred;    /* (L, B, 3, 4) predicted poses */
+    const float* gt;      /* (B, 3, 4) ground truth */
+    double* rot_hist;
+    double* trans_hist;
+    double* acc;
+    double thresh_rot, thresh_trans;
+    int L, B, offset, hist_cap;
+} regtr_pose_err_args;
+int regtr_pose_errors(const regtr_pose_err_args* args, void* stream);
+
 /* ---- status word helpers (device uint32) ------------------------------------------ */
 int regtr_status_clear(uint32_t* status, void* stream);
 

@@ -57,6 +57,9 @@ def regtr_3dmatch() -> Cfg:
         dataset='3dmatch', scheduler_param=[205860, 0.5], num_layers=4, neighborhood_limits=[40, 40, 40, 40],
         first_subsampling_dl=0.025, first_feats_dim=128, conv_radius=2.5, overlap_radius=0.0375,
         r_p=0.2, r_n=0.4,
+        # dataset / train_options sections (conf/3dmatch.yaml 4-15): read by regtr_b200.train
+        root='../data/indoor', augment_noise=0.005, perturb_pose='small', train_batch_size=2, val_batch_size=2,
+        test_batch_size=1, niter=-70,
         architecture=['simple', 'resnetb', 'resnetb_strided', 'resnetb', 'resnetb',
                       'resnetb_strided', 'resnetb', 'resnetb', 'resnetb_strided',
                       'resnetb', 'resnetb'],

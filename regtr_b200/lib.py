@@ -96,6 +96,8 @@ SIGNATURES = {
     'regtr_train_augment_state_bytes': (_Z, [_I]),
     'regtr_train_augment': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _c.c_ulonglong, _c.c_ulonglong, _c.c_double, _I,
                                  _P, _I, _P, _P, _P, _P, _I, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_meter_update': (_I, [_P, _P]),
+    'regtr_pose_errors': (_I, [_P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),
 }
 

@@ -10,6 +10,7 @@ import contextlib
 import itertools
 import math
 
+import numpy as np
 import torch
 
 from . import lib as _lib
@@ -1064,3 +1065,68 @@ def train_augment(xyz, offs, B: int, n_src: int, pose, nn, pert, flags, seed: in
                                      _stream()), 'regtr_train_augment')
     _count(5 if out_total > 0 else 4)
     return out_xyz, out_mask, out_pose, corr, corr_offs
+
+
+# --------------------------------------------------------------------------- training-loop bookkeeping
+
+METER_MAX_KEYS, METER_MAX_BANKS = 16, 4                                   # REGTR_METER_MAX_*
+METER_ARGS = np.dtype([('vals', '<u8', (METER_MAX_KEYS,)), ('banks', '<u8', (METER_MAX_BANKS,)), ('smooth', '<u8'),
+                       ('log', '<u8'), ('step', '<i8'), ('n_keys', '<i4'), ('n_banks', '<i4'), ('total_key', '<i4'),
+                       ('log_cap', '<i4')])
+POSE_ERR_ARGS = np.dtype([('pred', '<u8'), ('gt', '<u8'), ('rot_hist', '<u8'), ('trans_hist', '<u8'), ('acc', '<u8'),
+                          ('thresh_rot', '<f8'), ('thresh_trans', '<f8'), ('L', '<i4'), ('B', '<i4'),
+                          ('offset', '<i4'), ('hist_cap', '<i4')])
+assert (METER_ARGS.itemsize, POSE_ERR_ARGS.itemsize) == (200, 72)        # the C structs' sizes
+
+
+def meter_update(vals, banks, step: int, total_key: int = -1, smooth=None, log=None):
+    """One step's loss values into meter banks (regtr_meter_update): vals, a list of 0-d fp32 CUDA tensors (one per
+    key, in the banks' key order); banks, (n_keys, 4) fp64 tensors (val, sum, sq_sum, count); smooth (2,) fp64 and
+    log (1 + capacity,) int64 for the EMA of vals[total_key].  One launch, no host sync."""
+    L = _lib.load()
+    if not 1 <= len(vals) <= METER_MAX_KEYS or len(banks) > METER_MAX_BANKS:
+        raise ValueError(f'meter_update: {len(vals)} keys, {len(banks)} banks (at most {METER_MAX_KEYS}, '
+                         f'{METER_MAX_BANKS})')
+    a = np.zeros((), METER_ARGS)
+    for k, v in enumerate(vals):
+        if v.numel() != 1:
+            raise ValueError('meter_update: every value must be a single element')
+        _chk(v, torch.float32, 'meter value')
+        a['vals'][k] = v.data_ptr()
+    for b, t in enumerate(banks):
+        _chk(t, torch.float64, 'meter bank', 2)
+        if tuple(t.shape) != (len(vals), 4):
+            raise ValueError(f'meter bank: expected ({len(vals)}, 4), got {tuple(t.shape)}')
+        a['banks'][b] = t.data_ptr()
+    if smooth is not None:
+        _chk(smooth, torch.float64, 'smooth', 1)
+    if log is not None:
+        _chk(log, torch.int64, 'log', 1)
+    a['smooth'], a['log'] = _p(smooth) or 0, _p(log) or 0
+    a['step'], a['n_keys'], a['n_banks'] = int(step), len(vals), len(banks)
+    a['total_key'] = int(total_key) if smooth is not None else -1
+    a['log_cap'] = log.numel() - 1 if log is not None else 0
+    _lib.check(L.regtr_meter_update(a.ctypes.data, _stream()), 'regtr_meter_update')
+    _count(1)
+
+
+def pose_errors(pred, gt, rot_hist, trans_hist, acc, offset: int, thresh_rot: float, thresh_trans: float):
+    """Pose errors of one validation batch (regtr_pose_errors): pred (L,B,3,4) and gt (B,3,4) fp32; writes
+    rot_hist / trans_hist (L, cap) fp64 at columns [offset, offset + B) and accumulates acc (L, 4) fp64
+    (sum rot, sum trans, n_success, n).  One launch, no host sync."""
+    L_ = _lib.load()
+    _chk(pred, torch.float32, 'pred', 4); _chk(gt, torch.float32, 'gt', 3)
+    _chk(rot_hist, torch.float64, 'rot_hist', 2); _chk(trans_hist, torch.float64, 'trans_hist', 2)
+    _chk(acc, torch.float64, 'acc', 2)
+    nl, B = pred.shape[0], pred.shape[1]
+    if tuple(pred.shape[2:]) != (3, 4) or tuple(gt.shape) != (B, 3, 4):
+        raise ValueError(f'pose_errors: pred {tuple(pred.shape)}, gt {tuple(gt.shape)}')
+    if tuple(acc.shape) != (nl, 4) or rot_hist.shape != trans_hist.shape or rot_hist.shape[0] != nl:
+        raise ValueError('pose_errors: history / accumulator shapes do not match the layers')
+    a = np.zeros((), POSE_ERR_ARGS)
+    a['pred'], a['gt'], a['rot_hist'], a['trans_hist'], a['acc'] = (
+        pred.data_ptr(), gt.data_ptr(), rot_hist.data_ptr(), trans_hist.data_ptr(), acc.data_ptr())
+    a['thresh_rot'], a['thresh_trans'] = float(thresh_rot), float(thresh_trans)
+    a['L'], a['B'], a['offset'], a['hist_cap'] = nl, B, int(offset), rot_hist.shape[1]
+    _lib.check(L_.regtr_pose_errors(a.ctypes.data, _stream()), 'regtr_pose_errors')
+    _count(1 if B else 0)
