@@ -486,6 +486,45 @@ int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src
                         int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
                         void* stream);
 
+/* ---- training data (ModelNet40) --------------------------------------------------- */
+
+#define REGTR_STATUS_INPUT 16u    /* ModelNet pairs: a shape index out of range or a coordinate that is not finite */
+#define REGTR_STATUS_CROP 32u     /* ModelNet pairs: a crop kept fewer than n_out points */
+#define REGTR_MODELNET_MAX_PTS 2048
+#define REGTR_MODELNET_PARAMS 18  /* doubles per pair in params: dir_src[3], dir_tgt[3], transform[12] */
+
+/* The reference's ModelNet crop chain (data_loaders/modelnet_transforms.py: SplitSourceRef -> RandomCrop ->
+ * RandomTransformSE3_euler -> Resampler -> RandomJitter -> ShufflePoints) for B pairs, one CTA per pair.  Pair b
+ * takes shape items[b] of shapes (n_shapes, n_pts <= REGTR_MODELNET_MAX_PTS, 3) fp32 and, per side (0 = source,
+ * 1 = target) with the crop direction of params[b]:
+ *   centroid c = fp32(S / n_pts), S the float64 sum of the points in a fixed order (see modelnet.cu);
+ *   d_i = ((fp64(x_i - c) u0 + fp64(y_i - c) u1) + fp64(z_i - c) u2), the differences in fp32, no contraction;
+ *   kept = d_i > thr, thr = numpy's linear interpolation between order statistics k and k + 1 of d with weight
+ *   gamma, or thr = 0 when k < 0 (RandomCrop with p_keep == 0.5);
+ *   the first n_out positions of a keyed Feistel bijection over the kept points, in ascending raw index, choose the
+ *   ordered subset; a source point is moved by params' 3x4 transform in float64 and rounded once to fp32; every point
+ *   gets fp32(fp64(x) + clip(noise * N(0,1), -clip, clip)), N(0,1) from Philox4x32-10 keyed by (seed, step, pair,
+ *   side, raw index).
+ * out_xyz (2B, n_out, 3): src_0..src_{B-1}, tgt_0..tgt_{B-1}; out_mask (2B, n_out): the raw point survives the other
+ * side's crop; corr (B, 2, n_out): (source position, target position) of every raw point present in both outputs, in
+ * ascending raw index, corr_n (B) of them.  A crop with fewer than n_out points raises REGTR_STATUS_CROP, a bad item
+ * or a non-finite coordinate REGTR_STATUS_INPUT; such a pair gets corr_n = 0.  The struct is passed by value.
+ * One launch. */
+typedef struct {
+    const float* shapes;
+    const double* params;     /* (B, REGTR_MODELNET_PARAMS) */
+    const int32_t* items;     /* (B) */
+    float* out_xyz;
+    uint8_t* out_mask;
+    int32_t* corr;
+    int32_t* corr_n;
+    uint32_t* status;
+    unsigned long long seed, step;
+    double gamma, noise, clip;
+    int n_shapes, n_pts, n_out, k, B;
+} regtr_modelnet_args;
+int regtr_modelnet_augment(const regtr_modelnet_args* args, void* stream);
+
 /* ---- training-loop bookkeeping ---------------------------------------------------- */
 
 #define REGTR_METER_MAX_KEYS 16

@@ -74,6 +74,12 @@ def regtr_modelnet() -> Cfg:
         dataset='modelnet', scheduler_param=[127800, 0.5], num_layers=2, neighborhood_limits=[50, 50],
         first_subsampling_dl=0.03, first_feats_dim=512, conv_radius=2.75, overlap_radius=0.04,
         r_p=0.12, r_n=0.24,
+        # dataset / train_options sections (conf/modelnet.yaml 4-23): read by regtr_b200.train and .modelnet
+        root='../data/modelnet40_ply_hdf5_2048', train_categoryfile='datasets/modelnet/modelnet40_half1.txt',
+        val_categoryfile='datasets/modelnet/modelnet40_half1.txt',
+        test_categoryfile='datasets/modelnet/modelnet40_half2.txt', partial=[0.7, 0.7], num_points=1024,
+        noise_type='crop', rot_mag=45.0, trans_mag=0.5, train_batch_size=4, val_batch_size=4, test_batch_size=1,
+        niter=-400,
         architecture=['simple', 'resnetb', 'resnetb', 'resnetb_strided', 'resnetb', 'resnetb'],
     )
     return Cfg(c)

@@ -98,6 +98,7 @@ SIGNATURES = {
                                  _P, _I, _P, _P, _P, _P, _I, _P, _P, _Z, _P, _Z, _P]),
     'regtr_meter_update': (_I, [_P, _P]),
     'regtr_pose_errors': (_I, [_P, _P]),
+    'regtr_modelnet_augment': (_I, [_P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),
 }
 

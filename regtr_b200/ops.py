@@ -1130,3 +1130,43 @@ def pose_errors(pred, gt, rot_hist, trans_hist, acc, offset: int, thresh_rot: fl
     a['L'], a['B'], a['offset'], a['hist_cap'] = nl, B, int(offset), rot_hist.shape[1]
     _lib.check(L_.regtr_pose_errors(a.ctypes.data, _stream()), 'regtr_pose_errors')
     _count(1 if B else 0)
+
+
+# --------------------------------------------------------------------------- training data (ModelNet40)
+
+STATUS_INPUT, STATUS_CROP = 16, 32                                        # REGTR_STATUS_INPUT / _CROP
+MODELNET_MAX_PTS, MODELNET_PARAMS = 2048, 18                              # REGTR_MODELNET_*
+MODELNET_ARGS = np.dtype([('shapes', '<u8'), ('params', '<u8'), ('items', '<u8'), ('out_xyz', '<u8'),
+                          ('out_mask', '<u8'), ('corr', '<u8'), ('corr_n', '<u8'), ('status', '<u8'), ('seed', '<u8'),
+                          ('step', '<u8'), ('gamma', '<f8'), ('noise', '<f8'), ('clip', '<f8'), ('n_shapes', '<i4'),
+                          ('n_pts', '<i4'), ('n_out', '<i4'), ('k', '<i4'), ('B', '<i4')], align=True)
+assert MODELNET_ARGS.itemsize == 128                                      # the C struct's size
+
+
+def modelnet_augment(shapes, params, items, seed: int, step: int, k: int, gamma: float, noise: float, clip: float,
+                     n_out: int, status):
+    """The ModelNet crop chain of B pairs (regtr_modelnet_augment): shapes (S, n_pts, 3) fp32; params
+    (B, MODELNET_PARAMS) fp64 = crop direction of the source, of the target, the source's 3x4 transform; items (B)
+    int32 shape indices.  -> (out_xyz (2B, n_out, 3) f32, out_mask (2B, n_out) bool, corr (B, 2, n_out) i32,
+    corr_n (B,) i32).  One launch, no host sync."""
+    L = _lib.load()
+    _chk(shapes, torch.float32, 'shapes', 3); _chk(params, torch.float64, 'params', 2); _chk(items, torch.int32, 'items', 1)
+    _chk(status, torch.int32, 'status', 1)
+    B = items.shape[0]
+    if tuple(params.shape) != (B, MODELNET_PARAMS):
+        raise ValueError(f'modelnet_augment: params {tuple(params.shape)}, expected ({B}, {MODELNET_PARAMS})')
+    dev = shapes.device
+    out_xyz = torch.empty((2 * B, n_out, 3), dtype=torch.float32, device=dev)
+    out_mask = torch.empty((2 * B, n_out), dtype=torch.bool, device=dev)
+    corr = torch.empty((B, 2, n_out), dtype=torch.int32, device=dev)
+    corr_n = torch.empty(B, dtype=torch.int32, device=dev)
+    a = np.zeros((), MODELNET_ARGS)
+    for f, t in (('shapes', shapes), ('params', params), ('items', items), ('out_xyz', out_xyz), ('out_mask', out_mask),
+                 ('corr', corr), ('corr_n', corr_n), ('status', status)):
+        a[f] = t.data_ptr()
+    a['seed'], a['step'] = int(seed) & (2**64 - 1), int(step) & (2**64 - 1)
+    a['gamma'], a['noise'], a['clip'] = float(gamma), float(noise), float(clip)
+    a['n_shapes'], a['n_pts'], a['n_out'], a['k'], a['B'] = shapes.shape[0], shapes.shape[1], int(n_out), int(k), B
+    _lib.check(L.regtr_modelnet_augment(a.ctypes.data, _stream()), 'regtr_modelnet_augment')
+    _count(1)
+    return out_xyz, out_mask, corr, corr_n

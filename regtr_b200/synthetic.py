@@ -158,3 +158,30 @@ def make_batch(config_id: int, n_pairs: int, first_pair: int = 0, n_target: int 
         for k in out:
             out[k].append(p[k])
     return out
+
+
+def make_modelnet_shapes(n_shapes: int, seed: int = 0, n_points: int = 2048, n_dup: int = 8) -> np.ndarray:
+    """(n_shapes, n_points, 3) float32 ModelNet40-like shapes (the h5 files hold 2048 points per shape): unions of
+    ellipsoid and box surfaces inside the unit ball, with `n_dup` points repeated so that crop distances tie."""
+    rng = np.random.default_rng(seed)
+    out = np.empty((n_shapes, n_points, 3), np.float32)
+    for s in range(n_shapes):
+        parts = []
+        k = int(rng.integers(2, 5))
+        sizes = np.diff(np.sort(np.concatenate([[0, n_points], rng.choice(np.arange(1, n_points), k - 1, replace=False)])))
+        for n in sizes:
+            c, r = rng.uniform(-0.3, 0.3, 3), rng.uniform(0.15, 0.45, 3)
+            if rng.random() < 0.5:
+                v = rng.normal(size=(n, 3)); v /= np.linalg.norm(v, axis=1, keepdims=True)
+                parts.append(c + v * r)
+            else:
+                f = rng.integers(0, 3, n); sign = rng.choice([-1.0, 1.0], n)
+                p = rng.uniform(-1, 1, (n, 3)); p[np.arange(n), f] = sign
+                parts.append(c + p * r)
+        shape = np.concatenate(parts, 0)
+        shape /= np.linalg.norm(shape, axis=1).max()
+        if n_dup:
+            dst = rng.choice(n_points, n_dup, replace=False)
+            shape[dst] = shape[rng.choice(np.setdiff1d(np.arange(n_points), dst), n_dup, replace=False)]
+        out[s] = shape
+    return out

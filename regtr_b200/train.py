@@ -1,13 +1,14 @@
-"""Train RegTR on 3DMatch: the reference's `src/train.py` on the library path.
+"""Train RegTR on 3DMatch or ModelNet40: the reference's `src/train.py` on the library path.
 
-    python -m regtr_b200.train --config 3dmatch [--logdir ../logs] [--name NAME] [--summary_every 500]
+    python -m regtr_b200.train --config 3dmatch|modelnet [--logdir ../logs] [--name NAME] [--summary_every 500]
         [--validate_every -1] [--debug] [--num_workers 4] [--resume CKPT] [--nb_sanity_val_steps 2]
         [--info-dir datasets/3dmatch] [--seed 0]
 
 --config is a reference-format YAML file (conf/3dmatch.yaml) or a builtin config name.  The training and validation
 pairs are listed in <info-dir>/train_info.pkl and <info-dir>/val_info.pkl (the reference reads the same files
-relative to its working directory); the clouds are under cfg.root.  Logs, config.yaml, tensorboard summaries and
-ckpt/ go to <logdir>/<dataset>/<yymmdd_HHMMSS>[_<name>].  With --resume and no --config, the config.yaml next to the
+relative to its working directory); the clouds are under cfg.root.  ModelNet40 reads the h5 files under cfg.root
+(this needs h5py) with the category files of the config, relative to the working directory as in the reference.
+Logs, config.yaml, tensorboard summaries and ckpt/ go to <logdir>/<dataset>/<yymmdd_HHMMSS>[_<name>].  With --resume and no --config, the config.yaml next to the
 checkpoint directory is used.  The reference's --dev flag (which deletes a log directory) is not provided.
 """
 from __future__ import annotations
@@ -23,7 +24,7 @@ BUILTIN = ('3dmatch', 'modelnet')
 
 def parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(prog='python -m regtr_b200.train')
-    ap.add_argument('--config', type=str, help='Path to the config file, or a builtin config name (3dmatch).')
+    ap.add_argument('--config', type=str, help='Path to the config file, or a builtin config name (3dmatch, modelnet).')
     ap.add_argument('--logdir', type=str, default='../logs', help='Directory to store logs, summaries, checkpoints.')
     ap.add_argument('--name', type=str, help='Experiment name (used to name output directory')
     ap.add_argument('--summary_every', type=int, default=500, help='Interval to save tensorboard summaries')
@@ -97,9 +98,9 @@ def main(argv=None):
     opt.config = resolve_config(opt)
     cfg = load_cfg(opt.config)
     if cfg.dataset == 'modelnet':
-        raise NotImplementedError('ModelNet training needs the ModelNet40 h5 loader and its transforms '
-                                  '(data_loaders/modelnet.py), which this package does not provide')
-    if cfg.dataset != '3dmatch':
+        from .modelnet import h5_reader
+        h5_reader()                      # fail before anything is created when the h5 files cannot be read
+    elif cfg.dataset != '3dmatch':
         raise NotImplementedError(f'dataset {cfg.dataset!r}')
     opt.logdir = os.path.join(opt.logdir, cfg.dataset)
     if opt.name is None and len(cfg.get('expt_name', '')) > 0:
@@ -112,8 +113,14 @@ def main(argv=None):
     from .trainer import Trainer
     if not os.path.isdir(cfg.root):
         raise AssertionError(f'Dataset not found in {cfg.root}')
-    train_set = ThreeDMatchPairs(cfg.root, os.path.join(opt.info_dir, 'train_info.pkl'), pin=True, float64=True)
-    val_set = ThreeDMatchPairs(cfg.root, os.path.join(opt.info_dir, 'val_info.pkl'), pin=True, float64=True)
+    if cfg.dataset == 'modelnet':
+        from . import modelnet as MN
+        train_set = MN.ModelNetShapes(cfg.root, 'train', MN.read_categories(cfg.get('train_categoryfile')))
+        val_set = MN.ModelNetPairs(MN.ModelNetShapes(cfg.root, 'test', MN.read_categories(cfg.get('val_categoryfile'))),
+                                   cfg)
+    else:
+        train_set = ThreeDMatchPairs(cfg.root, os.path.join(opt.info_dir, 'train_info.pkl'), pin=True, float64=True)
+        val_set = ThreeDMatchPairs(cfg.root, os.path.join(opt.info_dir, 'val_info.pkl'), pin=True, float64=True)
     model = RegTR(cfg)
     trainer = Trainer(opt, niter=cfg.niter, grad_clip=cfg.grad_clip, seed=opt.seed)
     trainer.fit(model, train_set, val_set)

@@ -1,9 +1,13 @@
-"""Training loop for RegTR on 3DMatch (SURVEY.md 8f N3): the reference's `Trainer.fit` / `_run_validation`
+"""Training loop for RegTR on 3DMatch and ModelNet40 (SURVEY.md 8f N3): the reference's `Trainer.fit` / `_run_validation`
 (src/trainer.py:38-175, 213-269), its `CheckPointManager` (cvhelpers/torch_helpers.py:98-242) and the bookkeeping of
 `GenericRegModel` (training_step, train_summary_fn, validation_step, validation_epoch_end), on the library path:
 
     data.PairStream (read-ahead, pinned float64 clouds) -> augment.TrainingPrep -> RegTR.forward_train(train_encoder=True)
     -> compute_loss -> backward -> optim.clip_grad_norm_ -> optim.AdamW.step -> StepLR.step -> ops.meter_update
+
+ModelNet40 (`model.cfg.dataset == 'modelnet'`): the training shapes live on the device and every batch is built by
+`modelnet.ModelNetPrep` from the epoch order's shape indices (one launch, no host data path); validation runs over
+the deterministic pairs of `modelnet.ModelNetPairs`.
 
 The reference reads every loss to the host on every step (AverageMeter.update calls .item(), and so does the
 loss_smooth EMA).  Here the meters, the EMA and the log of non-finite totals live on the device and are updated by one
@@ -263,7 +267,11 @@ class Trainer:
         model.to(dev)
         model.configure_optimizers()
         self.device = dev
-        self.prep = TrainingPrep(model.cfg, seed=self.seed)
+        if model.cfg.get('dataset') == 'modelnet':
+            from .modelnet import ModelNetPrep
+            self.prep = ModelNetPrep(model.cfg, train_set.to(dev), seed=self.seed)
+        else:
+            self.prep = TrainingPrep(model.cfg, seed=self.seed)
         self.epoch_meter = self.summary_meter = None
         self._smooth = torch.zeros(2, dtype=torch.float64, device=dev)
         self._log = torch.zeros(1 + LOG_CAPACITY, dtype=torch.int64, device=dev)
@@ -405,7 +413,10 @@ class Trainer:
                 model.train()
                 torch.set_grad_enabled(True)
                 t_epoch = time.perf_counter()
-                stream = iter(PairStream(train_set, batches[skip:], workers=opt.num_workers))
+                if model.cfg.get('dataset') == 'modelnet':
+                    stream = ({'idx': bt} for bt in batches[skip:])
+                else:
+                    stream = iter(PairStream(train_set, batches[skip:], workers=opt.num_workers))
                 try:
                     for batch_idx, batch in enumerate(stream, start=skip):
                         global_step += 1
@@ -460,11 +471,14 @@ class Trainer:
             self.logger.info(f'Running validation (step {step})...')
         n_pairs = sum(len(b) for b in batches)
         model.eval()
-        prep = TrainingPrep(cfg, seed=self.seed)
+        if cfg.get('dataset') == 'modelnet':          # deterministic pairs, already prepared
+            prep, stream = None, (val_set.collate(bt, self.device) for bt in batches)
+        else:
+            prep, stream = TrainingPrep(cfg, seed=self.seed), PairStream(val_set, batches, workers=self.opt.num_workers)
         meter, hist, acc, offset = None, None, None, 0
         with torch.no_grad():
-            for batch in PairStream(val_set, batches, workers=self.opt.num_workers):
-                b = prep(batch, augment=False)
+            for batch in stream:
+                b = batch if prep is None else prep(batch, augment=False)
                 pred = model(b)
                 losses = model.compute_loss(pred, b)
                 if meter is None:
@@ -477,7 +491,8 @@ class Trainer:
                 ops.pose_errors(pred['pose'].contiguous(), b['pose'].contiguous(), hist[0], hist[1], acc, offset,
                                 cfg.reg_success_thresh_rot, cfg.reg_success_thresh_trans)
                 offset += len(batch['src_xyz'])
-            prep.check()
+            if prep is not None:
+                prep.check()
         val_losses = meter.averages() if meter is not None else {}
         metrics = pose_metrics(acc, hist[:, :, :offset]) if acc is not None else {}
         if metrics:
