@@ -279,8 +279,10 @@ int regtr_mha_varlen_fwd_lse(const float* Q, int ldq, const float* K, int ldk, c
  * has no queries).  Each key row must belong to the key range of exactly one problem (true of the self and of the
  * cross table of regtr_attention_plan); dQ / dK / dV may be column slices of one packed [n_rows, 3E] buffer.
  * n_rows: rows of Q / lse (an upper bound of every query row index + 1); max_k_len: host bound of k_len[].
- * Deterministic (no atomics): one pass owns the query rows, a second one the key rows.
- * ws: regtr_mha_varlen_bwd_ws_bytes(n_rows, n_heads) bytes (rowsum(dO * O) per query and head). */
+ * Deterministic (no atomics): one pass owns the query rows, a second one the key rows.  The softmax is renormalised
+ * from the backward's own recomputed scores, and delta = sum_k P dP is formed from them too, so O is checked for
+ * NULL but its values are not read.
+ * ws: regtr_mha_varlen_bwd_ws_bytes(n_rows, n_heads) bytes (delta and 1 / sum_k exp2(s - lse) per query and head). */
 size_t regtr_mha_varlen_bwd_ws_bytes(int n_rows, int n_heads);
 int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
                          const float* O, int ldo, const float* dO, int lddo, const float* lse,

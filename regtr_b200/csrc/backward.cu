@@ -49,21 +49,47 @@ __device__ __forceinline__ void store_row(float* __restrict__ p, const float (&r
         reinterpret_cast<float4*>(p)[d] = make_float4(r[4 * d] * s, r[4 * d + 1] * s, r[4 * d + 2] * s, r[4 * d + 3] * s);
 }
 
+// keys / values [r0, r0 + nk) of one head into shared memory
+__device__ __forceinline__ void stage_kv(float (&sK)[CH][HD], float (&sV)[CH][HD], const float* __restrict__ Kp, int ldk,
+                                         const float* __restrict__ Vp, int ldv, size_t r0, int nk, int col) {
+    for (int f = threadIdx.x; f < nk * (HD / 4); f += BT) {
+        const int r = f >> 3, c4 = f & 7;
+        reinterpret_cast<float4*>(&sK[r][0])[c4] =
+            __ldg(reinterpret_cast<const float4*>(Kp + (r0 + r) * ldk + col) + c4);
+        reinterpret_cast<float4*>(&sV[r][0])[c4] =
+            __ldg(reinterpret_cast<const float4*>(Vp + (r0 + r) * ldv + col) + c4);
+    }
+}
+
+// s + c += x with the rounding error of the add carried in c (Knuth's TwoSum: exact for any order of magnitudes)
+__device__ __forceinline__ void two_sum_add(float& s, float& c, float x) {
+    const float t = __fadd_rn(s, x), b = __fsub_rn(t, s);       // _rn: never contracted into an FMA
+    c = __fadd_rn(c, __fadd_rn(__fsub_rn(s, __fsub_rn(t, b)), __fsub_rn(x, b)));
+    s = t;
+}
+
 // ---- attention backward ------------------------------------------------------------------------------------------
 // Scores are recomputed exactly as the forward (k_mha_tf32x3) scales them: s = (q * scale*log2e) . k, in base 2, and
-// P = exp2(s - lse) with the forward's ex2.approx.  The dot products run in fp32 FMA chains (round-to-nearest at every
+// p = exp2(s - lse) with the forward's ex2.approx.  The dot products run in fp32 FMA chains (round-to-nearest at every
 // step), which is at least as accurate as the forward's 3xTF32 tensor-core products.
 //
+// The softmax is made self-consistent in the backward's own arithmetic.  The forward's lse comes from 3xTF32 scores,
+// so sum_k p differs from 1 by about |s| * 1e-7, and rowsum(dO * O) from the forward's O differs from sum_k P dP by
+// as much.  Neither cancels in sum_k dS, and dQ / dK pick that error up multiplied by whatever k / q share (the
+// in-projection bias: softmax ignores a vector added to every key, so sum_k dK = 0 and dQ does not change).  So
+// pass 1 first sweeps the keys: Z = sum_k p and D = sum_k p dP, both compensated sums, give the normalised
+// P = p / Z and delta = D / Z = sum_k P dP from the very p and dP both passes use.
+//
 // Pass 1 (this kernel): block = (64-query tile, head, problem), one query per thread; keys stream through shared
-// memory.  delta = rowsum(dO * O);  dS = P * (dP - delta) with dP = dO . v;  dQ = scale * sum_k dS k.  delta is also
-// stored for pass 2.  Every query row belongs to exactly one problem, so every dQ row is written exactly once.
-// A problem with an empty key range has O = 0 and writes dQ = 0.
+// memory, twice.  dS = P * (dP - delta) with dP = dO . v;  dQ = scale * sum_k dS k.  delta and 1 / Z are stored for
+// pass 2.  Every query row belongs to exactly one problem, so every dQ row is written exactly once.  A problem with an
+// empty key range has Z = 0 and writes dQ = 0.
 __global__ void __launch_bounds__(BT)
 k_mha_bwd_dq(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp, int ldk, const float* __restrict__ Vp,
-             int ldv, const float* __restrict__ O, int ldo, const float* __restrict__ dO, int lddo,
-             const float* __restrict__ lse, float* __restrict__ delta, float* __restrict__ dQ, int lddq,
-             const int32_t* __restrict__ q_start, const int32_t* __restrict__ q_len, const int32_t* __restrict__ k_start,
-             const int32_t* __restrict__ k_len, float qscale, float scale) {
+             int ldv, const float* __restrict__ dO, int lddo, const float* __restrict__ lse, float* __restrict__ delta,
+             float* __restrict__ rnorm, float* __restrict__ dQ, int lddq, const int32_t* __restrict__ q_start,
+             const int32_t* __restrict__ q_len, const int32_t* __restrict__ k_start, const int32_t* __restrict__ k_len,
+             float qscale, float scale) {
     __shared__ __align__(16) float sK[CH][HD], sV[CH][HD];
     const int prob = blockIdx.z, head = blockIdx.y, tile = blockIdx.x, nh = gridDim.y;
     const int ql = q_len[prob];
@@ -77,25 +103,36 @@ k_mha_bwd_dq(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
     float q[HD], g[HD], acc[HD];
     load_row(Q + row * ldq + col, q, qscale);
     load_row(dO + row * lddo + col, g);
-    load_row(O + row * ldo + col, acc);
-    float dl = 0.f;
-#pragma unroll
-    for (int d = 0; d < HD; ++d) dl = fmaf(g[d], acc[d], dl);
-#pragma unroll
-    for (int d = 0; d < HD; ++d) acc[d] = 0.f;
     const float L = lse[row * nh + head];
-    if (active) delta[row * nh + head] = dl;
 
+    // compensated sums (TwoSum, and TwoProduct for p * dP): Z and D to about one rounding, whatever the key count
+    float z = 0.f, zc = 0.f, dsum = 0.f, dc = 0.f;
     for (int kb = 0; kb < kl; kb += CH) {
         const int nk = min(CH, kl - kb);
         __syncthreads();
-        for (int f = threadIdx.x; f < nk * (HD / 4); f += BT) {
-            const int r = f >> 3, c4 = f & 7;
-            reinterpret_cast<float4*>(&sK[r][0])[c4] =
-                __ldg(reinterpret_cast<const float4*>(Kp + (size_t)(k0 + kb + r) * ldk + col) + c4);
-            reinterpret_cast<float4*>(&sV[r][0])[c4] =
-                __ldg(reinterpret_cast<const float4*>(Vp + (size_t)(k0 + kb + r) * ldv + col) + c4);
+        stage_kv(sK, sV, Kp, ldk, Vp, ldv, (size_t)(k0 + kb), nk, col);
+        __syncthreads();
+        for (int j = 0; j < nk; ++j) {
+            const float p = fast_exp2(dot_smem(q, &sK[j][0]) - L);
+            two_sum_add(z, zc, p);
+            const float dp = dot_smem(g, &sV[j][0]);
+            const float pr = __fmul_rn(p, dp);
+            dc += fmaf(p, dp, -pr);
+            two_sum_add(dsum, dc, pr);
         }
+    }
+    z += zc;
+    dsum += dc;
+    const float rz = z > 0.f ? 1.f / z : 0.f;
+    const float dl = z > 0.f ? dsum / z : 0.f;
+    if (active) { delta[row * nh + head] = dl; rnorm[row * nh + head] = rz; }
+
+#pragma unroll
+    for (int d = 0; d < HD; ++d) acc[d] = 0.f;
+    for (int kb = 0; kb < kl; kb += CH) {
+        const int nk = min(CH, kl - kb);
+        __syncthreads();
+        stage_kv(sK, sV, Kp, ldk, Vp, ldv, (size_t)(k0 + kb), nk, col);
         __syncthreads();
         for (int j = 0; j < nk; ++j) {
             const float p = fast_exp2(dot_smem(q, &sK[j][0]) - L);
@@ -103,11 +140,11 @@ k_mha_bwd_dq(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
             axpy_smem(acc, ds, &sK[j][0]);
         }
     }
-    if (active) store_row(dQ + (size_t)(q0 + qi) * lddq + col, acc, scale);
+    if (active) store_row(dQ + (size_t)(q0 + qi) * lddq + col, acc, scale * rz);
 }
 
 // Pass 2: block = (64-key tile, head, problem), one key per thread; the problem's queries stream through shared
-// memory.  dV = sum_q P dO,  dK = scale * sum_q dS q.
+// memory.  P = exp2(s - lse) / Z with the same FMA chain for s as pass 1;  dV = sum_q P dO,  dK = scale * sum_q dS q.
 // Row ownership (what makes this pass atomic-free): every key row is written by the one problem whose key range
 // holds it.  In the self table each token is a key of exactly one problem (its own cloud); in the cross table each
 // cloud is the key range of exactly one problem (its partner's).  Callers with other tables must keep the key
@@ -115,11 +152,11 @@ k_mha_bwd_dq(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
 __global__ void __launch_bounds__(BT)
 k_mha_bwd_dkv(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp, int ldk, const float* __restrict__ Vp,
               int ldv, const float* __restrict__ dO, int lddo, const float* __restrict__ lse,
-              const float* __restrict__ delta, float* __restrict__ dK, int lddk, float* __restrict__ dV, int lddv,
-              const int32_t* __restrict__ q_start, const int32_t* __restrict__ q_len, const int32_t* __restrict__ k_start,
-              const int32_t* __restrict__ k_len, float qscale, float kscale) {
+              const float* __restrict__ delta, const float* __restrict__ rnorm, float* __restrict__ dK, int lddk,
+              float* __restrict__ dV, int lddv, const int32_t* __restrict__ q_start, const int32_t* __restrict__ q_len,
+              const int32_t* __restrict__ k_start, const int32_t* __restrict__ k_len, float qscale, float kscale) {
     __shared__ __align__(16) float sQ[CH][HD], sG[CH][HD];
-    __shared__ float sL[CH], sD[CH];
+    __shared__ float sL[CH], sD[CH], sR[CH];
     const int prob = blockIdx.z, head = blockIdx.y, tile = blockIdx.x, nh = gridDim.y;
     const int kl = k_len[prob];
     if (tile * BT >= kl) return;
@@ -149,10 +186,11 @@ k_mha_bwd_dkv(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp
             const size_t qr = (size_t)(q0 + qb + threadIdx.x);
             sL[threadIdx.x] = lse[qr * nh + head];
             sD[threadIdx.x] = delta[qr * nh + head];
+            sR[threadIdx.x] = rnorm[qr * nh + head];
         }
         __syncthreads();
         for (int i = 0; i < nq; ++i) {
-            const float p = fast_exp2(dot_smem(k, &sQ[i][0]) - sL[i]);
+            const float p = fast_exp2(dot_smem(k, &sQ[i][0]) - sL[i]) * sR[i];
             axpy_smem(dv, p, &sG[i][0]);
             const float ds = p * (dot_smem(v, &sG[i][0]) - sD[i]);
             axpy_smem(dk, ds, &sQ[i][0]);
@@ -313,7 +351,7 @@ WgradLayout wgrad_layout(int M, int N, int K) {
 extern "C" {
 
 size_t regtr_mha_varlen_bwd_ws_bytes(int n_rows, int n_heads) {
-    return regtr_align((size_t)(n_rows > 0 ? n_rows : 1) * (size_t)(n_heads > 0 ? n_heads : 1) * sizeof(float));
+    return regtr_align(2 * (size_t)(n_rows > 0 ? n_rows : 1) * (size_t)(n_heads > 0 ? n_heads : 1) * sizeof(float));
 }
 
 int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, const float* O,
@@ -331,16 +369,17 @@ int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const
         return REGTR_ERR_ARG;
     if (!ws || ws_bytes < regtr_mha_varlen_bwd_ws_bytes(n_rows, n_heads)) return REGTR_ERR_WORKSPACE;
     float* delta = (float*)ws;
+    float* rnorm = delta + (size_t)n_rows * n_heads;
     const float qscale = scale * 1.4426950408889634f;
     if (max_q_len > 0) {
         k_mha_bwd_dq<<<dim3(regtr_cdiv(max_q_len, BT), n_heads, n_problems), BT, 0, st>>>(
-            Q, ldq, K, ldk, V, ldv, O, ldo, dO, lddo, lse, delta, dQ, lddq, q_start, q_len, k_start, k_len, qscale, scale);
+            Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dQ, lddq, q_start, q_len, k_start, k_len, qscale, scale);
         REGTR_CHECK_LAUNCH();
     }
     if (max_k_len > 0) {
         k_mha_bwd_dkv<<<dim3(regtr_cdiv(max_k_len, BT), n_heads, n_problems), BT, 0, st>>>(
-            Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, dK, lddk, dV, lddv, q_start, q_len, k_start, k_len, qscale,
-            LN2);
+            Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dK, lddk, dV, lddv, q_start, q_len, k_start, k_len,
+            qscale, LN2);
         REGTR_CHECK_LAUNCH();
     }
     return REGTR_OK;

@@ -1,0 +1,160 @@
+"""Float64 reference of the attention core (softmax(q k^T / sqrt(32)) v per head over (query range, key range)
+problems) and the checks of its backward that tests/test_gpu_attention_backward.py and tests/test_gpu_grad_stages.py
+share.
+
+A problem is (q_start, q_len, k_start, k_len): rows of the packed [n, E] q / dO / O matrices and of the packed k / v
+matrices, E = n_heads * 32.  Every key row lies in the key range of at most one problem.
+
+Besides the yardstick rows (tests/grad_yardstick.py), three invariants of exact arithmetic are checked per problem
+and head, each against the fp32 reference's deviation from it:
+  * sum_j dK_j = 0: softmax does not change when one vector is added to every key;
+  * sum_j dV_j = sum_i dO_i: every row of P sums to 1;
+  * dQ with every key shifted by one vector c equals the float64 dQ: the same invariance, seen from the query side.
+A kernel whose sum_j dS_ij is off by e gets dQ off by e * (the part the keys share) and dK off by e * (the part the
+queries share), so these catch errors that zero-mean inputs hide.
+"""
+import math
+
+import torch
+
+from grad_yardstick import FACTOR, FLOOR
+
+HD = 32
+SCALE = 1.0 / math.sqrt(HD)
+
+
+def problems_of(q_start, q_len, k_start, k_len):
+    """Problem tuples from the (device) tables."""
+    return list(zip(*(t.tolist() for t in (q_start, q_len, k_start, k_len))))
+
+
+def _heads(x, start, length, n_heads):
+    return x[start:start + length].view(length, n_heads, HD).transpose(0, 1)
+
+
+def reference(q, k, v, d_o, problems, n_heads, dtype=torch.float64):
+    """Autograd of the core in `dtype` on the CPU.  -> dict of [n, E] CPU tensors o, dq, dk, dv (0 on rows outside
+    every problem), lse [n, n_heads] (base 2, -inf for a query without keys) and, in float64, ddq / ddk: how much
+    dQ and dK fall when delta_i = sum_j P_ij dP_ij is raised by the fraction 1 (dS_ij = P_ij (dP_ij - delta_i), so
+    dQ_i falls by scale * delta_i * sum_j P_ij k_j and dK_j by scale * sum_i P_ij delta_i q_i)."""
+    n, E = q.shape
+    x = [t.detach().cpu().to(dtype).requires_grad_(True) for t in (q, k, v)]
+    g = d_o.detach().cpu().to(dtype)
+    o = torch.zeros(n, E, dtype=dtype)
+    lse = torch.full((n, n_heads), -math.inf, dtype=dtype)
+    ddq, ddk = torch.zeros(n, E, dtype=torch.float64), torch.zeros(n, E, dtype=torch.float64)
+    outs, gouts = [], []
+    for qs, ql, ks, kl in problems:
+        if ql == 0 or kl == 0:
+            continue
+        Q, K, V = _heads(x[0], qs, ql, n_heads), _heads(x[1], ks, kl, n_heads), _heads(x[2], ks, kl, n_heads)
+        s = Q @ K.transpose(1, 2) * SCALE
+        p = torch.softmax(s, -1)
+        out = p @ V
+        go = _heads(g, qs, ql, n_heads)
+        outs.append(out)
+        gouts.append(go)
+        o[qs:qs + ql] = out.detach().transpose(0, 1).reshape(ql, E)
+        lse[qs:qs + ql] = (torch.logsumexp(s.detach(), -1) / math.log(2)).transpose(0, 1)
+        if dtype == torch.float64:
+            with torch.no_grad():
+                P, Qd, Kd = p.detach(), Q.detach(), K.detach()
+                delta = (go * out.detach()).sum(-1, keepdim=True)
+                ddq[qs:qs + ql] = (SCALE * delta * (P @ Kd)).transpose(0, 1).reshape(ql, E)
+                ddk[ks:ks + kl] += (SCALE * P.transpose(1, 2) @ (delta * Qd)).transpose(0, 1).reshape(kl, E)
+    grads = torch.autograd.grad(outs, x, gouts, allow_unused=True) if outs else (None,) * 3
+    dq, dk, dv = (gr if gr is not None else torch.zeros(n, E, dtype=dtype) for gr in grads)
+    return dict(o=o, lse=lse, dq=dq, dk=dk, dv=dv, ddq=ddq, ddk=ddk)
+
+
+def key_shift(k, problems, n_heads, seed=0):
+    """[1, E] fp32: per head a vector of 4x the rms spread of that head's keys (about their mean), in a seeded random
+    direction.  Added to every key it changes neither the softmax nor dQ."""
+    rows = torch.cat([torch.arange(ks, ks + kl) for _, _, ks, kl in problems if kl > 0])
+    kh = k.detach().cpu().double()[rows].view(-1, n_heads, HD)
+    spread = (kh - kh.mean(0)).pow(2).sum(-1).mean(0).sqrt()                      # [n_heads]
+    u = torch.randn(n_heads, HD, generator=torch.Generator().manual_seed(seed), dtype=torch.float64)
+    return (4 * spread[:, None] * u / u.norm(dim=1, keepdim=True)).reshape(1, -1).float()
+
+
+def run_kernel(q, k, v, d_o, problems, n_heads, o=None, lse=None):
+    """The CUDA backward (after the training forward, unless O and lse are given) on CUDA or CPU fp32 q, k, v, dO
+    packed as one [n, 3E] matrix, as the model packs them -> dict of CPU dq, dk, dv."""
+    from regtr_b200 import ops
+    dev = 'cuda:0'
+    E = q.shape[1]
+    tb = [torch.tensor(c, dtype=torch.int32, device=dev) for c in zip(*problems)]
+    mq, mk = max(p[1] for p in problems), max(p[3] for p in problems)
+    qkv = torch.cat([t.to(dev) for t in (q, k, v)], 1)
+    qd, kd, vd = qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:]
+    if o is None:
+        o, lse = ops.mha_varlen_lse(qd, kd, vd, *tb, mq, n_heads)
+    d = torch.zeros_like(qkv)
+    ops.mha_varlen_bwd(qd, kd, vd, o.to(dev), lse.to(dev), d_o.to(dev).contiguous(), d[:, :E], d[:, E:2 * E],
+                       d[:, 2 * E:], *tb, mq, mk, n_heads)
+    torch.cuda.synchronize()
+    d = d.cpu()
+    return dict(dq=d[:, :E], dk=d[:, E:2 * E], dv=d[:, 2 * E:])
+
+
+def rows_of(problems, which):
+    """Concatenated query ('q') or key ('k') rows of the problems."""
+    i = 0 if which == 'q' else 2
+    parts = [torch.arange(p[i], p[i] + p[i + 1]) for p in problems]
+    return torch.cat(parts) if parts else torch.zeros(0, dtype=torch.long)
+
+
+def add_rows(ys, prefix, problems, got, fp32, ref):
+    """One yardstick row each for dq (query rows), dk and dv (key rows) of the problems."""
+    qr, kr = rows_of(problems, 'q'), rows_of(problems, 'k')
+    for name, rows in (('dq', qr), ('dk', kr), ('dv', kr)):
+        ys.add(f'{prefix}{name}', got[name][rows], fp32[name][rows], ref[name][rows])
+
+
+def invariants(problems, n_heads, d_o, got, fp32, ref, got_shift, fp32_shift, ref_shift):
+    """The three invariants per problem with queries and keys, and head.  got / fp32 / ref: dicts with dk, dv (the
+    kernel's, the fp32 reference's, the float64 reference's); *_shift: the same runs with keys k + c (dq is read).
+    -> [(check, (q_len, k_len), head, kernel deviation, fp32 deviation, bound)]; the kernel passes a row when its
+    deviation <= FACTOR * fp32 deviation + FLOOR * max|float64 gradient over the problem|."""
+    g = d_o.detach().cpu().double()
+    out = []
+
+    def dev_sum(t, s, length, target=None):
+        x = t.detach().double()[s:s + length].view(length, n_heads, HD).sum(0)
+        return (x if target is None else x - target).abs().amax(-1)                  # [n_heads]
+
+    for qs, ql, ks, kl in problems:
+        if ql == 0 or kl == 0:
+            continue
+        sum_do = g[qs:qs + ql].view(ql, n_heads, HD).sum(0)
+        checks = (
+            ('sum dK = 0', [dev_sum(t['dk'], ks, kl) for t in (got, fp32)], ref['dk'][ks:ks + kl]),
+            ('sum dV = sum dO', [dev_sum(t['dv'], ks, kl, sum_do) for t in (got, fp32)], ref['dv'][ks:ks + kl]),
+            ('dQ(k + c)', [(t['dq'].detach().double()[qs:qs + ql] - ref_shift['dq'][qs:qs + ql]).view(ql, n_heads, HD)
+                           .abs().amax(-1).amax(0) for t in (got_shift, fp32_shift)], ref_shift['dq'][qs:qs + ql]),
+        )
+        for name, (dg, df), r in checks:
+            if kl == 1 and name != 'sum dV = sum dO':
+                continue            # one key: dQ = dK = 0 exactly, no scale for an absolute bound (rows check them)
+            bound = FACTOR * df + FLOOR * float(r.abs().max())
+            for h in range(n_heads):
+                out.append((name, (ql, kl), h, float(dg[h]), float(df[h]), float(bound[h])))
+    return out
+
+
+def failed(rows):
+    return [r for r in rows if not r[3] <= r[5]]
+
+
+def report_invariants(title, rows):
+    """Per check: the worst (kernel deviation / bound) over problems and heads, and how many rows fail."""
+    print(f'\n{title}\n  invariants per problem and head; pass: kernel deviation <= {FACTOR:g} x fp32 deviation + '
+          f'{FLOOR:g} x max|float64 gradient over the problem|')
+    wn = max([len(r[0]) for r in rows] + [16])
+    print(f'  {"check":{wn}s} {"worst ratio":>11s}  {"at (q_len, k_len, head)":>24s} {"kernel":>9s} {"fp32":>9s}  failing')
+    for name in dict.fromkeys(r[0] for r in rows):
+        rs = [r for r in rows if r[0] == name]
+        w = max(rs, key=lambda r: r[3] / max(r[5], 1e-300))
+        at = f'({w[1][0]}, {w[1][1]}, {w[2]})'
+        print(f'  {name:{wn}s} {w[3] / max(w[5], 1e-300):11.3g}  {at:>24s} {w[3]:9.2e} {w[4]:9.2e}  '
+              f'{len(failed(rs))}/{len(rs)}')

@@ -32,6 +32,18 @@ class Yardstick:
         self.rows.append((name, eg, ef, ok))
         return ok
 
+    def add_abs(self, name, gpu, fp32, ref, scale):
+        """A row for a tensor that is zero in exact arithmetic: both measures are taken against `scale` (max-abs /
+        scale and rms / scale) instead of the reference's own size."""
+        def err(t):
+            d = t.detach().double().cpu() - ref.detach().double().cpu()
+            return (float(d.abs().max()) / scale, float(d.norm()) / (scale * max(d.numel(), 1) ** 0.5)) \
+                if d.numel() else (0.0, 0.0)
+        eg, ef = err(gpu), err(fp32)
+        ok = all(a <= FACTOR * b + FLOOR for a, b in zip(eg, ef))
+        self.rows.append((name, eg, ef, ok))
+        return ok
+
     def report(self):
         w = max([len(r[0]) for r in self.rows] + [6])
         print(f'\n{self.title}\n  errors against float64: max-abs / max|ref| and relative Frobenius norm; '

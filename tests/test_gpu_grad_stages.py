@@ -11,7 +11,9 @@ counts).  Then:
     decisions, under the fp32 yardstick (tests/grad_yardstick.py), and the decisions that the unforced float64
     forward takes differently are counted;
   * the float64 oracle's d(feats_un) is fed to the GPU encoder alone, and every encoder parameter gradient is compared
-    with the float64 oracle encoder's under the same yardstick.
+    with the float64 oracle encoder's under the same yardstick;
+  * each attention core's recorded q, k, v, O, lse and output gradient are run through the core's backward alone and
+    checked as tests/test_gpu_attention_backward.py checks synthetic inputs (tests/attention_oracle.py).
 """
 import inspect
 import os
@@ -22,6 +24,7 @@ import numpy as np
 import pytest
 import torch
 
+import attention_oracle as ao
 from conftest import FORWARD_CASES, make_case
 from grad_yardstick import Yardstick, errors
 
@@ -34,7 +37,7 @@ DEV = 'cuda:0'
 CASES = ['fwd_3dmatch_small_b2', 'fwd_modelnet_b1']
 ENC = 'kpf_encoder.encoder_blocks.'
 XENC = 'transformer_encoder.layers.'
-_RECORDED_OPS = ('instnorm_act', 'instnorm_apply', 'max_pool', 'kpconv', 'linear_instats', 'linear')
+_RECORDED_OPS = ('instnorm_act', 'instnorm_apply', 'max_pool', 'kpconv', 'linear_instats', 'linear', 'mha_varlen_lse')
 
 
 class _Tap(torch.autograd.Function):
@@ -54,9 +57,11 @@ class _Tap(torch.autograd.Function):
 def _record(model, mp):
     """Wrap every encoder block's forward, every cross-encoder layer's forward_train_packed and the ops they call.
     Per block / layer: 'x' (input), 'rest' (the other arguments), 'calls' [(op, arguments, result)], and after the
-    backward 'dout' (gradient at the output) and 'dx' (gradient the block sends to its input, if it needs one)."""
+    backward 'dout' (gradient at the output) and 'dx' (gradient the block sends to its input, if it needs one).
+    Every attention-core backward is kept in rec['mha_bwd'], keyed by the address of the O it was given: its dO and
+    copies of the dq, dk, dv it wrote."""
     from regtr_b200 import ops
-    rec = dict(enc=[], xenc=[], cur=None)
+    rec = dict(enc=[], xenc=[], cur=None, mha_bwd={})
 
     def recording(name, fn):
         sig = inspect.signature(fn)
@@ -72,6 +77,14 @@ def _record(model, mp):
 
     for name in _RECORDED_OPS:
         mp.setattr(ops, name, recording(name, getattr(ops, name)))
+    mha_bwd = ops.mha_varlen_bwd
+    bwd_sig = inspect.signature(mha_bwd)
+
+    def recording_bwd(*a, **k):
+        mha_bwd(*a, **k)
+        b = bwd_sig.bind(*a, **k).arguments
+        rec['mha_bwd'][b['o'].data_ptr()] = dict(d_o=b['d_o'], **{t: b[t].clone() for t in ('dq', 'dk', 'dv')})
+    mp.setattr(ops, 'mha_varlen_bwd', recording_bwd)
 
     def tap(mod, method, box):
         fn = getattr(mod, method)
@@ -257,6 +270,20 @@ def _oracle_layer(run, i, x, pos, dout, dtype, masks, names):
     return torch.autograd.grad(outs, [xin] + [leaves[n] for n in names], gouts)
 
 
+def _add_in_proj_rows(ys, label, g, a, b):
+    """The q, k and v row blocks of an in-projection gradient, one yardstick row each: the k / v blocks are much
+    larger than the q block, so a whole-tensor row would hide an error in dQ.  The k block of the bias gradient is
+    sum_j dK_j, zero in exact arithmetic (softmax ignores a vector added to every key): it is measured against the
+    larger of the q and v blocks instead of itself."""
+    E = g.shape[0] // 3
+    for part, blk in zip('qkv', (slice(0, E), slice(E, 2 * E), slice(2 * E, 3 * E))):
+        if part == 'k' and label.endswith('bias'):
+            scale = max(float(b[:E].abs().max()), float(b[2 * E:].abs().max()))
+            ys.add_abs(f'{label}[k]', g[blk], a[blk], b[blk], scale)
+        else:
+            ys.add(f'{label}[{part}]', g[blk], a[blk], b[blk])
+
+
 @pytest.mark.parametrize('case', CASES)
 def test_cross_encoder_layers_backward_layer_local(case):
     run = _full_run(case)
@@ -278,7 +305,10 @@ def test_cross_encoder_layers_backward_layer_local(case):
         g64 = _oracle_layer(run, i, r['x'], pos, r['dout'], torch.float64, mask, names)
         g32 = _oracle_layer(run, i, r['x'], pos, r['dout'], torch.float32, mask, names)
         for lab, g, a, b in zip(labels, full, g32, g64):
-            ys.add(f'{i}.{lab}', g, a, b)
+            if lab.endswith('.in_proj_weight') or lab.endswith('.in_proj_bias'):
+                _add_in_proj_rows(ys, f'{i}.{lab}', g, a, b)
+            else:
+                ys.add(f'{i}.{lab}', g, a, b)
         with torch.no_grad():
             free = _oracle_layer(run, i, r['x'], pos, r['dout'], torch.float64, None, names)
         flips.append(f'  layer {i}: ReLU {int((free != mask).sum())}/{mask.numel()}')
@@ -286,6 +316,40 @@ def test_cross_encoder_layers_backward_layer_local(case):
     print('  decisions of the unforced float64 forward that differ from the GPU\'s:\n' + '\n'.join(flips))
     assert not not_identical, f'layer-local rerun not bit-identical to the full backward: {not_identical}'
     assert not ys.failures(), ys.failures()
+
+
+@pytest.mark.parametrize('case', CASES)
+def test_cross_encoder_attention_cores_on_recorded_tensors(case):
+    """Every cross-encoder layer's self- and cross-attention core, on the q, k, v, O, lse and output gradient the
+    training step gave it: the step's dq / dk / dv equal a rerun of the backward bit for bit and meet the yardstick as
+    separate rows against float64 autograd of the core, and the invariants of tests/attention_oracle.py hold per
+    problem and head (the dQ(k + c) check reruns the forward and backward with shifted keys)."""
+    run = _full_run(case)
+    H = run['model'].transformer_encoder.layers[0].nhead
+    ys = Yardstick(f'{case}: cross-encoder attention cores on the recorded tensors')
+    inv, not_identical = [], []
+    for i, r in enumerate(run['rec']['xenc']):
+        cores = [(a, res) for name, a, res in r['calls'] if name == 'mha_varlen_lse']
+        assert len(cores) == 2, (i, len(cores))
+        for which, (a, (o, lse)) in zip(('self', 'cross'), cores):
+            b = run['rec']['mha_bwd'][o.data_ptr()]
+            q, k, v, d_o = a['q'], a['k'], a['v'], b['d_o']
+            problems = ao.problems_of(a['q_start'], a['q_len'], a['k_start'], a['k_len'])
+            rerun = ao.run_kernel(q, k, v, d_o, problems, H, o, lse)
+            not_identical += [f'{i}.{which}.{t}' for t in rerun if not torch.equal(rerun[t], b[t].cpu())]
+            got = {t: b[t].cpu() for t in ('dq', 'dk', 'dv')}
+            ks = k.cpu() + ao.key_shift(k, problems, H)
+            r64, r32 = (ao.reference(q, k, v, d_o, problems, H, dt) for dt in (torch.float64, torch.float32))
+            s64, s32 = (ao.reference(q, ks, v, d_o, problems, H, dt) for dt in (torch.float64, torch.float32))
+            ao.add_rows(ys, f'{i}.{which} ', problems, got, r32, r64)
+            got_shift = ao.run_kernel(q, ks, v, d_o, problems, H)
+            inv += [(f'{i}.{which} {c}',) + tuple(rest) for c, *rest in
+                    ao.invariants(problems, H, d_o, got, r32, r64, got_shift, s32, s64)]
+    ys.report()
+    ao.report_invariants(f'{case}: cross-encoder attention cores on the recorded tensors', inv)
+    assert not not_identical, f'attention backward rerun not bit-identical to the training step: {not_identical}'
+    assert not ys.failures(), ys.failures()
+    assert not ao.failed(inv), ao.failed(inv)[:8]
 
 
 # ------------------------------------------------------------------------------------------------ stage chain
