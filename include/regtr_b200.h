@@ -461,6 +461,17 @@ int regtr_overlap_nn(const double* xyz, const int32_t* offs, int B, int n_cap, c
                      float cell, int32_t* nn, uint32_t* status, void* ws, size_t ws_bytes, void* state,
                      size_t state_bytes, void* stream);
 
+/* Fitness and inlier RMSE of B registered pairs (the definitions of Open3D's evaluate_registration, which the
+ * reference's demo.py leaves to a viewer), from the matches of regtr_overlap_nn: xyz, offs, pose and radius as given
+ * to it, nn its output.  out (B,4) float64 per pair = (fitness_src, rmse_src, fitness_tgt, rmse_tgt):
+ *   fitness = |{i : nn_i >= 0}| / n (0 for an empty cloud), rmse = sqrt(sum d_i^2 / n_inliers) (0 without inliers),
+ * d_i^2 the float64 squared distance of regtr_overlap_nn (the source moved by ((r0 x + r1 y) + r2 z) + t, no
+ * contraction), so every summed distance is one that passed "strictly below radius".  Sums in a fixed order, one CTA
+ * per (pair, direction): the result is bit-reproducible.  A match index outside the partner cloud, or a distance not
+ * below radius, is not counted and raises REGTR_STATUS_INPUT.  n_cap >= offs[2B].  One launch. */
+int regtr_registration_fit(const double* xyz, const int32_t* offs, int B, int n_cap, const double* pose,
+                           double radius, const int32_t* nn, double* out, uint32_t* status, void* stream);
+
 /* Per-pair flags of regtr_train_augment */
 #define REGTR_PREP_PERTURB_SRC 1  /* the perturbation moves the source (else the target) */
 #define REGTR_PREP_CENTRE 2       /* rotate about the perturbed cloud's centroid ('small' mode) */
@@ -490,7 +501,8 @@ int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src
 
 /* ---- training data (ModelNet40) --------------------------------------------------- */
 
-#define REGTR_STATUS_INPUT 16u    /* ModelNet pairs: a shape index out of range or a coordinate that is not finite */
+#define REGTR_STATUS_INPUT 16u    /* ModelNet pairs: a shape index out of range or a coordinate that is not finite;
+                                     registration fit: a match that regtr_overlap_nn cannot have produced */
 #define REGTR_STATUS_CROP 32u     /* ModelNet pairs: a crop kept fewer than n_out points */
 #define REGTR_MODELNET_MAX_PTS 2048
 #define REGTR_MODELNET_PARAMS 18  /* doubles per pair in params: dir_src[3], dir_tgt[3], transform[12] */

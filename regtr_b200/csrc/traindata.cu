@@ -110,6 +110,57 @@ k_overlap_nn(const double* __restrict__ xa, const float* __restrict__ x32, const
     }
 }
 
+// ------------------------------------------------------------------------------------------------- registration fit
+// One CTA per (pair, direction): cloud c < B is source b = c (queries moved by pose b, partners the raw target),
+// c >= B is target b = c - B (partners the moved source).  Per inlier the squared distance is k_overlap_nn's
+// ((dx dx + dy dy) + dz dz) on k_align's moved source (rt_row), so it is the value that passed "< r2".  Each thread
+// sums its strided points in ascending order, then a fixed shared-memory tree: deterministic, no atomics on values.
+// A match outside the partner cloud or not strictly within the radius is not counted and raises
+// REGTR_STATUS_INPUT (nn then did not come from regtr_overlap_nn on these inputs).
+constexpr int FIT_THREADS = 256;
+
+__global__ void __launch_bounds__(FIT_THREADS)
+k_registration_fit(const double* __restrict__ xyz, const int32_t* __restrict__ offs, int B,
+                   const double* __restrict__ pose, double r2, const int32_t* __restrict__ nn,
+                   double* __restrict__ out, uint32_t* status) {
+    __shared__ double s_sum[FIT_THREADS];
+    __shared__ int s_cnt[FIT_THREADS];
+    const int c = blockIdx.x, t = threadIdx.x;
+    const int b = c < B ? c : c - B, pc = c < B ? c + B : c - B;
+    const double* m = pose + 12 * b;
+    const int a0 = offs[c], a1 = offs[c + 1], p0 = offs[pc], np_ = offs[pc + 1] - p0;
+    double sum = 0.0;
+    int cnt = 0;
+    bool bad = false;
+    for (int i = a0 + t; i < a1; i += FIT_THREADS) {
+        const int j = nn[i];
+        if (j < 0) continue;
+        if (j >= np_) { bad = true; continue; }
+        const double* s = xyz + 3 * (size_t)(c < B ? i : p0 + j);     // the source end of the match
+        const double* q = xyz + 3 * (size_t)(c < B ? p0 + j : i);     // the target end
+        const double sx = s[0], sy = s[1], sz = s[2];
+        const double dx = __dsub_rn(rt_row(m, sx, sy, sz), q[0]), dy = __dsub_rn(rt_row(m + 4, sx, sy, sz), q[1]),
+                     dz = __dsub_rn(rt_row(m + 8, sx, sy, sz), q[2]);
+        const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+        if (!(d2 < r2)) { bad = true; continue; }
+        sum = __dadd_rn(sum, d2);
+        ++cnt;
+    }
+    if (bad) atomicOr(status, REGTR_STATUS_INPUT);
+    s_sum[t] = sum;
+    s_cnt[t] = cnt;
+    __syncthreads();
+    for (int h = FIT_THREADS / 2; h > 0; h >>= 1) {
+        if (t < h) { s_sum[t] = __dadd_rn(s_sum[t], s_sum[t + h]); s_cnt[t] += s_cnt[t + h]; }
+        __syncthreads();
+    }
+    if (t != 0) return;
+    const int n = a1 - a0, k = s_cnt[0];
+    double* o = out + 4 * b + (c < B ? 0 : 2);
+    o[0] = n > 0 ? __ddiv_rn((double)k, (double)n) : 0.0;
+    o[1] = k > 0 ? __dsqrt_rn(__ddiv_rn(s_sum[0], (double)k)) : 0.0;
+}
+
 // ------------------------------------------------------------------------------------------------- augmentation
 // One CTA per pair.  pert[b] = (R | t) of the host-drawn perturbation; flags: REGTR_PREP_*.  With CENTRE ('small'),
 // the rotation turns about the centroid c of the perturbed cloud (float64 mean in a fixed order): t' = (t + c) - R c.
@@ -340,6 +391,17 @@ int regtr_overlap_nn(const double* xyz, const int32_t* offs, int B, int n_cap, c
     k_overlap_nn<<<blocks < 8 * REGTR_NUM_SMS ? blocks : 8 * REGTR_NUM_SMS, NN_WARPS * 32, 0, st>>>(
         w.xa, w.x32, offs, B, n_cap, w.order, grid_table(w.grid, (size_t)n_cap), cell_table_log2(n_cap),
         grid_sxyzi(w.grid), cell, radius * radius, nn);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_registration_fit(const double* xyz, const int32_t* offs, int B, int n_cap, const double* pose,
+                           double radius, const int32_t* nn, double* out, uint32_t* status, void* stream_) {
+    if (!offs || !pose || !out || !status || B <= 0 || 2 * B > 32767 || n_cap < 0 || !(radius > 0.0))
+        return REGTR_ERR_ARG;
+    if (n_cap > 0 && (!xyz || !nn)) return REGTR_ERR_ARG;
+    k_registration_fit<<<2 * B, FIT_THREADS, 0, (cudaStream_t)stream_>>>(xyz, offs, B, pose, radius * radius, nn,
+                                                                        out, status);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
 }

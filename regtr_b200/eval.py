@@ -6,6 +6,7 @@ Host-side mirror of
     (/root/reference/src/models/generic_reg_model.py:175-229, 260-281),
   * the 3DMatch / 3DLoMatch registration-recall benchmark of Predator
     (/root/reference/src/benchmark/benchmark_predator.py:17-375),
+  * the 3DMatch success rate of Deep Global Registration (benchmark/benchmark_3dmatch.py:benchmark_dgr),
   * the ModelNet metrics of RPMNet (/root/reference/src/benchmark/benchmark_modelnet.py:33-97).
 Same file formats (Redwood `gt.log` / `gt.info` / `est.log`), same definitions, same summary strings,
 so a run of this package can be scored with either implementation.  Pure numpy / torch: none of this is
@@ -257,6 +258,59 @@ def benchmark_3dmatch(est_folder, gt_folder, save_flags=False):
     out += "Mean median RRE: {:.3f}: +- {:.3f}\n".format(np.mean(re_med), np.std(re_med))
     out += "Mean median RTE: {:.3F}: +- {:.3f}\n".format(np.mean(te_med), np.std(te_med))
     return out, float(np.mean(recall)), per_scene
+
+
+# ------------------------------------------------------ 3DMatch success rate of Deep Global Registration
+
+
+def compute_rre(R_est, R):
+    """Degrees; the cosine is clipped to [-1 + 1e-16, 1 - 1e-16] (benchmark_3dmatch.py:compute_rre)."""
+    eps = 1e-16
+    return np.arccos(np.clip((np.trace(R_est.T @ R) - 1) / 2, -1 + eps, 1 - eps)) * 180. / np.pi
+
+
+def compute_rte(t, t_est):
+    return np.linalg.norm(t - t_est)
+
+
+def benchmark_dgr(est_folder, gt_folder, re_thres=15, te_thres=0.3):
+    """DGR success rate (RRE < re_thres degrees and RTE < te_thres) over the scenes of `gt_folder`
+    (benchmark/benchmark_3dmatch.py:benchmark_dgr), with the reference's rules: the i-th est.log entry is scored
+    against the i-th gt.log entry whatever their keys, and the errors are those of the inverted poses.
+    -> (summary string identical to the reference's, {scene: dict(rre, rte, success) arrays per est.log entry})."""
+    import warnings
+    scenes = sorted(os.listdir(gt_folder))
+    out = "Scene\t¦ success.\t¦ rre\t¦ rte\t¦ rre_all\t¦ rte_all\t¦\n"
+    success, rre_ok, rte_ok, rre_all, rte_all = [], [], [], [], []
+    per_scene = {}
+
+    def row(name, s, ro, to, ra, ta):
+        with warnings.catch_warnings():            # np.mean([]) of a scene without a success is nan, as in the reference
+            warnings.simplefilter('ignore', RuntimeWarning)
+            return "{}\t¦ {:.3f}\t¦ {:.3f}\t¦ {:.3f}\t¦ {:.3f}\t¦ {:.3f}¦\n".format(
+                name, np.mean(s), np.mean(ro), np.mean(to), np.mean(ra), np.mean(ta))
+
+    for idx, scene in enumerate(scenes):
+        _, gt_traj = read_trajectory(os.path.join(gt_folder, scene, 'gt.log'))
+        _, est_traj = read_trajectory(os.path.join(est_folder, scene, 'est.log'))
+        s_flag, s_ro, s_to, s_ra, s_ta = [], [], [], [], []
+        for i in range(len(est_traj)):
+            est_inv, gt_inv = np.linalg.inv(est_traj[i]), np.linalg.inv(gt_traj[i])
+            rot_error = compute_rre(est_inv[:3, :3], gt_inv[:3, :3])
+            trans_error = compute_rte(est_inv[:3, 3], gt_inv[:3, 3])
+            s_ra.append(rot_error)
+            s_ta.append(trans_error)
+            ok = bool(rot_error < re_thres and trans_error < te_thres)
+            s_flag.append(ok)
+            if ok:
+                s_ro.append(rot_error)
+                s_to.append(trans_error)
+        out += row(SHORT_NAMES[idx] if idx < len(SHORT_NAMES) else scene, s_flag, s_ro, s_to, s_ra, s_ta)
+        per_scene[scene] = dict(rre=np.array(s_ra, dtype=np.float64), rte=np.array(s_ta, dtype=np.float64),
+                                success=np.array(s_flag, dtype=bool))
+        success += s_flag; rre_ok += s_ro; rte_ok += s_to; rre_all += s_ra; rte_all += s_ta
+    out += row('Avg', success, rre_ok, rte_ok, rre_all, rte_all)
+    return out, per_scene
 
 
 # ------------------------------------------------------------------------------ ModelNet metrics

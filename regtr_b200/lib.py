@@ -92,6 +92,7 @@ SIGNATURES = {
     'regtr_overlap_ws_bytes': (_Z, [_I]),
     'regtr_overlap_state_bytes': (_Z, [_I]),
     'regtr_overlap_nn': (_I, [_P, _P, _I, _I, _P, _c.c_double, _F, _P, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_registration_fit': (_I, [_P, _P, _I, _I, _P, _c.c_double, _P, _P, _P, _P]),
     'regtr_train_augment_ws_bytes': (_Z, [_I, _I]),
     'regtr_train_augment_state_bytes': (_Z, [_I]),
     'regtr_train_augment': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _c.c_ulonglong, _c.c_ulonglong, _c.c_double, _I,

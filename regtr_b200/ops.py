@@ -1042,6 +1042,57 @@ def overlap_nn(xyz, offs, B: int, pose, radius: float, status):
     return nn[:n]
 
 
+
+def registration_fit(src_list, tgt_list, pose, radius: float, status=None):
+    """Fitness and inlier RMSE of B registered pairs (regtr_registration_fit on the matches of `overlap_nn`):
+    src_list / tgt_list, B clouds (n,3) each (numpy or torch, any float dtype; stacked in float64 on the device),
+    pose (B,3,4) source -> target.  -> (B,4) float64 device tensor (fitness_src, rmse_src, fitness_tgt, rmse_tgt).
+    status: a device word (`new_status`) that the caller checks with `check_fit_status` where it syncs; this call does
+    not read it.  status=None: a word of this call, read and checked before returning.  A coordinate of the moved source or the
+    target beyond `overlap_coord_bound(radius)` raises RegtrLibError there."""
+    L = _lib.load()
+    B = len(src_list)
+    if B == 0 or len(tgt_list) != B:
+        raise ValueError('registration_fit: expected as many source as target clouds, at least one pair')
+    dev = pose.device if torch.is_tensor(pose) and pose.is_cuda else torch.device('cuda', torch.cuda.current_device())
+    clouds = [torch.as_tensor(c) for c in list(src_list) + list(tgt_list)]
+    for c in clouds:
+        if c.dim() != 2 or c.shape[1] != 3:
+            raise ValueError(f'registration_fit: expected (n,3) clouds, got {tuple(c.shape)}')
+    lens = [int(c.shape[0]) for c in clouds]
+    n = sum(lens)
+    xyz = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    a = 0
+    for c, ln in zip(clouds, lens):
+        xyz[a:a + ln].copy_(c.to(dev, torch.float64))
+        a += ln
+    pose64 = torch.as_tensor(pose).to(dev, torch.float64).reshape(B, 3, 4).contiguous()
+    offs = make_offsets(lens, dev)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    nn = overlap_nn(xyz, offs, B, pose64, radius, status)
+    out = torch.empty((B, 4), dtype=torch.float64, device=dev)
+    _lib.check(L.regtr_registration_fit(_p(xyz), _p(offs), B, n, _p(pose64), float(radius), _p(nn), _p(out),
+                                        _p(status), _stream()), 'regtr_registration_fit')
+    _count(1)
+    if own:
+        check_fit_status(status, radius)
+    return out
+
+
+def check_fit_status(status, radius: float):
+    """Read the status word of `registration_fit` (a host sync) and raise RegtrLibError if the fit is not exact."""
+    word = int(status.item())
+    if word & (STATUS_RANGE | 1):             # REGTR_STATUS_RANGE | REGTR_STATUS_KEY_RANGE
+        raise _lib.RegtrLibError(
+            f'registration_fit: a coordinate of the moved source or of the target lies beyond +-'
+            f'{overlap_coord_bound(radius):.3f} (overlap_coord_bound({radius})), the range in which the nearest-'
+            f'neighbour search at this radius is exact, or is not finite (status {word:#x})')
+    if word & STATUS_INPUT:                   # REGTR_STATUS_INPUT (defined below)
+        raise _lib.RegtrLibError(f'registration_fit: a match the overlap search cannot have produced (status {word:#x})')
+
+
 def train_augment(xyz, offs, B: int, n_src: int, pose, nn, pert, flags, seed: int, step: int, noise: float,
                   max_pts: int, out_offs, out_total: int):
     """The augmentations of regtr_train_augment on the clouds / overlap of `overlap_nn`.
