@@ -42,9 +42,10 @@ constexpr QkvOut NO_QKV = {nullptr, 0, nullptr, 0, 0, nullptr, 0, nullptr, 0, 0,
 
 // Optional InstanceNorm statistics of the OUTPUT (per cloud, per column: mean and 1/sqrt(var + eps) over the
 // cloud's rows, kpconv_blocks.py:497-519) WITHOUT a separate pass over C: every epilogue warp reduces its 32 rows
-// per column in a fixed shuffle tree (sum and sum of squares, fp32) and stores the pair to part[row / 32][column];
-// k_in_finalize_part then adds the partials of the 32-row groups that lie inside a cloud in a fixed order (fp64) and
-// reads the few rows of the groups that straddle a cloud boundary straight from C.  No atomics anywhere: the
+// per column in a fixed shuffle tree (sum and sum of squares of v - p, p = the group's first row; fp32) and stores the
+// pair to part[row / 32][column]; k_in_finalize_part then re-centres the partials of the 32-row groups that lie inside
+// a cloud on the cloud's first row and adds them in a fixed order (fp64), reading p and the few rows of the groups that
+// straddle a cloud boundary straight from C.  No atomics anywhere: the
 // statistics are bit-identical from run to run.  (Two earlier versions accumulated with 64-bit integer atomics
 // into per-(cloud, column) fixed-point accumulators: exact and order-independent, but ~10^4 warps adding to the
 // same few hundred addresses made the level-0 GEMMs 2x slower than the separate statistics kernel they replaced.)
@@ -78,15 +79,20 @@ k_in_finalize_part(const float2* __restrict__ part, const float* __restrict__ C,
     int g_lo = (a + 31) >> 5, g_hi = b >> 5;                    // 32-row groups [g_lo, g_hi) lie inside the cloud
     const bool full = !direct_all && g_lo < g_hi;
     const int head_end = full ? 32 * g_lo : b, tail_start = full ? 32 * g_hi : b;
-    double s = 0.0, q = 0.0;
-    if (col < N) {
+    // s = sum (v - k0), q = sum (v - k0)^2 in fp64 about the cloud's first row k0.  A group's partial (D, Q) is taken
+    // about its own first row p: sum (v - k0) = D + 32 (p - k0), sum (v - k0)^2 = Q + 2 (p - k0) D + 32 (p - k0)^2.
+    double s = 0.0, q = 0.0, k0 = 0.0;
+    if (col < N && b > a) {
+        k0 = (double)C[(size_t)a * ldc + col];
         if (full)
             for (int g = g_lo + w; g < g_hi; g += 8) {
                 const float2 p = part[(size_t)g * N + col];
-                s += (double)p.x; q += (double)p.y;
+                const double d = (double)C[(size_t)g * 32 * ldc + col] - k0;
+                s += (double)p.x + 32.0 * d;
+                q += (double)p.y + d * (2.0 * (double)p.x + 32.0 * d);
             }
-        for (int r = a + w; r < head_end; r += 8) { const double v = (double)C[(size_t)r * ldc + col]; s += v; q += v * v; }
-        for (int r = tail_start + w; r < b; r += 8) { const double v = (double)C[(size_t)r * ldc + col]; s += v; q += v * v; }
+        for (int r = a + w; r < head_end; r += 8) { const double v = (double)C[(size_t)r * ldc + col] - k0; s += v; q += v * v; }
+        for (int r = tail_start + w; r < b; r += 8) { const double v = (double)C[(size_t)r * ldc + col] - k0; s += v; q += v * v; }
     }
     red[w][threadIdx.x][0] = s; red[w][threadIdx.x][1] = q;
     __syncthreads();
@@ -94,10 +100,10 @@ k_in_finalize_part(const float2* __restrict__ part, const float* __restrict__ C,
         for (int t = 1; t < 8; ++t) { s += red[t][threadIdx.x][0]; q += red[t][threadIdx.x][1]; }
         const int n = b - a;
         const double dn = n > 0 ? (double)n : 1.0;
-        const double mean = s / dn;
-        double var = q / dn - mean * mean;           // biased variance (InstanceNorm)
+        const double shift = s / dn;
+        double var = q / dn - shift * shift;         // biased variance (InstanceNorm); |shift| ~ std: no cancellation
         var = var > 0.0 ? var : 0.0;
-        stats[(size_t)c * N + col] = make_float2((float)mean, (float)(1.0 / sqrt(var + (double)eps)));
+        stats[(size_t)c * N + col] = make_float2((float)(k0 + shift), (float)(1.0 / sqrt(var + (double)eps)));
     }
 }
 
@@ -382,11 +388,17 @@ k_gemm_tf32x3_wg(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 }
             }
             if (part) {                                        // host guarantees N % 32 == 0 in this mode
-                // per-column sum / sum of squares over this warp's 32 rows (fixed shuffle tree), one float2 per
-                // (32-row group, column); groups that straddle a cloud boundary or M are ignored by the finaliser
+                // per-column sums of d = v - p and d^2 over this warp's 32 rows (fixed shuffle tree), p = the
+                // group's first row (lane 0), which the finaliser reads back from C; one float2 per (32-row group,
+                // column); groups that straddle a cloud boundary or M are ignored by the finaliser.  Centred sums
+                // keep the variance accurate when |mean| >> std: fp32 sums of v and v^2 would lose
+                // (mean / std)^2 ulps to the cancellation in E[v^2] - mean^2.
                 float sq[32];
 #pragma unroll
-                for (int j = 0; j < 32; ++j) sq[j] = v[j] * v[j];
+                for (int j = 0; j < 32; ++j) {
+                    v[j] -= __shfl_sync(0xffffffffu, v[j], 0);
+                    sq[j] = v[j] * v[j];
+                }
                 const float s1 = warp_transpose_sum(v, lane);
                 const float s2 = warp_transpose_sum(sq, lane);
                 part[(size_t)((m0 >> 5) + q) * N + col0 + lane] = make_float2(s1, s2);

@@ -21,6 +21,47 @@ from grad_yardstick import FACTOR, FLOOR
 
 HD = 32
 SCALE = 1.0 / math.sqrt(HD)
+SELF_LENS = [1, 17, 64, 65, 731, 1500]
+CROSS_LENS = [40, 130, 77, 0]
+FAMILIES = ['zero_mean', 'bias', 'flat', 'peaked', 'shared_do']
+PEAK = 60.0                      # largest |base-2 score| of the peaked family
+
+
+def layout(self_lens=SELF_LENS, cross_lens=CROSS_LENS):
+    """(self problems, cross problems, rows): every key row in exactly one problem's key range.  The cross problems
+    pair clouds 0 <-> 1 and 2 <-> 3 of `cross_lens`."""
+    self_p, r = [], 0
+    for n in self_lens:
+        self_p.append((r, n, r, n))
+        r += n
+    c = []
+    for n in cross_lens:
+        c.append(r)
+        r += n
+    L = cross_lens
+    cross_p = [(c[0], L[0], c[1], L[1]), (c[1], L[1], c[0], L[0]), (c[2], L[2], c[3], L[3]), (c[3], L[3], c[2], L[2])]
+    return self_p, cross_p, r
+
+
+def family(name, n, problems, n_heads, seed=0):
+    """q, k, v, dO [n, n_heads * HD] fp32 (CPU) of an input family (tests/test_gpu_attention_backward.py describes
+    them)."""
+    E = n_heads * HD
+    g = torch.Generator().manual_seed(seed)
+    r = lambda s=1.0: torch.randn(n, E, generator=g) * s
+    head = lambda s: torch.randn(1, E, generator=g) * s             # one vector per head, shared by every row
+    q, k, v, d_o = r(1.5), r(1.5), r(1.5), r()
+    if name == 'bias':
+        q, k = r(0.5) + head(1.5), r(0.5) + head(1.5)
+    elif name == 'flat':
+        q, v = r(0.02), r(0.3) + head(1.0)
+    elif name == 'peaked':
+        smax = max(float((_heads(q, qs, ql, n_heads) @ _heads(k, ks, kl, n_heads).transpose(1, 2)).abs().max())
+                   for qs, ql, ks, kl in problems if ql and kl) * SCALE * 1.4426950408889634
+        q = q * (PEAK / smax)
+    elif name == 'shared_do':
+        d_o = r() + head(10.0)
+    return q, k, v, d_o
 
 
 def problems_of(q_start, q_len, k_start, k_len):

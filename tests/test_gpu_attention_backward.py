@@ -22,45 +22,8 @@ from grad_yardstick import Yardstick
 
 pytestmark = pytest.mark.gpu
 
-E, H = 256, 8
-SELF_LENS = [1, 17, 64, 65, 731, 1500]
-CROSS_LENS = [40, 130, 77, 0]
-FAMILIES = ['zero_mean', 'bias', 'flat', 'peaked', 'shared_do']
-PEAK = 60.0                      # largest |base-2 score| of the peaked family
-
-
-def _layout():
-    """(self problems, cross problems, rows): every key row in exactly one problem's key range."""
-    self_p, r = [], 0
-    for n in SELF_LENS:
-        self_p.append((r, n, r, n))
-        r += n
-    c = []
-    for n in CROSS_LENS:
-        c.append(r)
-        r += n
-    L = CROSS_LENS
-    cross_p = [(c[0], L[0], c[1], L[1]), (c[1], L[1], c[0], L[0]), (c[2], L[2], c[3], L[3]), (c[3], L[3], c[2], L[2])]
-    return self_p, cross_p, r
-
-
-def _family(name, n, problems, seed=0):
-    """q, k, v, dO [n, E] fp32 (CPU) of an input family."""
-    g = torch.Generator().manual_seed(seed)
-    r = lambda s=1.0: torch.randn(n, E, generator=g) * s
-    head = lambda s: torch.randn(1, E, generator=g) * s             # one vector per head, shared by every row
-    q, k, v, d_o = r(1.5), r(1.5), r(1.5), r()
-    if name == 'bias':
-        q, k = r(0.5) + head(1.5), r(0.5) + head(1.5)
-    elif name == 'flat':
-        q, v = r(0.02), r(0.3) + head(1.0)
-    elif name == 'peaked':
-        smax = max(float((ao._heads(q, qs, ql, H) @ ao._heads(k, ks, kl, H).transpose(1, 2)).abs().max())
-                   for qs, ql, ks, kl in problems if ql and kl) * ao.SCALE * 1.4426950408889634
-        q = q * (PEAK / smax)
-    elif name == 'shared_do':
-        d_o = r() + head(10.0)
-    return q, k, v, d_o
+H = 8
+FAMILIES = ao.FAMILIES
 
 
 def _gpu(q, k, v, d_o, problems, o=None, lse=None):
@@ -74,9 +37,9 @@ def _case(family):
     """Inputs and CPU references of a family (computed once per session): the float64 and fp32 references with keys
     k and with keys k + c."""
     if family not in _CASES:
-        self_p, cross_p, n = _layout()
+        self_p, cross_p, n = ao.layout()
         problems = self_p + cross_p
-        q, k, v, d_o = _family(family, n, problems)
+        q, k, v, d_o = ao.family(family, n, problems, H)
         ks = k + ao.key_shift(k, problems, H)
         ref = {(dt, sh): ao.reference(q, kk, v, d_o, problems, H, dt)
                for dt in (torch.float64, torch.float32) for sh, kk in ((False, k), (True, ks))}
