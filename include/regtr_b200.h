@@ -583,6 +583,94 @@ typedef struct {
 } regtr_pose_err_args;
 int regtr_pose_errors(const regtr_pose_err_args* args, void* stream);
 
+/* ---- training losses --------------------------------------------------------------- */
+
+#define REGTR_LOSS_DIM 256       /* d_embed of the InfoNCE kernels */
+#define REGTR_LOSS_MAX_LEVELS 8
+#define REGTR_LOSS_MAX_LAYERS 8
+#define REGTR_LOSS_MAX_TERMS 8
+
+/* Ground-truth overlap of every pyramid level (compute_overlaps, kpconv.py:540-566).  pyr[0] (n[0]) is given: the
+ * stacked level-0 masks as fp32.  Level p >= 1:
+ *   pyr[p][i] = clamp(sum_{valid k} pyr[p-1][pool[p][i,k]] / #valid, 0, 1),  valid: pool[p][i,k] < *n_prev[p],
+ * summed over the K[p] slots in ascending order in fp32, one fp32 division; 0 / 0 stays NaN.  pool[p] is the
+ * (n[p], K[p]) int32 pooling table from level p-1 to level p; n_prev[p] points at the device int32 number of points of
+ * level p-1.  Index 0 of pool, K and n_prev is unused.  One launch per level. */
+typedef struct {
+    float* pyr[REGTR_LOSS_MAX_LEVELS];
+    const int32_t* pool[REGTR_LOSS_MAX_LEVELS];
+    const int32_t* n_prev[REGTR_LOSS_MAX_LEVELS];
+    int n[REGTR_LOSS_MAX_LEVELS];
+    int K[REGTR_LOSS_MAX_LEVELS];
+    int n_levels;
+} regtr_overlap_pyr_args;
+int regtr_overlap_pyramid(const regtr_overlap_pyr_args* args, void* stream);
+
+/* Ws = triu(W) + triu(W)^T of a (256, 256) matrix, written as the TF32 halves regtr_gemm_tf32x3 reads (Ws = hi + lo,
+ * rounded as regtr_split_tf32 rounds), and its adjoint dW += triu(dWs + dWs^T).  One launch each. */
+int regtr_sym_weight(const float* W, float* Ws_hi, float* Ws_lo, void* stream);
+int regtr_sym_weight_bwd(const float* dWs, float* dW, void* stream);
+
+/* The losses of one batch of B pairs on the N packed coarse tokens (source clouds 0..B-1, then target clouds; offs
+ * (2B+1) int32 device starts).  The struct lives in host memory and is passed to the kernels by value; every pointer
+ * inside is device memory.  vals (n_vals) receives the fp32 loss values at the indices named by ov_val / corr_val
+ * (per decoder layer, -1: that layer has no such loss) and term_val (per InfoNCE term).
+ *
+ * regtr_loss_pointwise (one launch): per layer l, the BCE with logits of logit[l] against w, meaned over N, and
+ *   sum w |corr[l] - gt|_1 / max(sum w, 1e-6) over the source tokens (gt = R x + t of the pair's pose) plus the same
+ *   over the target tokens (inverse pose); partial sums in fp64 into ws, and the gradients for a unit upstream
+ *   gradient into dlogit (L, N) and dcorr (L, N, 3) (zeros for a layer without the loss).
+ * regtr_infonce_match (one launch): src_gt (moved source key points), pos (nearest target token of the pair, -1 if
+ *   the target cloud is empty) and anchor (nearest distance < r_p) of every source token; rule in csrc/loss.cu.
+ * regtr_infonce_fwd (one launch): per term t and source token i, lse[t, i] = log sum_j exp(s_ij) over the pair's
+ *   target tokens that are not ignored, s_ij = <q[t][i], feat[t][j]>, and row_loss[t, i] = lse - s_i,pos(i).
+ * regtr_loss_finalize (one launch, one CTA): n_anchor (B), pair_loss[t, b] = sum_anchors row_loss / n_anchor in fp64
+ *   (NaN without an anchor), vals[term_val[t]] = mean_b pair_loss, and the pointwise values from ws.
+ * regtr_loss_pointwise_bwd (one launch): dlogit_out = g[ov_val[l]] * dlogit, dcorr_out = g[corr_val[l]] * dcorr.
+ * regtr_infonce_bwd (two launches): with c_i = anchor_i g[term_val[t]] / (n_anchor(b) B) and
+ *   G_ij = c_i (exp(s_ij - lse_i) - [j = pos(i)]):  dq[t] rows of the source tokens = G feat[t],  dfeat[t] rows of
+ *   the target tokens = G^T q[t].  Source and target rows are owned by different CTAs: no atomics. */
+typedef struct {
+    const float* xyz;       /* (N, 3) coarse key points */
+    const int32_t* offs;    /* (2B + 1) */
+    const float* pose;      /* (B, 3, 4) ground truth */
+    const float* w;         /* (N) coarsest overlap level */
+    const float* logit;     /* (L, N) */
+    const float* corr;      /* (L, N, 3) */
+    float* dlogit;          /* (L, N) unit-upstream gradients */
+    float* dcorr;           /* (L, N, 3) */
+    float* dlogit_out;      /* backward outputs */
+    float* dcorr_out;
+    const float* q[REGTR_LOSS_MAX_TERMS];     /* (>= n_src, 256): source features times Ws */
+    const float* feat[REGTR_LOSS_MAX_TERMS];  /* (N, 256): the term's packed features */
+    float* dq[REGTR_LOSS_MAX_TERMS];          /* (>= n_src, 256) */
+    float* dfeat[REGTR_LOSS_MAX_TERMS];       /* (N, 256): target rows are written */
+    float* src_gt;          /* (N, 3) */
+    int32_t* pos;           /* (N) */
+    int32_t* anchor;        /* (N) */
+    float* lse;             /* (n_terms, N) */
+    float* row_loss;        /* (n_terms, N) */
+    double* pair_loss;      /* (n_terms, B) */
+    int32_t* n_anchor;      /* (B) */
+    float* vals;            /* (n_vals) */
+    const float* g;         /* (n_vals) upstream gradient of vals */
+    double* ws;             /* regtr_loss_ws_bytes(N, L) */
+    size_t ws_bytes;
+    double rp2, rn2;        /* r_p^2, r_n^2 */
+    int N, B, L;
+    int max_src, max_tgt;   /* longest source / target cloud (grid sizes) */
+    int n_terms, n_vals;
+    int ov_val[REGTR_LOSS_MAX_LAYERS], corr_val[REGTR_LOSS_MAX_LAYERS], term_val[REGTR_LOSS_MAX_TERMS];
+    int pad_;
+} regtr_loss_args;
+size_t regtr_loss_ws_bytes(int N, int L);
+int regtr_loss_pointwise(const regtr_loss_args* args, void* stream);
+int regtr_loss_pointwise_bwd(const regtr_loss_args* args, void* stream);
+int regtr_infonce_match(const regtr_loss_args* args, void* stream);
+int regtr_infonce_fwd(const regtr_loss_args* args, void* stream);
+int regtr_infonce_bwd(const regtr_loss_args* args, void* stream);
+int regtr_loss_finalize(const regtr_loss_args* args, void* stream);
+
 /* ---- status word helpers (device uint32) ------------------------------------------ */
 int regtr_status_clear(uint32_t* status, void* stream);
 

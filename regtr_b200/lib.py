@@ -100,6 +100,16 @@ SIGNATURES = {
     'regtr_meter_update': (_I, [_P, _P]),
     'regtr_pose_errors': (_I, [_P, _P]),
     'regtr_modelnet_augment': (_I, [_P, _P]),
+    'regtr_overlap_pyramid': (_I, [_P, _P]),
+    'regtr_sym_weight': (_I, [_P, _P, _P, _P]),
+    'regtr_sym_weight_bwd': (_I, [_P, _P, _P]),
+    'regtr_loss_ws_bytes': (_Z, [_I, _I]),
+    'regtr_loss_pointwise': (_I, [_P, _P]),
+    'regtr_loss_pointwise_bwd': (_I, [_P, _P]),
+    'regtr_infonce_match': (_I, [_P, _P]),
+    'regtr_infonce_fwd': (_I, [_P, _P]),
+    'regtr_infonce_bwd': (_I, [_P, _P]),
+    'regtr_loss_finalize': (_I, [_P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),
 }
 

@@ -5,8 +5,9 @@ Mirror of
   * `compute_overlaps` (/root/reference/src/models/backbone_kpconv/kpconv.py:540-566),
   * `CorrCriterion` (/root/reference/src/models/losses/corr_loss.py:9-40),
   * `InfoNCELossFull` (/root/reference/src/models/losses/feature_loss.py:246-314).
-Plain torch ops on whatever device the predictions live on: this is bookkeeping around the hot path, not part
-of it.  Differentiable: on outputs of `RegTR.forward_train` the gradient flows on into the library's backward
+`compute_loss` is plain torch ops on whatever device the predictions live on: the restatement pinned against the
+reference, and the yardstick of `compute_loss_device`, the same losses on the library's kernels (csrc/loss.cu), which
+`RegTR.compute_loss` takes for the model's own CUDA outputs.  Differentiable: on outputs of `RegTR.forward_train` the gradient flows on into the library's backward
 kernels (everything after the KPConv encoder)."""
 from __future__ import annotations
 
@@ -116,4 +117,58 @@ def compute_loss(model, pred: Dict, batch: Dict) -> Dict[str, torch.Tensor]:
         losses[f'corr_{i}'] = s + t
     wd = loss_weights(cfg)
     losses['total'] = torch.sum(torch.stack([losses[k] * wd[k] for k in losses]))
+    return losses
+
+
+_weight_vectors = {}
+
+
+def _weight_vector(wd: Dict[str, float], keys, device) -> torch.Tensor:
+    """fp32 device vector of the weights of `keys`, uploaded once per (device, weights)."""
+    key = (str(device), tuple((k, float(wd[k])) for k in keys))
+    if key not in _weight_vectors:
+        _weight_vectors[key] = torch.tensor([wd[k] for k in keys], dtype=torch.float32, device=device)
+    return _weight_vectors[key]
+
+
+def device_route(model, pred, batch) -> bool:
+    """True when `compute_loss_device` applies: `pred` carries the packed CUDA tensors its views were cut from, at
+    exact shapes and 256 channels, the InfoNCE loss is configured, and the pyramid has an int32 pooling table for every
+    level."""
+    core = getattr(pred, 'core', None)
+    if core is None or model.cfg.feature_loss_type != 'infonce' or not core['both_un'].is_cuda:
+        return False
+    from . import ops
+    from .kpconv import _meta_private
+    meta = _meta_private(batch['kpconv_meta'], core['both_un'].device)
+    n = sum(meta['_lens'][-1])
+    return (core['both_un'].shape == (n, ops.LOSS_DIM) and core['cond'].shape[1] == n and
+            core['cond'].shape[0] <= ops.LOSS_MAX_LAYERS and len(meta['_points']) <= ops.LOSS_MAX_LEVELS and
+            len(meta['_lens'][-1]) >= 2 and all(p is not None for p in meta['_pools32'][:len(meta['_points']) - 1]))
+
+
+def compute_loss_device(model, pred, batch) -> Dict[str, torch.Tensor]:
+    """`compute_loss` on the library's loss kernels (csrc/loss.cu), for a `pred` that `device_route` accepts: same
+    keys in the same order, same total.  Reads the packed tensors `pred.core`, not the per-cloud views; the number of
+    launches does not depend on the number of pairs and nothing synchronises with the host.  Fills
+    batch['overlap_pyr'] like `compute_loss`."""
+    from . import ops
+    from .kpconv import _meta_private
+    cfg, core = model.cfg, pred.core
+    dev = core['both_un'].device
+    meta = _meta_private(batch['kpconv_meta'], dev)
+    n_lvl = len(meta['_points'])
+    pyr0 = torch.cat(list(batch['src_overlap']) + list(batch['tgt_overlap']), dim=0).type(torch.float)
+    pyr = ops.overlap_pyramid(pyr0, meta['_pools32'][:n_lvl - 1], meta['_offs'], meta['_n_clouds'])
+    batch['overlap_pyr'] = {f'pyr_{p}': t for p, t in enumerate(pyr)}
+    pose = batch['pose']
+    pose = pose if torch.is_tensor(pose) else torch.stack(list(pose))
+    pose = pose[..., :3, :].to(device=dev, dtype=torch.float32).contiguous()
+    geo = ops.LossGeometry(core['xyz_c'], meta['_offs'][-1], meta['_lens'][-1], pose, pyr[-1], cfg.overlap_loss_on,
+                           cfg.feature_loss_on, cfg.corr_loss_on, cfg.r_p, cfg.r_n)
+    vals = ops.loss_values(core['both_un'], core['cond'], core['corr'], core['logit'], model.feature_criterion.W,
+                           model.feature_criterion_un.W, geo)
+    keys = geo.keys()
+    losses = {k: vals[j] for j, k in enumerate(keys)}
+    losses['total'] = torch.sum(vals * _weight_vector(loss_weights(cfg), keys, dev))
     return losses

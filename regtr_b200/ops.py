@@ -1221,3 +1221,202 @@ def modelnet_augment(shapes, params, items, seed: int, step: int, k: int, gamma:
     _lib.check(L.regtr_modelnet_augment(a.ctypes.data, _stream()), 'regtr_modelnet_augment')
     _count(1)
     return out_xyz, out_mask, corr, corr_n
+
+
+# --------------------------------------------------------------------------- training losses
+
+LOSS_DIM, LOSS_MAX_LEVELS, LOSS_MAX_LAYERS, LOSS_MAX_TERMS = 256, 8, 8, 8              # REGTR_LOSS_*
+OVERLAP_PYR_ARGS = np.dtype([('pyr', '<u8', (LOSS_MAX_LEVELS,)), ('pool', '<u8', (LOSS_MAX_LEVELS,)),
+                             ('n_prev', '<u8', (LOSS_MAX_LEVELS,)), ('n', '<i4', (LOSS_MAX_LEVELS,)),
+                             ('K', '<i4', (LOSS_MAX_LEVELS,)), ('n_levels', '<i4')], align=True)
+LOSS_ARGS = np.dtype([('xyz', '<u8'), ('offs', '<u8'), ('pose', '<u8'), ('w', '<u8'), ('logit', '<u8'), ('corr', '<u8'),
+                      ('dlogit', '<u8'), ('dcorr', '<u8'), ('dlogit_out', '<u8'), ('dcorr_out', '<u8'),
+                      ('q', '<u8', (LOSS_MAX_TERMS,)), ('feat', '<u8', (LOSS_MAX_TERMS,)),
+                      ('dq', '<u8', (LOSS_MAX_TERMS,)), ('dfeat', '<u8', (LOSS_MAX_TERMS,)), ('src_gt', '<u8'),
+                      ('pos', '<u8'), ('anchor', '<u8'), ('lse', '<u8'), ('row_loss', '<u8'), ('pair_loss', '<u8'),
+                      ('n_anchor', '<u8'), ('vals', '<u8'), ('g', '<u8'), ('ws', '<u8'), ('ws_bytes', '<u8'),
+                      ('rp2', '<f8'), ('rn2', '<f8'), ('N', '<i4'), ('B', '<i4'), ('L', '<i4'), ('max_src', '<i4'),
+                      ('max_tgt', '<i4'), ('n_terms', '<i4'), ('n_vals', '<i4'), ('ov_val', '<i4', (LOSS_MAX_LAYERS,)),
+                      ('corr_val', '<i4', (LOSS_MAX_LAYERS,)), ('term_val', '<i4', (LOSS_MAX_TERMS,)), ('pad_', '<i4')],
+                     align=True)
+assert (OVERLAP_PYR_ARGS.itemsize, LOSS_ARGS.itemsize) == (264, 568)     # the C structs' sizes
+
+
+def overlap_pyramid(pyr0, pools32, offs, n_clouds: int):
+    """Ground-truth overlap of every pyramid level (regtr_overlap_pyramid): pyr0 (n_0) fp32 level-0 masks; pools32[p-1]
+    the (n_p, K) int32 pooling table into level p; offs[p] the (n_clouds + 1) int32 device offsets of level p.
+    -> [pyr_0, pyr_1, ...].  One launch per level, no host sync."""
+    L = _lib.load()
+    _chk(pyr0, torch.float32, 'pyr0', 1)
+    n_levels = len(pools32) + 1
+    if n_levels > LOSS_MAX_LEVELS or len(offs) < n_levels - 1:
+        raise ValueError(f'overlap_pyramid: {n_levels} levels (at most {LOSS_MAX_LEVELS}), {len(offs)} offset rows')
+    a = np.zeros((), OVERLAP_PYR_ARGS)
+    out = [pyr0]
+    a['pyr'][0], a['n'][0], a['n_levels'] = pyr0.data_ptr(), pyr0.shape[0], n_levels
+    n_launch = 0
+    for p in range(1, n_levels):
+        pool = _chk(pools32[p - 1], torch.int32, 'pool', 2)
+        _chk(offs[p - 1], torch.int32, 'offs', 1)
+        lvl = torch.empty(pool.shape[0], dtype=torch.float32, device=pyr0.device)
+        out.append(lvl)
+        a['pyr'][p], a['pool'][p], a['n'][p], a['K'][p] = lvl.data_ptr(), pool.data_ptr(), pool.shape[0], pool.shape[1]
+        a['n_prev'][p] = offs[p - 1].data_ptr() + 4 * n_clouds
+        n_launch += int(pool.shape[0] > 0)
+    _lib.check(L.regtr_overlap_pyramid(a.ctypes.data, _stream()), 'regtr_overlap_pyramid')
+    _count(n_launch)
+    return out
+
+
+def sym_weight(W):
+    """Ws = triu(W) + triu(W)^T of InfoNCELossFull's (256, 256) matrix, as the (hi, lo) TF32 halves `gemm` reads
+    (regtr_sym_weight): Ws changes with every optimizer step, so it is split where it is built and never cached."""
+    L = _lib.load()
+    _chk(W, torch.float32, 'W', 2)
+    if tuple(W.shape) != (LOSS_DIM, LOSS_DIM):
+        raise _lib.RegtrLibError(f'sym_weight: W {tuple(W.shape)}; the InfoNCE kernels are built for d_embed = {LOSS_DIM}')
+    hi, lo = torch.empty_like(W), torch.empty_like(W)
+    _lib.check(L.regtr_sym_weight(_p(W), _p(hi), _p(lo), _stream()), 'regtr_sym_weight')
+    _count(1)
+    return hi, lo
+
+
+def sym_weight_bwd(dWs, dW):
+    """dW += triu(dWs + dWs^T) (regtr_sym_weight_bwd)."""
+    L = _lib.load()
+    _chk(dWs, torch.float32, 'dWs', 2); _chk(dW, torch.float32, 'dW', 2)
+    _lib.check(L.regtr_sym_weight_bwd(_p(dWs), _p(dW), _stream()), 'regtr_sym_weight_bwd')
+    _count(1)
+
+
+class LossGeometry:
+    """What the device loss reads besides the predictions: xyz (N, 3) coarse key points (source clouds, then target
+    clouds), offs (2B + 1) int32 device offsets and lens, the same lengths on the host, pose (B, 3, 4) fp32 ground
+    truth, w (N) coarsest ground-truth overlap, the layers each loss is applied to, and the InfoNCE radii."""
+
+    def __init__(self, xyz, offs, lens, pose, w, overlap_on, feature_on, corr_on, r_p: float, r_n: float):
+        self.xyz, self.offs, self.lens, self.pose, self.w = xyz, offs, [int(v) for v in lens], pose, w
+        self.B = len(self.lens) // 2
+        self.overlap_on, self.feature_on, self.corr_on = list(overlap_on), list(feature_on), list(corr_on)
+        self.r_p, self.r_n = float(r_p), float(r_n)
+
+    def keys(self):
+        """The loss names in the order of the values vector (the reference's insertion order)."""
+        return [f'overlap_{i}' for i in self.overlap_on] + [f'feature_{i}' for i in self.feature_on] + \
+            ['feature_un'] + [f'corr_{i}' for i in self.corr_on]
+
+
+def loss_forward(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
+    """Loss values of packed predictions: both_un (N, 256), cond (L, N, 256), corr (L, N, 3), logit (L, N, 1), the two
+    InfoNCE matrices.  -> state dict; 'vals' is the fp32 vector of geo.keys(), the rest feeds loss_backward
+    ('pair_loss' (terms, B) fp64 and 'n_anchor' (B) are the per-pair InfoNCE results).  The number of launches does
+    not depend on B; no host sync."""
+    L = _lib.load()
+    dev = both_un.device
+    both_un, cond = _chk(both_un.detach().contiguous(), torch.float32, 'both_un', 2), \
+        _chk(cond.detach().contiguous(), torch.float32, 'cond', 3)
+    corr, logit = _chk(corr.detach().contiguous(), torch.float32, 'corr', 3), \
+        _chk(logit.detach().contiguous(), torch.float32, 'logit', 3)
+    xyz, pose, w = _chk(geo.xyz, torch.float32, 'xyz', 2), _chk(geo.pose, torch.float32, 'pose', 3), \
+        _chk(geo.w, torch.float32, 'w', 1)
+    offs = _chk(geo.offs, torch.int32, 'offs', 1)
+    nl, N, B = cond.shape[0], cond.shape[1], geo.B
+    keys = geo.keys()
+    if both_un.shape != (N, LOSS_DIM) or cond.shape[2] != LOSS_DIM or corr.shape != (nl, N, 3) or \
+            logit.shape != (nl, N, 1) or xyz.shape != (N, 3) or w.shape[0] != N or sum(geo.lens) != N or \
+            tuple(pose.shape) != (B, 3, 4) or offs.shape[0] != 2 * B + 1 or B < 1:
+        raise ValueError('loss_forward: inconsistent shapes')
+    if nl > LOSS_MAX_LAYERS or len(geo.feature_on) + 1 > LOSS_MAX_TERMS or \
+            any(not 0 <= i < nl for i in geo.overlap_on + geo.feature_on + geo.corr_on):
+        raise ValueError(f'loss_forward: {nl} layers, loss layers {geo.overlap_on} {geo.feature_on} {geo.corr_on}')
+    n_src = sum(geo.lens[:B])
+    term_layers = list(geo.feature_on) + [-1]                    # -1: feature_un on both_un with W_un
+    feats = [cond[l] if l >= 0 else both_un for l in term_layers]
+    Ws = [sym_weight(W.detach()), sym_weight(W_un.detach())]
+    T = len(term_layers)
+    q = [gemm(x[:n_src], *Ws[0 if l >= 0 else 1]) if n_src else x.new_zeros((1, LOSS_DIM))
+         for x, l in zip(feats, term_layers)]
+    f32 = dict(dtype=torch.float32, device=dev)
+    st = dict(geo=geo, keys=keys, term_layers=term_layers, feats=feats, Ws=Ws, q=q, n_src=n_src, shape=(nl, N),
+              vals=torch.empty(len(keys), **f32), dlogit=torch.empty((nl, N), **f32), dcorr=torch.empty((nl, N, 3), **f32),
+              src_gt=torch.empty((N, 3), **f32), pos=torch.empty(N, dtype=torch.int32, device=dev),
+              anchor=torch.empty(N, dtype=torch.int32, device=dev), lse=torch.empty((T, N), **f32),
+              row_loss=torch.empty((T, N), **f32), pair_loss=torch.empty((T, B), dtype=torch.float64, device=dev),
+              n_anchor=torch.empty(B, dtype=torch.int32, device=dev))
+    ws = workspace(L.regtr_loss_ws_bytes(N, nl), dev, 'loss')
+    a = np.zeros((), LOSS_ARGS)
+    for f, t in (('xyz', xyz), ('offs', offs), ('pose', pose), ('w', w), ('logit', logit), ('corr', corr), ('ws', ws)):
+        a[f] = t.data_ptr()
+    for f in ('dlogit', 'dcorr', 'src_gt', 'pos', 'anchor', 'lse', 'row_loss', 'pair_loss', 'n_anchor', 'vals'):
+        a[f] = st[f].data_ptr()
+    a['ws_bytes'], a['rp2'], a['rn2'] = ws.numel(), geo.r_p * geo.r_p, geo.r_n * geo.r_n
+    a['N'], a['B'], a['L'], a['n_terms'], a['n_vals'] = N, B, nl, T, len(keys)
+    a['max_src'], a['max_tgt'] = max(geo.lens[:B]), max(geo.lens[B:])
+    a['ov_val'][:], a['corr_val'][:] = -1, -1
+    for i in geo.overlap_on:
+        a['ov_val'][i] = keys.index(f'overlap_{i}')
+    for i in geo.corr_on:
+        a['corr_val'][i] = keys.index(f'corr_{i}')
+    for t, l in enumerate(term_layers):
+        a['q'][t], a['feat'][t] = q[t].data_ptr(), feats[t].data_ptr()
+        a['term_val'][t] = keys.index(f'feature_{l}' if l >= 0 else 'feature_un')
+    st['args'], st['hold'] = a, (xyz, offs, pose, w, logit, corr)
+    s = _stream()
+    _lib.check(L.regtr_loss_pointwise(a.ctypes.data, s), 'regtr_loss_pointwise')
+    _lib.check(L.regtr_infonce_match(a.ctypes.data, s), 'regtr_infonce_match')
+    _lib.check(L.regtr_infonce_fwd(a.ctypes.data, s), 'regtr_infonce_fwd')
+    _lib.check(L.regtr_loss_finalize(a.ctypes.data, s), 'regtr_loss_finalize')
+    _count(int(N > 0 and nl > 0) + 2 * int(a['max_src'] > 0) + 1)
+    return st
+
+
+def loss_backward(st, g):
+    """Gradients of loss_forward's inputs for the upstream gradient g of its values vector (read on the device).
+    -> (d both_un (N, 256), d cond (L, N, 256), d corr (L, N, 3), d logit (L, N, 1), dW, dW_un)."""
+    L = _lib.load()
+    g = _chk(g.contiguous(), torch.float32, 'g', 1)
+    nl, N = st['shape']
+    n_src, term_layers, q = st['n_src'], st['term_layers'], st['q']
+    dev = g.device
+    f32 = dict(dtype=torch.float32, device=dev)
+    d_logit, d_corr = torch.empty((nl, N, 1), **f32), torch.empty((nl, N, 3), **f32)
+    d_un, d_cond = torch.zeros((N, LOSS_DIM), **f32), torch.zeros((nl, N, LOSS_DIM), **f32)
+    dq = torch.zeros((len(term_layers), max(n_src, 1), LOSS_DIM), **f32)
+    dfeat = [d_cond[l] if l >= 0 else d_un for l in term_layers]
+    a = st['args'].copy()
+    a['g'], a['dlogit_out'], a['dcorr_out'] = g.data_ptr(), d_logit.data_ptr(), d_corr.data_ptr()
+    for t in range(len(term_layers)):
+        a['dq'][t], a['dfeat'][t] = dq[t].data_ptr(), dfeat[t].data_ptr()
+    s = _stream()
+    _lib.check(L.regtr_loss_pointwise_bwd(a.ctypes.data, s), 'regtr_loss_pointwise_bwd')
+    _lib.check(L.regtr_infonce_bwd(a.ctypes.data, s), 'regtr_infonce_bwd')
+    _count(int(N > 0 and nl > 0) + int(a['max_src'] > 0) + int(a['max_tgt'] > 0))
+    dW = [torch.zeros((LOSS_DIM, LOSS_DIM), **f32), torch.zeros((LOSS_DIM, LOSS_DIM), **f32)]
+    if n_src:
+        for t, l in enumerate(term_layers):
+            k = 0 if l >= 0 else 1
+            gemm(dq[t, :n_src], *st['Ws'][k], out=dfeat[t][:n_src])          # Ws is symmetric: dA = dQ Ws = dQ Ws^T
+            dWs, _ = linear_wgrad(st['feats'][t][:n_src], dq[t, :n_src], False)
+            sym_weight_bwd(dWs, dW[k])
+    return d_un, d_cond, d_corr, d_logit, dW[0], dW[1]
+
+
+class _LossFn(torch.autograd.Function):
+    """values vector of loss_forward; backward on loss_backward."""
+
+    @staticmethod
+    def forward(ctx, both_un, cond, corr, logit, W, W_un, geo):
+        st = loss_forward(both_un, cond, corr, logit, W, W_un, geo)
+        ctx.st = {k: v for k, v in st.items() if k != 'vals'}    # the output must not be reachable from its own node
+        return st['vals']
+
+    @staticmethod
+    def backward(ctx, g):
+        need = ctx.needs_input_grad
+        grads = loss_backward(ctx.st, g)
+        return tuple(d if n else None for d, n in zip(grads, need)) + (None,)
+
+
+def loss_values(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
+    """The fp32 vector of geo.keys() loss values, differentiable with respect to the packed predictions and both W."""
+    return _LossFn.apply(both_un, cond, corr, logit, W, W_un, geo)

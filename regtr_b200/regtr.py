@@ -45,6 +45,14 @@ class _LossParam(nn.Module):
         self.W = nn.Parameter(torch.zeros(d_embed, d_embed), requires_grad=True)
 
 
+class PackedOutput(dict):
+    """The reference's output dict, plus `core`: the packed tensors (`both_un`, `xyz_c`, `cond`, `corr`, `logit`,
+    `pose`) its per-cloud views were cut from.  Keys and values are those of a plain dict; `compute_loss` reads `core`
+    to run the loss kernels on the packed tokens."""
+
+    core = None
+
+
 class CorrespondenceRegressor(nn.Module):
     """MLP 256->256->256->3 + Linear 256->1 on every layer's features (regtr.py:399-443)."""
 
@@ -176,25 +184,31 @@ class RegTR(nn.Module):
         split = lambda t, dim=0: torch.split(t.narrow(dim, 0, n), lens_c, dim=dim)
         un, kp = split(core['both_un']), split(core['xyz_c'])
         feat, warped, ovl = split(core['cond'], 1), split(core['corr'], 1), split(core['logit'], 1)
-        return {
+        out = PackedOutput({
             'src_feat_un': un[:B], 'tgt_feat_un': un[B:],
             'src_feat': list(feat[:B]), 'tgt_feat': list(feat[B:]),
             'src_kp': kp[:B], 'src_kp_warped': list(warped[:B]),
             'tgt_kp': kp[B:], 'tgt_kp_warped': list(warped[B:]),
             'src_overlap': list(ovl[:B]), 'tgt_overlap': list(ovl[B:]),
             'pose': core['pose'],
-        }
+        })
+        out.core = core
+        return out
 
     def compute_loss(self, pred, batch):
         """Losses of a forward (regtr.py:237-294: overlap BCE, InfoNCE feature losses, L1 correspondence loss,
         weighted total).  For outputs of `forward_train` (which carry autograd history) `total` is differentiable;
         for outputs of `forward` the values are computed without grad, as `test_step` reports them.
-        Needs batch['pose'], ['src_overlap'], ['tgt_overlap'], ['kpconv_meta']."""
+        Needs batch['pose'], ['src_overlap'], ['tgt_overlap'], ['kpconv_meta'].
+        An output of this model's own `forward` / `forward_train` on CUDA goes through the loss kernels
+        (`losses.compute_loss_device`: no host synchronisation, a launch count independent of B); any other `pred`
+        (a hand-built or oracle dict, CPU tensors) goes through the torch restatement `losses.compute_loss`."""
         from . import losses
+        fn = losses.compute_loss_device if losses.device_route(self, pred, batch) else losses.compute_loss
         if torch.is_grad_enabled() and pred['src_feat'][0].requires_grad:
-            return losses.compute_loss(self, pred, batch)
+            return fn(self, pred, batch)
         with torch.no_grad():
-            return losses.compute_loss(self, pred, batch)
+            return fn(self, pred, batch)
 
     def configure_optimizers(self):
         """The reference's solver (generic_reg_model.py:28-62) over self.parameters(), on the library's optimizer:
