@@ -385,6 +385,19 @@ int regtr_grad_norm(const regtr_grad_ref* table, int n_tensors, int n_chunks, fl
 /* g *= *coef for every gradient of the table (coef: device fp32, e.g. out + 1 of regtr_grad_norm).  One launch. */
 int regtr_grad_scale(const regtr_grad_ref* table, int n_tensors, int n_chunks, const float* coef, void* stream);
 
+/* One tensor of a flat fp32 bucket (data-parallel gradient exchange: one collective for every gradient). */
+typedef struct {
+    float* t;             /* fp32 tensor; NULL: packs zeros, unpacks nothing */
+    long long n;          /* elements */
+    long long first;      /* first chunk (REGTR_OPTIM_CHUNK elements) */
+    long long off;        /* first element in the bucket */
+} regtr_bucket_ref;
+
+/* unpack == 0: bucket[off, off + n) = t for every entry; unpack != 0: t = bucket[off, off + n).  One launch, plain
+ * copies (a pack and an unpack round-trip bit for bit). */
+int regtr_bucket_copy(const regtr_bucket_ref* table, int n_tensors, int n_chunks, float* bucket, int unpack,
+                      void* stream);
+
 #define REGTR_ADAM_FRESH 1u      /* state just created: exp_avg / exp_avg_sq are read as zero (and written) */
 #define REGTR_ADAM_COUPLED 2u    /* Adam weight decay: g += wd * p */
 #define REGTR_ADAM_DECOUPLED 4u  /* AdamW weight decay: p *= decay */
@@ -498,6 +511,14 @@ int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src
                         float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
                         int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
                         void* stream);
+/* regtr_train_augment with the device draws of pair b keyed by pair_base + b (0 <= pair_base <= 2^30): a slice of a
+ * batch that starts at global pair pair_base draws exactly what those pairs draw in the whole batch. */
+int regtr_train_augment_at(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
+                           const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
+                           unsigned long long step, int pair_base, double noise, int max_pts, const int32_t* out_offs,
+                           int out_cap, float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
+                           int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
+                           void* stream);
 
 /* ---- training data (ModelNet40) --------------------------------------------------- */
 
@@ -538,6 +559,8 @@ typedef struct {
     int n_shapes, n_pts, n_out, k, B;
 } regtr_modelnet_args;
 int regtr_modelnet_augment(const regtr_modelnet_args* args, void* stream);
+/* regtr_modelnet_augment with the device draws of pair b keyed by pair_base + b (0 <= pair_base <= 2^30). */
+int regtr_modelnet_augment_at(const regtr_modelnet_args* args, int pair_base, void* stream);
 
 /* ---- training-loop bookkeeping ---------------------------------------------------- */
 
@@ -670,6 +693,20 @@ int regtr_infonce_match(const regtr_loss_args* args, void* stream);
 int regtr_infonce_fwd(const regtr_loss_args* args, void* stream);
 int regtr_infonce_bwd(const regtr_loss_args* args, void* stream);
 int regtr_loss_finalize(const regtr_loss_args* args, void* stream);
+
+/* Batch-global normalisers for data-parallel training, where each rank holds a slice of the pairs.
+ * regtr_loss_norms (one launch): out (4 doubles, device) = (N, sum w over the source tokens, sum w over the target
+ *   tokens, B) of this call, the sums in the order regtr_loss_pointwise takes them.
+ * The *_norm variants are regtr_loss_pointwise / regtr_infonce_bwd / regtr_loss_finalize with these four normalisers
+ *   read from `norm` (device) instead of this call's own: the BCE is meaned over norm[0] tokens, the L1 terms divided
+ *   by max(norm[1], 1e-6) and max(norm[2], 1e-6), the InfoNCE terms meaned over norm[3] pairs.  With norm = the
+ *   element-wise sum of every rank's regtr_loss_norms, each rank's values and gradients are its exact share of the
+ *   whole batch's, and the shares add up to them; with norm = this call's own regtr_loss_norms the results are
+ *   bit-identical to the plain entry points.  norm = NULL is the plain entry point. */
+int regtr_loss_norms(const regtr_loss_args* args, double* out, void* stream);
+int regtr_loss_pointwise_norm(const regtr_loss_args* args, const double* norm, void* stream);
+int regtr_infonce_bwd_norm(const regtr_loss_args* args, const double* norm, void* stream);
+int regtr_loss_finalize_norm(const regtr_loss_args* args, const double* norm, void* stream);
 
 /* ---- status word helpers (device uint32) ------------------------------------------ */
 int regtr_status_clear(uint32_t* status, void* stream);

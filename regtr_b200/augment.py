@@ -40,15 +40,15 @@ def pair_draws(seed: int, step: int, pair: int):
     return rng.random(N_UNIFORM), rng.standard_normal(N_NORMAL)
 
 
-def sample_draws(seed: int, step: int, B: int) -> Dict[str, np.ndarray]:
-    """Per-pair scalars of RigidPerturb and RandomSwap:
+def sample_draws(seed: int, step: int, B: int, pair_base: int = 0) -> Dict[str, np.ndarray]:
+    """Per-pair scalars of RigidPerturb and RandomSwap of pairs pair_base .. pair_base + B - 1 of the batch:
       axis (B,3): uniform on the sphere (so3_common.uniform_2_sphere: phi ~ U[0, 2 pi), cos theta ~ U[-1, 1));
       angle (B,): N(0,1) * 0.1 pi / sqrt(3) (SO3.sample_small, std 0.1); trans (B,3): N(0,1) * 0.1 / sqrt(3);
       euler (B,3): U[0, 2 pi) (z, y, x angles of _sample_pose_large);
       perturb_source (B,): `random.random() > 0.5`; swap (B,): `random.random() > 0.5`."""
     u = np.empty((B, N_UNIFORM)); g = np.empty((B, N_NORMAL))
     for b in range(B):
-        u[b], g[b] = pair_draws(seed, step, b)
+        u[b], g[b] = pair_draws(seed, step, pair_base + b)
     phi, cos_t = 2 * np.pi * u[:, 0], 2.0 * u[:, 1] - 1.0
     sin_t = np.sin(np.arccos(cos_t))
     return dict(axis=np.stack([sin_t * np.cos(phi), sin_t * np.sin(phi), cos_t], axis=1),
@@ -99,7 +99,9 @@ class TrainingPrep:
       src_path / tgt_path (swapped where the pair was swapped), idx, overlap_p; aug: the host draws, the flags,
       seed and step.
     augment=False is the reference's val phase: overlap ground truth only, the clouds and the pose as given.
-    `step` counts the calls; the draws of a call depend on (seed, step) only."""
+    `step` counts the calls; the draws of a call depend on (seed, step) only.  pair_base: the position of the first
+    pair in the global batch when `batch` is a slice of it (data parallelism): pair b draws what pair pair_base + b
+    of the whole batch draws."""
 
     def __init__(self, cfg, seed: int = 0, max_pts: int = MAX_PTS, perturb_mode=None, noise=None):
         self.radius = float(cfg.overlap_radius)
@@ -135,7 +137,7 @@ class TrainingPrep:
         self._check_pending(block=True)
 
     # ------------------------------------------------------------------------------------------------------ call
-    def __call__(self, batch: Dict, augment: bool = True) -> LazyDict:
+    def __call__(self, batch: Dict, augment: bool = True, pair_base: int = 0) -> LazyDict:
         self._check_pending(block=False)
         src, tgt = list(batch['src_xyz']), list(batch['tgt_xyz'])
         B = len(src)
@@ -156,7 +158,7 @@ class TrainingPrep:
             raise ValueError(f'{n} points in one batch: at most 2^30 are supported')
 
         if augment:
-            draws = sample_draws(self.seed, step, B)
+            draws = sample_draws(self.seed, step, B, pair_base)
             P = perturbations(draws, self.mode)
             flags = (ops.PREP_PERTURB_SRC * draws['perturb_source'] + ops.PREP_SWAP * draws['swap'] +
                      ops.PREP_CENTRE * (self.mode == 'small') + ops.PREP_SHUFFLE).astype(np.int32)
@@ -197,7 +199,8 @@ class TrainingPrep:
         status = ops.new_status(dev)
         nn = ops.overlap_nn(xyz, offs_d, B, pose64, self.radius, status)
         out_xyz, out_mask, out_pose, corr, corr_offs = ops.train_augment(
-            xyz, offs_d, B, n_src, pose64, nn, pert, flags_d, self.seed, step, noise, max_pts, out_offs_d, n_out)
+            xyz, offs_d, B, n_src, pose64, nn, pert, flags_d, self.seed, step, noise, max_pts, out_offs_d, n_out,
+            pair_base)
         word = torch.empty(1, dtype=torch.int32, pin_memory=True)
         word.copy_(status, non_blocking=True)
         ev = torch.cuda.Event()

@@ -114,17 +114,37 @@ __global__ void k_sym_weight_bwd(const float* __restrict__ dWs, float* __restric
 
 // ---------------------------------------------------------------------------------------------- BCE and L1
 
-// ws: [L][n_chunks][3] partial sums (bce, src w*err, tgt w*err), then the two denominators max(sum w, 1e-6).
-__global__ void __launch_bounds__(PW) k_loss_pointwise(const regtr_loss_args a) {
-    __shared__ double red[PW / 32];
-    const int l = blockIdx.y, chunk = blockIdx.x, n_chunks = gridDim.x;
+// Sum of w over the source and over the target tokens, in the one order every normaliser of this file uses.
+__device__ __forceinline__ void weight_sums(const regtr_loss_args& a, double* red, double& ws, double& wt) {
     const int n_src = a.offs[a.B];
-    double ws = 0.0, wt = 0.0;
+    ws = 0.0;
+    wt = 0.0;
     for (int i = threadIdx.x; i < a.N; i += PW) {
         const double v = (double)a.w[i];
         if (i < n_src) ws += v; else wt += v;
     }
-    const double den_s = fmax(block_sum(ws, red), 1e-6), den_t = fmax(block_sum(wt, red), 1e-6);
+    ws = block_sum(ws, red);
+    wt = block_sum(wt, red);
+}
+
+// The normalisers of the batch: (token count, source sum w, target sum w, pair count) from `norm` when given (the sums
+// over the ranks of a data-parallel step), else this call's own.
+struct Norms {
+    double n, ws, wt, b;
+};
+
+__device__ __forceinline__ Norms batch_norms(const regtr_loss_args& a, const double* __restrict__ norm) {
+    if (norm) return Norms{norm[0], norm[1], norm[2], norm[3]};
+    return Norms{(double)a.N, 0.0, 0.0, (double)a.B};
+}
+
+// ws: [L][n_chunks][3] partial sums (bce, src w*err, tgt w*err), then the two denominators max(sum w, 1e-6).
+__global__ void __launch_bounds__(PW) k_loss_pointwise(const regtr_loss_args a, const double* __restrict__ norm) {
+    __shared__ double red[PW / 32];
+    const int l = blockIdx.y, chunk = blockIdx.x, n_chunks = gridDim.x;
+    Norms nm = batch_norms(a, norm);
+    if (!norm) weight_sums(a, red, nm.ws, nm.wt);
+    const double den_s = fmax(nm.ws, 1e-6), den_t = fmax(nm.wt, 1e-6);
     const bool ov_on = a.ov_val[l] >= 0, corr_on = a.corr_val[l] >= 0;
     const int i = chunk * PW + threadIdx.x;
     double bce = 0.0, es = 0.0, et = 0.0;
@@ -136,7 +156,7 @@ __global__ void __launch_bounds__(PW) k_loss_pointwise(const regtr_loss_args a) 
         const float x = a.logit[li];
         if (ov_on) {
             bce = (double)(fmaxf(x, 0.f) - x * y + log1pf(expf(-fabsf(x))));
-            a.dlogit[li] = (1.f / (1.f + expf(-x)) - y) / (float)a.N;
+            a.dlogit[li] = (1.f / (1.f + expf(-x)) - y) / (float)nm.n;
         } else {
             a.dlogit[li] = 0.f;
         }
@@ -267,12 +287,13 @@ __device__ __forceinline__ void load_tgt_meta(Tile& T, const regtr_loss_args& a,
 }
 
 // Gradient weight c_i of a source row: anchor / (anchors of the pair * B) times the upstream gradient of the term.
-__device__ __forceinline__ void load_src_grad(Tile& T, const regtr_loss_args& a, int term, int b, int i0, int n_i) {
+__device__ __forceinline__ void load_src_grad(Tile& T, const regtr_loss_args& a, int term, int b, int i0, int n_i,
+                                              double n_pairs) {
     if (threadIdx.x >= 64 && threadIdx.x < 64 + TM) {
         const int r = threadIdx.x - 64;
         float c = 0.f, lse = 0.f;
         if (r < n_i && a.anchor[i0 + r]) {
-            c = (float)((double)a.g[a.term_val[term]] / ((double)a.n_anchor[b] * (double)a.B));
+            c = (float)((double)a.g[a.term_val[term]] / ((double)a.n_anchor[b] * n_pairs));
             lse = a.lse[(long long)term * a.N + i0 + r];
         }
         T.c[r] = c;
@@ -329,7 +350,7 @@ __global__ void __launch_bounds__(256) k_infonce_fwd(const regtr_loss_args a) {
 }
 
 // dQ = G P, one CTA per tile of source rows; thread c owns channel c of all its rows.
-__global__ void __launch_bounds__(256) k_infonce_bwd_src(const regtr_loss_args a) {
+__global__ void __launch_bounds__(256) k_infonce_bwd_src(const regtr_loss_args a, const double* __restrict__ norm) {
     __shared__ Tile T;
     const int term = blockIdx.z, b = blockIdx.y;
     const int s0 = a.offs[b], t0 = a.offs[a.B + b], n_t = a.offs[a.B + b + 1] - t0;
@@ -338,7 +359,7 @@ __global__ void __launch_bounds__(256) k_infonce_bwd_src(const regtr_loss_args a
     const int ro = 2 * (threadIdx.x >> 4), co = 2 * (threadIdx.x & 15), ch = threadIdx.x;
     load_resident(T, a.q[term] + (long long)i0 * D, n_i);
     load_src_meta(T, a, i0, n_i);
-    load_src_grad(T, a, term, b, i0, n_i);
+    load_src_grad(T, a, term, b, i0, n_i, batch_norms(a, norm).b);
     float out[TM];
 #pragma unroll
     for (int r = 0; r < TM; ++r) out[r] = 0.f;
@@ -367,7 +388,7 @@ __global__ void __launch_bounds__(256) k_infonce_bwd_src(const regtr_loss_args a
 }
 
 // dP = G^T Q, one CTA per tile of target rows, written into the term's packed feature gradient.
-__global__ void __launch_bounds__(256) k_infonce_bwd_tgt(const regtr_loss_args a) {
+__global__ void __launch_bounds__(256) k_infonce_bwd_tgt(const regtr_loss_args a, const double* __restrict__ norm) {
     __shared__ Tile T;
     const int term = blockIdx.z, b = blockIdx.y;
     const int s0 = a.offs[b], n_s = a.offs[b + 1] - s0, t0 = a.offs[a.B + b];
@@ -383,7 +404,7 @@ __global__ void __launch_bounds__(256) k_infonce_bwd_tgt(const regtr_loss_args a
         const int n_i = min(TM, n_s - i0);
         __syncthreads();
         load_src_meta(T, a, s0 + i0, n_i);
-        load_src_grad(T, a, term, b, s0 + i0, n_i);
+        load_src_grad(T, a, term, b, s0 + i0, n_i, batch_norms(a, norm).b);
         float acc[2][2];                                          // [target ro + u][source co + v]
         const float* Q = a.q[term] + (long long)(s0 + i0) * D;
         tile_dots(T, Q, n_i, acc);
@@ -406,7 +427,8 @@ __global__ void __launch_bounds__(256) k_infonce_bwd_tgt(const regtr_loss_args a
 
 // ---------------------------------------------------------------------------------------------- loss values
 
-__global__ void k_loss_finalize(const regtr_loss_args a, int n_chunks) {
+__global__ void k_loss_finalize(const regtr_loss_args a, int n_chunks, const double* __restrict__ norm) {
+    const Norms nm = batch_norms(a, norm);
     for (int b = threadIdx.x; b < a.B; b += blockDim.x) {
         int n = 0;
         for (int i = a.offs[b]; i < a.offs[b + 1]; ++i) n += a.anchor[i];
@@ -424,7 +446,7 @@ __global__ void k_loss_finalize(const regtr_loss_args a, int n_chunks) {
     for (int t = threadIdx.x; t < a.n_terms; t += blockDim.x) {
         double s = 0.0;
         for (int b = 0; b < a.B; ++b) s += a.pair_loss[t * a.B + b];
-        a.vals[a.term_val[t]] = (float)(s / (double)a.B);
+        a.vals[a.term_val[t]] = (float)(s / nm.b);
     }
     const double* den = a.ws + (long long)a.L * n_chunks * 3;
     for (int l = threadIdx.x; l < a.L; l += blockDim.x) {
@@ -433,8 +455,17 @@ __global__ void k_loss_finalize(const regtr_loss_args a, int n_chunks) {
             const double* p = a.ws + ((long long)l * n_chunks + c) * 3;
             bce += p[0]; es += p[1]; et += p[2];
         }
-        if (a.ov_val[l] >= 0) a.vals[a.ov_val[l]] = (float)(bce / (double)a.N);
+        if (a.ov_val[l] >= 0) a.vals[a.ov_val[l]] = (float)(bce / nm.n);
         if (a.corr_val[l] >= 0) a.vals[a.corr_val[l]] = (float)(es / den[0] + et / den[1]);
+    }
+}
+
+__global__ void __launch_bounds__(PW) k_loss_norms(const regtr_loss_args a, double* __restrict__ out) {
+    __shared__ double red[PW / 32];
+    double ws, wt;
+    weight_sums(a, red, ws, wt);
+    if (threadIdx.x == 0) {
+        out[0] = (double)a.N; out[1] = ws; out[2] = wt; out[3] = (double)a.B;
     }
 }
 
@@ -484,16 +515,29 @@ size_t regtr_loss_ws_bytes(int N, int L) {
     return regtr_align(((size_t)(L > 0 ? L : 0) * n_chunks_of(N) * 3 + 2) * sizeof(double));
 }
 
-int regtr_loss_pointwise(const regtr_loss_args* args, void* stream_) {
+int regtr_loss_norms(const regtr_loss_args* args, double* out, void* stream_) {
+    const int rc = check_args(args);
+    if (rc) return rc;
+    if (!out || (args->N > 0 && !args->w)) return REGTR_ERR_ARG;
+    k_loss_norms<<<1, PW, 0, (cudaStream_t)stream_>>>(*args, out);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_loss_pointwise_norm(const regtr_loss_args* args, const double* norm, void* stream_) {
     const int rc = check_args(args);
     if (rc) return rc;
     const regtr_loss_args& a = *args;
     if (a.N == 0 || a.L == 0) return REGTR_OK;
     if (!a.xyz || !a.pose || !a.w || !a.logit || !a.corr || !a.dlogit || !a.dcorr || !a.ws) return REGTR_ERR_ARG;
     if (a.ws_bytes < regtr_loss_ws_bytes(a.N, a.L)) return REGTR_ERR_WORKSPACE;
-    k_loss_pointwise<<<dim3(n_chunks_of(a.N), a.L), PW, 0, (cudaStream_t)stream_>>>(a);
+    k_loss_pointwise<<<dim3(n_chunks_of(a.N), a.L), PW, 0, (cudaStream_t)stream_>>>(a, norm);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
+}
+
+int regtr_loss_pointwise(const regtr_loss_args* args, void* stream_) {
+    return regtr_loss_pointwise_norm(args, nullptr, stream_);
 }
 
 int regtr_loss_pointwise_bwd(const regtr_loss_args* args, void* stream_) {
@@ -538,24 +582,28 @@ int regtr_infonce_fwd(const regtr_loss_args* args, void* stream_) {
     return REGTR_OK;
 }
 
-int regtr_infonce_bwd(const regtr_loss_args* args, void* stream_) {
+int regtr_infonce_bwd_norm(const regtr_loss_args* args, const double* norm, void* stream_) {
     int rc = check_args(args);
     if (rc) return rc;
     const regtr_loss_args& a = *args;
     if (a.n_terms == 0) return REGTR_OK;
     if ((rc = check_terms(a, true)) || !a.g || !a.n_anchor) return REGTR_ERR_ARG;
     if (a.max_src > 0) {
-        k_infonce_bwd_src<<<dim3(regtr_cdiv(a.max_src, TM), a.B, a.n_terms), 256, 0, (cudaStream_t)stream_>>>(a);
+        k_infonce_bwd_src<<<dim3(regtr_cdiv(a.max_src, TM), a.B, a.n_terms), 256, 0, (cudaStream_t)stream_>>>(a, norm);
         REGTR_CHECK_LAUNCH();
     }
     if (a.max_tgt > 0) {
-        k_infonce_bwd_tgt<<<dim3(regtr_cdiv(a.max_tgt, TM), a.B, a.n_terms), 256, 0, (cudaStream_t)stream_>>>(a);
+        k_infonce_bwd_tgt<<<dim3(regtr_cdiv(a.max_tgt, TM), a.B, a.n_terms), 256, 0, (cudaStream_t)stream_>>>(a, norm);
         REGTR_CHECK_LAUNCH();
     }
     return REGTR_OK;
 }
 
-int regtr_loss_finalize(const regtr_loss_args* args, void* stream_) {
+int regtr_infonce_bwd(const regtr_loss_args* args, void* stream_) {
+    return regtr_infonce_bwd_norm(args, nullptr, stream_);
+}
+
+int regtr_loss_finalize_norm(const regtr_loss_args* args, const double* norm, void* stream_) {
     const int rc = check_args(args);
     if (rc) return rc;
     const regtr_loss_args& a = *args;
@@ -563,9 +611,13 @@ int regtr_loss_finalize(const regtr_loss_args* args, void* stream_) {
     if (a.ws_bytes < regtr_loss_ws_bytes(a.N, a.L)) return REGTR_ERR_WORKSPACE;
     for (int l = 0; l < a.L; ++l)
         if (a.ov_val[l] >= a.n_vals || a.corr_val[l] >= a.n_vals) return REGTR_ERR_ARG;
-    k_loss_finalize<<<1, 256, 0, (cudaStream_t)stream_>>>(a, n_chunks_of(a.N));
+    k_loss_finalize<<<1, 256, 0, (cudaStream_t)stream_>>>(a, n_chunks_of(a.N), norm);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
+}
+
+int regtr_loss_finalize(const regtr_loss_args* args, void* stream_) {
+    return regtr_loss_finalize_norm(args, nullptr, stream_);
 }
 
 }  // extern "C"

@@ -59,7 +59,7 @@ __device__ __forceinline__ int cta_excl_scan(int v, int* s_warp, int& total) {
     return base + inc - v;
 }
 
-__global__ void __launch_bounds__(MN_T, 1) k_modelnet_augment(const regtr_modelnet_args a) {
+__global__ void __launch_bounds__(MN_T, 1) k_modelnet_augment(const regtr_modelnet_args a, int pair_base) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     MnSmem& s = *reinterpret_cast<MnSmem*>(smem_raw);
     const int b = blockIdx.x, t = threadIdx.x, n = a.n_pts, n_out = a.n_out;
@@ -175,7 +175,7 @@ __global__ void __launch_bounds__(MN_T, 1) k_modelnet_augment(const regtr_modeln
     // 5-7. the ordered subset, the transform of the source, the jitter
     const Keys ks = make_keys(a.seed, a.step);
     for (int side = 0; side < 2; ++side) {
-        const Perm pm = make_perm(n_kept[side], true, ks, b, side);
+        const Perm pm = make_perm(n_kept[side], true, ks, pair_base + b, side);
         const size_t slot = (size_t)(side * a.B + b) * n_out;
         for (int j = t; j < n_out; j += MN_T) {
             const int i = kept[side * MN_N + (int)perm_fwd(pm, (unsigned)j)];
@@ -192,7 +192,8 @@ __global__ void __launch_bounds__(MN_T, 1) k_modelnet_augment(const regtr_modeln
                 for (int ax = 0; ax < 3; ++ax) v[ax] = (double)w[ax];
             }
             if (a.noise != 0.0) {
-                const U4 r = philox(U4{(unsigned)i, 2u * (unsigned)b + (unsigned)side, ks.s0, ks.s1}, ks.k0, ks.k1);
+                const U4 r = philox(U4{(unsigned)i, 2u * (unsigned)(pair_base + b) + (unsigned)side, ks.s0, ks.s1},
+                                    ks.k0, ks.k1);
                 const double m0 = sqrt(-2.0 * log(u01(r.x))), m1 = sqrt(-2.0 * log(u01(r.z)));
                 double s0, c0, s1, c1;
                 sincospi(2.0 * u01(r.y), &s0, &c0);
@@ -229,8 +230,8 @@ __global__ void __launch_bounds__(MN_T, 1) k_modelnet_augment(const regtr_modeln
 
 }  // namespace
 
-extern "C" int regtr_modelnet_augment(const regtr_modelnet_args* args, void* stream_) {
-    if (!args) return REGTR_ERR_ARG;
+extern "C" int regtr_modelnet_augment_at(const regtr_modelnet_args* args, int pair_base, void* stream_) {
+    if (!args || pair_base < 0 || pair_base > (1 << 30)) return REGTR_ERR_ARG;
     const regtr_modelnet_args& a = *args;
     if (a.B <= 0 || a.B > 65535 || a.n_pts <= 0 || a.n_pts > REGTR_MODELNET_MAX_PTS || a.n_shapes <= 0 ||
         a.n_out <= 0 || a.n_out > a.n_pts || a.k < -1 || a.k > a.n_pts - 2 || !(a.gamma >= 0.0 && a.gamma < 1.0) ||
@@ -240,7 +241,11 @@ extern "C" int regtr_modelnet_augment(const regtr_modelnet_args* args, void* str
     const size_t smem = sizeof(MnSmem);
     if (cudaFuncSetAttribute(k_modelnet_augment, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
         return REGTR_ERR_UNSUPPORTED;
-    k_modelnet_augment<<<a.B, MN_T, smem, (cudaStream_t)stream_>>>(a);
+    k_modelnet_augment<<<a.B, MN_T, smem, (cudaStream_t)stream_>>>(a, pair_base);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
+}
+
+extern "C" int regtr_modelnet_augment(const regtr_modelnet_args* args, void* stream_) {
+    return regtr_modelnet_augment_at(args, 0, stream_);
 }

@@ -13,6 +13,7 @@
 static_assert(sizeof(regtr_grad_ref) == 24, "regtr_grad_ref layout");
 static_assert(sizeof(regtr_adam_tensor) == 88, "regtr_adam_tensor layout");
 static_assert(sizeof(regtr_split_view) == 56, "regtr_split_view layout");
+static_assert(sizeof(regtr_bucket_ref) == 32, "regtr_bucket_ref layout");
 
 namespace {
 
@@ -31,6 +32,25 @@ __device__ __forceinline__ int owner_of(const T* __restrict__ tab, int n, long l
         if (tab[mid].first <= t) lo = mid; else hi = mid;
     }
     return lo;
+}
+
+// ---- gradient bucket -------------------------------------------------------------------------------------------
+// One CTA per chunk of one tensor: pack copies the tensor into bucket[off, off + n) (zeros for a null tensor), unpack
+// copies it back (nothing for a null tensor).  Plain copies: the values are bit-identical after a round trip.
+__global__ void __launch_bounds__(UPD_THREADS)
+k_bucket_chunks(const regtr_bucket_ref* __restrict__ tab, int n_tensors, float* __restrict__ bucket, bool unpack) {
+    const long long c = blockIdx.x;
+    const int i = owner_of(tab, n_tensors, c);
+    float* __restrict__ t = tab[i].t;
+    const long long base = (c - tab[i].first) * CHUNK;
+    const int len = (int)min((long long)CHUNK, tab[i].n - base);
+    float* __restrict__ b = bucket + tab[i].off + base;
+    if (unpack) {
+        if (t)
+            for (int k = threadIdx.x; k < len; k += UPD_THREADS) t[base + k] = b[k];
+    } else {
+        for (int k = threadIdx.x; k < len; k += UPD_THREADS) b[k] = t ? t[base + k] : 0.f;
+    }
 }
 
 // ---- gradient norm ----------------------------------------------------------------------------------------------
@@ -215,6 +235,15 @@ int regtr_grad_norm(const regtr_grad_ref* table, int n_tensors, int n_chunks, fl
     double* partial = static_cast<double*>(ws);
     if (n_chunks > 0) k_sumsq_chunks<<<n_chunks, NORM_THREADS, 0, st>>>(table, n_tensors, partial);
     k_norm_finalize<<<1, FIN_THREADS, 0, st>>>(partial, n_chunks, max_norm, out);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_bucket_copy(const regtr_bucket_ref* table, int n_tensors, int n_chunks, float* bucket, int unpack,
+                      void* stream_) {
+    if (n_tensors < 0 || n_chunks < 0 || !bucket || (n_chunks > 0 && (!table || n_tensors == 0))) return REGTR_ERR_ARG;
+    if (n_chunks == 0) return REGTR_OK;
+    k_bucket_chunks<<<n_chunks, UPD_THREADS, 0, (cudaStream_t)stream_>>>(table, n_tensors, bucket, unpack != 0);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
 }

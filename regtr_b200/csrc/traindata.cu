@@ -237,11 +237,12 @@ __device__ __forceinline__ int input_cloud(int s, int B, const int32_t* __restri
 
 // One thread per output point: out[k] of slot s = transform(in[perm(k)]) + noise, one fp32 rounding of the float64
 // value; the overlap mask follows the permutation.  The noise of input point j of (pair, side) is
-// sigma * Box-Muller(Philox(counter = (j, 2 pair + side, step), key = seed)).
+// sigma * Box-Muller(Philox(counter = (j, 2 pair + side, step), key = seed)), pair = pair_base + b: the position of
+// the pair in the global batch, so a slice of a batch draws what the same pairs draw in the whole batch.
 __global__ void k_augment_points(const double* __restrict__ xyz, const int32_t* __restrict__ offs, int B,
                                  const int32_t* __restrict__ nn, const double* __restrict__ mat,
                                  const int32_t* __restrict__ flags, const int32_t* __restrict__ out_offs, int out_cap,
-                                 unsigned long long seed, unsigned long long step, double noise,
+                                 unsigned long long seed, unsigned long long step, int pair_base, double noise,
                                  float* __restrict__ out_xyz, uint8_t* __restrict__ out_mask) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= out_cap || p >= out_offs[2 * B]) return;
@@ -250,14 +251,14 @@ __global__ void k_augment_points(const double* __restrict__ xyz, const int32_t* 
     const int b = cin < B ? cin : cin - B, side = cin < B ? 0 : 1;
     const Keys ks = make_keys(seed, step);
     const int a0 = offs[cin];
-    const Perm pm = make_perm(offs[cin + 1] - a0, (flags[b] & REGTR_PREP_SHUFFLE) != 0, ks, b, side);
+    const Perm pm = make_perm(offs[cin + 1] - a0, (flags[b] & REGTR_PREP_SHUFFLE) != 0, ks, pair_base + b, side);
     const unsigned j = perm_fwd(pm, (unsigned)(p - out_offs[s]));
     const int i = a0 + (int)j;
     const double* m = mat + 12 * cin;
     const double x = xyz[3 * i + 0], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
     double v[3] = {rt_row(m, x, y, z), rt_row(m + 4, x, y, z), rt_row(m + 8, x, y, z)};
     if (noise != 0.0) {
-        const U4 r = philox(U4{j, 2u * (unsigned)b + (unsigned)side, ks.s0, ks.s1}, ks.k0, ks.k1);
+        const U4 r = philox(U4{j, 2u * (unsigned)(pair_base + b) + (unsigned)side, ks.s0, ks.s1}, ks.k0, ks.k1);
         const double m0 = sqrt(-2.0 * log(u01(r.x))), m1 = sqrt(-2.0 * log(u01(r.z)));
         double s0, c0, s1, c1;
         sincospi(2.0 * u01(r.y), &s0, &c0);
@@ -274,7 +275,7 @@ __global__ void k_augment_points(const double* __restrict__ xyz, const int32_t* 
 // (new source index, new target index) before the swap.  flag[n_src_cap] = 0 (the scan's total).
 __global__ void k_corr_flags(const int32_t* __restrict__ offs, int B, int n_src_cap, const int32_t* __restrict__ nn,
                              const int32_t* __restrict__ flags, unsigned long long seed, unsigned long long step,
-                             int max_pts, int32_t* __restrict__ flag, int2* __restrict__ pos) {
+                             int pair_base, int max_pts, int32_t* __restrict__ flag, int2* __restrict__ pos) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i > n_src_cap) return;
     int keep = 0;
@@ -285,8 +286,8 @@ __global__ void k_corr_flags(const int32_t* __restrict__ offs, int B, int n_src_
         if (s > 0 && nn[offs[B + b] + s] == il) {
             const Keys ks = make_keys(seed, step);
             const bool sh = (flags[b] & REGTR_PREP_SHUFFLE) != 0;
-            const int a = (int)perm_inv(make_perm(ns, sh, ks, b, 0), (unsigned)il);
-            const int t = (int)perm_inv(make_perm(nt, sh, ks, b, 1), (unsigned)s);
+            const int a = (int)perm_inv(make_perm(ns, sh, ks, pair_base + b, 0), (unsigned)il);
+            const int t = (int)perm_inv(make_perm(nt, sh, ks, pair_base + b, 1), (unsigned)s);
             if (a < min(ns, max_pts) && t < min(nt, max_pts)) { keep = 1; pos[i] = make_int2(a, t); }
         }
     }
@@ -409,13 +410,14 @@ int regtr_registration_fit(const double* xyz, const int32_t* offs, int B, int n_
 size_t regtr_train_augment_ws_bytes(int n_src_cap, int B) { return carve_aug(nullptr, n_src_cap, B).total; }
 size_t regtr_train_augment_state_bytes(int n_src_cap) { return scan_state_bytes((long long)n_src_cap + 1); }
 
-int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
-                        const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
-                        unsigned long long step, double noise, int max_pts, const int32_t* out_offs, int out_cap,
-                        float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
-                        int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
-                        void* stream_) {
+int regtr_train_augment_at(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
+                           const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
+                           unsigned long long step, int pair_base, double noise, int max_pts, const int32_t* out_offs,
+                           int out_cap, float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
+                           int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
+                           void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
+    if (pair_base < 0 || pair_base > (1 << 30)) return REGTR_ERR_ARG;
     if (!offs || !pose || !pert || !flags || !out_offs || !out_pose || !corr_offs || B <= 0 || 2 * B > 32767 ||
         n_src_cap < 0 || n_src_cap >= (1 << 30) || out_cap < 0 || corr_cap < n_src_cap || max_pts < 0 ||
         !(noise >= 0.0) || !ws || !state)
@@ -428,11 +430,11 @@ int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src
     REGTR_CHECK_LAUNCH();
     if (out_cap > 0) {
         k_augment_points<<<regtr_cdiv(out_cap, T), T, 0, st>>>(xyz, offs, B, nn, w.mat, flags, out_offs, out_cap, seed,
-                                                               step, noise, out_xyz, out_mask);
+                                                               step, pair_base, noise, out_xyz, out_mask);
         REGTR_CHECK_LAUNCH();
     }
-    k_corr_flags<<<regtr_cdiv(n_src_cap + 1, T), T, 0, st>>>(offs, B, n_src_cap, nn, flags, seed, step, max_pts,
-                                                            w.flag, w.pos);
+    k_corr_flags<<<regtr_cdiv(n_src_cap + 1, T), T, 0, st>>>(offs, B, n_src_cap, nn, flags, seed, step, pair_base,
+                                                            max_pts, w.flag, w.pos);
     REGTR_CHECK_LAUNCH();
     const int rc = launch_scan<0>(w.flag, w.pre, n_src_cap + 1, nullptr, state, st);
     if (rc != REGTR_OK) return rc;
@@ -441,6 +443,17 @@ int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src
                                                                                   corr_offs);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
+}
+
+int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
+                        const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
+                        unsigned long long step, double noise, int max_pts, const int32_t* out_offs, int out_cap,
+                        float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
+                        int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
+                        void* stream_) {
+    return regtr_train_augment_at(xyz, offs, B, n_src_cap, pose, nn, pert, flags, seed, step, 0, noise, max_pts,
+                                  out_offs, out_cap, out_xyz, out_mask, out_pose, corr, corr_cap, corr_offs, ws,
+                                  ws_bytes, state, state_bytes, stream_);
 }
 
 }  // extern "C"

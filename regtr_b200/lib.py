@@ -84,6 +84,7 @@ SIGNATURES = {
     'regtr_grad_norm_ws_bytes': (_Z, [_I]),
     'regtr_grad_norm': (_I, [_P, _I, _I, _F, _P, _P, _Z, _P]),
     'regtr_grad_scale': (_I, [_P, _I, _I, _P, _P]),
+    'regtr_bucket_copy': (_I, [_P, _I, _I, _P, _I, _P]),
     'regtr_adam_step': (_I, [_P, _I, _I, _P]),
     'regtr_split_refresh': (_I, [_P, _I, _I, _P]),
     'regtr_kabsch_fwd': (_I, [_P, _P, _P, _P, _I, _P, _P]),
@@ -97,9 +98,12 @@ SIGNATURES = {
     'regtr_train_augment_state_bytes': (_Z, [_I]),
     'regtr_train_augment': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _c.c_ulonglong, _c.c_ulonglong, _c.c_double, _I,
                                  _P, _I, _P, _P, _P, _P, _I, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_train_augment_at': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _c.c_ulonglong, _c.c_ulonglong, _I, _c.c_double,
+                                    _I, _P, _I, _P, _P, _P, _P, _I, _P, _P, _Z, _P, _Z, _P]),
     'regtr_meter_update': (_I, [_P, _P]),
     'regtr_pose_errors': (_I, [_P, _P]),
     'regtr_modelnet_augment': (_I, [_P, _P]),
+    'regtr_modelnet_augment_at': (_I, [_P, _I, _P]),
     'regtr_overlap_pyramid': (_I, [_P, _P]),
     'regtr_sym_weight': (_I, [_P, _P, _P, _P]),
     'regtr_sym_weight_bwd': (_I, [_P, _P, _P]),
@@ -110,6 +114,10 @@ SIGNATURES = {
     'regtr_infonce_fwd': (_I, [_P, _P]),
     'regtr_infonce_bwd': (_I, [_P, _P]),
     'regtr_loss_finalize': (_I, [_P, _P]),
+    'regtr_loss_norms': (_I, [_P, _P, _P]),
+    'regtr_loss_pointwise_norm': (_I, [_P, _P, _P]),
+    'regtr_infonce_bwd_norm': (_I, [_P, _P, _P]),
+    'regtr_loss_finalize_norm': (_I, [_P, _P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),
 }
 

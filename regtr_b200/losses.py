@@ -120,6 +120,12 @@ def compute_loss(model, pred: Dict, batch: Dict) -> Dict[str, torch.Tensor]:
     return losses
 
 
+def loss_keys(cfg) -> List[str]:
+    """The keys of `compute_loss_device`'s result in order (`ops.LossGeometry.keys` and 'total')."""
+    return [f'overlap_{i}' for i in cfg.overlap_loss_on] + [f'feature_{i}' for i in cfg.feature_loss_on] + \
+        ['feature_un'] + [f'corr_{i}' for i in cfg.corr_loss_on] + ['total']
+
+
 _weight_vectors = {}
 
 
@@ -147,11 +153,15 @@ def device_route(model, pred, batch) -> bool:
             len(meta['_lens'][-1]) >= 2 and all(p is not None for p in meta['_pools32'][:len(meta['_points']) - 1]))
 
 
-def compute_loss_device(model, pred, batch) -> Dict[str, torch.Tensor]:
+def compute_loss_device(model, pred, batch, reduce_norms=None) -> Dict[str, torch.Tensor]:
     """`compute_loss` on the library's loss kernels (csrc/loss.cu), for a `pred` that `device_route` accepts: same
     keys in the same order, same total.  Reads the packed tensors `pred.core`, not the per-cloud views; the number of
     launches does not depend on the number of pairs and nothing synchronises with the host.  Fills
-    batch['overlap_pyr'] like `compute_loss`."""
+    batch['overlap_pyr'] like `compute_loss`.
+
+    reduce_norms: for a batch that is a slice of a larger one (data parallelism), a callable that sums the (4,) fp64
+    normaliser vector of `ops.loss_norms` in place over every slice (an all-reduce); the values and their gradients
+    are then this slice's share of the whole batch's losses, and the shares add up to them."""
     from . import ops
     from .kpconv import _meta_private
     cfg, core = model.cfg, pred.core
@@ -166,6 +176,9 @@ def compute_loss_device(model, pred, batch) -> Dict[str, torch.Tensor]:
     pose = pose[..., :3, :].to(device=dev, dtype=torch.float32).contiguous()
     geo = ops.LossGeometry(core['xyz_c'], meta['_offs'][-1], meta['_lens'][-1], pose, pyr[-1], cfg.overlap_loss_on,
                            cfg.feature_loss_on, cfg.corr_loss_on, cfg.r_p, cfg.r_n)
+    if reduce_norms is not None:
+        geo.norm = ops.loss_norms(geo)
+        reduce_norms(geo.norm)
     vals = ops.loss_values(core['both_un'], core['cond'], core['corr'], core['logit'], model.feature_criterion.W,
                            model.feature_criterion_un.W, geo)
     keys = geo.keys()

@@ -309,7 +309,9 @@ class ModelNetPrep:
     source's and of the target's crop direction, the three Euler draws and the translation (U[-trans_mag,
     trans_mag] = -trans_mag + 2 trans_mag u); the float32 transform and pose come from `euler_transform`, the
     restatement's own expressions.  The subset, its order and the jitter are drawn on the device from (seed, step,
-    pair, side, raw index).  `step` counts the calls unless given.  The status word of every call is checked
+    pair, side, raw index).  `step` counts the calls unless given.  pair_base: the position of the first pair in the
+    global batch when `items` is a slice of it (data parallelism): pair b draws what pair pair_base + b of the whole
+    batch draws.  The status word of every call is checked
     asynchronously at the next call, when the correspondences are read, or by `check()`."""
 
     def __init__(self, cfg, shapes: ModelNetShapes, seed: int = 0, noise: float = JITTER_SCALE,
@@ -349,10 +351,10 @@ class ModelNetPrep:
         """Wait for every earlier call and raise ValueError if one met bad input."""
         self._check_pending(block=True)
 
-    def draws(self, step: int, B: int) -> Dict[str, np.ndarray]:
-        """The host draws of a call: directions (B,2,3), euler (B,3) U[0,1), trans (B,3), transform and pose
-        (B,3,4) float32."""
-        u = np.stack([pair_draws(self.seed, step, b) for b in range(B)]) if B else np.zeros((0, N_UNIFORM))
+    def draws(self, step: int, B: int, pair_base: int = 0) -> Dict[str, np.ndarray]:
+        """The host draws of a call (pairs pair_base .. pair_base + B - 1): directions (B,2,3), euler (B,3) U[0,1),
+        trans (B,3), transform and pose (B,3,4) float32."""
+        u = np.stack([pair_draws(self.seed, step, pair_base + b) for b in range(B)]) if B else np.zeros((0, N_UNIFORM))
         dirs = np.stack([sphere_direction(2 * np.pi * u[:, 2 * s], -1.0 + 2.0 * u[:, 2 * s + 1]) for s in (0, 1)],
                         axis=1)
         trans = -self.trans_mag + (2 * self.trans_mag) * u[:, 7:10]
@@ -360,7 +362,7 @@ class ModelNetPrep:
         return dict(uniforms=u, directions=dirs, euler=u[:, 4:7], trans=trans,
                     transform=np.stack([m for m, _ in mats]), pose=np.stack([p for _, p in mats]))
 
-    def __call__(self, items, step: Optional[int] = None) -> LazyDict:
+    def __call__(self, items, step: Optional[int] = None, pair_base: int = 0) -> LazyDict:
         self._check_pending(block=False)
         if isinstance(items, dict):
             items = items['idx']
@@ -374,7 +376,7 @@ class ModelNetPrep:
             step = self.step
         self.step = step + 1
         dev = self.shapes.device_points.device
-        dr = self.draws(step, B)
+        dr = self.draws(step, B, pair_base)
 
         # the per-pair scalars, the pose and the items in one pinned buffer, one asynchronous copy
         dbl = np.concatenate([dr['directions'].reshape(B, 6), dr['transform'].reshape(B, 12).astype(np.float64)],
@@ -393,7 +395,7 @@ class ModelNetPrep:
         status = ops.new_status(dev)
         out_xyz, out_mask, corr, corr_n = ops.modelnet_augment(
             self.shapes.device_points, pdbl, items_d, self.seed, step, self.k, self.gamma, self.noise, self.clip,
-            RESAMPLE_POINTS, status)
+            RESAMPLE_POINTS, status, pair_base)
         word = torch.empty(1, dtype=torch.int32, pin_memory=True)
         word.copy_(status, non_blocking=True)
         ev = torch.cuda.Event()

@@ -1094,8 +1094,9 @@ def check_fit_status(status, radius: float):
 
 
 def train_augment(xyz, offs, B: int, n_src: int, pose, nn, pert, flags, seed: int, step: int, noise: float,
-                  max_pts: int, out_offs, out_total: int):
-    """The augmentations of regtr_train_augment on the clouds / overlap of `overlap_nn`.
+                  max_pts: int, out_offs, out_total: int, pair_base: int = 0):
+    """The augmentations of regtr_train_augment_at on the clouds / overlap of `overlap_nn`; the device draws of pair b
+    are keyed by pair_base + b.
     -> (out_xyz (out_total,3) f32, out_mask (out_total,) bool, out_pose (B,3,4) f32, corr (2, n_src) i32,
         corr_offs (B+1) i32).  No host sync."""
     L = _lib.load()
@@ -1109,11 +1110,11 @@ def train_augment(xyz, offs, B: int, n_src: int, pose, nn, pert, flags, seed: in
     corr_offs = torch.empty(B + 1, dtype=torch.int32, device=dev)
     ws = workspace(L.regtr_train_augment_ws_bytes(n_src, B), dev)
     state = workspace(L.regtr_train_augment_state_bytes(n_src), dev, 'scan_state', zero=True)
-    _lib.check(L.regtr_train_augment(_p(xyz), _p(offs), B, n_src, _p(pose), _p(nn), _p(pert), _p(flags),
-                                     int(seed) & (2**64 - 1), int(step) & (2**64 - 1), float(noise), int(max_pts),
-                                     _p(out_offs), out_total, _p(out_xyz), _p(out_mask), _p(out_pose), _p(corr),
-                                     corr.shape[1], _p(corr_offs), _p(ws), ws.numel(), _p(state), state.numel(),
-                                     _stream()), 'regtr_train_augment')
+    _lib.check(L.regtr_train_augment_at(_p(xyz), _p(offs), B, n_src, _p(pose), _p(nn), _p(pert), _p(flags),
+                                        int(seed) & (2**64 - 1), int(step) & (2**64 - 1), int(pair_base), float(noise),
+                                        int(max_pts), _p(out_offs), out_total, _p(out_xyz), _p(out_mask), _p(out_pose),
+                                        _p(corr), corr.shape[1], _p(corr_offs), _p(ws), ws.numel(), _p(state),
+                                        state.numel(), _stream()), 'regtr_train_augment_at')
     _count(5 if out_total > 0 else 4)
     return out_xyz, out_mask, out_pose, corr, corr_offs
 
@@ -1195,11 +1196,11 @@ assert MODELNET_ARGS.itemsize == 128                                      # the 
 
 
 def modelnet_augment(shapes, params, items, seed: int, step: int, k: int, gamma: float, noise: float, clip: float,
-                     n_out: int, status):
+                     n_out: int, status, pair_base: int = 0):
     """The ModelNet crop chain of B pairs (regtr_modelnet_augment): shapes (S, n_pts, 3) fp32; params
     (B, MODELNET_PARAMS) fp64 = crop direction of the source, of the target, the source's 3x4 transform; items (B)
     int32 shape indices.  -> (out_xyz (2B, n_out, 3) f32, out_mask (2B, n_out) bool, corr (B, 2, n_out) i32,
-    corr_n (B,) i32).  One launch, no host sync."""
+    corr_n (B,) i32).  The device draws of pair b are keyed by pair_base + b.  One launch, no host sync."""
     L = _lib.load()
     _chk(shapes, torch.float32, 'shapes', 3); _chk(params, torch.float64, 'params', 2); _chk(items, torch.int32, 'items', 1)
     _chk(status, torch.int32, 'status', 1)
@@ -1218,7 +1219,7 @@ def modelnet_augment(shapes, params, items, seed: int, step: int, k: int, gamma:
     a['seed'], a['step'] = int(seed) & (2**64 - 1), int(step) & (2**64 - 1)
     a['gamma'], a['noise'], a['clip'] = float(gamma), float(noise), float(clip)
     a['n_shapes'], a['n_pts'], a['n_out'], a['k'], a['B'] = shapes.shape[0], shapes.shape[1], int(n_out), int(k), B
-    _lib.check(L.regtr_modelnet_augment(a.ctypes.data, _stream()), 'regtr_modelnet_augment')
+    _lib.check(L.regtr_modelnet_augment_at(a.ctypes.data, int(pair_base), _stream()), 'regtr_modelnet_augment_at')
     _count(1)
     return out_xyz, out_mask, corr, corr_n
 
@@ -1292,10 +1293,13 @@ def sym_weight_bwd(dWs, dW):
 class LossGeometry:
     """What the device loss reads besides the predictions: xyz (N, 3) coarse key points (source clouds, then target
     clouds), offs (2B + 1) int32 device offsets and lens, the same lengths on the host, pose (B, 3, 4) fp32 ground
-    truth, w (N) coarsest ground-truth overlap, the layers each loss is applied to, and the InfoNCE radii."""
+    truth, w (N) coarsest ground-truth overlap, the layers each loss is applied to, and the InfoNCE radii.
+    norm: None, or the (4,) fp64 device normalisers of the whole batch (`loss_norms` summed over the ranks that each
+    hold a slice of it): the values and gradients are then this slice's share of the batch's."""
 
-    def __init__(self, xyz, offs, lens, pose, w, overlap_on, feature_on, corr_on, r_p: float, r_n: float):
+    def __init__(self, xyz, offs, lens, pose, w, overlap_on, feature_on, corr_on, r_p: float, r_n: float, norm=None):
         self.xyz, self.offs, self.lens, self.pose, self.w = xyz, offs, [int(v) for v in lens], pose, w
+        self.norm = None if norm is None else _chk(norm, torch.float64, 'norm', 1)
         self.B = len(self.lens) // 2
         self.overlap_on, self.feature_on, self.corr_on = list(overlap_on), list(feature_on), list(corr_on)
         self.r_p, self.r_n = float(r_p), float(r_n)
@@ -1304,6 +1308,21 @@ class LossGeometry:
         """The loss names in the order of the values vector (the reference's insertion order)."""
         return [f'overlap_{i}' for i in self.overlap_on] + [f'feature_{i}' for i in self.feature_on] + \
             ['feature_un'] + [f'corr_{i}' for i in self.corr_on]
+
+
+def loss_norms(geo: LossGeometry):
+    """(4,) fp64 device vector of this batch's loss normalisers (regtr_loss_norms): token count, sum of the
+    coarsest overlap over the source and over the target tokens, pair count.  One launch, no host sync."""
+    L = _lib.load()
+    w, offs = _chk(geo.w, torch.float32, 'w', 1), _chk(geo.offs, torch.int32, 'offs', 1)
+    if sum(geo.lens) != w.shape[0] or offs.shape[0] != 2 * geo.B + 1 or geo.B < 1:
+        raise ValueError('loss_norms: inconsistent shapes')
+    out = torch.empty(4, dtype=torch.float64, device=w.device)
+    a = np.zeros((), LOSS_ARGS)
+    a['w'], a['offs'], a['N'], a['B'] = w.data_ptr(), offs.data_ptr(), w.shape[0], geo.B
+    _lib.check(L.regtr_loss_norms(a.ctypes.data, out.data_ptr(), _stream()), 'regtr_loss_norms')
+    _count(1)
+    return out
 
 
 def loss_forward(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
@@ -1362,10 +1381,16 @@ def loss_forward(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
         a['term_val'][t] = keys.index(f'feature_{l}' if l >= 0 else 'feature_un')
     st['args'], st['hold'] = a, (xyz, offs, pose, w, logit, corr)
     s = _stream()
-    _lib.check(L.regtr_loss_pointwise(a.ctypes.data, s), 'regtr_loss_pointwise')
+    if geo.norm is None:
+        _lib.check(L.regtr_loss_pointwise(a.ctypes.data, s), 'regtr_loss_pointwise')
+    else:
+        _lib.check(L.regtr_loss_pointwise_norm(a.ctypes.data, geo.norm.data_ptr(), s), 'regtr_loss_pointwise_norm')
     _lib.check(L.regtr_infonce_match(a.ctypes.data, s), 'regtr_infonce_match')
     _lib.check(L.regtr_infonce_fwd(a.ctypes.data, s), 'regtr_infonce_fwd')
-    _lib.check(L.regtr_loss_finalize(a.ctypes.data, s), 'regtr_loss_finalize')
+    if geo.norm is None:
+        _lib.check(L.regtr_loss_finalize(a.ctypes.data, s), 'regtr_loss_finalize')
+    else:
+        _lib.check(L.regtr_loss_finalize_norm(a.ctypes.data, geo.norm.data_ptr(), s), 'regtr_loss_finalize_norm')
     _count(int(N > 0 and nl > 0) + 2 * int(a['max_src'] > 0) + 1)
     return st
 
@@ -1389,7 +1414,11 @@ def loss_backward(st, g):
         a['dq'][t], a['dfeat'][t] = dq[t].data_ptr(), dfeat[t].data_ptr()
     s = _stream()
     _lib.check(L.regtr_loss_pointwise_bwd(a.ctypes.data, s), 'regtr_loss_pointwise_bwd')
-    _lib.check(L.regtr_infonce_bwd(a.ctypes.data, s), 'regtr_infonce_bwd')
+    norm = st['geo'].norm
+    if norm is None:
+        _lib.check(L.regtr_infonce_bwd(a.ctypes.data, s), 'regtr_infonce_bwd')
+    else:
+        _lib.check(L.regtr_infonce_bwd_norm(a.ctypes.data, norm.data_ptr(), s), 'regtr_infonce_bwd_norm')
     _count(int(N > 0 and nl > 0) + int(a['max_src'] > 0) + int(a['max_tgt'] > 0))
     dW = [torch.zeros((LOSS_DIM, LOSS_DIM), **f32), torch.zeros((LOSS_DIM, LOSS_DIM), **f32)]
     if n_src:

@@ -10,6 +10,14 @@ relative to its working directory); the clouds are under cfg.root.  ModelNet40 r
 (this needs h5py) with the category files of the config, relative to the working directory as in the reference.
 Logs, config.yaml, tensorboard summaries and ckpt/ go to <logdir>/<dataset>/<yymmdd_HHMMSS>[_<name>].  With --resume and no --config, the config.yaml next to the
 checkpoint directory is used.  The reference's --dev flag (which deletes a log directory) is not provided.
+
+Data-parallel training on W GPUs of one machine (the batch size of the config stays the global batch):
+
+    torchrun --standalone --nproc_per_node=W -m regtr_b200.train --config 3dmatch
+
+reads RANK, WORLD_SIZE and LOCAL_RANK, runs one rank per GPU over NCCL (process-group timeout
+dist.DEFAULT_TIMEOUT_S), and lets rank 0 alone create the log directory, write config.yaml, summaries and
+checkpoints; every rank loads --resume.
 """
 from __future__ import annotations
 
@@ -17,7 +25,7 @@ import argparse
 import logging
 import os
 import sys
-from datetime import datetime
+from datetime import datetime, timedelta
 
 BUILTIN = ('3dmatch', 'modelnet')
 
@@ -93,8 +101,36 @@ def write_config(cfg, source: str, out: str):
             yaml.safe_dump({'config': dict(cfg)}, fid, sort_keys=False)
 
 
+def init_distributed(environ=None):
+    """The NCCL process group of a torchrun launch with WORLD_SIZE > 1 (this rank's GPU made current), else None."""
+    import torch
+    import torch.distributed as dist
+
+    from .dist import DEFAULT_TIMEOUT_S, torchrun_env
+    env = torchrun_env(environ)
+    if env is None or env[1] == 1:
+        return None
+    rank, world, local = env
+    torch.cuda.set_device(local)
+    dist.init_process_group('nccl', rank=rank, world_size=world, timeout=timedelta(seconds=DEFAULT_TIMEOUT_S),
+                            device_id=torch.device('cuda', local))
+    return dist.group.WORLD
+
+
 def main(argv=None):
     opt = parser().parse_args(argv)
+    group = init_distributed()
+    try:
+        return _main(opt, group)
+    finally:
+        if group is not None:
+            import torch.distributed as dist
+            dist.destroy_process_group()
+
+
+def _main(opt, group):
+    from .dist import broadcast_string, group_rank_world
+    rank, _ = group_rank_world(group)
     opt.config = resolve_config(opt)
     cfg = load_cfg(opt.config)
     if cfg.dataset == 'modelnet':
@@ -105,8 +141,13 @@ def main(argv=None):
     opt.logdir = os.path.join(opt.logdir, cfg.dataset)
     if opt.name is None and len(cfg.get('expt_name', '')) > 0:
         opt.name = cfg.expt_name
-    opt.log_path = prepare_logger(opt)
-    write_config(cfg, opt.config, os.path.join(opt.log_path, 'config.yaml'))
+    if rank == 0:
+        opt.log_path = prepare_logger(opt)
+        write_config(cfg, opt.config, os.path.join(opt.log_path, 'config.yaml'))
+    else:
+        logging.basicConfig(level=logging.WARNING)
+    if group is not None:
+        opt.log_path = broadcast_string(opt.log_path if rank == 0 else None, group)
 
     from .data import ThreeDMatchPairs
     from .regtr import RegTR
@@ -122,7 +163,7 @@ def main(argv=None):
         train_set = ThreeDMatchPairs(cfg.root, os.path.join(opt.info_dir, 'train_info.pkl'), pin=True, float64=True)
         val_set = ThreeDMatchPairs(cfg.root, os.path.join(opt.info_dir, 'val_info.pkl'), pin=True, float64=True)
     model = RegTR(cfg)
-    trainer = Trainer(opt, niter=cfg.niter, grad_clip=cfg.grad_clip, seed=opt.seed)
+    trainer = Trainer(opt, niter=cfg.niter, grad_clip=cfg.grad_clip, seed=opt.seed, process_group=group)
     trainer.fit(model, train_set, val_set)
     return opt.log_path
 

@@ -22,6 +22,16 @@ Differences from the reference, on purpose:
   * the warning for a non-finite total is logged when the meters are read back, not during the step;
   * the progress bar's loss is updated at summaries, not every step;
   * validation losses are the meters' means (fp64 sums), not the fp32 torch.mean of the stacked values.
+
+Data parallelism (`process_group` of world size W > 1): train_batch_size stays the global batch and every rank walks
+the same epoch order; rank r takes the slice `dist.shard_range(B, r, W)` of each batch and prepares it with its global
+pair offset, so it draws the augmentations those pairs draw on one GPU.  The loss is normalised over the whole batch
+(one all-reduce of four normalisers), each rank back-propagates its share, and one all-reduce of a flat gradient
+bucket that also carries the loss values and a failure flag gives every rank the batch's gradient and losses; the
+clipping, AdamW and StepLR steps then run unchanged and leave the weights bit-identical on every rank.  A rank whose
+step raises still joins both collectives with zeros and its flag, and every rank skips that update.  Validation shards
+its batches the same way and sums the per-batch losses, pose accumulators and histories over the ranks.  Rank 0 alone
+writes summaries and checkpoints; every rank loads on resume.
 """
 from __future__ import annotations
 
@@ -36,6 +46,7 @@ from typing import Dict, List, Optional
 import numpy as np
 import torch
 
+from . import dist as D
 from . import ops
 
 LOG_CAPACITY = 1024           # non-finite totals remembered between two read-backs
@@ -238,18 +249,29 @@ class Trainer:
     """`Trainer(opt, niter, grad_clip, seed).fit(model, train_set, val_set)`: the reference's training loop for a
     `RegTR` on `ThreeDMatchPairs(float64=True, pin=True)` datasets.  `opt` carries the reference's command-line
     options: log_path, resume, debug, summary_every, validate_every, nb_sanity_val_steps, num_workers.  The batch
-    sizes, augmentation and validation thresholds come from `model.cfg`.  Needs a CUDA device."""
+    sizes, augmentation and validation thresholds come from `model.cfg`.  Needs a CUDA device.
 
-    def __init__(self, opt, niter: int, grad_clip: float = 0.0, seed: int = 0):
+    process_group: a torch.distributed group of W ranks (one per GPU) for data-parallel training (module docstring);
+    None or W = 1 is the single-GPU loop.  Only rank 0 writes summaries and checkpoints."""
+
+    def __init__(self, opt, niter: int, grad_clip: float = 0.0, seed: int = 0, process_group=None):
         self.logger = logging.getLogger(__name__)
         self.opt = opt
         self.niter = int(niter)
         self.grad_clip = float(grad_clip)
         self.seed = int(seed)
         self.log_path = opt.log_path
-        self.train_writer, self.val_writer = _summary_writers(self.log_path)
-        self.saver = CheckpointManager(os.path.join(self.log_path, 'ckpt', 'model'), max_to_keep=6,
-                                       keep_checkpoint_every_n_hours=3.0)
+        self.rank, self.world = D.group_rank_world(process_group)
+        self.group = process_group if self.world > 1 else None
+        if self.rank == 0:
+            self.train_writer, self.val_writer = _summary_writers(self.log_path)
+            self.saver = CheckpointManager(os.path.join(self.log_path, 'ckpt', 'model'), max_to_keep=6,
+                                           keep_checkpoint_every_n_hours=3.0)
+        else:
+            self.train_writer = self.val_writer = None
+            self.saver = CheckpointManager(None)
+        self._bucket = None
+        self._norms_joined = False
         self.prep = None
         self.epoch_meter = self.summary_meter = None
         self._smooth = self._log = None
@@ -280,6 +302,11 @@ class Trainer:
             bs = int(model.cfg.train_batch_size)
             self._trainer_info = dict(seed=self.seed, steps_per_epoch=steps_per_epoch(len(train_set), bs),
                                       batch_size=bs, dataset_len=len(train_set))
+        if self.group is not None:
+            from .losses import loss_keys
+            D.check_batch_size(int(model.cfg.train_batch_size), self.world)
+            D.broadcast_tensors(list(model.parameters()) + list(model.buffers()), self.group)
+            self._bucket = D.GradBucket(list(model.parameters()), len(loss_keys(model.cfg)))
 
     def training_step(self, model, batch, global_step: int):
         """Step `global_step` (counted from 1) on a collated batch: TrainingPrep at step global_step - 1,
@@ -303,14 +330,74 @@ class Trainer:
             self._batch_info[global_step] = (b['idx'] if 'idx' in b else None, b.get('src_path'), b.get('tgt_path'))
             self._update_meters(losses, global_step)
         except Exception as inst:
-            _, _, tb = sys.exc_info()
-            while tb.tb_next is not None:
-                tb = tb.tb_next
-            fname = os.path.split(tb.tb_frame.f_code.co_filename)[1]
-            self.logger.error(f'{type(inst)} at {fname}:{tb.tb_lineno} - {inst}\n'
-                              f'Instance {batch.get("idx")}, src_path: {batch.get("src_path")}, '
-                              f'tgt_path: {batch.get("tgt_path")}')
-            self.logger.debug(traceback.format_exc())
+            self._log_failure(inst, batch)
+        return losses
+
+    # ------------------------------------------------------------------------------------------ data parallel
+    def _reduce_norms(self, norm: torch.Tensor):
+        torch.distributed.all_reduce(norm, op=torch.distributed.ReduceOp.SUM, group=self.group)
+        self._norms_joined = True
+
+    def _local_losses(self, model, pred, b):
+        """This rank's share of the batch losses (the loss kernels with batch-global normalisers)."""
+        from . import losses as LS
+        if not LS.device_route(model, pred, b):
+            raise RuntimeError('data-parallel training needs the loss kernels (losses.compute_loss_device); this '
+                               'prediction does not carry the packed CUDA tensors they read')
+        return LS.compute_loss_device(model, pred, b, reduce_norms=self._reduce_norms)
+
+    def _join_norms(self, device):
+        """Contribute zeros to this step's normaliser all-reduce if this rank has not joined it."""
+        if not self._norms_joined:
+            self._reduce_norms(torch.zeros(4, dtype=torch.float64, device=device))
+
+    def _log_failure(self, inst, batch):
+        _, _, tb = sys.exc_info()
+        while tb.tb_next is not None:
+            tb = tb.tb_next
+        fname = os.path.split(tb.tb_frame.f_code.co_filename)[1]
+        batch = batch or {}
+        self.logger.error(f'{type(inst)} at {fname}:{tb.tb_lineno} - {inst}\n'
+                          f'Instance {batch.get("idx")}, src_path: {batch.get("src_path")}, '
+                          f'tgt_path: {batch.get("tgt_path")}')
+        self.logger.debug(traceback.format_exc())
+
+    def dp_training_step(self, model, batch, pair_base: int, global_step: int):
+        """training_step of one rank under data parallelism: `batch` is this rank's slice of the global batch (None
+        when the slice is empty), starting at global pair `pair_base`.  Every rank calls it for every step, in
+        lockstep: it joins the normaliser and the gradient all-reduces whatever happens locally.  Returns the batch
+        losses (summed over the ranks) or None when the step was skipped on every rank."""
+        from .losses import loss_keys
+        self.prep.step = global_step - 1
+        self._norms_joined = False
+        keys = loss_keys(model.cfg)
+        vals, failed = None, False
+        try:
+            model.optimizer.zero_grad()
+            if batch is not None:
+                b = self.prep(batch, pair_base=pair_base)
+                pred = model.forward_train(b, train_encoder=True)
+                losses = self._local_losses(model, pred, b)
+                if losses['total'].requires_grad:
+                    losses['total'].backward()
+                vals = [losses[k].detach() for k in keys]
+                self._batch_info[global_step] = (b['idx'] if 'idx' in b else None, b.get('src_path'),
+                                                 b.get('tgt_path'))
+        except Exception as inst:
+            self._log_failure(inst, batch)
+            failed = True
+        self._join_norms(self.device)
+        total = self._bucket.exchange(vals, failed, self.group)
+        if total is None:
+            self.logger.warning(f'Step {global_step} failed on at least one rank: the update is skipped on every rank')
+            return None
+        if self.grad_clip > 0:
+            from .optim import clip_grad_norm_
+            clip_grad_norm_(model.parameters(), max_norm=self.grad_clip)
+        model.optimizer.step()
+        model.scheduler.step()
+        losses = {k: total[j:j + 1].view(()) for j, k in enumerate(keys)}
+        self._update_meters(losses, global_step)
         return losses
 
     def _update_meters(self, losses, global_step: int):
@@ -409,26 +496,32 @@ class Trainer:
                 batches = epoch_batches(self.seed, epoch, n, bs)
                 self.logger.info('Starting epoch {} (steps {} - {})'.format(epoch, global_step,
                                                                             global_step + len(batches) - skip))
-                tbar = tqdm(total=len(batches), initial=skip, ncols=80, smoothing=0)
+                tbar = tqdm(total=len(batches), initial=skip, ncols=80, smoothing=0, disable=self.rank != 0)
                 model.train()
                 torch.set_grad_enabled(True)
                 t_epoch = time.perf_counter()
-                if model.cfg.get('dataset') == 'modelnet':
+                if self.group is not None:
+                    stream = self._local_stream(model, train_set, batches[skip:], opt.num_workers)
+                elif model.cfg.get('dataset') == 'modelnet':
                     stream = ({'idx': bt} for bt in batches[skip:])
                 else:
                     stream = iter(PairStream(train_set, batches[skip:], workers=opt.num_workers))
                 try:
                     for batch_idx, batch in enumerate(stream, start=skip):
                         global_step += 1
-                        self.training_step(model, batch, global_step)
+                        if self.group is not None:
+                            self.dp_training_step(model, batch[0], batch[1], global_step)
+                        else:
+                            self.training_step(model, batch, global_step)
                         tbar.update(1)
                         if global_step == first_step + 1 or global_step % opt.summary_every == 0:
                             self._train_summary(model, global_step, tbar)
                         if global_step % opt.validate_every == 0:
-                            desc = tbar.desc
+                            desc = getattr(tbar, 'desc', '')         # a disabled bar has none
                             tbar.close()
                             self._run_validation(model, val_set, step=global_step)
-                            tbar = tqdm(total=len(batches), ncols=80, initial=batch_idx + 1, desc=desc[:-2])
+                            tbar = tqdm(total=len(batches), ncols=80, initial=batch_idx + 1, desc=desc[:-2],
+                                        disable=self.rank != 0)
                         if global_step - first_step >= total_iter:
                             done = True
                             break
@@ -446,6 +539,21 @@ class Trainer:
             self.logger.info('Ending training. Number of training steps = {}'.format(global_step))
         finally:
             self.close()
+
+    def _local_stream(self, model, dataset, batches, workers: int):
+        """(this rank's slice of each global batch or None when it is empty, the slice's first global pair)."""
+        from .data import PairStream
+        slices = [shard_slice(bt, self.rank, self.world) for bt in batches]
+        if model.cfg.get('dataset') == 'modelnet':
+            for lo, part in slices:
+                yield ({'idx': part} if part else None), lo
+            return
+        inner = iter(PairStream(dataset, [part for _, part in slices if part], workers=workers))
+        try:
+            for lo, part in slices:
+                yield (next(inner) if part else None), lo
+        finally:
+            inner.close()
 
     def close(self):
         """Flush and close the summary writers."""
@@ -470,6 +578,8 @@ class Trainer:
         else:
             self.logger.info(f'Running validation (step {step})...')
         n_pairs = sum(len(b) for b in batches)
+        if self.group is not None:
+            return self._run_validation_dp(model, val_set, batches, n_pairs, step, save_ckpt)
         model.eval()
         if cfg.get('dataset') == 'modelnet':          # deterministic pairs, already prepared
             prep, stream = None, (val_set.collate(bt, self.device) for bt in batches)
@@ -497,6 +607,9 @@ class Trainer:
         metrics = pose_metrics(acc, hist[:, :, :offset]) if acc is not None else {}
         if metrics:
             self.logger.info(f'Aggregating metrics, total number of instances: {offset}')
+        return self._finish_validation(model, step, val_losses, metrics, save_ckpt)
+
+    def _finish_validation(self, model, step, val_losses, metrics, save_ckpt):
         score = metrics.get('reg_success_final', 0.0)
         self._write_scalars(self.val_writer, model, step, losses=val_losses, metrics=metrics)
         if self.val_writer is not None:
@@ -505,11 +618,71 @@ class Trainer:
                     self.val_writer.add_histogram(f'metrics/{k}', v, step)
         log_str = ['Validation ended:', metrics_to_string(val_losses, '[Losses]'), metrics_to_string(metrics, '[Metrics]')]
         self.logger.info('\n'.join(log_str))
-        if save_ckpt:
+        if save_ckpt and self.rank == 0:
             self.saver.save(model, step, score, optimizer=model.optimizer, scheduler=model.scheduler,
                             trainer=dict(self._trainer_info))
         model.train()
         return score
+
+    def _run_validation_dp(self, model, val_set, batches, n_pairs: int, step: int, save_ckpt: bool):
+        """_run_validation on this rank's slice of every validation batch: the per-batch losses are summed over the
+        ranks before they reach the meters, and each rank writes the pose errors of its pairs at their global
+        positions, so one all-reduce of the accumulators and histories at the end gives every rank the single-GPU
+        metrics."""
+        from .augment import TrainingPrep
+        from .data import PairStream
+        from .losses import loss_keys
+        cfg, dev = model.cfg, self.device
+        keys = loss_keys(cfg)
+        nl = int(cfg.num_encoder_layers)
+        meter = DeviceMeters(keys, dev)
+        hist = torch.zeros((2, nl, max(n_pairs, 1)), dtype=torch.float64, device=dev)
+        acc = torch.zeros((nl, 4), dtype=torch.float64, device=dev)
+        slices = [shard_slice(bt, self.rank, self.world) for bt in batches]
+        modelnet = cfg.get('dataset') == 'modelnet'
+        prep = None if modelnet else TrainingPrep(cfg, seed=self.seed)
+        stream = None if modelnet else iter(PairStream(val_set, [p for _, p in slices if p],
+                                                       workers=self.opt.num_workers))
+        model.eval()
+        start = 0
+        try:
+            with torch.no_grad():
+                for (lo, part), bt in zip(slices, batches):
+                    self._norms_joined = False
+                    vals = torch.zeros(len(keys), dtype=torch.float32, device=dev)
+                    if part:
+                        batch = val_set.collate(part, dev) if modelnet else next(stream)
+                        b = batch if prep is None else prep(batch, augment=False)
+                        pred = model(b)
+                        losses = self._local_losses(model, pred, b)
+                        vals = torch.stack([losses[k].reshape(()) for k in keys])
+                        if pred['pose'].shape[0] != nl:
+                            raise RuntimeError(f'{pred["pose"].shape[0]} pose layers, expected {nl}')
+                        ops.pose_errors(pred['pose'].contiguous(), b['pose'].contiguous(), hist[0], hist[1], acc,
+                                        start + lo, cfg.reg_success_thresh_rot, cfg.reg_success_thresh_trans)
+                    self._join_norms(dev)
+                    torch.distributed.all_reduce(vals, op=torch.distributed.ReduceOp.SUM, group=self.group)
+                    ops.meter_update([vals[j:j + 1] for j in range(len(keys))], [meter.stats], step)
+                    meter.fed = True
+                    start += len(bt)
+            if prep is not None:
+                prep.check()
+        finally:
+            if stream is not None:
+                stream.close()
+        torch.distributed.all_reduce(acc, op=torch.distributed.ReduceOp.SUM, group=self.group)
+        torch.distributed.all_reduce(hist, op=torch.distributed.ReduceOp.SUM, group=self.group)
+        val_losses = meter.averages()
+        metrics = pose_metrics(acc, hist[:, :, :n_pairs]) if n_pairs else {}
+        if metrics:
+            self.logger.info(f'Aggregating metrics, total number of instances: {n_pairs}')
+        return self._finish_validation(model, step, val_losses, metrics, save_ckpt)
+
+
+def shard_slice(batch: List[int], rank: int, world: int):
+    """(first global pair, this rank's pairs) of one batch: `dist.shard_range` of its length."""
+    lo, hi = D.shard_range(len(batch), rank, world)
+    return lo, list(batch[lo:hi])
 
 
 def pose_metrics(acc: torch.Tensor, hist: torch.Tensor) -> Dict:
