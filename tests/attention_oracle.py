@@ -199,3 +199,33 @@ def report_invariants(title, rows):
         at = f'({w[1][0]}, {w[1][1]}, {w[2]})'
         print(f'  {name:{wn}s} {w[3] / max(w[5], 1e-300):11.3g}  {at:>24s} {w[3]:9.2e} {w[4]:9.2e}  '
               f'{len(failed(rs))}/{len(rs)}')
+
+
+def forward_reference(q, k, v, problems, n_heads, dtype):
+    """softmax(q k^T / sqrt(32)) v per head and problem in `dtype` on the CPU -> (O [n, E], base-2 lse [n, n_heads]);
+    rows outside every problem stay 0 / -inf."""
+    n, E = q.shape
+    q, k, v = (t.detach().cpu().to(dtype) for t in (q, k, v))
+    o = torch.zeros(n, E, dtype=dtype)
+    lse = torch.full((n, n_heads), -math.inf, dtype=dtype)
+    for qs, ql, ks, kl in problems:
+        if ql == 0 or kl == 0:
+            continue
+        s = _heads(q, qs, ql, n_heads) @ _heads(k, ks, kl, n_heads).transpose(1, 2) * SCALE
+        o[qs:qs + ql] = (torch.softmax(s, -1) @ _heads(v, ks, kl, n_heads)).transpose(0, 1).reshape(ql, E)
+        lse[qs:qs + ql] = (torch.logsumexp(s, -1) / math.log(2)).transpose(0, 1)
+    return o, lse
+
+
+def per_problem(name, problems, n_heads, hd, got, fp32, ref):
+    """Invariant rows (name, (q_len, k_len), head, kernel deviation, fp32 deviation, bound) of the [n, n_heads * hd]
+    tensors got / fp32 against ref over each problem's query rows; bound as in `invariants`."""
+    out = []
+    for qs, ql, ks, kl in problems:
+        if ql == 0 or kl == 0:
+            continue
+        r = ref[qs:qs + ql].double()
+        dg, df = ((t[qs:qs + ql].double() - r).view(ql, n_heads, hd).abs().amax(-1).amax(0) for t in (got, fp32))
+        bound = FACTOR * df + FLOOR * float(r.abs().max())
+        out += [(name, (ql, kl), h, float(dg[h]), float(df[h]), float(bound[h])) for h in range(n_heads)]
+    return out

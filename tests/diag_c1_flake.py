@@ -1,4 +1,6 @@
-"""Flake hunt for test_kpconv_all_channel_paths_vs_oracle[1-64-*]: which side varies on the first call of a process?"""
+"""Flake hunt for the Cin = 1, Cout = 64 KPConv comparison (random points near the origin, K = 40): which side varies
+on the first call of a process?  tests/test_gpu_forward_ops.py::test_kpconv_vs_float64 prints both sides' errors
+against float64 on every path."""
 import os, sys
 import numpy as np, torch
 HERE = os.path.dirname(os.path.abspath(__file__))

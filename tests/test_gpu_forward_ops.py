@@ -24,7 +24,7 @@ import pytest
 import torch
 
 import attention_oracle as ao
-from grad_yardstick import FACTOR, FLOOR, Yardstick
+from grad_yardstick import Yardstick
 
 pytestmark = pytest.mark.gpu
 
@@ -33,20 +33,6 @@ DEV = 'cuda:0'
 
 def _dev_tables(problems):
     return [torch.tensor(c, dtype=torch.int32, device=DEV) for c in zip(*problems)]
-
-
-def _per_problem(name, problems, n_heads, hd, got, fp32, ref):
-    """Invariant rows (name, (q_len, k_len), head, kernel deviation, fp32 deviation, bound) of the [n, n_heads * hd]
-    tensors got / fp32 against ref over each problem's query rows; bound as in attention_oracle.invariants."""
-    out = []
-    for qs, ql, ks, kl in problems:
-        if ql == 0 or kl == 0:
-            continue
-        r = ref[qs:qs + ql].double()
-        dg, df = ((t[qs:qs + ql].double() - r).view(ql, n_heads, hd).abs().amax(-1).amax(0) for t in (got, fp32))
-        bound = FACTOR * df + FLOOR * float(r.abs().max())
-        out += [(name, (ql, kl), h, float(dg[h]), float(df[h]), float(bound[h])) for h in range(n_heads)]
-    return out
 
 
 # ------------------------------------------------------------------------------------ InstanceNorm statistics
@@ -178,18 +164,7 @@ FWD_FAMILIES = [f for f in ao.FAMILIES if f != 'shared_do']    # shared_do chang
 
 
 def _attn_ref(q, k, v, problems, dtype):
-    """softmax(q k^T / sqrt(32)) v per head and problem in `dtype` on the CPU -> (O [n, E], base-2 lse [n, H])."""
-    n = q.shape[0]
-    q, k, v = (t.detach().cpu().to(dtype) for t in (q, k, v))
-    o = torch.zeros(n, E, dtype=dtype)
-    lse = torch.full((n, H), -math.inf, dtype=dtype)
-    for qs, ql, ks, kl in problems:
-        if ql == 0 or kl == 0:
-            continue
-        s = ao._heads(q, qs, ql, H) @ ao._heads(k, ks, kl, H).transpose(1, 2) * ao.SCALE
-        o[qs:qs + ql] = (torch.softmax(s, -1) @ ao._heads(v, ks, kl, H)).transpose(0, 1).reshape(ql, E)
-        lse[qs:qs + ql] = (torch.logsumexp(s, -1) / math.log(2)).transpose(0, 1)
-    return o, lse
+    return ao.forward_reference(q, k, v, problems, H, dtype)
 
 
 def _head_shift(x, problems, seed):
@@ -305,8 +280,8 @@ def _attn_checks(title, res, o=None, o_v=None):
             ys.add(f'{part} lse', res['lse'][rows], res['l32'][rows], res['l64'][rows])
     ys.report()
     cv = c['cv'].double()
-    inv = _per_problem('O(k + c) = O', problems, H, ao.HD, res['o_k'], res['k32'], res['r64'])
-    inv += _per_problem('O(v + c) = O + c', problems, H, ao.HD, o_v.double() - cv, res['v32'].double() - cv,
+    inv = ao.per_problem('O(k + c) = O', problems, H, ao.HD, res['o_k'], res['k32'], res['r64'])
+    inv += ao.per_problem('O(v + c) = O + c', problems, H, ao.HD, o_v.double() - cv, res['v32'].double() - cv,
                         res['r64'])
     ao.report_invariants(title, inv)
     return ys.failures(), ao.failed(inv)
@@ -404,8 +379,8 @@ def _corr_checks(title, c, got=None, got_t=None):
     ys.report()
     layered = [(l * n + qs, ql, l * n + ks, kl) for l in range(CORR_L) for qs, ql, ks, kl in _corr_problems()]
     t = c['t'].double()
-    inv = _per_problem('corr(xyz + t) = corr + t', layered, 1, 3, got_t.double() - t, c['t32'].double() - t, c['r64'])
-    inv += _per_problem('corr(kp + c) = corr', layered, 1, 3, c['got_k'], c['k32'], c['r64'])
+    inv = ao.per_problem('corr(xyz + t) = corr + t', layered, 1, 3, got_t.double() - t, c['t32'].double() - t, c['r64'])
+    inv += ao.per_problem('corr(kp + c) = corr', layered, 1, 3, c['got_k'], c['k32'], c['r64'])
     ao.report_invariants(title, inv)
     return ys.failures(), ao.failed(inv)
 
@@ -558,3 +533,310 @@ def test_pose_from_corr_layers_and_pairs_vs_float64():
             _pose_check(f'layer {l} pair {b}', pose[l, b], a, bb, w, True, table, fails)
     print('\npose_from_corr against float64 Kabsch (bound 1e-6)\n' + '\n'.join(table))
     assert not fails, fails
+
+
+# ------------------------------------------------------------------------------------------------------ KPConv
+
+KP_OFFSET = np.array(XYZ_OFFSET)
+KP_NQ, KP_EXTENT, KP_RADIUS = 301, 0.05, 0.0625         # the 3DMatch config's first level
+KP_PATHS = ([(1, 'fused'), (1, 'aggregate'), (4, 'default')] +
+            [(c, impl) for c in (32, 64, 128, 256) for impl in ('default', 'mma', 'ffma')])
+_KPC = {}
+
+
+def _kp_inputs(cin, K):
+    """Model-like KPConv inputs: queries ~2.5 m from the origin, per query its own support rows -- three at a kernel
+    point's extent (exactly, and 2 ulp inside / outside), the rest in the radius ball -- scattered over the K slots
+    with shadow slots (id == Ns) between them.  Feature rows: every 5th sums to exactly 0, every 7th is negative (both
+    uncounted: they move the divisor).  Query 7 has no valid neighbour, query 11 no counted one."""
+    rng = np.random.default_rng(100 * cin + K)
+    kp = np.zeros((15, 3))
+    d = rng.normal(size=(14, 3))
+    kp[1:] = d / np.linalg.norm(d, axis=1, keepdims=True) * rng.uniform(0.25, 0.65, (14, 1)) * KP_RADIUS
+    kp = kp.astype(np.float32)
+    ext = float(np.float32(KP_EXTENT))
+    q = (KP_OFFSET + rng.normal(size=(KP_NQ, 3)) * 0.4).astype(np.float32)
+    s_rows, idx = [], np.empty((KP_NQ, K), dtype=np.int64)
+    for i in range(KP_NQ):
+        n = 0 if i == 7 else int(rng.integers(1, K + 1)) if i % 3 else K
+        rel = rng.normal(size=(n, 3))
+        rel = rel / np.linalg.norm(rel, axis=1, keepdims=True) * KP_RADIUS * rng.uniform(0, 1, (n, 1)) ** (1 / 3)
+        for j, f in enumerate((1.0, 1 - 1e-5, 1 + 1e-5)[:n]):   # at, just inside, just outside kernel point j's extent
+            u = rng.normal(size=3)
+            rel[j] = kp[j + 3] + u / np.linalg.norm(u) * ext * f
+        slots = np.sort(rng.choice(K, size=n, replace=False))
+        idx[i] = -1
+        idx[i, slots] = len(s_rows) + np.arange(n)
+        s_rows.extend(q[i] + rel)
+    Ns = len(s_rows)
+    s = np.asarray(s_rows, dtype=np.float32)
+    idx[idx < 0] = Ns                                                    # shadow slots, also between real ones
+    x = (rng.normal(size=(Ns, cin)) * 0.8 + 0.3).astype(np.float32)
+    x[::7] = -np.abs(x[::7]) - 0.1
+    x[::5] = 0
+    if cin > 1:
+        c = rng.uniform(0.5, 2, size=len(x[::5])).astype(np.float32)
+        x[::5, 0], x[::5, 1] = c, -c
+    own = idx[11][idx[11] < Ns]
+    x[own] = -np.abs(x[own]) - 0.1
+    x[own[::2]] = 0
+    W = (rng.normal(size=(15, cin, 32 if cin == 4 else 64 if cin == 1 else cin)) / math.sqrt(15 * cin)).astype(np.float32)
+    return dict(q=q, s=s, idx=idx, x=x, W=W, kp=kp, extent=ext, Ns=Ns)
+
+
+def _kp_ref(c, dtype):
+    """(wf [Nq, 15 Cin], out [Nq, Cout]) of oracle.regtr_oracle.kpconv's operations in `dtype`, with the divisor of the
+    exact row sums (no fp32 rounding decides a count); wf is the influence-weighted sum already divided, as the
+    kernels store it."""
+    from oracle import regtr_oracle as O
+    q, s, x, W, kp = (torch.from_numpy(c[k]).to(dtype) for k in ('q', 's', 'x', 'W', 'kp'))
+    idx = torch.from_numpy(c['idx'])
+    count = O.kpconv_count(idx, torch.from_numpy(c['x']).double())
+    nb = torch.cat([s, torch.full_like(s[:1], 1e6)])[idx] - q[:, None]
+    d2 = ((nb[:, :, None] - kp) ** 2).sum(-1)
+    infl = torch.clamp(1 - torch.sqrt(d2) / c['extent'], min=0.0).transpose(1, 2)
+    wf = infl @ torch.cat([x, torch.zeros_like(x[:1])])[idx] / count[:, None, None].to(dtype)
+    out = O.kpconv(q, s, idx, x, W, kp, c['extent'], count=count)
+    return wf.reshape(len(q), -1), out
+
+
+def _kp_case(cin, impl, K, monkeypatch):
+    """GPU results of one path on _kp_inputs, exact-shaped and capacity-shaped, and the float64 / fp32 references."""
+    key = (cin, impl, K)
+    if key in _KPC:
+        return _KPC[key]
+    from regtr_b200 import ops
+    if impl in ('mma', 'ffma'):
+        monkeypatch.setenv('REGTR_AGG_IMPL', impl)
+    else:
+        monkeypatch.delenv('REGTR_AGG_IMPL', raising=False)
+    c = _kp_inputs(cin, K)
+    G = lambda a, dt=None: torch.from_numpy(np.ascontiguousarray(a)).to(DEV, dt)
+    q, s, idx, x, W, kp = G(c['q']), G(c['s']), G(c['idx'], torch.int32), G(c['x']), G(c['W']), G(c['kp'])
+    r = dict(ref=c)
+    if not (cin == 1 and impl == 'fused'):
+        r['wf'] = ops.kpconv_aggregate(q, s, idx, x, kp, c['extent']).cpu()
+        r['wf2'] = ops.kpconv_aggregate(q, s, idx, x, kp, c['extent']).cpu()
+    if impl != 'aggregate':
+        r['out'] = ops.kpconv(q, s, idx, x, W, kp, c['extent']).cpu()
+        r['out2'] = ops.kpconv(q, s, idx, x, W, kp, c['extent']).cpu()
+    if cin > 1 and impl != 'aggregate':            # the InstanceNorm-statistics GEMM epilogue, two clouds
+        lens = [180, KP_NQ - 180]
+        o, st = ops.kpconv(q, s, idx, x, W, kp, c['extent'], instats=(ops.make_offsets(lens, DEV), 2))
+        r['instats'] = (lens, o.cpu(), st.cpu())
+    # capacity form: garbage query / support / feature rows past nq_dev / ns_dev; the real rows' shadow id Ns is a
+    # garbage row of the capacity buffer and must still count as the shadow
+    g = np.random.default_rng(1)
+    pq, ps = 100, 20
+    qc = G(np.r_[c['q'], g.uniform(-1e3, 1e3, (pq, 3))].astype(np.float32))
+    sc = G(np.r_[c['s'], g.uniform(-1e3, 1e3, (ps, 3))].astype(np.float32))
+    xc = G(np.r_[c['x'], np.full((ps, cin), 1e3)].astype(np.float32))
+    ic = G(np.r_[c['idx'], g.integers(0, c['Ns'] + ps, (pq, K))], torch.int32)
+    nq_dev, ns_dev = (torch.tensor([v], dtype=torch.int32, device=DEV) for v in (KP_NQ, c['Ns']))
+    if not (cin == 1 and impl == 'fused'):
+        wf = torch.full((KP_NQ + pq, 15 * cin), math.nan, device=DEV)
+        ops.kpconv_aggregate(qc, sc, ic, xc, kp, c['extent'], wf=wf, nq_dev=nq_dev, ns_dev=ns_dev)
+        r['wf_cap'] = wf.cpu()
+    if impl != 'aggregate':
+        out = torch.full((KP_NQ + pq, W.shape[2]), math.nan, device=DEV)
+        ops.kpconv(qc, sc, ic, xc, W, kp, c['extent'], out=out, nq_dev=nq_dev, ns_dev=ns_dev)
+        r['out_cap'] = out.cpu()
+    torch.cuda.synchronize()
+    (r['wf64'], r['out64']), (r['wf32'], r['out32']) = _kp_ref(c, torch.float64), _kp_ref(c, torch.float32)
+    _KPC[key] = r
+    return r
+
+
+def _kp_rows(title, r, wf=None, out=None):
+    """Yardstick rows: wf (aggregation) and out, exact-shaped and capacity-shaped; mean / rstd / normalised output of
+    the statistics epilogue per cloud.  wf / out replace the kernel's (sharpness checks) -> Yardstick."""
+    from oracle import regtr_oracle as O
+    ys = Yardstick(title)
+    wf = r.get('wf') if wf is None else wf
+    out = r.get('out') if out is None else out
+    if wf is not None:
+        ys.add('wf', wf, r['wf32'], r['wf64'])
+        ys.add('wf, capacity form', r['wf_cap'][:KP_NQ], r['wf32'], r['wf64'])
+    if out is not None:
+        ys.add('out', out, r['out32'], r['out64'])
+        ys.add('out, capacity form', r['out_cap'][:KP_NQ], r['out32'], r['out64'])
+    if 'instats' in r:
+        lens, o, st = r['instats']
+        ys.add('out, statistics epilogue', o, r['out32'], r['out64'])
+        m64, s64 = _in_stats(r['out64'], lens, torch.float64)
+        m32, s32 = _in_stats(r['out32'], lens, torch.float32)
+        ys.add('  mean', st[..., 0], m32, m64)
+        ys.add('  rstd', st[..., 1], s32, s64)
+    ys.report()
+    return ys
+
+
+@pytest.mark.parametrize('K', [40, 50, 72])
+@pytest.mark.parametrize('cin,impl', KP_PATHS, ids=[f'{c}-{i}' for c, i in KP_PATHS])
+def test_kpconv_vs_float64(cin, impl, K, monkeypatch):
+    """Every KPConv dispatch path -- Cin = 1 fused (regtr_kpconv_fwd) and aggregate-only, the small-Cin kernel, Cin 32
+    to 256 through the default pipelined kernel (K <= 64; K = 72 falls through to the staged tensor-core kernel),
+    REGTR_AGG_IMPL=mma and ffma, and the statistics GEMM epilogue -- under the yardstick against float64, at K = 40
+    and 50 (the configs' limits) and 72.  Two calls are bit-identical; the capacity form's real rows equal the
+    exact-shaped call's aggregation bit for bit, and its padding rows up to the consumer GEMM's 128-row tile are 0."""
+    r = _kp_case(cin, impl, K, monkeypatch)
+    ys = _kp_rows(f'kpconv Cin={cin} {impl}, K={K}', r)
+    for a, b in (('wf', 'wf2'), ('out', 'out2')):
+        if a in r:
+            assert torch.equal(r[a], r[b]), f'{a} not bit-identical from call to call'
+    if 'wf' in r:
+        assert torch.equal(r['wf_cap'][:KP_NQ], r['wf']), 'capacity-form aggregation differs from the exact-shaped one'
+        band = (KP_NQ + 127) // 128 * 128
+        assert torch.equal(r['wf_cap'][KP_NQ:band], torch.zeros_like(r['wf_cap'][KP_NQ:band])), 'padding rows not 0'
+    if 'out' in r and cin == 1:
+        band = (KP_NQ + 127) // 128 * 128
+        assert torch.equal(r['out_cap'][KP_NQ:band], torch.zeros_like(r['out_cap'][KP_NQ:band])), 'padding rows not 0'
+    empty = r.get('out', r.get('wf'))[7]
+    assert float(empty.abs().max()) == 0.0, 'a query without valid neighbours must give 0'
+    assert not ys.failures(), ys.failures()
+
+
+def test_kpconv_checks_are_sharp(monkeypatch):
+    """wf or out multiplied by (1 + 1e-5) fails its row, on the fused Cin = 1 path and the default Cin = 64 path."""
+    for cin, impl in ((1, 'aggregate'), (1, 'fused'), (64, 'default')):
+        r = _kp_case(cin, impl, 40, monkeypatch)
+        if 'wf' in r:
+            assert 'wf' in _kp_rows(f'kpconv Cin={cin} {impl}, wf x (1 + 1e-5)', r, wf=r['wf'] * (1 + 1e-5)).failures()
+        if 'out' in r:
+            assert 'out' in _kp_rows(f'kpconv Cin={cin} {impl}, out x (1 + 1e-5)', r, out=r['out'] * (1 + 1e-5)).failures()
+
+
+# ---------------------------------------------------------------------------------------------------- max_pool
+
+@pytest.mark.parametrize('C', [128, 6], ids=['vector', 'scalar'])
+def test_max_pool_bit_exact(C):
+    """max_pool equals oracle.regtr_oracle.max_pool bit for bit: C % 4 != 0 takes the scalar kernel; queries whose
+    real neighbours are all negative take the zero shadow row when they have a shadow slot and their largest
+    negative value when they have none; a query of shadows only gives 0; the capacity form (ns_dev, the shadow id
+    pointing at a garbage row of the buffer) gives the same result."""
+    from oracle import regtr_oracle as O
+    from regtr_b200 import ops
+    rng = np.random.default_rng(C)
+    Nq, Ns, K = 500, 900, 40
+    x = rng.normal(size=(Ns, C)).astype(np.float32)
+    x[::3] = -np.abs(x[::3]) - 1e-3                                      # all-negative rows
+    idx = rng.integers(0, Ns, size=(Nq, K))
+    idx[:, 5:K:4] = np.where(rng.random((Nq, len(range(5, K, 4)))) < 0.5, Ns, idx[:, 5:K:4])   # shadows mid-row
+    neg = np.arange(0, Ns, 3)
+    idx[10:20] = rng.choice(neg, size=(10, K))                           # all negative, no shadow slot
+    idx[20:30] = rng.choice(neg, size=(10, K))
+    idx[20:30, 17] = Ns                                                  # all negative, one shadow slot
+    idx[30] = Ns
+    want = O.max_pool(torch.from_numpy(x), torch.from_numpy(idx))
+    assert float(want[10:20].max()) < 0 and float(want[20:31].abs().max()) == 0
+    G = lambda a, dt=None: torch.from_numpy(np.ascontiguousarray(a)).to(DEV, dt)
+    got = ops.max_pool(G(x), G(idx, torch.int32)).cpu()
+    xc = G(np.r_[x, np.full((50, C), 1e3, dtype=np.float32)])
+    got_cap = ops.max_pool(xc, G(idx, torch.int32), ns_dev=torch.tensor([Ns], dtype=torch.int32, device=DEV)).cpu()
+    assert torch.equal(got, want), int((got != want).sum())
+    assert torch.equal(got_cap, want), int((got_cap != want).sum())
+
+
+# ----------------------------------------------------------------------------------------------- layernorm_pos
+
+LN_E, LN_N = 256, 400
+
+
+def _ln_case():
+    """Rows of mean / std 0, 3, 30 and 300 (row r: RATIOS[r % 4]) with std from 1e-2 to 10, model-like gamma, beta
+    and position embedding."""
+    rng = np.random.default_rng(12)
+    sd = 10 ** rng.uniform(-2, 1, size=(LN_N, 1))
+    ratio = np.array(RATIOS)[np.arange(LN_N) % len(RATIOS)][:, None]
+    x = (rng.normal(size=(LN_N, LN_E)) + ratio * rng.choice([-1.0, 1.0], size=(LN_N, 1))) * sd
+    gamma = 1 + 0.2 * rng.normal(size=LN_E)
+    beta = 0.2 * rng.normal(size=LN_E)
+    pos = rng.uniform(-1, 1, size=(LN_N, LN_E))
+    return [torch.from_numpy(a.astype(np.float32)) for a in (x, gamma, beta, pos)]
+
+
+def _ln_rows(title, got, got_pos, x, gamma, beta, pos):
+    """Plain and +pos outputs per mean / std family, GPU against float64 and fp32 F.layer_norm."""
+    ys = Yardstick(title)
+    refs = {dt: torch.nn.functional.layer_norm(x.to(dt), (LN_E,), gamma.to(dt), beta.to(dt), 1e-5)
+            for dt in (torch.float64, torch.float32)}
+    fam = torch.arange(LN_N) % len(RATIOS)
+    for g, ratio in enumerate(RATIOS):
+        rows = torch.nonzero(fam == g).squeeze(1)
+        ys.add(f'mean/std {ratio:3d}: LN(x)', got[rows], refs[torch.float32][rows], refs[torch.float64][rows])
+        ys.add(f'mean/std {ratio:3d}: LN(x) + pos', got_pos[rows], refs[torch.float32][rows] + pos[rows],
+               refs[torch.float64][rows] + pos[rows].double())
+    ys.report()
+    return ys
+
+
+def test_layernorm_pos_vs_float64():
+    """layernorm_pos under the yardstick, plain and +pos, per mean / std family; the capacity form (n_dev, garbage
+    rows past it) gives the exact-shaped call's rows bit for bit."""
+    from regtr_b200 import ops
+    x, gamma, beta, pos = _ln_case()
+    D = lambda t: t.to(DEV)
+    y, yp = ops.layernorm_pos(D(x), D(gamma), D(beta), D(pos))
+    y, yp = y.cpu(), yp.cpu()
+    ys = _ln_rows(f'layernorm_pos, E = {LN_E}', y, yp, x, gamma, beta, pos)
+    xc = D(torch.cat([x, torch.full((60, LN_E), 1e3)]))
+    pc = D(torch.cat([pos, torch.full((60, LN_E), 1e3)]))
+    yc, ypc = ops.layernorm_pos(xc, D(gamma), D(beta), pc, n_dev=torch.tensor([LN_N], dtype=torch.int32, device=DEV))
+    assert torch.equal(yc[:LN_N].cpu(), y) and torch.equal(ypc[:LN_N].cpu(), yp), 'capacity form differs'
+    assert not ys.failures(), ys.failures()
+
+
+def test_layernorm_pos_checks_are_sharp():
+    """Outputs x (1 + 1e-5) fail the rows of mean / std 0 and 3.  At 30 and 300 the fp32 oracle itself is about 1.5e-6
+    and 1.2e-5 off float64 (the rounding of a mean 30 or 300 std from zero, carried into every output), so the
+    yardstick cannot tell a 1e-5 error from fp32 rounding there."""
+    from regtr_b200 import ops
+    x, gamma, beta, pos = _ln_case()
+    D = lambda t: t.to(DEV)
+    y, yp = (t.cpu() for t in ops.layernorm_pos(D(x), D(gamma), D(beta), D(pos)))
+    fails = set(_ln_rows('layernorm_pos, outputs x (1 + 1e-5)', y * (1 + 1e-5), yp * (1 + 1e-5), x, gamma, beta,
+                         pos).failures())
+    assert {f'mean/std {q:3d}: LN(x){p}' for q in RATIOS[:2] for p in ('', ' + pos')} <= fails, fails
+
+
+# ---------------------------------------------------------------------------------------------- pos_embed_sine
+
+def _pe_rows(title, got, xyz):
+    """The sine and the cosine columns against float64 of the same operation on the same fp32 coordinates and the
+    same fp32 frequency table (oracle.regtr_oracle.pos_embed_sine), and the fp32 oracle."""
+    from oracle import regtr_oracle as O
+    r64, r32 = O.pos_embed_sine(xyz.double()), O.pos_embed_sine(xyz)
+    ys = Yardstick(title)
+    n_freq = 256 // 3 // 2 * 2
+    cols = torch.arange(3 * n_freq)
+    for name, sel in (('sin', cols[(cols % n_freq) % 2 == 0]), ('cos', cols[(cols % n_freq) % 2 == 1])):
+        ys.add(name, got[:, sel], r32[:, sel], r64[:, sel])
+    ys.add('zero padding', got[:, 3 * n_freq:], r32[:, 3 * n_freq:], r64[:, 3 * n_freq:])
+    ys.report()
+    return ys
+
+
+def _pe_inputs(span):
+    rng = np.random.default_rng(int(span))
+    xyz = rng.uniform(-span, span, size=(3000, 3))
+    xyz[:8] = np.array([[span, -span, 0.0], [-span, span, 1e-7], [0, 0, 0], [span / 2, span / 3, -span / 7]] * 2)
+    return torch.from_numpy(xyz.astype(np.float32))
+
+
+@pytest.mark.parametrize('span', [5.0, 1.0], ids=['world_5m', 'modelnet_unit'])
+def test_pos_embed_sine_vs_float64(span):
+    """Coordinates up to +-5 m (arguments up to 10 pi) and the ModelNet unit range."""
+    from regtr_b200 import ops
+    xyz = _pe_inputs(span)
+    got = ops.pos_embed_sine(xyz.to(DEV)).cpu()
+    ys = _pe_rows(f'pos_embed_sine, coordinates in [-{span:g}, {span:g}]', got, xyz)
+    assert float(got[:, 3 * (256 // 3 // 2 * 2):].abs().max()) == 0.0
+    assert not ys.failures(), ys.failures()
+
+
+def test_pos_embed_sine_checks_are_sharp():
+    from regtr_b200 import ops
+    xyz = _pe_inputs(5.0)
+    got = ops.pos_embed_sine(xyz.to(DEV)).cpu()
+    fails = _pe_rows('pos_embed_sine, output x (1 + 1e-5)', got * (1 + 1e-5), xyz).failures()
+    assert {'sin', 'cos'} <= set(fails), fails

@@ -15,9 +15,6 @@ counts).  Then:
   * each attention core's recorded q, k, v, O, lse and output gradient are run through the core's backward alone and
     checked as tests/test_gpu_attention_backward.py checks synthetic inputs (tests/attention_oracle.py).
 """
-import inspect
-import os
-import sys
 import types
 
 import numpy as np
@@ -25,189 +22,14 @@ import pytest
 import torch
 
 import attention_oracle as ao
-from conftest import FORWARD_CASES, make_case
 from grad_yardstick import Yardstick, errors
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden'))
-import eval_inputs as ei  # noqa: E402
+from stage_oracle import (DEV, ENC, XENC, ei, flips as _flips, gpu_decisions as _gpu_decisions, leaves as _leaves,
+                          oracle_block as _oracle_block, oracle_layer as _oracle_layer, block_sites as _block_sites,
+                          train_run as _full_run, trainable as _trainable)
 
 pytestmark = pytest.mark.gpu
 
-DEV = 'cuda:0'
 CASES = ['fwd_3dmatch_small_b2', 'fwd_modelnet_b1']
-ENC = 'kpf_encoder.encoder_blocks.'
-XENC = 'transformer_encoder.layers.'
-_RECORDED_OPS = ('instnorm_act', 'instnorm_apply', 'max_pool', 'kpconv', 'linear_instats', 'linear', 'mha_varlen_lse')
-
-
-class _Tap(torch.autograd.Function):
-    """Identity that keeps a copy of the gradient flowing back through it in box[key]."""
-
-    @staticmethod
-    def forward(ctx, x, box, key):
-        ctx.box, ctx.key = box, key
-        return x.clone()
-
-    @staticmethod
-    def backward(ctx, g):
-        ctx.box[ctx.key] = g.clone()
-        return g, None, None
-
-
-def _record(model, mp):
-    """Wrap every encoder block's forward, every cross-encoder layer's forward_train_packed and the ops they call.
-    Per block / layer: 'x' (input), 'rest' (the other arguments), 'calls' [(op, arguments, result)], and after the
-    backward 'dout' (gradient at the output) and 'dx' (gradient the block sends to its input, if it needs one).
-    Every attention-core backward is kept in rec['mha_bwd'], keyed by the address of the O it was given: its dO and
-    copies of the dq, dk, dv it wrote."""
-    from regtr_b200 import ops
-    rec = dict(enc=[], xenc=[], cur=None, mha_bwd={})
-
-    def recording(name, fn):
-        sig = inspect.signature(fn)
-
-        def wrapped(*a, **k):
-            r = fn(*a, **k)
-            if rec['cur'] is not None:
-                bound = sig.bind(*a, **k)
-                bound.apply_defaults()
-                rec['cur'].append((name, dict(bound.arguments), r))
-            return r
-        return wrapped
-
-    for name in _RECORDED_OPS:
-        mp.setattr(ops, name, recording(name, getattr(ops, name)))
-    mha_bwd = ops.mha_varlen_bwd
-    bwd_sig = inspect.signature(mha_bwd)
-
-    def recording_bwd(*a, **k):
-        mha_bwd(*a, **k)
-        b = bwd_sig.bind(*a, **k).arguments
-        rec['mha_bwd'][b['o'].data_ptr()] = dict(d_o=b['d_o'], **{t: b[t].clone() for t in ('dq', 'dk', 'dv')})
-    mp.setattr(ops, 'mha_varlen_bwd', recording_bwd)
-
-    def tap(mod, method, box):
-        fn = getattr(mod, method)
-
-        def wrapped(x, *rest):
-            box.update(x=x.detach(), rest=rest, calls=[])
-            rec['cur'] = box['calls']
-            y = fn(_Tap.apply(x, box, 'dx') if x.requires_grad else x, *rest)
-            rec['cur'] = None
-            box['y'] = y.detach()
-            return _Tap.apply(y, box, 'dout')
-        mp.setattr(mod, method, wrapped)
-
-    for blk in model.kpf_encoder.encoder_blocks:
-        rec['enc'].append({})
-        tap(blk, 'forward', rec['enc'][-1])
-    for layer in model.transformer_encoder.layers:
-        rec['xenc'].append({})
-        tap(layer, 'forward_train_packed', rec['xenc'][-1])
-    return rec
-
-
-def _pairs(case):
-    from regtr_b200.synthetic import make_3dmatch_pair, make_modelnet_pair
-    return [(make_modelnet_pair if kind == 'modelnet' else make_3dmatch_pair)(*args)
-            for kind, args in FORWARD_CASES[case][2]]
-
-
-_RUNS = {}
-
-
-def _full_run(case):
-    """The recorded training step of a case (computed once per session)."""
-    if case in _RUNS:
-        return _RUNS[case]
-    from regtr_b200.regtr import RegTR
-    cfg, sd0, src, tgt = make_case(case)
-    sd = ei.loss_state_dict(sd0)
-    model = RegTR(cfg).to(DEV)
-    model.load_state_dict(sd, strict=True)
-    li = ei.loss_inputs(_pairs(case), [len(s) for s in src], [len(t) for t in tgt])
-    batch = {'src_xyz': [torch.from_numpy(s).to(DEV) for s in src], 'tgt_xyz': [torch.from_numpy(t).to(DEV) for t in tgt],
-             'pose': li['pose'].to(DEV), 'src_overlap': [m.to(DEV) for m in li['src_overlap']],
-             'tgt_overlap': [m.to(DEV) for m in li['tgt_overlap']]}
-    with pytest.MonkeyPatch.context() as mp:
-        rec = _record(model, mp)
-        model.compute_loss(model.forward_train(batch, train_encoder=True), batch)['total'].backward()
-    meta = batch['kpconv_meta']
-    run = dict(cfg=cfg, sd=sd, model=model, rec=rec, meta=meta, src=src, tgt=tgt, li=li,
-               grads={n: p.grad.detach().clone() for n, p in model.named_parameters() if p.grad is not None},
-               meta_cpu={k: [torch.as_tensor(v).cpu() for v in meta[k]]
-                         for k in ('points', 'neighbors', 'pools', 'stack_lengths')})
-    _RUNS[case] = run
-    return run
-
-
-def _trainable(model, prefix):
-    return [(n, p) for n, p in model.named_parameters() if n.startswith(prefix) and p.requires_grad]
-
-
-def _leaves(sd, names, dtype):
-    return {n: sd[n].detach().clone().to(dtype).requires_grad_(True) for n in names}
-
-
-# ----------------------------------------------------------------------------------------------- decisions
-
-def _block_sites(cfg, i):
-    from regtr_b200.config import pyramid_plan
-    b = pyramid_plan(cfg)[1][i]
-    if b['kind'] == 'simple':
-        return b, ['out']
-    return b, (['unary1'] if b['in_dim'] != b['out_dim'] // 4 else []) + ['conv', 'out']
-
-
-def _gpu_decisions(cfg, i, calls):
-    """The branch decisions the GPU took in encoder block i, in oracle.regtr_oracle.encoder_block's terms."""
-    from oracle import regtr_oracle as O
-    from regtr_b200 import ops
-    b, sites = _block_sites(cfg, i)
-    acts = [r for name, a, r in calls if name in ('instnorm_act', 'instnorm_apply') and a['slope'] >= 0]
-    assert len(acts) == len(sites), (i, len(acts), sites)
-    d = {site: ((r[0] if isinstance(r, tuple) else r).detach() > 0).cpu() for site, r in zip(sites, acts)}
-    (_, a, _), = [c for c in calls if c[0] == 'kpconv']
-    x, flags = a['x'].detach(), a['row_flags']
-    if flags is None:           # counted by the aggregation itself: from x's row sums (Cin > 1) or from x (Cin = 1)
-        flags = ops._kpconv_wf(a['q_pts'], a['s_pts'], a['idx32'], x, a['kernel_points'], a['extent'], None)[1] \
-            if x.shape[1] > 1 else x[:, 0] > 0
-    flags = torch.cat([flags[:x.shape[0]].bool().cpu(), torch.zeros(1, dtype=torch.bool)])
-    d['kpconv'] = flags[a['idx32'].long().cpu()].sum(-1).clamp(min=1)
-    pools = [c for c in calls if c[0] == 'max_pool']
-    assert len(pools) == (b['strided'] and b['kind'] != 'simple')
-    for _, a, r in pools:
-        xs, idx = a['x'].detach().cpu(), a['idx32'].long().cpu()
-        d['pool'] = O.max_pool_winner(xs, idx)
-        assert torch.equal(O.max_pool(xs, idx, d['pool']), r.detach().cpu())      # the slots the GPU's output took
-    return d
-
-
-def _flips(gpu, free, pool_idx=None):
-    """Number of decisions the unforced float64 forward takes differently, per site (a max-pool decision is the
-    winning support row; all shadow slots are one row)."""
-    out = []
-    for k, v in gpu.items():
-        w = free[k]
-        if k == 'pool':
-            v, w = pool_idx.gather(1, v), pool_idx.gather(1, w)
-        out.append(f'{k} {int((v != w).sum())}/{v.numel()}')
-    return ', '.join(out)
-
-
-# ------------------------------------------------------------------------------------- block-local encoder
-
-def _oracle_block(run, i, x, need_dx, dout, dtype, decisions, names):
-    from oracle import regtr_oracle as O
-    sd = run['sd']
-    leaves = _leaves(sd, names, dtype)
-    sdd = {k: leaves.get(k, v) for k, v in sd.items() if k.startswith(f'{ENC}{i}.')}
-    xin = x.detach().cpu().to(dtype).requires_grad_(need_dx)
-    d = dict(decisions)
-    y = O.encoder_block(sdd, run['cfg'], i, xin, run['meta_cpu'], dtype, d)
-    assert d.keys() == decisions.keys()                  # every branch of the block was forced
-    ins = ([xin] if xin.requires_grad else []) + [leaves[n] for n in names]
-    return torch.autograd.grad(y, ins, dout.cpu().to(dtype))
 
 
 @pytest.mark.parametrize('case', CASES)
@@ -245,30 +67,6 @@ def test_encoder_blocks_backward_block_local(case):
 
 
 # -------------------------------------------------------------------------------- layer-local cross-encoder
-
-def _oracle_layer(run, i, x, pos, dout, dtype, masks, names):
-    """float64 / fp32 autograd of oracle.cross_encoder_layer over the pairs of the packed tokens x; masks: the
-    feed-forward ReLU masks per packed row, or None for the unforced forward (-> its masks, no gradients)."""
-    from oracle import regtr_oracle as O
-    lens = [int(v) for v in run['meta']['_lens'][-1]]
-    st = np.concatenate([[0], np.cumsum(lens)])
-    B = len(lens) // 2
-    leaves = _leaves(run['sd'], names, dtype)
-    xin = x.cpu().to(dtype).requires_grad_(True)
-    pe = pos.cpu().to(dtype) if pos is not None else torch.zeros_like(xin)
-    outs, gouts, free = [], [], []
-    for b in range(B):
-        rs, rt = slice(st[b], st[b + 1]), slice(st[B + b], st[B + b + 1])
-        d = {} if masks is None else {'ffn_src': masks[rs], 'ffn_tgt': masks[rt]}
-        so, to = O.cross_encoder_layer(leaves, run['cfg'], i, xin[rs], xin[rt], pe[rs], pe[rt], d)
-        assert len(d) == 2
-        outs += [so, to]
-        gouts += [dout[rs].cpu().to(dtype), dout[rt].cpu().to(dtype)]
-        free.append(d)
-    if masks is None:                                     # packed order: the B sources, then the B targets
-        return torch.cat([d['ffn_src'] for d in free] + [d['ffn_tgt'] for d in free])
-    return torch.autograd.grad(outs, [xin] + [leaves[n] for n in names], gouts)
-
 
 def _add_in_proj_rows(ys, label, g, a, b):
     """The q, k and v row blocks of an in-projection gradient, one yardstick row each: the k / v blocks are much

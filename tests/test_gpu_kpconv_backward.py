@@ -331,9 +331,10 @@ def test_train_encoder_gradients_match_reference_backward():
                    'entries (criterion 5e-3; 10 of the 35 encoder parameters over it).  Not kernel arithmetic: every '
                    'block and layer backward and the encoder backward fed the float64 d(feats_un) are as close to '
                    'float64 as the fp32 oracle, with no branch decision flipped (tests/test_gpu_grad_stages.py).  The '
-                   'GPU encoder forward output is 2.4e-6 off float64 (3.2e-6 before the InstanceNorm statistics were '
-                   'centred), and the stages after it turn that into a 4.75e-4 change of d(feats_un); DESIGN.md '
-                   'section 9')
+                   'GPU encoder forward output is 2.4e-6 off float64 and the fp32 oracle encoder\'s is 2.6e-6; every '
+                   'forward stage is within 0.7-1.05x the fp32 oracle\'s error (tests/test_gpu_forward_stages.py), so '
+                   'this is what an fp32 forward gets.  The stages after the encoder turn it into a 4.75e-4 change '
+                   'of d(feats_un); DESIGN.md section 9')
 def test_train_encoder_gradients_match_oracle_3dmatch_b2():
     """fwd_3dmatch_small_b2 (two pairs of different sizes, four pyramid levels, every Cin path): every parameter
     gradient, encoder included, against the CPU oracle's autograd."""

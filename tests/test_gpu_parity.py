@@ -41,43 +41,6 @@ def test_kpconv_vs_reference_golden(ops_golden):
     assert np.all(N(y)[3] == 0)
 
 
-@pytest.mark.parametrize('impl', ['pipe', 'mma', 'ffma'])
-@pytest.mark.parametrize('cin,cout', [(1, 64), (4, 16), (32, 32), (64, 64), (128, 128), (256, 256)])
-def test_kpconv_all_channel_paths_vs_oracle(cin, cout, impl, monkeypatch):
-    """The aggregation implementations (software-pipelined persistent tensor-core kernel = the default; the
-    one-query-per-warp tensor-core kernel and the CUDA-core kernels kept for A/B and as the large-K fallback)
-    on every channel-width path, incl. the fused Cin=1 block."""
-    from oracle import regtr_oracle as O
-    from regtr_b200 import ops
-    if impl == 'pipe':
-        monkeypatch.delenv('REGTR_AGG_IMPL', raising=False)
-    else:
-        monkeypatch.setenv('REGTR_AGG_IMPL', impl)
-    rng = np.random.default_rng(cin)
-    Nq, Ns, K = 301, 457, 40
-    q = rng.normal(size=(Nq, 3)).astype(np.float32) * 0.05
-    s = rng.normal(size=(Ns, 3)).astype(np.float32) * 0.05
-    idx = rng.integers(0, Ns + 1, size=(Nq, K))
-    idx[:, 30:] = np.where(rng.random((Nq, 10)) < 0.7, Ns, idx[:, 30:])     # shadow tails
-    idx[7] = Ns
-    x = rng.normal(size=(Ns, cin)).astype(np.float32) + (1.0 if cin == 1 else 0.0)
-    W = (rng.normal(size=(15, cin, cout)) / np.sqrt(15 * cin)).astype(np.float32)
-    kp = (rng.normal(size=(15, 3)) * 0.03).astype(np.float32)
-    want = O.kpconv(*(torch.from_numpy(a) for a in (q, s)), torch.from_numpy(idx), torch.from_numpy(x),
-                    torch.from_numpy(W), torch.from_numpy(kp), 0.05).numpy()
-    got = N(ops.kpconv(G(q), G(s), G(idx, torch.int32), G(x), G(W), G(kp), 0.05))
-    # which side a deviation comes from: both against the same math in float64
-    w64 = O.kpconv(*(torch.from_numpy(a).double() for a in (q, s)), torch.from_numpy(idx),
-                   *(torch.from_numpy(a).double() for a in (x, W, kp)), 0.05).numpy()
-    scale = np.abs(w64).max()
-    print(f'kpconv cin={cin} cout={cout} {impl}: vs float64, GPU {np.abs(got - w64).max() / scale:.2e}, '
-          f'fp32 oracle {np.abs(want - w64).max() / scale:.2e}')
-    # SURVEY 8c feature tolerance (1e-4 * max|ref|); the kernels measure ~2e-7 here.  Twice in ~20 suite runs the
-    # Cin = 1 case came out 5e-5 off on a few entries (not reproduced in isolated processes, sanitizer-clean:
-    # DESIGN.md 9), hence not the tighter 2e-5 the other paths would allow.
-    assert np.abs(got - want).max() <= 1e-4 * np.abs(want).max(), np.abs(got - want).max() / np.abs(want).max()
-
-
 def test_maxpool_instnorm_posemb_vs_reference_golden(ops_golden):
     from regtr_b200 import ops
     g = ops_golden
