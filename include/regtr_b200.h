@@ -156,8 +156,10 @@ int regtr_instnorm_apply(const float* x, const int32_t* offs, int n_clouds, int 
 
 /* ---- dense layers ---------------------------------------------------------------- */
 
-/* x = hi + lo with both halves exactly representable in TF32 (low 13 mantissa bits zero);
- * used to pre-split weight matrices for regtr_gemm_tf32x3. */
+/* The two TF32 halves of x (low 13 mantissa bits zero), each rounded to nearest, ties to even:
+ *   hi = tf32_rne(x),  lo = tf32_rne(x - hi)   (x - hi is exact in fp32).
+ * hi + lo is not x in general: lo drops the low bits of x - hi, so |x - (hi + lo)| <= half a TF32 ulp of
+ * x - hi, about 2^-22 |x|.  Used to pre-split weight matrices for regtr_gemm_tf32x3. */
 int regtr_split_tf32(const float* x, long long n, float* hi, float* lo, void* stream);
 
 /* fp32-accurate GEMM on the Hopper tensor cores (wgmma, 3xTF32):
@@ -165,8 +167,10 @@ int regtr_split_tf32(const float* x, long long n, float* hi, float* lo, void* st
  * Replaces nn.Linear (kpconv_blocks.py:546, regtr.py:36/145, transformers.py:95-101,
  * regtr.py:404-411) and the KPConv weight contraction (kpconv_blocks.py:401-406).
  * Row-major fp32; lda/ldb multiples of 4 and 16-byte aligned bases (TMA); bias / R optional;
- * m_dev (optional device int32): actual row count when M is a capacity; relu != 0 applies ReLU.
- * ws: regtr_gemm_ws_bytes(M,N,K) bytes (deterministic split-K planes for skinny long-K shapes). */
+ * C, R and bias may be any views (the epilogue uses 16-byte accesses only where their bases and
+ * pitches allow); m_dev (optional device int32): actual row count when M is a capacity; relu != 0
+ * applies ReLU.  ws: regtr_gemm_ws_bytes(M,N,K) bytes, 16-byte aligned (deterministic split-K
+ * planes for skinny long-K shapes). */
 size_t regtr_gemm_ws_bytes(int M, int N, int K);
 int regtr_gemm_tf32x3(const float* A, int lda, const float* B_hi, const float* B_lo, int ldb,
                       float* C, int ldc, const float* bias, const float* R, int ldr,
@@ -253,7 +257,9 @@ int regtr_mha_bf16_tc_fwd(const void* QK, int ld_qk, const void* Vt, int ld_vt, 
  * fp32 softmax.  Inputs from regtr_gemm_tf32x3_qkv_split, the packed in-projection (N = 3E: q | k | v) whose
  * epilogue writes every value as its two TF32 halves: qk4 [n_tokens, 4E] fp32 = [Q_hi | Q_lo | K_hi | K_lo] with q
  * pre-multiplied by qscale (pass softmax_scale * log2(e)); vt2 [2E, ld_vt] fp32 = v transposed, hi rows then lo rows
- * (columns >= the real token count must be finite, e.g. zero).  O [n_tokens, E] fp32.  head_dim must be 32.
+ * (columns >= the real token count must be finite, e.g. zero; the epilogue leaves them untouched).  Both halves are
+ * rounded to nearest with ties away from zero: hi = rna(x), lo = rna(x - hi).  The in-projection's bias is read
+ * 16 bytes at a time: its base must be 16-byte aligned.  O [n_tokens, E] fp32.  head_dim must be 32.
  * Problem tables as for regtr_mha_varlen_fwd. */
 int regtr_gemm_tf32x3_qkv_split(const float* A, int lda, const float* B_hi, const float* B_lo, int ldb,
                                 const float* bias, int M, int N, int K, int E, float qscale, float* qk4, int ld4,
@@ -305,7 +311,8 @@ int regtr_relu_bwd(const float* dh, const float* h, long long n, float* out, voi
 
 /* Weight gradient of a dense layer Y = X W^T + b:  dW[N,K] = dY^T X,  db[N] = sum_rows dY (db optional),
  * 3xTF32 on regtr_gemm_tf32x3 (the reduction over the M rows uses its deterministic split-K).  X (M,K) and
- * dY (M,N) row-major with leading dimensions ldx / ldy.  ws: regtr_linear_wgrad_ws_bytes(M, N, K) bytes,
+ * dY (M,N) row-major with leading dimensions ldx / ldy; M = 0 writes dW = 0 and db = 0 (X, dY and their
+ * leading dimensions are then not read: an empty tensor's data pointer is null and its strides arbitrary).  ws: regtr_linear_wgrad_ws_bytes(M, N, K) bytes,
  * 256-byte aligned (transposed, TF32-split operands and the product). */
 size_t regtr_linear_wgrad_ws_bytes(int M, int N, int K);
 int regtr_linear_wgrad(const float* X, int ldx, const float* dY, int ldy, int M, int N, int K,

@@ -428,8 +428,8 @@ size_t regtr_linear_wgrad_ws_bytes(int M, int N, int K) {
 int regtr_linear_wgrad(const float* X, int ldx, const float* dY, int ldy, int M, int N, int K, float* dW, float* db,
                        void* ws, size_t ws_bytes, void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
-    if (M < 0 || N <= 0 || K <= 0 || ldx < K || ldy < N) return REGTR_ERR_ARG;
-    if (!X || !dY || !dW) return REGTR_ERR_ARG;
+    if (M < 0 || N <= 0 || K <= 0 || (M > 0 && (ldx < K || ldy < N))) return REGTR_ERR_ARG;
+    if (!dW || (M > 0 && (!X || !dY))) return REGTR_ERR_ARG;      // no tokens: dW = 0, db = 0, X and dY unread
     const WgradLayout w = wgrad_layout(M > 0 ? M : 1, N, K);
     if (!ws || ((uintptr_t)ws & 255) || ws_bytes < w.total) return REGTR_ERR_WORKSPACE;
     char* base = (char*)ws;

@@ -164,8 +164,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, CfgT<BN, ST>::MIN_CTAS)
 k_gemm_tf32x3_wg(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
                  const __grid_constant__ CUtensorMap tmBlo, float* __restrict__ C, int ldc,
                  const float* __restrict__ bias, const float* __restrict__ R, int ldr, int M, int N, int K,
-                 const int32_t* __restrict__ m_dev, int relu, int kb_per_split, size_t split_stride, QkvOut qkv,
-                 float2* __restrict__ part) {
+                 const int32_t* __restrict__ m_dev, int relu, int vec, int kb_per_split, size_t split_stride,
+                 QkvOut qkv, float2* __restrict__ part) {
     using P = CfgT<BN, ST>;
     extern __shared__ unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -356,7 +356,7 @@ k_gemm_tf32x3_wg(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 }
                 continue;
             }
-            if (col0 + 32 <= N && (ldc & 3) == 0 && (!R || (ldr & 3) == 0)) {
+            if (col0 + 32 <= N && vec) {
                 // the block's rows leave as 128-byte row segments, 4 rows per warp instruction -- 4 memory wavefronts
                 // instead of 32 per store, and the residual is read the same way
                 const int cq = lane & 7, rsub = lane >> 3;
@@ -530,6 +530,10 @@ int launch_gemm(const float* A, int lda, const float* Bhi, const float* Blo, int
     }
     const int nkb = regtr_cdiv(K, BK);
     const int tiles = regtr_cdiv(M, BM) * regtr_cdiv(N, BN);
+    // float4 epilogue (C stores, R and bias loads) only where every row segment it touches is 16-byte aligned; a
+    // view whose base or pitch is not takes the scalar path
+    const int vec = (ldc & 3) == 0 && ((uintptr_t)C & 15) == 0 && (!R || ((ldr & 3) == 0 && ((uintptr_t)R & 15) == 0)) &&
+                    ((uintptr_t)bias & 15) == 0;
     if (splits <= 1) {
         // Launches of several waves walk their tiles with fewer CTAs: ~4 tiles per CTA, between half and twice the SM
         // count, so that one set-up serves several tiles and the other forwards' kernels still find free SMs.
@@ -540,7 +544,7 @@ int launch_gemm(const float* A, int lda, const float* Bhi, const float* Blo, int
             if (grid > tiles) grid = tiles;
         }
         k_gemm_tf32x3_wg<BN, ST><<<grid, GEMM_THREADS, P::SMEM, st>>>(tA, tBh, tBl, C, ldc, bias, R, ldr, M, N, K, m_dev,
-                                                                      relu, nkb, 0, qkv, part);
+                                                                      relu, vec, nkb, 0, qkv, part);
         REGTR_CHECK_LAUNCH();
         return REGTR_OK;
     }
@@ -548,7 +552,7 @@ int launch_gemm(const float* A, int lda, const float* Bhi, const float* Blo, int
     const int z = regtr_cdiv(nkb, per);                     // every plane gets >= 1 k-block
     const size_t stride = (size_t)M * N;
     k_gemm_tf32x3_wg<BN, ST><<<dim3(tiles, 1, z), GEMM_THREADS, P::SMEM, st>>>(tA, tBh, tBl, ws, N, nullptr, nullptr, 0, M, N,
-                                                                               K, m_dev, 0, per, stride, NO_QKV, nullptr);
+                                                                               K, m_dev, 0, 1, per, stride, NO_QKV, nullptr);
     REGTR_CHECK_LAUNCH();
     k_splitk_reduce<<<regtr_cdiv((long long)M * (N / 4), 256), 256, 0, st>>>(ws, z, stride, C, ldc, bias, R, ldr, M, N,
                                                                             m_dev, relu);
@@ -598,7 +602,7 @@ static int gemm_dispatch(const float* A, int lda, const float* B_hi, const float
     const int bn = choose_bn(M, N);
     int splits = choose_splits(M, N, K, bn);
     if (used_splits) *used_splits = splits;
-    if (splits > 1 && (!ws || ws_bytes < regtr_gemm_ws_bytes(M, N, K))) return REGTR_ERR_WORKSPACE;
+    if (splits > 1 && (!ws || ((uintptr_t)ws & 15) || ws_bytes < regtr_gemm_ws_bytes(M, N, K))) return REGTR_ERR_WORKSPACE;
     float2* p = splits > 1 ? nullptr : part;
     // Stages: as deep as keeps the epilogue tile beside them; the 32-wide tile takes 3 so that two CTAs share an SM.
     if (bn == 128) return launch_gemm<128, 3>(A, lda, B_hi, B_lo, ldb, C, ldc, bias, R, ldr, M, N, K, m_dev, relu, splits, (float*)ws, st, NO_QKV, p);
@@ -663,7 +667,7 @@ int regtr_gemm_tf32x3_qkv_split(const float* A, int lda, const float* B_hi, cons
     if (M == 0) return REGTR_OK;
     if (!A || !B_hi || !B_lo || !qk4 || !vt2) return REGTR_ERR_ARG;
     if ((E & 31) || (ld4 & 3) || ld4 < 4 * E || ((uintptr_t)qk4 & 15) || (lda & 3) || (ldb & 3) || ((uintptr_t)A & 15) ||
-        ((uintptr_t)B_hi & 15) || ((uintptr_t)B_lo & 15) || ld_vt < M)
+        ((uintptr_t)B_hi & 15) || ((uintptr_t)B_lo & 15) || ((uintptr_t)bias & 15) || ld_vt < M)
         return REGTR_ERR_UNSUPPORTED;
     QkvOut q = NO_QKV;
     q.qk4 = qk4; q.ld4 = ld4; q.vt2 = vt2; q.ld_vtf = ld_vt; q.E = E; q.qscale = qscale;
