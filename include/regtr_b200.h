@@ -715,6 +715,38 @@ int regtr_loss_pointwise_norm(const regtr_loss_args* args, const double* norm, v
 int regtr_infonce_bwd_norm(const regtr_loss_args* args, const double* norm, void* stream);
 int regtr_loss_finalize_norm(const regtr_loss_args* args, const double* norm, void* stream);
 
+/* The circle feature loss (CircleLossFull(dist_type='euclidean'), feature_loss_type = 'circle') in place of InfoNCE, on
+ * the same regtr_loss_args: feat[t] (N, 256) are the term's packed features, source and target rows alike; q, dq,
+ * pos, anchor, lse, row_loss and n_anchor are not read.  The circle-only buffers, all device memory: */
+typedef struct {
+    int32_t* n_pos;     /* (N) positives of each token: a source token's over its pair's target tokens, a target
+                           token's over its pair's source tokens */
+    int32_t* n_neg;     /* (N) negatives, the same way */
+    int32_t* n_sel;     /* (2B) selected tokens (a positive and a negative) of each cloud, offs order */
+    double* lse_pos;    /* (n_terms, N) log-sum-exp of the positive exponents of each token's row / column */
+    double* lse_neg;    /* (n_terms, N) of the negative exponents */
+} regtr_circle_args;
+/* Rule and arithmetic in csrc/loss.cu.  D_ij = sqrt(|f_i - f_j|^2 + 1e-12); positive: key-point distance < r_p,
+ * negative: > r_n (source key points moved by the ground truth); z+ = 10 (D - 0.1) max(D - 0.1, 0) on positives,
+ * z- = 10 (1.4 - D) max(1.4 - D, 0) on negatives, 0 elsewhere.
+ * regtr_circle_match (one launch): src_gt, n_pos and n_neg of every token.
+ * regtr_circle_fwd (two launches): lse_pos / lse_neg of every source row over its pair's target tokens (one launch)
+ *   and of every target column over its pair's source tokens (the other); -inf when the other cloud is empty.
+ * regtr_circle_finalize (one launch, one CTA): n_sel; pair_loss[t, b] = (mean over the selected source tokens +
+ *   mean over the selected target tokens of softplus(lse_pos + lse_neg) / 10) / 2 in fp64 (NaN when a side has no
+ *   selected token; softplus is x above 20); vals[term_val[t]] = mean_b pair_loss; the pointwise values from ws.
+ * regtr_circle_bwd (two launches): with H_ij = (dL/dD_ij) / D_ij for the upstream gradient g,
+ *   dfeat[t] rows of the source tokens = sum_j H_ij (f_i - f_j) (one launch) and of the target tokens
+ *   sum_i H_ij (f_j - f_i) (the other).  Source and target rows are owned by different CTAs: no atomics.
+ * The *_norm variants mean the terms over norm[3] pairs, as regtr_loss_finalize_norm / regtr_infonce_bwd_norm. */
+int regtr_circle_match(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream);
+int regtr_circle_fwd(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream);
+int regtr_circle_finalize(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream);
+int regtr_circle_bwd(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream);
+int regtr_circle_finalize_norm(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm,
+                               void* stream);
+int regtr_circle_bwd_norm(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm, void* stream);
+
 /* ---- status word helpers (device uint32) ------------------------------------------ */
 int regtr_status_clear(uint32_t* status, void* stream);
 

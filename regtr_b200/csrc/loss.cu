@@ -427,6 +427,29 @@ __global__ void __launch_bounds__(256) k_infonce_bwd_tgt(const regtr_loss_args a
 
 // ---------------------------------------------------------------------------------------------- loss values
 
+// vals of the feature terms: the mean of pair_loss over the pairs, in pair order.  Block-strided over the terms.
+__device__ __forceinline__ void term_values(const regtr_loss_args& a, const Norms& nm) {
+    for (int t = threadIdx.x; t < a.n_terms; t += blockDim.x) {
+        double s = 0.0;
+        for (int b = 0; b < a.B; ++b) s += a.pair_loss[t * a.B + b];
+        a.vals[a.term_val[t]] = (float)(s / nm.b);
+    }
+}
+
+// vals of the BCE and L1 terms from the partial sums regtr_loss_pointwise left in ws.  Block-strided over the layers.
+__device__ __forceinline__ void pointwise_values(const regtr_loss_args& a, int n_chunks, const Norms& nm) {
+    const double* den = a.ws + (long long)a.L * n_chunks * 3;
+    for (int l = threadIdx.x; l < a.L; l += blockDim.x) {
+        double bce = 0.0, es = 0.0, et = 0.0;
+        for (int c = 0; c < n_chunks; ++c) {
+            const double* p = a.ws + ((long long)l * n_chunks + c) * 3;
+            bce += p[0]; es += p[1]; et += p[2];
+        }
+        if (a.ov_val[l] >= 0) a.vals[a.ov_val[l]] = (float)(bce / nm.n);
+        if (a.corr_val[l] >= 0) a.vals[a.corr_val[l]] = (float)(es / den[0] + et / den[1]);
+    }
+}
+
 __global__ void k_loss_finalize(const regtr_loss_args a, int n_chunks, const double* __restrict__ norm) {
     const Norms nm = batch_norms(a, norm);
     for (int b = threadIdx.x; b < a.B; b += blockDim.x) {
@@ -443,21 +466,8 @@ __global__ void k_loss_finalize(const regtr_loss_args a, int n_chunks, const dou
         a.pair_loss[e] = s / (double)a.n_anchor[b];               // no anchor: 0 / 0 = NaN, as the reference
     }
     __syncthreads();
-    for (int t = threadIdx.x; t < a.n_terms; t += blockDim.x) {
-        double s = 0.0;
-        for (int b = 0; b < a.B; ++b) s += a.pair_loss[t * a.B + b];
-        a.vals[a.term_val[t]] = (float)(s / nm.b);
-    }
-    const double* den = a.ws + (long long)a.L * n_chunks * 3;
-    for (int l = threadIdx.x; l < a.L; l += blockDim.x) {
-        double bce = 0.0, es = 0.0, et = 0.0;
-        for (int c = 0; c < n_chunks; ++c) {
-            const double* p = a.ws + ((long long)l * n_chunks + c) * 3;
-            bce += p[0]; es += p[1]; et += p[2];
-        }
-        if (a.ov_val[l] >= 0) a.vals[a.ov_val[l]] = (float)(bce / nm.n);
-        if (a.corr_val[l] >= 0) a.vals[a.corr_val[l]] = (float)(es / den[0] + et / den[1]);
-    }
+    term_values(a, nm);
+    pointwise_values(a, n_chunks, nm);
 }
 
 __global__ void __launch_bounds__(PW) k_loss_norms(const regtr_loss_args a, double* __restrict__ out) {
@@ -467,6 +477,312 @@ __global__ void __launch_bounds__(PW) k_loss_norms(const regtr_loss_args a, doub
     if (threadIdx.x == 0) {
         out[0] = (double)a.N; out[1] = ws; out[2] = wt; out[3] = (double)a.B;
     }
+}
+
+// ---------------------------------------------------------------------------------------------- circle loss
+//
+// CircleLossFull(dist_type='euclidean') of feature_loss.py:160-243 per pair: D_ij = sqrt(|a_i - b_j|^2 + 1e-12), an
+// entry is positive when the key points are closer than r_p and negative when farther than r_n (the InfoNCE geometry
+// rule above), z+ = 10 (D - 0.1) max(D - 0.1, 0) on positives and z- = 10 (1.4 - D) max(1.4 - D, 0) on negatives, 0 on
+// every other entry (the reference's detached weights vanish there, so exp(0) = 1 enters each log-sum-exp).  A source
+// row's loss is softplus(lse_j z+ + lse_j z-) / 10, a target column's the same over i; the pair's loss is the mean
+// over the rows with a positive and a negative plus the mean over such columns, halved (NaN when either set is empty).
+//
+// The squared distance is one fmaf chain of the squared channel differences in ascending order; (x - y)^2 = (y - x)^2
+// exactly, so every pass gets the same D whichever side is resident.  The |a|^2 + |b|^2 - 2ab form is not used: the
+// features are LayerNorm outputs with |a|^2 in the hundreds, and near the margins its cancellation costs several
+// digits.  For the same reason the backward takes the differences explicitly: dA_i = sum_j H_ij (a_i - b_j) with
+// H_ij = (dL/dD_ij) / D_ij, not a_i sum_j H_ij - sum_j H_ij b_j.
+
+constexpr int CKC = 32;     // channels of the streamed rows staged per step (two score tiles share the 48 KB)
+
+struct CircleTile {
+    float res[TM][D + 1];       // the CTA's own rows, all channels
+    float chunk[TM][CKC + 1];   // CKC channels of the streamed rows
+    float zp[TM][TM + 1];       // [resident][streamed]: z+, then H in the backward
+    float zn[TM][TM + 1];       // z-
+    float rxyz[TM][3];          // key points of the resident rows (sources: moved by the ground truth)
+    float sxyz[TM][3];          // key points of the streamed rows
+    float rc[TM], sc[TM];       // backward: gradient factor of each resident / streamed row
+    double rlp[TM], rln[TM], slp[TM], sln[TM];   // backward: their positive / negative log-sum-exps
+};
+
+__device__ __forceinline__ void circle_load_resident(CircleTile& T, const float* __restrict__ base, int n_rows) {
+    for (int e = threadIdx.x; e < TM * D; e += blockDim.x) {
+        const int r = e / D, k = e - r * D;
+        T.res[r][k] = r < n_rows ? base[(long long)r * D + k] : 0.f;
+    }
+}
+
+// acc[u][v] = |res[ro + u] - streamed row co + v|^2.  Begins and ends with the block in step.
+__device__ __forceinline__ void tile_sqdist(CircleTile& T, const float* __restrict__ stream, int n_stream,
+                                            float acc[2][2]) {
+    const int ro = 2 * (threadIdx.x >> 4), co = 2 * (threadIdx.x & 15);
+    acc[0][0] = acc[0][1] = acc[1][0] = acc[1][1] = 0.f;
+    for (int kc = 0; kc < D; kc += CKC) {
+        __syncthreads();
+        for (int e = threadIdx.x; e < TM * CKC; e += blockDim.x) {
+            const int r = e / CKC, k = e - r * CKC;
+            T.chunk[r][k] = r < n_stream ? stream[(long long)r * D + kc + k] : 0.f;
+        }
+        __syncthreads();
+#pragma unroll 8
+        for (int k = 0; k < CKC; ++k) {
+            const float r0 = T.res[ro][kc + k], r1 = T.res[ro + 1][kc + k];
+            const float c0 = T.chunk[co][k], c1 = T.chunk[co + 1][k];
+            const float d00 = r0 - c0, d01 = r0 - c1, d10 = r1 - c0, d11 = r1 - c1;
+            acc[0][0] = fmaf(d00, d00, acc[0][0]);
+            acc[0][1] = fmaf(d01, d01, acc[0][1]);
+            acc[1][0] = fmaf(d10, d10, acc[1][0]);
+            acc[1][1] = fmaf(d11, d11, acc[1][1]);
+        }
+    }
+}
+
+// Key points of `n` rows starting at token `i0` of side `side` (0: moved source points, 1: target points) into dst,
+// by the 32 threads starting at thread `t0`.
+__device__ __forceinline__ void circle_load_xyz(float (*dst)[3], const regtr_loss_args& a, int side, int i0, int n,
+                                                int t0) {
+    const int r = (int)threadIdx.x - t0;
+    if (r >= 0 && r < TM) {
+        const float* src = side == 0 ? a.src_gt : a.xyz;
+        for (int k = 0; k < 3; ++k) dst[r][k] = r < n ? src[3 * (long long)(i0 + r) + k] : 0.f;
+    }
+}
+
+// The exponents of one entry and their derivatives with respect to D (the weights are detached).
+struct CircleZ {
+    float zp, zn, dzp, dzn;
+};
+
+__device__ __forceinline__ CircleZ circle_z(float dist, double g2, double rp2, double rn2) {
+    CircleZ z{0.f, 0.f, 0.f, 0.f};
+    if (g2 < rp2) {
+        const float u = dist - 0.1f, w = fmaxf(u, 0.f);
+        z.zp = (10.f * u) * w;
+        z.dzp = 10.f * w;
+    }
+    if (g2 > rn2) {
+        const float u = 1.4f - dist, w = fmaxf(u, 0.f);
+        z.zn = (10.f * u) * w;
+        z.dzn = -10.f * w;
+    }
+    return z;
+}
+
+__device__ __forceinline__ float circle_dist(float sq) { return sqrtf(sq + 1e-12f); }
+
+// Online log-sum-exp of n finite values: running maximum m and the sum of exp(z - m) in fp64.
+__device__ __forceinline__ void lse_update(const float* z, int n, float& m, double& s) {
+    float mt = -INFINITY;
+    for (int j = 0; j < n; ++j) mt = fmaxf(mt, z[j]);
+    if (mt > -INFINITY) {
+        const float mn = fmaxf(m, mt);
+        s *= (double)expf(m - mn);
+        for (int j = 0; j < n; ++j) s += (double)expf(z[j] - mn);
+        m = mn;
+    }
+}
+
+__device__ __forceinline__ bool circle_selected(const regtr_circle_args& c, int i) {
+    return c.n_pos[i] > 0 && c.n_neg[i] > 0;
+}
+
+// softplus with torch's threshold: x above 20 is returned as it is (and its derivative is 1).
+__device__ __forceinline__ double softplus20(double x) { return x > 20.0 ? x : log1p(exp(x)); }
+__device__ __forceinline__ double softplus20_grad(double x) { return x > 20.0 ? 1.0 : 1.0 / (1.0 + exp(-x)); }
+
+// Positive / negative counts of every token over the other cloud of its pair; the moved source points into src_gt.
+// grid (tiles of 128 tokens, B, side).
+__global__ void k_circle_match(const regtr_loss_args a, const regtr_circle_args c) {
+    const int b = blockIdx.y, side = blockIdx.z;
+    const int c0 = a.offs[side * a.B + b], c1 = a.offs[side * a.B + b + 1];
+    const int o0 = a.offs[(1 - side) * a.B + b], o1 = a.offs[(1 - side) * a.B + b + 1];
+    const int i = c0 + blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= c1) return;
+    float p[3];
+    if (side == 0) {
+        gt_point(a.pose, b, false, a.xyz + 3 * (long long)i, p);
+        for (int k = 0; k < 3; ++k) a.src_gt[3 * (long long)i + k] = p[k];
+    } else {
+        for (int k = 0; k < 3; ++k) p[k] = a.xyz[3 * (long long)i + k];
+    }
+    int np = 0, nn = 0;
+    for (int j = o0; j < o1; ++j) {
+        float q[3];
+        if (side == 0) {
+            for (int k = 0; k < 3; ++k) q[k] = a.xyz[3 * (long long)j + k];
+        } else {
+            gt_point(a.pose, b, false, a.xyz + 3 * (long long)j, q);
+        }
+        const double g2 = dist2(p, q);
+        np += g2 < a.rp2;
+        nn += g2 > a.rn2;
+    }
+    c.n_pos[i] = np;
+    c.n_neg[i] = nn;
+}
+
+// Positive and negative log-sum-exps of the tokens of side SIDE (0: source rows over the pair's target tokens, 1:
+// target columns over its source tokens); one CTA per tile of TM tokens, streaming the other side.
+template <int SIDE>
+__global__ void __launch_bounds__(256) k_circle_lse(const regtr_loss_args a, const regtr_circle_args c) {
+    __shared__ CircleTile T;
+    const int term = blockIdx.z, b = blockIdx.y;
+    const int i0 = a.offs[SIDE * a.B + b] + blockIdx.x * TM, n_i = min(TM, a.offs[SIDE * a.B + b + 1] - i0);
+    if (n_i <= 0) return;
+    const int o0 = a.offs[(1 - SIDE) * a.B + b], n_o = a.offs[(1 - SIDE) * a.B + b + 1] - o0;
+    const int ro = 2 * (threadIdx.x >> 4), co = 2 * (threadIdx.x & 15);
+    const float* F = a.feat[term];
+    circle_load_resident(T, F + (long long)i0 * D, n_i);
+    circle_load_xyz(T.rxyz, a, SIDE, i0, n_i, 0);
+    float mp = -INFINITY, mn = -INFINITY;                       // of row threadIdx.x (threads < TM)
+    double sp = 0.0, sn = 0.0;
+    for (int j0 = 0; j0 < n_o; j0 += TM) {
+        const int n_j = min(TM, n_o - j0);
+        __syncthreads();
+        circle_load_xyz(T.sxyz, a, 1 - SIDE, o0 + j0, n_j, 32);
+        float acc[2][2];
+        tile_sqdist(T, F + (long long)(o0 + j0) * D, n_j, acc);
+        for (int u = 0; u < 2; ++u)
+            for (int v = 0; v < 2; ++v) {
+                const int i = ro + u, j = co + v;
+                if (i < n_i && j < n_j) {
+                    const CircleZ z = circle_z(circle_dist(acc[u][v]), dist2(T.rxyz[i], T.sxyz[j]), a.rp2, a.rn2);
+                    T.zp[i][j] = z.zp;
+                    T.zn[i][j] = z.zn;
+                }
+            }
+        __syncthreads();
+        if (threadIdx.x < n_i) {
+            lse_update(T.zp[threadIdx.x], n_j, mp, sp);
+            lse_update(T.zn[threadIdx.x], n_j, mn, sn);
+        }
+    }
+    if (threadIdx.x < n_i) {
+        const long long k = (long long)term * a.N + i0 + threadIdx.x;
+        c.lse_pos[k] = (double)mp + log(sp);                    // empty other side: -inf
+        c.lse_neg[k] = (double)mn + log(sn);
+    }
+}
+
+// Gradient factor of token i (cloud cl) in term t: dL/d(lse+ + lse-) = g softplus'(x) / (20 n_sel(cl) n_pairs) when
+// the token is selected, else 0; and its two log-sum-exps.
+__device__ __forceinline__ void circle_coef(const regtr_loss_args& a, const regtr_circle_args& c, int t, int cl, int i,
+                                            double n_pairs, float& f, double& lp, double& ln) {
+    const long long k = (long long)t * a.N + i;
+    lp = c.lse_pos[k];
+    ln = c.lse_neg[k];
+    f = circle_selected(c, i)
+        ? (float)((double)a.g[a.term_val[t]] * softplus20_grad(lp + ln) / (20.0 * (double)c.n_sel[cl] * n_pairs))
+        : 0.f;
+}
+
+__device__ __forceinline__ float circle_dldd(const CircleZ& z, float f, double lp, double ln) {
+    if (f == 0.f) return 0.f;
+    float s = 0.f;
+    if (z.dzp != 0.f) s += expf((float)((double)z.zp - lp)) * z.dzp;
+    if (z.dzn != 0.f) s += expf((float)((double)z.zn - ln)) * z.dzn;
+    return f * s;
+}
+
+// d feat[t] of the tokens of side SIDE: one CTA per tile of TM tokens streaming the other side; thread ch owns channel
+// ch of all its rows.  Both sides are written by their own CTAs: no atomics.
+template <int SIDE>
+__global__ void __launch_bounds__(256) k_circle_bwd(const regtr_loss_args a, const regtr_circle_args c,
+                                                    const double* __restrict__ norm) {
+    __shared__ CircleTile T;
+    const int term = blockIdx.z, b = blockIdx.y;
+    const int rcl = SIDE * a.B + b, scl = (1 - SIDE) * a.B + b;
+    const int i0 = a.offs[rcl] + blockIdx.x * TM, n_i = min(TM, a.offs[rcl + 1] - i0);
+    if (n_i <= 0) return;
+    const int o0 = a.offs[scl], n_o = a.offs[scl + 1] - o0;
+    const int ro = 2 * (threadIdx.x >> 4), co = 2 * (threadIdx.x & 15), ch = threadIdx.x;
+    const double n_pairs = batch_norms(a, norm).b;
+    const float* F = a.feat[term];
+    circle_load_resident(T, F + (long long)i0 * D, n_i);
+    circle_load_xyz(T.rxyz, a, SIDE, i0, n_i, 0);
+    if (threadIdx.x >= 64 && threadIdx.x < 64 + TM) {
+        const int r = threadIdx.x - 64;
+        float f = 0.f;
+        double lp = 0.0, ln = 0.0;
+        if (r < n_i) circle_coef(a, c, term, rcl, i0 + r, n_pairs, f, lp, ln);
+        T.rc[r] = f; T.rlp[r] = lp; T.rln[r] = ln;
+    }
+    __syncthreads();
+    float own[TM], out[TM];
+#pragma unroll
+    for (int r = 0; r < TM; ++r) {
+        own[r] = T.res[r][ch];
+        out[r] = 0.f;
+    }
+    for (int j0 = 0; j0 < n_o; j0 += TM) {
+        const int n_j = min(TM, n_o - j0);
+        __syncthreads();
+        circle_load_xyz(T.sxyz, a, 1 - SIDE, o0 + j0, n_j, 32);
+        if (threadIdx.x >= 96 && threadIdx.x < 96 + TM) {
+            const int r = threadIdx.x - 96;
+            float f = 0.f;
+            double lp = 0.0, ln = 0.0;
+            if (r < n_j) circle_coef(a, c, term, scl, o0 + j0 + r, n_pairs, f, lp, ln);
+            T.sc[r] = f; T.slp[r] = lp; T.sln[r] = ln;
+        }
+        float acc[2][2];
+        const float* S = F + (long long)(o0 + j0) * D;
+        tile_sqdist(T, S, n_j, acc);
+        for (int u = 0; u < 2; ++u)
+            for (int v = 0; v < 2; ++v) {
+                const int i = ro + u, j = co + v;
+                float h = 0.f;
+                if (i < n_i && j < n_j) {
+                    const float dist = circle_dist(acc[u][v]);
+                    const CircleZ z = circle_z(dist, dist2(T.rxyz[i], T.sxyz[j]), a.rp2, a.rn2);
+                    h = (circle_dldd(z, T.rc[i], T.rlp[i], T.rln[i]) + circle_dldd(z, T.sc[j], T.slp[j], T.sln[j])) /
+                        dist;
+                }
+                T.zp[i][j] = h;
+            }
+        __syncthreads();
+        for (int j = 0; j < n_j; ++j) {
+            const float s = S[(long long)j * D + ch];
+#pragma unroll
+            for (int r = 0; r < TM; ++r) out[r] = fmaf(T.zp[r][j], own[r] - s, out[r]);
+        }
+    }
+#pragma unroll
+    for (int r = 0; r < TM; ++r)
+        if (r < n_i) a.dfeat[term][(long long)(i0 + r) * D + ch] = out[r];
+}
+
+// n_sel, pair_loss[t, b] in fp64 in token order, vals of the feature terms (mean over the pairs) and of the pointwise
+// terms.  One CTA.
+__global__ void k_circle_finalize(const regtr_loss_args a, const regtr_circle_args c, int n_chunks,
+                                  const double* __restrict__ norm) {
+    const Norms nm = batch_norms(a, norm);
+    for (int cl = threadIdx.x; cl < 2 * a.B; cl += blockDim.x) {
+        int n = 0;
+        for (int i = a.offs[cl]; i < a.offs[cl + 1]; ++i) n += circle_selected(c, i);
+        c.n_sel[cl] = n;
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < a.n_terms * a.B; e += blockDim.x) {
+        const int t = e / a.B, b = e - t * a.B;
+        double half[2];
+        for (int side = 0; side < 2; ++side) {
+            const int cl = side * a.B + b;
+            double s = 0.0;
+            for (int i = a.offs[cl]; i < a.offs[cl + 1]; ++i)
+                if (circle_selected(c, i)) {
+                    const long long k = (long long)t * a.N + i;
+                    s += softplus20(c.lse_pos[k] + c.lse_neg[k]) / 10.0;
+                }
+            half[side] = s / (double)c.n_sel[cl];                   // nothing selected: 0 / 0 = NaN, as the reference
+        }
+        a.pair_loss[e] = (half[0] + half[1]) / 2.0;
+    }
+    __syncthreads();
+    term_values(a, nm);
+    pointwise_values(a, n_chunks, nm);
 }
 
 int check_args(const regtr_loss_args* args) {
@@ -618,6 +934,88 @@ int regtr_loss_finalize_norm(const regtr_loss_args* args, const double* norm, vo
 
 int regtr_loss_finalize(const regtr_loss_args* args, void* stream_) {
     return regtr_loss_finalize_norm(args, nullptr, stream_);
+}
+
+static int check_circle(const regtr_loss_args* args, const regtr_circle_args* circ, bool bwd) {
+    const int rc = check_args(args);
+    if (rc) return rc;
+    const regtr_loss_args& a = *args;
+    if (!circ || !circ->n_pos || !circ->n_neg || !circ->n_sel || !circ->lse_pos || !circ->lse_neg) return REGTR_ERR_ARG;
+    if (a.N > 0 && (!a.xyz || !a.pose || !a.src_gt)) return REGTR_ERR_ARG;
+    for (int t = 0; t < a.n_terms; ++t) {
+        if (!a.feat[t] || a.term_val[t] < 0 || a.term_val[t] >= a.n_vals) return REGTR_ERR_ARG;
+        if (bwd && !a.dfeat[t]) return REGTR_ERR_ARG;
+    }
+    return REGTR_OK;
+}
+
+int regtr_circle_match(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream_) {
+    const int rc = check_circle(args, circ, false);
+    if (rc) return rc;
+    const regtr_loss_args& a = *args;
+    const int n = max(a.max_src, a.max_tgt);
+    if (n == 0) return REGTR_OK;
+    k_circle_match<<<dim3(regtr_cdiv(n, 128), a.B, 2), 128, 0, (cudaStream_t)stream_>>>(a, *circ);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_circle_fwd(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream_) {
+    const int rc = check_circle(args, circ, false);
+    if (rc) return rc;
+    const regtr_loss_args& a = *args;
+    if (a.n_terms == 0) return REGTR_OK;
+    if (a.max_src > 0) {
+        k_circle_lse<0><<<dim3(regtr_cdiv(a.max_src, TM), a.B, a.n_terms), 256, 0, (cudaStream_t)stream_>>>(a, *circ);
+        REGTR_CHECK_LAUNCH();
+    }
+    if (a.max_tgt > 0) {
+        k_circle_lse<1><<<dim3(regtr_cdiv(a.max_tgt, TM), a.B, a.n_terms), 256, 0, (cudaStream_t)stream_>>>(a, *circ);
+        REGTR_CHECK_LAUNCH();
+    }
+    return REGTR_OK;
+}
+
+int regtr_circle_bwd_norm(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm,
+                          void* stream_) {
+    const int rc = check_circle(args, circ, true);
+    if (rc) return rc;
+    const regtr_loss_args& a = *args;
+    if (a.n_terms == 0) return REGTR_OK;
+    if (!a.g) return REGTR_ERR_ARG;
+    if (a.max_src > 0) {
+        k_circle_bwd<0><<<dim3(regtr_cdiv(a.max_src, TM), a.B, a.n_terms), 256, 0, (cudaStream_t)stream_>>>(
+            a, *circ, norm);
+        REGTR_CHECK_LAUNCH();
+    }
+    if (a.max_tgt > 0) {
+        k_circle_bwd<1><<<dim3(regtr_cdiv(a.max_tgt, TM), a.B, a.n_terms), 256, 0, (cudaStream_t)stream_>>>(
+            a, *circ, norm);
+        REGTR_CHECK_LAUNCH();
+    }
+    return REGTR_OK;
+}
+
+int regtr_circle_bwd(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream_) {
+    return regtr_circle_bwd_norm(args, circ, nullptr, stream_);
+}
+
+int regtr_circle_finalize_norm(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm,
+                               void* stream_) {
+    const int rc = check_circle(args, circ, false);
+    if (rc) return rc;
+    const regtr_loss_args& a = *args;
+    if (!a.vals || !a.pair_loss || !a.ws) return REGTR_ERR_ARG;
+    if (a.ws_bytes < regtr_loss_ws_bytes(a.N, a.L)) return REGTR_ERR_WORKSPACE;
+    for (int l = 0; l < a.L; ++l)
+        if (a.ov_val[l] >= a.n_vals || a.corr_val[l] >= a.n_vals) return REGTR_ERR_ARG;
+    k_circle_finalize<<<1, 256, 0, (cudaStream_t)stream_>>>(a, *circ, n_chunks_of(a.N), norm);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_circle_finalize(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream_) {
+    return regtr_circle_finalize_norm(args, circ, nullptr, stream_);
 }
 
 }  // extern "C"

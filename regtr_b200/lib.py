@@ -118,6 +118,12 @@ SIGNATURES = {
     'regtr_loss_pointwise_norm': (_I, [_P, _P, _P]),
     'regtr_infonce_bwd_norm': (_I, [_P, _P, _P]),
     'regtr_loss_finalize_norm': (_I, [_P, _P, _P]),
+    'regtr_circle_match': (_I, [_P, _P, _P]),
+    'regtr_circle_fwd': (_I, [_P, _P, _P]),
+    'regtr_circle_finalize': (_I, [_P, _P, _P]),
+    'regtr_circle_bwd': (_I, [_P, _P, _P]),
+    'regtr_circle_finalize_norm': (_I, [_P, _P, _P, _P]),
+    'regtr_circle_bwd_norm': (_I, [_P, _P, _P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),
 }
 

@@ -4,7 +4,8 @@ Mirror of
   * `RegTR.compute_loss` (/root/reference/src/models/regtr.py:237-294) and its `weight_dict` (regtr.py:89-93),
   * `compute_overlaps` (/root/reference/src/models/backbone_kpconv/kpconv.py:540-566),
   * `CorrCriterion` (/root/reference/src/models/losses/corr_loss.py:9-40),
-  * `InfoNCELossFull` (/root/reference/src/models/losses/feature_loss.py:246-314).
+  * `InfoNCELossFull` (/root/reference/src/models/losses/feature_loss.py:246-314),
+  * `CircleLossFull(dist_type='euclidean')` (/root/reference/src/models/losses/feature_loss.py:160-243).
 `compute_loss` is plain torch ops on whatever device the predictions live on: the restatement pinned against the
 reference, and the yardstick of `compute_loss_device`, the same losses on the library's kernels (csrc/loss.cu), which
 `RegTR.compute_loss` takes for the model's own CUDA outputs.  Differentiable: on outputs of `RegTR.forward_train` the gradient flows on into the library's backward
@@ -74,6 +75,31 @@ def infonce_loss(W, src_feat, tgt_feat, src_xyz, tgt_xyz, r_p: float, r_n: float
     return torch.mean(torch.stack(per_pair))
 
 
+def circle_loss(src_feat, tgt_feat, src_xyz, tgt_xyz, r_p: float, r_n: float, log_scale: float = 10.0,
+                pos_margin: float = 0.1, neg_margin: float = 1.4):
+    """CircleLossFull.forward / get_circle_loss (feature_loss.py:191-243) with dist_type='euclidean', as written:
+    feature distances from explicit differences plus 1e-12 under the square root, masked entries offset by 1e5 so
+    that their detached weight is 0 and exp(0) = 1 enters every log-sum-exp, F.softplus (linear above 20), and the
+    mean over an empty selection, which is NaN.  The pair losses are meaned over the pairs."""
+    total = 0
+    for a, p, ax, px in zip(src_feat, tgt_feat, src_xyz, tgt_xyz):
+        coords = torch.cdist(ax, px)
+        feats = torch.sqrt(torch.sum((a.T[..., :, None] - p.T[..., None, :]) ** 2, dim=-3) + 1e-12)
+        pos_mask, neg_mask = coords < r_p, coords > r_n
+        row_sel = ((pos_mask.sum(-1) > 0) * (neg_mask.sum(-1) > 0)).detach()
+        col_sel = ((pos_mask.sum(-2) > 0) * (neg_mask.sum(-2) > 0)).detach()
+        pos = feats - 1e5 * (~pos_mask).to(feats.dtype)
+        pos_weight = torch.clamp_min(pos - pos_margin, min=0).detach()
+        zp = log_scale * (pos - pos_margin) * pos_weight
+        neg = feats + 1e5 * (~neg_mask).to(feats.dtype)
+        neg_weight = torch.clamp_min(neg_margin - neg, min=0).detach()
+        zn = log_scale * (neg_margin - neg) * neg_weight
+        loss_row = F.softplus(torch.logsumexp(zp, dim=-1) + torch.logsumexp(zn, dim=-1)) / log_scale
+        loss_col = F.softplus(torch.logsumexp(zp, dim=-2) + torch.logsumexp(zn, dim=-2)) / log_scale
+        total = total + (loss_row[row_sel].mean() + loss_col[col_sel].mean()) / 2
+    return total / len(src_feat)
+
+
 def loss_weights(cfg) -> Dict[str, float]:
     """regtr.py:89-93."""
     wd = {}
@@ -85,12 +111,12 @@ def loss_weights(cfg) -> Dict[str, float]:
 
 
 def compute_loss(model, pred: Dict, batch: Dict) -> Dict[str, torch.Tensor]:
-    """RegTR.compute_loss (regtr.py:237-294).  `model` supplies cfg and the two InfoNCE matrices
-    (`feature_criterion.W`, `feature_criterion_un.W`); batch needs `kpconv_meta`, `pose`, `src_overlap`,
-    `tgt_overlap` (the dataset's level-0 overlap masks)."""
+    """RegTR.compute_loss (regtr.py:237-294).  `model` supplies cfg and, for the InfoNCE feature loss, the two InfoNCE
+    matrices (`feature_criterion.W`, `feature_criterion_un.W`; the circle loss has no parameter); batch needs
+    `kpconv_meta`, `pose`, `src_overlap`, `tgt_overlap` (the dataset's level-0 overlap masks)."""
     cfg = model.cfg
-    if cfg.feature_loss_type != 'infonce':
-        raise NotImplementedError('only the InfoNCE feature loss is configured by the reference')
+    if cfg.feature_loss_type not in ('infonce', 'circle'):
+        raise NotImplementedError(f'feature_loss_type {cfg.feature_loss_type!r}')
     meta, pose_gt = batch['kpconv_meta'], batch['pose']
     p = len(meta['stack_lengths']) - 1
     batch['overlap_pyr'] = compute_overlaps(batch)
@@ -104,12 +130,15 @@ def compute_loss(model, pred: Dict, batch: Dict) -> Dict[str, torch.Tensor]:
     for i in cfg.overlap_loss_on:
         losses[f'overlap_{i}'] = F.binary_cross_entropy_with_logits(all_pred[i, :, 0], all_gt)
     src_kp_gt = se3_transform_list(pose_gt, list(pred['src_kp']))
+    if cfg.feature_loss_type == 'circle':
+        feature = lambda _crit, s, t: circle_loss(s, t, src_kp_gt, list(pred['tgt_kp']), cfg.r_p, cfg.r_n)
+    else:
+        feature = lambda crit, s, t: infonce_loss(crit.W, s, t, src_kp_gt, list(pred['tgt_kp']), cfg.r_p, cfg.r_n)
     for i in cfg.feature_loss_on:
-        losses[f'feature_{i}'] = infonce_loss(model.feature_criterion.W, [s[i] for s in pred['src_feat']],
-                                              [t[i] for t in pred['tgt_feat']], src_kp_gt, list(pred['tgt_kp']),
-                                              cfg.r_p, cfg.r_n)
-    losses['feature_un'] = infonce_loss(model.feature_criterion_un.W, list(pred['src_feat_un']),
-                                        list(pred['tgt_feat_un']), src_kp_gt, list(pred['tgt_kp']), cfg.r_p, cfg.r_n)
+        losses[f'feature_{i}'] = feature(getattr(model, 'feature_criterion', None), [s[i] for s in pred['src_feat']],
+                                         [t[i] for t in pred['tgt_feat']])
+    losses['feature_un'] = feature(getattr(model, 'feature_criterion_un', None), list(pred['src_feat_un']),
+                                   list(pred['tgt_feat_un']))
     for i in cfg.corr_loss_on:
         s = corr_loss(list(pred['src_kp']), [w[i] for w in pred['src_kp_warped']], pose_gt, src_ov)
         t = corr_loss(list(pred['tgt_kp']), [w[i] for w in pred['tgt_kp_warped']],
@@ -139,10 +168,10 @@ def _weight_vector(wd: Dict[str, float], keys, device) -> torch.Tensor:
 
 def device_route(model, pred, batch) -> bool:
     """True when `compute_loss_device` applies: `pred` carries the packed CUDA tensors its views were cut from, at
-    exact shapes and 256 channels, the InfoNCE loss is configured, and the pyramid has an int32 pooling table for every
-    level."""
+    exact shapes and 256 channels, the InfoNCE or the circle loss is configured, and the pyramid has an int32 pooling
+    table for every level."""
     core = getattr(pred, 'core', None)
-    if core is None or model.cfg.feature_loss_type != 'infonce' or not core['both_un'].is_cuda:
+    if core is None or model.cfg.feature_loss_type not in ('infonce', 'circle') or not core['both_un'].is_cuda:
         return False
     from . import ops
     from .kpconv import _meta_private
@@ -175,12 +204,14 @@ def compute_loss_device(model, pred, batch, reduce_norms=None) -> Dict[str, torc
     pose = pose if torch.is_tensor(pose) else torch.stack(list(pose))
     pose = pose[..., :3, :].to(device=dev, dtype=torch.float32).contiguous()
     geo = ops.LossGeometry(core['xyz_c'], meta['_offs'][-1], meta['_lens'][-1], pose, pyr[-1], cfg.overlap_loss_on,
-                           cfg.feature_loss_on, cfg.corr_loss_on, cfg.r_p, cfg.r_n)
+                           cfg.feature_loss_on, cfg.corr_loss_on, cfg.r_p, cfg.r_n, feature_loss=cfg.feature_loss_type)
     if reduce_norms is not None:
         geo.norm = ops.loss_norms(geo)
         reduce_norms(geo.norm)
-    vals = ops.loss_values(core['both_un'], core['cond'], core['corr'], core['logit'], model.feature_criterion.W,
-                           model.feature_criterion_un.W, geo)
+    circle = cfg.feature_loss_type == 'circle'                  # CircleLossFull has no parameter
+    vals = ops.loss_values(core['both_un'], core['cond'], core['corr'], core['logit'],
+                           None if circle else model.feature_criterion.W,
+                           None if circle else model.feature_criterion_un.W, geo)
     keys = geo.keys()
     losses = {k: vals[j] for j, k in enumerate(keys)}
     losses['total'] = torch.sum(vals * _weight_vector(loss_weights(cfg), keys, dev))

@@ -1241,6 +1241,8 @@ LOSS_ARGS = np.dtype([('xyz', '<u8'), ('offs', '<u8'), ('pose', '<u8'), ('w', '<
                       ('corr_val', '<i4', (LOSS_MAX_LAYERS,)), ('term_val', '<i4', (LOSS_MAX_TERMS,)), ('pad_', '<i4')],
                      align=True)
 assert (OVERLAP_PYR_ARGS.itemsize, LOSS_ARGS.itemsize) == (264, 568)     # the C structs' sizes
+CIRCLE_ARGS = np.dtype([('n_pos', '<u8'), ('n_neg', '<u8'), ('n_sel', '<u8'), ('lse_pos', '<u8'), ('lse_neg', '<u8')],
+                       align=True)
 
 
 def overlap_pyramid(pyr0, pools32, offs, n_clouds: int):
@@ -1293,13 +1295,19 @@ def sym_weight_bwd(dWs, dW):
 class LossGeometry:
     """What the device loss reads besides the predictions: xyz (N, 3) coarse key points (source clouds, then target
     clouds), offs (2B + 1) int32 device offsets and lens, the same lengths on the host, pose (B, 3, 4) fp32 ground
-    truth, w (N) coarsest ground-truth overlap, the layers each loss is applied to, and the InfoNCE radii.
+    truth, w (N) coarsest ground-truth overlap, the layers each loss is applied to, and the feature loss's radii.
     norm: None, or the (4,) fp64 device normalisers of the whole batch (`loss_norms` summed over the ranks that each
-    hold a slice of it): the values and gradients are then this slice's share of the batch's."""
+    hold a slice of it): the values and gradients are then this slice's share of the batch's.
+    feature_loss: 'infonce' (InfoNCELossFull, with its two W) or 'circle' (CircleLossFull(dist_type='euclidean'),
+    no parameters)."""
 
-    def __init__(self, xyz, offs, lens, pose, w, overlap_on, feature_on, corr_on, r_p: float, r_n: float, norm=None):
+    def __init__(self, xyz, offs, lens, pose, w, overlap_on, feature_on, corr_on, r_p: float, r_n: float, norm=None,
+                 feature_loss: str = 'infonce'):
+        if feature_loss not in ('infonce', 'circle'):
+            raise ValueError(f'LossGeometry: feature_loss {feature_loss!r}')
         self.xyz, self.offs, self.lens, self.pose, self.w = xyz, offs, [int(v) for v in lens], pose, w
         self.norm = None if norm is None else _chk(norm, torch.float64, 'norm', 1)
+        self.feature_loss = feature_loss
         self.B = len(self.lens) // 2
         self.overlap_on, self.feature_on, self.corr_on = list(overlap_on), list(feature_on), list(corr_on)
         self.r_p, self.r_n = float(r_p), float(r_n)
@@ -1329,7 +1337,9 @@ def loss_forward(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
     """Loss values of packed predictions: both_un (N, 256), cond (L, N, 256), corr (L, N, 3), logit (L, N, 1), the two
     InfoNCE matrices.  -> state dict; 'vals' is the fp32 vector of geo.keys(), the rest feeds loss_backward
     ('pair_loss' (terms, B) fp64 and 'n_anchor' (B) are the per-pair InfoNCE results).  The number of launches does
-    not depend on B; no host sync."""
+    not depend on B; no host sync.  With geo.feature_loss == 'circle' the feature terms are the circle loss (W and W_un
+    are None): 'pair_loss' holds its per-pair values, 'n_pos' / 'n_neg' (N) the geometric counts, 'n_sel' (2B) the
+    selected tokens of each cloud and 'lse_pos' / 'lse_neg' (terms, N) the fp64 row and column log-sum-exps."""
     L = _lib.load()
     dev = both_un.device
     both_un, cond = _chk(both_un.detach().contiguous(), torch.float32, 'both_un', 2), \
@@ -1351,10 +1361,16 @@ def loss_forward(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
     n_src = sum(geo.lens[:B])
     term_layers = list(geo.feature_on) + [-1]                    # -1: feature_un on both_un with W_un
     feats = [cond[l] if l >= 0 else both_un for l in term_layers]
-    Ws = [sym_weight(W.detach()), sym_weight(W_un.detach())]
     T = len(term_layers)
-    q = [gemm(x[:n_src], *Ws[0 if l >= 0 else 1]) if n_src else x.new_zeros((1, LOSS_DIM))
-         for x, l in zip(feats, term_layers)]
+    circle = geo.feature_loss == 'circle'
+    if circle:
+        if W is not None or W_un is not None:
+            raise ValueError('loss_forward: the circle loss has no W')
+        Ws, q = None, None
+    else:
+        Ws = [sym_weight(W.detach()), sym_weight(W_un.detach())]
+        q = [gemm(x[:n_src], *Ws[0 if l >= 0 else 1]) if n_src else x.new_zeros((1, LOSS_DIM))
+             for x, l in zip(feats, term_layers)]
     f32 = dict(dtype=torch.float32, device=dev)
     st = dict(geo=geo, keys=keys, term_layers=term_layers, feats=feats, Ws=Ws, q=q, n_src=n_src, shape=(nl, N),
               vals=torch.empty(len(keys), **f32), dlogit=torch.empty((nl, N), **f32), dcorr=torch.empty((nl, N, 3), **f32),
@@ -1377,7 +1393,9 @@ def loss_forward(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
     for i in geo.corr_on:
         a['corr_val'][i] = keys.index(f'corr_{i}')
     for t, l in enumerate(term_layers):
-        a['q'][t], a['feat'][t] = q[t].data_ptr(), feats[t].data_ptr()
+        a['feat'][t] = feats[t].data_ptr()
+        if not circle:
+            a['q'][t] = q[t].data_ptr()
         a['term_val'][t] = keys.index(f'feature_{l}' if l >= 0 else 'feature_un')
     st['args'], st['hold'] = a, (xyz, offs, pose, w, logit, corr)
     s = _stream()
@@ -1385,6 +1403,9 @@ def loss_forward(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
         _lib.check(L.regtr_loss_pointwise(a.ctypes.data, s), 'regtr_loss_pointwise')
     else:
         _lib.check(L.regtr_loss_pointwise_norm(a.ctypes.data, geo.norm.data_ptr(), s), 'regtr_loss_pointwise_norm')
+    if circle:
+        _circle_forward(L, st, a, s)
+        return st
     _lib.check(L.regtr_infonce_match(a.ctypes.data, s), 'regtr_infonce_match')
     _lib.check(L.regtr_infonce_fwd(a.ctypes.data, s), 'regtr_infonce_fwd')
     if geo.norm is None:
@@ -1406,6 +1427,8 @@ def loss_backward(st, g):
     f32 = dict(dtype=torch.float32, device=dev)
     d_logit, d_corr = torch.empty((nl, N, 1), **f32), torch.empty((nl, N, 3), **f32)
     d_un, d_cond = torch.zeros((N, LOSS_DIM), **f32), torch.zeros((nl, N, LOSS_DIM), **f32)
+    if st['geo'].feature_loss == 'circle':
+        return _circle_backward(L, st, g, d_un, d_cond, d_corr, d_logit)
     dq = torch.zeros((len(term_layers), max(n_src, 1), LOSS_DIM), **f32)
     dfeat = [d_cond[l] if l >= 0 else d_un for l in term_layers]
     a = st['args'].copy()
@@ -1430,6 +1453,47 @@ def loss_backward(st, g):
     return d_un, d_cond, d_corr, d_logit, dW[0], dW[1]
 
 
+def _circle_forward(L, st, a, s):
+    """loss_forward's circle part (regtr_circle_*): geometry, row and column log-sum-exps, values."""
+    geo, N, B, T = st['geo'], st['shape'][1], st['geo'].B, len(st['term_layers'])
+    dev = st['vals'].device
+    i32 = dict(dtype=torch.int32, device=dev)
+    st.update(n_pos=torch.empty(N, **i32), n_neg=torch.empty(N, **i32), n_sel=torch.empty(2 * B, **i32),
+              lse_pos=torch.empty((T, N), dtype=torch.float64, device=dev),
+              lse_neg=torch.empty((T, N), dtype=torch.float64, device=dev))
+    c = np.zeros((), CIRCLE_ARGS)
+    for f in CIRCLE_ARGS.names:
+        c[f] = st[f].data_ptr()
+    st['circle_args'] = c
+    _lib.check(L.regtr_circle_match(a.ctypes.data, c.ctypes.data, s), 'regtr_circle_match')
+    _lib.check(L.regtr_circle_fwd(a.ctypes.data, c.ctypes.data, s), 'regtr_circle_fwd')
+    if geo.norm is None:
+        _lib.check(L.regtr_circle_finalize(a.ctypes.data, c.ctypes.data, s), 'regtr_circle_finalize')
+    else:
+        _lib.check(L.regtr_circle_finalize_norm(a.ctypes.data, c.ctypes.data, geo.norm.data_ptr(), s),
+                   'regtr_circle_finalize_norm')
+    n_launch = int(N > 0 and st['shape'][0] > 0) + int(max(a['max_src'], a['max_tgt']) > 0) + \
+        int(a['max_src'] > 0) + int(a['max_tgt'] > 0) + 1
+    _count(n_launch)
+
+
+def _circle_backward(L, st, g, d_un, d_cond, d_corr, d_logit):
+    """loss_backward's circle part: both sides' feature gradients come from regtr_circle_bwd; there is no W."""
+    nl, N = st['shape']
+    a = st['args'].copy()
+    a['g'], a['dlogit_out'], a['dcorr_out'] = g.data_ptr(), d_logit.data_ptr(), d_corr.data_ptr()
+    for t, l in enumerate(st['term_layers']):
+        a['dfeat'][t] = (d_cond[l] if l >= 0 else d_un).data_ptr()
+    c, s, norm = st['circle_args'], _stream(), st['geo'].norm
+    _lib.check(L.regtr_loss_pointwise_bwd(a.ctypes.data, s), 'regtr_loss_pointwise_bwd')
+    if norm is None:
+        _lib.check(L.regtr_circle_bwd(a.ctypes.data, c.ctypes.data, s), 'regtr_circle_bwd')
+    else:
+        _lib.check(L.regtr_circle_bwd_norm(a.ctypes.data, c.ctypes.data, norm.data_ptr(), s), 'regtr_circle_bwd_norm')
+    _count(int(N > 0 and nl > 0) + int(a['max_src'] > 0) + int(a['max_tgt'] > 0))
+    return d_un, d_cond, d_corr, d_logit, None, None
+
+
 class _LossFn(torch.autograd.Function):
     """values vector of loss_forward; backward on loss_backward."""
 
@@ -1447,5 +1511,6 @@ class _LossFn(torch.autograd.Function):
 
 
 def loss_values(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
-    """The fp32 vector of geo.keys() loss values, differentiable with respect to the packed predictions and both W."""
+    """The fp32 vector of geo.keys() loss values, differentiable with respect to the packed predictions and both W
+    (for the circle loss, `geo.feature_loss == 'circle'`, W and W_un are None)."""
     return _LossFn.apply(both_un, cond, corr, logit, W, W_un, geo)

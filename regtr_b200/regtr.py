@@ -196,8 +196,8 @@ class RegTR(nn.Module):
         return out
 
     def compute_loss(self, pred, batch):
-        """Losses of a forward (regtr.py:237-294: overlap BCE, InfoNCE feature losses, L1 correspondence loss,
-        weighted total).  For outputs of `forward_train` (which carry autograd history) `total` is differentiable;
+        """Losses of a forward (regtr.py:237-294: overlap BCE, InfoNCE or circle feature losses (cfg.feature_loss_type),
+        L1 correspondence loss, weighted total).  For outputs of `forward_train` (which carry autograd history) `total` is differentiable;
         for outputs of `forward` the values are computed without grad, as `test_step` reports them.
         Needs batch['pose'], ['src_overlap'], ['tgt_overlap'], ['kpconv_meta'].
         An output of this model's own `forward` / `forward_train` on CUDA goes through the loss kernels
