@@ -278,6 +278,20 @@ int regtr_mha_varlen_fwd_lse(const float* Q, int ldq, const float* K, int ldk, c
                              const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
                              int n_heads, int head_dim, float scale, void* stream);
 
+/* Head-averaged attention probabilities (analysis; TransformerCrossEncoder.get_attentions):
+ *   P[q, k] = (1/H) sum_h softmax_k(Q_h[q] . K_h[k] * scale)
+ * for every (query range, key range) problem of the tables above -- nn.MultiheadAttention's weights with
+ * average_attn_weights=True.  Q / K are row-major with leading dims ldq / ldk (column slices allowed, 16-byte
+ * aligned, ld % 4 == 0).  Problem p writes its q_len[p] x k_len[p] block at P + p_offset[p] with row pitch p_pitch[p]
+ * (>= k_len[p]), so one launch fills e.g. a padded (B, Lq_max, Lk_max) layout directly; every other element of P is
+ * left untouched (the caller zero-fills padding), and a problem with an empty query or key range writes nothing.
+ * Scores on 3xTF32 mma.sync (fp32-accurate); base-2 softmax from a per-(row, head) maximum and sum computed by the
+ * kernel itself in a first sweep (no workspace).  No atomics: reruns are bit-identical.  head_dim 32, n_heads <= 16. */
+int regtr_mha_probs_avg(const float* Q, int ldq, const float* K, int ldk, float* P, const int64_t* p_offset,
+                        const int32_t* p_pitch, const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
+                        const int32_t* k_len, int n_problems, int max_q_len, int n_heads, int head_dim, float scale,
+                        void* stream);
+
 /* ---- backward (training) ---------------------------------------------------------- */
 
 /* Backward of the attention core over the same problem tables: given O and lse from regtr_mha_varlen_fwd_lse and

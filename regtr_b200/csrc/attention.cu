@@ -395,6 +395,160 @@ k_corr_attention(const float* __restrict__ Qp, const float* __restrict__ Kp, int
     }
 }
 
+// ---- head-averaged attention probabilities (analysis: TransformerCrossEncoder.get_attentions) -----------------
+// P[q, k] = (1/H) sum_h softmax_k(q_h . k_h * scale), what nn.MultiheadAttention returns with its default
+// average_attn_weights=True.  Block = (64-query tile, problem): 4 warps x 16 query rows, scores on mma.sync 3xTF32
+// exactly as in k_mha_tf32x3 (same fragments, same split), keys staged per head in chunks of 64.
+//   sweep 1: per head, the online row maximum m and sum l of exp2(s - m) over the whole key range; kept in shared
+//            memory as (m, 1 / l) -- the log-sum-exp in two parts, so that exp2 reads s - m with m exact;
+//   sweep 2: per key chunk, for every head the same scores again (bit for bit), exp2(s - m) / l summed over the heads
+//            in registers, then written once, scaled by 1/H.
+// No atomics: every output element has one writer.  Nothing outside [q_len x k_len] of a problem is written.
+constexpr int PQ = 64, PK = 64, PH_MAX = 16;
+
+__device__ __forceinline__ void probs_load_q(const float* __restrict__ Q, int ldq, int q0, int ql, int r0, int r1,
+                                             int col, int t, float scale, uint32_t (&qh)[4][4], uint32_t (&qlo)[4][4]) {
+    const float* p0 = Q + (size_t)(q0 + min(r0, ql - 1)) * ldq + col;
+    const float* p1 = Q + (size_t)(q0 + min(r1, ql - 1)) * ldq + col;
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        const float v[4] = {p0[8 * kk + t] * scale, p1[8 * kk + t] * scale, p0[8 * kk + t + 4] * scale,
+                            p1[8 * kk + t + 4] * scale};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) { qh[kk][e] = tf32_head(v[e]); qlo[kk][e] = tf32_head(v[e] - __uint_as_float(qh[kk][e])); }
+    }
+}
+
+// stage keys [kb, kb + PK) of one head, split into TF32 (hi, lo); zeros beyond the key range
+__device__ __forceinline__ void probs_stage_k(const float* __restrict__ Kp, int ldk, int k0, int kl, int kb, int col,
+                                              float (*sKh)[MLD], float (*sKl)[MLD]) {
+#pragma unroll
+    for (int j = 0; j < (PK * 8) / 128; ++j) {
+        const int f = threadIdx.x + 128 * j, r = f >> 3, c4 = f & 7;
+        float4 kv = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (kb + r < kl) kv = __ldg(reinterpret_cast<const float4*>(Kp + (size_t)(k0 + kb + r) * ldk + col) + c4);
+        const float kx[4] = {kv.x, kv.y, kv.z, kv.w};
+        float kh[4], kl4[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) { kh[e] = __uint_as_float(tf32_head(kx[e])); kl4[e] = __uint_as_float(tf32_head(kx[e] - kh[e])); }
+        *reinterpret_cast<float4*>(&sKh[r][4 * c4]) = make_float4(kh[0], kh[1], kh[2], kh[3]);
+        *reinterpret_cast<float4*>(&sKl[r][4 * c4]) = make_float4(kl4[0], kl4[1], kl4[2], kl4[3]);
+    }
+}
+
+// S = Q K^T over one staged chunk (C fragments: (r0, 2t), (r0, 2t+1), (r1, 2t), (r1, 2t+1) of each 8-key n-tile);
+// keys beyond the range get -inf
+__device__ __forceinline__ void probs_scores(const uint32_t (&qh)[4][4], const uint32_t (&qlo)[4][4],
+                                             const float (*sKh)[MLD], const float (*sKl)[MLD], int g, int t, int kb,
+                                             int kl, float (&S)[8][4]) {
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) S[nt][e] = 0.f;
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t bh0 = __float_as_uint(sKh[8 * nt + g][8 * kk + t]), bh1 = __float_as_uint(sKh[8 * nt + g][8 * kk + t + 4]);
+            const uint32_t bl0 = __float_as_uint(sKl[8 * nt + g][8 * kk + t]), bl1 = __float_as_uint(sKl[8 * nt + g][8 * kk + t + 4]);
+            mma_tf32(S[nt], qlo[kk], bh0, bh1);
+            mma_tf32(S[nt], qh[kk], bl0, bl1);
+            mma_tf32(S[nt], qh[kk], bh0, bh1);
+        }
+        const int key = kb + 8 * nt + 2 * t;
+        if (key >= kl) { S[nt][0] = -INFINITY; S[nt][2] = -INFINITY; }
+        if (key + 1 >= kl) { S[nt][1] = -INFINITY; S[nt][3] = -INFINITY; }
+    }
+}
+
+__global__ void __launch_bounds__(128)
+k_mha_probs_avg(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp, int ldk, float* __restrict__ P,
+                const int64_t* __restrict__ p_offset, const int32_t* __restrict__ p_pitch,
+                const int32_t* __restrict__ q_start, const int32_t* __restrict__ q_len,
+                const int32_t* __restrict__ k_start, const int32_t* __restrict__ k_len, int n_heads, float scale,
+                float inv_heads) {
+    __shared__ __align__(16) float sKh[PK][MLD], sKl[PK][MLD];
+    __shared__ float sM[PH_MAX][PQ], sI[PH_MAX][PQ];
+    const int tile = blockIdx.x, prob = blockIdx.y;
+    const int ql = q_len[prob], kl = k_len[prob];
+    if (tile * PQ >= ql || kl <= 0) return;                 // empty query or key range: nothing is written
+    const int q0 = q_start[prob], k0 = k_start[prob];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const int rl0 = warp * 16 + g, rl1 = rl0 + 8;              // rows inside the tile
+    const int r0 = tile * PQ + rl0, r1 = tile * PQ + rl1;       // rows inside the problem
+    uint32_t qh[4][4], qlo[4][4];
+    float S[8][4];
+
+    // sweep 1: row maximum and sum of every head
+    for (int h = 0; h < n_heads; ++h) {
+        probs_load_q(Q, ldq, q0, ql, r0, r1, h * HD, t, scale, qh, qlo);
+        float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+        for (int kb = 0; kb < kl; kb += PK) {
+            __syncthreads();
+            probs_stage_k(Kp, ldk, k0, kl, kb, h * HD, sKh, sKl);
+            __syncthreads();
+            probs_scores(qh, qlo, sKh, sKl, g, t, kb, kl, S);
+            float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+            for (int nt = 0; nt < 8; ++nt) {
+                mx0 = fmaxf(mx0, fmaxf(S[nt][0], S[nt][1]));
+                mx1 = fmaxf(mx1, fmaxf(S[nt][2], S[nt][3]));
+            }
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+            const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);   // finite: every chunk holds >= 1 valid key
+            l0 *= exp2f(m0 - mn0); l1 *= exp2f(m1 - mn1);            // exp2(-inf) = 0 on the first chunk
+            m0 = mn0; m1 = mn1;
+#pragma unroll
+            for (int nt = 0; nt < 8; ++nt) {
+                l0 += exp2f(S[nt][0] - mn0) + exp2f(S[nt][1] - mn0);
+                l1 += exp2f(S[nt][2] - mn1) + exp2f(S[nt][3] - mn1);
+            }
+        }
+        l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+        l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+        if (t == 0) { sM[h][rl0] = m0; sI[h][rl0] = 1.f / l0; sM[h][rl1] = m1; sI[h][rl1] = 1.f / l1; }
+    }
+
+    // sweep 2: head-averaged probabilities, one key chunk at a time
+    const int64_t base = p_offset[prob];
+    const int pitch = p_pitch[prob];
+    float* row0 = P + base + (int64_t)r0 * pitch;
+    float* row1 = P + base + (int64_t)r1 * pitch;
+    for (int kb = 0; kb < kl; kb += PK) {
+        float acc[8][4];
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) acc[nt][e] = 0.f;
+        for (int h = 0; h < n_heads; ++h) {
+            probs_load_q(Q, ldq, q0, ql, r0, r1, h * HD, t, scale, qh, qlo);
+            __syncthreads();                                   // also orders sweep 1's sM / sI stores before the loads
+            probs_stage_k(Kp, ldk, k0, kl, kb, h * HD, sKh, sKl);
+            __syncthreads();
+            probs_scores(qh, qlo, sKh, sKl, g, t, kb, kl, S);
+            const float m0 = sM[h][rl0], i0 = sI[h][rl0], m1 = sM[h][rl1], i1 = sI[h][rl1];
+#pragma unroll
+            for (int nt = 0; nt < 8; ++nt) {
+                acc[nt][0] = fmaf(exp2f(S[nt][0] - m0), i0, acc[nt][0]);
+                acc[nt][1] = fmaf(exp2f(S[nt][1] - m0), i0, acc[nt][1]);
+                acc[nt][2] = fmaf(exp2f(S[nt][2] - m1), i1, acc[nt][2]);
+                acc[nt][3] = fmaf(exp2f(S[nt][3] - m1), i1, acc[nt][3]);
+            }
+        }
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+            const int key = kb + 8 * nt + 2 * t;
+            if (r0 < ql) {
+                if (key < kl) row0[key] = acc[nt][0] * inv_heads;
+                if (key + 1 < kl) row0[key + 1] = acc[nt][1] * inv_heads;
+            }
+            if (r1 < ql) {
+                if (key < kl) row1[key] = acc[nt][2] * inv_heads;
+                if (key + 1 < kl) row1[key + 1] = acc[nt][3] * inv_heads;
+            }
+        }
+    }
+}
+
 // plan rows (pitch 2B + 1): q_start, q_len, cross k_start, cross k_len for cloud c of a (src x B, tgt x B) stack,
 // then the exclusive prefix of the number of 64-query and 128-query tiles per problem (entry 2B = total): the
 // attention kernels are launched over a LINEAR tile index and find their problem in this table, so that a
@@ -478,6 +632,24 @@ extern "C" int regtr_mha_varlen_fwd_lse(const float* Q, int ldq, const float* K,
     if (!lse) return REGTR_ERR_ARG;
     return mha_varlen_fwd(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, n_problems, max_q_len,
                           nullptr, 0, n_heads, head_dim, scale, lse, (cudaStream_t)stream_);
+}
+
+extern "C" int regtr_mha_probs_avg(const float* Q, int ldq, const float* K, int ldk, float* P,
+                                   const int64_t* p_offset, const int32_t* p_pitch, const int32_t* q_start,
+                                   const int32_t* q_len, const int32_t* k_start, const int32_t* k_len, int n_problems,
+                                   int max_q_len, int n_heads, int head_dim, float scale, void* stream_) {
+    if (n_problems < 0 || max_q_len < 0 || n_heads <= 0) return REGTR_ERR_ARG;
+    if (head_dim != HD || n_heads > PH_MAX) return REGTR_ERR_UNSUPPORTED;
+    if (n_problems == 0 || max_q_len == 0) return REGTR_OK;
+    if (!Q || !K || !P || !p_offset || !p_pitch || !q_start || !q_len || !k_start || !k_len) return REGTR_ERR_ARG;
+    if (ldq % 4 != 0 || ldk % 4 != 0 || ldq < n_heads * HD || ldk < n_heads * HD) return REGTR_ERR_ARG;
+    if (((uintptr_t)Q | (uintptr_t)K) % 16 != 0 || n_problems > 65535) return REGTR_ERR_ARG;
+    const dim3 grid(regtr_cdiv(max_q_len, PQ), n_problems);
+    k_mha_probs_avg<<<grid, 128, 0, (cudaStream_t)stream_>>>(Q, ldq, K, ldk, P, p_offset, p_pitch, q_start, q_len,
+                                                            k_start, k_len, n_heads, scale * 1.4426950408889634f,
+                                                            1.f / (float)n_heads);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
 }
 
 extern "C" int regtr_corr_decode_fwd(const float* Qp, const float* Kp, int ld, const float* xyz, float* out,

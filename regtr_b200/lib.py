@@ -65,6 +65,7 @@ SIGNATURES = {
     'regtr_gemm_tf32x3_qkv_split': (_I, [_P, _I, _P, _P, _I, _P, _I, _I, _I, _I, _F, _P, _I, _P, _I, _P, _P]),
     'regtr_mha_tf32_tc_fwd': (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _P, _P, _P, _I, _I, _P, _I, _I, _I, _P]),
     'regtr_mha_varlen_fwd_lse': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
+    'regtr_mha_probs_avg': (_I, [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     'regtr_mha_varlen_bwd_ws_bytes': (_Z, [_I, _I]),
     'regtr_mha_varlen_bwd': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _I, _P, _I, _P, _I,
                                   _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P, _Z, _P]),

@@ -578,6 +578,33 @@ def mha_varlen(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_heads:
     return out
 
 
+def mha_probs_avg(q, k, out, p_offset, p_pitch, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int):
+    """Head-averaged attention probabilities (1/H) sum_h softmax(q_h k_h^T / sqrt(dh)) of every (query range, key
+    range) problem, written into `out` (flat fp32): problem p's block at p_offset[p] (int64) with row pitch p_pitch[p]
+    (int32).  Elements outside every block are not written.  q / k may be column slices of a wider matrix."""
+    L = _lib.load()
+    for t, nm in ((q, 'q'), (k, 'k')):
+        if not t.is_cuda or t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1:
+            raise ValueError(f'mha_probs_avg: {nm} must be a CUDA fp32 matrix with unit column stride')
+    _chk(out, torch.float32, 'out'); _chk(p_offset, torch.int64, 'p_offset', 1); _chk(p_pitch, torch.int32, 'p_pitch', 1)
+    E = q.shape[1]
+    dh = E // n_heads
+    n_prob = q_start.numel()
+    if p_offset.numel() != n_prob or p_pitch.numel() != n_prob:
+        raise ValueError('mha_probs_avg: one output offset and pitch per problem')
+
+    def launch():
+        return L.regtr_mha_probs_avg(_p(q), q.stride(0), _p(k), k.stride(0), _p(out), _p(p_offset), _p(p_pitch),
+                                     _p(q_start), _p(q_len), _p(k_start), _p(k_len), n_prob, int(max_q_len),
+                                     n_heads, dh, 1.0 / math.sqrt(dh), _stream())
+    if TRACE is not None:
+        ql, kl = q_len.tolist(), k_len.tolist()
+        TRACE.append(('mha_probs', dict(pairs_qk=sum(a * b for a, b in zip(ql, kl)), E=E, tokens=sum(ql)), launch))
+    _lib.check(launch(), 'regtr_mha_probs_avg')
+    _count(1)
+    return out
+
+
 def mha_bf16_tc(x, in_w, in_b, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int, m_dev=None):
     """Attention block core in the fast precision mode: packed in-projection (3xTF32 GEMM, bf16
     epilogue) + wgmma bf16 attention.  x (N,E) fp32 (already LN + pos); returns O (N,E) fp32."""

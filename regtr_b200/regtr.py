@@ -285,6 +285,9 @@ class RegTR(nn.Module):
         encoder backward kernels, and every encoder parameter that requires grad receives one (kernel_points must
         stay frozen, as in the reference); its output is bit-identical to the inference encoder's.
         Exact shapes, eager only."""
+        if self.transformer_encoder.record_attentions:
+            raise RuntimeError('forward_train: attention maps are recorded by the eager inference forward only; set '
+                               'transformer_encoder.record_attentions = False to train')
         self._check_trainable(train_encoder)
         B = len(batch['src_xyz'])
         with torch.no_grad():
@@ -468,6 +471,9 @@ class GraphedRegTR:
         """Enqueue one forward on the current stream (no host synchronisation): copy the clouds into the
         static buffers, replay the graph, start the D2H of (level sizes, status, pose).  Returns a ticket
         for `result`."""
+        if self.model.transformer_encoder.record_attentions:
+            raise RuntimeError('GraphedRegTR: attention maps are recorded by the eager RegTR.forward only (the captured '
+                               'graphs never record them); set transformer_encoder.record_attentions = False')
         src, tgt = batch['src_xyz'], batch['tgt_xyz']
         B = len(src)
         clouds = list(src) + list(tgt)

@@ -17,6 +17,7 @@ reference-style `forward` is kept as a thin adaptor around `forward_packed`.
 from __future__ import annotations
 
 import copy
+import math
 from typing import Optional
 
 import torch
@@ -114,6 +115,11 @@ class AttentionPlan:
             table = torch.tensor(rows, dtype=torch.int32).to(device)
             max_len = max(lens) if n2 else 0
             max_tiles = (t64[-1], t128[-1])
+            self.lens = lens                # host lengths: only plans built from them can record attention maps
+        else:
+            self.lens = None
+        self.map_dims = None                # (Ns, Nt) of the recorded maps; None: the longest src / tgt cloud
+        self._map_tables = None
         n2 = table.shape[1] - 1
         self.q_start, self.q_len = table[0, :n2], table[1, :n2]
         self.xk_start, self.xk_len = table[2, :n2], table[3, :n2]
@@ -129,6 +135,42 @@ class AttentionPlan:
         n2 = 2 * B                          # sum_p ceil(len_p / T) <= capacity / T + number of problems
         return cls(table=ops.attention_plan(offs, B), max_len=max_len, n_dev=offs[2 * B:2 * B + 1],
                    max_tiles=(max_len // 64 + n2, max_len // 128 + n2))
+
+    def map_tables(self, device):
+        """Device (offset, pitch) tables of the self and cross problems into one flat per-layer map buffer, built once
+        per plan (see `attention_map_layout`)."""
+        if self.lens is None:
+            raise RuntimeError('recording attention maps needs host-side cloud lengths (an eager forward); '
+                               'this plan was built on the device')
+        if self._map_tables is None:
+            lay = attention_map_layout(self.lens, *(self.map_dims or (None, None)))
+            dev = lambda v, dt: torch.tensor(v, dtype=dt).to(device)
+            self._map_tables = dict(lay, self_tab=(dev(lay['self_offset'], torch.int64), dev(lay['self_pitch'], torch.int32)),
+                                    cross_tab=(dev(lay['cross_offset'], torch.int64), dev(lay['cross_pitch'], torch.int32)))
+        return self._map_tables
+
+
+def attention_map_layout(lens, Ns=None, Nt=None):
+    """Where the head-averaged attention maps of a (src x B, tgt x B) batch go in one flat buffer, in the reference's
+    padded layout: src_satt (B, Ns, Ns) | tgt_satt (B, Nt, Nt) | src_xatt (B, Ns, Nt) | tgt_xatt (B, Nt, Ns).
+    Ns / Nt default to the longest src / tgt cloud.  Problem c of the plan (cloud c as query, itself or its partner
+    as key) writes its (len_q, len_k) block at `*_offset[c]` with row pitch `*_pitch[c]`; the rest stays as filled.
+    Host only (plain Python): -> dict(self_offset, self_pitch, cross_offset, cross_pitch, shapes, numel, Ns, Nt)."""
+    lens = [int(v) for v in lens]
+    B = len(lens) // 2
+    s, t = lens[:B], lens[B:]
+    Ns = max(s, default=0) if Ns is None else int(Ns)
+    Nt = max(t, default=0) if Nt is None else int(Nt)
+    if any(v > Ns for v in s) or any(v > Nt for v in t):
+        raise ValueError(f'attention_map_layout: cloud lengths {lens} exceed the map sizes ({Ns}, {Nt})')
+    shapes = [(B, Ns, Ns), (B, Nt, Nt), (B, Ns, Nt), (B, Nt, Ns)]
+    base = [0]
+    for sh in shapes:
+        base.append(base[-1] + sh[0] * sh[1] * sh[2])
+    self_off = [base[0] + c * Ns * Ns for c in range(B)] + [base[1] + c * Nt * Nt for c in range(B)]
+    cross_off = [base[2] + c * Ns * Nt for c in range(B)] + [base[3] + c * Nt * Ns for c in range(B)]
+    return dict(self_offset=self_off, self_pitch=[Ns] * B + [Nt] * B, cross_offset=cross_off,
+                cross_pitch=[Nt] * B + [Ns] * B, shapes=shapes, bases=base[:4], numel=base[4], Ns=Ns, Nt=Nt)
 
 
 class TransformerCrossEncoderLayer(nn.Module):
@@ -155,30 +197,59 @@ class TransformerCrossEncoderLayer(nn.Module):
         self.nhead = nhead
         self.normalize_before = normalize_before
         self.sa_val_has_pos_emb, self.ca_val_has_pos_emb = sa_val_has_pos_emb, ca_val_has_pos_emb
-        self.satt_weights, self.xatt_weights = None, None   # analysis only (reference: get_attentions)
+        # analysis only (reference: get_attentions): filled by every forward while record_attentions is on
+        self.satt_weights, self.xatt_weights = None, None
+        self.record_attentions = False
 
     def _attend(self, mha: _MHAParams, x2, x2p, val_has_pos, plan: AttentionPlan, cross: bool):
         E = mha.embed_dim
         W, b = mha.in_proj_weight, mha.in_proj_bias
         ks, kl = (plan.xk_start, plan.xk_len) if cross else (plan.q_start, plan.q_len)
+        nd = plan.n_dev
+        q = k = None
         if self.attention_impl == 'bf16_tc' and val_has_pos:
             # fast mode: in-projection with a bf16 epilogue + wgmma attention core (TMA-fed, register accumulators)
-            return ops.mha_bf16_tc(x2p, W, b, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead,
-                                   m_dev=plan.n_dev)
-        if self.attention_impl == 'tf32_tc' and val_has_pos:
+            o = ops.mha_bf16_tc(x2p, W, b, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead, m_dev=nd)
+        elif self.attention_impl == 'tf32_tc' and val_has_pos:
             # parity mode on the tensor cores: split-epilogue in-projection + TMA-fed wgmma 3xTF32 attention core
-            return ops.mha_tf32_tc(x2p, W, b, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead,
-                                   m_dev=plan.n_dev, tiles=plan.tiles128)
-        nd = plan.n_dev
-        if val_has_pos:
-            qkv = ops.linear(x2p, W, b, m_dev=nd)         # one packed in-projection GEMM
-            q, k, v = qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:]
+            o = ops.mha_tf32_tc(x2p, W, b, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead,
+                                m_dev=nd, tiles=plan.tiles128)
         else:
-            qk = ops.linear(x2p, W[:2 * E], b[:2 * E], m_dev=nd)
-            q, k = qk[:, :E], qk[:, E:]
-            v = ops.linear(x2, W[2 * E:], b[2 * E:], m_dev=nd)
-        o = ops.mha_varlen(q, k, v, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead, tiles=plan.tiles64)
+            if val_has_pos:
+                qkv = ops.linear(x2p, W, b, m_dev=nd)         # one packed in-projection GEMM
+                q, k, v = qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:]
+            else:
+                qk = ops.linear(x2p, W[:2 * E], b[:2 * E], m_dev=nd)
+                q, k = qk[:, :E], qk[:, E:]
+                v = ops.linear(x2, W[2 * E:], b[2 * E:], m_dev=nd)
+            o = ops.mha_varlen(q, k, v, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead, tiles=plan.tiles64)
+        if self.record_attentions:
+            if q is None:
+                # the fused tensor-core in-projections never hold fp32 q and k: project them on the library GEMM (the
+                # maps are then the fp32 attention of the same weights, also under bf16_tc)
+                qk = ops.linear(x2p, W[:2 * E], b[:2 * E], m_dev=nd)
+                q, k = qk[:, :E], qk[:, E:]
+            self._record_map(q, k, plan, cross)
         return o
+
+    def _record_map(self, q, k, plan: AttentionPlan, cross: bool):
+        """Head-averaged probabilities of this attention into a fresh zero-filled buffer in the reference's padded
+        layout (`attention_map_layout`): sets satt_weights after the self attention, xatt_weights after the cross."""
+        tabs = plan.map_tables(q.device)
+        if not cross:       # self attention runs first in both layer variants: one buffer per layer and forward
+            self._map_buf = torch.zeros(tabs['numel'], dtype=torch.float32, device=q.device)
+        buf = self._map_buf
+        off, pitch = tabs['cross_tab' if cross else 'self_tab']
+        ks, kl = (plan.xk_start, plan.xk_len) if cross else (plan.q_start, plan.q_len)
+        ops.mha_probs_avg(q, k, buf, off, pitch, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead)
+        i = 2 if cross else 0
+        views = tuple(buf.narrow(0, tabs['bases'][j], math.prod(tabs['shapes'][j])).view(tabs['shapes'][j])
+                      for j in (i, i + 1))
+        if cross:
+            self.xatt_weights = views
+            del self._map_buf
+        else:
+            self.satt_weights = views
 
     def forward_packed(self, x, pos, plan: AttentionPlan):
         """x, pos: (N,E) packed tokens (src clouds then tgt clouds).  Returns updated x."""
@@ -254,6 +325,34 @@ class TransformerCrossEncoder(nn.Module):
         self.num_layers = num_layers
         self.norm = norm
         self.return_intermediate = return_intermediate
+        self._record_attentions = False
+
+    @property
+    def record_attentions(self) -> bool:
+        """Opt-in analysis switch (off by default).  While on, every eager forward (`forward_packed`, hence
+        `RegTR.forward`, and the padded `forward`) also computes each layer's head-averaged attention maps for
+        `get_attentions()`; the forward's own outputs are unchanged, bit for bit.  Turning it off drops the maps."""
+        return self._record_attentions
+
+    @record_attentions.setter
+    def record_attentions(self, on: bool):
+        self._record_attentions = bool(on)
+        for layer in self.layers:
+            layer.record_attentions = bool(on)
+            if not on:
+                layer.satt_weights, layer.xatt_weights = None, None
+
+    def get_attentions(self):
+        """For analysis: the attention maps of the last recorded forward (transformers.py:61-81), stacked over the
+        layers: ((src_satt, tgt_satt), (src_xatt, tgt_xatt)) of shapes (L, B, Ns, Ns), (L, B, Nt, Nt), (L, B, Ns, Nt),
+        (L, B, Nt, Ns), Ns / Nt the longest src / tgt cloud (the padded length in the padded `forward`).  Each map is
+        the head average of the softmax probabilities; padded key columns and padded query rows are 0.  Under
+        attention_impl='bf16_tc' the maps are the fp32 attention of the same weights, not the bf16 core's own."""
+        if any(layer.satt_weights is None or layer.xatt_weights is None for layer in self.layers):
+            raise RuntimeError('get_attentions: no attention maps recorded; set record_attentions = True on the '
+                               'TransformerCrossEncoder and run a forward first')
+        st = lambda side, which: torch.stack([getattr(layer, which)[side] for layer in self.layers])
+        return (st(0, 'satt_weights'), st(1, 'satt_weights')), (st(0, 'xatt_weights'), st(1, 'xatt_weights'))
 
     def forward_packed(self, x, pos, plan: AttentionPlan):
         """-> (n_out, N, E): final-normed output of every layer (return_intermediate) or the last."""
@@ -269,6 +368,9 @@ class TransformerCrossEncoder(nn.Module):
     def forward_train_packed(self, x, pos, plan: AttentionPlan):
         """Differentiable `forward_packed` (pre-norm layers with a final norm, return_intermediate): -> (L, N, E).
         The final norm of each intermediate output passes x on to the next layer (skip=True)."""
+        if self.record_attentions:
+            raise RuntimeError('attention maps are recorded by the inference forward only; turn record_attentions off '
+                               'to train')
         outs = []
         for layer in self.layers:
             x = layer.forward_train_packed(x, pos, plan)
@@ -299,6 +401,7 @@ class TransformerCrossEncoder(nn.Module):
         if src_pos is not None:
             pos = torch.cat(pack(src_pos, s_lens) + pack(tgt_pos, t_lens), 0).contiguous()
         plan = AttentionPlan(s_lens + t_lens, x.device)
+        plan.map_dims = (src.shape[0], tgt.shape[0])        # recorded maps in the caller's padded sizes
         out = self.forward_packed(x, pos, plan)
         parts = torch.split(out, s_lens + t_lens, dim=1)
         pad = torch.nn.utils.rnn.pad_sequence
