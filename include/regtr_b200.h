@@ -761,6 +761,75 @@ int regtr_circle_finalize_norm(const regtr_loss_args* args, const regtr_circle_a
                                void* stream);
 int regtr_circle_bwd_norm(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm, void* stream);
 
+/* ---- transformer dropout (training) ------------------------------------------------ */
+
+/* The six dropouts of TransformerCrossEncoderLayer.forward_pre in train mode (transformers.py:85-110, 183-244), all
+ * with the same p: site 1 the self-attention probabilities, 2 the self-attention output (dropout1), 3 the cross-
+ * attention probabilities, 4 the cross-attention output (dropout2), 5 relu(linear1) (dropout), 6 the linear2 output
+ * (dropout3).  Masks are regenerated, never stored: the keep decision of (row, column) of a site is a Philox4x32-10
+ * draw keyed by (seed, step, global cloud 2 (pair_base + b) + side, layer, site, head, row, column) -- independent of
+ * the batch size, packing, rank and launch configuration (counter layout: regtr_b200/csrc/philox.cuh).  Row: token
+ * within the (query) cloud; column: key index within the key cloud (sites 1, 3) or feature index (head 0).  Local
+ * cloud c of the (src x B, tgt x B) stack is pair c % B, side c / B (B = n_pairs).  A value is dropped when its 16-bit
+ * draw is below `threshold` = round(p 65536); kept values are multiplied by `scale` = fp32(1 / (1 - p)).  Limits:
+ * 2 (pair_base + n_pairs) <= 2^20, layer < 16, head < 16, clouds shorter than 2^16 tokens.  Passed by host pointer. */
+typedef struct regtr_dropout_args {
+    unsigned long long seed, step;
+    int32_t pair_base;      /* global index of the batch's first pair */
+    int32_t layer;          /* 0..15 */
+    int32_t site;           /* 1..6 */
+    uint32_t threshold;     /* round(p * 65536), <= 65536 */
+    float scale;            /* fp32(1 / (1 - p)) */
+    int32_t n_pairs;        /* B */
+} regtr_dropout_args;
+
+/* Keep mask (analysis / tests): out[r * cols + j] = 1 if row r, column j of local cloud `cloud` (query cloud of an
+ * attention site), head `head`, is kept, for r < rows, j < cols.  out: rows x cols uint8. */
+int regtr_dropout_keep_mask(const regtr_dropout_args* args, int cloud, int head, int rows, int cols, uint8_t* out,
+                            void* stream);
+
+/* regtr_mha_varlen_fwd_lse with the attention-probability dropout (site 1 or 3; the problem tables of
+ * regtr_attention_plan, problem c = query cloud c): O = scale * sum_k m_qk P_qk V_k, the mask applied to the
+ * probabilities in registers before the P V product; lse is that of the undropped probabilities. */
+int regtr_mha_varlen_fwd_lse_dropout(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                                     float* O, int ldo, float* lse, const int32_t* q_start, const int32_t* q_len,
+                                     const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
+                                     int n_heads, int head_dim, float scale, const regtr_dropout_args* drop,
+                                     void* stream);
+
+/* regtr_mha_varlen_bwd of regtr_mha_varlen_fwd_lse_dropout (same arguments plus the mask key): dP_qk becomes
+ * g_qk = m_qk scale (dO_q . V_k), delta = sum_k P g, dV_k = sum_q P_qk m_qk scale dO_q. */
+int regtr_mha_varlen_bwd_dropout(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                                 const float* O, int ldo, const float* dO, int lddo, const float* lse,
+                                 float* dQ, int lddq, float* dK, int lddk, float* dV, int lddv,
+                                 const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
+                                 const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len,
+                                 int n_heads, int head_dim, float scale, const regtr_dropout_args* drop, void* ws,
+                                 size_t ws_bytes, void* stream);
+
+/* Residual dropout fused into the LayerNorm that follows it (sites 2, 4, 6):  x' = x + m scale z  (z: the
+ * out-projection / linear2 output), x_out = x', then regtr_layernorm_pos of x'.  offs (2B + 1, device): cloud
+ * offsets of the packed rows (n = offs[2B]).  x_out must not alias x or z. */
+int regtr_layernorm_pos_dropout(const float* x, const float* z, const float* gamma, const float* beta,
+                                const float* pos, int n, const int32_t* offs, int E, float eps, float* y,
+                                float* y_pos, float* x_out, const regtr_dropout_args* drop, void* stream);
+
+/* Backward of regtr_layernorm_pos_dropout (x = the forward's x_out): dx as regtr_layernorm_bwd (the gradient of
+ * x', dres included), plus dz = dx m scale.  ws: regtr_layernorm_bwd_ws_bytes(n, E). */
+int regtr_layernorm_bwd_dropout(const float* x, const float* gamma, const float* dy, const float* dy_pos,
+                                const float* dres, int n, const int32_t* offs, int E, float eps, float* dx,
+                                float* dz, float* dgamma, float* dbeta, const regtr_dropout_args* drop, void* ws,
+                                size_t ws_bytes, void* stream);
+
+/* Feed-forward dropout (site 5), in place: h[r, j] = m scale h[r, j] over the n x F packed rows of the clouds of
+ * offs (2B + 1, device); max_len: host bound of the cloud lengths. */
+int regtr_dropout_rows(float* h, int n, int F, const int32_t* offs, int max_len, const regtr_dropout_args* drop,
+                       void* stream);
+
+/* ReLU + dropout backward: out = dh * scale where h > 0, else 0 (h: the dropped ReLU output of regtr_dropout_rows,
+ * positive exactly where the ReLU passed and the mask kept). */
+int regtr_relu_dropout_bwd(const float* dh, const float* h, long long n, float scale, float* out, void* stream);
+
 /* ---- status word helpers (device uint32) ------------------------------------------ */
 int regtr_status_clear(uint32_t* status, void* stream);
 

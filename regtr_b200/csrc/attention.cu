@@ -14,6 +14,7 @@
 #include <cstdlib>
 
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace {
 
@@ -140,6 +141,11 @@ k_mha_fp32(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp, i
 //   O += P V:   the C fragment of S is reused as the A fragment of P under the key permutation
 //               (A column t <-> key 2t, column t+4 <-> key 2t+1); B = V[key][d] with the same permutation.
 // Row stride 36 floats makes every fragment LDS bank-conflict free.
+// DROP (training with the attention-probability dropout, regtr_mha_varlen_fwd_lse_dropout): the keep mask multiplies
+// the P fragments in registers before the split for P V, and the output normalisation carries the dropout scale; the
+// row sums l (hence lse) stay those of the undropped probabilities.  Per 64-key chunk every lane draws the blocks of
+// key kb + lane and kb + 32 + lane for the warp's two 8-row groups (4 Philox blocks), and each lane fetches the bits
+// of its two keys per n-tile with two shuffles.
 constexpr int MQ = 64, MK = 64, MLD = 36;
 
 __device__ __forceinline__ uint32_t tf32_head(float x) { return (__float_as_uint(x) + 0x1000u) & 0xffffe000u; }
@@ -150,11 +156,12 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
 }
 __device__ __forceinline__ float fast_exp2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
+template <bool DROP>
 __global__ void __launch_bounds__(128)
 k_mha_tf32x3(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp, int ldk, const float* __restrict__ Vp,
              int ldv, float* __restrict__ O, int ldo, const int32_t* __restrict__ q_start,
              const int32_t* __restrict__ q_len, const int32_t* __restrict__ k_start, const int32_t* __restrict__ k_len,
-             const int32_t* __restrict__ tile_base, int n_prob, float scale, float* __restrict__ lse) {
+             const int32_t* __restrict__ tile_base, int n_prob, float scale, float* __restrict__ lse, DropKey drop) {
     __shared__ __align__(16) float sKh[MK][MLD], sKl[MK][MLD], sVh[MK][MLD], sVl[MK][MLD];
     int prob = blockIdx.z, tile = blockIdx.x;
     const int head = blockIdx.y;
@@ -185,6 +192,8 @@ k_mha_tf32x3(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
 #pragma unroll
         for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    unsigned dw1 = 0, drg = 0;
+    if constexpr (DROP) { dw1 = drop_word1(drop, prob, head); drg = (unsigned)(tile * MQ + warp * 16) >> 3; }
 
     for (int kb = 0; kb < kl; kb += MK) {
         __syncthreads();
@@ -255,6 +264,12 @@ k_mha_tf32x3(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
             l0 += S[nt][0] + S[nt][1];
             l1 += S[nt][2] + S[nt][3];
         }
+        unsigned mk0 = 0, mk1 = 0;              // keys kb + lane, kb + 32 + lane: bits 0-7 rows r0 - g.., 8-15 rows r1 - g..
+        if constexpr (DROP) {
+            const unsigned c0 = (unsigned)(kb + lane), c1 = c0 + 32u;
+            mk0 = drop_keep8(drop, dw1, drg, c0) | (drop_keep8(drop, dw1, drg + 1u, c0) << 8);
+            mk1 = drop_keep8(drop, dw1, drg, c1) | (drop_keep8(drop, dw1, drg + 1u, c1) << 8);
+        }
         // O = O * c + P V.  The chunk's P V is accumulated from zero and added to the running output with a
         // round-to-nearest FMA: the tensor core truncates when it adds into its accumulator, and a chain through
         // every key of a 700-token cloud (264 MMAs) biased the outputs by ~1e-5 relative (tests/diag_accuracy.py).
@@ -266,7 +281,15 @@ k_mha_tf32x3(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt) {
             // A fragment of P: a0 (r0, key 2t) a1 (r1, key 2t) a2 (r0, key 2t+1) a3 (r1, key 2t+1)
-            const float pv[4] = {S[nt][0], S[nt][2], S[nt][1], S[nt][3]};
+            float pv[4] = {S[nt][0], S[nt][2], S[nt][1], S[nt][3]};
+            if constexpr (DROP) {
+                const unsigned ma = __shfl_sync(0xffffffffu, nt < 4 ? mk0 : mk1, (8 * nt + 2 * t) & 31);
+                const unsigned mb = __shfl_sync(0xffffffffu, nt < 4 ? mk0 : mk1, (8 * nt + 2 * t + 1) & 31);
+                if (!((ma >> g) & 1u)) pv[0] = 0.f;
+                if (!((ma >> (8 + g)) & 1u)) pv[1] = 0.f;
+                if (!((mb >> g) & 1u)) pv[2] = 0.f;
+                if (!((mb >> (8 + g)) & 1u)) pv[3] = 0.f;
+            }
             uint32_t ph[4], pl[4];
 #pragma unroll
             for (int e = 0; e < 4; ++e) { ph[e] = tf32_head(pv[e]); pl[e] = tf32_head(pv[e] - __uint_as_float(ph[e])); }
@@ -287,7 +310,8 @@ k_mha_tf32x3(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
     }
     l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
     l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-    const float i0 = l0 > 0.f ? 1.f / l0 : 0.f, i1 = l1 > 0.f ? 1.f / l1 : 0.f;
+    float i0 = l0 > 0.f ? 1.f / l0 : 0.f, i1 = l1 > 0.f ? 1.f / l1 : 0.f;
+    if constexpr (DROP) { i0 *= drop.scale; i1 *= drop.scale; }
     if (lse && t == 0) {                         // base-2 log-sum-exp of the scaled scores (-inf: empty key range)
         const int nh = gridDim.y;
         if (r0 < ql) lse[(size_t)(q0 + r0) * nh + head] = m0 + log2f(l0);
@@ -589,7 +613,7 @@ extern "C" int regtr_attention_plan(const int32_t* offs, int B, int32_t* plan, v
 static int mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, float* O, int ldo,
                           const int32_t* q_start, const int32_t* q_len, const int32_t* k_start, const int32_t* k_len,
                           int n_problems, int max_q_len, const int32_t* tile_base, int max_tiles, int n_heads,
-                          int head_dim, float scale, float* lse, cudaStream_t st) {
+                          int head_dim, float scale, float* lse, cudaStream_t st, const DropKey* drop = nullptr) {
     if (n_problems < 0 || max_q_len < 0 || n_heads <= 0 || max_tiles < 0) return REGTR_ERR_ARG;
     if (head_dim != HD) return REGTR_ERR_UNSUPPORTED;
     if (n_problems == 0 || max_q_len == 0 || (tile_base && max_tiles == 0)) return REGTR_OK;
@@ -601,8 +625,12 @@ static int mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, cons
         // with the tile table: linear 64-query tile index (max_tiles = host bound of the total); else one grid
         // column per problem sized by the longest sequence
         const dim3 grid = tile_base ? dim3(max_tiles, n_heads, 1) : dim3(regtr_cdiv(max_q_len, MQ), n_heads, n_problems);
-        k_mha_tf32x3<<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, tile_base,
-                                          n_problems, scale * 1.4426950408889634f, lse);
+        if (drop)
+            k_mha_tf32x3<true><<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len,
+                                                     tile_base, n_problems, scale * 1.4426950408889634f, lse, *drop);
+        else
+            k_mha_tf32x3<false><<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len,
+                                                      tile_base, n_problems, scale * 1.4426950408889634f, lse, DropKey{});
         REGTR_CHECK_LAUNCH();
         return REGTR_OK;
     }
@@ -632,6 +660,17 @@ extern "C" int regtr_mha_varlen_fwd_lse(const float* Q, int ldq, const float* K,
     if (!lse) return REGTR_ERR_ARG;
     return mha_varlen_fwd(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, n_problems, max_q_len,
                           nullptr, 0, n_heads, head_dim, scale, lse, (cudaStream_t)stream_);
+}
+
+extern "C" int regtr_mha_varlen_fwd_lse_dropout(const float* Q, int ldq, const float* K, int ldk, const float* V,
+                                                int ldv, float* O, int ldo, float* lse, const int32_t* q_start,
+                                                const int32_t* q_len, const int32_t* k_start, const int32_t* k_len,
+                                                int n_problems, int max_q_len, int n_heads, int head_dim, float scale,
+                                                const regtr_dropout_args* drop, void* stream_) {
+    DropKey dk;
+    if (!lse || drop_key_of(drop, dk) != REGTR_OK || n_heads > 16 || 2 * drop->n_pairs != n_problems) return REGTR_ERR_ARG;
+    return mha_varlen_fwd(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, n_problems, max_q_len,
+                          nullptr, 0, n_heads, head_dim, scale, lse, (cudaStream_t)stream_, &dk);
 }
 
 extern "C" int regtr_mha_probs_avg(const float* Q, int ldq, const float* K, int ldk, float* P,

@@ -5,6 +5,7 @@
 // (paths relative to /root/reference/src).  Every reduction runs in a fixed order with no atomics: two backward
 // passes over the same inputs are bit-identical.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace {
 
@@ -84,12 +85,17 @@ __device__ __forceinline__ void two_sum_add(float& s, float& c, float x) {
 // memory, twice.  dS = P * (dP - delta) with dP = dO . v;  dQ = scale * sum_k dS k.  delta and 1 / Z are stored for
 // pass 2.  Every query row belongs to exactly one problem, so every dQ row is written exactly once.  A problem with an
 // empty key range has Z = 0 and writes dQ = 0.
+// DROP (attention-probability dropout, the regtr_mha_varlen_fwd_lse_dropout forward): dP = dO . v becomes
+// g = m * scale * dP in both sweeps, so D = sum_k p g and delta = D / Z are formed from the very g the second sweep
+// uses and sum_k dS = 0 still holds in this arithmetic.  The 8 threads of an aligned 8-query group share one Philox
+// block per key: per 8 keys each draws the block of one key and the bits are passed round with one shuffle per key.
+template <bool DROP>
 __global__ void __launch_bounds__(BT)
 k_mha_bwd_dq(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp, int ldk, const float* __restrict__ Vp,
              int ldv, const float* __restrict__ dO, int lddo, const float* __restrict__ lse, float* __restrict__ delta,
              float* __restrict__ rnorm, float* __restrict__ dQ, int lddq, const int32_t* __restrict__ q_start,
              const int32_t* __restrict__ q_len, const int32_t* __restrict__ k_start, const int32_t* __restrict__ k_len,
-             float qscale, float scale) {
+             float qscale, float scale, DropKey drop) {
     __shared__ __align__(16) float sK[CH][HD], sV[CH][HD];
     const int prob = blockIdx.z, head = blockIdx.y, tile = blockIdx.x, nh = gridDim.y;
     const int ql = q_len[prob];
@@ -107,6 +113,54 @@ k_mha_bwd_dq(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
 
     // compensated sums (TwoSum, and TwoProduct for p * dP): Z and D to about one rounding, whatever the key count
     float z = 0.f, zc = 0.f, dsum = 0.f, dc = 0.f;
+    if constexpr (DROP) {
+        const unsigned w1 = drop_word1(drop, prob, head), rg = (unsigned)qi >> 3, u = threadIdx.x & 7;
+        const int gl = threadIdx.x & 24;                 // first lane of this thread's 8-query group
+        for (int kb = 0; kb < kl; kb += CH) {
+            const int nk = min(CH, kl - kb);
+            __syncthreads();
+            stage_kv(sK, sV, Kp, ldk, Vp, ldv, (size_t)(k0 + kb), nk, col);
+            __syncthreads();
+            for (int j0 = 0; j0 < nk; j0 += 8) {
+                const unsigned mine = drop_keep8(drop, w1, rg, (unsigned)(kb + j0) + u);
+                for (int jj = 0; jj < 8 && j0 + jj < nk; ++jj) {
+                    const int j = j0 + jj;
+                    const unsigned mb = __shfl_sync(0xffffffffu, mine, gl | jj);
+                    const float p = fast_exp2(dot_smem(q, &sK[j][0]) - L);
+                    two_sum_add(z, zc, p);
+                    const float dp = ((mb >> u) & 1u) ? __fmul_rn(dot_smem(g, &sV[j][0]), drop.scale) : 0.f;
+                    const float pr = __fmul_rn(p, dp);
+                    dc += fmaf(p, dp, -pr);
+                    two_sum_add(dsum, dc, pr);
+                }
+            }
+        }
+        z += zc;
+        dsum += dc;
+        const float rz = z > 0.f ? 1.f / z : 0.f;
+        const float dl = z > 0.f ? dsum / z : 0.f;
+        if (active) { delta[row * nh + head] = dl; rnorm[row * nh + head] = rz; }
+#pragma unroll
+        for (int d = 0; d < HD; ++d) acc[d] = 0.f;
+        for (int kb = 0; kb < kl; kb += CH) {
+            const int nk = min(CH, kl - kb);
+            __syncthreads();
+            stage_kv(sK, sV, Kp, ldk, Vp, ldv, (size_t)(k0 + kb), nk, col);
+            __syncthreads();
+            for (int j0 = 0; j0 < nk; j0 += 8) {
+                const unsigned mine = drop_keep8(drop, w1, rg, (unsigned)(kb + j0) + u);
+                for (int jj = 0; jj < 8 && j0 + jj < nk; ++jj) {
+                    const int j = j0 + jj;
+                    const unsigned mb = __shfl_sync(0xffffffffu, mine, gl | jj);
+                    const float p = fast_exp2(dot_smem(q, &sK[j][0]) - L);
+                    const float dp = ((mb >> u) & 1u) ? __fmul_rn(dot_smem(g, &sV[j][0]), drop.scale) : 0.f;
+                    axpy_smem(acc, p * (dp - dl), &sK[j][0]);
+                }
+            }
+        }
+        if (active) store_row(dQ + (size_t)(q0 + qi) * lddq + col, acc, scale * rz);
+        return;
+    }
     for (int kb = 0; kb < kl; kb += CH) {
         const int nk = min(CH, kl - kb);
         __syncthreads();
@@ -149,12 +203,15 @@ k_mha_bwd_dq(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
 // holds it.  In the self table each token is a key of exactly one problem (its own cloud); in the cross table each
 // cloud is the key range of exactly one problem (its partner's).  Callers with other tables must keep the key
 // ranges disjoint.  A key range whose problem has no queries gets dK = dV = 0.
+// DROP: dV = sum_q m scale P dO and dP -> g = m scale dP; each thread draws one Philox block per 8 queries of its key.
+template <bool DROP>
 __global__ void __launch_bounds__(BT)
 k_mha_bwd_dkv(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp, int ldk, const float* __restrict__ Vp,
               int ldv, const float* __restrict__ dO, int lddo, const float* __restrict__ lse,
               const float* __restrict__ delta, const float* __restrict__ rnorm, float* __restrict__ dK, int lddk,
               float* __restrict__ dV, int lddv, const int32_t* __restrict__ q_start, const int32_t* __restrict__ q_len,
-              const int32_t* __restrict__ k_start, const int32_t* __restrict__ k_len, float qscale, float kscale) {
+              const int32_t* __restrict__ k_start, const int32_t* __restrict__ k_len, float qscale, float kscale,
+              DropKey drop) {
     __shared__ __align__(16) float sQ[CH][HD], sG[CH][HD];
     __shared__ float sL[CH], sD[CH], sR[CH];
     const int prob = blockIdx.z, head = blockIdx.y, tile = blockIdx.x, nh = gridDim.y;
@@ -189,6 +246,21 @@ k_mha_bwd_dkv(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp
             sR[threadIdx.x] = rnorm[qr * nh + head];
         }
         __syncthreads();
+        if constexpr (DROP) {
+            const unsigned w1 = drop_word1(drop, prob, head);
+            for (int i0 = 0; i0 < nq; i0 += 8) {
+                const unsigned mb = drop_keep8(drop, w1, (unsigned)(qb + i0) >> 3, (unsigned)kj);
+                for (int ii = 0; ii < 8 && i0 + ii < nq; ++ii) {
+                    const int i = i0 + ii;
+                    const bool keep = (mb >> ii) & 1u;
+                    const float p = fast_exp2(dot_smem(k, &sQ[i][0]) - sL[i]) * sR[i];
+                    axpy_smem(dv, keep ? __fmul_rn(p, drop.scale) : 0.f, &sG[i][0]);
+                    const float dp = keep ? __fmul_rn(dot_smem(v, &sG[i][0]), drop.scale) : 0.f;
+                    axpy_smem(dk, p * (dp - sD[i]), &sQ[i][0]);
+                }
+            }
+            continue;
+        }
         for (int i = 0; i < nq; ++i) {
             const float p = fast_exp2(dot_smem(k, &sQ[i][0]) - sL[i]) * sR[i];
             axpy_smem(dv, p, &sG[i][0]);
@@ -210,10 +282,13 @@ k_mha_bwd_dkv(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp
 // partials, the block adds its 8 warps in order and stores one partial row; k_colsum adds the blocks in order.
 constexpr int LNB_WARPS = 8, LNB_ROWS = 64, LN_PER = 8;     // E <= 32 * LN_PER = 256
 
+// DROP (regtr_layernorm_bwd_dropout): also dz = dx * m * scale, the gradient of the dropped residual branch.
+template <bool DROP>
 __global__ void __launch_bounds__(32 * LNB_WARPS)
 k_layernorm_bwd(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ dy,
                 const float* __restrict__ dyp, const float* __restrict__ dres, int n, int E, float eps,
-                float* __restrict__ dx, float* __restrict__ part) {
+                float* __restrict__ dx, float* __restrict__ part, float* __restrict__ dz,
+                const int32_t* __restrict__ offs, DropKey drop) {
     __shared__ float red[LNB_WARPS][2][32 * LN_PER];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, per = E / 32;
     float gm[LN_PER], ag[LN_PER], ab[LN_PER];
@@ -248,6 +323,12 @@ k_layernorm_bwd(const float* __restrict__ x, const float* __restrict__ gamma, co
                 ag[j] = fmaf(g[j], v[j], ag[j]); ab[j] += g[j];
             }
         s1 = warp_sum(s1) / (float)E; s2 = warp_sum(s2) / (float)E;
+        unsigned w1 = 0, rr = 0;
+        if constexpr (DROP) {
+            const int c = regtr_cloud_of(offs, 2 * drop.n_pairs, row);
+            w1 = drop_word1(drop, c, 0);
+            rr = (unsigned)(row - offs[c]);
+        }
 #pragma unroll
         for (int j = 0; j < LN_PER; ++j)
             if (j < per) {
@@ -255,6 +336,7 @@ k_layernorm_bwd(const float* __restrict__ x, const float* __restrict__ gamma, co
                 float d = rstd * (g[j] * gm[j] - s1 - v[j] * s2);
                 if (dres) d += dres[o + c];
                 dx[o + c] = d;
+                if constexpr (DROP) dz[o + c] = drop_keep(drop, w1, rr, (unsigned)c) ? __fmul_rn(d, drop.scale) : 0.f;
             }
     }
 #pragma unroll
@@ -285,6 +367,13 @@ __global__ void k_colsum(const float* __restrict__ part, int n_blocks, int ld, i
 __global__ void k_relu_bwd(const float* __restrict__ dh, const float* __restrict__ h, long long n, float* __restrict__ out) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = h[i] > 0.f ? dh[i] : 0.f;
+}
+
+// ReLU + dropout (site 5): h is the dropped ReLU output, positive exactly where the ReLU passed and the mask kept
+__global__ void k_relu_dropout_bwd(const float* __restrict__ dh, const float* __restrict__ h, long long n, float scale,
+                                   float* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = h[i] > 0.f ? __fmul_rn(dh[i], scale) : 0.f;
 }
 
 __device__ __forceinline__ float tf32_rn(float x) {
@@ -354,12 +443,11 @@ size_t regtr_mha_varlen_bwd_ws_bytes(int n_rows, int n_heads) {
     return regtr_align(2 * (size_t)(n_rows > 0 ? n_rows : 1) * (size_t)(n_heads > 0 ? n_heads : 1) * sizeof(float));
 }
 
-int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, const float* O,
-                         int ldo, const float* dO, int lddo, const float* lse, float* dQ, int lddq, float* dK, int lddk,
-                         float* dV, int lddv, const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
-                         const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len, int n_heads,
-                         int head_dim, float scale, void* ws, size_t ws_bytes, void* stream_) {
-    cudaStream_t st = (cudaStream_t)stream_;
+static int mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, const float* O,
+                          int ldo, const float* dO, int lddo, const float* lse, float* dQ, int lddq, float* dK, int lddk,
+                          float* dV, int lddv, const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
+                          const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len, int n_heads,
+                          int head_dim, float scale, void* ws, size_t ws_bytes, cudaStream_t st, const DropKey* drop) {
     if (n_problems < 0 || n_rows < 0 || max_q_len < 0 || max_k_len < 0 || n_heads <= 0) return REGTR_ERR_ARG;
     if (head_dim != HD) return REGTR_ERR_UNSUPPORTED;
     if (n_problems == 0 || n_rows == 0) return REGTR_OK;
@@ -372,17 +460,49 @@ int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const
     float* rnorm = delta + (size_t)n_rows * n_heads;
     const float qscale = scale * 1.4426950408889634f;
     if (max_q_len > 0) {
-        k_mha_bwd_dq<<<dim3(regtr_cdiv(max_q_len, BT), n_heads, n_problems), BT, 0, st>>>(
-            Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dQ, lddq, q_start, q_len, k_start, k_len, qscale, scale);
+        const dim3 grid(regtr_cdiv(max_q_len, BT), n_heads, n_problems);
+        if (drop)
+            k_mha_bwd_dq<true><<<grid, BT, 0, st>>>(Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dQ, lddq, q_start,
+                                                    q_len, k_start, k_len, qscale, scale, *drop);
+        else
+            k_mha_bwd_dq<false><<<grid, BT, 0, st>>>(Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dQ, lddq, q_start,
+                                                     q_len, k_start, k_len, qscale, scale, DropKey{});
         REGTR_CHECK_LAUNCH();
     }
     if (max_k_len > 0) {
-        k_mha_bwd_dkv<<<dim3(regtr_cdiv(max_k_len, BT), n_heads, n_problems), BT, 0, st>>>(
-            Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dK, lddk, dV, lddv, q_start, q_len, k_start, k_len,
-            qscale, LN2);
+        const dim3 grid(regtr_cdiv(max_k_len, BT), n_heads, n_problems);
+        if (drop)
+            k_mha_bwd_dkv<true><<<grid, BT, 0, st>>>(Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dK, lddk, dV,
+                                                     lddv, q_start, q_len, k_start, k_len, qscale, LN2, *drop);
+        else
+            k_mha_bwd_dkv<false><<<grid, BT, 0, st>>>(Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dK, lddk, dV,
+                                                      lddv, q_start, q_len, k_start, k_len, qscale, LN2, DropKey{});
         REGTR_CHECK_LAUNCH();
     }
     return REGTR_OK;
+}
+
+int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, const float* O,
+                         int ldo, const float* dO, int lddo, const float* lse, float* dQ, int lddq, float* dK, int lddk,
+                         float* dV, int lddv, const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
+                         const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len, int n_heads,
+                         int head_dim, float scale, void* ws, size_t ws_bytes, void* stream_) {
+    return mha_varlen_bwd(Q, ldq, K, ldk, V, ldv, O, ldo, dO, lddo, lse, dQ, lddq, dK, lddk, dV, lddv, q_start, q_len,
+                          k_start, k_len, n_problems, n_rows, max_q_len, max_k_len, n_heads, head_dim, scale, ws,
+                          ws_bytes, (cudaStream_t)stream_, nullptr);
+}
+
+int regtr_mha_varlen_bwd_dropout(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                                 const float* O, int ldo, const float* dO, int lddo, const float* lse, float* dQ,
+                                 int lddq, float* dK, int lddk, float* dV, int lddv, const int32_t* q_start,
+                                 const int32_t* q_len, const int32_t* k_start, const int32_t* k_len, int n_problems,
+                                 int n_rows, int max_q_len, int max_k_len, int n_heads, int head_dim, float scale,
+                                 const regtr_dropout_args* drop, void* ws, size_t ws_bytes, void* stream_) {
+    DropKey dk;
+    if (drop_key_of(drop, dk) != REGTR_OK || n_heads > 16 || 2 * drop->n_pairs != n_problems) return REGTR_ERR_ARG;
+    return mha_varlen_bwd(Q, ldq, K, ldk, V, ldv, O, ldo, dO, lddo, lse, dQ, lddq, dK, lddk, dV, lddv, q_start, q_len,
+                          k_start, k_len, n_problems, n_rows, max_q_len, max_k_len, n_heads, head_dim, scale, ws,
+                          ws_bytes, (cudaStream_t)stream_, &dk);
 }
 
 size_t regtr_layernorm_bwd_ws_bytes(int n, int E) {
@@ -400,10 +520,42 @@ int regtr_layernorm_bwd(const float* x, const float* gamma, const float* dy, con
     float* part = (float*)ws;
     const int nb = n > 0 ? regtr_cdiv(n, LNB_ROWS) : 0;
     if (nb > 0) {
-        k_layernorm_bwd<<<nb, 32 * LNB_WARPS, 0, st>>>(x, gamma, dy, dy_pos, dres, n, E, eps, dx, part);
+        k_layernorm_bwd<false><<<nb, 32 * LNB_WARPS, 0, st>>>(x, gamma, dy, dy_pos, dres, n, E, eps, dx, part, nullptr,
+                                                              nullptr, DropKey{});
         REGTR_CHECK_LAUNCH();
     }
     k_colsum<<<regtr_cdiv(2 * E, 256), 256, 0, st>>>(part, nb, 2 * E, 2 * E, dgamma, E, dbeta);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_layernorm_bwd_dropout(const float* x, const float* gamma, const float* dy, const float* dy_pos,
+                                const float* dres, int n, const int32_t* offs, int E, float eps, float* dx, float* dz,
+                                float* dgamma, float* dbeta, const regtr_dropout_args* drop, void* ws, size_t ws_bytes,
+                                void* stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    DropKey dk;
+    if (drop_key_of(drop, dk) != REGTR_OK) return REGTR_ERR_ARG;
+    if (n < 0 || E <= 0 || E % 32 != 0) return REGTR_ERR_ARG;
+    if (E > 32 * LN_PER) return REGTR_ERR_UNSUPPORTED;
+    if (!x || !gamma || !dx || !dz || !dgamma || !dbeta || !offs) return REGTR_ERR_ARG;
+    if (!ws || ws_bytes < regtr_layernorm_bwd_ws_bytes(n, E)) return REGTR_ERR_WORKSPACE;
+    float* part = (float*)ws;
+    const int nb = n > 0 ? regtr_cdiv(n, LNB_ROWS) : 0;
+    if (nb > 0) {
+        k_layernorm_bwd<true><<<nb, 32 * LNB_WARPS, 0, st>>>(x, gamma, dy, dy_pos, dres, n, E, eps, dx, part, dz, offs, dk);
+        REGTR_CHECK_LAUNCH();
+    }
+    k_colsum<<<regtr_cdiv(2 * E, 256), 256, 0, st>>>(part, nb, 2 * E, 2 * E, dgamma, E, dbeta);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_relu_dropout_bwd(const float* dh, const float* h, long long n, float scale, float* out, void* stream_) {
+    if (n < 0) return REGTR_ERR_ARG;
+    if (n == 0) return REGTR_OK;
+    if (!dh || !h || !out) return REGTR_ERR_ARG;
+    k_relu_dropout_bwd<<<regtr_cdiv(n, 256), 256, 0, (cudaStream_t)stream_>>>(dh, h, n, scale, out);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
 }

@@ -4,6 +4,7 @@
 //   3-D sine position embedding                        -- position_embedding.py:29-50
 // (paths relative to /root/reference/src)
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace {
 
@@ -189,13 +190,16 @@ __global__ void k_in_apply(const float* x, const int32_t* __restrict__ offs, int
 }
 
 // One warp per row; E = 32 * per <= 32 * PER (PER = 8: the model width 256; PER = 32: anything up to 1024).
-template <int PER>
+// DROP (regtr_layernorm_pos_dropout): the row is first x + m * scale * z (the residual add of a dropped branch),
+// written to x_out, and normalised from there.
+template <int PER, bool DROP = false>
 __global__ void k_layernorm_pos(const float* __restrict__ x, const float* __restrict__ gamma,
                                 const float* __restrict__ beta, const float* __restrict__ pos, int n,
                                 const int32_t* __restrict__ n_dev, int E, float eps, float* __restrict__ y,
-                                float* __restrict__ y_pos) {
+                                float* __restrict__ y_pos, const float* __restrict__ z = nullptr,
+                                float* __restrict__ x_out = nullptr, DropKey drop = DropKey{}) {
     const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (n_dev) n = min(n, *n_dev);               // capacity-shaped launch: rows beyond the real count are skipped
+    if (!DROP && n_dev) n = min(n, *n_dev);               // capacity-shaped launch: rows beyond the real count are skipped
     if (row >= n) return;
     const float* xr = x + (size_t)row * E;
     const int per = E / 32;
@@ -208,6 +212,18 @@ __global__ void k_layernorm_pos(const float* __restrict__ x, const float* __rest
             v[j] = xr[c]; gm[j] = __ldg(gamma + c); bt[j] = __ldg(beta + c);
             ps[j] = (y_pos && pos) ? pos[(size_t)row * E + c] : 0.f;
         }
+    if constexpr (DROP) {               // n_dev carries the cloud offsets here
+        const int cl = regtr_cloud_of(n_dev, 2 * drop.n_pairs, row);
+        const unsigned w1 = drop_word1(drop, cl, 0), rr = (unsigned)(row - n_dev[cl]);
+#pragma unroll
+        for (int j = 0; j < PER; ++j)
+            if (j < per) {
+                const int c = j * 32 + lane;
+                const float zv = z[(size_t)row * E + c];
+                v[j] = __fadd_rn(v[j], drop_keep(drop, w1, rr, (unsigned)c) ? __fmul_rn(zv, drop.scale) : 0.f);
+                x_out[(size_t)row * E + c] = v[j];
+            }
+    }
     float s = 0.f;
 #pragma unroll
     for (int j = 0; j < PER; ++j) if (j < per) s += v[j];
@@ -326,6 +342,25 @@ int regtr_layernorm_pos(const float* x, const float* gamma, const float* beta, c
         k_layernorm_pos<8><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, n_dev, E, eps, y, y_pos);
     else
         k_layernorm_pos<32><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, n_dev, E, eps, y, y_pos);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_layernorm_pos_dropout(const float* x, const float* z, const float* gamma, const float* beta,
+                                const float* pos, int n, const int32_t* offs, int E, float eps, float* y,
+                                float* y_pos, float* x_out, const regtr_dropout_args* drop, void* stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    DropKey dk;
+    if (drop_key_of(drop, dk) != REGTR_OK) return REGTR_ERR_ARG;
+    if (n < 0 || E <= 0 || E % 32 != 0 || E > 1024) return REGTR_ERR_ARG;
+    if (n == 0) return REGTR_OK;
+    if (!x || !z || !gamma || !beta || !offs || !x_out || (!y && !y_pos) || x_out == x || x_out == z) return REGTR_ERR_ARG;
+    if (E <= 256)
+        k_layernorm_pos<8, true><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, offs, E, eps,
+                                                                                     y, y_pos, z, x_out, dk);
+    else
+        k_layernorm_pos<32, true><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, offs, E,
+                                                                                      eps, y, y_pos, z, x_out, dk);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
 }

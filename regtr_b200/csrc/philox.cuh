@@ -3,6 +3,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "../../include/regtr_b200.h"
+
 namespace {
 
 // ------------------------------------------------------------------------------------------- counter-based randomness
@@ -83,5 +85,58 @@ __device__ __forceinline__ unsigned perm_inv(const Perm& p, unsigned y) {
 }
 
 __device__ __forceinline__ double u01(unsigned v) { return ((double)v + 0.5) * 2.3283064365386963e-10; }   // (0, 1)
+
+// ------------------------------------------------------------------------------------------ transformer dropout
+// Keep decisions of the cross-encoder's six dropouts (regtr_dropout_args in include/regtr_b200.h).  Same Philox key
+// and counter words 2..3 as the augmentation draws of (seed, step); the streams are told apart by counter word 1:
+//   augmentation   c = (index,                 2 pair + side                        , step lo, step hi)   c1 < 2^31
+//   dropout        c = (row group << 16 | col,  2^31 | cloud << 11 | layer << 7 | site << 4 | head, step lo, step hi)
+// with cloud = 2 (pair_base + b) + side the GLOBAL cloud index, row / col the row within the (query) cloud and the
+// column (key index within the key cloud, or feature index), row group = row / 8.  One Philox block holds the
+// decisions of 8 consecutive rows of one column, 16 bits each: row 8 rg + r reads half (r & 1) of word r >> 1 and is
+// kept when that 16-bit value is >= threshold = round(p 65536).  The attention passes use a whole block at a time:
+// the key-major dK / dV pass owns a column and walks the rows; the query-major passes have 8 lanes draw 8 columns
+// and swap them with shuffles.  The elementwise sites (the LayerNorm prologue and its backward, one warp per row)
+// draw one block per element and use 1/8 of it: 256 blocks per 256-wide row, which costs a few microseconds per
+// launch at the model's token counts; the feed-forward dropout has a thread own 8 rows and uses whole blocks.
+// Fields: cloud < 2^20, layer < 16, site 1..6, head < 16, row < 2^19, col < 2^16.
+struct DropKey {
+    Keys ks;
+    unsigned thr;           // round(p * 65536)
+    float scale;            // fp32(1 / (1 - p))
+    int pair_base, n_pairs, layer, site;
+};
+
+// counter word 1 of local cloud c (plan order: src clouds 0..B-1, then tgt clouds)
+__device__ __forceinline__ unsigned drop_word1(const DropKey& d, int c, int head) {
+    const unsigned cloud = 2u * (unsigned)(d.pair_base + c % d.n_pairs) + (unsigned)(c / d.n_pairs);
+    return 0x80000000u | (cloud << 11) | ((unsigned)d.layer << 7) | ((unsigned)d.site << 4) | (unsigned)head;
+}
+
+// bit r set: row 8 rg + r of column col is kept
+__device__ __forceinline__ unsigned drop_keep8(const DropKey& d, unsigned w1, unsigned rg, unsigned col) {
+    const U4 v = philox(U4{(rg << 16) | col, w1, d.ks.s0, d.ks.s1}, d.ks.k0, d.ks.k1);
+    const unsigned w[4] = {v.x, v.y, v.z, v.w};
+    unsigned m = 0;
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+        m |= ((unsigned)((w[e] & 0xffffu) >= d.thr) << (2 * e)) | ((unsigned)((w[e] >> 16) >= d.thr) << (2 * e + 1));
+    return m;
+}
+
+__device__ __forceinline__ bool drop_keep(const DropKey& d, unsigned w1, unsigned row, unsigned col) {
+    return (drop_keep8(d, w1, row >> 3, col) >> (row & 7u)) & 1u;
+}
+
+// host: REGTR_OK and the kernel-side key, or REGTR_ERR_ARG for fields outside the counter layout
+static inline int drop_key_of(const regtr_dropout_args* a, DropKey& d) {
+    if (!a || a->pair_base < 0 || a->n_pairs <= 0 || 2ll * (a->pair_base + a->n_pairs) > (1ll << 20)) return REGTR_ERR_ARG;
+    if (a->layer < 0 || a->layer > 15 || a->site < 1 || a->site > 6 || a->threshold > 65536u) return REGTR_ERR_ARG;
+    d.ks = Keys{(unsigned)a->seed, (unsigned)(a->seed >> 32), (unsigned)a->step, (unsigned)(a->step >> 32)};
+    d.thr = a->threshold;
+    d.scale = a->scale;
+    d.pair_base = a->pair_base; d.n_pairs = a->n_pairs; d.layer = a->layer; d.site = a->site;
+    return REGTR_OK;
+}
 
 }  // namespace

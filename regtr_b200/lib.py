@@ -125,6 +125,15 @@ SIGNATURES = {
     'regtr_circle_bwd': (_I, [_P, _P, _P]),
     'regtr_circle_finalize_norm': (_I, [_P, _P, _P, _P]),
     'regtr_circle_bwd_norm': (_I, [_P, _P, _P, _P]),
+    'regtr_dropout_keep_mask': (_I, [_P, _I, _I, _I, _I, _P, _P]),
+    'regtr_mha_varlen_fwd_lse_dropout': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F,
+                                              _P, _P]),
+    'regtr_mha_varlen_bwd_dropout': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _I, _P, _I, _P, _I,
+                                          _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P, _P, _Z, _P]),
+    'regtr_layernorm_pos_dropout': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _F, _P, _P, _P, _P, _P]),
+    'regtr_layernorm_bwd_dropout': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _F, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    'regtr_dropout_rows': (_I, [_P, _I, _I, _P, _I, _P, _P]),
+    'regtr_relu_dropout_bwd': (_I, [_P, _P, _c.c_longlong, _F, _P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),
 }
 

@@ -7,8 +7,10 @@ Tensors must live on a CUDA device; there is no CPU fallback.
 from __future__ import annotations
 
 import contextlib
+import ctypes
 import itertools
 import math
+import os
 
 import numpy as np
 import torch
@@ -819,6 +821,259 @@ class _MHAPackedFn(torch.autograd.Function):
         mha_varlen_bwd(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], o, lse, g.contiguous(), d[:, :E], d[:, E:2 * E],
                        d[:, 2 * E:], qs, ql, ks, kl, ctx.max_len, ctx.max_len, ctx.n_heads)
         return d, None, None, None, None, None, None
+
+
+# ------------------------------------------------------------------ transformer dropout (training)
+# The six dropouts of TransformerCrossEncoderLayer.forward_pre (transformers.py:183-244), numbered as in
+# include/regtr_b200.h: masks are regenerated from (seed, step, global cloud, layer, site, head, row, column), never
+# stored (keep rule: csrc/philox.cuh).
+SITE_SELF_ATTN, SITE_SELF_OUT, SITE_CROSS_ATTN, SITE_CROSS_OUT, SITE_FFN, SITE_FFN_OUT = 1, 2, 3, 4, 5, 6
+
+
+class _DropoutArgs(ctypes.Structure):
+    _fields_ = [('seed', ctypes.c_ulonglong), ('step', ctypes.c_ulonglong), ('pair_base', ctypes.c_int32),
+                ('layer', ctypes.c_int32), ('site', ctypes.c_int32), ('threshold', ctypes.c_uint32),
+                ('scale', ctypes.c_float), ('n_pairs', ctypes.c_int32)]
+
+
+def dropout_threshold(p: float) -> int:
+    """16-bit drop threshold: a value is dropped when its draw (0..65535) is below round(p * 65536)."""
+    return int(round(float(p) * 65536.0))
+
+
+def dropout_scale(p: float) -> float:
+    """The fp32 value of 1 / (1 - p) that kept values are multiplied by."""
+    return float(np.float32(1.0 / (1.0 - float(p))))
+
+
+class DropoutKey:
+    """The dropout masks of one training step of a (src x B, tgt x B) batch whose first pair is global pair
+    `pair_base`: `args(layer, site)` is the C argument block of one site.  `offs` (2B + 1 int32, device) are the cloud
+    offsets of the packed tokens and `max_len` a host bound of the cloud lengths (the elementwise sites need them)."""
+
+    def __init__(self, p: float, seed: int, step: int, pair_base: int, n_pairs: int, offs=None, max_len: int = 0):
+        if not 0.0 < float(p) < 1.0:
+            raise ValueError(f'DropoutKey: p={p} outside (0, 1)')
+        self.p, self.seed, self.step = float(p), int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1)
+        self.pair_base, self.n_pairs = int(pair_base), int(n_pairs)
+        self.threshold, self.scale = dropout_threshold(p), dropout_scale(p)
+        self.offs, self.max_len = offs, int(max_len)
+        if self.max_len >= 1 << 16:
+            raise ValueError('dropout: clouds of 2^16 tokens or more are outside the mask counter layout')
+        self._args = {}
+
+    def args(self, layer: int, site: int) -> _DropoutArgs:
+        a = self._args.get((layer, site))
+        if a is None:
+            a = self._args[(layer, site)] = _DropoutArgs(self.seed, self.step, self.pair_base, int(layer), int(site),
+                                                         self.threshold, self.scale, self.n_pairs)
+        return a
+
+    def site(self, layer: int, site: int):
+        return _DropSite(self, int(layer), int(site))
+
+
+class _DropSite:
+    """One (layer, site) of a DropoutKey: what the kernels of that site take."""
+
+    def __init__(self, key: DropoutKey, layer: int, site: int):
+        self.key, self.layer, self.site = key, layer, site
+        self.scale = key.scale
+
+    @property
+    def ptr(self):
+        return ctypes.addressof(self.key.args(self.layer, self.site))
+
+
+def dropout_keep_mask(p: float, seed: int, step: int, pair_base: int, n_pairs: int, cloud: int, layer: int, site: int,
+                      head: int, rows: int, cols: int, device=None):
+    """(rows, cols) uint8 keep mask (1 = kept) of local cloud `cloud` (0..2B-1: src clouds, then tgt clouds) at one
+    site, layer and head, from the same device function the kernels use (tests and analysis)."""
+    L = _lib.load()
+    key = DropoutKey(p, seed, step, pair_base, n_pairs)
+    out = torch.empty((int(rows), int(cols)), dtype=torch.uint8, device=device or 'cuda')
+    _lib.check(L.regtr_dropout_keep_mask(ctypes.addressof(key.args(layer, site)), int(cloud), int(head), int(rows),
+                                         int(cols), _p(out), _stream()), 'regtr_dropout_keep_mask')
+    _count(1)
+    return out
+
+
+def _check_drop_core():
+    impl = os.environ.get('REGTR_MHA_IMPL')
+    if impl and impl[0] == 'f':
+        raise _lib.RegtrLibError('attention dropout runs on the default 3xTF32 attention core only; unset '
+                                 'REGTR_MHA_IMPL=ffma (the CUDA-core A/B kernel) to train with dropout > 0')
+
+
+def mha_varlen_lse_dropout(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int, drop: _DropSite):
+    """mha_varlen_lse with the attention-probability dropout of `drop` (problem c = local query cloud c)."""
+    L = _lib.load()
+    _check_drop_core()
+    for t, nm in ((q, 'q'), (k, 'k'), (v, 'v')):
+        if not t.is_cuda or t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1:
+            raise ValueError(f'mha_varlen: {nm} must be a CUDA fp32 matrix with unit column stride')
+    E = q.shape[1]
+    dh = E // n_heads
+    out = torch.empty((q.shape[0], E), dtype=torch.float32, device=q.device)
+    lse = torch.empty((q.shape[0], n_heads), dtype=torch.float32, device=q.device)
+    _lib.check(L.regtr_mha_varlen_fwd_lse_dropout(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(out),
+                                                  out.stride(0), _p(lse), _p(q_start), _p(q_len), _p(k_start),
+                                                  _p(k_len), q_start.numel(), int(max_q_len), n_heads, dh,
+                                                  1.0 / math.sqrt(dh), drop.ptr, _stream()),
+               'regtr_mha_varlen_fwd_lse_dropout')
+    _count(1)
+    return out, lse
+
+
+def mha_varlen_bwd_dropout(q, k, v, o, lse, d_o, dq, dk, dv, q_start, q_len, k_start, k_len, max_q_len: int,
+                           max_k_len: int, n_heads: int, drop: _DropSite):
+    """mha_varlen_bwd of mha_varlen_lse_dropout."""
+    L = _lib.load()
+    _chk(d_o, torch.float32, 'dO', 2)
+    E = q.shape[1]
+    dh = E // n_heads
+    n_rows = q.shape[0]
+    ws = workspace(L.regtr_mha_varlen_bwd_ws_bytes(n_rows, n_heads), q.device, 'mha_bwd')
+    _lib.check(L.regtr_mha_varlen_bwd_dropout(
+        _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(o), o.stride(0), _p(d_o), d_o.stride(0), _p(lse),
+        _p(dq), dq.stride(0), _p(dk), dk.stride(0), _p(dv), dv.stride(0), _p(q_start), _p(q_len), _p(k_start),
+        _p(k_len), q_start.numel(), n_rows, int(max_q_len), int(max_k_len), n_heads, dh, 1.0 / math.sqrt(dh), drop.ptr,
+        _p(ws), ws.numel(), _stream()), 'regtr_mha_varlen_bwd_dropout')
+    _count(2)
+
+
+class _MHAPackedDropFn(torch.autograd.Function):
+    """_MHAPackedFn with the attention-probability dropout (site 1 or 3)."""
+
+    @staticmethod
+    def forward(ctx, qkv, q_start, q_len, k_start, k_len, max_len, n_heads, drop):
+        E = qkv.shape[1] // 3
+        o, lse = mha_varlen_lse_dropout(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], q_start, q_len, k_start, k_len,
+                                        max_len, n_heads, drop)
+        ctx.save_for_backward(qkv, o, lse, q_start, q_len, k_start, k_len)
+        ctx.max_len, ctx.n_heads, ctx.drop = max_len, n_heads, drop
+        return o
+
+    @staticmethod
+    def backward(ctx, g):
+        qkv, o, lse, qs, ql, ks, kl = ctx.saved_tensors
+        E = qkv.shape[1] // 3
+        d = torch.zeros_like(qkv)
+        mha_varlen_bwd_dropout(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], o, lse, g.contiguous(), d[:, :E],
+                               d[:, E:2 * E], d[:, 2 * E:], qs, ql, ks, kl, ctx.max_len, ctx.max_len, ctx.n_heads,
+                               ctx.drop)
+        return d, None, None, None, None, None, None, None
+
+
+def mha_packed_dropout(qkv, q_start, q_len, k_start, k_len, max_len: int, n_heads: int, drop: _DropSite):
+    """mha_packed (differentiable) with the attention-probability dropout of `drop`."""
+    return _MHAPackedDropFn.apply(qkv, q_start, q_len, k_start, k_len, int(max_len), int(n_heads), drop)
+
+
+def _layernorm_pos_dropout_fwd(x, z, gamma, beta, pos, eps, want_plain, want_pos, drop: _DropSite):
+    L = _lib.load()
+    _chk(x, torch.float32, 'x', 2); _chk(z, torch.float32, 'z', 2)
+    if z.shape != x.shape:
+        raise ValueError('layernorm_pos_dropout: x and z must have the same shape')
+    n, E = x.shape
+    y = torch.empty_like(x) if want_plain else None
+    yp = torch.empty_like(x) if want_pos else None
+    xo = torch.empty_like(x)
+    _lib.check(L.regtr_layernorm_pos_dropout(_p(x), _p(z), _p(gamma), _p(beta), _p(pos), n, _p(drop.key.offs), E,
+                                             float(eps), _p(y), _p(yp), _p(xo), drop.ptr, _stream()),
+               'regtr_layernorm_pos_dropout')
+    _count(1)
+    return y, yp, xo
+
+
+class _LayerNormDropFn(torch.autograd.Function):
+    """(LN(x'), LN(x') + pos, x') with x' = x + dropout(z): a residual dropout (site 2, 4 or 6) fused into the
+    LayerNorm that follows the residual add."""
+
+    @staticmethod
+    def forward(ctx, x, z, gamma, beta, pos, eps, want_plain, want_pos, drop):
+        ctx.set_materialize_grads(False)
+        y, yp, xo = _layernorm_pos_dropout_fwd(x, z, gamma, beta, pos, eps, want_plain, want_pos, drop)
+        ctx.save_for_backward(xo, gamma)
+        ctx.eps, ctx.drop = eps, drop
+        return y, yp, xo
+
+    @staticmethod
+    def backward(ctx, dy, dyp, dres):
+        xo, gamma = ctx.saved_tensors
+        L = _lib.load()
+        c = lambda t: None if t is None else t.contiguous()
+        dy, dyp, dres = c(dy), c(dyp), c(dres)
+        n, E = xo.shape
+        dx, dz = torch.empty_like(xo), torch.empty_like(xo)
+        dg, db = torch.empty_like(gamma), torch.empty_like(gamma)
+        ws = workspace(L.regtr_layernorm_bwd_ws_bytes(n, E), xo.device, 'ln_bwd')
+        d = ctx.drop
+        _lib.check(L.regtr_layernorm_bwd_dropout(_p(xo), _p(gamma), _p(dy), _p(dyp), _p(dres), n, _p(d.key.offs), E,
+                                                 float(ctx.eps), _p(dx), _p(dz), _p(dg), _p(db), d.ptr, _p(ws),
+                                                 ws.numel(), _stream()), 'regtr_layernorm_bwd_dropout')
+        _count(2)
+        need = ctx.needs_input_grad
+        return (dx if need[0] else None), (dz if need[1] else None), (dg if need[2] else None), \
+            (db if need[3] else None), None, None, None, None, None
+
+
+def layernorm_pos_dropout(x, z, gamma, beta, pos, eps: float, want_plain: bool, want_pos: bool, drop: _DropSite):
+    """-> (LN(x'), LN(x') + pos, x'), x' = x + m * scale * z: the residual add of a dropped branch z (the
+    out-projection or linear2 output, computed without residual=) and the LayerNorm after it, one launch."""
+    if _wants_grad(x, z, gamma, beta):
+        return _LayerNormDropFn.apply(x, z, gamma, beta, pos, float(eps), bool(want_plain), bool(want_pos), drop)
+    return _layernorm_pos_dropout_fwd(x, z, gamma, beta, pos, eps, want_plain, want_pos, drop)
+
+
+def dropout_rows_(h, drop: _DropSite):
+    """Feed-forward dropout (site 5) in place on the packed (N, F) rows of the batch's clouds."""
+    L = _lib.load()
+    _chk(h, torch.float32, 'h', 2)
+    k = drop.key
+    _lib.check(L.regtr_dropout_rows(_p(h), h.shape[0], h.shape[1], _p(k.offs), k.max_len, drop.ptr, _stream()),
+               'regtr_dropout_rows')
+    _count(1)
+    return h
+
+
+def relu_dropout_bwd(dh, h, scale: float):
+    L = _lib.load()
+    out = torch.empty_like(dh)
+    _lib.check(L.regtr_relu_dropout_bwd(_p(dh), _p(h), dh.numel(), float(scale), _p(out), _stream()),
+               'regtr_relu_dropout_bwd')
+    _count(1)
+    return out
+
+
+class _LinearReluDropFn(torch.autograd.Function):
+    """dropout(relu(x W^T + b)) (site 5): the GEMM with its ReLU epilogue, then the mask in place; the backward folds
+    the mask into the ReLU backward (the dropped output is positive exactly where both passed)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, drop):
+        h = dropout_rows_(_linear_fwd(x, weight, bias, None, True), drop)
+        ctx.save_for_backward(x, h)
+        ctx.weight, ctx.has_bias, ctx.scale = weight, bias is not None, drop.scale
+        return h
+
+    @staticmethod
+    def backward(ctx, g):
+        x, h = ctx.saved_tensors
+        g = relu_dropout_bwd(g.contiguous(), h, ctx.scale)
+        need = ctx.needs_input_grad
+        dx = linear_dgrad(g, ctx.weight) if need[0] else None
+        dw = db = None
+        if need[1] or need[2]:
+            dw, db = linear_wgrad(x, g, ctx.has_bias and need[2])
+        return dx, (dw if need[1] else None), db, None
+
+
+def linear_relu_dropout(x, weight, bias, drop: _DropSite):
+    """dropout(relu(linear(x))) of the feed-forward block (differentiable when grad mode is on)."""
+    if _wants_grad(x, weight, bias):
+        return _LinearReluDropFn.apply(x, weight, bias, drop)
+    return dropout_rows_(_linear_fwd(x, weight, bias, None, True), drop)
 
 
 # ------------------------------------------------------------------ encoder backward

@@ -33,7 +33,7 @@ import torch.nn.functional as F
 from . import ops
 from .kpconv import KPFEncoder, PreprocessorGPU
 from .lazy import LazyDict
-from .transformer import (AttentionPlan, PositionEmbeddingCoordsSine, PositionEmbeddingLearned,
+from .transformer import (AttentionPlan, PositionEmbeddingCoordsSine, PositionEmbeddingLearned, warn_dropout_eval_only,
                           TransformerCrossEncoder, TransformerCrossEncoderLayer)
 
 
@@ -263,27 +263,33 @@ class RegTR(nn.Module):
         if unsupported:
             raise NotImplementedError('forward_train: no backward for ' + ', '.join(unsupported))
 
-    def _stage_attention_train(self, feats_un, xyz_c, offs_c, B: int, plan: AttentionPlan):
+    def _stage_attention_train(self, feats_un, xyz_c, offs_c, B: int, plan: AttentionPlan, drop=None):
         """Differentiable stages after the encoder: feature projection, cross-encoder, correspondence heads.
-        The position embedding and the pose carry no gradient (the reference loss does not use the pose)."""
+        The position embedding and the pose carry no gradient (the reference loss does not use the pose).
+        drop: the cross-encoder's dropout masks (ops.DropoutKey) or None."""
         cfg = self.cfg
         both_un = ops.linear(feats_un, self.feat_proj.weight, self.feat_proj.bias)             # regtr.py:145
         with torch.no_grad():
             pe = self.pos_embed(xyz_c)
         cond = self.transformer_encoder.forward_train_packed(
-            both_un, pe if cfg.transformer_encoder_has_pos_emb else None, plan)
+            both_un, pe if cfg.transformer_encoder_has_pos_emb else None, plan, drop=drop)
         corr, logit = self.correspondence_decoder.forward_packed(cond, xyz_c, pe, plan)
         with torch.no_grad():
             pose = ops.pose_from_corr(xyz_c, corr.detach().contiguous(), logit.detach()[..., 0].contiguous(), offs_c, B)
         return dict(both_un=both_un, xyz_c=xyz_c, cond=cond, corr=corr, logit=logit, pose=pose)
 
-    def forward_train(self, batch, train_encoder: bool = False):
+    def forward_train(self, batch, train_encoder: bool = False, *, dropout_key=None):
         """`forward` with autograd: same output dict, whose src/tgt_feat(_un), *_kp_warped and *_overlap carry
         history back to every parameter after the KPConv encoder.  The pyramid always runs without grad.
         train_encoder=False: the encoder runs without grad and must be frozen
         (model.kpf_encoder.requires_grad_(False)).  train_encoder=True: the encoder runs under autograd too, on the
         encoder backward kernels, and every encoder parameter that requires grad receives one (kernel_points must
         stay frozen, as in the reference); its output is bit-identical to the inference encoder's.
+        Dropout (cfg.dropout > 0, training mode only): the cross-encoder applies the reference's six dropouts, with
+        masks drawn from dropout_key = (seed, step, pair_base) -- pair_base the global index of the batch's first
+        pair, so a pair gets the same masks in any batch, on any rank, and a resumed run repeats them.  dropout_key
+        None draws a fresh seed from torch's default CPU generator on every call.  In eval mode or at dropout 0 the
+        key is ignored and the step runs exactly as without it.
         Exact shapes, eager only."""
         if self.transformer_encoder.record_attentions:
             raise RuntimeError('forward_train: attention maps are recorded by the eager inference forward only; set '
@@ -298,12 +304,21 @@ class RegTR(nn.Module):
             feats_un, _ = self.kpf_encoder(torch.ones_like(pts[0][:, 0:1]), meta)             # regtr.py:122-136
         lens_c = meta['_lens'][-1]
         plan = AttentionPlan(lens_c, pts[-1].device)
-        core = self._stage_attention_train(feats_un, pts[-1], meta['_offs'][-1], B, plan)
+        drop = None
+        p = self.transformer_encoder.dropout_p
+        if self.training and p > 0.0:
+            if dropout_key is None:
+                dropout_key = (int(torch.randint(0, 2 ** 62, (1,)).item()), 0, 0)
+            seed, step, pair_base = dropout_key
+            drop = ops.DropoutKey(p, seed, step, pair_base, B, offs=meta['_offs'][-1], max_len=plan.max_len)
+        core = self._stage_attention_train(feats_un, pts[-1], meta['_offs'][-1], B, plan, drop)
         return self._assemble(core, lens_c, B)
 
     @torch.no_grad()
     def forward(self, batch):
-        """Eager path: exact shapes, one host sync (pyramid sizes) before the encoder."""
+        """Eager path: exact shapes, one host sync (pyramid sizes) before the encoder.  An inference executor: dropout
+        never applies (a training-mode model with dropout > 0 logs one warning; see forward_train)."""
+        warn_dropout_eval_only(self)
         B = len(batch['src_xyz'])
         meta = self.preprocessor(list(batch['src_xyz']) + list(batch['tgt_xyz']), lazy_upsamples=True)   # regtr.py:117-118
         batch['kpconv_meta'] = meta

@@ -308,6 +308,14 @@ class Trainer:
             D.broadcast_tensors(list(model.parameters()) + list(model.buffers()), self.group)
             self._bucket = D.GradBucket(list(model.parameters()), len(loss_keys(model.cfg)))
 
+    def _forward_train(self, model, b, global_step: int, pair_base: int):
+        """forward_train of a step; a model with transformer dropout gets its masks keyed by (seed, step, first pair),
+        so a resumed run and every data-parallel rank draw the masks a single uninterrupted process draws."""
+        enc = getattr(model, 'transformer_encoder', None)
+        if model.training and enc is not None and enc.dropout_p > 0:
+            return model.forward_train(b, train_encoder=True, dropout_key=(self.seed, global_step, pair_base))
+        return model.forward_train(b, train_encoder=True)
+
     def training_step(self, model, batch, global_step: int):
         """Step `global_step` (counted from 1) on a collated batch: TrainingPrep at step global_step - 1,
         forward_train, compute_loss, zero_grad; then, if the total is differentiable, backward, clipping, optimizer
@@ -317,7 +325,7 @@ class Trainer:
         losses = None
         try:
             b = self.prep(batch)
-            pred = model.forward_train(b, train_encoder=True)
+            pred = self._forward_train(model, b, global_step, 0)
             losses = model.compute_loss(pred, b)
             model.optimizer.zero_grad()
             if 'total' in losses and losses['total'].requires_grad:
@@ -376,7 +384,7 @@ class Trainer:
             model.optimizer.zero_grad()
             if batch is not None:
                 b = self.prep(batch, pair_base=pair_base)
-                pred = model.forward_train(b, train_encoder=True)
+                pred = self._forward_train(model, b, global_step, pair_base)
                 losses = self._local_losses(model, pred, b)
                 if losses['total'].requires_grad:
                     losses['total'].backward()

@@ -185,8 +185,10 @@ class TransformerCrossEncoderLayer(nn.Module):
             raise NotImplementedError
         if activation != 'relu':
             raise NotImplementedError('only relu is on the hot path')
-        if dropout != 0.0:
-            raise NotImplementedError('dropout > 0 is a training-only branch')
+        if not (isinstance(dropout, (int, float)) and 0.0 <= dropout < 1.0):
+            raise ValueError(f'dropout must be in [0, 1), got {dropout!r}')
+        # the six dropouts of forward_pre apply in forward_train_packed (training mode only); they add no state
+        self.dropout_p = float(dropout)
         self.self_attn = _MHAParams(d_model, nhead)
         self.multihead_attn = _MHAParams(d_model, nhead)
         self.linear1 = nn.Linear(d_model, dim_feedforward)
@@ -275,11 +277,15 @@ class TransformerCrossEncoderLayer(nn.Module):
         return x
 
 
-    def forward_train_packed(self, x, pos, plan: AttentionPlan):
+    def forward_train_packed(self, x, pos, plan: AttentionPlan, drop=None, layer_idx: int = 0):
         """Differentiable pre-norm layer (exact shapes) for the branches both reference configs select: pre-norm,
         values carrying the position embedding, the default 3xTF32 attention core.  Same math as `forward_packed`;
         every LayerNorm also hands x on to the residual add that follows it (layernorm_pos(skip=True)), so the
-        residual gradient is added inside the LayerNorm backward."""
+        residual gradient is added inside the LayerNorm backward.
+        drop (an ops.DropoutKey): apply the six dropouts of layer `layer_idx` and return (x, z) -- the last residual
+        branch z = linear2(...) is not added yet: its dropout and residual add run in the LayerNorm that follows."""
+        if drop is not None:
+            return self._forward_train_dropout(x, pos, plan, drop, layer_idx)
         has_pos = pos is not None
         for mha, norm, cross in ((self.self_attn, self.norm1, False), (self.multihead_attn, self.norm2, True)):
             y, yp, x = ops.layernorm_pos(x, norm.weight, norm.bias, pos, norm.eps, want_plain=not has_pos,
@@ -292,6 +298,31 @@ class TransformerCrossEncoderLayer(nn.Module):
                                      want_plain=True, want_pos=False, skip=True)
         h = ops.linear(x2, self.linear1.weight, self.linear1.bias, relu=True)
         return ops.linear(h, self.linear2.weight, self.linear2.bias, residual=x)
+
+    def _forward_train_dropout(self, x, pos, plan: AttentionPlan, drop, li: int):
+        """forward_train_packed with the six dropouts of transformers.py:183-244 (train mode).  The out-projection and
+        linear2 GEMMs run without residual=; each dropped branch z is added as x + m * scale * z in the prologue of
+        the LayerNorm that follows it (norm2, norm3, then the encoder's final norm), which also hands x' on."""
+        has_pos = pos is not None
+        z = None
+        for mha, norm, cross, att_site, out_prev in ((self.self_attn, self.norm1, False, ops.SITE_SELF_ATTN, None),
+                                                     (self.multihead_attn, self.norm2, True, ops.SITE_CROSS_ATTN,
+                                                      ops.SITE_SELF_OUT)):
+            if z is None:
+                y, yp, x = ops.layernorm_pos(x, norm.weight, norm.bias, pos, norm.eps, want_plain=not has_pos,
+                                             want_pos=has_pos, skip=True)
+            else:
+                y, yp, x = ops.layernorm_pos_dropout(x, z, norm.weight, norm.bias, pos, norm.eps, not has_pos, has_pos,
+                                                     drop.site(li, out_prev))
+            qkv = ops.linear(yp if has_pos else y, mha.in_proj_weight, mha.in_proj_bias)
+            ks, kl = (plan.xk_start, plan.xk_len) if cross else (plan.q_start, plan.q_len)
+            o = ops.mha_packed_dropout(qkv, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead,
+                                       drop.site(li, att_site))
+            z = ops.linear(o, mha.out_proj.weight, mha.out_proj.bias)
+        x2, _, x = ops.layernorm_pos_dropout(x, z, self.norm3.weight, self.norm3.bias, None, self.norm3.eps, True, False,
+                                             drop.site(li, ops.SITE_CROSS_OUT))
+        h = ops.linear_relu_dropout(x2, self.linear1.weight, self.linear1.bias, drop.site(li, ops.SITE_FFN))
+        return x, ops.linear(h, self.linear2.weight, self.linear2.bias)
 
     def forward_post_packed(self, x, pos, plan: AttentionPlan):
         """Post-norm layer (transformers.py:121-181): attention on x (+pos), then LayerNorm(x + update)."""
@@ -312,6 +343,18 @@ class TransformerCrossEncoderLayer(nn.Module):
         y = ops.linear(h, self.linear2.weight, self.linear2.bias, residual=x, m_dev=nd)
         x, _ = ln(y, self.norm3, False)
         return x
+
+
+def warn_dropout_eval_only(module):
+    """One warning per module when an inference executor runs a dropout > 0 model in training mode."""
+    enc = module if isinstance(module, TransformerCrossEncoder) else getattr(module, 'transformer_encoder', None)
+    if enc is None or not module.training or enc.dropout_p == 0.0 or module.__dict__.get('_dropout_warned'):
+        return
+    module.__dict__['_dropout_warned'] = True
+    import logging
+    logging.getLogger(type(module).__name__).warning(
+        f'dropout={enc.dropout_p} is applied by forward_train only; this forward is an inference executor and runs '
+        'without dropout (as in eval mode)')
 
 
 def _get_clones(module, N):
@@ -365,12 +408,28 @@ class TransformerCrossEncoder(nn.Module):
             outs.append(self._final(x, plan.n_dev))
         return torch.stack(outs)
 
-    def forward_train_packed(self, x, pos, plan: AttentionPlan):
+    @property
+    def dropout_p(self) -> float:
+        return self.layers[0].dropout_p if len(self.layers) else 0.0
+
+    def forward_train_packed(self, x, pos, plan: AttentionPlan, drop=None):
         """Differentiable `forward_packed` (pre-norm layers with a final norm, return_intermediate): -> (L, N, E).
-        The final norm of each intermediate output passes x on to the next layer (skip=True)."""
+        The final norm of each intermediate output passes x on to the next layer (skip=True).
+        drop (an ops.DropoutKey, or None): the masks of the six dropouts of every layer; layer l's dropout3 and
+        residual add run in the prologue of its final norm."""
         if self.record_attentions:
             raise RuntimeError('attention maps are recorded by the inference forward only; turn record_attentions off '
                                'to train')
+        if drop is not None:
+            if len(self.layers) > 16:
+                raise ValueError('dropout: more than 16 layers are outside the mask counter layout')
+            outs = []
+            for li, layer in enumerate(self.layers):
+                x, z = layer.forward_train_packed(x, pos, plan, drop, li)
+                y, _, x = ops.layernorm_pos_dropout(x, z, self.norm.weight, self.norm.bias, None, self.norm.eps, True,
+                                                    False, drop.site(li, ops.SITE_FFN_OUT))
+                outs.append(y)
+            return torch.stack(outs)
         outs = []
         for layer in self.layers:
             x = layer.forward_train_packed(x, pos, plan)
@@ -388,7 +447,9 @@ class TransformerCrossEncoder(nn.Module):
                 src_key_padding_mask: Optional[Tensor] = None, tgt_key_padding_mask: Optional[Tensor] = None,
                 src_pos: Optional[Tensor] = None, tgt_pos: Optional[Tensor] = None):
         """Reference-compatible padded interface (transformers.py:27-59): (L,B,D) in, (n_out,L,B,D) out.
-        Padded rows of the outputs are zero (the reference leaves unspecified values there)."""
+        Padded rows of the outputs are zero (the reference leaves unspecified values there).  An inference executor:
+        dropout never applies here (see `forward_train_packed`)."""
+        warn_dropout_eval_only(self)
         assert src_mask is None and tgt_mask is None, 'Masking not implemented'
         B = src.shape[1]
         s_lens = (~src_key_padding_mask).sum(1).tolist() if src_key_padding_mask is not None else [src.shape[0]] * B

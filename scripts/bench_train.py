@@ -57,6 +57,11 @@ def main():
     ap.add_argument('--train-encoder', action='store_true', help='train the KPConv encoder too (full training step)')
     ap.add_argument('--optimizer', default='none', choices=['none', 'library', 'torch'],
                     help='add clip + AdamW + StepLR on the library kernels or torch\'s to every step')
+    ap.add_argument('--dropout', type=float, default=0.0,
+                    help='model.dropout: the six transformer dropouts in training mode (masks keyed by the step)')
+    ap.add_argument('--kernel-times', action='store_true',
+                    help='also report the GPU time per step of the attention forward and backward kernels '
+                         '(torch.profiler over the timed steps)')
     args = ap.parse_args()
     if args.steps < 1:
         ap.error('--steps must be >= 1')
@@ -64,7 +69,7 @@ def main():
     dev = torch.device('cuda:0')
     B = args.pairs or {2: 1, 3: 8}[args.config]
 
-    cfg = get_config('3dmatch')
+    cfg = get_config('3dmatch', dropout=args.dropout) if args.dropout else get_config('3dmatch')
     model = RegTR(cfg).to(dev)
     model.load_state_dict(random_state_dict(cfg, WEIGHT_SEED), strict=True)
     if not args.train_encoder:
@@ -94,7 +99,8 @@ def main():
         model.zero_grad(set_to_none=True)
         if evs:
             evs[0].record()
-        total = model.compute_loss(model.forward_train(batch, train_encoder=args.train_encoder), batch)['total']
+        pred = model.forward_train(batch, train_encoder=args.train_encoder, dropout_key=(WEIGHT_SEED, i, 0))
+        total = model.compute_loss(pred, batch)['total']
         if evs:
             evs[1].record()
         total.backward()
@@ -119,15 +125,34 @@ def main():
         step(args.warmup + i, evs)
         timed.append(evs)
     torch.cuda.synchronize()
+    prof = None
+    if args.kernel_times:            # a separate pass after the timed steps: the step times above are untraced
+        prof = torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA])
+        with prof:
+            for i in range(args.steps):
+                flush.zero_()
+                step(args.warmup + args.steps + i)
+            torch.cuda.synchronize()
+        kt = {}
+        for ev in prof.key_averages():
+            for tag, pat in (('attention_fwd', 'k_mha_tf32x3'), ('attention_bwd_dq', 'k_mha_bwd_dq'),
+                             ('attention_bwd_dkv', 'k_mha_bwd_dkv'), ('dropout_rows', 'k_dropout_rows')):
+                if pat in ev.key:
+                    kt[tag + '_ms_per_step'] = kt.get(tag + '_ms_per_step', 0.0) + \
+                        getattr(ev, 'device_time_total', getattr(ev, 'cuda_time_total', 0.0)) / 1e3 / args.steps
     fwd = sum(e[0].elapsed_time(e[1]) for e in timed)
     bwd = sum(e[1].elapsed_time(e[2]) for e in timed)
     name, power = card()
     extra = {}
+    if args.dropout:
+        extra['dropout'] = args.dropout
+    if prof is not None:
+        extra.update(kt)
     if opt is not None:
         ost = sum(e[2].elapsed_time(e[3]) for e in timed)
-        extra = dict(optimizer=args.optimizer, optimizer_ms_per_step=ost / args.steps,
+        extra.update(optimizer=args.optimizer, optimizer_ms_per_step=ost / args.steps,
                      train_ms_per_step_with_optimizer=(fwd + bwd + ost) / args.steps,
-                     optimizer_library_launches_per_step=sum(opt_launches) / args.steps)
+                     optimizer_library_launches_per_step=sum(opt_launches[:args.steps]) / args.steps)
     print(json.dumps(dict(
         metric='training steps/s of forward_train + compute_loss + backward ' +
                ('(KPConv encoder trained)' if args.train_encoder else '(KPConv encoder frozen)'),
