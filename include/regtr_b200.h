@@ -217,7 +217,8 @@ int regtr_attention_plan(const int32_t* offs, int B, int32_t* plan, void* stream
  * Problem i attends queries rows [q_start[i], q_start[i]+q_len[i]) of Q to key rows
  * [k_start[i], k_start[i]+k_len[i]) of K/V.  Q/K/V/O are row-major with leading
  * dimensions ldq/ldk/ldv/ldo (floats); head h uses columns [h*head_dim, (h+1)*head_dim).
- * head_dim must be 32.  max_q_len: host upper bound of q_len[]. */
+ * head_dim must be 32; ldo must be even (REGTR_ERR_UNSUPPORTED otherwise).  max_q_len: host upper bound of
+ * q_len[]. */
 int regtr_mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
                          float* O, int ldo, const int32_t* q_start, const int32_t* q_len,
                          const int32_t* k_start, const int32_t* k_len, int n_problems,
@@ -270,7 +271,7 @@ int regtr_mha_tf32_tc_fwd(const float* qk4, int ld4, const float* vt2, int ld_vt
                           int max_tiles, int n_heads, int head_dim, void* stream);
 /* (tile_base / max_tiles as for regtr_mha_varlen_fwd, with 128-query tiles.) */
 
-/* Training forward of the regtr_mha_varlen_fwd core (the default 3xTF32 mma.sync kernel): same O, bit for bit, plus
+/* Training forward of the regtr_mha_varlen_fwd core (the 3xTF32 mma.sync kernel): same O, bit for bit, plus
  * lse [n_tokens, n_heads] = log2(sum_k exp2(s_qk)) of the base-2 scores s = (q * scale * log2 e) . k -- what
  * regtr_mha_varlen_bwd recomputes the softmax from (-inf for a query whose key range is empty).  No tile table. */
 int regtr_mha_varlen_fwd_lse(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,

@@ -1,17 +1,10 @@
-// Variable-length multi-head attention core, fp32-accurate parity path: a tensor-core kernel
-// (mma.sync 3xTF32, the default) and the CUDA-core kernel it replaced (REGTR_MHA_IMPL=ffma).
+// Variable-length multi-head attention core, fp32-accurate parity path (mma.sync 3xTF32).
 //
 // Replaces the softmax(QK^T/sqrt(d))V core of nn.MultiheadAttention as called by
 // TransformerCrossEncoderLayer.forward_pre (/root/reference/src/models/transformer/
 // transformers.py:197-226).  The reference pads sequences to a common length and masks
 // padded keys with -inf; here every (query range, key range) problem is explicit, which is
 // equivalent because masked keys receive exactly zero weight.
-//
-// CUDA-core kernel, work decomposition: block = (problem, head, tile of 32 queries); 4 warps split the keys
-// 4 ways (key j handled by warp j % 4), each thread keeps one query row (32 floats), an
-// online-softmax state and a 32-float accumulator; K/V tiles of 128 keys are staged in
-// shared memory and read as warp-wide broadcasts; the 4 partial states are merged at the end.
-#include <cstdlib>
 
 #include "common.cuh"
 #include "philox.cuh"
@@ -29,108 +22,8 @@ __device__ __forceinline__ bool find_tile(const int32_t* __restrict__ tile_base,
     tile -= tile_base[p];
     return true;
 }
-constexpr int QT = 32;        // queries per block
-constexpr int KSPLIT = 4;     // warps per block
-constexpr int KT = 128;       // keys per shared-memory tile
 
-__global__ void __launch_bounds__(QT * KSPLIT)
-k_mha_fp32(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp, int ldk, const float* __restrict__ Vp,
-           int ldv, float* __restrict__ O, int ldo, const int32_t* __restrict__ q_start,
-           const int32_t* __restrict__ q_len, const int32_t* __restrict__ k_start, const int32_t* __restrict__ k_len,
-           int n_heads, float scale) {
-    __shared__ __align__(16) float sK[KT][HD];
-    __shared__ __align__(16) float sV[KT][HD];
-    __shared__ float sM[KSPLIT][QT], sL[KSPLIT][QT];
-    const int prob = blockIdx.z, head = blockIdx.y, tile = blockIdx.x;
-    const int ql = q_len[prob];
-    if (tile * QT >= ql) return;
-    const int q0 = q_start[prob], k0 = k_start[prob], kl = k_len[prob];
-    const int lane = threadIdx.x & 31, ks = threadIdx.x >> 5;
-    const int qi = tile * QT + lane;
-    const bool active = qi < ql;
-    const int col = head * HD;
-
-    float qv[HD], acc[HD];
-#pragma unroll
-    for (int d = 0; d < HD; ++d) { qv[d] = 0.f; acc[d] = 0.f; }
-    if (active) {
-        const float4* src = reinterpret_cast<const float4*>(Q + (size_t)(q0 + qi) * ldq + col);
-#pragma unroll
-        for (int d = 0; d < HD / 4; ++d) {
-            const float4 t = src[d];
-            qv[4 * d] = t.x * scale; qv[4 * d + 1] = t.y * scale; qv[4 * d + 2] = t.z * scale; qv[4 * d + 3] = t.w * scale;
-        }
-    }
-    float m = -INFINITY, l = 0.f;
-
-    for (int kb = 0; kb < kl; kb += KT) {
-        const int nk = min(KT, kl - kb);
-        __syncthreads();
-        for (int t = threadIdx.x; t < nk * (HD / 4); t += QT * KSPLIT) {
-            const int r = t / (HD / 4), c4 = t % (HD / 4);
-            reinterpret_cast<float4*>(&sK[r][0])[c4] =
-                *reinterpret_cast<const float4*>(Kp + (size_t)(k0 + kb + r) * ldk + col + 4 * c4);
-            reinterpret_cast<float4*>(&sV[r][0])[c4] =
-                *reinterpret_cast<const float4*>(Vp + (size_t)(k0 + kb + r) * ldv + col + 4 * c4);
-        }
-        __syncthreads();
-        for (int j = ks; j < nk; j += KSPLIT) {
-            float sdot = 0.f;
-            const float4* kr = reinterpret_cast<const float4*>(&sK[j][0]);
-#pragma unroll
-            for (int d = 0; d < HD / 4; ++d) {
-                const float4 t = kr[d];
-                sdot = fmaf(qv[4 * d], t.x, sdot); sdot = fmaf(qv[4 * d + 1], t.y, sdot);
-                sdot = fmaf(qv[4 * d + 2], t.z, sdot); sdot = fmaf(qv[4 * d + 3], t.w, sdot);
-            }
-            const float mn = fmaxf(m, sdot);
-            const float corr = exp2f(m - mn);            // scores carry log2(e): exp2(-inf) = 0 on the first key
-            const float p = exp2f(sdot - mn);
-            l = l * corr + p;
-            const float4* vr = reinterpret_cast<const float4*>(&sV[j][0]);
-#pragma unroll
-            for (int d = 0; d < HD / 4; ++d) {
-                const float4 t = vr[d];
-                acc[4 * d] = fmaf(acc[4 * d], corr, p * t.x); acc[4 * d + 1] = fmaf(acc[4 * d + 1], corr, p * t.y);
-                acc[4 * d + 2] = fmaf(acc[4 * d + 2], corr, p * t.z); acc[4 * d + 3] = fmaf(acc[4 * d + 3], corr, p * t.w);
-            }
-            m = mn;
-        }
-    }
-
-    // merge the KSPLIT partial softmax states of each query
-    __syncthreads();
-    sM[ks][lane] = m;
-    __syncthreads();
-    float mg = -INFINITY;
-#pragma unroll
-    for (int t = 0; t < KSPLIT; ++t) mg = fmaxf(mg, sM[t][lane]);
-    const float w = (m == -INFINITY) ? 0.f : exp2f(m - mg);
-    sL[ks][lane] = l * w;
-    // reuse sK as the accumulator exchange buffer: [KSPLIT][QT][HD] floats = 16 KB = sizeof(sK)
-    float* xb = &sK[0][0];
-    __syncthreads();
-#pragma unroll
-    for (int d = 0; d < HD; ++d) xb[(ks * QT + lane) * HD + ((d + lane) & (HD - 1))] = acc[d] * w;
-    __syncthreads();
-    if (!active) return;
-    float lg = 0.f;
-#pragma unroll
-    for (int t = 0; t < KSPLIT; ++t) lg += sL[t][lane];
-    const float inv = lg > 0.f ? 1.f / lg : 0.f;
-    // warp ks writes dims [ks*8, ks*8+8) of every query in the tile
-    float* dst = O + (size_t)(q0 + qi) * ldo + col;
-#pragma unroll
-    for (int dd = 0; dd < HD / KSPLIT; ++dd) {
-        const int d = ks * (HD / KSPLIT) + dd;
-        float s = 0.f;
-#pragma unroll
-        for (int t = 0; t < KSPLIT; ++t) s += xb[(t * QT + lane) * HD + ((d + lane) & (HD - 1))];
-        dst[d] = s * inv;
-    }
-}
-
-// ---- tensor-core fp32-accurate core (default) ------------------------------------------------------
+// ---- tensor-core fp32-accurate core --------------------------------------------------------------
 // Flash-attention on mma.sync m16n8k8 TF32 with the 3xTF32 split (x = hi + lo; hi*hi + hi*lo + lo*hi in
 // fp32 accumulators), so scores and outputs keep fp32 accuracy while the 2 x 32 MACs per (query, key)
 // run on the tensor cores.  Block = (problem, head, 64 queries): 4 warps x 16 query rows; keys stream
@@ -272,7 +165,7 @@ k_mha_tf32x3(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp,
         }
         // O = O * c + P V.  The chunk's P V is accumulated from zero and added to the running output with a
         // round-to-nearest FMA: the tensor core truncates when it adds into its accumulator, and a chain through
-        // every key of a 700-token cloud (264 MMAs) biased the outputs by ~1e-5 relative (tests/diag_accuracy.py).
+        // every key of a 700-token cloud (264 MMAs) biased the outputs by ~1e-5 relative against float64.
         float pacc[4][4];
 #pragma unroll
         for (int j = 0; j < 4; ++j)
@@ -619,25 +512,17 @@ static int mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, cons
     if (n_problems == 0 || max_q_len == 0 || (tile_base && max_tiles == 0)) return REGTR_OK;
     if (!Q || !K || !V || !O || !q_start || !q_len || !k_start || !k_len) return REGTR_ERR_ARG;
     if ((ldq | ldk | ldv) % 4 != 0 || n_problems > 65535 || n_heads > 65535) return REGTR_ERR_ARG;
-    const char* impl = getenv("REGTR_MHA_IMPL");           // "ffma": CUDA-core kernel (A/B measurements)
-    if (lse || (!(impl && impl[0] == 'f') && (ldo % 2) == 0)) {
-        if (ldo % 2) return REGTR_ERR_UNSUPPORTED;
-        // with the tile table: linear 64-query tile index (max_tiles = host bound of the total); else one grid
-        // column per problem sized by the longest sequence
-        const dim3 grid = tile_base ? dim3(max_tiles, n_heads, 1) : dim3(regtr_cdiv(max_q_len, MQ), n_heads, n_problems);
-        if (drop)
-            k_mha_tf32x3<true><<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len,
-                                                     tile_base, n_problems, scale * 1.4426950408889634f, lse, *drop);
-        else
-            k_mha_tf32x3<false><<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len,
-                                                      tile_base, n_problems, scale * 1.4426950408889634f, lse, DropKey{});
-        REGTR_CHECK_LAUNCH();
-        return REGTR_OK;
-    }
-    dim3 grid(regtr_cdiv(max_q_len, QT), n_heads, n_problems);
-    // softmax in base 2: q is pre-scaled by scale * log2(e) (<= 2 ulp exp2f instead of two ~20-instruction expf)
-    k_mha_fp32<<<grid, QT * KSPLIT, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, n_heads,
-                                            scale * 1.4426950408889634f);
+    if (ldo % 2) return REGTR_ERR_UNSUPPORTED;              // float2 output stores
+    // with the tile table: linear 64-query tile index (max_tiles = host bound of the total); else one grid
+    // column per problem sized by the longest sequence
+    const dim3 grid = tile_base ? dim3(max_tiles, n_heads, 1) : dim3(regtr_cdiv(max_q_len, MQ), n_heads, n_problems);
+    // softmax in base 2: q is pre-scaled by scale * log2(e)
+    if (drop)
+        k_mha_tf32x3<true><<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len,
+                                                 tile_base, n_problems, scale * 1.4426950408889634f, lse, *drop);
+    else
+        k_mha_tf32x3<false><<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len,
+                                                  tile_base, n_problems, scale * 1.4426950408889634f, lse, DropKey{});
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
 }

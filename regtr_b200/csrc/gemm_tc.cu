@@ -14,7 +14,6 @@
 
 
 #include "common.cuh"
-#include <stdlib.h>
 
 #include "tc.cuh"
 
@@ -442,25 +441,6 @@ __global__ void k_splitk_reduce(const float* __restrict__ P, int splits, size_t 
     o[0] = acc.x; o[1] = acc.y; o[2] = acc.z; o[3] = acc.w;
 }
 
-// CUDA-core reference (REGTR_GEMM_IMPL=ffma; A/B accuracy measurements only, tests/diag_accuracy.py): one thread
-// per output element, sequential round-to-nearest FMA over K -- what an fp32 SGEMM computes.
-__global__ void k_gemm_ffma(const float* __restrict__ A, int lda, const float* __restrict__ Bhi,
-                            const float* __restrict__ Blo, int ldb, float* __restrict__ C, int ldc,
-                            const float* __restrict__ bias, const float* __restrict__ R, int ldr, int M, int N, int K,
-                            const int32_t* __restrict__ m_dev, int relu) {
-    if (m_dev) M = min(M, *m_dev);
-    const int n = blockIdx.x * blockDim.x + threadIdx.x;
-    if (n >= N) return;
-    for (int m = blockIdx.y; m < M; m += gridDim.y) {
-        float acc = 0.f;
-        for (int k = 0; k < K; ++k) acc = fmaf(A[(size_t)m * lda + k], Bhi[(size_t)n * ldb + k] + Blo[(size_t)n * ldb + k], acc);
-        if (bias) acc += bias[n];
-        if (R) acc += R[(size_t)m * ldr + n];
-        if (relu) acc = fmaxf(acc, 0.f);
-        C[(size_t)m * ldc + n] = acc;
-    }
-}
-
 // split count: only for skinny problems (few output tiles) with a long K, to fill the machine
 // (ceil(REGTR_NUM_SMS / tiles) planes, each of at least 8 k-blocks); the planes are summed in a fixed order by the
 // reduction kernel.  At most 16 k-blocks (K = 512) per plane keeps the split's partial sums short as well.
@@ -589,16 +569,6 @@ static int gemm_dispatch(const float* A, int lda, const float* B_hi, const float
     // TMA: 16-byte aligned bases and row pitches
     if ((lda & 3) || (ldb & 3) || ((uintptr_t)A & 15) || ((uintptr_t)B_hi & 15) || ((uintptr_t)B_lo & 15))
         return REGTR_ERR_UNSUPPORTED;
-    {
-        const char* impl = getenv("REGTR_GEMM_IMPL");
-        if (impl && impl[0] == 'f') {
-            if (used_splits) *used_splits = 2;                  // statistics: read every row from C
-            k_gemm_ffma<<<dim3(regtr_cdiv(N, 128), M < 32768 ? M : 32768), 128, 0, st>>>(A, lda, B_hi, B_lo, ldb, C, ldc, bias, R, ldr, M, N, K,
-                                                                    m_dev, relu);
-            REGTR_CHECK_LAUNCH();
-            return REGTR_OK;
-        }
-    }
     const int bn = choose_bn(M, N);
     int splits = choose_splits(M, N, K, bn);
     if (used_splits) *used_splits = splits;

@@ -6,7 +6,6 @@
 //   models/backbone_kpconv/kpconv_blocks.py:269-414  KPConv.forward (rigid, linear, sum)
 //   models/backbone_kpconv/kpconv_blocks.py:127-143  max_pool
 #include <algorithm>
-#include <cstdlib>
 
 #include "common.cuh"
 
@@ -32,12 +31,6 @@ __global__ void k_row_flags(const float* __restrict__ x, int n, int C, uint8_t* 
 // that works in 128-row tiles, skips tiles beyond n and never stores rows >= n, so padding rows need
 // defined (zero) contents only inside the tile that straddles n; the rest of the capacity is left untouched.
 __device__ __forceinline__ int pad_band_end(int n) { return (n + 127) & ~127; }
-
-// ---- fp32 pairs: kernel points (2j, 2j+1) side by side, one round-to-nearest FMA each
-typedef float2 f2;
-__device__ __forceinline__ f2 f2_dup(float x) { return make_float2(x, x); }
-__device__ __forceinline__ f2 f2_fma(f2 a, f2 b, f2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
-__device__ __forceinline__ void f2_unpack(f2 v, float& lo, float& hi) { lo = v.x; hi = v.y; }
 
 // Phase 1 (lanes own neighbours): compact the valid (non-shadow) neighbours of one query into
 // shared memory as (relative position, id) and count those whose feature row sums to > 0.
@@ -88,102 +81,6 @@ __device__ __forceinline__ void stage_neighbours(const float* __restrict__ s, co
     __syncwarp();
     n_valid = base;
     n_counted = counted;
-}
-
-// Cin = 32 * VEC: lane owns VEC channels; per valid neighbour one coalesced row load, four
-// broadcast LDS.128 of the 16 influences and 8 * VEC packed fp32x2 FMAs.
-template <int VEC, int UNROLL, int MINB>
-__global__ void __launch_bounds__(AGG_WARPS * 32, MINB)
-k_kpconv_agg(const float* __restrict__ q, const float* __restrict__ s, const int32_t* __restrict__ idx,
-             const float* __restrict__ x, const uint8_t* __restrict__ flags, const float* __restrict__ kp,
-             int Nq, int Ns, const int32_t* __restrict__ nq_dev, const int32_t* __restrict__ ns_dev, int K,
-             float extent, float* __restrict__ wf) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    constexpr int CIN = VEC * 32;
-    constexpr int NV4 = VEC >= 4 ? VEC / 4 : 1;          // float4 loads per lane
-    float* kp_s = reinterpret_cast<float*>(smem_raw);     // 48 floats
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int Kp = (K + 3) & ~3;
-    float* w_s = kp_s + 48 + warp * (Kp * (KPP + 4 + 1));            // per warp: w[Kp][16] | rel[Kp] (float4) | id[Kp]
-    float4* rel_s = reinterpret_cast<float4*>(w_s + Kp * KPP);
-    int* id_s = reinterpret_cast<int*>(w_s + Kp * (KPP + 4));
-    if (threadIdx.x < 3 * KP) kp_s[threadIdx.x] = kp[threadIdx.x];
-    __syncthreads();
-    const int qi = blockIdx.x * AGG_WARPS + warp;
-    if (qi >= Nq) return;
-    if (ns_dev) Ns = min(Ns, *ns_dev);
-    if (nq_dev && qi >= *nq_dev) {               // capacity padding row
-        if (qi < pad_band_end(*nq_dev)) {
-            float* o = wf + (size_t)qi * (KP * CIN);
-            for (int t = lane; t < KP * CIN; t += 32) o[t] = 0.f;
-        }
-        return;
-    }
-
-    int n_valid, n_counted;
-    stage_neighbours(s, idx + (size_t)qi * K, flags, kp_s, q[3 * qi], q[3 * qi + 1], q[3 * qi + 2], Ns, K,
-                     1.f / extent, w_s, rel_s, id_s, lane, n_valid, n_counted);
-
-    f2 acc[8][VEC];                               // acc[j] = kernel points (2j, 2j+1); slot 15 is padding
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int v = 0; v < VEC; ++v) acc[j][v] = make_float2(0.f, 0.f);
-
-    const int n_pad = (n_valid + 3) & ~3;          // UNROLL divides 4; padded slots carry zero influences
-    for (int k0 = 0; k0 < n_pad; k0 += UNROLL) {
-        float xv[UNROLL][VEC];
-#pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
-            const float* row = x + (size_t)id_s[k0 + u] * CIN;
-            if constexpr (VEC == 1) {
-                xv[u][0] = __ldg(row + lane);
-            } else if constexpr (VEC == 2) {
-                const float2 t = __ldg(reinterpret_cast<const float2*>(row) + lane);
-                xv[u][0] = t.x; xv[u][1] = t.y;
-            } else {
-#pragma unroll
-                for (int j = 0; j < NV4; ++j) {
-                    const float4 t = __ldg(reinterpret_cast<const float4*>(row) + j * 32 + lane);
-                    xv[u][4 * j + 0] = t.x; xv[u][4 * j + 1] = t.y; xv[u][4 * j + 2] = t.z; xv[u][4 * j + 3] = t.w;
-                }
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
-            const float4* wr = reinterpret_cast<const float4*>(w_s + (k0 + u) * KPP);
-            const float4 a = wr[0], b = wr[1], c = wr[2], d = wr[3];
-            const f2 w2[8] = {make_float2(a.x, a.y), make_float2(a.z, a.w), make_float2(b.x, b.y), make_float2(b.z, b.w),
-                              make_float2(c.x, c.y), make_float2(c.z, c.w), make_float2(d.x, d.y), make_float2(d.z, d.w)};
-#pragma unroll
-            for (int v = 0; v < VEC; ++v) {
-                const f2 xx = f2_dup(xv[u][v]);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) acc[j][v] = f2_fma(w2[j], xx, acc[j][v]);
-            }
-        }
-    }
-
-    const float inv = 1.f / (float)max(n_counted, 1);
-    float* out = wf + (size_t)qi * (KP * CIN);
-    float r[KPP][VEC];
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int v = 0; v < VEC; ++v) f2_unpack(acc[j][v], r[2 * j][v], r[2 * j + 1][v]);
-#pragma unroll
-    for (int p = 0; p < KP; ++p) {
-        if constexpr (VEC == 1) {
-            out[p * CIN + lane] = r[p][0] * inv;
-        } else if constexpr (VEC == 2) {
-            reinterpret_cast<float2*>(out + p * CIN)[lane] = make_float2(r[p][0] * inv, r[p][1] * inv);
-        } else {
-#pragma unroll
-            for (int j = 0; j < NV4; ++j)
-                reinterpret_cast<float4*>(out + p * CIN)[j * 32 + lane] =
-                    make_float4(r[p][4 * j] * inv, r[p][4 * j + 1] * inv, r[p][4 * j + 2] * inv, r[p][4 * j + 3] * inv);
-        }
-    }
 }
 
 // ---- aggregation on the tensor cores ---------------------------------------------------------------
@@ -617,7 +514,7 @@ k_kpconv_c1(const float* __restrict__ q, const float* __restrict__ s, const int3
     }
 }
 
-// Small Cin (2..16): same staging; then lane
+// Small Cin (2..16): neighbours and influences staged by stage_neighbours; then lane
 // (p, half) sums w[k][p] * x[id_k][c] over its half of the neighbours, halves combined by shuffle.
 __global__ void __launch_bounds__(AGG_WARPS * 32)
 k_kpconv_agg_small(const float* __restrict__ q, const float* __restrict__ s, const int32_t* __restrict__ idx,
@@ -734,28 +631,17 @@ size_t agg_smem_bytes(int K) {
     return sizeof(float) * 48 + (size_t)AGG_WARPS * Kp * (KPP + 4 + 1) * sizeof(float);
 }
 
-template <int VEC, int UNROLL, int MINB>
-int launch_agg(const float* q, const float* s, const int32_t* idx, const float* x, const uint8_t* flags,
-               const float* kp, int Nq, int Ns, const int32_t* nq_dev, const int32_t* ns_dev, int K, float extent,
-               float* wf, cudaStream_t st) {
-    const size_t smem = agg_smem_bytes(K);
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(k_kpconv_agg<VEC, UNROLL, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)smem);
-        if (e != cudaSuccess) return -(1000 + (int)e);
-    }
-    k_kpconv_agg<VEC, UNROLL, MINB><<<regtr_cdiv(Nq, AGG_WARPS), AGG_WARPS * 32, smem, st>>>(
-        q, s, idx, x, flags, kp, Nq, Ns, nq_dev, ns_dev, K, extent, wf);
-    REGTR_CHECK_LAUNCH();
-    return REGTR_OK;
+// k_kpconv_agg_mma: per warp, Kp staged rows of 32 NH floats plus a float4 and an id per neighbour
+size_t agg_mma_smem_bytes(int K, int nh) {
+    const int Kp = (K + 7) & ~7;
+    return (size_t)AGG_WARPS * Kp * (32 * nh + 5) * sizeof(float);
 }
 
 template <int NH, int MINB>
 int launch_agg_mma(const float* q, const float* s, const int32_t* idx, const float* x, const uint8_t* flags,
                    const float* kp, int Nq, int Ns, const int32_t* nq_dev, const int32_t* ns_dev, int K, int Cin,
                    float extent, float* wf, cudaStream_t st) {
-    const int Kp = (K + 7) & ~7;
-    const size_t smem = (size_t)AGG_WARPS * Kp * (32 * NH + 5) * sizeof(float);
+    const size_t smem = agg_mma_smem_bytes(K, NH);
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(k_kpconv_agg_mma<NH, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return REGTR_ERR_UNSUPPORTED;       // K too large for the staged kernel
@@ -767,19 +653,17 @@ int launch_agg_mma(const float* q, const float* s, const int32_t* idx, const flo
     return REGTR_OK;
 }
 
-// channel groups per warp: as wide as possible while the grid still has >= min_warps warps
-int agg_mma_nh(int Nq, int Cin) {
-    const char* e = getenv("REGTR_AGG_MIN_WARPS");          // tuning knob, default from the level-size sweep
-    const int min_warps = e ? atoi(e) : 8192;
-    int nh = Cin / 32 > 2 ? 2 : Cin / 32;      // staged rows: 128 NH bytes of smem per neighbour and warp
-    while (nh > 1 && (long long)Nq * (Cin / (32 * nh)) < min_warps) nh >>= 1;
-    return nh;
-}
+// Channel slicing of k_kpconv_agg_mma: the grid keeps at least this many warps (from the level-size sweep).
+constexpr long long AGG_MMA_MIN_WARPS = 8192;
+constexpr size_t SMEM_OPTIN = 227 * 1024;           // sm_90 opt-in shared memory per block
 
-// REGTR_AGG_IMPL=ffma selects the CUDA-core aggregation kernels (A/B measurements); default: tensor cores.
-bool agg_use_mma() {
-    const char* e = getenv("REGTR_AGG_IMPL");
-    return !(e && e[0] == 'f');
+// channel groups per warp: as wide as possible while the grid still has >= AGG_MMA_MIN_WARPS warps and the staged
+// rows fit in shared memory (NH = 2 up to K = 104)
+int agg_mma_nh(int Nq, int K, int Cin) {
+    int nh = Cin / 32 > 2 ? 2 : Cin / 32;      // staged rows: 128 NH bytes of smem per neighbour and warp
+    while (nh > 1 && ((long long)Nq * (Cin / (32 * nh)) < AGG_MMA_MIN_WARPS || agg_mma_smem_bytes(K, nh) > SMEM_OPTIN))
+        nh >>= 1;
+    return nh;
 }
 
 }  // namespace
@@ -830,11 +714,10 @@ int regtr_kpconv_aggregate(const float* q, const float* s, const int32_t* idx, c
         REGTR_CHECK_LAUNCH();
         return REGTR_OK;
     }
-    {   // default: software-pipelined persistent kernel (REGTR_AGG_IMPL=mma / ffma select the older kernels for A/B)
-        const char* e = getenv("REGTR_AGG_IMPL");
+    {   // software-pipelined persistent kernel up to K = 64
         const int nh = (Cin % 64 == 0) ? 2 : 1;
         const int S = Cin / (32 * nh);
-        if (!e && K <= 64 && Cin % 32 == 0 && (S & (S - 1)) == 0) {
+        if (K <= 64 && Cin % 32 == 0 && (S & (S - 1)) == 0) {
             const int Kp = (K + 7) & ~7;
             const size_t smem = (size_t)PIPE_WARPS * 2 * Kp * (32 * nh + 5) * sizeof(float);
             if (smem > 200 * 1024) return REGTR_ERR_UNSUPPORTED;
@@ -862,21 +745,10 @@ int regtr_kpconv_aggregate(const float* q, const float* s, const int32_t* idx, c
             return REGTR_OK;
         }
     }
-    if (agg_use_mma()) {
-        int rc = REGTR_ERR_UNSUPPORTED;
-        switch (agg_mma_nh(Nq, Cin)) {
-            case 1: rc = launch_agg_mma<1, 4>(q, s, idx, x, rowflag_ws, kp, Nq, Ns, nq_dev, ns_dev, K, Cin, extent, wf, st); break;
-            case 2: rc = launch_agg_mma<2, 2>(q, s, idx, x, rowflag_ws, kp, Nq, Ns, nq_dev, ns_dev, K, Cin, extent, wf, st); break;
-        }
-        if (rc != REGTR_ERR_UNSUPPORTED) return rc;
-    }
-    switch (Cin / 32) {
-        case 1: return launch_agg<1, 4, 5>(q, s, idx, x, rowflag_ws, kp, Nq, Ns, nq_dev, ns_dev, K, extent, wf, st);
-        case 2: return launch_agg<2, 4, 4>(q, s, idx, x, rowflag_ws, kp, Nq, Ns, nq_dev, ns_dev, K, extent, wf, st);
-        case 4: return launch_agg<4, 4, 2>(q, s, idx, x, rowflag_ws, kp, Nq, Ns, nq_dev, ns_dev, K, extent, wf, st);
-        case 8: return launch_agg<8, 2, 1>(q, s, idx, x, rowflag_ws, kp, Nq, Ns, nq_dev, ns_dev, K, extent, wf, st);
-    }
-    return REGTR_ERR_UNSUPPORTED;
+    // longer neighbour lists: the staged kernel, one query per warp
+    if (agg_mma_nh(Nq, K, Cin) == 2)
+        return launch_agg_mma<2, 2>(q, s, idx, x, rowflag_ws, kp, Nq, Ns, nq_dev, ns_dev, K, Cin, extent, wf, st);
+    return launch_agg_mma<1, 4>(q, s, idx, x, rowflag_ws, kp, Nq, Ns, nq_dev, ns_dev, K, Cin, extent, wf, st);
 }
 
 int regtr_kpconv_fwd(const float* q, const float* s, const int32_t* idx, const float* x, const float* W,

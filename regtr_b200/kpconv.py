@@ -44,11 +44,6 @@ def level_capacities(cfg, cap0: int, ratio: float = 0.40, quantum: int = 256):
     return caps
 
 
-# InstanceNorm statistics from the producing GEMM's epilogue (32-row partial sums); False: the stand-alone
-# two-pass statistics kernel (A/B accuracy and timing measurements, tests/diag_accuracy.py)
-EPILOGUE_STATS = True
-
-
 class DenseGridOverflow(RuntimeError):
     """REGTR_STATUS_GRID: redo the pyramid with the sort-based voxel sub-sampling (`build(dense=False)`)."""
 
@@ -326,7 +321,7 @@ class UnaryBlock(nn.Module):
         """skip=True also returns x, as the last element, for the block's shortcut branch: in training its gradient
         is then added in this layer's dX GEMM (ops.linear_instats) instead of by autograd."""
         slope = final_slope if final_slope is not None else (-1.0 if self.no_relu else 0.1)
-        if self.use_bn and self.out_dim % 32 == 0 and EPILOGUE_STATS:
+        if self.use_bn and self.out_dim % 32 == 0:
             # Linear with the InstanceNorm statistics accumulated in the GEMM epilogue, then the apply pass
             y, stats, *xs = ops.linear_instats(x, self.mlp.weight, offs, n_clouds, m_dev=m_dev, skip=skip)
             out = self.batch_norm.apply(y, stats, offs, n_clouds, res=res, slope=slope, want_flags=want_flags)
@@ -407,7 +402,7 @@ class ResnetBottleneckBlock(nn.Module):
         else:
             x = self.unary1.fuse(features, offs_pre, nc, m_dev=ns_dev) if isinstance(self.unary1, UnaryBlock) \
                 else features
-        if self.use_bn and self.KPConv.out_channels % 32 == 0 and EPILOGUE_STATS:
+        if self.use_bn and self.KPConv.out_channels % 32 == 0:
             x, stats = self.KPConv(q, s, idx, x, nq_dev, ns_dev, row_flags=flags, instats=(offs_post, nc))
             x = self.batch_norm_conv.apply(x, stats, offs_post, nc, slope=0.1)
         else:

@@ -10,7 +10,6 @@ import contextlib
 import ctypes
 import itertools
 import math
-import os
 
 import numpy as np
 import torch
@@ -898,17 +897,9 @@ def dropout_keep_mask(p: float, seed: int, step: int, pair_base: int, n_pairs: i
     return out
 
 
-def _check_drop_core():
-    impl = os.environ.get('REGTR_MHA_IMPL')
-    if impl and impl[0] == 'f':
-        raise _lib.RegtrLibError('attention dropout runs on the default 3xTF32 attention core only; unset '
-                                 'REGTR_MHA_IMPL=ffma (the CUDA-core A/B kernel) to train with dropout > 0')
-
-
 def mha_varlen_lse_dropout(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int, drop: _DropSite):
     """mha_varlen_lse with the attention-probability dropout of `drop` (problem c = local query cloud c)."""
     L = _lib.load()
-    _check_drop_core()
     for t, nm in ((q, 'q'), (k, 'k'), (v, 'v')):
         if not t.is_cuda or t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1:
             raise ValueError(f'mha_varlen: {nm} must be a CUDA fp32 matrix with unit column stride')

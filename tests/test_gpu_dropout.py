@@ -391,15 +391,6 @@ def test_training_with_dropout_lowers_the_loss():
     assert after < before
 
 
-def test_ffma_core_refuses_dropout(monkeypatch):
-    from regtr_b200 import lib
-    case = 'fwd_modelnet_b1'
-    _, m1, src, tgt = _models(case)
-    monkeypatch.setenv('REGTR_MHA_IMPL', 'ffma')
-    with pytest.raises(lib.RegtrLibError, match='REGTR_MHA_IMPL'):
-        m1.forward_train(_batch(case, src, tgt), dropout_key=(0, 0, 0))
-
-
 # ----------------------------------------------------------------------------------------- against the reference
 
 @pytest.mark.parametrize('case', ['fwd_modelnet_b1', 'fwd_3dmatch_small_b2'])

@@ -7,7 +7,7 @@ tests/attention_oracle.py.  The inputs target the places where these kernels go 
   * InstanceNorm statistics (`gemm_instats` -> `instnorm_apply`, and `instnorm_act`): channels whose mean is 0, 3, 30
     and 300 times their spread, clouds of 1, 31, 32, 33, 700 and 4000 rows whose boundaries fall inside the GEMM
     epilogue's 32-row groups, and a split-K shape;
-  * attention forward cores (`mha_varlen` in both implementations, the lse of `mha_varlen_lse`, `mha_tf32_tc`): the
+  * attention forward cores (`mha_varlen`, the lse of `mha_varlen_lse`, `mha_tf32_tc`): the
     input families of tests/attention_oracle.py, self problems around the 64- and 128-query tiles, O(k + c) = O and
     O(v + c) = O + c per problem and head;
   * `corr_decode`: six layers, key clouds of 1, 31, 32 and 33 points around the 32-key chunk, a peaked softmax,
@@ -211,7 +211,7 @@ def _proj(x, w, b, dtype):
     return y[:, :E], y[:, E:2 * E], y[:, 2 * E:]
 
 
-def _run_core(core, c, dk=None, dv=None, monkeypatch=None):
+def _run_core(core, c, dk=None, dv=None):
     """The core's O (and lse for 'lse') on the family's inputs with c added to every key (dk) / value (dv)."""
     from regtr_b200 import ops
     tb = _dev_tables(c['problems'])
@@ -233,7 +233,6 @@ def _run_core(core, c, dk=None, dv=None, monkeypatch=None):
     if core == 'lse':
         o, lse = ops.mha_varlen_lse(*args)
         return o.cpu(), lse.cpu()
-    monkeypatch.setenv('REGTR_MHA_IMPL', core)
     return ops.mha_varlen(*args).cpu(), None
 
 
@@ -252,12 +251,12 @@ def _refs(c, core, dk=None, dv=None):
     return out
 
 
-def _attn_results(core, family, monkeypatch):
+def _attn_results(core, family):
     c = _attn_case(family)
     res = dict(c=c)
-    res['o'], res['lse'] = _run_core(core, c, monkeypatch=monkeypatch)
-    res['o_k'], _ = _run_core(core, c, dk=c['ck'], monkeypatch=monkeypatch)
-    res['o_v'], _ = _run_core(core, c, dv=c['cv'], monkeypatch=monkeypatch)
+    res['o'], res['lse'] = _run_core(core, c)
+    res['o_k'], _ = _run_core(core, c, dk=c['ck'])
+    res['o_v'], _ = _run_core(core, c, dv=c['cv'])
     (res['r64'], res['l64']), (res['r32'], res['l32']) = _refs(c, core)
     res['k32'] = _refs(c, core, dk=c['ck'])[1][0]
     res['v64'], res['v32'] = (r[0] for r in _refs(c, core, dv=c['cv']))
@@ -288,12 +287,12 @@ def _attn_checks(title, res, o=None, o_v=None):
 
 
 @pytest.mark.parametrize('family', FWD_FAMILIES)
-@pytest.mark.parametrize('core', ['mma', 'ffma', 'lse', 'tf32_tc'])
-def test_attention_forward_core_vs_float64(core, family, monkeypatch):
+@pytest.mark.parametrize('core', ['mma', 'lse', 'tf32_tc'])
+def test_attention_forward_core_vs_float64(core, family):
     """O (and the lse of mha_varlen_lse) under the yardstick for the self and the cross problems; O(k + c) = O and
-    O(v + c) = O + c per problem and head.  Cores: mha_varlen ('mma': the 3xTF32 mma.sync default, 'ffma': CUDA
-    cores), mha_varlen_lse ('lse') and mha_tf32_tc (in-projection included, the families built through its bias)."""
-    res = _attn_results(core, family, monkeypatch)
+    O(v + c) = O + c per problem and head.  Cores: mha_varlen ('mma': the 3xTF32 mma.sync kernel), mha_varlen_lse
+    ('lse') and mha_tf32_tc (in-projection included, the families built through its bias)."""
+    res = _attn_results(core, family)
     rows, inv = _attn_checks(f'attention forward, core {core}, {family} inputs', res)
     e = res['c']['problems'][-2]                          # queries of the empty-key cross problem: not rows above
     assert e[3] == 0 and e[1] > 0
@@ -301,14 +300,25 @@ def test_attention_forward_core_vs_float64(core, family, monkeypatch):
     assert not inv, inv[:8]
 
 
-def test_attention_forward_checks_are_sharp(monkeypatch):
-    """On the bias family and the default core: O x (1 + 1e-5) fails the self and cross O rows; O(v + c) + 1e-5 c, what
-    a P whose rows sum to 1 + 1e-5 gives, fails the O(v + c) invariant."""
-    res = _attn_results('mma', 'bias', monkeypatch)
+def test_attention_forward_checks_are_sharp():
+    """On the bias family and the mha_varlen core: O x (1 + 1e-5) fails the self and cross O rows; O(v + c) + 1e-5 c,
+    what a P whose rows sum to 1 + 1e-5 gives, fails the O(v + c) invariant."""
+    res = _attn_results('mma', 'bias')
     rows, _ = _attn_checks('bias inputs, O x (1 + 1e-5)', res, o=res['o'] * (1 + 1e-5))
     assert {'self O', 'cross O'} <= set(rows), rows
     _, inv = _attn_checks('bias inputs, O(v + c) + 1e-5 c', res, o_v=res['o_v'].double() + 1e-5 * res['c']['cv'].double())
     assert 'O(v + c) = O + c' in {r[0] for r in inv}, inv[:4]
+
+
+def test_mha_varlen_rejects_odd_ldo():
+    """The core stores its output two floats at a time: an odd output leading dimension is refused, not written."""
+    from regtr_b200 import lib, ops
+    c = _attn_case('zero_mean')
+    q, k, v = (t.to(DEV) for t in c['qkv'])
+    out = torch.zeros((q.shape[0], E + 1), device=DEV)[:, :E]
+    with pytest.raises(lib.RegtrLibError, match='REGTR_ERR_UNSUPPORTED'):
+        ops.mha_varlen(q, k, v, *_dev_tables(c['problems']), max(p[1] for p in c['problems']), H, out=out)
+    assert not out.any()
 
 
 # ------------------------------------------------------------------------------------------------ corr_decode
@@ -539,12 +549,11 @@ def test_pose_from_corr_layers_and_pairs_vs_float64():
 
 KP_OFFSET = np.array(XYZ_OFFSET)
 KP_NQ, KP_EXTENT, KP_RADIUS = 301, 0.05, 0.0625         # the 3DMatch config's first level
-KP_PATHS = ([(1, 'fused'), (1, 'aggregate'), (4, 'default')] +
-            [(c, impl) for c in (32, 64, 128, 256) for impl in ('default', 'mma', 'ffma')])
+KP_PATHS = [(1, 'fused'), (1, 'aggregate'), (4, 'default')] + [(c, 'default') for c in (32, 64, 128, 256)]
 _KPC = {}
 
 
-def _kp_inputs(cin, K):
+def _kp_inputs(cin, K, nq=KP_NQ):
     """Model-like KPConv inputs: queries ~2.5 m from the origin, per query its own support rows -- three at a kernel
     point's extent (exactly, and 2 ulp inside / outside), the rest in the radius ball -- scattered over the K slots
     with shadow slots (id == Ns) between them.  Feature rows: every 5th sums to exactly 0, every 7th is negative (both
@@ -555,9 +564,9 @@ def _kp_inputs(cin, K):
     kp[1:] = d / np.linalg.norm(d, axis=1, keepdims=True) * rng.uniform(0.25, 0.65, (14, 1)) * KP_RADIUS
     kp = kp.astype(np.float32)
     ext = float(np.float32(KP_EXTENT))
-    q = (KP_OFFSET + rng.normal(size=(KP_NQ, 3)) * 0.4).astype(np.float32)
-    s_rows, idx = [], np.empty((KP_NQ, K), dtype=np.int64)
-    for i in range(KP_NQ):
+    q = (KP_OFFSET + rng.normal(size=(nq, 3)) * 0.4).astype(np.float32)
+    s_rows, idx = [], np.empty((nq, K), dtype=np.int64)
+    for i in range(nq):
         n = 0 if i == 7 else int(rng.integers(1, K + 1)) if i % 3 else K
         rel = rng.normal(size=(n, 3))
         rel = rel / np.linalg.norm(rel, axis=1, keepdims=True) * KP_RADIUS * rng.uniform(0, 1, (n, 1)) ** (1 / 3)
@@ -600,17 +609,13 @@ def _kp_ref(c, dtype):
     return wf.reshape(len(q), -1), out
 
 
-def _kp_case(cin, impl, K, monkeypatch):
+def _kp_case(cin, impl, K, nq=KP_NQ):
     """GPU results of one path on _kp_inputs, exact-shaped and capacity-shaped, and the float64 / fp32 references."""
-    key = (cin, impl, K)
+    key = (cin, impl, K, nq)
     if key in _KPC:
         return _KPC[key]
     from regtr_b200 import ops
-    if impl in ('mma', 'ffma'):
-        monkeypatch.setenv('REGTR_AGG_IMPL', impl)
-    else:
-        monkeypatch.delenv('REGTR_AGG_IMPL', raising=False)
-    c = _kp_inputs(cin, K)
+    c = _kp_inputs(cin, K, nq)
     G = lambda a, dt=None: torch.from_numpy(np.ascontiguousarray(a)).to(DEV, dt)
     q, s, idx, x, W, kp = G(c['q']), G(c['s']), G(c['idx'], torch.int32), G(c['x']), G(c['W']), G(c['kp'])
     r = dict(ref=c)
@@ -621,7 +626,7 @@ def _kp_case(cin, impl, K, monkeypatch):
         r['out'] = ops.kpconv(q, s, idx, x, W, kp, c['extent']).cpu()
         r['out2'] = ops.kpconv(q, s, idx, x, W, kp, c['extent']).cpu()
     if cin > 1 and impl != 'aggregate':            # the InstanceNorm-statistics GEMM epilogue, two clouds
-        lens = [180, KP_NQ - 180]
+        lens = [180, nq - 180]
         o, st = ops.kpconv(q, s, idx, x, W, kp, c['extent'], instats=(ops.make_offsets(lens, DEV), 2))
         r['instats'] = (lens, o.cpu(), st.cpu())
     # capacity form: garbage query / support / feature rows past nq_dev / ns_dev; the real rows' shadow id Ns is a
@@ -632,13 +637,13 @@ def _kp_case(cin, impl, K, monkeypatch):
     sc = G(np.r_[c['s'], g.uniform(-1e3, 1e3, (ps, 3))].astype(np.float32))
     xc = G(np.r_[c['x'], np.full((ps, cin), 1e3)].astype(np.float32))
     ic = G(np.r_[c['idx'], g.integers(0, c['Ns'] + ps, (pq, K))], torch.int32)
-    nq_dev, ns_dev = (torch.tensor([v], dtype=torch.int32, device=DEV) for v in (KP_NQ, c['Ns']))
+    nq_dev, ns_dev = (torch.tensor([v], dtype=torch.int32, device=DEV) for v in (nq, c['Ns']))
     if not (cin == 1 and impl == 'fused'):
-        wf = torch.full((KP_NQ + pq, 15 * cin), math.nan, device=DEV)
+        wf = torch.full((nq + pq, 15 * cin), math.nan, device=DEV)
         ops.kpconv_aggregate(qc, sc, ic, xc, kp, c['extent'], wf=wf, nq_dev=nq_dev, ns_dev=ns_dev)
         r['wf_cap'] = wf.cpu()
     if impl != 'aggregate':
-        out = torch.full((KP_NQ + pq, W.shape[2]), math.nan, device=DEV)
+        out = torch.full((nq + pq, W.shape[2]), math.nan, device=DEV)
         ops.kpconv(qc, sc, ic, xc, W, kp, c['extent'], out=out, nq_dev=nq_dev, ns_dev=ns_dev)
         r['out_cap'] = out.cpu()
     torch.cuda.synchronize()
@@ -654,12 +659,13 @@ def _kp_rows(title, r, wf=None, out=None):
     ys = Yardstick(title)
     wf = r.get('wf') if wf is None else wf
     out = r.get('out') if out is None else out
+    nq = len(r['ref']['q'])
     if wf is not None:
         ys.add('wf', wf, r['wf32'], r['wf64'])
-        ys.add('wf, capacity form', r['wf_cap'][:KP_NQ], r['wf32'], r['wf64'])
+        ys.add('wf, capacity form', r['wf_cap'][:nq], r['wf32'], r['wf64'])
     if out is not None:
         ys.add('out', out, r['out32'], r['out64'])
-        ys.add('out, capacity form', r['out_cap'][:KP_NQ], r['out32'], r['out64'])
+        ys.add('out, capacity form', r['out_cap'][:nq], r['out32'], r['out64'])
     if 'instats' in r:
         lens, o, st = r['instats']
         ys.add('out, statistics epilogue', o, r['out32'], r['out64'])
@@ -671,35 +677,45 @@ def _kp_rows(title, r, wf=None, out=None):
     return ys
 
 
-@pytest.mark.parametrize('K', [40, 50, 72])
-@pytest.mark.parametrize('cin,impl', KP_PATHS, ids=[f'{c}-{i}' for c, i in KP_PATHS])
-def test_kpconv_vs_float64(cin, impl, K, monkeypatch):
-    """Every KPConv dispatch path -- Cin = 1 fused (regtr_kpconv_fwd) and aggregate-only, the small-Cin kernel, Cin 32
-    to 256 through the default pipelined kernel (K <= 64; K = 72 falls through to the staged tensor-core kernel),
-    REGTR_AGG_IMPL=mma and ffma, and the statistics GEMM epilogue -- under the yardstick against float64, at K = 40
-    and 50 (the configs' limits) and 72.  Two calls are bit-identical; the capacity form's real rows equal the
-    exact-shaped call's aggregation bit for bit, and its padding rows up to the consumer GEMM's 128-row tile are 0."""
-    r = _kp_case(cin, impl, K, monkeypatch)
-    ys = _kp_rows(f'kpconv Cin={cin} {impl}, K={K}', r)
+def _kp_check(cin, impl, K, nq=KP_NQ):
+    """One path under the yardstick against float64; two calls are bit-identical; the capacity form's real rows equal
+    the exact-shaped call's aggregation bit for bit, and its padding rows up to the consumer GEMM's 128-row tile are 0."""
+    r = _kp_case(cin, impl, K, nq)
+    ys = _kp_rows(f'kpconv Cin={cin} {impl}, K={K}, Nq={nq}', r)
     for a, b in (('wf', 'wf2'), ('out', 'out2')):
         if a in r:
             assert torch.equal(r[a], r[b]), f'{a} not bit-identical from call to call'
+    band = (nq + 127) // 128 * 128
     if 'wf' in r:
-        assert torch.equal(r['wf_cap'][:KP_NQ], r['wf']), 'capacity-form aggregation differs from the exact-shaped one'
-        band = (KP_NQ + 127) // 128 * 128
-        assert torch.equal(r['wf_cap'][KP_NQ:band], torch.zeros_like(r['wf_cap'][KP_NQ:band])), 'padding rows not 0'
+        assert torch.equal(r['wf_cap'][:nq], r['wf']), 'capacity-form aggregation differs from the exact-shaped one'
+        assert torch.equal(r['wf_cap'][nq:band], torch.zeros_like(r['wf_cap'][nq:band])), 'padding rows not 0'
     if 'out' in r and cin == 1:
-        band = (KP_NQ + 127) // 128 * 128
-        assert torch.equal(r['out_cap'][KP_NQ:band], torch.zeros_like(r['out_cap'][KP_NQ:band])), 'padding rows not 0'
+        assert torch.equal(r['out_cap'][nq:band], torch.zeros_like(r['out_cap'][nq:band])), 'padding rows not 0'
     empty = r.get('out', r.get('wf'))[7]
     assert float(empty.abs().max()) == 0.0, 'a query without valid neighbours must give 0'
     assert not ys.failures(), ys.failures()
 
 
-def test_kpconv_checks_are_sharp(monkeypatch):
+@pytest.mark.parametrize('K', [40, 50, 72])
+@pytest.mark.parametrize('cin,impl', KP_PATHS, ids=[f'{c}-{i}' for c, i in KP_PATHS])
+def test_kpconv_vs_float64(cin, impl, K):
+    """Every KPConv dispatch path -- Cin = 1 fused (regtr_kpconv_fwd) and aggregate-only, the small-Cin kernel, Cin 32
+    to 256 through the pipelined kernel (K <= 64) and the staged tensor-core kernel (K = 72, one 32-channel group per
+    warp at this query count), and the statistics GEMM epilogue -- at K = 40 and 50 (the configs' limits) and 72."""
+    _kp_check(cin, impl, K)
+
+
+@pytest.mark.parametrize('K', [72, 128])
+def test_kpconv_channel_groups_vs_float64(K):
+    """The staged tensor-core kernel at Cin = 256 with 2048 queries, enough warps for two 32-channel groups per warp:
+    at K = 72 it takes two; at K = 128 two groups' staged rows exceed the shared memory, and it takes one."""
+    _kp_check(256, 'default', K, 2048)
+
+
+def test_kpconv_checks_are_sharp():
     """wf or out multiplied by (1 + 1e-5) fails its row, on the fused Cin = 1 path and the default Cin = 64 path."""
     for cin, impl in ((1, 'aggregate'), (1, 'fused'), (64, 'default')):
-        r = _kp_case(cin, impl, 40, monkeypatch)
+        r = _kp_case(cin, impl, 40)
         if 'wf' in r:
             assert 'wf' in _kp_rows(f'kpconv Cin={cin} {impl}, wf x (1 + 1e-5)', r, wf=r['wf'] * (1 + 1e-5)).failures()
         if 'out' in r:
