@@ -507,6 +507,25 @@ int regtr_overlap_nn(const double* xyz, const int32_t* offs, int B, int n_cap, c
 int regtr_registration_fit(const double* xyz, const int32_t* offs, int B, int n_cap, const double* pose,
                            double radius, const int32_t* nn, double* out, uint32_t* status, void* stream);
 
+/* Point-to-point ICP of B pairs (Open3D's registration_icp with TransformationEstimationPointToPoint, no scaling,
+ * and ICPConvergenceCriteria(rel_fitness, rel_rmse, max_iter)).  xyz (n_cap,3) float64 stacked src_0..src_{B-1},
+ * tgt_0..tgt_{B-1} with offs (2B+1) i32; init (B,3,4) float64 source -> target.  Per pair: P = init . source
+ * (((r0 x + r1 y) + r2 z) + t, no contraction), T = init; correspondences are regtr_overlap_nn's (the nearest target
+ * point with float64 d^2 strictly below max_dist^2, ties to the lowest index), fitness = k / n_src,
+ * rmse = sqrt(sum d^2 / k) (both 0 without inliers).  Then up to max_iter times: the Umeyama update without scaling
+ * on the correspondences (the identity when k = 0), T = update . T, P moved by the update in place, re-match; stop
+ * when |d fitness| < rel_fitness and |d rmse| < rel_rmse.  pose_out (B,3,4) float64 = T; result (B,4) float64 =
+ * (fitness, rmse, k, iterations run).  One cell list over the targets (cell `cell`, use max_dist * (1 + 1e-3)), then
+ * 3 launches per round for max_iter + 1 rounds whatever B and convergence; no host synchronisation; sums in a fixed
+ * order, so the result is bit-reproducible and independent of the batch.  A coordinate of a moved source or of a
+ * target beyond regtr_overlap_coord_bound(max_dist, cell), or not finite, raises REGTR_STATUS_RANGE.  ws / state:
+ * the *_bytes functions below (state ZERO before the first call; every call leaves it zero). */
+size_t regtr_icp_ws_bytes(int n_cap, int B);
+size_t regtr_icp_state_bytes(int n_cap);
+int regtr_icp(const double* xyz, const int32_t* offs, int B, int n_cap, const double* init, double max_dist,
+              float cell, int max_iter, double rel_fitness, double rel_rmse, double* pose_out, double* result,
+              uint32_t* status, void* ws, size_t ws_bytes, void* state, size_t state_bytes, void* stream);
+
 /* Per-pair flags of regtr_train_augment */
 #define REGTR_PREP_PERTURB_SRC 1  /* the perturbation moves the source (else the target) */
 #define REGTR_PREP_CENTRE 2       /* rotate about the perturbed cloud's centroid ('small' mode) */

@@ -7,88 +7,11 @@
 // condition number); singular values are sorted descending so that the reflection fix
 // flips the direction of the smallest one, exactly as `v_neg[..., 2] *= -1` does on
 // torch.svd's descending output (se3_torch.py:143-148).
-#include "common.cuh"
+#include "rigid.cuh"
 
 namespace {
 
 struct Mat3 { double m[3][3]; };
-
-__device__ void svd3_jacobi(const double A_in[3][3], double U[3][3], double S[3], double V[3][3]) {
-    double A[3][3];
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) { A[i][j] = A_in[i][j]; V[i][j] = (i == j) ? 1.0 : 0.0; }
-    for (int sweep = 0; sweep < 30; ++sweep) {
-        double off = 0.0;
-        for (int p = 0; p < 2; ++p) {
-            for (int q = p + 1; q < 3; ++q) {
-                double alpha = 0.0, beta = 0.0, gamma = 0.0;
-                for (int i = 0; i < 3; ++i) {
-                    alpha += A[i][p] * A[i][p];
-                    beta += A[i][q] * A[i][q];
-                    gamma += A[i][p] * A[i][q];
-                }
-                if (gamma == 0.0) continue;
-                const double lim = sqrt(alpha * beta);
-                if (fabs(gamma) <= 1e-300 || fabs(gamma) <= 1e-17 * lim) continue;
-                off = fmax(off, fabs(gamma) / (lim > 0.0 ? lim : 1.0));
-                const double zeta = (beta - alpha) / (2.0 * gamma);
-                const double t = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
-                const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
-                for (int i = 0; i < 3; ++i) {
-                    const double ap = A[i][p], aq = A[i][q];
-                    A[i][p] = c * ap - s * aq;
-                    A[i][q] = s * ap + c * aq;
-                    const double vp = V[i][p], vq = V[i][q];
-                    V[i][p] = c * vp - s * vq;
-                    V[i][q] = s * vp + c * vq;
-                }
-            }
-        }
-        if (off < 1e-15) break;
-    }
-    for (int j = 0; j < 3; ++j) S[j] = sqrt(A[0][j] * A[0][j] + A[1][j] * A[1][j] + A[2][j] * A[2][j]);
-    // sort columns by descending singular value
-    int ord[3] = {0, 1, 2};
-    for (int a = 0; a < 2; ++a)
-        for (int b = a + 1; b < 3; ++b)
-            if (S[ord[b]] > S[ord[a]]) { int t = ord[a]; ord[a] = ord[b]; ord[b] = t; }
-    double As[3][3], Vs[3][3], Ss[3];
-    for (int j = 0; j < 3; ++j) {
-        Ss[j] = S[ord[j]];
-        for (int i = 0; i < 3; ++i) { As[i][j] = A[i][ord[j]]; Vs[i][j] = V[i][ord[j]]; }
-    }
-    for (int j = 0; j < 3; ++j) {
-        S[j] = Ss[j];
-        for (int i = 0; i < 3; ++i) V[i][j] = Vs[i][j];
-    }
-    // U columns = A columns / sigma; complete degenerate directions by cross products
-    const double tiny = 1e-200 + 1e-14 * S[0];
-    for (int j = 0; j < 3; ++j) {
-        if (S[j] > tiny) {
-            for (int i = 0; i < 3; ++i) U[i][j] = As[i][j] / S[j];
-        } else if (j == 0) {
-            U[0][0] = 1.0; U[1][0] = 0.0; U[2][0] = 0.0;
-        } else if (j == 1) {
-            // any unit vector orthogonal to u0
-            const double ax = fabs(U[0][0]), ay = fabs(U[1][0]), az = fabs(U[2][0]);
-            double e[3] = {0.0, 0.0, 0.0};
-            if (ax <= ay && ax <= az) e[0] = 1.0; else if (ay <= az) e[1] = 1.0; else e[2] = 1.0;
-            double d = e[0] * U[0][0] + e[1] * U[1][0] + e[2] * U[2][0];
-            double w[3] = {e[0] - d * U[0][0], e[1] - d * U[1][0], e[2] - d * U[2][0]};
-            const double n = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
-            for (int i = 0; i < 3; ++i) U[i][1] = w[i] / n;
-        } else {
-            U[0][2] = U[1][0] * U[2][1] - U[2][0] * U[1][1];
-            U[1][2] = U[2][0] * U[0][1] - U[0][0] * U[2][1];
-            U[2][2] = U[0][0] * U[1][1] - U[1][0] * U[0][1];
-        }
-    }
-}
-
-__device__ __forceinline__ double det3(const double M[3][3]) {
-    return M[0][0] * (M[1][1] * M[2][2] - M[1][2] * M[2][1]) - M[0][1] * (M[1][0] * M[2][2] - M[1][2] * M[2][0]) +
-           M[0][2] * (M[1][0] * M[2][1] - M[1][1] * M[2][0]);
-}
 
 // Loader abstraction: point i of a problem -> (a, b, w).
 struct PlainLoader {

@@ -10,6 +10,7 @@
 // the whole batch, and nothing synchronises with the host.
 #include "cellgrid.cuh"
 #include "philox.cuh"
+#include "rigid.cuh"
 
 extern "C" int regtr_cellgrid_build(const float* xyz, const int32_t* offs, int n_clouds, int n_cap, float cell,
                                     void* grid, int32_t* order, uint32_t* status, void* ws, size_t ws_bytes,
@@ -21,11 +22,6 @@ extern "C" size_t regtr_cellgrid_state_bytes(int n_cap);
 namespace {
 
 constexpr int NN_WARPS = 8;
-
-// ((m0 x + m1 y) + m2 z) + m3 in float64, no contraction: the fixed operation order of every rigid transform here
-__device__ __forceinline__ double rt_row(const double* m, double x, double y, double z) {
-    return __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(m[0], x), __dmul_rn(m[1], y)), __dmul_rn(m[2], z)), m[3]);
-}
 
 // ------------------------------------------------------------------------------------------------- overlap
 // Source clouds moved by the ground-truth pose in float64 (the reference's se3_transform(pose, src_xyz) on the

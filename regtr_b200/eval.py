@@ -376,6 +376,25 @@ def summarize_modelnet_metrics(metrics: Dict[str, np.ndarray]) -> Dict[str, floa
 # ------------------------------------------------------------------- test loop (reference: test.py)
 
 
+def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None):
+    """Wrap `forward_fn(batch) -> pred` so that the final pose of every pair is refined by point-to-point ICP on the
+    batch's full clouds: -> a NEW dict with pred's entries, pose (1,B,3,4) float64 the refined poses and pose_coarse
+    (1,B,3,4) float64 the network's final poses (so that `compute_metrics` reports both, and EstLogWriter writes the
+    refined ones).  pred's own tensors are not written to (a graphed forward owns them).
+    icp(src_list, tgt_list, init (B,3,4), radius, max_iteration) -> (pose (B,3,4), result): default `ops.icp`."""
+    if icp is None:
+        from .ops import icp
+    def run(batch):
+        pred = forward_fn(batch)
+        coarse = pred['pose'][-1].to(torch.float64)                     # (B,3,4), a new tensor
+        pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration)
+        out = dict(pred)
+        out['pose'] = torch.as_tensor(pose, dtype=torch.float64, device=coarse.device).reshape(coarse.shape)[None]
+        out['pose_coarse'] = coarse[None]
+        return out
+    return run
+
+
 def run_3dmatch_benchmark(batches: Iterable[Dict], forward_fn, log_path: str, benchmark: str, gt_folder: str,
                           thresh_rot=10.0, thresh_trans=0.1):
     """`Trainer.test` + `GenericRegModel.test_step/test_epoch_end` for the 3DMatch benchmarks
@@ -388,7 +407,7 @@ def run_3dmatch_benchmark(batches: Iterable[Dict], forward_fn, log_path: str, be
     for batch in batches:
         pred = forward_fn(batch)
         writer.append_batch(batch, pred)
-        gt = batch['pose'].to(pred['pose'].device)
+        gt = batch['pose'].to(pred['pose'].device, pred['pose'].dtype)
         per_batch.append({k: v.detach().cpu() for k, v in compute_metrics(pred, gt).items()})
     summary, recall, per_scene = benchmark_3dmatch(writer.root, gt_folder)
     return dict(summary=summary, recall=recall, per_scene=per_scene,

@@ -1354,16 +1354,77 @@ def registration_fit(src_list, tgt_list, pose, radius: float, status=None):
     return out
 
 
-def check_fit_status(status, radius: float):
-    """Read the status word of `registration_fit` (a host sync) and raise RegtrLibError if the fit is not exact."""
+def _stack_pairs(src_list, tgt_list, what: str, device=None):
+    """src_0..src_{B-1}, tgt_0..tgt_{B-1} stacked in float64 on the device -> (xyz (n,3), offs (2B+1), lens)."""
+    B = len(src_list)
+    if B == 0 or len(tgt_list) != B:
+        raise ValueError(f'{what}: expected as many source as target clouds, at least one pair')
+    dev = device if device is not None else torch.device('cuda', torch.cuda.current_device())
+    clouds = [torch.as_tensor(c) for c in list(src_list) + list(tgt_list)]
+    for c in clouds:
+        if c.dim() != 2 or c.shape[1] != 3:
+            raise ValueError(f'{what}: expected (n,3) clouds, got {tuple(c.shape)}')
+    lens = [int(c.shape[0]) for c in clouds]
+    xyz = torch.empty((max(sum(lens), 1), 3), dtype=torch.float64, device=dev)
+    a = 0
+    for c, ln in zip(clouds, lens):
+        xyz[a:a + ln].copy_(c.to(dev, torch.float64))
+        a += ln
+    return xyz, make_offsets(lens, dev), lens
+
+
+def icp_launches(max_iteration: int) -> int:
+    """Kernel launches of one `icp` call: the set-up, the targets' cell list (4), then 3 per round."""
+    return 5 + 3 * (int(max_iteration) + 1)
+
+
+def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iteration: int = 30,
+        relative_fitness: float = 1e-6, relative_rmse: float = 1e-6, status=None):
+    """Point-to-point ICP of B pairs (regtr_icp): Open3D's registration_icp with TransformationEstimationPointToPoint
+    (no scaling) and ICPConvergenceCriteria(relative_fitness, relative_rmse, max_iteration), on the device.
+    src_list / tgt_list: B clouds (n,3) each (numpy or torch, any float dtype; stacked in float64 on the device);
+    init (B,3,4) source -> target.  -> (pose (B,3,4) float64, result (B,4) float64 = fitness, inlier_rmse, n_corr,
+    iterations), both device tensors.  No host sync unless status is None: then a word of this call is read and a
+    coordinate of a moved source or of a target beyond `overlap_coord_bound(max_correspondence_distance)` raises
+    RegtrLibError; with the caller's word, `check_fit_status` does that where the caller syncs."""
+    L = _lib.load()
+    r = float(max_correspondence_distance)
+    if not r > 0.0 or int(max_iteration) < 0 or not (relative_fitness >= 0.0 and relative_rmse >= 0.0):
+        raise ValueError(f'icp: max_correspondence_distance {r} must be > 0, max_iteration {max_iteration} >= 0, '
+                         f'relative_fitness / relative_rmse >= 0')
+    B = len(src_list)
+    dev = init.device if torch.is_tensor(init) and init.is_cuda else None
+    xyz, offs, lens = _stack_pairs(src_list, tgt_list, 'icp', dev)
+    dev = xyz.device
+    init64 = torch.as_tensor(init).to(dev, torch.float64).reshape(B, 3, 4).contiguous()
+    n = sum(lens)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    pose = torch.empty((B, 3, 4), dtype=torch.float64, device=dev)
+    out = torch.empty((B, 4), dtype=torch.float64, device=dev)
+    ws = workspace(L.regtr_icp_ws_bytes(n, B), dev)
+    state = workspace(L.regtr_icp_state_bytes(n), dev, 'scan_state', zero=True)
+    _lib.check(L.regtr_icp(_p(xyz), _p(offs), B, n, _p(init64), r, overlap_cell(r), int(max_iteration),
+                           float(relative_fitness), float(relative_rmse), _p(pose), _p(out), _p(status), _p(ws),
+                           ws.numel(), _p(state), state.numel(), _stream()), 'regtr_icp')
+    _count(icp_launches(max_iteration))
+    if own:
+        check_fit_status(status, r, 'icp')
+    return pose, out
+
+
+def check_fit_status(status, radius: float, what: str = 'registration_fit'):
+    """Read the status word of `registration_fit` or `icp` (a host sync) and raise RegtrLibError if the result is not
+    exact."""
     word = int(status.item())
     if word & (STATUS_RANGE | 1):             # REGTR_STATUS_RANGE | REGTR_STATUS_KEY_RANGE
         raise _lib.RegtrLibError(
-            f'registration_fit: a coordinate of the moved source or of the target lies beyond +-'
+            f'{what}: a coordinate of the moved source or of the target lies beyond +-'
             f'{overlap_coord_bound(radius):.3f} (overlap_coord_bound({radius})), the range in which the nearest-'
             f'neighbour search at this radius is exact, or is not finite (status {word:#x})')
     if word & STATUS_INPUT:                   # REGTR_STATUS_INPUT (defined below)
-        raise _lib.RegtrLibError(f'registration_fit: a match the overlap search cannot have produced (status {word:#x})')
+        raise _lib.RegtrLibError(f'{what}: a match the overlap search cannot have produced (status {word:#x})')
 
 
 def train_augment(xyz, offs, B: int, n_src: int, pose, nn, pert, flags, seed: int, step: int, noise: float,

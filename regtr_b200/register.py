@@ -1,7 +1,7 @@
 """Register two point-cloud files with a trained RegTR: the reference's `src/demo.py` on the library path.
 
     python -m regtr_b200.register SRC TGT --ckpt <logdir>/ckpt/model-best.pth [--config <yaml>] \\
-        [--threshold 0.5] [--fit_radius R] [--out DIR]
+        [--threshold 0.5] [--fit_radius R] [--icp R [--icp_iters 30]] [--out DIR]
 
 SRC / TGT: .ply, .pth, .bin or .npy (regtr_b200.pointio).  The config is the config.yaml one level above the
 checkpoint's directory, the layout `python -m regtr_b200.train` writes, unless --config names another.  Instead of the
@@ -13,7 +13,12 @@ demo's viewer, the result is judged by the fitness and inlier RMSE of the final 
   src_registered.ply   the source moved by the pose;
   src_kp.ply, src_kp_warped.ply   the source keypoints with predicted overlap > --threshold and their predicted
                        positions in the target, with an `overlap` property (the demo's two upper panels).
-One JSON line on stdout: the pose, the four fit numbers and the point counts.
+With --icp R the final decoder layer's pose is refined by point-to-point ICP on the cropped full-resolution clouds
+(`ops.icp`, Open3D's registration_icp with max_correspondence_distance R and --icp_iters iterations at most);
+pose.txt, src_registered.ply and fit then use the refined pose, result.npz gains pose_coarse (the network's final
+pose), pose_icp (the refined one) and icp (4,) = fitness, inlier_rmse, correspondences, iterations.
+One JSON line on stdout: the pose, the four fit numbers and the point counts (with --icp, also icp_fitness, icp_rmse,
+icp_iterations and icp_radius).
 """
 from __future__ import annotations
 
@@ -37,6 +42,9 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument('--threshold', type=float, default=0.5,
                     help='Keypoints with predicted overlap above this go to src_kp.ply / src_kp_warped.ply')
     ap.add_argument('--fit_radius', type=float, help='Inlier radius of the fitness / RMSE (default: overlap_radius)')
+    ap.add_argument('--icp', type=float, metavar='R',
+                    help='Refine the pose with point-to-point ICP, max correspondence distance R (default: no ICP)')
+    ap.add_argument('--icp_iters', type=int, default=30, help='ICP iterations at most (with --icp)')
     ap.add_argument('--out', default='.', help='Output directory')
     return ap
 
@@ -63,10 +71,14 @@ def load_model(cfg, ckpt: str, device=None):
     return model
 
 
-def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: float = None) -> Dict:
+def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: float = None,
+             icp_radius: float = None, icp_iters: int = 30) -> Dict:
     """Crop, forward and fit one pair.  src_xyz / tgt_xyz (N,3) float64 host arrays.
     -> dict of host arrays: src_xyz / tgt_xyz (cropped, float64), pose (L,3,4) fp32, src_kp, src_kp_warped (final
-    layer), src_overlap (sigmoid of the final layer's logit, (n,)), the same for tgt, fit (4,) float64."""
+    layer), src_overlap (sigmoid of the final layer's logit, (n,)), the same for tgt, fit (4,) float64.
+    icp_radius: refine the final layer's pose by point-to-point ICP (`ops.icp`, at most icp_iters iterations) on the
+    cropped clouds; fit is then that of the refined pose, and the dict gains pose_coarse (3,4) fp32 (the network's
+    final pose), pose_icp (3,4) float64 and icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations."""
     from . import ops
     src_xyz = crop(cfg, np.asarray(src_xyz, dtype=np.float64))
     tgt_xyz = crop(cfg, np.asarray(tgt_xyz, dtype=np.float64))
@@ -78,8 +90,13 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
         pose = out['pose'][:, 0]                                             # (L,3,4), pair 0
         radius = float(cfg['overlap_radius'] if fit_radius is None else fit_radius)
         status = ops.new_status(dev)
-        fit = ops.registration_fit([src_xyz], [tgt_xyz], pose[-1:], radius, status)
+        final = pose[-1:]
+        if icp_radius is not None:
+            final, icp = ops.icp([src_xyz], [tgt_xyz], pose[-1:], icp_radius, icp_iters)
+        fit = ops.registration_fit([src_xyz], [tgt_xyz], final, radius, status)
         res = {'src_xyz': src_xyz, 'tgt_xyz': tgt_xyz, 'pose': pose.cpu().numpy()}
+        if icp_radius is not None:
+            res.update(pose_coarse=res['pose'][-1], pose_icp=final[0].cpu().numpy(), icp=icp[0].cpu().numpy())
         for side in ('src', 'tgt'):
             res[f'{side}_kp'] = out[f'{side}_kp'][0].cpu().numpy()
             res[f'{side}_kp_warped'] = out[f'{side}_kp_warped'][0][-1].cpu().numpy()
@@ -103,11 +120,13 @@ def pose_text(pose34) -> str:
 def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
     from .pointio import write_ply
     os.makedirs(out_dir, exist_ok=True)
-    final = res['pose'][-1]
+    final = res['pose_icp'] if 'pose_icp' in res else res['pose'][-1]
     with open(os.path.join(out_dir, 'pose.txt'), 'w') as fh:
         fh.write(pose_text(final))
-    np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in (
-        'pose', 'src_kp', 'src_kp_warped', 'src_overlap', 'tgt_kp', 'tgt_kp_warped', 'tgt_overlap', 'fit')})
+    keys = ('pose', 'src_kp', 'src_kp_warped', 'src_overlap', 'tgt_kp', 'tgt_kp_warped', 'tgt_overlap', 'fit')
+    if 'pose_icp' in res:
+        keys += ('pose_coarse', 'pose_icp', 'icp')
+    np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
     p = final.astype(np.float64)
     write_ply(os.path.join(out_dir, 'src_registered.ply'), res['src_xyz'] @ p[:, :3].T + p[:, 3])
     m = res['src_overlap'] > threshold
@@ -125,14 +144,20 @@ def main(argv=None):
         raise SystemExit(f'config not found: {cfg_file} (pass --config)')
     cfg = load_config(str(cfg_file))
     model = load_model(cfg, opt.ckpt)
-    res = register(model, cfg, load_point_cloud(opt.src), load_point_cloud(opt.tgt), opt.fit_radius)
+    res = register(model, cfg, load_point_cloud(opt.src), load_point_cloud(opt.tgt), opt.fit_radius, opt.icp,
+                   opt.icp_iters)
     n_shown = write_outputs(res, opt.out, opt.threshold)
     f = [float(v) for v in res['fit']]
-    print(json.dumps({'pose': pose44(res['pose'][-1]).tolist(), 'fitness_src': f[0], 'rmse_src': f[1],
-                      'fitness_tgt': f[2], 'rmse_tgt': f[3], 'n_src': int(res['src_xyz'].shape[0]),
-                      'n_tgt': int(res['tgt_xyz'].shape[0]), 'n_src_kp': int(res['src_kp'].shape[0]),
-                      'n_tgt_kp': int(res['tgt_kp'].shape[0]), 'n_src_kp_above_threshold': n_shown,
-                      'fit_radius': float(cfg['overlap_radius'] if opt.fit_radius is None else opt.fit_radius)}))
+    line = {'pose': pose44(res['pose_icp'] if opt.icp is not None else res['pose'][-1]).tolist(),
+            'fitness_src': f[0], 'rmse_src': f[1],
+            'fitness_tgt': f[2], 'rmse_tgt': f[3], 'n_src': int(res['src_xyz'].shape[0]),
+            'n_tgt': int(res['tgt_xyz'].shape[0]), 'n_src_kp': int(res['src_kp'].shape[0]),
+            'n_tgt_kp': int(res['tgt_kp'].shape[0]), 'n_src_kp_above_threshold': n_shown,
+            'fit_radius': float(cfg['overlap_radius'] if opt.fit_radius is None else opt.fit_radius)}
+    if opt.icp is not None:
+        icp = [float(v) for v in res['icp']]
+        line.update(icp_fitness=icp[0], icp_rmse=icp[1], icp_iterations=int(icp[3]), icp_radius=float(opt.icp))
+    print(json.dumps(line))
     return res
 
 
