@@ -197,12 +197,37 @@ int regtr_gemm_tf32x3_instats(const float* A, int lda, const float* B_hi, const 
 int regtr_pos_embed_sine(const float* xyz, int n, const float* dim_t, int n_freq, int d_model,
                          float scale, float* out, void* stream);
 
+/* The six dropouts of TransformerCrossEncoderLayer.forward_pre in train mode (transformers.py:85-110, 183-244), all
+ * with the same p: site 1 the self-attention probabilities, 2 the self-attention output (dropout1), 3 the cross-
+ * attention probabilities, 4 the cross-attention output (dropout2), 5 relu(linear1) (dropout), 6 the linear2 output
+ * (dropout3).  Masks are regenerated, never stored: the keep decision of (row, column) of a site is a Philox4x32-10
+ * draw keyed by (seed, step, global cloud 2 (pair_base + b) + side, layer, site, head, row, column) -- independent of
+ * the batch size, packing, rank and launch configuration (counter layout: regtr_b200/csrc/philox.cuh).  Row: token
+ * within the (query) cloud; column: key index within the key cloud (sites 1, 3) or feature index (head 0).  Local
+ * cloud c of the (src x B, tgt x B) stack is pair c % B, side c / B (B = n_pairs).  A value is dropped when its 16-bit
+ * draw is below `threshold` = round(p 65536); kept values are multiplied by `scale` = fp32(1 / (1 - p)).  Limits:
+ * 2 (pair_base + n_pairs) <= 2^20, layer < 16, head < 16, clouds shorter than 2^16 tokens.  Passed by host pointer. */
+typedef struct regtr_dropout_args {
+    unsigned long long seed, step;
+    int32_t pair_base;      /* global index of the batch's first pair */
+    int32_t layer;          /* 0..15 */
+    int32_t site;           /* 1..6 */
+    uint32_t threshold;     /* round(p * 65536), <= 65536 */
+    float scale;            /* fp32(1 / (1 - p)) */
+    int32_t n_pairs;        /* B */
+} regtr_dropout_args;
+
 /* LayerNorm over the last dim with optional position add:  y = LN(x)*g + b ;
  * y_pos = y + pos.  Replaces nn.LayerNorm + with_pos_embed (transformers.py:117-119,
  * 194-196, 213-215, 232).  Any of y / y_pos may be NULL.  n_dev (optional, device): the real row count
- * when n is a capacity; rows beyond it are left untouched. */
-int regtr_layernorm_pos(const float* x, const float* gamma, const float* beta, const float* pos,
-                        int n, const int32_t* n_dev, int E, float eps, float* y, float* y_pos, void* stream);
+ * when n is a capacity; rows beyond it are left untouched.
+ * drop (optional): the residual dropout fused into the LayerNorm that follows it (sites 2, 4, 6):  x' = x + m scale z
+ * (z: the out-projection / linear2 output), x_out = x', and the LayerNorm is that of x'.  offs (2B + 1, device): cloud
+ * offsets of the packed rows (n = offs[2B]).  z, offs, x_out and drop are all NULL or all set, and n_dev is NULL with
+ * drop; x_out must not alias x or z. */
+int regtr_layernorm_pos(const float* x, const float* z, const float* gamma, const float* beta, const float* pos, int n,
+                        const int32_t* n_dev, const int32_t* offs, int E, float eps, float* y, float* y_pos,
+                        float* x_out, const regtr_dropout_args* drop, void* stream);
 
 /* Device-side attention problem table for a (src x B, tgt x B) token stack with cloud offsets
  * offs (2B+1): plan (6, 2B+1) i32 rows = q_start, q_len, cross k_start, cross k_len (the cross
@@ -218,15 +243,22 @@ int regtr_attention_plan(const int32_t* offs, int B, int32_t* plan, void* stream
  * [k_start[i], k_start[i]+k_len[i]) of K/V.  Q/K/V/O are row-major with leading
  * dimensions ldq/ldk/ldv/ldo (floats); head h uses columns [h*head_dim, (h+1)*head_dim).
  * head_dim must be 32; ldo must be even (REGTR_ERR_UNSUPPORTED otherwise).  max_q_len: host upper bound of
- * q_len[]. */
-int regtr_mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
-                         float* O, int ldo, const int32_t* q_start, const int32_t* q_len,
-                         const int32_t* k_start, const int32_t* k_len, int n_problems,
-                         int max_q_len, const int32_t* tile_base, int max_tiles,
-                         int n_heads, int head_dim, float scale, void* stream);
-/* tile_base (optional, n_problems + 1, device): exclusive prefix of ceil(q_len / 64) with the total last; the launch
+ * q_len[].
+ * tile_base (optional, n_problems + 1, device): exclusive prefix of ceil(q_len / 64) with the total last; the launch
  * then covers max_tiles (a host bound of that total, e.g. capacity / 64 + n_problems) linear tiles instead of
- * ceil(max_q_len / 64) tiles per problem -- capacity-shaped launches know the per-problem lengths on the device only. */
+ * ceil(max_q_len / 64) tiles per problem -- capacity-shaped launches know the per-problem lengths on the device only.
+ * lse (optional, training): also writes lse [n_tokens, n_heads] = log2(sum_k exp2(s_qk)) of the base-2 scores
+ * s = (q * scale * log2 e) . k -- what regtr_mha_varlen_bwd recomputes the softmax from (-inf for a query whose key
+ * range is empty); O is the same, bit for bit.
+ * drop (optional, training; needs lse): the attention-probability dropout (site 1 or 3; the problem tables of
+ * regtr_attention_plan, problem c = query cloud c, n_heads <= 16): O = scale * sum_k m_qk P_qk V_k, the mask applied to
+ * the probabilities in registers before the P V product; lse is that of the undropped probabilities.
+ * tile_base together with lse or drop is REGTR_ERR_UNSUPPORTED. */
+int regtr_mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                         float* O, int ldo, float* lse, const int32_t* q_start, const int32_t* q_len,
+                         const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
+                         const int32_t* tile_base, int max_tiles, int n_heads, int head_dim, float scale,
+                         const regtr_dropout_args* drop, void* stream);
 
 /* CorrespondenceDecoder.simple_attention (regtr.py:316-351, the `direct_regress_coor: False` branch):
  * single-head attention whose values are the key coordinates,
@@ -271,14 +303,6 @@ int regtr_mha_tf32_tc_fwd(const float* qk4, int ld4, const float* vt2, int ld_vt
                           int max_tiles, int n_heads, int head_dim, void* stream);
 /* (tile_base / max_tiles as for regtr_mha_varlen_fwd, with 128-query tiles.) */
 
-/* Training forward of the regtr_mha_varlen_fwd core (the 3xTF32 mma.sync kernel): same O, bit for bit, plus
- * lse [n_tokens, n_heads] = log2(sum_k exp2(s_qk)) of the base-2 scores s = (q * scale * log2 e) . k -- what
- * regtr_mha_varlen_bwd recomputes the softmax from (-inf for a query whose key range is empty).  No tile table. */
-int regtr_mha_varlen_fwd_lse(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
-                             float* O, int ldo, float* lse, const int32_t* q_start, const int32_t* q_len,
-                             const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
-                             int n_heads, int head_dim, float scale, void* stream);
-
 /* Head-averaged attention probabilities (analysis; TransformerCrossEncoder.get_attentions):
  *   P[q, k] = (1/H) sum_h softmax_k(Q_h[q] . K_h[k] * scale)
  * for every (query range, key range) problem of the tables above -- nn.MultiheadAttention's weights with
@@ -295,7 +319,7 @@ int regtr_mha_probs_avg(const float* Q, int ldq, const float* K, int ldk, float*
 
 /* ---- backward (training) ---------------------------------------------------------- */
 
-/* Backward of the attention core over the same problem tables: given O and lse from regtr_mha_varlen_fwd_lse and
+/* Backward of the attention core over the same problem tables: given O and lse from regtr_mha_varlen_fwd and
  * dO, writes dQ (rows of every query range), dK and dV (rows of every key range; 0 for a key range whose problem
  * has no queries).  Each key row must belong to the key range of exactly one problem (true of the self and of the
  * cross table of regtr_attention_plan); dQ / dK / dV may be column slices of one packed [n_rows, 3E] buffer.
@@ -303,6 +327,8 @@ int regtr_mha_probs_avg(const float* Q, int ldq, const float* K, int ldk, float*
  * Deterministic (no atomics): one pass owns the query rows, a second one the key rows.  The softmax is renormalised
  * from the backward's own recomputed scores, and delta = sum_k P dP is formed from them too, so O is checked for
  * NULL but its values are not read.
+ * drop (optional): the forward's dropout key; dP_qk becomes g_qk = m_qk scale (dO_q . V_k), delta = sum_k P g,
+ * dV_k = sum_q P_qk m_qk scale dO_q.
  * ws: regtr_mha_varlen_bwd_ws_bytes(n_rows, n_heads) bytes (delta and 1 / sum_k exp2(s - lse) per query and head). */
 size_t regtr_mha_varlen_bwd_ws_bytes(int n_rows, int n_heads);
 int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
@@ -310,19 +336,24 @@ int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const
                          float* dQ, int lddq, float* dK, int lddk, float* dV, int lddv,
                          const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
                          const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len,
-                         int n_heads, int head_dim, float scale, void* ws, size_t ws_bytes, void* stream);
+                         int n_heads, int head_dim, float scale, const regtr_dropout_args* drop, void* ws,
+                         size_t ws_bytes, void* stream);
 
 /* Backward of regtr_layernorm_pos: dy and dy_pos (either may be NULL; they add) are the gradients of y and y_pos,
  * dres (optional) a gradient of x arriving through a residual connection, added to dx.  Mean and rstd are
  * recomputed from x.  dgamma / dbeta (E) from per-block column partials summed in a fixed order.  E % 32 == 0,
- * E <= 256.  ws: regtr_layernorm_bwd_ws_bytes(n, E) bytes. */
+ * E <= 256.  ws: regtr_layernorm_bwd_ws_bytes(n, E) bytes.
+ * drop (optional; offs, dz and drop are all NULL or all set): the backward of the residual dropout, with x = the
+ * forward's x_out: dx is the gradient of x' (dres included), plus dz = dx m scale. */
 size_t regtr_layernorm_bwd_ws_bytes(int n, int E);
 int regtr_layernorm_bwd(const float* x, const float* gamma, const float* dy, const float* dy_pos, const float* dres,
-                        int n, int E, float eps, float* dx, float* dgamma, float* dbeta,
-                        void* ws, size_t ws_bytes, void* stream);
+                        int n, const int32_t* offs, int E, float eps, float* dx, float* dz, float* dgamma, float* dbeta,
+                        const regtr_dropout_args* drop, void* ws, size_t ws_bytes, void* stream);
 
-/* ReLU backward: out = dh * (h > 0), h the ReLU's output (n elements; out may alias dh). */
-int regtr_relu_bwd(const float* dh, const float* h, long long n, float* out, void* stream);
+/* ReLU backward: out = dh * scale where h > 0, else 0 (n elements; out may alias dh).  h is the ReLU's output and
+ * scale = 1, or, with the feed-forward dropout, h is the dropped ReLU output of regtr_dropout_rows (positive exactly
+ * where the ReLU passed and the mask kept) and scale the dropout's. */
+int regtr_relu_bwd(const float* dh, const float* h, long long n, float scale, float* out, void* stream);
 
 /* Weight gradient of a dense layer Y = X W^T + b:  dW[N,K] = dY^T X,  db[N] = sum_rows dY (db optional),
  * 3xTF32 on regtr_gemm_tf32x3 (the reduction over the M rows uses its deterministic split-K).  X (M,K) and
@@ -543,23 +574,17 @@ int regtr_icp(const double* xyz, const int32_t* offs, int B, int n_cap, const do
  * corr (2, corr_cap >= n_src_cap) i32: mutual matches with a nonzero target index whose ends survive the truncation,
  * in ascending source index, remapped through the permutation (rows swapped for swapped pairs); pair b owns columns
  * [corr_offs[b], corr_offs[b+1]).  n_src_cap >= offs[B].  ws / state: the *_bytes functions (state ZERO before the
- * first call; every call leaves it zero). */
+ * first call; every call leaves it zero).  The device draws of pair b are keyed by pair_base + b (0 <= pair_base <=
+ * 2^30): a slice of a batch that starts at global pair pair_base draws exactly what those pairs draw in the whole
+ * batch; a whole batch passes 0. */
 size_t regtr_train_augment_ws_bytes(int n_src_cap, int B);
 size_t regtr_train_augment_state_bytes(int n_src_cap);
 int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
                         const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
-                        unsigned long long step, double noise, int max_pts, const int32_t* out_offs, int out_cap,
-                        float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
+                        unsigned long long step, int pair_base, double noise, int max_pts, const int32_t* out_offs,
+                        int out_cap, float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
                         int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
                         void* stream);
-/* regtr_train_augment with the device draws of pair b keyed by pair_base + b (0 <= pair_base <= 2^30): a slice of a
- * batch that starts at global pair pair_base draws exactly what those pairs draw in the whole batch. */
-int regtr_train_augment_at(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
-                           const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
-                           unsigned long long step, int pair_base, double noise, int max_pts, const int32_t* out_offs,
-                           int out_cap, float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
-                           int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
-                           void* stream);
 
 /* ---- training data (ModelNet40) --------------------------------------------------- */
 
@@ -585,6 +610,7 @@ int regtr_train_augment_at(const double* xyz, const int32_t* offs, int B, int n_
  * side's crop; corr (B, 2, n_out): (source position, target position) of every raw point present in both outputs, in
  * ascending raw index, corr_n (B) of them.  A crop with fewer than n_out points raises REGTR_STATUS_CROP, a bad item
  * or a non-finite coordinate REGTR_STATUS_INPUT; such a pair gets corr_n = 0.  The struct is passed by value.
+ * The device draws of pair b are keyed by pair_base + b (0 <= pair_base <= 2^30), as for regtr_train_augment.
  * One launch. */
 typedef struct {
     const float* shapes;
@@ -599,9 +625,7 @@ typedef struct {
     double gamma, noise, clip;
     int n_shapes, n_pts, n_out, k, B;
 } regtr_modelnet_args;
-int regtr_modelnet_augment(const regtr_modelnet_args* args, void* stream);
-/* regtr_modelnet_augment with the device draws of pair b keyed by pair_base + b (0 <= pair_base <= 2^30). */
-int regtr_modelnet_augment_at(const regtr_modelnet_args* args, int pair_base, void* stream);
+int regtr_modelnet_augment(const regtr_modelnet_args* args, int pair_base, void* stream);
 
 /* ---- training-loop bookkeeping ---------------------------------------------------- */
 
@@ -728,26 +752,23 @@ typedef struct {
     int pad_;
 } regtr_loss_args;
 size_t regtr_loss_ws_bytes(int N, int L);
-int regtr_loss_pointwise(const regtr_loss_args* args, void* stream);
+int regtr_loss_pointwise(const regtr_loss_args* args, const double* norm, void* stream);
 int regtr_loss_pointwise_bwd(const regtr_loss_args* args, void* stream);
 int regtr_infonce_match(const regtr_loss_args* args, void* stream);
 int regtr_infonce_fwd(const regtr_loss_args* args, void* stream);
-int regtr_infonce_bwd(const regtr_loss_args* args, void* stream);
-int regtr_loss_finalize(const regtr_loss_args* args, void* stream);
+int regtr_infonce_bwd(const regtr_loss_args* args, const double* norm, void* stream);
+int regtr_loss_finalize(const regtr_loss_args* args, const double* norm, void* stream);
 
 /* Batch-global normalisers for data-parallel training, where each rank holds a slice of the pairs.
  * regtr_loss_norms (one launch): out (4 doubles, device) = (N, sum w over the source tokens, sum w over the target
  *   tokens, B) of this call, the sums in the order regtr_loss_pointwise takes them.
- * The *_norm variants are regtr_loss_pointwise / regtr_infonce_bwd / regtr_loss_finalize with these four normalisers
- *   read from `norm` (device) instead of this call's own: the BCE is meaned over norm[0] tokens, the L1 terms divided
- *   by max(norm[1], 1e-6) and max(norm[2], 1e-6), the InfoNCE terms meaned over norm[3] pairs.  With norm = the
- *   element-wise sum of every rank's regtr_loss_norms, each rank's values and gradients are its exact share of the
- *   whole batch's, and the shares add up to them; with norm = this call's own regtr_loss_norms the results are
- *   bit-identical to the plain entry points.  norm = NULL is the plain entry point. */
+ * norm (optional, device; regtr_loss_pointwise, regtr_infonce_bwd, regtr_loss_finalize and the circle loss's
+ *   regtr_circle_finalize and regtr_circle_bwd): these four normalisers in place of this call's own.  The BCE is meaned
+ *   over norm[0] tokens, the L1 terms divided by max(norm[1], 1e-6) and max(norm[2], 1e-6), the InfoNCE and circle
+ *   terms meaned over norm[3] pairs.  With norm = the element-wise sum of every rank's regtr_loss_norms, each rank's
+ *   values and gradients are its exact share of the whole batch's, and the shares add up to them; norm = NULL uses
+ *   this call's own, bit-identical to passing this call's regtr_loss_norms. */
 int regtr_loss_norms(const regtr_loss_args* args, double* out, void* stream);
-int regtr_loss_pointwise_norm(const regtr_loss_args* args, const double* norm, void* stream);
-int regtr_infonce_bwd_norm(const regtr_loss_args* args, const double* norm, void* stream);
-int regtr_loss_finalize_norm(const regtr_loss_args* args, const double* norm, void* stream);
 
 /* The circle feature loss (CircleLossFull(dist_type='euclidean'), feature_loss_type = 'circle') in place of InfoNCE, on
  * the same regtr_loss_args: feat[t] (N, 256) are the term's packed features, source and target rows alike; q, dq,
@@ -772,83 +793,24 @@ typedef struct {
  * regtr_circle_bwd (two launches): with H_ij = (dL/dD_ij) / D_ij for the upstream gradient g,
  *   dfeat[t] rows of the source tokens = sum_j H_ij (f_i - f_j) (one launch) and of the target tokens
  *   sum_i H_ij (f_j - f_i) (the other).  Source and target rows are owned by different CTAs: no atomics.
- * The *_norm variants mean the terms over norm[3] pairs, as regtr_loss_finalize_norm / regtr_infonce_bwd_norm. */
+ * norm (optional): the batch-global normalisers of regtr_loss_norms; the terms are meaned over norm[3] pairs. */
 int regtr_circle_match(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream);
 int regtr_circle_fwd(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream);
-int regtr_circle_finalize(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream);
-int regtr_circle_bwd(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream);
-int regtr_circle_finalize_norm(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm,
-                               void* stream);
-int regtr_circle_bwd_norm(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm, void* stream);
+int regtr_circle_finalize(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm,
+                          void* stream);
+int regtr_circle_bwd(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm, void* stream);
 
 /* ---- transformer dropout (training) ------------------------------------------------ */
-
-/* The six dropouts of TransformerCrossEncoderLayer.forward_pre in train mode (transformers.py:85-110, 183-244), all
- * with the same p: site 1 the self-attention probabilities, 2 the self-attention output (dropout1), 3 the cross-
- * attention probabilities, 4 the cross-attention output (dropout2), 5 relu(linear1) (dropout), 6 the linear2 output
- * (dropout3).  Masks are regenerated, never stored: the keep decision of (row, column) of a site is a Philox4x32-10
- * draw keyed by (seed, step, global cloud 2 (pair_base + b) + side, layer, site, head, row, column) -- independent of
- * the batch size, packing, rank and launch configuration (counter layout: regtr_b200/csrc/philox.cuh).  Row: token
- * within the (query) cloud; column: key index within the key cloud (sites 1, 3) or feature index (head 0).  Local
- * cloud c of the (src x B, tgt x B) stack is pair c % B, side c / B (B = n_pairs).  A value is dropped when its 16-bit
- * draw is below `threshold` = round(p 65536); kept values are multiplied by `scale` = fp32(1 / (1 - p)).  Limits:
- * 2 (pair_base + n_pairs) <= 2^20, layer < 16, head < 16, clouds shorter than 2^16 tokens.  Passed by host pointer. */
-typedef struct regtr_dropout_args {
-    unsigned long long seed, step;
-    int32_t pair_base;      /* global index of the batch's first pair */
-    int32_t layer;          /* 0..15 */
-    int32_t site;           /* 1..6 */
-    uint32_t threshold;     /* round(p * 65536), <= 65536 */
-    float scale;            /* fp32(1 / (1 - p)) */
-    int32_t n_pairs;        /* B */
-} regtr_dropout_args;
 
 /* Keep mask (analysis / tests): out[r * cols + j] = 1 if row r, column j of local cloud `cloud` (query cloud of an
  * attention site), head `head`, is kept, for r < rows, j < cols.  out: rows x cols uint8. */
 int regtr_dropout_keep_mask(const regtr_dropout_args* args, int cloud, int head, int rows, int cols, uint8_t* out,
                             void* stream);
 
-/* regtr_mha_varlen_fwd_lse with the attention-probability dropout (site 1 or 3; the problem tables of
- * regtr_attention_plan, problem c = query cloud c): O = scale * sum_k m_qk P_qk V_k, the mask applied to the
- * probabilities in registers before the P V product; lse is that of the undropped probabilities. */
-int regtr_mha_varlen_fwd_lse_dropout(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
-                                     float* O, int ldo, float* lse, const int32_t* q_start, const int32_t* q_len,
-                                     const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
-                                     int n_heads, int head_dim, float scale, const regtr_dropout_args* drop,
-                                     void* stream);
-
-/* regtr_mha_varlen_bwd of regtr_mha_varlen_fwd_lse_dropout (same arguments plus the mask key): dP_qk becomes
- * g_qk = m_qk scale (dO_q . V_k), delta = sum_k P g, dV_k = sum_q P_qk m_qk scale dO_q. */
-int regtr_mha_varlen_bwd_dropout(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
-                                 const float* O, int ldo, const float* dO, int lddo, const float* lse,
-                                 float* dQ, int lddq, float* dK, int lddk, float* dV, int lddv,
-                                 const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
-                                 const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len,
-                                 int n_heads, int head_dim, float scale, const regtr_dropout_args* drop, void* ws,
-                                 size_t ws_bytes, void* stream);
-
-/* Residual dropout fused into the LayerNorm that follows it (sites 2, 4, 6):  x' = x + m scale z  (z: the
- * out-projection / linear2 output), x_out = x', then regtr_layernorm_pos of x'.  offs (2B + 1, device): cloud
- * offsets of the packed rows (n = offs[2B]).  x_out must not alias x or z. */
-int regtr_layernorm_pos_dropout(const float* x, const float* z, const float* gamma, const float* beta,
-                                const float* pos, int n, const int32_t* offs, int E, float eps, float* y,
-                                float* y_pos, float* x_out, const regtr_dropout_args* drop, void* stream);
-
-/* Backward of regtr_layernorm_pos_dropout (x = the forward's x_out): dx as regtr_layernorm_bwd (the gradient of
- * x', dres included), plus dz = dx m scale.  ws: regtr_layernorm_bwd_ws_bytes(n, E). */
-int regtr_layernorm_bwd_dropout(const float* x, const float* gamma, const float* dy, const float* dy_pos,
-                                const float* dres, int n, const int32_t* offs, int E, float eps, float* dx,
-                                float* dz, float* dgamma, float* dbeta, const regtr_dropout_args* drop, void* ws,
-                                size_t ws_bytes, void* stream);
-
 /* Feed-forward dropout (site 5), in place: h[r, j] = m scale h[r, j] over the n x F packed rows of the clouds of
  * offs (2B + 1, device); max_len: host bound of the cloud lengths. */
 int regtr_dropout_rows(float* h, int n, int F, const int32_t* offs, int max_len, const regtr_dropout_args* drop,
                        void* stream);
-
-/* ReLU + dropout backward: out = dh * scale where h > 0, else 0 (h: the dropped ReLU output of regtr_dropout_rows,
- * positive exactly where the ReLU passed and the mask kept). */
-int regtr_relu_dropout_bwd(const float* dh, const float* h, long long n, float scale, float* out, void* stream);
 
 /* ---- status word helpers (device uint32) ------------------------------------------ */
 int regtr_status_clear(uint32_t* status, void* stream);

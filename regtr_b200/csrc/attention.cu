@@ -34,11 +34,11 @@ __device__ __forceinline__ bool find_tile(const int32_t* __restrict__ tile_base,
 //   O += P V:   the C fragment of S is reused as the A fragment of P under the key permutation
 //               (A column t <-> key 2t, column t+4 <-> key 2t+1); B = V[key][d] with the same permutation.
 // Row stride 36 floats makes every fragment LDS bank-conflict free.
-// DROP (training with the attention-probability dropout, regtr_mha_varlen_fwd_lse_dropout): the keep mask multiplies
-// the P fragments in registers before the split for P V, and the output normalisation carries the dropout scale; the
-// row sums l (hence lse) stay those of the undropped probabilities.  Per 64-key chunk every lane draws the blocks of
-// key kb + lane and kb + 32 + lane for the warp's two 8-row groups (4 Philox blocks), and each lane fetches the bits
-// of its two keys per n-tile with two shuffles.
+// DROP (training with the attention-probability dropout, regtr_mha_varlen_fwd with a dropout key): the keep mask
+// multiplies the P fragments in registers before the split for P V, and the output normalisation carries the dropout
+// scale; the row sums l (hence lse) stay those of the undropped probabilities.  Per 64-key chunk every lane draws the
+// blocks of key kb + lane and kb + 32 + lane for the warp's two 8-row groups (4 Philox blocks), and each lane fetches
+// the bits of its two keys per n-tile with two shuffles.
 constexpr int MQ = 64, MK = 64, MLD = 36;
 
 __device__ __forceinline__ uint32_t tf32_head(float x) { return (__float_as_uint(x) + 0x1000u) & 0xffffe000u; }
@@ -503,10 +503,17 @@ extern "C" int regtr_attention_plan(const int32_t* offs, int B, int32_t* plan, v
     return REGTR_OK;
 }
 
-static int mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, float* O, int ldo,
-                          const int32_t* q_start, const int32_t* q_len, const int32_t* k_start, const int32_t* k_len,
-                          int n_problems, int max_q_len, const int32_t* tile_base, int max_tiles, int n_heads,
-                          int head_dim, float scale, float* lse, cudaStream_t st, const DropKey* drop = nullptr) {
+// lse (training): the per-(row, head) base-2 log-sum-exp that the backward recomputes the softmax from.
+extern "C" int regtr_mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
+                                    float* O, int ldo, float* lse, const int32_t* q_start, const int32_t* q_len,
+                                    const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
+                                    const int32_t* tile_base, int max_tiles, int n_heads, int head_dim, float scale,
+                                    const regtr_dropout_args* drop, void* stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (tile_base && (lse || drop)) return REGTR_ERR_UNSUPPORTED;       // training launches have no tile table
+    DropKey dk;
+    if (drop && (!lse || drop_key_of(drop, dk) != REGTR_OK || n_heads > 16 || 2 * drop->n_pairs != n_problems))
+        return REGTR_ERR_ARG;
     if (n_problems < 0 || max_q_len < 0 || n_heads <= 0 || max_tiles < 0) return REGTR_ERR_ARG;
     if (head_dim != HD) return REGTR_ERR_UNSUPPORTED;
     if (n_problems == 0 || max_q_len == 0 || (tile_base && max_tiles == 0)) return REGTR_OK;
@@ -519,43 +526,12 @@ static int mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, cons
     // softmax in base 2: q is pre-scaled by scale * log2(e)
     if (drop)
         k_mha_tf32x3<true><<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len,
-                                                 tile_base, n_problems, scale * 1.4426950408889634f, lse, *drop);
+                                                 tile_base, n_problems, scale * 1.4426950408889634f, lse, dk);
     else
         k_mha_tf32x3<false><<<grid, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len,
                                                   tile_base, n_problems, scale * 1.4426950408889634f, lse, DropKey{});
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
-}
-
-extern "C" int regtr_mha_varlen_fwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
-                                    float* O, int ldo, const int32_t* q_start, const int32_t* q_len,
-                                    const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
-                                    const int32_t* tile_base, int max_tiles, int n_heads, int head_dim, float scale,
-                                    void* stream_) {
-    return mha_varlen_fwd(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, n_problems, max_q_len,
-                          tile_base, max_tiles, n_heads, head_dim, scale, nullptr, (cudaStream_t)stream_);
-}
-
-// Training forward: the same 3xTF32 core, which also stores the per-(row, head) base-2 log-sum-exp that the backward
-// recomputes the softmax from.
-extern "C" int regtr_mha_varlen_fwd_lse(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
-                                        float* O, int ldo, float* lse, const int32_t* q_start, const int32_t* q_len,
-                                        const int32_t* k_start, const int32_t* k_len, int n_problems, int max_q_len,
-                                        int n_heads, int head_dim, float scale, void* stream_) {
-    if (!lse) return REGTR_ERR_ARG;
-    return mha_varlen_fwd(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, n_problems, max_q_len,
-                          nullptr, 0, n_heads, head_dim, scale, lse, (cudaStream_t)stream_);
-}
-
-extern "C" int regtr_mha_varlen_fwd_lse_dropout(const float* Q, int ldq, const float* K, int ldk, const float* V,
-                                                int ldv, float* O, int ldo, float* lse, const int32_t* q_start,
-                                                const int32_t* q_len, const int32_t* k_start, const int32_t* k_len,
-                                                int n_problems, int max_q_len, int n_heads, int head_dim, float scale,
-                                                const regtr_dropout_args* drop, void* stream_) {
-    DropKey dk;
-    if (!lse || drop_key_of(drop, dk) != REGTR_OK || n_heads > 16 || 2 * drop->n_pairs != n_problems) return REGTR_ERR_ARG;
-    return mha_varlen_fwd(Q, ldq, K, ldk, V, ldv, O, ldo, q_start, q_len, k_start, k_len, n_problems, max_q_len,
-                          nullptr, 0, n_heads, head_dim, scale, lse, (cudaStream_t)stream_, &dk);
 }
 
 extern "C" int regtr_mha_probs_avg(const float* Q, int ldq, const float* K, int ldk, float* P,

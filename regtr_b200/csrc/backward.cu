@@ -85,7 +85,7 @@ __device__ __forceinline__ void two_sum_add(float& s, float& c, float x) {
 // memory, twice.  dS = P * (dP - delta) with dP = dO . v;  dQ = scale * sum_k dS k.  delta and 1 / Z are stored for
 // pass 2.  Every query row belongs to exactly one problem, so every dQ row is written exactly once.  A problem with an
 // empty key range has Z = 0 and writes dQ = 0.
-// DROP (attention-probability dropout, the regtr_mha_varlen_fwd_lse_dropout forward): dP = dO . v becomes
+// DROP (attention-probability dropout, the regtr_mha_varlen_fwd forward with a dropout key): dP = dO . v becomes
 // g = m * scale * dP in both sweeps, so D = sum_k p g and delta = D / Z are formed from the very g the second sweep
 // uses and sum_k dS = 0 still holds in this arithmetic.  The 8 threads of an aligned 8-query group share one Philox
 // block per key: per 8 keys each draws the block of one key and the bits are passed round with one shuffle per key.
@@ -282,7 +282,7 @@ k_mha_bwd_dkv(const float* __restrict__ Q, int ldq, const float* __restrict__ Kp
 // partials, the block adds its 8 warps in order and stores one partial row; k_colsum adds the blocks in order.
 constexpr int LNB_WARPS = 8, LNB_ROWS = 64, LN_PER = 8;     // E <= 32 * LN_PER = 256
 
-// DROP (regtr_layernorm_bwd_dropout): also dz = dx * m * scale, the gradient of the dropped residual branch.
+// DROP (regtr_layernorm_bwd with a dropout key): also dz = dx * m * scale, the gradient of the dropped residual branch.
 template <bool DROP>
 __global__ void __launch_bounds__(32 * LNB_WARPS)
 k_layernorm_bwd(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ dy,
@@ -363,15 +363,11 @@ __global__ void k_colsum(const float* __restrict__ part, int n_blocks, int ld, i
 }
 
 // ---- dense layers ----------------------------------------------------------------------------------------------
-// dH * (H > 0): the ReLU mask applied to an incoming gradient (H = the ReLU's output)
-__global__ void k_relu_bwd(const float* __restrict__ dh, const float* __restrict__ h, long long n, float* __restrict__ out) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = h[i] > 0.f ? dh[i] : 0.f;
-}
-
-// ReLU + dropout (site 5): h is the dropped ReLU output, positive exactly where the ReLU passed and the mask kept
-__global__ void k_relu_dropout_bwd(const float* __restrict__ dh, const float* __restrict__ h, long long n, float scale,
-                                   float* __restrict__ out) {
+// dH * scale where H > 0: the ReLU mask applied to an incoming gradient (H = the ReLU's output).  With the
+// feed-forward dropout (site 5) H is the dropped ReLU output, positive exactly where the ReLU passed and the mask kept,
+// and scale is the dropout's 1 / (1 - p); without it scale = 1 and dh * 1 is dh (no -ftz / fast-math in the build).
+__global__ void k_relu_bwd(const float* __restrict__ dh, const float* __restrict__ h, long long n, float scale,
+                           float* __restrict__ out) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = h[i] > 0.f ? __fmul_rn(dh[i], scale) : 0.f;
 }
@@ -443,11 +439,16 @@ size_t regtr_mha_varlen_bwd_ws_bytes(int n_rows, int n_heads) {
     return regtr_align(2 * (size_t)(n_rows > 0 ? n_rows : 1) * (size_t)(n_heads > 0 ? n_heads : 1) * sizeof(float));
 }
 
-static int mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, const float* O,
-                          int ldo, const float* dO, int lddo, const float* lse, float* dQ, int lddq, float* dK, int lddk,
-                          float* dV, int lddv, const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
-                          const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len, int n_heads,
-                          int head_dim, float scale, void* ws, size_t ws_bytes, cudaStream_t st, const DropKey* drop) {
+int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, const float* O,
+                         int ldo, const float* dO, int lddo, const float* lse, float* dQ, int lddq, float* dK, int lddk,
+                         float* dV, int lddv, const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
+                         const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len, int n_heads,
+                         int head_dim, float scale, const regtr_dropout_args* drop, void* ws, size_t ws_bytes,
+                         void* stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    DropKey dk;
+    if (drop && (drop_key_of(drop, dk) != REGTR_OK || n_heads > 16 || 2 * drop->n_pairs != n_problems))
+        return REGTR_ERR_ARG;
     if (n_problems < 0 || n_rows < 0 || max_q_len < 0 || max_k_len < 0 || n_heads <= 0) return REGTR_ERR_ARG;
     if (head_dim != HD) return REGTR_ERR_UNSUPPORTED;
     if (n_problems == 0 || n_rows == 0) return REGTR_OK;
@@ -463,7 +464,7 @@ static int mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, cons
         const dim3 grid(regtr_cdiv(max_q_len, BT), n_heads, n_problems);
         if (drop)
             k_mha_bwd_dq<true><<<grid, BT, 0, st>>>(Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dQ, lddq, q_start,
-                                                    q_len, k_start, k_len, qscale, scale, *drop);
+                                                    q_len, k_start, k_len, qscale, scale, dk);
         else
             k_mha_bwd_dq<false><<<grid, BT, 0, st>>>(Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dQ, lddq, q_start,
                                                      q_len, k_start, k_len, qscale, scale, DropKey{});
@@ -473,7 +474,7 @@ static int mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, cons
         const dim3 grid(regtr_cdiv(max_k_len, BT), n_heads, n_problems);
         if (drop)
             k_mha_bwd_dkv<true><<<grid, BT, 0, st>>>(Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dK, lddk, dV,
-                                                     lddv, q_start, q_len, k_start, k_len, qscale, LN2, *drop);
+                                                     lddv, q_start, q_len, k_start, k_len, qscale, LN2, dk);
         else
             k_mha_bwd_dkv<false><<<grid, BT, 0, st>>>(Q, ldq, K, ldk, V, ldv, dO, lddo, lse, delta, rnorm, dK, lddk, dV,
                                                       lddv, q_start, q_len, k_start, k_len, qscale, LN2, DropKey{});
@@ -482,37 +483,17 @@ static int mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, cons
     return REGTR_OK;
 }
 
-int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv, const float* O,
-                         int ldo, const float* dO, int lddo, const float* lse, float* dQ, int lddq, float* dK, int lddk,
-                         float* dV, int lddv, const int32_t* q_start, const int32_t* q_len, const int32_t* k_start,
-                         const int32_t* k_len, int n_problems, int n_rows, int max_q_len, int max_k_len, int n_heads,
-                         int head_dim, float scale, void* ws, size_t ws_bytes, void* stream_) {
-    return mha_varlen_bwd(Q, ldq, K, ldk, V, ldv, O, ldo, dO, lddo, lse, dQ, lddq, dK, lddk, dV, lddv, q_start, q_len,
-                          k_start, k_len, n_problems, n_rows, max_q_len, max_k_len, n_heads, head_dim, scale, ws,
-                          ws_bytes, (cudaStream_t)stream_, nullptr);
-}
-
-int regtr_mha_varlen_bwd_dropout(const float* Q, int ldq, const float* K, int ldk, const float* V, int ldv,
-                                 const float* O, int ldo, const float* dO, int lddo, const float* lse, float* dQ,
-                                 int lddq, float* dK, int lddk, float* dV, int lddv, const int32_t* q_start,
-                                 const int32_t* q_len, const int32_t* k_start, const int32_t* k_len, int n_problems,
-                                 int n_rows, int max_q_len, int max_k_len, int n_heads, int head_dim, float scale,
-                                 const regtr_dropout_args* drop, void* ws, size_t ws_bytes, void* stream_) {
-    DropKey dk;
-    if (drop_key_of(drop, dk) != REGTR_OK || n_heads > 16 || 2 * drop->n_pairs != n_problems) return REGTR_ERR_ARG;
-    return mha_varlen_bwd(Q, ldq, K, ldk, V, ldv, O, ldo, dO, lddo, lse, dQ, lddq, dK, lddk, dV, lddv, q_start, q_len,
-                          k_start, k_len, n_problems, n_rows, max_q_len, max_k_len, n_heads, head_dim, scale, ws,
-                          ws_bytes, (cudaStream_t)stream_, &dk);
-}
-
 size_t regtr_layernorm_bwd_ws_bytes(int n, int E) {
     return regtr_align((size_t)regtr_cdiv(n > 0 ? n : 1, LNB_ROWS) * 2 * (size_t)(E > 0 ? E : 1) * sizeof(float));
 }
 
 int regtr_layernorm_bwd(const float* x, const float* gamma, const float* dy, const float* dy_pos, const float* dres,
-                        int n, int E, float eps, float* dx, float* dgamma, float* dbeta, void* ws, size_t ws_bytes,
-                        void* stream_) {
+                        int n, const int32_t* offs, int E, float eps, float* dx, float* dz, float* dgamma, float* dbeta,
+                        const regtr_dropout_args* drop, void* ws, size_t ws_bytes, void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
+    if (!offs != !drop || !dz != !drop) return REGTR_ERR_ARG;            // offs, dz and drop come together
+    DropKey dk;
+    if (drop && drop_key_of(drop, dk) != REGTR_OK) return REGTR_ERR_ARG;
     if (n < 0 || E <= 0 || E % 32 != 0) return REGTR_ERR_ARG;
     if (E > 32 * LN_PER) return REGTR_ERR_UNSUPPORTED;
     if (!x || !gamma || !dx || !dgamma || !dbeta) return REGTR_ERR_ARG;
@@ -520,8 +501,12 @@ int regtr_layernorm_bwd(const float* x, const float* gamma, const float* dy, con
     float* part = (float*)ws;
     const int nb = n > 0 ? regtr_cdiv(n, LNB_ROWS) : 0;
     if (nb > 0) {
-        k_layernorm_bwd<false><<<nb, 32 * LNB_WARPS, 0, st>>>(x, gamma, dy, dy_pos, dres, n, E, eps, dx, part, nullptr,
-                                                              nullptr, DropKey{});
+        if (drop)
+            k_layernorm_bwd<true><<<nb, 32 * LNB_WARPS, 0, st>>>(x, gamma, dy, dy_pos, dres, n, E, eps, dx, part, dz, offs,
+                                                                 dk);
+        else
+            k_layernorm_bwd<false><<<nb, 32 * LNB_WARPS, 0, st>>>(x, gamma, dy, dy_pos, dres, n, E, eps, dx, part, nullptr,
+                                                                  nullptr, DropKey{});
         REGTR_CHECK_LAUNCH();
     }
     k_colsum<<<regtr_cdiv(2 * E, 256), 256, 0, st>>>(part, nb, 2 * E, 2 * E, dgamma, E, dbeta);
@@ -529,42 +514,11 @@ int regtr_layernorm_bwd(const float* x, const float* gamma, const float* dy, con
     return REGTR_OK;
 }
 
-int regtr_layernorm_bwd_dropout(const float* x, const float* gamma, const float* dy, const float* dy_pos,
-                                const float* dres, int n, const int32_t* offs, int E, float eps, float* dx, float* dz,
-                                float* dgamma, float* dbeta, const regtr_dropout_args* drop, void* ws, size_t ws_bytes,
-                                void* stream_) {
-    cudaStream_t st = (cudaStream_t)stream_;
-    DropKey dk;
-    if (drop_key_of(drop, dk) != REGTR_OK) return REGTR_ERR_ARG;
-    if (n < 0 || E <= 0 || E % 32 != 0) return REGTR_ERR_ARG;
-    if (E > 32 * LN_PER) return REGTR_ERR_UNSUPPORTED;
-    if (!x || !gamma || !dx || !dz || !dgamma || !dbeta || !offs) return REGTR_ERR_ARG;
-    if (!ws || ws_bytes < regtr_layernorm_bwd_ws_bytes(n, E)) return REGTR_ERR_WORKSPACE;
-    float* part = (float*)ws;
-    const int nb = n > 0 ? regtr_cdiv(n, LNB_ROWS) : 0;
-    if (nb > 0) {
-        k_layernorm_bwd<true><<<nb, 32 * LNB_WARPS, 0, st>>>(x, gamma, dy, dy_pos, dres, n, E, eps, dx, part, dz, offs, dk);
-        REGTR_CHECK_LAUNCH();
-    }
-    k_colsum<<<regtr_cdiv(2 * E, 256), 256, 0, st>>>(part, nb, 2 * E, 2 * E, dgamma, E, dbeta);
-    REGTR_CHECK_LAUNCH();
-    return REGTR_OK;
-}
-
-int regtr_relu_dropout_bwd(const float* dh, const float* h, long long n, float scale, float* out, void* stream_) {
+int regtr_relu_bwd(const float* dh, const float* h, long long n, float scale, float* out, void* stream_) {
     if (n < 0) return REGTR_ERR_ARG;
     if (n == 0) return REGTR_OK;
     if (!dh || !h || !out) return REGTR_ERR_ARG;
-    k_relu_dropout_bwd<<<regtr_cdiv(n, 256), 256, 0, (cudaStream_t)stream_>>>(dh, h, n, scale, out);
-    REGTR_CHECK_LAUNCH();
-    return REGTR_OK;
-}
-
-int regtr_relu_bwd(const float* dh, const float* h, long long n, float* out, void* stream_) {
-    if (n < 0) return REGTR_ERR_ARG;
-    if (n == 0) return REGTR_OK;
-    if (!dh || !h || !out) return REGTR_ERR_ARG;
-    k_relu_bwd<<<regtr_cdiv(n, 256), 256, 0, (cudaStream_t)stream_>>>(dh, h, n, out);
+    k_relu_bwd<<<regtr_cdiv(n, 256), 256, 0, (cudaStream_t)stream_>>>(dh, h, n, scale, out);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
 }

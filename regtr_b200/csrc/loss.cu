@@ -840,7 +840,7 @@ int regtr_loss_norms(const regtr_loss_args* args, double* out, void* stream_) {
     return REGTR_OK;
 }
 
-int regtr_loss_pointwise_norm(const regtr_loss_args* args, const double* norm, void* stream_) {
+int regtr_loss_pointwise(const regtr_loss_args* args, const double* norm, void* stream_) {
     const int rc = check_args(args);
     if (rc) return rc;
     const regtr_loss_args& a = *args;
@@ -850,10 +850,6 @@ int regtr_loss_pointwise_norm(const regtr_loss_args* args, const double* norm, v
     k_loss_pointwise<<<dim3(n_chunks_of(a.N), a.L), PW, 0, (cudaStream_t)stream_>>>(a, norm);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
-}
-
-int regtr_loss_pointwise(const regtr_loss_args* args, void* stream_) {
-    return regtr_loss_pointwise_norm(args, nullptr, stream_);
 }
 
 int regtr_loss_pointwise_bwd(const regtr_loss_args* args, void* stream_) {
@@ -898,7 +894,7 @@ int regtr_infonce_fwd(const regtr_loss_args* args, void* stream_) {
     return REGTR_OK;
 }
 
-int regtr_infonce_bwd_norm(const regtr_loss_args* args, const double* norm, void* stream_) {
+int regtr_infonce_bwd(const regtr_loss_args* args, const double* norm, void* stream_) {
     int rc = check_args(args);
     if (rc) return rc;
     const regtr_loss_args& a = *args;
@@ -915,11 +911,7 @@ int regtr_infonce_bwd_norm(const regtr_loss_args* args, const double* norm, void
     return REGTR_OK;
 }
 
-int regtr_infonce_bwd(const regtr_loss_args* args, void* stream_) {
-    return regtr_infonce_bwd_norm(args, nullptr, stream_);
-}
-
-int regtr_loss_finalize_norm(const regtr_loss_args* args, const double* norm, void* stream_) {
+int regtr_loss_finalize(const regtr_loss_args* args, const double* norm, void* stream_) {
     const int rc = check_args(args);
     if (rc) return rc;
     const regtr_loss_args& a = *args;
@@ -930,10 +922,6 @@ int regtr_loss_finalize_norm(const regtr_loss_args* args, const double* norm, vo
     k_loss_finalize<<<1, 256, 0, (cudaStream_t)stream_>>>(a, n_chunks_of(a.N), norm);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
-}
-
-int regtr_loss_finalize(const regtr_loss_args* args, void* stream_) {
-    return regtr_loss_finalize_norm(args, nullptr, stream_);
 }
 
 static int check_circle(const regtr_loss_args* args, const regtr_circle_args* circ, bool bwd) {
@@ -976,8 +964,7 @@ int regtr_circle_fwd(const regtr_loss_args* args, const regtr_circle_args* circ,
     return REGTR_OK;
 }
 
-int regtr_circle_bwd_norm(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm,
-                          void* stream_) {
+int regtr_circle_bwd(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm, void* stream_) {
     const int rc = check_circle(args, circ, true);
     if (rc) return rc;
     const regtr_loss_args& a = *args;
@@ -996,12 +983,8 @@ int regtr_circle_bwd_norm(const regtr_loss_args* args, const regtr_circle_args* 
     return REGTR_OK;
 }
 
-int regtr_circle_bwd(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream_) {
-    return regtr_circle_bwd_norm(args, circ, nullptr, stream_);
-}
-
-int regtr_circle_finalize_norm(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm,
-                               void* stream_) {
+int regtr_circle_finalize(const regtr_loss_args* args, const regtr_circle_args* circ, const double* norm,
+                          void* stream_) {
     const int rc = check_circle(args, circ, false);
     if (rc) return rc;
     const regtr_loss_args& a = *args;
@@ -1012,10 +995,6 @@ int regtr_circle_finalize_norm(const regtr_loss_args* args, const regtr_circle_a
     k_circle_finalize<<<1, 256, 0, (cudaStream_t)stream_>>>(a, *circ, n_chunks_of(a.N), norm);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
-}
-
-int regtr_circle_finalize(const regtr_loss_args* args, const regtr_circle_args* circ, void* stream_) {
-    return regtr_circle_finalize_norm(args, circ, nullptr, stream_);
 }
 
 }  // extern "C"

@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(MN_T, 1) k_modelnet_augment(const regtr_modeln
 
 }  // namespace
 
-extern "C" int regtr_modelnet_augment_at(const regtr_modelnet_args* args, int pair_base, void* stream_) {
+extern "C" int regtr_modelnet_augment(const regtr_modelnet_args* args, int pair_base, void* stream_) {
     if (!args || pair_base < 0 || pair_base > (1 << 30)) return REGTR_ERR_ARG;
     const regtr_modelnet_args& a = *args;
     if (a.B <= 0 || a.B > 65535 || a.n_pts <= 0 || a.n_pts > REGTR_MODELNET_MAX_PTS || a.n_shapes <= 0 ||
@@ -244,8 +244,4 @@ extern "C" int regtr_modelnet_augment_at(const regtr_modelnet_args* args, int pa
     k_modelnet_augment<<<a.B, MN_T, smem, (cudaStream_t)stream_>>>(a, pair_base);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
-}
-
-extern "C" int regtr_modelnet_augment(const regtr_modelnet_args* args, void* stream_) {
-    return regtr_modelnet_augment_at(args, 0, stream_);
 }

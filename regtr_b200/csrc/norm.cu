@@ -190,8 +190,8 @@ __global__ void k_in_apply(const float* x, const int32_t* __restrict__ offs, int
 }
 
 // One warp per row; E = 32 * per <= 32 * PER (PER = 8: the model width 256; PER = 32: anything up to 1024).
-// DROP (regtr_layernorm_pos_dropout): the row is first x + m * scale * z (the residual add of a dropped branch),
-// written to x_out, and normalised from there.
+// DROP (regtr_layernorm_pos with a dropout key): the row is first x + m * scale * z (the residual add of a dropped
+// branch), written to x_out, and normalised from there.
 template <int PER, bool DROP = false>
 __global__ void k_layernorm_pos(const float* __restrict__ x, const float* __restrict__ gamma,
                                 const float* __restrict__ beta, const float* __restrict__ pos, int n,
@@ -332,35 +332,27 @@ int regtr_instnorm_apply(const float* x, const int32_t* offs, int n_clouds, int 
     return REGTR_OK;
 }
 
-int regtr_layernorm_pos(const float* x, const float* gamma, const float* beta, const float* pos, int n,
-                        const int32_t* n_dev, int E, float eps, float* y, float* y_pos, void* stream_) {
+int regtr_layernorm_pos(const float* x, const float* z, const float* gamma, const float* beta, const float* pos, int n,
+                        const int32_t* n_dev, const int32_t* offs, int E, float eps, float* y, float* y_pos,
+                        float* x_out, const regtr_dropout_args* drop, void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
+    // z, offs, x_out and drop come together; the dropout launch uses the kernel's n_dev slot for offs
+    if (!z != !drop || !offs != !drop || !x_out != !drop || (drop && n_dev)) return REGTR_ERR_ARG;
+    DropKey dk;
+    if (drop && (drop_key_of(drop, dk) != REGTR_OK || x_out == x || x_out == z)) return REGTR_ERR_ARG;
     if (n < 0 || E <= 0 || E % 32 != 0 || E > 1024) return REGTR_ERR_ARG;
     if (n == 0) return REGTR_OK;
     if (!x || !gamma || !beta || (!y && !y_pos)) return REGTR_ERR_ARG;
-    if (E <= 256)
+    if (drop && E <= 256)
+        k_layernorm_pos<8, true><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, offs, E, eps,
+                                                                                     y, y_pos, z, x_out, dk);
+    else if (drop)
+        k_layernorm_pos<32, true><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, offs, E,
+                                                                                      eps, y, y_pos, z, x_out, dk);
+    else if (E <= 256)
         k_layernorm_pos<8><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, n_dev, E, eps, y, y_pos);
     else
         k_layernorm_pos<32><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, n_dev, E, eps, y, y_pos);
-    REGTR_CHECK_LAUNCH();
-    return REGTR_OK;
-}
-
-int regtr_layernorm_pos_dropout(const float* x, const float* z, const float* gamma, const float* beta,
-                                const float* pos, int n, const int32_t* offs, int E, float eps, float* y,
-                                float* y_pos, float* x_out, const regtr_dropout_args* drop, void* stream_) {
-    cudaStream_t st = (cudaStream_t)stream_;
-    DropKey dk;
-    if (drop_key_of(drop, dk) != REGTR_OK) return REGTR_ERR_ARG;
-    if (n < 0 || E <= 0 || E % 32 != 0 || E > 1024) return REGTR_ERR_ARG;
-    if (n == 0) return REGTR_OK;
-    if (!x || !z || !gamma || !beta || !offs || !x_out || (!y && !y_pos) || x_out == x || x_out == z) return REGTR_ERR_ARG;
-    if (E <= 256)
-        k_layernorm_pos<8, true><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, offs, E, eps,
-                                                                                     y, y_pos, z, x_out, dk);
-    else
-        k_layernorm_pos<32, true><<<regtr_cdiv((long long)n * 32, 256), 256, 0, st>>>(x, gamma, beta, pos, n, offs, E,
-                                                                                      eps, y, y_pos, z, x_out, dk);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
 }

@@ -406,12 +406,12 @@ int regtr_registration_fit(const double* xyz, const int32_t* offs, int B, int n_
 size_t regtr_train_augment_ws_bytes(int n_src_cap, int B) { return carve_aug(nullptr, n_src_cap, B).total; }
 size_t regtr_train_augment_state_bytes(int n_src_cap) { return scan_state_bytes((long long)n_src_cap + 1); }
 
-int regtr_train_augment_at(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
-                           const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
-                           unsigned long long step, int pair_base, double noise, int max_pts, const int32_t* out_offs,
-                           int out_cap, float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
-                           int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
-                           void* stream_) {
+int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
+                        const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
+                        unsigned long long step, int pair_base, double noise, int max_pts, const int32_t* out_offs,
+                        int out_cap, float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
+                        int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
+                        void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (pair_base < 0 || pair_base > (1 << 30)) return REGTR_ERR_ARG;
     if (!offs || !pose || !pert || !flags || !out_offs || !out_pose || !corr_offs || B <= 0 || 2 * B > 32767 ||
@@ -439,17 +439,6 @@ int regtr_train_augment_at(const double* xyz, const int32_t* offs, int B, int n_
                                                                                   corr_offs);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
-}
-
-int regtr_train_augment(const double* xyz, const int32_t* offs, int B, int n_src_cap, const double* pose,
-                        const int32_t* nn, const double* pert, const int32_t* flags, unsigned long long seed,
-                        unsigned long long step, double noise, int max_pts, const int32_t* out_offs, int out_cap,
-                        float* out_xyz, uint8_t* out_mask, float* out_pose, int32_t* corr, int corr_cap,
-                        int32_t* corr_offs, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
-                        void* stream_) {
-    return regtr_train_augment_at(xyz, offs, B, n_src_cap, pose, nn, pert, flags, seed, step, 0, noise, max_pts,
-                                  out_offs, out_cap, out_xyz, out_mask, out_pose, corr, corr_cap, corr_offs, ws,
-                                  ws_bytes, state, state_bytes, stream_);
 }
 
 }  // extern "C"

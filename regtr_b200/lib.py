@@ -56,22 +56,22 @@ SIGNATURES = {
     'regtr_gemm_ws_bytes': (_Z, [_I, _I, _I]),
     'regtr_gemm_tf32x3': (_I, [_P, _I, _P, _P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _P, _I, _P, _Z, _P]),
     'regtr_pos_embed_sine': (_I, [_P, _I, _P, _I, _I, _F, _P, _P]),
-    'regtr_layernorm_pos': (_I, [_P, _P, _P, _P, _I, _P, _I, _F, _P, _P, _P]),
+    'regtr_layernorm_pos': (_I, [_P, _P, _P, _P, _P, _I, _P, _P, _I, _F, _P, _P, _P, _P, _P]),
     'regtr_attention_plan': (_I, [_P, _I, _P, _P]),
     'regtr_corr_decode_fwd': (_I, [_P, _P, _I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
-    'regtr_mha_varlen_fwd': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _I, _I, _P, _I, _I, _I, _F, _P]),
+    'regtr_mha_varlen_fwd': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _I, _I, _P, _I, _I, _I, _F,
+                                  _P, _P]),
     'regtr_gemm_tf32x3_qkv_bf16': (_I, [_P, _I, _P, _P, _I, _P, _I, _I, _I, _I, _P, _I, _P, _I, _P, _P]),
     'regtr_mha_bf16_tc_fwd': (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     'regtr_gemm_tf32x3_qkv_split': (_I, [_P, _I, _P, _P, _I, _P, _I, _I, _I, _I, _F, _P, _I, _P, _I, _P, _P]),
     'regtr_mha_tf32_tc_fwd': (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _P, _P, _P, _I, _I, _P, _I, _I, _I, _P]),
-    'regtr_mha_varlen_fwd_lse': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     'regtr_mha_probs_avg': (_I, [_P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     'regtr_mha_varlen_bwd_ws_bytes': (_Z, [_I, _I]),
     'regtr_mha_varlen_bwd': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _I, _P, _I, _P, _I,
-                                  _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P, _Z, _P]),
+                                  _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P, _P, _Z, _P]),
     'regtr_layernorm_bwd_ws_bytes': (_Z, [_I, _I]),
-    'regtr_layernorm_bwd': (_I, [_P, _P, _P, _P, _P, _I, _I, _F, _P, _P, _P, _P, _Z, _P]),
-    'regtr_relu_bwd': (_I, [_P, _P, _c.c_longlong, _P, _P]),
+    'regtr_layernorm_bwd': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _F, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    'regtr_relu_bwd': (_I, [_P, _P, _c.c_longlong, _F, _P, _P]),
     'regtr_linear_wgrad_ws_bytes': (_Z, [_I, _I, _I]),
     'regtr_linear_wgrad': (_I, [_P, _I, _P, _I, _I, _I, _I, _P, _P, _P, _Z, _P]),
     'regtr_neighbor_csr_ws_bytes': (_Z, [_I]),
@@ -101,43 +101,28 @@ SIGNATURES = {
                        _Z, _P]),
     'regtr_train_augment_ws_bytes': (_Z, [_I, _I]),
     'regtr_train_augment_state_bytes': (_Z, [_I]),
-    'regtr_train_augment': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _c.c_ulonglong, _c.c_ulonglong, _c.c_double, _I,
-                                 _P, _I, _P, _P, _P, _P, _I, _P, _P, _Z, _P, _Z, _P]),
-    'regtr_train_augment_at': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _c.c_ulonglong, _c.c_ulonglong, _I, _c.c_double,
-                                    _I, _P, _I, _P, _P, _P, _P, _I, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_train_augment': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _c.c_ulonglong, _c.c_ulonglong, _I, _c.c_double,
+                                 _I, _P, _I, _P, _P, _P, _P, _I, _P, _P, _Z, _P, _Z, _P]),
     'regtr_meter_update': (_I, [_P, _P]),
     'regtr_pose_errors': (_I, [_P, _P]),
-    'regtr_modelnet_augment': (_I, [_P, _P]),
-    'regtr_modelnet_augment_at': (_I, [_P, _I, _P]),
+    'regtr_modelnet_augment': (_I, [_P, _I, _P]),
     'regtr_overlap_pyramid': (_I, [_P, _P]),
     'regtr_sym_weight': (_I, [_P, _P, _P, _P]),
     'regtr_sym_weight_bwd': (_I, [_P, _P, _P]),
     'regtr_loss_ws_bytes': (_Z, [_I, _I]),
-    'regtr_loss_pointwise': (_I, [_P, _P]),
+    'regtr_loss_pointwise': (_I, [_P, _P, _P]),
     'regtr_loss_pointwise_bwd': (_I, [_P, _P]),
     'regtr_infonce_match': (_I, [_P, _P]),
     'regtr_infonce_fwd': (_I, [_P, _P]),
-    'regtr_infonce_bwd': (_I, [_P, _P]),
-    'regtr_loss_finalize': (_I, [_P, _P]),
+    'regtr_infonce_bwd': (_I, [_P, _P, _P]),
+    'regtr_loss_finalize': (_I, [_P, _P, _P]),
     'regtr_loss_norms': (_I, [_P, _P, _P]),
-    'regtr_loss_pointwise_norm': (_I, [_P, _P, _P]),
-    'regtr_infonce_bwd_norm': (_I, [_P, _P, _P]),
-    'regtr_loss_finalize_norm': (_I, [_P, _P, _P]),
     'regtr_circle_match': (_I, [_P, _P, _P]),
     'regtr_circle_fwd': (_I, [_P, _P, _P]),
-    'regtr_circle_finalize': (_I, [_P, _P, _P]),
-    'regtr_circle_bwd': (_I, [_P, _P, _P]),
-    'regtr_circle_finalize_norm': (_I, [_P, _P, _P, _P]),
-    'regtr_circle_bwd_norm': (_I, [_P, _P, _P, _P]),
+    'regtr_circle_finalize': (_I, [_P, _P, _P, _P]),
+    'regtr_circle_bwd': (_I, [_P, _P, _P, _P]),
     'regtr_dropout_keep_mask': (_I, [_P, _I, _I, _I, _I, _P, _P]),
-    'regtr_mha_varlen_fwd_lse_dropout': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F,
-                                              _P, _P]),
-    'regtr_mha_varlen_bwd_dropout': (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _P, _I, _P, _P, _I, _P, _I, _P, _I,
-                                          _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P, _P, _Z, _P]),
-    'regtr_layernorm_pos_dropout': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _F, _P, _P, _P, _P, _P]),
-    'regtr_layernorm_bwd_dropout': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _F, _P, _P, _P, _P, _P, _P, _Z, _P]),
     'regtr_dropout_rows': (_I, [_P, _I, _I, _P, _I, _P, _P]),
-    'regtr_relu_dropout_bwd': (_I, [_P, _P, _c.c_longlong, _F, _P, _P]),
     'regtr_status_clear': (_I, [_P, _P]),
 }
 

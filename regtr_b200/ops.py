@@ -449,16 +449,21 @@ def _wants_grad(*ts):
     return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ts)
 
 
-def linear(x, weight, bias=None, residual=None, relu=False, m_dev=None):
+def linear(x, weight, bias=None, residual=None, relu=False, m_dev=None, drop=None):
     """nn.Linear forward (x @ weight^T + bias) (+ residual, + ReLU) on the 3xTF32 wgmma GEMM of this
     library.  The TMA row pitch needs K % 4 == 0 and 16-byte aligned rows; anything else raises (callers
     with an odd K zero-pad it, see PositionEmbeddingLearned) -- there is no library fallback.
-    Differentiable (_LinearFn) when grad mode is on and an input requires grad (exact shapes only)."""
+    Differentiable (_LinearFn) when grad mode is on and an input requires grad (exact shapes only).
+    drop (a dropout site, training): dropout(relu(x W^T + b)) of the feed-forward block (site 5), the mask applied in
+    place after the GEMM; it needs relu=True and no residual."""
+    if drop is not None and (residual is not None or not relu):
+        raise ValueError('linear: the feed-forward dropout follows a ReLU and takes no residual')
     if _wants_grad(x, weight, bias, residual):
         if m_dev is not None:
             raise ValueError('linear: the backward needs exact shapes (no m_dev)')
-        return _LinearFn.apply(x, weight, bias, residual, bool(relu))
-    return _linear_fwd(x, weight, bias, residual, relu, m_dev)
+        return _LinearFn.apply(x, weight, bias, residual, bool(relu), drop)
+    out = _linear_fwd(x, weight, bias, residual, relu, m_dev)
+    return out if drop is None else dropout_rows_(out, drop)
 
 
 def _linear_fwd(x, weight, bias=None, residual=None, relu=False, m_dev=None):
@@ -501,30 +506,42 @@ def pos_embed_sine(xyz, d_model: int = 256, temperature: float = 10000.0, scale:
 
 
 def layernorm_pos(x, gamma, beta, pos=None, eps: float = 1e-5, want_plain=True, want_pos=True, n_dev=None,
-                  skip=False):
+                  skip=False, z=None, drop=None):
     """-> (LN(x), LN(x)+pos); either may be skipped.  n_dev: device row count when x is capacity-shaped.
     Differentiable (_LayerNormPosFn) when grad mode is on and an input requires grad.  skip=True (training path)
     also returns x itself as a third output, for the residual connection that adds x back: its gradient then reaches
-    the LayerNorm backward as `dres` and is added there, so x has one consumer in the autograd graph."""
-    if _wants_grad(x, gamma, beta):
+    the LayerNorm backward as `dres` and is added there, so x has one consumer in the autograd graph.
+    z, drop (a dropout site, training): the residual dropout (site 2, 4 or 6) of a branch z (the out-projection or
+    linear2 output, computed without residual=) fused into this LayerNorm: -> (LN(x'), LN(x')+pos, x') with
+    x' = x + m * scale * z, one launch."""
+    skip = bool(skip) or drop is not None
+    if _wants_grad(x, gamma, beta, z):
         if n_dev is not None:
             raise ValueError('layernorm_pos: the backward needs exact shapes (no n_dev)')
-        outs = _LayerNormPosFn.apply(x, gamma, beta, pos, float(eps), bool(want_plain), bool(want_pos), bool(skip))
+        outs = _LayerNormPosFn.apply(x, gamma, beta, pos, float(eps), bool(want_plain), bool(want_pos), skip, z, drop)
         return outs if skip else outs[:2]
-    outs = _layernorm_pos_fwd(x, gamma, beta, pos, eps, want_plain, want_pos, n_dev)
-    return outs + (x,) if skip else outs
+    outs = _layernorm_pos_fwd(x, gamma, beta, pos, eps, want_plain, want_pos, n_dev, z, drop)
+    return outs if skip else outs[:2]
 
 
-def _layernorm_pos_fwd(x, gamma, beta, pos=None, eps: float = 1e-5, want_plain=True, want_pos=True, n_dev=None):
+def _layernorm_pos_fwd(x, gamma, beta, pos=None, eps: float = 1e-5, want_plain=True, want_pos=True, n_dev=None,
+                       z=None, drop=None):
+    """-> (y, y_pos, x'), x' = x without a dropout site."""
     L = _lib.load()
     _chk(x, torch.float32, 'x', 2)
     n, E = x.shape
     y = torch.empty_like(x) if want_plain else None
     yp = torch.empty_like(x) if want_pos else None
-    _lib.check(L.regtr_layernorm_pos(_p(x), _p(gamma), _p(beta), _p(pos), n, _p(n_dev), E, float(eps), _p(y), _p(yp),
-                                     _stream()), 'regtr_layernorm_pos')
+    offs = xo = dp = None
+    if drop is not None:
+        _chk(z, torch.float32, 'z', 2)
+        if z.shape != x.shape:
+            raise ValueError('layernorm_pos: x and z must have the same shape')
+        offs, xo, dp = drop.key.offs, torch.empty_like(x), drop.ptr
+    _lib.check(L.regtr_layernorm_pos(_p(x), _p(z), _p(gamma), _p(beta), _p(pos), n, _p(n_dev), _p(offs), E, float(eps),
+                                     _p(y), _p(yp), _p(xo), dp, _stream()), 'regtr_layernorm_pos')
     _count(1)
-    return y, yp
+    return y, yp, (x if xo is None else xo)
 
 
 def attention_plan(offs, B: int):
@@ -572,9 +589,9 @@ def mha_varlen(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_heads:
                       lambda: mha_varlen(q, k, v, q_start, q_len, k_start, k_len, max_q_len, n_heads, out=out, tiles=tiles)))
     tb, mt = (tiles[0], int(tiles[1])) if tiles is not None else (None, 0)     # (device tile table, host bound)
     _lib.check(L.regtr_mha_varlen_fwd(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(out),
-                                      out.stride(0), _p(q_start), _p(q_len), _p(k_start), _p(k_len),
+                                      out.stride(0), None, _p(q_start), _p(q_len), _p(k_start), _p(k_len),
                                       q_start.numel(), int(max_q_len), _p(tb), mt, n_heads, dh, 1.0 / math.sqrt(dh),
-                                      _stream()), 'regtr_mha_varlen_fwd')
+                                      None, _stream()), 'regtr_mha_varlen_fwd')
     _count(1)
     return out
 
@@ -662,9 +679,10 @@ def mha_tf32_tc(x, in_w, in_b, q_start, q_len, k_start, k_len, max_q_len: int, n
     return out
 
 
-def mha_varlen_lse(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int):
+def mha_varlen_lse(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int, drop=None):
     """Training forward of `mha_varlen` (the default 3xTF32 core): -> (O (N,E), lse (N, n_heads)), lse the base-2
-    log-sum-exp of the scaled scores that `mha_varlen_bwd` recomputes the softmax from."""
+    log-sum-exp of the scaled scores that `mha_varlen_bwd` recomputes the softmax from.  drop (a dropout site,
+    site 1 or 3): the attention-probability dropout (problem c = local query cloud c)."""
     L = _lib.load()
     for t, nm in ((q, 'q'), (k, 'k'), (v, 'v')):
         if not t.is_cuda or t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1:
@@ -673,18 +691,19 @@ def mha_varlen_lse(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_he
     dh = E // n_heads
     out = torch.empty((q.shape[0], E), dtype=torch.float32, device=q.device)
     lse = torch.empty((q.shape[0], n_heads), dtype=torch.float32, device=q.device)
-    _lib.check(L.regtr_mha_varlen_fwd_lse(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(out),
-                                          out.stride(0), _p(lse), _p(q_start), _p(q_len), _p(k_start), _p(k_len),
-                                          q_start.numel(), int(max_q_len), n_heads, dh, 1.0 / math.sqrt(dh), _stream()),
-               'regtr_mha_varlen_fwd_lse')
+    _lib.check(L.regtr_mha_varlen_fwd(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(out),
+                                      out.stride(0), _p(lse), _p(q_start), _p(q_len), _p(k_start), _p(k_len),
+                                      q_start.numel(), int(max_q_len), None, 0, n_heads, dh, 1.0 / math.sqrt(dh),
+                                      None if drop is None else drop.ptr, _stream()), 'regtr_mha_varlen_fwd')
     _count(1)
     return out, lse
 
 
 def mha_varlen_bwd(q, k, v, o, lse, d_o, dq, dk, dv, q_start, q_len, k_start, k_len, max_q_len: int, max_k_len: int,
-                   n_heads: int):
+                   n_heads: int, drop=None):
     """Backward of the attention core: writes dq / dk / dv (views of the caller's buffers, e.g. column slices of one
-    packed [N, 3E] gradient).  Every key row must lie in the key range of exactly one problem."""
+    packed [N, 3E] gradient).  Every key row must lie in the key range of exactly one problem.  drop: the forward's
+    dropout site."""
     L = _lib.load()
     _chk(d_o, torch.float32, 'dO', 2)
     E = q.shape[1]
@@ -695,21 +714,24 @@ def mha_varlen_bwd(q, k, v, o, lse, d_o, dq, dk, dv, q_start, q_len, k_start, k_
                                       _p(d_o), d_o.stride(0), _p(lse), _p(dq), dq.stride(0), _p(dk), dk.stride(0),
                                       _p(dv), dv.stride(0), _p(q_start), _p(q_len), _p(k_start), _p(k_len),
                                       q_start.numel(), n_rows, int(max_q_len), int(max_k_len), n_heads, dh,
-                                      1.0 / math.sqrt(dh), _p(ws), ws.numel(), _stream()), 'regtr_mha_varlen_bwd')
+                                      1.0 / math.sqrt(dh), None if drop is None else drop.ptr, _p(ws), ws.numel(),
+                                      _stream()), 'regtr_mha_varlen_bwd')
     _count(2)
 
 
-def mha_packed(qkv, q_start, q_len, k_start, k_len, max_len: int, n_heads: int):
+def mha_packed(qkv, q_start, q_len, k_start, k_len, max_len: int, n_heads: int, drop=None):
     """Attention core over a packed in-projection output qkv (N, 3E) = [q | k | v]; differentiable with respect to
-    qkv (one packed (N, 3E) gradient, written by the backward kernels directly) when grad mode is on."""
+    qkv (one packed (N, 3E) gradient, written by the backward kernels directly) when grad mode is on.  drop (a dropout
+    site, site 1 or 3): the attention-probability dropout, on the training core."""
     E = qkv.shape[1] // 3
-    if _wants_grad(qkv):
-        return _MHAPackedFn.apply(qkv, q_start, q_len, k_start, k_len, int(max_len), int(n_heads))
+    if drop is not None or _wants_grad(qkv):
+        return _MHAPackedFn.apply(qkv, q_start, q_len, k_start, k_len, int(max_len), int(n_heads), drop)
     return mha_varlen(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], q_start, q_len, k_start, k_len, max_len, n_heads)
 
 
-def layernorm_bwd(x, gamma, dy, dy_pos, dres, eps: float):
-    """-> (dx, dgamma, dbeta) of regtr_layernorm_pos; dy / dy_pos / dres may be None."""
+def layernorm_bwd(x, gamma, dy, dy_pos, dres, eps: float, drop=None):
+    """-> (dx, dgamma, dbeta) of regtr_layernorm_pos; dy / dy_pos / dres may be None.  drop (the forward's dropout
+    site; x = the forward's x'): -> (dx, dgamma, dbeta, dz), dz the gradient of the dropped branch z."""
     L = _lib.load()
     _chk(x, torch.float32, 'x', 2)
     n, E = x.shape
@@ -719,17 +741,22 @@ def layernorm_bwd(x, gamma, dy, dy_pos, dres, eps: float):
     dx = torch.empty_like(x)
     dg = torch.empty_like(gamma)
     db = torch.empty_like(gamma)
+    offs = dz = dp = None
+    if drop is not None:
+        offs, dz, dp = drop.key.offs, torch.empty_like(x), drop.ptr
     ws = workspace(L.regtr_layernorm_bwd_ws_bytes(n, E), x.device, 'ln_bwd')
-    _lib.check(L.regtr_layernorm_bwd(_p(x), _p(gamma), _p(dy), _p(dy_pos), _p(dres), n, E, float(eps), _p(dx), _p(dg),
-                                     _p(db), _p(ws), ws.numel(), _stream()), 'regtr_layernorm_bwd')
+    _lib.check(L.regtr_layernorm_bwd(_p(x), _p(gamma), _p(dy), _p(dy_pos), _p(dres), n, _p(offs), E, float(eps), _p(dx),
+                                     _p(dz), _p(dg), _p(db), dp, _p(ws), ws.numel(), _stream()), 'regtr_layernorm_bwd')
     _count(2)
-    return dx, dg, db
+    return (dx, dg, db) if drop is None else (dx, dg, db, dz)
 
 
-def relu_bwd(dh, h):
+def relu_bwd(dh, h, scale: float = 1.0):
+    """dh * scale where h > 0, else 0; h the ReLU's output, or with the feed-forward dropout the dropped ReLU output
+    and scale the dropout's (h is positive exactly where both passed)."""
     L = _lib.load()
     out = torch.empty_like(dh)
-    _lib.check(L.regtr_relu_bwd(_p(dh), _p(h), dh.numel(), _p(out), _stream()), 'regtr_relu_bwd')
+    _lib.check(L.regtr_relu_bwd(_p(dh), _p(h), dh.numel(), float(scale), _p(out), _stream()), 'regtr_relu_bwd')
     _count(1)
     return out
 
@@ -760,13 +787,17 @@ def linear_wgrad(x, dy, want_bias: bool):
 
 
 class _LinearFn(torch.autograd.Function):
-    """act(x W^T + b + residual); backward on regtr_relu_bwd, the 3xTF32 GEMM (dX) and regtr_linear_wgrad."""
+    """act(x W^T + b + residual), then the feed-forward dropout if a site is given; backward on regtr_relu_bwd (which
+    also applies the dropout mask and scale), the 3xTF32 GEMM (dX) and regtr_linear_wgrad."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, residual, relu):
+    def forward(ctx, x, weight, bias, residual, relu, drop):
         out = _linear_fwd(x, weight, bias, residual, relu)
+        if drop is not None:
+            dropout_rows_(out, drop)
         ctx.save_for_backward(x, out if relu else None)
         ctx.weight, ctx.relu, ctx.has_bias = weight, relu, bias is not None   # the parameter itself: split cache
+        ctx.scale = 1.0 if drop is None else drop.scale
         return out
 
     @staticmethod
@@ -774,42 +805,45 @@ class _LinearFn(torch.autograd.Function):
         x, out = ctx.saved_tensors
         g = g.contiguous()
         if ctx.relu:
-            g = relu_bwd(g, out)
+            g = relu_bwd(g, out, ctx.scale)
         need = ctx.needs_input_grad
         dx = linear_dgrad(g, ctx.weight) if need[0] else None
         dw = db = None
         if need[1] or need[2]:
             dw, db = linear_wgrad(x, g, ctx.has_bias and need[2])
-        return dx, (dw if need[1] else None), db, (g if need[3] else None), None
+        return dx, (dw if need[1] else None), db, (g if need[3] else None), None, None
 
 
 class _LayerNormPosFn(torch.autograd.Function):
+    """(LN(x), LN(x) + pos, x); with a dropout site x is first x + m * scale * z (a residual dropout, site 2, 4 or 6,
+    fused into the LayerNorm that follows the residual add) and the third output is that x'."""
+
     @staticmethod
-    def forward(ctx, x, gamma, beta, pos, eps, want_plain, want_pos, skip):
+    def forward(ctx, x, gamma, beta, pos, eps, want_plain, want_pos, skip, z, drop):
         ctx.set_materialize_grads(False)
-        y, yp = _layernorm_pos_fwd(x, gamma, beta, pos, eps, want_plain, want_pos)
-        ctx.save_for_backward(x, gamma)
-        ctx.eps = eps
-        return y, yp, (x if skip else None)
+        y, yp, xo = _layernorm_pos_fwd(x, gamma, beta, pos, eps, want_plain, want_pos, None, z, drop)
+        ctx.save_for_backward(xo, gamma)
+        ctx.eps, ctx.drop = eps, drop
+        return y, yp, (xo if skip else None)
 
     @staticmethod
     def backward(ctx, dy, dyp, dres):
-        x, gamma = ctx.saved_tensors
+        xo, gamma = ctx.saved_tensors
         c = lambda t: None if t is None else t.contiguous()
-        dx, dg, db = layernorm_bwd(x, gamma, c(dy), c(dyp), c(dres), ctx.eps)
+        grads = layernorm_bwd(xo, gamma, c(dy), c(dyp), c(dres), ctx.eps, ctx.drop)
         need = ctx.needs_input_grad
-        return (dx if need[0] else None), (dg if need[1] else None), (db if need[2] else None), \
-            None, None, None, None, None
+        dx, dg, db = (g if n else None for g, n in zip(grads[:3], need))
+        return dx, dg, db, None, None, None, None, None, (grads[3] if need[8] else None), None
 
 
 class _MHAPackedFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, q_start, q_len, k_start, k_len, max_len, n_heads):
+    def forward(ctx, qkv, q_start, q_len, k_start, k_len, max_len, n_heads, drop):
         E = qkv.shape[1] // 3
         o, lse = mha_varlen_lse(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], q_start, q_len, k_start, k_len, max_len,
-                                n_heads)
+                                n_heads, drop)
         ctx.save_for_backward(qkv, o, lse, q_start, q_len, k_start, k_len)
-        ctx.max_len, ctx.n_heads = max_len, n_heads
+        ctx.max_len, ctx.n_heads, ctx.drop = max_len, n_heads, drop
         return o
 
     @staticmethod
@@ -818,8 +852,8 @@ class _MHAPackedFn(torch.autograd.Function):
         E = qkv.shape[1] // 3
         d = torch.zeros_like(qkv)            # rows outside every problem keep a zero gradient
         mha_varlen_bwd(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], o, lse, g.contiguous(), d[:, :E], d[:, E:2 * E],
-                       d[:, 2 * E:], qs, ql, ks, kl, ctx.max_len, ctx.max_len, ctx.n_heads)
-        return d, None, None, None, None, None, None
+                       d[:, 2 * E:], qs, ql, ks, kl, ctx.max_len, ctx.max_len, ctx.n_heads, ctx.drop)
+        return d, None, None, None, None, None, None, None
 
 
 # ------------------------------------------------------------------ transformer dropout (training)
@@ -897,126 +931,6 @@ def dropout_keep_mask(p: float, seed: int, step: int, pair_base: int, n_pairs: i
     return out
 
 
-def mha_varlen_lse_dropout(q, k, v, q_start, q_len, k_start, k_len, max_q_len: int, n_heads: int, drop: _DropSite):
-    """mha_varlen_lse with the attention-probability dropout of `drop` (problem c = local query cloud c)."""
-    L = _lib.load()
-    for t, nm in ((q, 'q'), (k, 'k'), (v, 'v')):
-        if not t.is_cuda or t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1:
-            raise ValueError(f'mha_varlen: {nm} must be a CUDA fp32 matrix with unit column stride')
-    E = q.shape[1]
-    dh = E // n_heads
-    out = torch.empty((q.shape[0], E), dtype=torch.float32, device=q.device)
-    lse = torch.empty((q.shape[0], n_heads), dtype=torch.float32, device=q.device)
-    _lib.check(L.regtr_mha_varlen_fwd_lse_dropout(_p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(out),
-                                                  out.stride(0), _p(lse), _p(q_start), _p(q_len), _p(k_start),
-                                                  _p(k_len), q_start.numel(), int(max_q_len), n_heads, dh,
-                                                  1.0 / math.sqrt(dh), drop.ptr, _stream()),
-               'regtr_mha_varlen_fwd_lse_dropout')
-    _count(1)
-    return out, lse
-
-
-def mha_varlen_bwd_dropout(q, k, v, o, lse, d_o, dq, dk, dv, q_start, q_len, k_start, k_len, max_q_len: int,
-                           max_k_len: int, n_heads: int, drop: _DropSite):
-    """mha_varlen_bwd of mha_varlen_lse_dropout."""
-    L = _lib.load()
-    _chk(d_o, torch.float32, 'dO', 2)
-    E = q.shape[1]
-    dh = E // n_heads
-    n_rows = q.shape[0]
-    ws = workspace(L.regtr_mha_varlen_bwd_ws_bytes(n_rows, n_heads), q.device, 'mha_bwd')
-    _lib.check(L.regtr_mha_varlen_bwd_dropout(
-        _p(q), q.stride(0), _p(k), k.stride(0), _p(v), v.stride(0), _p(o), o.stride(0), _p(d_o), d_o.stride(0), _p(lse),
-        _p(dq), dq.stride(0), _p(dk), dk.stride(0), _p(dv), dv.stride(0), _p(q_start), _p(q_len), _p(k_start),
-        _p(k_len), q_start.numel(), n_rows, int(max_q_len), int(max_k_len), n_heads, dh, 1.0 / math.sqrt(dh), drop.ptr,
-        _p(ws), ws.numel(), _stream()), 'regtr_mha_varlen_bwd_dropout')
-    _count(2)
-
-
-class _MHAPackedDropFn(torch.autograd.Function):
-    """_MHAPackedFn with the attention-probability dropout (site 1 or 3)."""
-
-    @staticmethod
-    def forward(ctx, qkv, q_start, q_len, k_start, k_len, max_len, n_heads, drop):
-        E = qkv.shape[1] // 3
-        o, lse = mha_varlen_lse_dropout(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], q_start, q_len, k_start, k_len,
-                                        max_len, n_heads, drop)
-        ctx.save_for_backward(qkv, o, lse, q_start, q_len, k_start, k_len)
-        ctx.max_len, ctx.n_heads, ctx.drop = max_len, n_heads, drop
-        return o
-
-    @staticmethod
-    def backward(ctx, g):
-        qkv, o, lse, qs, ql, ks, kl = ctx.saved_tensors
-        E = qkv.shape[1] // 3
-        d = torch.zeros_like(qkv)
-        mha_varlen_bwd_dropout(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], o, lse, g.contiguous(), d[:, :E],
-                               d[:, E:2 * E], d[:, 2 * E:], qs, ql, ks, kl, ctx.max_len, ctx.max_len, ctx.n_heads,
-                               ctx.drop)
-        return d, None, None, None, None, None, None, None
-
-
-def mha_packed_dropout(qkv, q_start, q_len, k_start, k_len, max_len: int, n_heads: int, drop: _DropSite):
-    """mha_packed (differentiable) with the attention-probability dropout of `drop`."""
-    return _MHAPackedDropFn.apply(qkv, q_start, q_len, k_start, k_len, int(max_len), int(n_heads), drop)
-
-
-def _layernorm_pos_dropout_fwd(x, z, gamma, beta, pos, eps, want_plain, want_pos, drop: _DropSite):
-    L = _lib.load()
-    _chk(x, torch.float32, 'x', 2); _chk(z, torch.float32, 'z', 2)
-    if z.shape != x.shape:
-        raise ValueError('layernorm_pos_dropout: x and z must have the same shape')
-    n, E = x.shape
-    y = torch.empty_like(x) if want_plain else None
-    yp = torch.empty_like(x) if want_pos else None
-    xo = torch.empty_like(x)
-    _lib.check(L.regtr_layernorm_pos_dropout(_p(x), _p(z), _p(gamma), _p(beta), _p(pos), n, _p(drop.key.offs), E,
-                                             float(eps), _p(y), _p(yp), _p(xo), drop.ptr, _stream()),
-               'regtr_layernorm_pos_dropout')
-    _count(1)
-    return y, yp, xo
-
-
-class _LayerNormDropFn(torch.autograd.Function):
-    """(LN(x'), LN(x') + pos, x') with x' = x + dropout(z): a residual dropout (site 2, 4 or 6) fused into the
-    LayerNorm that follows the residual add."""
-
-    @staticmethod
-    def forward(ctx, x, z, gamma, beta, pos, eps, want_plain, want_pos, drop):
-        ctx.set_materialize_grads(False)
-        y, yp, xo = _layernorm_pos_dropout_fwd(x, z, gamma, beta, pos, eps, want_plain, want_pos, drop)
-        ctx.save_for_backward(xo, gamma)
-        ctx.eps, ctx.drop = eps, drop
-        return y, yp, xo
-
-    @staticmethod
-    def backward(ctx, dy, dyp, dres):
-        xo, gamma = ctx.saved_tensors
-        L = _lib.load()
-        c = lambda t: None if t is None else t.contiguous()
-        dy, dyp, dres = c(dy), c(dyp), c(dres)
-        n, E = xo.shape
-        dx, dz = torch.empty_like(xo), torch.empty_like(xo)
-        dg, db = torch.empty_like(gamma), torch.empty_like(gamma)
-        ws = workspace(L.regtr_layernorm_bwd_ws_bytes(n, E), xo.device, 'ln_bwd')
-        d = ctx.drop
-        _lib.check(L.regtr_layernorm_bwd_dropout(_p(xo), _p(gamma), _p(dy), _p(dyp), _p(dres), n, _p(d.key.offs), E,
-                                                 float(ctx.eps), _p(dx), _p(dz), _p(dg), _p(db), d.ptr, _p(ws),
-                                                 ws.numel(), _stream()), 'regtr_layernorm_bwd_dropout')
-        _count(2)
-        need = ctx.needs_input_grad
-        return (dx if need[0] else None), (dz if need[1] else None), (dg if need[2] else None), \
-            (db if need[3] else None), None, None, None, None, None
-
-
-def layernorm_pos_dropout(x, z, gamma, beta, pos, eps: float, want_plain: bool, want_pos: bool, drop: _DropSite):
-    """-> (LN(x'), LN(x') + pos, x'), x' = x + m * scale * z: the residual add of a dropped branch z (the
-    out-projection or linear2 output, computed without residual=) and the LayerNorm after it, one launch."""
-    if _wants_grad(x, z, gamma, beta):
-        return _LayerNormDropFn.apply(x, z, gamma, beta, pos, float(eps), bool(want_plain), bool(want_pos), drop)
-    return _layernorm_pos_dropout_fwd(x, z, gamma, beta, pos, eps, want_plain, want_pos, drop)
-
-
 def dropout_rows_(h, drop: _DropSite):
     """Feed-forward dropout (site 5) in place on the packed (N, F) rows of the batch's clouds."""
     L = _lib.load()
@@ -1026,45 +940,6 @@ def dropout_rows_(h, drop: _DropSite):
                'regtr_dropout_rows')
     _count(1)
     return h
-
-
-def relu_dropout_bwd(dh, h, scale: float):
-    L = _lib.load()
-    out = torch.empty_like(dh)
-    _lib.check(L.regtr_relu_dropout_bwd(_p(dh), _p(h), dh.numel(), float(scale), _p(out), _stream()),
-               'regtr_relu_dropout_bwd')
-    _count(1)
-    return out
-
-
-class _LinearReluDropFn(torch.autograd.Function):
-    """dropout(relu(x W^T + b)) (site 5): the GEMM with its ReLU epilogue, then the mask in place; the backward folds
-    the mask into the ReLU backward (the dropped output is positive exactly where both passed)."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias, drop):
-        h = dropout_rows_(_linear_fwd(x, weight, bias, None, True), drop)
-        ctx.save_for_backward(x, h)
-        ctx.weight, ctx.has_bias, ctx.scale = weight, bias is not None, drop.scale
-        return h
-
-    @staticmethod
-    def backward(ctx, g):
-        x, h = ctx.saved_tensors
-        g = relu_dropout_bwd(g.contiguous(), h, ctx.scale)
-        need = ctx.needs_input_grad
-        dx = linear_dgrad(g, ctx.weight) if need[0] else None
-        dw = db = None
-        if need[1] or need[2]:
-            dw, db = linear_wgrad(x, g, ctx.has_bias and need[2])
-        return dx, (dw if need[1] else None), db, None
-
-
-def linear_relu_dropout(x, weight, bias, drop: _DropSite):
-    """dropout(relu(linear(x))) of the feed-forward block (differentiable when grad mode is on)."""
-    if _wants_grad(x, weight, bias):
-        return _LinearReluDropFn.apply(x, weight, bias, drop)
-    return dropout_rows_(_linear_fwd(x, weight, bias, None, True), drop)
 
 
 # ------------------------------------------------------------------ encoder backward
@@ -1429,7 +1304,7 @@ def check_fit_status(status, radius: float, what: str = 'registration_fit'):
 
 def train_augment(xyz, offs, B: int, n_src: int, pose, nn, pert, flags, seed: int, step: int, noise: float,
                   max_pts: int, out_offs, out_total: int, pair_base: int = 0):
-    """The augmentations of regtr_train_augment_at on the clouds / overlap of `overlap_nn`; the device draws of pair b
+    """The augmentations of regtr_train_augment on the clouds / overlap of `overlap_nn`; the device draws of pair b
     are keyed by pair_base + b.
     -> (out_xyz (out_total,3) f32, out_mask (out_total,) bool, out_pose (B,3,4) f32, corr (2, n_src) i32,
         corr_offs (B+1) i32).  No host sync."""
@@ -1444,11 +1319,11 @@ def train_augment(xyz, offs, B: int, n_src: int, pose, nn, pert, flags, seed: in
     corr_offs = torch.empty(B + 1, dtype=torch.int32, device=dev)
     ws = workspace(L.regtr_train_augment_ws_bytes(n_src, B), dev)
     state = workspace(L.regtr_train_augment_state_bytes(n_src), dev, 'scan_state', zero=True)
-    _lib.check(L.regtr_train_augment_at(_p(xyz), _p(offs), B, n_src, _p(pose), _p(nn), _p(pert), _p(flags),
-                                        int(seed) & (2**64 - 1), int(step) & (2**64 - 1), int(pair_base), float(noise),
-                                        int(max_pts), _p(out_offs), out_total, _p(out_xyz), _p(out_mask), _p(out_pose),
-                                        _p(corr), corr.shape[1], _p(corr_offs), _p(ws), ws.numel(), _p(state),
-                                        state.numel(), _stream()), 'regtr_train_augment_at')
+    _lib.check(L.regtr_train_augment(_p(xyz), _p(offs), B, n_src, _p(pose), _p(nn), _p(pert), _p(flags),
+                                     int(seed) & (2**64 - 1), int(step) & (2**64 - 1), int(pair_base), float(noise),
+                                     int(max_pts), _p(out_offs), out_total, _p(out_xyz), _p(out_mask), _p(out_pose),
+                                     _p(corr), corr.shape[1], _p(corr_offs), _p(ws), ws.numel(), _p(state),
+                                     state.numel(), _stream()), 'regtr_train_augment')
     _count(5 if out_total > 0 else 4)
     return out_xyz, out_mask, out_pose, corr, corr_offs
 
@@ -1553,7 +1428,7 @@ def modelnet_augment(shapes, params, items, seed: int, step: int, k: int, gamma:
     a['seed'], a['step'] = int(seed) & (2**64 - 1), int(step) & (2**64 - 1)
     a['gamma'], a['noise'], a['clip'] = float(gamma), float(noise), float(clip)
     a['n_shapes'], a['n_pts'], a['n_out'], a['k'], a['B'] = shapes.shape[0], shapes.shape[1], int(n_out), int(k), B
-    _lib.check(L.regtr_modelnet_augment_at(a.ctypes.data, int(pair_base), _stream()), 'regtr_modelnet_augment_at')
+    _lib.check(L.regtr_modelnet_augment(a.ctypes.data, int(pair_base), _stream()), 'regtr_modelnet_augment')
     _count(1)
     return out_xyz, out_mask, corr, corr_n
 
@@ -1733,19 +1608,13 @@ def loss_forward(both_un, cond, corr, logit, W, W_un, geo: LossGeometry):
         a['term_val'][t] = keys.index(f'feature_{l}' if l >= 0 else 'feature_un')
     st['args'], st['hold'] = a, (xyz, offs, pose, w, logit, corr)
     s = _stream()
-    if geo.norm is None:
-        _lib.check(L.regtr_loss_pointwise(a.ctypes.data, s), 'regtr_loss_pointwise')
-    else:
-        _lib.check(L.regtr_loss_pointwise_norm(a.ctypes.data, geo.norm.data_ptr(), s), 'regtr_loss_pointwise_norm')
+    _lib.check(L.regtr_loss_pointwise(a.ctypes.data, _p(geo.norm), s), 'regtr_loss_pointwise')
     if circle:
         _circle_forward(L, st, a, s)
         return st
     _lib.check(L.regtr_infonce_match(a.ctypes.data, s), 'regtr_infonce_match')
     _lib.check(L.regtr_infonce_fwd(a.ctypes.data, s), 'regtr_infonce_fwd')
-    if geo.norm is None:
-        _lib.check(L.regtr_loss_finalize(a.ctypes.data, s), 'regtr_loss_finalize')
-    else:
-        _lib.check(L.regtr_loss_finalize_norm(a.ctypes.data, geo.norm.data_ptr(), s), 'regtr_loss_finalize_norm')
+    _lib.check(L.regtr_loss_finalize(a.ctypes.data, _p(geo.norm), s), 'regtr_loss_finalize')
     _count(int(N > 0 and nl > 0) + 2 * int(a['max_src'] > 0) + 1)
     return st
 
@@ -1771,11 +1640,7 @@ def loss_backward(st, g):
         a['dq'][t], a['dfeat'][t] = dq[t].data_ptr(), dfeat[t].data_ptr()
     s = _stream()
     _lib.check(L.regtr_loss_pointwise_bwd(a.ctypes.data, s), 'regtr_loss_pointwise_bwd')
-    norm = st['geo'].norm
-    if norm is None:
-        _lib.check(L.regtr_infonce_bwd(a.ctypes.data, s), 'regtr_infonce_bwd')
-    else:
-        _lib.check(L.regtr_infonce_bwd_norm(a.ctypes.data, norm.data_ptr(), s), 'regtr_infonce_bwd_norm')
+    _lib.check(L.regtr_infonce_bwd(a.ctypes.data, _p(st['geo'].norm), s), 'regtr_infonce_bwd')
     _count(int(N > 0 and nl > 0) + int(a['max_src'] > 0) + int(a['max_tgt'] > 0))
     dW = [torch.zeros((LOSS_DIM, LOSS_DIM), **f32), torch.zeros((LOSS_DIM, LOSS_DIM), **f32)]
     if n_src:
@@ -1801,11 +1666,7 @@ def _circle_forward(L, st, a, s):
     st['circle_args'] = c
     _lib.check(L.regtr_circle_match(a.ctypes.data, c.ctypes.data, s), 'regtr_circle_match')
     _lib.check(L.regtr_circle_fwd(a.ctypes.data, c.ctypes.data, s), 'regtr_circle_fwd')
-    if geo.norm is None:
-        _lib.check(L.regtr_circle_finalize(a.ctypes.data, c.ctypes.data, s), 'regtr_circle_finalize')
-    else:
-        _lib.check(L.regtr_circle_finalize_norm(a.ctypes.data, c.ctypes.data, geo.norm.data_ptr(), s),
-                   'regtr_circle_finalize_norm')
+    _lib.check(L.regtr_circle_finalize(a.ctypes.data, c.ctypes.data, _p(geo.norm), s), 'regtr_circle_finalize')
     n_launch = int(N > 0 and st['shape'][0] > 0) + int(max(a['max_src'], a['max_tgt']) > 0) + \
         int(a['max_src'] > 0) + int(a['max_tgt'] > 0) + 1
     _count(n_launch)
@@ -1818,12 +1679,9 @@ def _circle_backward(L, st, g, d_un, d_cond, d_corr, d_logit):
     a['g'], a['dlogit_out'], a['dcorr_out'] = g.data_ptr(), d_logit.data_ptr(), d_corr.data_ptr()
     for t, l in enumerate(st['term_layers']):
         a['dfeat'][t] = (d_cond[l] if l >= 0 else d_un).data_ptr()
-    c, s, norm = st['circle_args'], _stream(), st['geo'].norm
+    c, s = st['circle_args'], _stream()
     _lib.check(L.regtr_loss_pointwise_bwd(a.ctypes.data, s), 'regtr_loss_pointwise_bwd')
-    if norm is None:
-        _lib.check(L.regtr_circle_bwd(a.ctypes.data, c.ctypes.data, s), 'regtr_circle_bwd')
-    else:
-        _lib.check(L.regtr_circle_bwd_norm(a.ctypes.data, c.ctypes.data, norm.data_ptr(), s), 'regtr_circle_bwd_norm')
+    _lib.check(L.regtr_circle_bwd(a.ctypes.data, c.ctypes.data, _p(st['geo'].norm), s), 'regtr_circle_bwd')
     _count(int(N > 0 and nl > 0) + int(a['max_src'] > 0) + int(a['max_tgt'] > 0))
     return d_un, d_cond, d_corr, d_logit, None, None
 

@@ -282,47 +282,35 @@ class TransformerCrossEncoderLayer(nn.Module):
         values carrying the position embedding, the default 3xTF32 attention core.  Same math as `forward_packed`;
         every LayerNorm also hands x on to the residual add that follows it (layernorm_pos(skip=True)), so the
         residual gradient is added inside the LayerNorm backward.
-        drop (an ops.DropoutKey): apply the six dropouts of layer `layer_idx` and return (x, z) -- the last residual
-        branch z = linear2(...) is not added yet: its dropout and residual add run in the LayerNorm that follows."""
-        if drop is not None:
-            return self._forward_train_dropout(x, pos, plan, drop, layer_idx)
+        drop (an ops.DropoutKey, or None): apply the six dropouts of layer `layer_idx` (transformers.py:183-244, train
+        mode) and return (x, z).  Without dropout the out-projection and linear2 GEMMs add the residual in their
+        epilogue and the layer returns x.  With it they run without residual=, and each dropped branch z is added as
+        x + m * scale * z in the prologue of the LayerNorm that follows it (norm2, norm3, then the encoder's final
+        norm), which also hands x' on: the last branch z = linear2(...) is returned not yet added."""
         has_pos = pos is not None
-        for mha, norm, cross in ((self.self_attn, self.norm1, False), (self.multihead_attn, self.norm2, True)):
-            y, yp, x = ops.layernorm_pos(x, norm.weight, norm.bias, pos, norm.eps, want_plain=not has_pos,
-                                         want_pos=has_pos, skip=True)
-            qkv = ops.linear(yp if has_pos else y, mha.in_proj_weight, mha.in_proj_bias)
-            ks, kl = (plan.xk_start, plan.xk_len) if cross else (plan.q_start, plan.q_len)
-            o = ops.mha_packed(qkv, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead)
-            x = ops.linear(o, mha.out_proj.weight, mha.out_proj.bias, residual=x)
-        x2, _, x = ops.layernorm_pos(x, self.norm3.weight, self.norm3.bias, None, self.norm3.eps,
-                                     want_plain=True, want_pos=False, skip=True)
-        h = ops.linear(x2, self.linear1.weight, self.linear1.bias, relu=True)
-        return ops.linear(h, self.linear2.weight, self.linear2.bias, residual=x)
+        site = lambda s: None if drop is None else drop.site(layer_idx, s)
 
-    def _forward_train_dropout(self, x, pos, plan: AttentionPlan, drop, li: int):
-        """forward_train_packed with the six dropouts of transformers.py:183-244 (train mode).  The out-projection and
-        linear2 GEMMs run without residual=; each dropped branch z is added as x + m * scale * z in the prologue of
-        the LayerNorm that follows it (norm2, norm3, then the encoder's final norm), which also hands x' on."""
-        has_pos = pos is not None
-        z = None
-        for mha, norm, cross, att_site, out_prev in ((self.self_attn, self.norm1, False, ops.SITE_SELF_ATTN, None),
-                                                     (self.multihead_attn, self.norm2, True, ops.SITE_CROSS_ATTN,
-                                                      ops.SITE_SELF_OUT)):
-            if z is None:
-                y, yp, x = ops.layernorm_pos(x, norm.weight, norm.bias, pos, norm.eps, want_plain=not has_pos,
-                                             want_pos=has_pos, skip=True)
-            else:
-                y, yp, x = ops.layernorm_pos_dropout(x, z, norm.weight, norm.bias, pos, norm.eps, not has_pos, has_pos,
-                                                     drop.site(li, out_prev))
+        def branch(h, lin, x):
+            if drop is None:
+                return ops.linear(h, lin.weight, lin.bias, residual=x), None
+            return x, ops.linear(h, lin.weight, lin.bias)
+
+        z = z_site = None
+        for mha, norm, cross, att_site, out_site in (
+                (self.self_attn, self.norm1, False, ops.SITE_SELF_ATTN, ops.SITE_SELF_OUT),
+                (self.multihead_attn, self.norm2, True, ops.SITE_CROSS_ATTN, ops.SITE_CROSS_OUT)):
+            y, yp, x = ops.layernorm_pos(x, norm.weight, norm.bias, pos, norm.eps, want_plain=not has_pos,
+                                         want_pos=has_pos, skip=True, z=z, drop=z_site)
             qkv = ops.linear(yp if has_pos else y, mha.in_proj_weight, mha.in_proj_bias)
             ks, kl = (plan.xk_start, plan.xk_len) if cross else (plan.q_start, plan.q_len)
-            o = ops.mha_packed_dropout(qkv, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead,
-                                       drop.site(li, att_site))
-            z = ops.linear(o, mha.out_proj.weight, mha.out_proj.bias)
-        x2, _, x = ops.layernorm_pos_dropout(x, z, self.norm3.weight, self.norm3.bias, None, self.norm3.eps, True, False,
-                                             drop.site(li, ops.SITE_CROSS_OUT))
-        h = ops.linear_relu_dropout(x2, self.linear1.weight, self.linear1.bias, drop.site(li, ops.SITE_FFN))
-        return x, ops.linear(h, self.linear2.weight, self.linear2.bias)
+            o = ops.mha_packed(qkv, plan.q_start, plan.q_len, ks, kl, plan.max_len, self.nhead, drop=site(att_site))
+            x, z = branch(o, mha.out_proj, x)
+            z_site = site(out_site)
+        x2, _, x = ops.layernorm_pos(x, self.norm3.weight, self.norm3.bias, None, self.norm3.eps,
+                                     want_plain=True, want_pos=False, skip=True, z=z, drop=z_site)
+        h = ops.linear(x2, self.linear1.weight, self.linear1.bias, relu=True, drop=site(ops.SITE_FFN))
+        x, z = branch(h, self.linear2, x)
+        return x if drop is None else (x, z)
 
     def forward_post_packed(self, x, pos, plan: AttentionPlan):
         """Post-norm layer (transformers.py:121-181): attention on x (+pos), then LayerNorm(x + update)."""
@@ -420,20 +408,16 @@ class TransformerCrossEncoder(nn.Module):
         if self.record_attentions:
             raise RuntimeError('attention maps are recorded by the inference forward only; turn record_attentions off '
                                'to train')
-        if drop is not None:
-            if len(self.layers) > 16:
-                raise ValueError('dropout: more than 16 layers are outside the mask counter layout')
-            outs = []
-            for li, layer in enumerate(self.layers):
-                x, z = layer.forward_train_packed(x, pos, plan, drop, li)
-                y, _, x = ops.layernorm_pos_dropout(x, z, self.norm.weight, self.norm.bias, None, self.norm.eps, True,
-                                                    False, drop.site(li, ops.SITE_FFN_OUT))
-                outs.append(y)
-            return torch.stack(outs)
+        if drop is not None and len(self.layers) > 16:
+            raise ValueError('dropout: more than 16 layers are outside the mask counter layout')
         outs = []
-        for layer in self.layers:
-            x = layer.forward_train_packed(x, pos, plan)
-            y, _, x = ops.layernorm_pos(x, self.norm.weight, self.norm.bias, None, self.norm.eps, True, False, skip=True)
+        for li, layer in enumerate(self.layers):
+            if drop is None:
+                x, z = layer.forward_train_packed(x, pos, plan), None
+            else:
+                x, z = layer.forward_train_packed(x, pos, plan, drop, li)
+            y, _, x = ops.layernorm_pos(x, self.norm.weight, self.norm.bias, None, self.norm.eps, True, False, skip=True,
+                                        z=z, drop=None if drop is None else drop.site(li, ops.SITE_FFN_OUT))
             outs.append(y)
         return torch.stack(outs)
 

@@ -72,7 +72,7 @@ def _attention_ref(qkv, d_o, lens, cross, key, layer, site, dtype):
 
 
 @pytest.mark.parametrize('cross', [False, True])
-def test_attention_core_with_dropout_matches_float64(cross):
+def test_attention_core_drop_argument_matches_float64(cross):
     """Dropout forward, dQ, dK and dV against float64 autograd with the same masks (fp32 yardstick), uneven clouds
     of 2 pairs; sum_k dK = 0 over every key range (sum_j dS_ij = 0 in the backward's own arithmetic)."""
     from regtr_b200 import ops
@@ -90,12 +90,12 @@ def test_attention_core_with_dropout_matches_float64(cross):
     key = ops.DropoutKey(P, SEED, STEP, 0, B)
     drop = key.site(layer, site)
     q, k, v = qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:]
-    o, lse = ops.mha_varlen_lse_dropout(q, k, v, plan.q_start, plan.q_len, ks, kl, plan.max_len, H, drop)
+    o, lse = ops.mha_varlen_lse(q, k, v, plan.q_start, plan.q_len, ks, kl, plan.max_len, H, drop=drop)
     _, lse0 = ops.mha_varlen_lse(q, k, v, plan.q_start, plan.q_len, ks, kl, plan.max_len, H)
     assert torch.equal(lse, lse0)                                   # lse of the undropped probabilities
     d = torch.zeros_like(qkv)
-    ops.mha_varlen_bwd_dropout(q, k, v, o, lse, d_o, d[:, :E], d[:, E:2 * E], d[:, 2 * E:], plan.q_start, plan.q_len,
-                               ks, kl, plan.max_len, plan.max_len, H, drop)
+    ops.mha_varlen_bwd(q, k, v, o, lse, d_o, d[:, :E], d[:, E:2 * E], d[:, 2 * E:], plan.q_start, plan.q_len,
+                       ks, kl, plan.max_len, plan.max_len, H, drop=drop)
     torch.cuda.synchronize()
     kk = (SEED, STEP, 0)
     o64, d64 = _attention_ref(qkv, d_o, lens, cross, kk, layer, site, torch.float64)
@@ -117,9 +117,69 @@ def test_attention_core_with_dropout_matches_float64(cross):
     o_nodrop = ops.mha_varlen(q, k, v, plan.q_start, plan.q_len, ks, kl, plan.max_len, H)
     assert float((o_nodrop - o).abs().max()) > 1e-2
     d2 = torch.zeros_like(qkv)
-    ops.mha_varlen_bwd_dropout(q, k, v, o, lse, d_o, d2[:, :E], d2[:, E:2 * E], d2[:, 2 * E:], plan.q_start,
-                               plan.q_len, ks, kl, plan.max_len, plan.max_len, H, drop)
+    ops.mha_varlen_bwd(q, k, v, o, lse, d_o, d2[:, :E], d2[:, E:2 * E], d2[:, 2 * E:], plan.q_start,
+                       plan.q_len, ks, kl, plan.max_len, plan.max_len, H, drop=drop)
     assert torch.equal(d, d2)
+
+
+def test_dropout_arguments_come_together():
+    """The attention forward and the LayerNorm forward and backward take their dropout arguments as optional pointers
+    that are all given or all NULL: every mixed combination returns its error code and launches nothing (the
+    NaN-filled outputs stay untouched)."""
+    from regtr_b200 import lib, ops
+    from regtr_b200.transformer import AttentionPlan
+    L = lib.load()
+    ERR_ARG, ERR_UNSUPPORTED = -1, -3
+    st = torch.cuda.current_stream().cuda_stream
+    lens, E, H = [37, 64], 256, 8
+    n = sum(lens)
+    g = torch.Generator().manual_seed(5)
+    qkv, x, z, dy = (torch.randn(n, c, generator=g).to(DEV) for c in (3 * E, E, E, E))
+    gamma, beta = torch.ones(E, device=DEV), torch.zeros(E, device=DEV)
+    offs, n_dev = _offs(lens), torch.tensor([n], dtype=torch.int32, device=DEV)
+    key = ops.DropoutKey(P, SEED, STEP, 0, 1, offs=offs, max_len=max(lens))
+    plan = AttentionPlan(lens, DEV)
+    p = lambda t: None if t is None else t.data_ptr()
+    nan = lambda *shape: torch.full(shape, float('nan'), device=DEV)
+    untouched = lambda *ts: all(bool(t.isnan().all()) for t in ts if t is not None)
+
+    # attention forward: a dropout key needs lse; a tile table takes neither lse nor a key
+    att = key.site(0, ops.SITE_SELF_ATTN).ptr
+    q, k, v = qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:]
+    tb, mt = plan.tiles64
+    for want_lse, tiles, drop, rc in ((False, None, att, ERR_ARG), (True, tb, None, ERR_UNSUPPORTED),
+                                      (False, tb, att, ERR_UNSUPPORTED), (True, tb, att, ERR_UNSUPPORTED)):
+        o, lse = nan(n, E), (nan(n, H) if want_lse else None)
+        got = L.regtr_mha_varlen_fwd(p(q), 3 * E, p(k), 3 * E, p(v), 3 * E, p(o), E, p(lse), p(plan.q_start),
+                                     p(plan.q_len), p(plan.q_start), p(plan.q_len), 2, plan.max_len, p(tiles),
+                                     mt if tiles is not None else 0, H, 32, 1 / math.sqrt(32), drop, st)
+        assert got == rc, (want_lse, tiles is not None, drop is not None)
+        assert untouched(o, lse)
+
+    # LayerNorm forward: z, offs, x_out and the key together, and no n_dev with the key
+    res = key.site(0, ops.SITE_SELF_OUT).ptr
+    xo = nan(n, E)
+    full = dict(z=z, offs=offs, x_out=xo, drop=res)
+    for kw in (dict(z=z), dict(offs=offs), dict(x_out=xo), dict(full, drop=None), dict(drop=res),
+               dict(z=z, offs=offs, drop=res), dict(full, n_dev=n_dev)):
+        a = dict(dict.fromkeys(('z', 'offs', 'x_out', 'drop', 'n_dev')), **kw)
+        y = nan(n, E)
+        got = L.regtr_layernorm_pos(p(x), p(a['z']), p(gamma), p(beta), None, n, p(a['n_dev']), p(a['offs']), E, 1e-5,
+                                    p(y), None, p(a['x_out']), a['drop'], st)
+        assert got == ERR_ARG, sorted(k for k, t in kw.items() if t is not None)
+        assert untouched(y, xo)
+
+    # LayerNorm backward: offs, dz and the key together
+    ws = torch.empty(L.regtr_layernorm_bwd_ws_bytes(n, E), dtype=torch.uint8, device=DEV)
+    dz = nan(n, E)
+    for kw in (dict(offs=offs), dict(dz=dz), dict(offs=offs, dz=dz), dict(drop=res), dict(offs=offs, drop=res),
+               dict(dz=dz, drop=res)):
+        a = dict(dict.fromkeys(('offs', 'dz', 'drop')), **kw)
+        dx, dg, db = nan(n, E), nan(E), nan(E)
+        got = L.regtr_layernorm_bwd(p(x), p(gamma), p(dy), None, None, n, p(a['offs']), E, 1e-5, p(dx), p(a['dz']),
+                                    p(dg), p(db), a['drop'], p(ws), ws.numel(), st)
+        assert got == ERR_ARG, sorted(kw)
+        assert untouched(dx, dg, db, dz)
 
 
 # --------------------------------------------------------------------------------------------- cross-encoder
@@ -201,7 +261,7 @@ def _model_activations(case):
 
 
 @pytest.mark.parametrize('inputs', ['random', 'fwd_modelnet_b1', 'fwd_3dmatch_small_b2'])
-def test_cross_encoder_with_dropout_matches_float64(inputs):
+def test_cross_encoder_drop_argument_matches_float64(inputs):
     """Pre-norm layers with all six dropouts (forward_train_packed with a DropoutKey) against float64 autograd of
     the reference's forward_pre with the same masks: every output and every gradient under the fp32 yardstick.
     'random': two layers with perturbed norms on randn tokens of two uneven pairs; the model cases: the model's own
@@ -225,17 +285,18 @@ def test_cross_encoder_with_dropout_matches_float64(inputs):
     x = x0.to(DEV).requires_grad_(True)
     plan = AttentionPlan(lens, DEV)
     drop = ops.DropoutKey(P, SEED, STEP, pair_base, B, offs=_offs(lens), max_len=max(lens))
-    hs, real = [], ops.linear_relu_dropout
+    hs, real = [], ops.linear
 
     def spy(*a, **k):
         h = real(*a, **k)
-        hs.append(h.detach().cpu())
+        if k.get('drop') is not None:                   # the feed-forward block's dropout(relu(linear1))
+            hs.append(h.detach().cpu())
         return h
-    ops.linear_relu_dropout = spy
+    ops.linear = spy
     try:
         out = enc.forward_train_packed(x, pos.to(DEV), plan, drop=drop)
     finally:
-        ops.linear_relu_dropout = real
+        ops.linear = real
     (out * gout.to(DEV)).sum().backward()
     key = (SEED, STEP, pair_base)
     # the GPU's ReLU decisions: where a unit is kept, the dropped output is positive exactly where the ReLU passed
