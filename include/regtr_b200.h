@@ -538,8 +538,9 @@ int regtr_overlap_nn(const double* xyz, const int32_t* offs, int B, int n_cap, c
 int regtr_registration_fit(const double* xyz, const int32_t* offs, int B, int n_cap, const double* pose,
                            double radius, const int32_t* nn, double* out, uint32_t* status, void* stream);
 
-/* Point-to-point ICP of B pairs (Open3D's registration_icp with TransformationEstimationPointToPoint, no scaling,
- * and ICPConvergenceCriteria(rel_fitness, rel_rmse, max_iter)).  xyz (n_cap,3) float64 stacked src_0..src_{B-1},
+/* ICP of B pairs (Open3D's registration_icp with TransformationEstimationPointToPoint, no scaling, or with
+ * TransformationEstimationPointToPlane, and ICPConvergenceCriteria(rel_fitness, rel_rmse, max_iter)).
+ * xyz (n_cap,3) float64 stacked src_0..src_{B-1},
  * tgt_0..tgt_{B-1} with offs (2B+1) i32; init (B,3,4) float64 source -> target.  Per pair: P = init . source
  * (((r0 x + r1 y) + r2 z) + t, no contraction), T = init; correspondences are regtr_overlap_nn's (the nearest target
  * point with float64 d^2 strictly below max_dist^2, ties to the lowest index), fitness = k / n_src,
@@ -550,12 +551,43 @@ int regtr_registration_fit(const double* xyz, const int32_t* offs, int B, int n_
  * 3 launches per round for max_iter + 1 rounds whatever B and convergence; no host synchronisation; sums in a fixed
  * order, so the result is bit-reproducible and independent of the batch.  A coordinate of a moved source or of a
  * target beyond regtr_overlap_coord_bound(max_dist, cell), or not finite, raises REGTR_STATUS_RANGE.  ws / state:
- * the *_bytes functions below (state ZERO before the first call; every call leaves it zero). */
+ * the *_bytes functions below (state ZERO before the first call; every call leaves it zero).
+ * tgt_normals NULL: point-to-point, as above.  Non-NULL: (offs[2B] - offs[B], 3) float64, row j - offs[B] the normal of
+ * target row j (regtr_estimate_normals); point-to-plane with the same correspondences, fitness, RMSE (point distances)
+ * and stop test.  Per correspondence (p moved source, q target, n its normal) r = (p - q) . n, J = [p x n ; n]; J^T J
+ * (21 unique entries) and J^T r summed per chunk in the fixed order; per pair J^T J x = -J^T r solved by LDL^T in
+ * float64; the update is the identity when k = 0, |det J^T J| < 1e-6 or det is not finite (Open3D's
+ * SolveLinearSystemPSD), else R = Rz(x2) Ry(x1) Rx(x0), t = (x3, x4, x5) (TransformVector6dToMatrix4d).  A zero
+ * normal drops its correspondence out of the update, not out of k.  Same launches as point-to-point. */
 size_t regtr_icp_ws_bytes(int n_cap, int B);
 size_t regtr_icp_state_bytes(int n_cap);
 int regtr_icp(const double* xyz, const int32_t* offs, int B, int n_cap, const double* init, double max_dist,
-              float cell, int max_iter, double rel_fitness, double rel_rmse, double* pose_out, double* result,
-              uint32_t* status, void* ws, size_t ws_bytes, void* state, size_t state_bytes, void* stream);
+              float cell, int max_iter, double rel_fitness, double rel_rmse, const double* tgt_normals,
+              double* pose_out, double* result, uint32_t* status, void* ws, size_t ws_bytes, void* state,
+              size_t state_bytes, void* stream);
+
+/* Normals of C stacked clouds (Open3D's estimate_normals(KDTreeSearchParamHybrid(radius, max_nn)) followed by
+ * orient_normals_towards_camera_location() at the origin, with this library's tie and boundary rules).
+ * xyz (n_cap,3) float64 with offs (C+1) i32, offs[0] = 0, C <= 32767; cell = radius * (1 + 1e-3) rounded to fp32
+ * (ops.overlap_cell); 1 <= max_nn <= 64 (else REGTR_ERR_ARG).  normals (n_cap,3) float64, rows >= offs[C] untouched.
+ *   Neighbours of point i: the points of i's own cloud with float64 d^2 = (dx dx + dy dy) + dz dz (no contraction)
+ *   strictly below radius^2, i itself included (d^2 = 0); the max_nn smallest by (d^2, index), ties to the lower index.
+ *   Found through one cell list over the fp32 copy (27-cell stencil), without a capacity limit or truncation.
+ *   Covariance: over the neighbours in ascending (d^2, index) order, the mean first, then the centred sum of outer
+ *   products / count, float64 sums in that fixed order.
+ *   Normal: the unit eigenvector of the covariance's smallest eigenvalue (the right singular vector of the smallest
+ *   singular value of a float64 one-sided Jacobi SVD), negated when ((nx px + ny py) + nz pz) > 0 (towards the origin).
+ *   Fewer than 3 neighbours: (0,0,0), so that the point drops out of point-to-plane ICP (Open3D returns an arbitrary
+ *   axis there).
+ * counts (n_cap) i32, nullable: the number of neighbours used per point.  A |coordinate| beyond
+ * regtr_overlap_coord_bound(radius, cell), or not finite, raises REGTR_STATUS_RANGE.  1 + 4 + 1 launches whatever C;
+ * no value atomics, no host synchronisation: the result is bit-identical whether a cloud is passed alone or in a stack.
+ * ws / state: the *_bytes functions below (state ZERO before the first call; every call leaves it zero). */
+size_t regtr_estimate_normals_ws_bytes(int n_cap);
+size_t regtr_estimate_normals_state_bytes(int n_cap);
+int regtr_estimate_normals(const double* xyz, const int32_t* offs, int C, int n_cap, double radius, float cell,
+                           int max_nn, double* normals, int32_t* counts, uint32_t* status, void* ws, size_t ws_bytes,
+                           void* state, size_t state_bytes, void* stream);
 
 /* Per-pair flags of regtr_train_augment */
 #define REGTR_PREP_PERTURB_SRC 1  /* the perturbation moves the source (else the target) */

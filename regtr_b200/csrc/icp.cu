@@ -1,5 +1,7 @@
-// Point-to-point ICP of B pairs at once: Open3D's registration_icp with TransformationEstimationPointToPoint (no
-// scaling) and ICPConvergenceCriteria, restated with this library's determinism rules (DESIGN.md section 8, "ICP").
+// ICP of B pairs at once: Open3D's registration_icp with TransformationEstimationPointToPoint (no scaling) or
+// TransformationEstimationPointToPlane, and ICPConvergenceCriteria, restated with this library's determinism rules
+// (DESIGN.md section 8, "ICP").  The method is a template argument of the reduction and the update kernels, so the
+// point-to-point instantiation is the same code as without the point-to-plane method.
 //
 // Stacked clouds as in the registration fit: src_0..src_{B-1}, tgt_0..tgt_{B-1} (float64) with int32 device offsets.
 // One cell list over the targets is built once; then every round is a fixed sequence of three launches (nearest
@@ -23,6 +25,7 @@ constexpr int CHUNK = 1024;            // source points per CTA of the reduction
 constexpr int RED_THREADS = 256;
 constexpr int RED_WARPS = RED_THREADS / 32;
 constexpr int PART = 17;               // k, sum d2, mean_src[3], mean_tgt[3], C[9] per chunk
+constexpr int PART_PLANE = 29;         // k, sum d2, J^T J[21] (upper triangle, row-major), J^T r[6] per chunk
 constexpr int UPD_THREADS = 64;
 
 // Per-pair state between rounds (written by k_icp_update only).
@@ -159,16 +162,50 @@ __device__ __forceinline__ double block_sum(double v, double* s_warp) {
 // depend on the batch).  Over the chunk's correspondences: count, sum of d2 and the two means, then, in a second pass
 // over the same points, C = sum (q - mean_q)(p - mean_p)^T (target rows, source columns).  part[g] = (k, sum d2,
 // mean_p, mean_q, C).  Fixed per-thread strides and a fixed tree: deterministic, no atomics.
+//
+// Point-to-plane (PLANE): per correspondence (p moved source, q target, n = tnrm[j - offs[B]] its normal)
+// r = (p - q) . n and J = [p x n ; n]; one pass gives part[g] = (k, sum d2, J^T J upper triangle row-major, J^T r).
+template <bool PLANE>
 __global__ void __launch_bounds__(RED_THREADS)
 k_icp_reduce(const double* __restrict__ xyz, const int32_t* __restrict__ offs, int B, const int32_t* __restrict__ cpre,
              const double* __restrict__ P, const int32_t* __restrict__ nn, const double* __restrict__ d2,
-             const IcpPair* __restrict__ pst, double* __restrict__ part) {
+             const IcpPair* __restrict__ pst, double* __restrict__ part, const double* __restrict__ tnrm) {
     __shared__ double s_warp[RED_WARPS];
     const int g = blockIdx.x, t = threadIdx.x;
     if (g >= cpre[B]) return;
     const int b = regtr_cloud_of(cpre, B, g);
     if (pst[b].done) return;
     const int i0 = offs[b] + (g - cpre[b]) * CHUNK, i1 = min(i0 + CHUNK, offs[b + 1]);
+    if constexpr (PLANE) {
+        const int t0 = offs[B];
+        double k = 0.0, sd = 0.0, H[21], v[6];
+        for (int e = 0; e < 21; ++e) H[e] = 0.0;
+        for (int e = 0; e < 6; ++e) v[e] = 0.0;
+        for (int i = i0 + t; i < i1; i += RED_THREADS) {
+            const int j = nn[i];
+            if (j < 0) continue;
+            k += 1.0;
+            sd += d2[i];
+            const double px = P[3 * i + 0], py = P[3 * i + 1], pz = P[3 * i + 2];
+            const double nx = tnrm[3 * (j - t0) + 0], ny = tnrm[3 * (j - t0) + 1], nz = tnrm[3 * (j - t0) + 2];
+            const double r = (px - xyz[3 * j + 0]) * nx + (py - xyz[3 * j + 1]) * ny + (pz - xyz[3 * j + 2]) * nz;
+            const double J[6] = {py * nz - pz * ny, pz * nx - px * nz, px * ny - py * nx, nx, ny, nz};
+            int e = 0;
+            for (int a = 0; a < 6; ++a) {
+                for (int c = a; c < 6; ++c) H[e++] += J[a] * J[c];
+                v[a] += J[a] * r;
+            }
+        }
+        double out[PART_PLANE];
+        out[0] = block_sum(k, s_warp);
+        out[1] = block_sum(sd, s_warp);
+        for (int e = 0; e < 21; ++e) out[2 + e] = block_sum(H[e], s_warp);
+        for (int e = 0; e < 6; ++e) out[23 + e] = block_sum(v[e], s_warp);
+        if (t != 0) return;
+        double* o = part + (size_t)PART_PLANE * g;
+        for (int e = 0; e < PART_PLANE; ++e) o[e] = out[e];
+        return;
+    }
     double k = 0.0, sd = 0.0, sp[3] = {0.0, 0.0, 0.0}, sq[3] = {0.0, 0.0, 0.0};
     for (int i = i0 + t; i < i1; i += RED_THREADS) {
         const int j = nn[i];
@@ -202,17 +239,127 @@ k_icp_reduce(const double* __restrict__ xyz, const int32_t* __restrict__ offs, i
     for (int e = 0; e < 9; ++e) o[8 + e] = out[8 + e];
 }
 
+// Solve A x = -v for the symmetric 6x6 A given by its upper triangle H (row-major) by LDL^T without pivoting, in a
+// fixed order.  False, x untouched, when |det A| = |prod D| < 1e-6 or det is not finite (Open3D's
+// SolveLinearSystemPSD check).
+__device__ __forceinline__ bool solve6_ldlt(const double H[21], const double v[6], double x[6]) {
+    double A[6][6], L[6][6], D[6];
+#pragma unroll
+    for (int a = 0, e = 0; a < 6; ++a)
+#pragma unroll
+        for (int c = a; c < 6; ++c, ++e) { A[a][c] = H[e]; A[c][a] = H[e]; }
+    double det = 1.0;
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+        double d = A[j][j];
+#pragma unroll
+        for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k] * D[k];
+        D[j] = d;
+        det *= d;
+#pragma unroll
+        for (int i = j + 1; i < 6; ++i) {
+            double a = A[i][j];
+#pragma unroll
+            for (int k = 0; k < j; ++k) a -= L[i][k] * L[j][k] * D[k];
+            L[i][j] = a / d;
+        }
+    }
+    if (!(fabs(det) >= 1e-6) || isinf(det)) return false;
+    double y[6];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) {                      // L y = -v
+        double a = -v[i];
+#pragma unroll
+        for (int k = 0; k < i; ++k) a -= L[i][k] * y[k];
+        y[i] = a;
+    }
+#pragma unroll
+    for (int i = 5; i >= 0; --i) {                     // L^T x = D^-1 y
+        double a = y[i] / D[i];
+#pragma unroll
+        for (int k = i + 1; k < 6; ++k) a -= L[k][i] * x[k];
+        x[i] = a;
+    }
+    return true;
+}
+
+// k_icp_update for point-to-plane, one thread per pair: combine the chunks in chunk order, the fitness, RMSE and stop
+// test of the point-to-point update, then the Gauss-Newton step of TransformationEstimationPointToPlane.
+__device__ __forceinline__ void plane_update(const int32_t* __restrict__ offs, int b, const int32_t* __restrict__ cpre,
+                                             const double* __restrict__ part, IcpPair* __restrict__ pst, int round,
+                                             int max_iter, double rel_fitness, double rel_rmse,
+                                             double* __restrict__ pose_out, double* __restrict__ result) {
+    IcpPair s = pst[b];
+    double K = 0.0, sd = 0.0, H[21], v[6];
+    for (int e = 0; e < 21; ++e) H[e] = 0.0;
+    for (int e = 0; e < 6; ++e) v[e] = 0.0;
+    for (int g = cpre[b]; g < cpre[b + 1]; ++g) {
+        const double* o = part + (size_t)PART_PLANE * g;
+        if (!(o[0] > 0.0)) continue;
+        K += o[0];
+        sd += o[1];
+        for (int e = 0; e < 21; ++e) H[e] += o[2 + e];
+        for (int e = 0; e < 6; ++e) v[e] += o[23 + e];
+    }
+    const int n_src = offs[b + 1] - offs[b];
+    const double fit = n_src > 0 ? K / (double)n_src : 0.0;
+    const double rmse = K > 0.0 ? sqrt(sd / K) : 0.0;
+    const bool conv = round > 0 && fabs(s.fit - fit) < rel_fitness && fabs(s.rmse - rmse) < rel_rmse;
+    s.fit = fit; s.rmse = rmse; s.k = (int)K;
+    if (conv || round >= max_iter) {
+        s.done = 1;
+    } else {
+        double R[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}}, t[3] = {0.0, 0.0, 0.0}, x[6];
+        if (K > 0.0 && solve6_ldlt(H, v, x)) {
+            double sa, ca, sb, cb, sc, cc;
+            sincos(x[0], &sa, &ca);
+            sincos(x[1], &sb, &cb);
+            sincos(x[2], &sc, &cc);
+            R[0][0] = cc * cb; R[0][1] = cc * sb * sa - sc * ca; R[0][2] = cc * sb * ca + sc * sa;
+            R[1][0] = sc * cb; R[1][1] = sc * sb * sa + cc * ca; R[1][2] = sc * sb * ca - cc * sa;
+            R[2][0] = -sb;     R[2][1] = cb * sa;                R[2][2] = cb * ca;
+            for (int r = 0; r < 3; ++r) t[r] = x[3 + r];
+        }
+        double* T = pose_out + 12 * b;
+        double N[12];
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) s.upd[4 * r + c] = R[r][c];
+            s.upd[4 * r + 3] = t[r];
+        }
+        for (int r = 0; r < 3; ++r)                       // update . T as rigid transforms, as point-to-point
+            for (int c = 0; c < 4; ++c) {
+                const double v = __dadd_rn(__dadd_rn(__dmul_rn(R[r][0], T[c]), __dmul_rn(R[r][1], T[4 + c])),
+                                           __dmul_rn(R[r][2], T[8 + c]));
+                N[4 * r + c] = c == 3 ? __dadd_rn(v, t[r]) : v;
+            }
+        for (int e = 0; e < 12; ++e) T[e] = N[e];
+        s.iters = round + 1;
+    }
+    pst[b] = s;
+    double* o = result + 4 * b;
+    o[0] = fit; o[1] = rmse; o[2] = K; o[3] = (double)s.iters;
+}
+
 // One thread per pair.  The pair's chunks are combined in chunk order (the pairwise update of means and
 // co-moments), giving k, fitness = k / n and inlier RMSE = sqrt(sum d2 / k) of the current correspondences.  After
 // round 0 the stop test |d fitness| < rel_fitness and |d rmse| < rel_rmse ends the pair; so does round max_iter.
 // Otherwise Umeyama without scaling on the correspondences: Sigma = C / k, SVD, reflection fix when
 // det(U) det(V) < 0, R = U S V^T, t = mean_q - R mean_p (the identity with k = 0); T = update . T.
+//
+// Point-to-plane (PLANE): the chunks' J^T J and J^T r are summed in chunk order, and J^T J x = -J^T r is solved by
+// LDL^T in float64 (Open3D's SolveLinearSystemPSD: the identity when k = 0 or |det J^T J| < 1e-6 or det is not
+// finite); the update is R = Rz(x2) Ry(x1) Rx(x0), t = (x3, x4, x5) (TransformVector6dToMatrix4d).
+template <bool PLANE>
 __global__ void __launch_bounds__(UPD_THREADS)
 k_icp_update(const int32_t* __restrict__ offs, int B, const int32_t* __restrict__ cpre,
              const double* __restrict__ part, IcpPair* __restrict__ pst, int round, int max_iter, double rel_fitness,
              double rel_rmse, double* __restrict__ pose_out, double* __restrict__ result) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B || pst[b].done) return;
+    if constexpr (PLANE) {
+        plane_update(offs, b, cpre, part, pst, round, max_iter, rel_fitness, rel_rmse, pose_out, result);
+        return;
+    }
     IcpPair s = pst[b];
     double K = 0.0, sd = 0.0, mp[3] = {0.0, 0.0, 0.0}, mq[3] = {0.0, 0.0, 0.0}, C[9];
     for (int e = 0; e < 9; ++e) C[e] = 0.0;
@@ -290,7 +437,7 @@ IcpWs carve_icp(void* ws, int n_cap, int B) {
     const size_t n = (size_t)n_cap;
     w.P = (double*)take(sizeof(double) * 3 * n);
     w.d2 = (double*)take(sizeof(double) * n);
-    w.part = (double*)take(sizeof(double) * PART * (size_t)n_chunks_cap(n_cap, B));
+    w.part = (double*)take(sizeof(double) * PART_PLANE * (size_t)n_chunks_cap(n_cap, B));   // the larger record
     w.x32 = (float*)take(sizeof(float) * 3 * n);
     w.tofs = (int32_t*)take(sizeof(int32_t) * ((size_t)B + 1));
     w.cpre = (int32_t*)take(sizeof(int32_t) * ((size_t)B + 1));
@@ -313,8 +460,9 @@ size_t regtr_icp_ws_bytes(int n_cap, int B) {
 size_t regtr_icp_state_bytes(int n_cap) { return regtr_cellgrid_state_bytes(n_cap > 0 ? n_cap : 1); }
 
 int regtr_icp(const double* xyz, const int32_t* offs, int B, int n_cap, const double* init, double max_dist,
-              float cell, int max_iter, double rel_fitness, double rel_rmse, double* pose_out, double* result,
-              uint32_t* status, void* ws, size_t ws_bytes, void* state, size_t state_bytes, void* stream_) {
+              float cell, int max_iter, double rel_fitness, double rel_rmse, const double* tgt_normals,
+              double* pose_out, double* result, uint32_t* status, void* ws, size_t ws_bytes, void* state,
+              size_t state_bytes, void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (!offs || !init || !pose_out || !result || !status || !ws || !state || B <= 0 || 2 * B > 32767 || n_cap < 0 ||
         !(max_dist > 0.0) || !((double)cell > max_dist) || max_iter < 0 || !(rel_fitness >= 0.0) ||
@@ -340,12 +488,19 @@ int regtr_icp(const double* xyz, const int32_t* offs, int B, int n_cap, const do
         k_icp_nn<<<nn_blocks, NN_WARPS * 32, 0, st>>>(xyz, offs, B, nc, w.P, w.pst, round > 0, table, log2t, sxyzi,
                                                       cell, max_dist * max_dist, bound, w.nn, w.d2, status);
         REGTR_CHECK_LAUNCH();
-        k_icp_reduce<<<n_chunks_cap(nc, B), RED_THREADS, 0, st>>>(xyz, offs, B, w.cpre, w.P, w.nn, w.d2, w.pst,
-                                                                  w.part);
-        REGTR_CHECK_LAUNCH();
-        k_icp_update<<<regtr_cdiv(B, UPD_THREADS), UPD_THREADS, 0, st>>>(offs, B, w.cpre, w.part, w.pst, round,
-                                                                         max_iter, rel_fitness, rel_rmse, pose_out,
-                                                                         result);
+        if (tgt_normals) {
+            k_icp_reduce<true><<<n_chunks_cap(nc, B), RED_THREADS, 0, st>>>(xyz, offs, B, w.cpre, w.P, w.nn, w.d2,
+                                                                            w.pst, w.part, tgt_normals);
+            REGTR_CHECK_LAUNCH();
+            k_icp_update<true><<<regtr_cdiv(B, UPD_THREADS), UPD_THREADS, 0, st>>>(
+                offs, B, w.cpre, w.part, w.pst, round, max_iter, rel_fitness, rel_rmse, pose_out, result);
+        } else {
+            k_icp_reduce<false><<<n_chunks_cap(nc, B), RED_THREADS, 0, st>>>(xyz, offs, B, w.cpre, w.P, w.nn, w.d2,
+                                                                             w.pst, w.part, nullptr);
+            REGTR_CHECK_LAUNCH();
+            k_icp_update<false><<<regtr_cdiv(B, UPD_THREADS), UPD_THREADS, 0, st>>>(
+                offs, B, w.cpre, w.part, w.pst, round, max_iter, rel_fitness, rel_rmse, pose_out, result);
+        }
         REGTR_CHECK_LAUNCH();
     }
     return REGTR_OK;

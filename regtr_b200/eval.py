@@ -376,18 +376,32 @@ def summarize_modelnet_metrics(metrics: Dict[str, np.ndarray]) -> Dict[str, floa
 # ------------------------------------------------------------------- test loop (reference: test.py)
 
 
-def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None):
-    """Wrap `forward_fn(batch) -> pred` so that the final pose of every pair is refined by point-to-point ICP on the
-    batch's full clouds: -> a NEW dict with pred's entries, pose (1,B,3,4) float64 the refined poses and pose_coarse
+def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None, method: str = 'point_to_point',
+                normal_radius: float = None, normal_max_nn: int = 30, estimate_normals=None):
+    """Wrap `forward_fn(batch) -> pred` so that the final pose of every pair is refined by ICP on the batch's full
+    clouds: -> a NEW dict with pred's entries, pose (1,B,3,4) float64 the refined poses and pose_coarse
     (1,B,3,4) float64 the network's final poses (so that `compute_metrics` reports both, and EstLogWriter writes the
     refined ones).  pred's own tensors are not written to (a graphed forward owns them).
-    icp(src_list, tgt_list, init (B,3,4), radius, max_iteration) -> (pose (B,3,4), result): default `ops.icp`."""
+    icp(src_list, tgt_list, init (B,3,4), radius, max_iteration) -> (pose (B,3,4), result): default `ops.icp`,
+    point-to-point.  method='point_to_plane': the targets' normals come from
+    estimate_normals(tgt_list, normal_radius (default 2 * radius), normal_max_nn) (default `ops.estimate_normals`) and
+    icp is called as icp(src_list, tgt_list, init, radius, max_iteration, method=method, tgt_normals=normals)."""
+    if method not in ('point_to_point', 'point_to_plane'):
+        raise ValueError(f'icp_forward: unknown method {method!r}')
     if icp is None:
         from .ops import icp
+    if method == 'point_to_plane' and estimate_normals is None:
+        from .ops import estimate_normals
+    nr = 2.0 * radius if normal_radius is None else normal_radius
     def run(batch):
         pred = forward_fn(batch)
         coarse = pred['pose'][-1].to(torch.float64)                     # (B,3,4), a new tensor
-        pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration)
+        if method == 'point_to_point':
+            pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration)
+        else:
+            normals = estimate_normals(batch['tgt_xyz'], nr, normal_max_nn)
+            pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, method=method,
+                          tgt_normals=normals)
         out = dict(pred)
         out['pose'] = torch.as_tensor(pose, dtype=torch.float64, device=coarse.device).reshape(coarse.shape)[None]
         out['pose_coarse'] = coarse[None]

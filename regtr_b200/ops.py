@@ -1253,24 +1253,48 @@ def icp_launches(max_iteration: int) -> int:
     return 5 + 3 * (int(max_iteration) + 1)
 
 
+ICP_METHODS = ('point_to_point', 'point_to_plane')
+
+
 def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iteration: int = 30,
-        relative_fitness: float = 1e-6, relative_rmse: float = 1e-6, status=None):
-    """Point-to-point ICP of B pairs (regtr_icp): Open3D's registration_icp with TransformationEstimationPointToPoint
-    (no scaling) and ICPConvergenceCriteria(relative_fitness, relative_rmse, max_iteration), on the device.
+        relative_fitness: float = 1e-6, relative_rmse: float = 1e-6, status=None, method: str = 'point_to_point',
+        tgt_normals=None):
+    """ICP of B pairs (regtr_icp): Open3D's registration_icp with TransformationEstimationPointToPoint (no scaling) or,
+    with method='point_to_plane', TransformationEstimationPointToPlane, and ICPConvergenceCriteria(relative_fitness,
+    relative_rmse, max_iteration), on the device.
     src_list / tgt_list: B clouds (n,3) each (numpy or torch, any float dtype; stacked in float64 on the device);
-    init (B,3,4) source -> target.  -> (pose (B,3,4) float64, result (B,4) float64 = fitness, inlier_rmse, n_corr,
-    iterations), both device tensors.  No host sync unless status is None: then a word of this call is read and a
-    coordinate of a moved source or of a target beyond `overlap_coord_bound(max_correspondence_distance)` raises
-    RegtrLibError; with the caller's word, `check_fit_status` does that where the caller syncs."""
+    init (B,3,4) source -> target.  tgt_normals: with 'point_to_plane', B (n,3) normals aligned with tgt_list (e.g.
+    `estimate_normals(tgt_list, ...)`); a zero normal drops its correspondence out of the update.
+    -> (pose (B,3,4) float64, result (B,4) float64 = fitness, inlier_rmse, n_corr, iterations), both device tensors.
+    No host sync unless status is None: then a word of this call is read and a coordinate of a moved source or of a
+    target beyond `overlap_coord_bound(max_correspondence_distance)` raises RegtrLibError; with the caller's word,
+    `check_fit_status` does that where the caller syncs."""
     L = _lib.load()
     r = float(max_correspondence_distance)
     if not r > 0.0 or int(max_iteration) < 0 or not (relative_fitness >= 0.0 and relative_rmse >= 0.0):
         raise ValueError(f'icp: max_correspondence_distance {r} must be > 0, max_iteration {max_iteration} >= 0, '
                          f'relative_fitness / relative_rmse >= 0')
+    if method not in ICP_METHODS:
+        raise ValueError(f'icp: method {method!r} is not one of {ICP_METHODS}')
+    plane = method == 'point_to_plane'
+    if plane and tgt_normals is None:
+        raise ValueError('icp: point_to_plane needs the target normals (tgt_normals), e.g. from estimate_normals')
     B = len(src_list)
     dev = init.device if torch.is_tensor(init) and init.is_cuda else None
     xyz, offs, lens = _stack_pairs(src_list, tgt_list, 'icp', dev)
     dev = xyz.device
+    nrm = None
+    if plane:
+        if len(tgt_normals) != B:
+            raise ValueError(f'icp: {len(tgt_normals)} target normal arrays for {B} pairs')
+        nrm = torch.empty((max(sum(lens[B:]), 1), 3), dtype=torch.float64, device=dev)
+        a = 0
+        for c, ln in zip(tgt_normals, lens[B:]):
+            c = torch.as_tensor(c)
+            if tuple(c.shape) != (ln, 3):
+                raise ValueError(f'icp: target normals {tuple(c.shape)} for a target of {ln} points')
+            nrm[a:a + ln].copy_(c.to(dev, torch.float64))
+            a += ln
     init64 = torch.as_tensor(init).to(dev, torch.float64).reshape(B, 3, 4).contiguous()
     n = sum(lens)
     own = status is None
@@ -1281,12 +1305,71 @@ def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iterat
     ws = workspace(L.regtr_icp_ws_bytes(n, B), dev)
     state = workspace(L.regtr_icp_state_bytes(n), dev, 'scan_state', zero=True)
     _lib.check(L.regtr_icp(_p(xyz), _p(offs), B, n, _p(init64), r, overlap_cell(r), int(max_iteration),
-                           float(relative_fitness), float(relative_rmse), _p(pose), _p(out), _p(status), _p(ws),
-                           ws.numel(), _p(state), state.numel(), _stream()), 'regtr_icp')
+                           float(relative_fitness), float(relative_rmse), _p(nrm), _p(pose),
+                           _p(out), _p(status), _p(ws), ws.numel(), _p(state), state.numel(), _stream()), 'regtr_icp')
     _count(icp_launches(max_iteration))
     if own:
         check_fit_status(status, r, 'icp')
     return pose, out
+
+
+NORMALS_MAX_NN = 64
+
+
+def normals_launches() -> int:
+    """Kernel launches of one `estimate_normals` call: the set-up, the cell list (4), the per-point solve."""
+    return 6
+
+
+def estimate_normals(clouds, radius: float, max_nn: int = 30, status=None, return_counts: bool = False):
+    """Normals of C clouds (regtr_estimate_normals): Open3D's estimate_normals(KDTreeSearchParamHybrid(radius,
+    max_nn)) oriented towards the origin, with the library's rules (the max_nn nearest points of the own cloud
+    strictly within `radius`, the point itself included, ties to the lower index; a zero normal with fewer than 3).
+    clouds: C (n,3) clouds (numpy or torch, any float dtype; stacked in float64 on the device).
+    -> list of C (n,3) float64 device tensors; with return_counts also the list of (n,) int32 neighbour counts.
+    No host sync unless status is None: then a word of this call is read and a coordinate beyond
+    `overlap_coord_bound(radius)`, or not finite, raises RegtrLibError; with the caller's word, `check_fit_status`
+    does that where the caller syncs."""
+    L = _lib.load()
+    r = float(radius)
+    if not r > 0.0 or not 1 <= int(max_nn) <= NORMALS_MAX_NN:
+        raise ValueError(f'estimate_normals: radius {r} must be > 0 and max_nn {max_nn} in 1..{NORMALS_MAX_NN}')
+    C = len(clouds)
+    if C == 0:
+        raise ValueError('estimate_normals: expected at least one cloud')
+    ts = [torch.as_tensor(c) for c in clouds]
+    for c in ts:
+        if c.dim() != 2 or c.shape[1] != 3:
+            raise ValueError(f'estimate_normals: expected (n,3) clouds, got {tuple(c.shape)}')
+    dev = next((c.device for c in ts if c.is_cuda), torch.device('cuda', torch.cuda.current_device()))
+    lens = [int(c.shape[0]) for c in ts]
+    n = sum(lens)
+    xyz = torch.empty((max(n, 1), 3), dtype=torch.float64, device=dev)
+    a = 0
+    for c, ln in zip(ts, lens):
+        xyz[a:a + ln].copy_(c.to(dev, torch.float64))
+        a += ln
+    offs = make_offsets(lens, dev)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    normals = torch.empty((max(n, 1), 3), dtype=torch.float64, device=dev)
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev) if return_counts else None
+    ws = workspace(L.regtr_estimate_normals_ws_bytes(n), dev)
+    state = workspace(L.regtr_estimate_normals_state_bytes(n), dev, 'scan_state', zero=True)
+    _lib.check(L.regtr_estimate_normals(_p(xyz), _p(offs), C, n, r, overlap_cell(r), int(max_nn), _p(normals),
+                                        _p(counts), _p(status), _p(ws), ws.numel(),
+                                        _p(state), state.numel(), _stream()), 'regtr_estimate_normals')
+    _count(normals_launches())
+    if own:
+        check_fit_status(status, r, 'estimate_normals')
+    bounds = [0]
+    for ln in lens:
+        bounds.append(bounds[-1] + ln)
+    out = [normals[bounds[k]:bounds[k + 1]] for k in range(C)]
+    if return_counts:
+        return out, [counts[bounds[k]:bounds[k + 1]] for k in range(C)]
+    return out
 
 
 def check_fit_status(status, radius: float, what: str = 'registration_fit'):

@@ -1,7 +1,9 @@
 """Register two point-cloud files with a trained RegTR: the reference's `src/demo.py` on the library path.
 
     python -m regtr_b200.register SRC TGT --ckpt <logdir>/ckpt/model-best.pth [--config <yaml>] \\
-        [--threshold 0.5] [--fit_radius R] [--icp R [--icp_iters 30]] [--out DIR]
+        [--threshold 0.5] [--fit_radius R] [--out DIR]
+        [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane [--normal_radius NR]
+         [--normal_max_nn 30]]]
 
 SRC / TGT: .ply, .pth, .bin or .npy (regtr_b200.pointio).  The config is the config.yaml one level above the
 checkpoint's directory, the layout `python -m regtr_b200.train` writes, unless --config names another.  Instead of the
@@ -13,12 +15,14 @@ demo's viewer, the result is judged by the fitness and inlier RMSE of the final 
   src_registered.ply   the source moved by the pose;
   src_kp.ply, src_kp_warped.ply   the source keypoints with predicted overlap > --threshold and their predicted
                        positions in the target, with an `overlap` property (the demo's two upper panels).
-With --icp R the final decoder layer's pose is refined by point-to-point ICP on the cropped full-resolution clouds
-(`ops.icp`, Open3D's registration_icp with max_correspondence_distance R and --icp_iters iterations at most);
+With --icp R the final decoder layer's pose is refined by ICP on the cropped full-resolution clouds (`ops.icp`,
+Open3D's registration_icp with max_correspondence_distance R and --icp_iters iterations at most), point-to-point by
+default; --icp_method point_to_plane first estimates the cropped target's normals (`ops.estimate_normals`, Open3D's
+estimate_normals with KDTreeSearchParamHybrid(--normal_radius, default 2 R, --normal_max_nn));
 pose.txt, src_registered.ply and fit then use the refined pose, result.npz gains pose_coarse (the network's final
 pose), pose_icp (the refined one) and icp (4,) = fitness, inlier_rmse, correspondences, iterations.
 One JSON line on stdout: the pose, the four fit numbers and the point counts (with --icp, also icp_fitness, icp_rmse,
-icp_iterations and icp_radius).
+icp_iterations, icp_radius and icp_method).
 """
 from __future__ import annotations
 
@@ -45,6 +49,12 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument('--icp', type=float, metavar='R',
                     help='Refine the pose with point-to-point ICP, max correspondence distance R (default: no ICP)')
     ap.add_argument('--icp_iters', type=int, default=30, help='ICP iterations at most (with --icp)')
+    ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane'), default='point_to_point',
+                    help='ICP error metric (with --icp); point_to_plane estimates the target normals first')
+    ap.add_argument('--normal_radius', type=float, metavar='NR',
+                    help='Normal estimation radius of point_to_plane ICP (default: 2 * the --icp radius)')
+    ap.add_argument('--normal_max_nn', type=int, default=30,
+                    help='Neighbours at most of the normal estimation (with point_to_plane ICP)')
     ap.add_argument('--out', default='.', help='Output directory')
     return ap
 
@@ -72,13 +82,16 @@ def load_model(cfg, ckpt: str, device=None):
 
 
 def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: float = None,
-             icp_radius: float = None, icp_iters: int = 30) -> Dict:
+             icp_radius: float = None, icp_iters: int = 30, icp_method: str = 'point_to_point',
+             normal_radius: float = None, normal_max_nn: int = 30) -> Dict:
     """Crop, forward and fit one pair.  src_xyz / tgt_xyz (N,3) float64 host arrays.
     -> dict of host arrays: src_xyz / tgt_xyz (cropped, float64), pose (L,3,4) fp32, src_kp, src_kp_warped (final
     layer), src_overlap (sigmoid of the final layer's logit, (n,)), the same for tgt, fit (4,) float64.
-    icp_radius: refine the final layer's pose by point-to-point ICP (`ops.icp`, at most icp_iters iterations) on the
+    icp_radius: refine the final layer's pose by ICP (`ops.icp` with icp_method, at most icp_iters iterations) on the
     cropped clouds; fit is then that of the refined pose, and the dict gains pose_coarse (3,4) fp32 (the network's
-    final pose), pose_icp (3,4) float64 and icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations."""
+    final pose), pose_icp (3,4) float64 and icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations.
+    icp_method 'point_to_plane' refines against the cropped target's normals from `ops.estimate_normals` at
+    normal_radius (default 2 * icp_radius) and normal_max_nn."""
     from . import ops
     src_xyz = crop(cfg, np.asarray(src_xyz, dtype=np.float64))
     tgt_xyz = crop(cfg, np.asarray(tgt_xyz, dtype=np.float64))
@@ -92,7 +105,12 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
         status = ops.new_status(dev)
         final = pose[-1:]
         if icp_radius is not None:
-            final, icp = ops.icp([src_xyz], [tgt_xyz], pose[-1:], icp_radius, icp_iters)
+            normals = None
+            if icp_method == 'point_to_plane':
+                nr = 2.0 * icp_radius if normal_radius is None else normal_radius
+                normals = ops.estimate_normals([tgt_xyz], nr, normal_max_nn)
+            final, icp = ops.icp([src_xyz], [tgt_xyz], pose[-1:], icp_radius, icp_iters, method=icp_method,
+                                 tgt_normals=normals)
         fit = ops.registration_fit([src_xyz], [tgt_xyz], final, radius, status)
         res = {'src_xyz': src_xyz, 'tgt_xyz': tgt_xyz, 'pose': pose.cpu().numpy()}
         if icp_radius is not None:
@@ -145,7 +163,7 @@ def main(argv=None):
     cfg = load_config(str(cfg_file))
     model = load_model(cfg, opt.ckpt)
     res = register(model, cfg, load_point_cloud(opt.src), load_point_cloud(opt.tgt), opt.fit_radius, opt.icp,
-                   opt.icp_iters)
+                   opt.icp_iters, opt.icp_method, opt.normal_radius, opt.normal_max_nn)
     n_shown = write_outputs(res, opt.out, opt.threshold)
     f = [float(v) for v in res['fit']]
     line = {'pose': pose44(res['pose_icp'] if opt.icp is not None else res['pose'][-1]).tolist(),
@@ -156,7 +174,8 @@ def main(argv=None):
             'fit_radius': float(cfg['overlap_radius'] if opt.fit_radius is None else opt.fit_radius)}
     if opt.icp is not None:
         icp = [float(v) for v in res['icp']]
-        line.update(icp_fitness=icp[0], icp_rmse=icp[1], icp_iterations=int(icp[3]), icp_radius=float(opt.icp))
+        line.update(icp_fitness=icp[0], icp_rmse=icp[1], icp_iterations=int(icp[3]), icp_radius=float(opt.icp),
+                    icp_method=opt.icp_method)
     print(json.dumps(line))
     return res
 

@@ -1,11 +1,14 @@
-"""Time point-to-point ICP (`ops.icp`) on synthetic 3DMatch-shaped pairs (~20k points per cloud), starting from the
-ground truth perturbed by a few degrees and centimetres, at B = 1 and B = 8; and the float64 CPU oracle
-(tests/icp_oracle.py) on the same inputs.
+"""Time ICP (`ops.icp`) on synthetic 3DMatch-shaped pairs (~20k points per cloud), starting from the ground truth
+perturbed by a few degrees and centimetres, at B = 1 and B = 8; and the float64 CPU oracle (tests/icp_oracle.py,
+tests/icp_plane_oracle.py) on the same inputs.
 
-    python scripts/bench_icp.py [--iters 30] [--radius 0.0375] [--blocks 7] [--reps 10]
+    python scripts/bench_icp.py [--method point_to_point|point_to_plane] [--iters 30] [--radius 0.0375]
+        [--normal_radius 2R] [--normal_max_nn 30] [--blocks 7] [--reps 10]
 
 CUDA events after warm-up: `--blocks` blocks of `--reps` calls each; the median and the spread (min..max) of the
-per-call block means.  Prints one JSON line with the card name and power limit read in the same run."""
+per-call block means.  With point_to_plane, the targets' normal estimation (`ops.estimate_normals`) and the ICP are
+timed separately, and the iterations each pair needed are reported under both methods.  Prints one JSON line with the
+card name and power limit read in the same run."""
 import argparse
 import json
 import os
@@ -49,30 +52,53 @@ def card():
     return name, power
 
 
-def time_device(pairs, iters, radius, blocks, reps):
+def time_calls(call, radius, what, blocks, reps):
+    """call(status) -> result: (per-call ms of each block, launches of one call, the result of one call)."""
     dev = torch.device('cuda:0')
-    src = [torch.from_numpy(s).to(dev) for s, _, _ in pairs]
-    tgt = [torch.from_numpy(t).to(dev) for _, t, _ in pairs]
-    init = torch.from_numpy(np.stack([p for _, _, p in pairs])).to(dev)
     status = ops.new_status(dev)
     for _ in range(3):
-        ops.icp(src, tgt, init, radius, iters, status=status)
+        call(status)
     torch.cuda.synchronize()
-    ops.check_fit_status(status, radius, 'icp')
+    ops.check_fit_status(status, radius, what)
     before = ops.LAUNCHES
-    _, res = ops.icp(src, tgt, init, radius, iters, status=status)
+    res = call(status)
     launches = ops.LAUNCHES - before
     per_call = []
     for _ in range(blocks):
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         for _ in range(reps):
-            ops.icp(src, tgt, init, radius, iters, status=status)
+            call(status)
         b.record()
         b.synchronize()
         per_call.append(a.elapsed_time(b) / reps)
-    ops.check_fit_status(status, radius, 'icp')
-    return per_call, launches, res.cpu().numpy()
+    ops.check_fit_status(status, radius, what)
+    return per_call, launches, res
+
+
+def time_device(pairs, iters, radius, blocks, reps, method='point_to_point', normal_radius=None, normal_max_nn=30):
+    """-> dict of the timings of one batch (ms per call, launches) and the iterations each pair needed."""
+    dev = torch.device('cuda:0')
+    src = [torch.from_numpy(s).to(dev) for s, _, _ in pairs]
+    tgt = [torch.from_numpy(t).to(dev) for _, t, _ in pairs]
+    init = torch.from_numpy(np.stack([p for _, _, p in pairs])).to(dev)
+    out = {}
+    normals = None
+    if method == 'point_to_plane':
+        ms, launches, normals = time_calls(lambda st: ops.estimate_normals(tgt, normal_radius, normal_max_nn, st),
+                                           normal_radius, 'estimate_normals', blocks, reps)
+        out.update(normals_ms_median=float(np.median(ms)), normals_ms_min=float(min(ms)),
+                   normals_ms_max=float(max(ms)), normals_launches_per_call=launches)
+        _, p2p = ops.icp(src, tgt, init, radius, iters)
+        out['iterations_needed_point_to_point'] = [int(v) for v in p2p[:, 3].cpu().numpy()]
+    ms, launches, (_, res) = time_calls(
+        lambda st: ops.icp(src, tgt, init, radius, iters, status=st, method=method, tgt_normals=normals), radius,
+        'icp', blocks, reps)
+    res = res.cpu().numpy()
+    out.update(gpu_ms_median=float(np.median(ms)), gpu_ms_min=float(min(ms)), gpu_ms_max=float(max(ms)),
+               launches_per_call=launches, iterations_needed=[int(v) for v in res[:, 3]],
+               fitness=[round(float(v), 4) for v in res[:, 0]])
+    return out, ([n.cpu().numpy() for n in normals] if normals is not None else None)
 
 
 def main():
@@ -82,25 +108,35 @@ def main():
     ap.add_argument('--blocks', type=int, default=7)
     ap.add_argument('--reps', type=int, default=10)
     ap.add_argument('--cpu-reps', type=int, default=1)
+    ap.add_argument('--method', choices=('point_to_point', 'point_to_plane'), default='point_to_point')
+    ap.add_argument('--normal_radius', type=float, help='default: 2 * --radius')
+    ap.add_argument('--normal_max_nn', type=int, default=30)
     opt = ap.parse_args()
     import icp_oracle as I
+    import icp_plane_oracle as N
+    nr = 2.0 * opt.radius if opt.normal_radius is None else opt.normal_radius
     name, power = card()
-    out = {'card': name, 'power_limit': power, 'iters': opt.iters, 'radius': opt.radius}
+    out = {'card': name, 'power_limit': power, 'method': opt.method, 'iters': opt.iters, 'radius': opt.radius}
+    if opt.method == 'point_to_plane':
+        out.update(normal_radius=nr, normal_max_nn=opt.normal_max_nn)
     for B in (1, 8):
         pairs = perturbed_pairs(B)
-        ms, launches, res = time_device(pairs, opt.iters, opt.radius, opt.blocks, opt.reps)
+        row, normals = time_device(pairs, opt.iters, opt.radius, opt.blocks, opt.reps, opt.method, nr,
+                                   opt.normal_max_nn)
         cpu = []
         for _ in range(opt.cpu_reps):
             t0 = time.perf_counter()
-            I.icp_batch([s for s, _, _ in pairs], [t for _, t, _ in pairs], np.stack([p for _, _, p in pairs]),
-                        opt.radius, opt.iters)
+            if opt.method == 'point_to_plane':        # the oracle's own normals and ICP
+                nrm = [N.estimate_normals(t, nr, opt.normal_max_nn)[0] for _, t, _ in pairs]
+                N.icp_batch([s for s, _, _ in pairs], [t for _, t, _ in pairs], nrm,
+                            np.stack([p for _, _, p in pairs]), opt.radius, opt.iters)
+            else:
+                I.icp_batch([s for s, _, _ in pairs], [t for _, t, _ in pairs], np.stack([p for _, _, p in pairs]),
+                            opt.radius, opt.iters)
             cpu.append((time.perf_counter() - t0) * 1e3)
-        out[f'B{B}'] = {'points_per_cloud': int(np.mean([len(s) for s, _, _ in pairs] + [len(t) for _, t, _ in pairs])),
-                        'gpu_ms_median': float(np.median(ms)), 'gpu_ms_min': float(min(ms)),
-                        'gpu_ms_max': float(max(ms)), 'launches_per_call': launches,
-                        'iterations_needed': [int(v) for v in res[:, 3]],
-                        'fitness': [round(float(v), 4) for v in res[:, 0]],
-                        'cpu_oracle_ms_median': float(np.median(cpu))}
+        out[f'B{B}'] = dict({'points_per_cloud': int(np.mean([len(s) for s, _, _ in pairs] +
+                                                             [len(t) for _, t, _ in pairs]))}, **row,
+                            cpu_oracle_ms_median=float(np.median(cpu)))
     print(json.dumps(out))
 
 
