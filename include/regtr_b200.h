@@ -538,6 +538,24 @@ int regtr_overlap_nn(const double* xyz, const int32_t* offs, int B, int n_cap, c
 int regtr_registration_fit(const double* xyz, const int32_t* offs, int B, int n_cap, const double* pose,
                            double radius, const int32_t* nn, double* out, uint32_t* status, void* stream);
 
+/* Information matrices of B registered pairs (Open3D's get_information_matrix_from_point_clouds on this library's
+ * match rule), from the matches of regtr_overlap_nn: xyz, offs, pose and radius as given to it, nn its output.
+ * out (B,6,6) float64 per pair = sum over the source points i with nn_i >= 0, in ascending i, of G^T G with q the
+ * matched TARGET point in the target's own frame and
+ *   G = [[0, q_z, -q_y, 1, 0, 0], [-q_z, 0, q_x, 0, 1, 0], [q_y, -q_x, 0, 0, 0, 1]],
+ * so out[5][5] is the match count.  Its 21 unique entries are ten float64 sums (y^2 + z^2, x^2 + z^2, x^2 + y^2, xy,
+ * xz, yz, x, y, z, 1), each in a fixed order, one CTA per pair: the result is bit-reproducible and independent of
+ * the batch.  A match index outside the target, or a distance not below radius, is not counted and raises
+ * REGTR_STATUS_INPUT, as in regtr_registration_fit.  n_cap >= offs[2B].  One launch. */
+int regtr_registration_information(const double* xyz, const int32_t* offs, int B, int n_cap, const double* pose,
+                                   double radius, const int32_t* nn, double* out, uint32_t* status, void* stream);
+
+/* C stacked clouds moved by one pose each: xyz (n_cap,3) float64 with offs (C+1) i32, pose (C,3,4) float64;
+ * out (n_cap,3) fp32 = fp32(((r0 x + r1 y) + r2 z) + t) in float64, no contraction; rows >= offs[C] untouched.
+ * C <= 32767.  One launch. */
+int regtr_transform_clouds(const double* xyz, const int32_t* offs, int C, int n_cap, const double* pose, float* out,
+                           void* stream);
+
 /* ICP of B pairs (Open3D's registration_icp with TransformationEstimationPointToPoint, no scaling, or with
  * TransformationEstimationPointToPlane, and ICPConvergenceCriteria(rel_fitness, rel_rmse, max_iter)).
  * xyz (n_cap,3) float64 stacked src_0..src_{B-1},
@@ -588,6 +606,65 @@ size_t regtr_estimate_normals_state_bytes(int n_cap);
 int regtr_estimate_normals(const double* xyz, const int32_t* offs, int C, int n_cap, double radius, float cell,
                            int max_nn, double* normals, int32_t* counts, uint32_t* status, void* ws, size_t ws_bytes,
                            void* state, size_t state_bytes, void* stream);
+
+/* ---- pose graph ------------------------------------------------------------------- */
+
+#define REGTR_POSE_GRAPH_MAX_NODES 256
+
+/* Options of regtr_pose_graph_optimize (Open3D's GlobalOptimizationOption and GlobalOptimizationConvergenceCriteria;
+ * defaults in brackets). */
+typedef struct {
+    double max_correspondence_distance;      /* d of the line process */
+    double edge_prune_threshold;             /* [0.25] */
+    double preference_loop_closure;          /* [1.0] */
+    double min_relative_increment;           /* [1e-6] */
+    double min_relative_residual_increment;  /* [1e-6] */
+    double min_right_term;                   /* [1e-6] */
+    double min_residual;                     /* [1e-6] */
+    double upper_scale_factor;               /* [2/3] */
+    double lower_scale_factor;               /* [1/3] */
+    int reference_node;                      /* [0] */
+    int max_iteration;                       /* [100] */
+    int max_iteration_lm;                    /* [20] */
+} regtr_pose_graph_options;
+
+/* Robust optimisation of G independent pose graphs (Open3D's global_optimization with
+ * GlobalOptimizationLevenbergMarquardt; Choi, Zhou and Koltun 2015, section 5).  All arithmetic is float64.
+ * Graph g owns nodes [node_offs[g], node_offs[g+1]) and edges [edge_offs[g], edge_offs[g+1]) (int32 device offsets);
+ * poses (n_nodes,3,4) fragment -> world, read as the initial poses and overwritten with the result; edges (n_edges,2)
+ * graph-local (s, t); X (n_edges,3,4) maps source-fragment into target-fragment coordinates (rigid: X^-1 is taken as
+ * [R^T | -R^T t]); info (n_edges,6,6); uncertain (n_edges) nonzero for a loop closure.
+ *   zeta_e = v(X^-1 P_t^-1 P_s), v(M) = ((M21-M12)/2, (M02-M20)/2, (M10-M01)/2, M03, M13, M23);
+ *   J_s[:,k] = v(X^-1 P_t^-1 A_k P_s) (A_k the generators of rotations about x, y, z and translations), J_t = -J_s;
+ *   P_n <- T(delta_n) P_n, T(delta) = [Rz(d2) Ry(d1) Rx(d0) | d3..5];
+ *   mu = preference * d^2 * mean Lambda_e[5][5]; F = sum c_e zeta^T Lambda zeta + mu sum (sqrt(c_e) - 1)^2;
+ *   H = sum c_e [J_s J_t]^T Lambda [J_s J_t], b = -sum c_e [J_s J_t]^T Lambda zeta (dense 6N system);
+ *   confidence update (uncertain edges only): c_e = (mu / (mu + zeta^T Lambda zeta))^2, certain edges c_e = 1.
+ * LM: lambda = 1e-5 max diag H, nu = 2; stop when max|b| < min_right_term.  Per outer iteration up to
+ * max_iteration_lm attempts: Cholesky of H + lambda I (a failure is a rejected step); stop when |delta| <
+ * min_rel_inc (|x| + min_rel_inc), x the stacked v(P_n); F' at the moved poses, rho = (F - F') / (delta . (lambda delta
+ * + b) + 1e-3); rho > 0 accepts the step (stop when |F - F'| < min_rel_res_inc F; recompute zeta, H, b; stop when
+ * max|b| < min_right_term; lambda *= max(lower, min(upper, 1 - (2 rho - 1)^3)), nu = 2), else lambda *= nu, nu *= 2;
+ * out of attempts stops.  Then the confidences, F, H and b are updated; stop when F < min_residual or at
+ * max_iteration.  A graph without edges or with H = 0 is returned unchanged.
+ * Two passes: all edges, then (from pass 1's poses and confidences, mu over the kept edges) the edges left after
+ * dropping every uncertain edge with c_e < edge_prune_threshold.  Gauge: P_n <- P_ref^0 P_ref^-1 P_n, the reference
+ * node written back bit for bit (nothing is touched when no step was accepted).
+ * confidence (n_edges) float64, kept (n_edges) uint8, result (G,4) float64 = (pass-1 iterations, pass-2 iterations,
+ * final objective, edges kept).  max_nodes >= every graph's node count: above REGTR_POSE_GRAPH_MAX_NODES
+ * REGTR_ERR_UNSUPPORTED.  sq_nodes = sum over the graphs of N_g^2 (graph g's dense system lives at 36 sum_{g'<g} N_g'^2
+ * doubles of the workspace).  A graph with more nodes than max_nodes or beyond sq_nodes, s = t, an index out of
+ * range, a reference node out of range or a non-finite pose, X or info raises REGTR_STATUS_INPUT and is left as it
+ * was (confidence 0, kept 0, result (0, 0, nan, 0)).  One persistent CTA per graph: one launch whatever G, N or convergence, no host
+ * synchronisation, sums in a fixed order: a graph's result is bit-identical alone or in a batch.
+ * ws: regtr_pose_graph_ws_bytes (36 * sq_nodes * 16 bytes for the dense systems and their factors, plus per-node
+ * and per-edge terms). */
+size_t regtr_pose_graph_ws_bytes(int G, int n_nodes, int n_edges, long long sq_nodes);
+int regtr_pose_graph_optimize(const int32_t* node_offs, const int32_t* edge_offs, int G, int n_nodes, int n_edges,
+                              int max_nodes, long long sq_nodes, double* poses, const int32_t* edges, const double* X,
+                              const double* info, const uint8_t* uncertain, const regtr_pose_graph_options* opt,
+                              double* confidence, uint8_t* kept, double* result, uint32_t* status, void* ws,
+                              size_t ws_bytes, void* stream);
 
 /* Per-pair flags of regtr_train_augment */
 #define REGTR_PREP_PERTURB_SRC 1  /* the perturbation moves the source (else the target) */

@@ -311,14 +311,7 @@ __device__ __forceinline__ void plane_update(const int32_t* __restrict__ offs, i
     } else {
         double R[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}}, t[3] = {0.0, 0.0, 0.0}, x[6];
         if (K > 0.0 && solve6_ldlt(H, v, x)) {
-            double sa, ca, sb, cb, sc, cc;
-            sincos(x[0], &sa, &ca);
-            sincos(x[1], &sb, &cb);
-            sincos(x[2], &sc, &cc);
-            R[0][0] = cc * cb; R[0][1] = cc * sb * sa - sc * ca; R[0][2] = cc * sb * ca + sc * sa;
-            R[1][0] = sc * cb; R[1][1] = sc * sb * sa + cc * ca; R[1][2] = sc * sb * ca - cc * sa;
-            R[2][0] = -sb;     R[2][1] = cb * sa;                R[2][2] = cb * ca;
-            for (int r = 0; r < 3; ++r) t[r] = x[3 + r];
+            rigid_from_vec6(x, R, t);
         }
         double* T = pose_out + 12 * b;
         double N[12];

@@ -1,5 +1,5 @@
 // Internal to the library: float64 rigid-transform helpers shared by the pose solve (kabsch.cu), the training-data
-// preparation (traindata.cu) and ICP (icp.cu).
+// preparation (traindata.cu), ICP (icp.cu) and the pose-graph optimiser (posegraph.cu).
 #pragma once
 
 #include "common.cuh"
@@ -9,6 +9,19 @@ namespace {
 // ((m0 x + m1 y) + m2 z) + m3 in float64, no contraction: the fixed operation order of every rigid transform here
 __device__ __forceinline__ double rt_row(const double* m, double x, double y, double z) {
     return __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(m[0], x), __dmul_rn(m[1], y)), __dmul_rn(m[2], z)), m[3]);
+}
+
+// x = (rx, ry, rz, tx, ty, tz) -> R = Rz(rz) Ry(ry) Rx(rx), t = (tx, ty, tz) (Open3D's TransformVector6dToMatrix4d):
+// the update of point-to-plane ICP (icp.cu) and of the pose-graph optimiser (posegraph.cu)
+__device__ __forceinline__ void rigid_from_vec6(const double x[6], double R[3][3], double t[3]) {
+    double sa, ca, sb, cb, sc, cc;
+    sincos(x[0], &sa, &ca);
+    sincos(x[1], &sb, &cb);
+    sincos(x[2], &sc, &cc);
+    R[0][0] = cc * cb; R[0][1] = cc * sb * sa - sc * ca; R[0][2] = cc * sb * ca + sc * sa;
+    R[1][0] = sc * cb; R[1][1] = sc * sb * sa + cc * ca; R[1][2] = sc * sb * ca - cc * sa;
+    R[2][0] = -sb;     R[2][1] = cb * sa;                R[2][2] = cb * ca;
+    for (int r = 0; r < 3; ++r) t[r] = x[3 + r];
 }
 
 // 3x3 SVD A = U diag(S) V^T in fp64: one-sided (Hestenes) Jacobi on A directly (no A^T A squaring of the condition

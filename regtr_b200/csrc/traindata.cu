@@ -44,6 +44,18 @@ __global__ void k_align(const double* __restrict__ xyz, const int32_t* __restric
     x32[3 * i + 0] = (float)x; x32[3 * i + 1] = (float)y; x32[3 * i + 2] = (float)z;
 }
 
+// Every point of cloud c moved by pose c in float64 (rt_row, as k_align), rounded once to fp32.
+__global__ void k_transform_clouds(const double* __restrict__ xyz, const int32_t* __restrict__ offs, int C, int n_cap,
+                                   const double* __restrict__ pose, float* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_cap || i >= offs[C]) return;
+    const double* m = pose + 12 * regtr_cloud_of(offs, C, i);
+    const double x = xyz[3 * i + 0], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
+    out[3 * i + 0] = (float)rt_row(m, x, y, z);
+    out[3 * i + 1] = (float)rt_row(m + 4, x, y, z);
+    out[3 * i + 2] = (float)rt_row(m + 8, x, y, z);
+}
+
 // One warp per query, in the cell-sorted order of the stacked set: lanes 0..26 look up one stencil cell each in the
 // PARTNER cloud (src_b <-> tgt_b), candidates are flattened 32 wide, the squared distance is evaluated in float64 on
 // the aligned coordinates ((dx dx + dy dy) + dz dz, no contraction); the nearest support with d2 < r2 wins, equal
@@ -155,6 +167,80 @@ k_registration_fit(const double* __restrict__ xyz, const int32_t* __restrict__ o
     double* o = out + 4 * b + (c < B ? 0 : 2);
     o[0] = n > 0 ? __ddiv_rn((double)k, (double)n) : 0.0;
     o[1] = k > 0 ? __dsqrt_rn(__ddiv_rn(s_sum[0], (double)k)) : 0.0;
+}
+
+// ------------------------------------------------------------------------------------------------- information
+// One CTA per pair: Lambda = sum G^T G over the source points with a match, q the matched target point.  The 21 unique
+// entries of G^T G are ten distinct sums (y^2 + z^2, x^2 + z^2, x^2 + y^2, xy, xz, yz, x, y, z, count); each thread
+// sums its strided points in ascending order, then a fixed shared-memory tree, as in k_registration_fit.  A match
+// outside the target or not strictly within the radius of the moved source point is skipped and raises
+// REGTR_STATUS_INPUT.
+constexpr int INFO_SUMS = 10;
+
+__global__ void __launch_bounds__(FIT_THREADS)
+k_registration_information(const double* __restrict__ xyz, const int32_t* __restrict__ offs, int B,
+                           const double* __restrict__ pose, double r2, const int32_t* __restrict__ nn,
+                           double* __restrict__ out, uint32_t* status) {
+    __shared__ double s_sum[INFO_SUMS][FIT_THREADS];
+    const int b = blockIdx.x, t = threadIdx.x;
+    const double* m = pose + 12 * b;
+    const int a0 = offs[b], a1 = offs[b + 1], p0 = offs[B + b], np_ = offs[B + b + 1] - p0;
+    double acc[INFO_SUMS];
+#pragma unroll
+    for (int k = 0; k < INFO_SUMS; ++k) acc[k] = 0.0;
+    bool bad = false;
+    for (int i = a0 + t; i < a1; i += FIT_THREADS) {
+        const int j = nn[i];
+        if (j < 0) continue;
+        if (j >= np_) { bad = true; continue; }
+        const double* s = xyz + 3 * (size_t)i;
+        const double* q = xyz + 3 * (size_t)(p0 + j);
+        const double x = q[0], y = q[1], z = q[2];
+        const double dx = __dsub_rn(rt_row(m, s[0], s[1], s[2]), x), dy = __dsub_rn(rt_row(m + 4, s[0], s[1], s[2]), y),
+                     dz = __dsub_rn(rt_row(m + 8, s[0], s[1], s[2]), z);
+        const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+        if (!(d2 < r2)) { bad = true; continue; }
+        const double xx = __dmul_rn(x, x), yy = __dmul_rn(y, y), zz = __dmul_rn(z, z);
+        acc[0] = __dadd_rn(acc[0], __dadd_rn(zz, yy));
+        acc[1] = __dadd_rn(acc[1], __dadd_rn(zz, xx));
+        acc[2] = __dadd_rn(acc[2], __dadd_rn(yy, xx));
+        acc[3] = __dadd_rn(acc[3], __dmul_rn(x, y));
+        acc[4] = __dadd_rn(acc[4], __dmul_rn(x, z));
+        acc[5] = __dadd_rn(acc[5], __dmul_rn(y, z));
+        acc[6] = __dadd_rn(acc[6], x);
+        acc[7] = __dadd_rn(acc[7], y);
+        acc[8] = __dadd_rn(acc[8], z);
+        acc[9] = __dadd_rn(acc[9], 1.0);
+    }
+    if (bad) atomicOr(status, REGTR_STATUS_INPUT);
+#pragma unroll
+    for (int k = 0; k < INFO_SUMS; ++k) s_sum[k][t] = acc[k];
+    __syncthreads();
+    for (int h = FIT_THREADS / 2; h > 0; h >>= 1) {
+        if (t < h)
+#pragma unroll
+            for (int k = 0; k < INFO_SUMS; ++k) s_sum[k][t] = __dadd_rn(s_sum[k][t], s_sum[k][t + h]);
+        __syncthreads();
+    }
+    if (t >= 36) return;
+    // G^T G: rows 0-2 the rotation block [[y2+z2, -xy, -xz], [-xy, x2+z2, -yz], [-xz, -yz, x2+y2]], the coupling
+    // [[0, -z, y], [z, 0, -x], [-y, x, 0]] and its transpose, the count on the translation diagonal
+    const int r = t / 6, c = t % 6, lo = r < c ? r : c, hi = r < c ? c : r;
+    double v = 0.0;
+    if (hi < 3) {
+        const int idx[3][3] = {{0, 3, 4}, {3, 1, 5}, {4, 5, 2}};
+        v = s_sum[idx[lo][hi]][0];
+        if (lo != hi) v = -v;
+    } else if (lo < 3) {
+        const int a = lo, k = hi - 3;                // coupling entry (a, 3 + k)
+        if (a != k) {
+            v = s_sum[6 + (3 - a - k)][0];           // the sum of the remaining axis' coordinate
+            if ((a + 1) % 3 == k) v = -v;            // (0,1): -z, (1,2): -x, (2,0): -y; the other order positive
+        }
+    } else if (lo == hi) {
+        v = s_sum[9][0];
+    }
+    out[36 * (size_t)b + t] = v;
 }
 
 // ------------------------------------------------------------------------------------------------- augmentation
@@ -399,6 +485,28 @@ int regtr_registration_fit(const double* xyz, const int32_t* offs, int B, int n_
     if (n_cap > 0 && (!xyz || !nn)) return REGTR_ERR_ARG;
     k_registration_fit<<<2 * B, FIT_THREADS, 0, (cudaStream_t)stream_>>>(xyz, offs, B, pose, radius * radius, nn,
                                                                         out, status);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_registration_information(const double* xyz, const int32_t* offs, int B, int n_cap, const double* pose,
+                                   double radius, const int32_t* nn, double* out, uint32_t* status, void* stream_) {
+    if (!offs || !pose || !out || !status || B <= 0 || 2 * B > 32767 || n_cap < 0 || !(radius > 0.0))
+        return REGTR_ERR_ARG;
+    if (n_cap > 0 && (!xyz || !nn)) return REGTR_ERR_ARG;
+    k_registration_information<<<B, FIT_THREADS, 0, (cudaStream_t)stream_>>>(xyz, offs, B, pose, radius * radius, nn,
+                                                                            out, status);
+    REGTR_CHECK_LAUNCH();
+    return REGTR_OK;
+}
+
+int regtr_transform_clouds(const double* xyz, const int32_t* offs, int C, int n_cap, const double* pose, float* out,
+                           void* stream_) {
+    if (!offs || !pose || C <= 0 || C > 32767 || n_cap < 0) return REGTR_ERR_ARG;
+    if (n_cap == 0) return REGTR_OK;
+    if (!xyz || !out) return REGTR_ERR_ARG;
+    const int T = 256;
+    k_transform_clouds<<<regtr_cdiv(n_cap, T), T, 0, (cudaStream_t)stream_>>>(xyz, offs, C, n_cap, pose, out);
     REGTR_CHECK_LAUNCH();
     return REGTR_OK;
 }

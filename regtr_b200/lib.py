@@ -95,6 +95,11 @@ SIGNATURES = {
     'regtr_overlap_state_bytes': (_Z, [_I]),
     'regtr_overlap_nn': (_I, [_P, _P, _I, _I, _P, _c.c_double, _F, _P, _P, _P, _Z, _P, _Z, _P]),
     'regtr_registration_fit': (_I, [_P, _P, _I, _I, _P, _c.c_double, _P, _P, _P, _P]),
+    'regtr_registration_information': (_I, [_P, _P, _I, _I, _P, _c.c_double, _P, _P, _P, _P]),
+    'regtr_transform_clouds': (_I, [_P, _P, _I, _I, _P, _P, _P]),
+    'regtr_pose_graph_ws_bytes': (_Z, [_I, _I, _I, _c.c_longlong]),
+    'regtr_pose_graph_optimize': (_I, [_P, _P, _I, _I, _I, _I, _c.c_longlong, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                       _P, _Z, _P]),
     'regtr_icp_ws_bytes': (_Z, [_I, _I]),
     'regtr_icp_state_bytes': (_Z, [_I]),
     'regtr_icp': (_I, [_P, _P, _I, _I, _P, _c.c_double, _F, _I, _c.c_double, _c.c_double, _P, _P, _P, _P, _P, _Z,

@@ -1372,6 +1372,141 @@ def estimate_normals(clouds, radius: float, max_nn: int = 30, status=None, retur
     return out
 
 
+def registration_information(src_list, tgt_list, pose, radius: float, status=None):
+    """Fit and information matrices of B registered pairs from one `overlap_nn` (regtr_registration_fit and
+    regtr_registration_information on the same matches): Open3D's evaluate_registration and
+    get_information_matrix_from_point_clouds at `radius`.  Arguments as `registration_fit`.
+    -> (fit (B,4) float64 = fitness_src, rmse_src, fitness_tgt, rmse_tgt; info (B,6,6) float64, info[:,5,5] the match
+    count), both device tensors.  status: as in `registration_fit`."""
+    L = _lib.load()
+    B = len(src_list)
+    dev = pose.device if torch.is_tensor(pose) and pose.is_cuda else None
+    xyz, offs, lens = _stack_pairs(src_list, tgt_list, 'registration_information', dev)
+    dev = xyz.device
+    n = sum(lens)
+    pose64 = torch.as_tensor(pose).to(dev, torch.float64).reshape(B, 3, 4).contiguous()
+    own = status is None
+    if own:
+        status = new_status(dev)
+    nn = overlap_nn(xyz[:n], offs, B, pose64, radius, status)
+    fit = torch.empty((B, 4), dtype=torch.float64, device=dev)
+    info = torch.empty((B, 6, 6), dtype=torch.float64, device=dev)
+    _lib.check(L.regtr_registration_fit(_p(xyz), _p(offs), B, n, _p(pose64), float(radius), _p(nn), _p(fit),
+                                        _p(status), _stream()), 'regtr_registration_fit')
+    _lib.check(L.regtr_registration_information(_p(xyz), _p(offs), B, n, _p(pose64), float(radius), _p(nn), _p(info),
+                                                _p(status), _stream()), 'regtr_registration_information')
+    _count(2)
+    if own:
+        check_fit_status(status, radius, 'registration_information')
+    return fit, info
+
+
+def transform_clouds(clouds, poses):
+    """C clouds (n,3) each moved by one (3,4) or (4,4) pose each, in float64 on the device (regtr_transform_clouds).
+    -> ((n_total,3) float32 device tensor of the stacked moved clouds, offs (C+1) int32)."""
+    L = _lib.load()
+    C = len(clouds)
+    if C == 0:
+        raise ValueError('transform_clouds: expected at least one cloud')
+    dev = torch.device('cuda', torch.cuda.current_device())
+    ts = [torch.as_tensor(c) for c in clouds]
+    lens = [int(c.shape[0]) for c in ts]
+    xyz = torch.empty((max(sum(lens), 1), 3), dtype=torch.float64, device=dev)
+    a = 0
+    for c, ln in zip(ts, lens):
+        xyz[a:a + ln].copy_(c.reshape(ln, 3).to(dev, torch.float64))
+        a += ln
+    offs = make_offsets(lens, dev)
+    n = sum(lens)
+    p = torch.as_tensor(poses).to(dev, torch.float64)[:, :3, :4].contiguous()
+    if p.shape[0] != C:
+        raise ValueError(f'transform_clouds: {p.shape[0]} poses for {C} clouds')
+    out = torch.empty((max(n, 1), 3), dtype=torch.float32, device=dev)
+    _lib.check(L.regtr_transform_clouds(_p(xyz), _p(offs), C, n, _p(p), _p(out), _stream()), 'regtr_transform_clouds')
+    _count(1 if n > 0 else 0)
+    return out[:n], offs
+
+
+class PoseGraphOptions(ctypes.Structure):
+    """regtr_pose_graph_options."""
+    _fields_ = [('max_correspondence_distance', ctypes.c_double), ('edge_prune_threshold', ctypes.c_double),
+                ('preference_loop_closure', ctypes.c_double), ('min_relative_increment', ctypes.c_double),
+                ('min_relative_residual_increment', ctypes.c_double), ('min_right_term', ctypes.c_double),
+                ('min_residual', ctypes.c_double), ('upper_scale_factor', ctypes.c_double),
+                ('lower_scale_factor', ctypes.c_double), ('reference_node', ctypes.c_int32),
+                ('max_iteration', ctypes.c_int32), ('max_iteration_lm', ctypes.c_int32)]
+
+
+POSE_GRAPH_MAX_NODES = 256                                                  # REGTR_POSE_GRAPH_MAX_NODES
+
+
+def pose_graph_optimize(poses, edges, transformation, information, uncertain, max_correspondence_distance: float,
+                        edge_prune_threshold: float = 0.25, preference_loop_closure: float = 1.0,
+                        reference_node: int = 0, max_iteration: int = 100, max_iteration_lm: int = 20,
+                        min_relative_increment: float = 1e-6, min_relative_residual_increment: float = 1e-6,
+                        min_right_term: float = 1e-6, min_residual: float = 1e-6,
+                        upper_scale_factor: float = 2.0 / 3.0, lower_scale_factor: float = 1.0 / 3.0, status=None):
+    """Robust optimisation of G pose graphs in one launch (regtr_pose_graph_optimize: Open3D's global_optimization with
+    GlobalOptimizationLevenbergMarquardt and its two passes).  Lists of G entries each: poses (N_g,3,4) or (N_g,4,4)
+    fragment -> world initial poses; edges (E_g,2) int (source, target) node indices; transformation (E_g,3,4) or
+    (E_g,4,4) source -> target; information (E_g,6,6); uncertain (E_g,) bool (loop closures).
+    -> (poses list of (N_g,3,4) float64, confidence list of (E_g,) float64, kept list of (E_g,) bool,
+    result (G,4) float64 = pass-1 iterations, pass-2 iterations, final objective, edges kept), all device tensors.
+    A graph above POSE_GRAPH_MAX_NODES nodes raises RegtrLibError (REGTR_ERR_UNSUPPORTED).  No host sync unless status
+    is None: then a word of this call is read and a rejected graph (s = t, an index out of range, a non-finite input)
+    raises RegtrLibError; with the caller's word the caller checks REGTR_STATUS_INPUT (`STATUS_INPUT`)."""
+    L = _lib.load()
+    G = len(poses)
+    if G == 0 or not (len(edges) == len(transformation) == len(information) == len(uncertain) == G):
+        raise ValueError('pose_graph_optimize: expected G >= 1 graphs with poses, edges, transformation, information '
+                         'and uncertain each')
+    dev = torch.device('cuda', torch.cuda.current_device())
+
+    def cat(items, tail, dtype):
+        ts = [torch.as_tensor(x).to(dev, dtype) for x in items]
+        ts = [t.reshape((-1,) + t.shape[-len(tail):] if tail else (-1,)) for t in ts]
+        ts = [t[(slice(None),) + tuple(slice(0, k) for k in tail)] for t in ts]       # (4,4) -> its (3,4) rows
+        return torch.cat(ts).contiguous()
+
+    n_nodes = [int(torch.as_tensor(p).shape[0]) for p in poses]
+    n_edges = [int(torch.as_tensor(e).reshape(-1, 2).shape[0]) for e in edges]
+    P = cat(poses, (3, 4), torch.float64)
+    Ed = cat(edges, (2,), torch.int32)
+    X = cat(transformation, (3, 4), torch.float64)
+    I6 = cat(information, (6, 6), torch.float64)
+    U = cat([torch.as_tensor(u).bool() for u in uncertain], (), torch.uint8)
+    for name, t, want in (('transformation', X, n_edges), ('information', I6, n_edges), ('uncertain', U, n_edges)):
+        if t.shape[0] != sum(want):
+            raise ValueError(f'pose_graph_optimize: {name} has {t.shape[0]} rows for {sum(want)} edges')
+    N, E = sum(n_nodes), sum(n_edges)
+    max_nodes = max(n_nodes)
+    node_offs, edge_offs = make_offsets(n_nodes, dev), make_offsets(n_edges, dev)
+    opt = PoseGraphOptions(float(max_correspondence_distance), float(edge_prune_threshold),
+                           float(preference_loop_closure), float(min_relative_increment),
+                           float(min_relative_residual_increment), float(min_right_term), float(min_residual),
+                           float(upper_scale_factor), float(lower_scale_factor), int(reference_node),
+                           int(max_iteration), int(max_iteration_lm))
+    conf = torch.empty(max(E, 1), dtype=torch.float64, device=dev)
+    kept = torch.empty(max(E, 1), dtype=torch.uint8, device=dev)
+    result = torch.empty((G, 4), dtype=torch.float64, device=dev)
+    P = P if N > 0 else torch.empty((1, 3, 4), dtype=torch.float64, device=dev)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    sq_nodes = sum(k * k for k in n_nodes) if max_nodes <= POSE_GRAPH_MAX_NODES else 0
+    ws = workspace(max(L.regtr_pose_graph_ws_bytes(G, N, E, sq_nodes), 1), dev)
+    _lib.check(L.regtr_pose_graph_optimize(_p(node_offs), _p(edge_offs), G, N, E, max_nodes, sq_nodes, _p(P), _p(Ed),
+                                           _p(X), _p(I6), _p(U), ctypes.byref(opt), _p(conf), _p(kept), _p(result),
+                                           _p(status), _p(ws), ws.numel(), _stream()), 'regtr_pose_graph_optimize')
+    _count(1)
+    if own and int(status.item()) & STATUS_INPUT:
+        raise _lib.RegtrLibError('pose_graph_optimize: a graph was rejected (s = t, a node index or the reference node '
+                                 'out of range, or a non-finite pose, transformation or information)')
+    nb, eb = np.concatenate([[0], np.cumsum(n_nodes)]), np.concatenate([[0], np.cumsum(n_edges)])
+    return ([P[nb[k]:nb[k + 1]] for k in range(G)], [conf[eb[k]:eb[k + 1]] for k in range(G)],
+            [kept[eb[k]:eb[k + 1]].bool() for k in range(G)], result)
+
+
 def check_fit_status(status, radius: float, what: str = 'registration_fit'):
     """Read the status word of `registration_fit` or `icp` (a host sync) and raise RegtrLibError if the result is not
     exact."""

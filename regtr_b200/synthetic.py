@@ -110,6 +110,40 @@ def make_3dmatch_pair(seed: int, n_target: int = 20000, overlap=(0.3, 0.6), voxe
                 pose=pose.astype(np.float32))
 
 
+def make_scene(seed: int, n_fragments: int, n_target: int = 20000, window: int = 4, voxel=0.025, noise=0.006):
+    """One synthetic room scanned along a camera path: `n_fragments` crops, each a slab of the room that overlaps the
+    next `window - 1` crops (overlap 1 - k / window with crop i + k), voxel-averaged at `voxel`, permuted, and put in
+    its own random local frame.  -> dict(fragments: list of (n,3) float32 in their local frames, poses (N,4,4) float64
+    fragment -> world)."""
+    rng = np.random.default_rng(seed)
+    span = max(1.0, (n_fragments + window - 1) / window)     # room length in crop widths
+    extent = np.array([3.0 * span, 2.3, 2.7])
+    patches = _room_surfaces(rng, extent, int(rng.integers(5, 9) * span), int(rng.integers(3, 7) * span))
+    frac = window / (n_fragments + window - 1)
+    area = sum(np.linalg.norm(np.cross(u, v)) for _, u, v in patches)
+    s = np.sqrt(n_target / (_PTS_PER_M2 * frac * area))
+    patches = [(o * s, u * s, v * s) for o, u, v in patches]
+    scene = _sample_patches(rng, patches, density=16000.0)
+    scene = scene + rng.normal(scale=noise, size=scene.shape)
+    d = np.array([1.0, rng.normal(scale=0.1), rng.normal(scale=0.05)])
+    d /= np.linalg.norm(d)
+    proj = scene @ d
+    lo, hi = proj.min(), proj.max()
+    step = (hi - lo) / (n_fragments + window - 1)
+    fragments, poses = [], []
+    for k in range(n_fragments):
+        c = scene[(proj >= lo + k * step) & (proj <= lo + (k + window) * step)]
+        c = _voxel_average(c, voxel)
+        c = c[rng.permutation(len(c))]
+        R = random_rotation(rng, 180.0)
+        t = c.mean(0) + rng.uniform(-0.5, 0.5, 3)
+        pose = np.eye(4)
+        pose[:3, :3], pose[:3, 3] = R, t
+        fragments.append(((c - t) @ R).astype(np.float32))              # local = R^T (world - t)
+        poses.append(pose)
+    return dict(fragments=fragments, poses=np.stack(poses))
+
+
 def make_modelnet_pair(seed: int, n_points: int = 1024, keep: float = 0.7):
     """One ModelNet-like pair: a union of ellipsoid / box surfaces in the unit cube,
     each cloud cropped to `keep` by a random half-space (conf/modelnet.yaml:16-19)."""
