@@ -557,7 +557,8 @@ int regtr_transform_clouds(const double* xyz, const int32_t* offs, int C, int n_
                            void* stream);
 
 /* ICP of B pairs (Open3D's registration_icp with TransformationEstimationPointToPoint, no scaling, or with
- * TransformationEstimationPointToPlane, and ICPConvergenceCriteria(rel_fitness, rel_rmse, max_iter)).
+ * TransformationEstimationPointToPlane, or registration_generalized_icp, and ICPConvergenceCriteria(rel_fitness,
+ * rel_rmse, max_iter)).
  * xyz (n_cap,3) float64 stacked src_0..src_{B-1},
  * tgt_0..tgt_{B-1} with offs (2B+1) i32; init (B,3,4) float64 source -> target.  Per pair: P = init . source
  * (((r0 x + r1 y) + r2 z) + t, no contraction), T = init; correspondences are regtr_overlap_nn's (the nearest target
@@ -576,13 +577,36 @@ int regtr_transform_clouds(const double* xyz, const int32_t* offs, int C, int n_
  * (21 unique entries) and J^T r summed per chunk in the fixed order; per pair J^T J x = -J^T r solved by LDL^T in
  * float64; the update is the identity when k = 0, |det J^T J| < 1e-6 or det is not finite (Open3D's
  * SolveLinearSystemPSD), else R = Rz(x2) Ry(x1) Rx(x0), t = (x3, x4, x5) (TransformVector6dToMatrix4d).  A zero
- * normal drops its correspondence out of the update, not out of k.  Same launches as point-to-point. */
+ * normal drops its correspondence out of the update, not out of k.  Same launches as point-to-point.
+ * src_normals NULL with opt NULL: the above, unchanged.  src_normals non-NULL (needs tgt_normals): generalized ICP
+ * (Open3D's registration_generalized_icp with TransformationEstimationForGeneralizedICP(epsilon, kernel)),
+ * (offs[B], 3) float64 stacked like the sources; every round they are rotated with the sources (first by init, then
+ * by each update) in a workspace copy.  Per correspondence (a moved source normal, b target normal, c = 1 - epsilon)
+ * M = (I - c a a^T) + (I - c b b^T) (a zero normal gives I), (U, S, V) its float64 Jacobi SVD,
+ * W = V diag(1 / sqrt(S)) V^T; the rows w_i of W give r_i = w_i . (p - q), J_i = [p x w_i ; w_i], each into J^T J and
+ * J^T r with weight loss(r_i); a correspondence whose M has an eigenvalue that is not > 0 or not finite leaves the
+ * update, not k.  opt (host memory, nullable: L2 and epsilon 1e-3): a loss other than REGTR_ICP_LOSS_L2 weights every
+ * residual row of point-to-plane (r = (p - q) . n) or generalized ICP by Open3D's RobustKernel::Weight(r):
+ * huber 1 if |r| <= k else k / |r|; cauchy 1 / (1 + (r/k)^2); gm k / (k + r^2)^2; tukey (1 - (r/k)^2)^2 if |r| <= k
+ * else 0.  REGTR_ERR_ARG: src_normals without tgt_normals, a loss other than L2 without tgt_normals, an unknown loss,
+ * loss_k not > 0 or not finite with a loss other than L2, epsilon outside (0, 1].  Same launches in every mode. */
+#define REGTR_ICP_LOSS_L2 0
+#define REGTR_ICP_LOSS_HUBER 1
+#define REGTR_ICP_LOSS_CAUCHY 2
+#define REGTR_ICP_LOSS_GM 3
+#define REGTR_ICP_LOSS_TUKEY 4
+typedef struct {
+    int loss;                                /* REGTR_ICP_LOSS_* [L2] */
+    double loss_k;                           /* the loss's parameter k, > 0 (ignored by L2) */
+    double epsilon;                          /* generalized ICP's covariance epsilon, 0 < epsilon <= 1 [1e-3] */
+} regtr_icp_options;
+
 size_t regtr_icp_ws_bytes(int n_cap, int B);
 size_t regtr_icp_state_bytes(int n_cap);
 int regtr_icp(const double* xyz, const int32_t* offs, int B, int n_cap, const double* init, double max_dist,
               float cell, int max_iter, double rel_fitness, double rel_rmse, const double* tgt_normals,
-              double* pose_out, double* result, uint32_t* status, void* ws, size_t ws_bytes, void* state,
-              size_t state_bytes, void* stream);
+              const double* src_normals, const regtr_icp_options* opt, double* pose_out, double* result,
+              uint32_t* status, void* ws, size_t ws_bytes, void* state, size_t state_bytes, void* stream);
 
 /* Normals of C stacked clouds (Open3D's estimate_normals(KDTreeSearchParamHybrid(radius, max_nn)) followed by
  * orient_normals_towards_camera_location() at the origin, with this library's tie and boundary rules).

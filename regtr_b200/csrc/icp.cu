@@ -1,13 +1,17 @@
 // ICP of B pairs at once: Open3D's registration_icp with TransformationEstimationPointToPoint (no scaling) or
 // TransformationEstimationPointToPlane, and ICPConvergenceCriteria, restated with this library's determinism rules
 // (DESIGN.md section 8, "ICP").  The method is a template argument of the reduction and the update kernels, so the
-// point-to-point instantiation is the same code as without the point-to-plane method.
+// point-to-point instantiation is the same code as without the point-to-plane method.  Generalized ICP and robust
+// point-to-plane swap the reduction for gicp.cu's and keep everything else.
 //
 // Stacked clouds as in the registration fit: src_0..src_{B-1}, tgt_0..tgt_{B-1} (float64) with int32 device offsets.
 // One cell list over the targets is built once; then every round is a fixed sequence of three launches (nearest
 // neighbours, per-chunk sums, per-pair update) enqueued without a host synchronisation.  A pair that has converged
 // reads its `done` flag on the device and skips its work, so the launch count depends on max_iter alone.
+#include <cfloat>
+
 #include "cellgrid.cuh"
+#include "icp.cuh"
 #include "rigid.cuh"
 
 extern "C" int regtr_cellgrid_build(const float* xyz, const int32_t* offs, int n_clouds, int n_cap, float cell,
@@ -20,20 +24,11 @@ extern "C" double regtr_overlap_coord_bound(double radius, float cell);
 
 namespace {
 
-constexpr int NN_WARPS = 8;
-constexpr int CHUNK = 1024;            // source points per CTA of the reduction
-constexpr int RED_THREADS = 256;
-constexpr int RED_WARPS = RED_THREADS / 32;
-constexpr int PART = 17;               // k, sum d2, mean_src[3], mean_tgt[3], C[9] per chunk
-constexpr int PART_PLANE = 29;         // k, sum d2, J^T J[21] (upper triangle, row-major), J^T r[6] per chunk
-constexpr int UPD_THREADS = 64;
+using namespace icp_shared;
 
-// Per-pair state between rounds (written by k_icp_update only).
-struct IcpPair {
-    double upd[12];                    // the update of the last round, applied to P by the next k_icp_nn
-    double fit, rmse;                  // the current correspondences' fitness and inlier RMSE
-    int k, iters, done, pad;
-};
+constexpr int NN_WARPS = 8;
+constexpr int PART = 17;               // k, sum d2, mean_src[3], mean_tgt[3], C[9] per chunk
+constexpr int UPD_THREADS = 64;
 
 // P = init . source (rt_row order), the fp32 copy of the targets for their cell list, the targets' own offsets
 // (tofs[c] = offs[B + c] - offs[B]), the chunk prefix of the reduction (pair b owns chunks [cpre[b], cpre[b+1]),
@@ -143,19 +138,6 @@ k_icp_nn(const double* __restrict__ xyz, const int32_t* __restrict__ offs, int B
         }
         if (lane == 0) { nn[qi] = bi; d2o[qi] = best; }
     }
-}
-
-// Sum over the CTA in a fixed order: the xor butterfly inside each warp, then the warp totals in warp order.  Every
-// thread returns the total.
-__device__ __forceinline__ double block_sum(double v, double* s_warp) {
-    v = warp_sum(v);
-    __syncthreads();                   // s_warp may still be read by the previous call
-    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double t = 0.0;
-#pragma unroll
-    for (int w = 0; w < RED_WARPS; ++w) t += s_warp[w];
-    return t;
 }
 
 // One CTA per chunk of CHUNK consecutive source points of one pair (chunks never straddle pairs, so the sums do not
@@ -412,7 +394,7 @@ k_icp_update(const int32_t* __restrict__ offs, int B, const int32_t* __restrict_
 }
 
 struct IcpWs {
-    double *P, *d2, *part;
+    double *P, *d2, *part, *snrm;
     float* x32;
     int32_t *tofs, *cpre, *nn;
     IcpPair* pst;
@@ -439,6 +421,7 @@ IcpWs carve_icp(void* ws, int n_cap, int B) {
     w.grid = take(regtr_cellgrid_bytes(n_cap));
     w.gws_bytes = regtr_cellgrid_ws_bytes(n_cap);
     w.gws = take(w.gws_bytes);
+    w.snrm = (double*)take(sizeof(double) * 3 * n);                  // generalized ICP's moved source normals
     w.total = off;
     return w;
 }
@@ -454,13 +437,19 @@ size_t regtr_icp_state_bytes(int n_cap) { return regtr_cellgrid_state_bytes(n_ca
 
 int regtr_icp(const double* xyz, const int32_t* offs, int B, int n_cap, const double* init, double max_dist,
               float cell, int max_iter, double rel_fitness, double rel_rmse, const double* tgt_normals,
-              double* pose_out, double* result, uint32_t* status, void* ws, size_t ws_bytes, void* state,
-              size_t state_bytes, void* stream_) {
+              const double* src_normals, const regtr_icp_options* opt, double* pose_out, double* result,
+              uint32_t* status, void* ws, size_t ws_bytes, void* state, size_t state_bytes, void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (!offs || !init || !pose_out || !result || !status || !ws || !state || B <= 0 || 2 * B > 32767 || n_cap < 0 ||
         !(max_dist > 0.0) || !((double)cell > max_dist) || max_iter < 0 || !(rel_fitness >= 0.0) ||
         !(rel_rmse >= 0.0) || (n_cap > 0 && !xyz))
         return REGTR_ERR_ARG;
+    const regtr_icp_options o = opt ? *opt : regtr_icp_options{REGTR_ICP_LOSS_L2, 1.0, 1e-3};
+    if (o.loss < REGTR_ICP_LOSS_L2 || o.loss > REGTR_ICP_LOSS_TUKEY || !(o.epsilon > 0.0 && o.epsilon <= 1.0) ||
+        (o.loss != REGTR_ICP_LOSS_L2 && !(o.loss_k > 0.0 && o.loss_k <= DBL_MAX)) ||
+        ((src_normals || o.loss != REGTR_ICP_LOSS_L2) && !tgt_normals))
+        return REGTR_ERR_ARG;
+    const bool robust = src_normals || o.loss != REGTR_ICP_LOSS_L2;   // gicp.cu's reduction
     const int nc = n_cap > 0 ? n_cap : 1;      // offs[2B] = 0 without points: every kernel then reads no xyz
     IcpWs w = carve_icp(ws, nc, B);
     if (ws_bytes < w.total || state_bytes < regtr_icp_state_bytes(n_cap)) return REGTR_ERR_WORKSPACE;
@@ -481,7 +470,14 @@ int regtr_icp(const double* xyz, const int32_t* offs, int B, int n_cap, const do
         k_icp_nn<<<nn_blocks, NN_WARPS * 32, 0, st>>>(xyz, offs, B, nc, w.P, w.pst, round > 0, table, log2t, sxyzi,
                                                       cell, max_dist * max_dist, bound, w.nn, w.d2, status);
         REGTR_CHECK_LAUNCH();
-        if (tgt_normals) {
+        if (robust) {
+            const int rc2 = icp_robust_reduce(src_normals != nullptr, n_chunks_cap(nc, B), st, xyz, offs, B, w.cpre,
+                                              w.P, w.nn, w.d2, w.pst, w.part, tgt_normals, src_normals, w.snrm, init,
+                                              round, o.loss, o.loss_k, o.epsilon);
+            if (rc2 != REGTR_OK) return rc2;
+            k_icp_update<true><<<regtr_cdiv(B, UPD_THREADS), UPD_THREADS, 0, st>>>(
+                offs, B, w.cpre, w.part, w.pst, round, max_iter, rel_fitness, rel_rmse, pose_out, result);
+        } else if (tgt_normals) {
             k_icp_reduce<true><<<n_chunks_cap(nc, B), RED_THREADS, 0, st>>>(xyz, offs, B, w.cpre, w.P, w.nn, w.d2,
                                                                             w.pst, w.part, tgt_normals);
             REGTR_CHECK_LAUNCH();

@@ -1,5 +1,5 @@
 // Internal to the library: float64 rigid-transform helpers shared by the pose solve (kabsch.cu), the training-data
-// preparation (traindata.cu), ICP (icp.cu) and the pose-graph optimiser (posegraph.cu).
+// preparation (traindata.cu), ICP (icp.cu, gicp.cu) and the pose-graph optimiser (posegraph.cu).
 #pragma once
 
 #include "common.cuh"
@@ -24,12 +24,9 @@ __device__ __forceinline__ void rigid_from_vec6(const double x[6], double R[3][3
     for (int r = 0; r < 3; ++r) t[r] = x[3 + r];
 }
 
-// 3x3 SVD A = U diag(S) V^T in fp64: one-sided (Hestenes) Jacobi on A directly (no A^T A squaring of the condition
-// number); singular values sorted descending, so that a reflection fix flips the direction of the smallest one.
-__device__ void svd3_jacobi(const double A_in[3][3], double U[3][3], double S[3], double V[3][3]) {
-    double A[3][3];
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) { A[i][j] = A_in[i][j]; V[i][j] = (i == j) ? 1.0 : 0.0; }
+// The sweeps of svd3_jacobi: one-sided (Hestenes) Jacobi rotations of A's column pairs, accumulated in V, until the
+// columns of A (now A_in V) are orthogonal; column j's norm is then the singular value of V's column j (unsorted).
+__device__ __forceinline__ void jacobi3_sweeps(double A[3][3], double V[3][3]) {
     for (int sweep = 0; sweep < 30; ++sweep) {
         double off = 0.0;
         for (int p = 0; p < 2; ++p) {
@@ -59,6 +56,15 @@ __device__ void svd3_jacobi(const double A_in[3][3], double U[3][3], double S[3]
         }
         if (off < 1e-15) break;
     }
+}
+
+// 3x3 SVD A = U diag(S) V^T in fp64: one-sided (Hestenes) Jacobi on A directly (no A^T A squaring of the condition
+// number); singular values sorted descending, so that a reflection fix flips the direction of the smallest one.
+__device__ void svd3_jacobi(const double A_in[3][3], double U[3][3], double S[3], double V[3][3]) {
+    double A[3][3];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) { A[i][j] = A_in[i][j]; V[i][j] = (i == j) ? 1.0 : 0.0; }
+    jacobi3_sweeps(A, V);
     for (int j = 0; j < 3; ++j) S[j] = sqrt(A[0][j] * A[0][j] + A[1][j] * A[1][j] + A[2][j] * A[2][j]);
     // sort columns by descending singular value
     int ord[3] = {0, 1, 2};

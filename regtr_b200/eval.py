@@ -377,7 +377,8 @@ def summarize_modelnet_metrics(metrics: Dict[str, np.ndarray]) -> Dict[str, floa
 
 
 def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None, method: str = 'point_to_point',
-                normal_radius: float = None, normal_max_nn: int = 30, estimate_normals=None):
+                normal_radius: float = None, normal_max_nn: int = 30, estimate_normals=None, epsilon: float = 1e-3,
+                loss: str = 'l2', loss_k: float = None):
     """Wrap `forward_fn(batch) -> pred` so that the final pose of every pair is refined by ICP on the batch's full
     clouds: -> a NEW dict with pred's entries, pose (1,B,3,4) float64 the refined poses and pose_coarse
     (1,B,3,4) float64 the network's final poses (so that `compute_metrics` reports both, and EstLogWriter writes the
@@ -385,23 +386,37 @@ def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None, me
     icp(src_list, tgt_list, init (B,3,4), radius, max_iteration) -> (pose (B,3,4), result): default `ops.icp`,
     point-to-point.  method='point_to_plane': the targets' normals come from
     estimate_normals(tgt_list, normal_radius (default 2 * radius), normal_max_nn) (default `ops.estimate_normals`) and
-    icp is called as icp(src_list, tgt_list, init, radius, max_iteration, method=method, tgt_normals=normals)."""
-    if method not in ('point_to_point', 'point_to_plane'):
+    icp is called as icp(src_list, tgt_list, init, radius, max_iteration, method=method, tgt_normals=normals).
+    method='generalized': the normals of src_list + tgt_list come from one estimate_normals call, and icp also gets
+    src_normals=.  epsilon, loss and loss_k (see `ops.icp`) are passed on only when they differ from their defaults."""
+    if method not in ('point_to_point', 'point_to_plane', 'generalized'):
         raise ValueError(f'icp_forward: unknown method {method!r}')
     if icp is None:
         from .ops import icp
-    if method == 'point_to_plane' and estimate_normals is None:
+    if method != 'point_to_point' and estimate_normals is None:
         from .ops import estimate_normals
     nr = 2.0 * radius if normal_radius is None else normal_radius
+    extra = {}
+    if epsilon != 1e-3:
+        extra['epsilon'] = epsilon
+    if loss != 'l2':
+        extra['loss'] = loss
+    if loss_k is not None:
+        extra['loss_k'] = loss_k
     def run(batch):
         pred = forward_fn(batch)
         coarse = pred['pose'][-1].to(torch.float64)                     # (B,3,4), a new tensor
         if method == 'point_to_point':
-            pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration)
-        else:
+            pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, **extra)
+        elif method == 'point_to_plane':
             normals = estimate_normals(batch['tgt_xyz'], nr, normal_max_nn)
             pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, method=method,
-                          tgt_normals=normals)
+                          tgt_normals=normals, **extra)
+        else:
+            B = len(batch['src_xyz'])
+            normals = estimate_normals(list(batch['src_xyz']) + list(batch['tgt_xyz']), nr, normal_max_nn)
+            pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, method=method,
+                          tgt_normals=normals[B:], src_normals=normals[:B], **extra)
         out = dict(pred)
         out['pose'] = torch.as_tensor(pose, dtype=torch.float64, device=coarse.device).reshape(coarse.shape)[None]
         out['pose_coarse'] = coarse[None]

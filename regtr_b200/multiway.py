@@ -2,14 +2,16 @@
 registration after RegTR's pairwise poses).
 
     python -m regtr_b200.multiway FRAG_0 FRAG_1 ... --ckpt <logdir>/ckpt/model-best.pth [--config <yaml>] --out DIR
-        [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane [--normal_radius NR]
-         [--normal_max_nn 30]]] [--info_radius D] [--min_overlap 0.3] [--preference_loop_closure 1.0]
+        [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized [--normal_radius NR]
+         [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
+        [--info_radius D] [--min_overlap 0.3] [--preference_loop_closure 1.0]
         [--voxel V] [--batch_pairs 8]
 
 Fragments are given in sequence order, in any format `pointio` reads; fragment index = position in the list (3DMatch
 scenes are numbered cloud_bin_0..N-1, so position is the benchmark index).  The config is found and the clouds are
 cropped as `register` does.  Every pair i < j is registered with source j and target i (the 3DMatch benchmark's
-direction) in eager forwards of --batch_pairs pairs, then refined by `ops.icp` with --icp as `register --icp` does.
+direction) in eager forwards of --batch_pairs pairs, then refined by `ops.icp` with --icp as `register --icp` does
+(generalized ICP uses each fragment's normals as source and as target normals).
 `ops.registration_information` at D (default: the config's overlap_radius) gives each pair its fit and information
 matrix.  Edge (source j, target i, X = the pair's pose): j = i + 1 is a certain odometry edge; any other pair is an
 uncertain loop-closure edge when Lambda[5,5] / min(n_j, n_i) >= --min_overlap (Open3D's reconstruction system's gate).
@@ -46,11 +48,16 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument('--out', required=True, help='Output directory')
     ap.add_argument('--icp', type=float, metavar='R', help='Refine every pair by ICP, max correspondence distance R')
     ap.add_argument('--icp_iters', type=int, default=30, help='ICP iterations at most (with --icp)')
-    ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane'), default='point_to_point',
-                    help='ICP error metric (with --icp)')
+    ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane', 'generalized'),
+                    default='point_to_point', help='ICP error metric (with --icp)')
     ap.add_argument('--normal_radius', type=float, metavar='NR',
-                    help='Normal estimation radius of point_to_plane ICP (default: 2 * the --icp radius)')
+                    help='Normal estimation radius of point_to_plane / generalized ICP (default: 2 * the --icp radius)')
     ap.add_argument('--normal_max_nn', type=int, default=30, help='Neighbours at most of the normal estimation')
+    ap.add_argument('--icp_epsilon', type=float, default=1e-3,
+                    help='Covariance epsilon of generalized ICP, in (0, 1]')
+    ap.add_argument('--icp_loss', choices=('l2', 'huber', 'cauchy', 'gm', 'tukey'), default='l2',
+                    help='Robust kernel of point_to_plane / generalized ICP (needs --icp_loss_k unless l2)')
+    ap.add_argument('--icp_loss_k', type=float, metavar='K', help='The robust kernel\'s parameter k')
     ap.add_argument('--info_radius', type=float, metavar='D',
                     help='Radius of the information matrices and the line process (default: overlap_radius)')
     ap.add_argument('--min_overlap', type=float, default=0.3,
@@ -68,15 +75,18 @@ def all_pairs(n: int):
 
 def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8, icp_radius: float = None,
                    icp_iters: int = 30, icp_method: str = 'point_to_point', normal_radius: float = None,
-                   normal_max_nn: int = 30) -> np.ndarray:
-    """RegTR's final-layer pose of every pair (i, j) of `all_pairs`, source j -> target i, optionally refined by ICP.
+                   normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
+                   icp_loss_k: float = None) -> np.ndarray:
+    """RegTR's final-layer pose of every pair (i, j) of `all_pairs`, source j -> target i, optionally refined by ICP
+    (`ops.icp` with icp_method, epsilon=icp_epsilon, loss=icp_loss, loss_k=icp_loss_k; the point-to-plane and
+    generalized methods use every fragment's normals, estimated once).
     fragments: (n,3) float64 host arrays (already cropped).  -> (P,3,4) float64."""
     from . import ops
     dev = model.device
     pairs = all_pairs(len(fragments))
     dev_frags = [torch.from_numpy(np.ascontiguousarray(f)).float().to(dev) for f in fragments]
     normals = None
-    if icp_radius is not None and icp_method == 'point_to_plane':
+    if icp_radius is not None and icp_method != 'point_to_point':
         nr = 2.0 * icp_radius if normal_radius is None else normal_radius
         normals = ops.estimate_normals(fragments, nr, normal_max_nn)
     out = []
@@ -88,7 +98,9 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
             if icp_radius is not None:
                 pose, _ = ops.icp([fragments[j] for _, j in chunk], [fragments[i] for i, _ in chunk], pose, icp_radius,
                                   icp_iters, method=icp_method,
-                                  tgt_normals=None if normals is None else [normals[i] for i, _ in chunk])
+                                  tgt_normals=None if normals is None else [normals[i] for i, _ in chunk],
+                                  src_normals=None if normals is None else [normals[j] for _, j in chunk],
+                                  epsilon=icp_epsilon, loss=icp_loss, loss_k=icp_loss_k)
             out.append(pose.cpu().numpy())
     return np.concatenate(out, 0)
 
@@ -198,7 +210,7 @@ def main(argv=None):
     model = load_model(cfg, opt.ckpt)
     frags = [crop(cfg, np.asarray(load_point_cloud(f), dtype=np.float64)) for f in opt.fragments]
     T = register_pairs(model, frags, opt.batch_pairs, opt.icp, opt.icp_iters, opt.icp_method, opt.normal_radius,
-                       opt.normal_max_nn)
+                       opt.normal_max_nn, opt.icp_epsilon, opt.icp_loss, opt.icp_loss_k)
     D = float(cfg['overlap_radius'] if opt.info_radius is None else opt.info_radius)
     res = optimize_scene(frags, T, D, opt.min_overlap, opt.preference_loop_closure)
     write_outputs(res, opt.out, scene_name(opt.fragments[0]), frags, opt.voxel)

@@ -1253,18 +1253,44 @@ def icp_launches(max_iteration: int) -> int:
     return 5 + 3 * (int(max_iteration) + 1)
 
 
-ICP_METHODS = ('point_to_point', 'point_to_plane')
+ICP_METHODS = ('point_to_point', 'point_to_plane', 'generalized')
+ICP_LOSSES = ('l2', 'huber', 'cauchy', 'gm', 'tukey')      # REGTR_ICP_LOSS_L2 .. REGTR_ICP_LOSS_TUKEY
+
+
+class IcpOptions(ctypes.Structure):
+    """regtr_icp_options (include/regtr_b200.h)."""
+    _fields_ = [('loss', ctypes.c_int), ('loss_k', ctypes.c_double), ('epsilon', ctypes.c_double)]
+
+
+def _stack_normals(normals, lens, what, dev):
+    """B (n,3) normal arrays aligned with clouds of `lens` points -> one (max(sum, 1), 3) float64 device tensor."""
+    if len(normals) != len(lens):
+        raise ValueError(f'icp: {len(normals)} {what} normal arrays for {len(lens)} pairs')
+    out = torch.empty((max(sum(lens), 1), 3), dtype=torch.float64, device=dev)
+    a = 0
+    for c, ln in zip(normals, lens):
+        c = torch.as_tensor(c)
+        if tuple(c.shape) != (ln, 3):
+            raise ValueError(f'icp: {what} normals {tuple(c.shape)} for a {what} of {ln} points')
+        out[a:a + ln].copy_(c.to(dev, torch.float64))
+        a += ln
+    return out
 
 
 def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iteration: int = 30,
         relative_fitness: float = 1e-6, relative_rmse: float = 1e-6, status=None, method: str = 'point_to_point',
-        tgt_normals=None):
+        tgt_normals=None, src_normals=None, epsilon: float = 1e-3, loss: str = 'l2', loss_k: float = None):
     """ICP of B pairs (regtr_icp): Open3D's registration_icp with TransformationEstimationPointToPoint (no scaling) or,
-    with method='point_to_plane', TransformationEstimationPointToPlane, and ICPConvergenceCriteria(relative_fitness,
-    relative_rmse, max_iteration), on the device.
+    with method='point_to_plane', TransformationEstimationPointToPlane, or with method='generalized',
+    registration_generalized_icp with TransformationEstimationForGeneralizedICP(epsilon), and
+    ICPConvergenceCriteria(relative_fitness, relative_rmse, max_iteration), on the device.
     src_list / tgt_list: B clouds (n,3) each (numpy or torch, any float dtype; stacked in float64 on the device);
-    init (B,3,4) source -> target.  tgt_normals: with 'point_to_plane', B (n,3) normals aligned with tgt_list (e.g.
-    `estimate_normals(tgt_list, ...)`); a zero normal drops its correspondence out of the update.
+    init (B,3,4) source -> target.  tgt_normals: with 'point_to_plane' and 'generalized', B (n,3) normals aligned with
+    tgt_list (e.g. `estimate_normals(tgt_list, ...)`); a zero normal drops its correspondence out of the point-to-plane
+    update.  src_normals: with 'generalized', B (n,3) normals aligned with src_list (a zero normal gives the identity
+    covariance); epsilon in (0, 1] the covariances' epsilon.  loss: one of ICP_LOSSES, Open3D's robust kernel of the
+    point-to-plane and generalized estimations, with loss_k its parameter k > 0 ('l2', the default, takes none; the
+    point-to-point estimation has no kernel).
     -> (pose (B,3,4) float64, result (B,4) float64 = fitness, inlier_rmse, n_corr, iterations), both device tensors.
     No host sync unless status is None: then a word of this call is read and a coordinate of a moved source or of a
     target beyond `overlap_coord_bound(max_correspondence_distance)` raises RegtrLibError; with the caller's word,
@@ -1276,25 +1302,28 @@ def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iterat
                          f'relative_fitness / relative_rmse >= 0')
     if method not in ICP_METHODS:
         raise ValueError(f'icp: method {method!r} is not one of {ICP_METHODS}')
-    plane = method == 'point_to_plane'
-    if plane and tgt_normals is None:
-        raise ValueError('icp: point_to_plane needs the target normals (tgt_normals), e.g. from estimate_normals')
+    if loss not in ICP_LOSSES:
+        raise ValueError(f'icp: loss {loss!r} is not one of {ICP_LOSSES}')
+    if loss != 'l2' and method == 'point_to_point':
+        raise ValueError(f'icp: the point_to_point estimation takes no robust loss (got {loss!r})')
+    if loss != 'l2' and not (loss_k is not None and math.isfinite(float(loss_k)) and float(loss_k) > 0.0):
+        raise ValueError(f'icp: loss {loss!r} needs a finite loss_k > 0, got {loss_k!r}')
+    gicp = method == 'generalized'
+    if gicp and not (0.0 < float(epsilon) <= 1.0):
+        raise ValueError(f'icp: epsilon {epsilon!r} must be in (0, 1]')
+    if method != 'point_to_point' and tgt_normals is None:
+        raise ValueError(f'icp: {method} needs the target normals (tgt_normals), e.g. from estimate_normals')
+    if gicp and src_normals is None:
+        raise ValueError('icp: generalized needs the source normals (src_normals), e.g. from estimate_normals')
     B = len(src_list)
     dev = init.device if torch.is_tensor(init) and init.is_cuda else None
     xyz, offs, lens = _stack_pairs(src_list, tgt_list, 'icp', dev)
     dev = xyz.device
-    nrm = None
-    if plane:
-        if len(tgt_normals) != B:
-            raise ValueError(f'icp: {len(tgt_normals)} target normal arrays for {B} pairs')
-        nrm = torch.empty((max(sum(lens[B:]), 1), 3), dtype=torch.float64, device=dev)
-        a = 0
-        for c, ln in zip(tgt_normals, lens[B:]):
-            c = torch.as_tensor(c)
-            if tuple(c.shape) != (ln, 3):
-                raise ValueError(f'icp: target normals {tuple(c.shape)} for a target of {ln} points')
-            nrm[a:a + ln].copy_(c.to(dev, torch.float64))
-            a += ln
+    nrm = None if method == 'point_to_point' else _stack_normals(tgt_normals, lens[B:], 'target', dev)
+    snrm = _stack_normals(src_normals, lens[:B], 'source', dev) if gicp else None
+    opt = None
+    if gicp or loss != 'l2':
+        opt = IcpOptions(ICP_LOSSES.index(loss), float(loss_k) if loss != 'l2' else 1.0, float(epsilon))
     init64 = torch.as_tensor(init).to(dev, torch.float64).reshape(B, 3, 4).contiguous()
     n = sum(lens)
     own = status is None
@@ -1305,8 +1334,9 @@ def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iterat
     ws = workspace(L.regtr_icp_ws_bytes(n, B), dev)
     state = workspace(L.regtr_icp_state_bytes(n), dev, 'scan_state', zero=True)
     _lib.check(L.regtr_icp(_p(xyz), _p(offs), B, n, _p(init64), r, overlap_cell(r), int(max_iteration),
-                           float(relative_fitness), float(relative_rmse), _p(nrm), _p(pose),
-                           _p(out), _p(status), _p(ws), ws.numel(), _p(state), state.numel(), _stream()), 'regtr_icp')
+                           float(relative_fitness), float(relative_rmse), _p(nrm), _p(snrm),
+                           None if opt is None else ctypes.addressof(opt), _p(pose), _p(out), _p(status), _p(ws),
+                           ws.numel(), _p(state), state.numel(), _stream()), 'regtr_icp')
     _count(icp_launches(max_iteration))
     if own:
         check_fit_status(status, r, 'icp')

@@ -2,8 +2,8 @@
 
     python -m regtr_b200.register SRC TGT --ckpt <logdir>/ckpt/model-best.pth [--config <yaml>] \\
         [--threshold 0.5] [--fit_radius R] [--out DIR]
-        [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane [--normal_radius NR]
-         [--normal_max_nn 30]]]
+        [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized [--normal_radius NR]
+         [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
 
 SRC / TGT: .ply, .pth, .bin or .npy (regtr_b200.pointio).  The config is the config.yaml one level above the
 checkpoint's directory, the layout `python -m regtr_b200.train` writes, unless --config names another.  Instead of the
@@ -18,11 +18,14 @@ demo's viewer, the result is judged by the fitness and inlier RMSE of the final 
 With --icp R the final decoder layer's pose is refined by ICP on the cropped full-resolution clouds (`ops.icp`,
 Open3D's registration_icp with max_correspondence_distance R and --icp_iters iterations at most), point-to-point by
 default; --icp_method point_to_plane first estimates the cropped target's normals (`ops.estimate_normals`, Open3D's
-estimate_normals with KDTreeSearchParamHybrid(--normal_radius, default 2 R, --normal_max_nn));
+estimate_normals with KDTreeSearchParamHybrid(--normal_radius, default 2 R, --normal_max_nn)); --icp_method
+generalized estimates the normals of both cropped clouds in one call and runs Open3D's registration_generalized_icp
+(covariance epsilon --icp_epsilon); --icp_loss with --icp_loss_k weights the point-to-plane or generalized residuals by
+Open3D's robust kernel of that name;
 pose.txt, src_registered.ply and fit then use the refined pose, result.npz gains pose_coarse (the network's final
 pose), pose_icp (the refined one) and icp (4,) = fitness, inlier_rmse, correspondences, iterations.
 One JSON line on stdout: the pose, the four fit numbers and the point counts (with --icp, also icp_fitness, icp_rmse,
-icp_iterations, icp_radius and icp_method).
+icp_iterations, icp_radius and icp_method, and icp_loss, icp_loss_k and icp_epsilon when they are given).
 """
 from __future__ import annotations
 
@@ -49,12 +52,19 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument('--icp', type=float, metavar='R',
                     help='Refine the pose with point-to-point ICP, max correspondence distance R (default: no ICP)')
     ap.add_argument('--icp_iters', type=int, default=30, help='ICP iterations at most (with --icp)')
-    ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane'), default='point_to_point',
-                    help='ICP error metric (with --icp); point_to_plane estimates the target normals first')
+    ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane', 'generalized'),
+                    default='point_to_point',
+                    help='ICP error metric (with --icp); point_to_plane estimates the target normals first, '
+                         'generalized those of both clouds')
     ap.add_argument('--normal_radius', type=float, metavar='NR',
-                    help='Normal estimation radius of point_to_plane ICP (default: 2 * the --icp radius)')
+                    help='Normal estimation radius of point_to_plane / generalized ICP (default: 2 * the --icp radius)')
     ap.add_argument('--normal_max_nn', type=int, default=30,
-                    help='Neighbours at most of the normal estimation (with point_to_plane ICP)')
+                    help='Neighbours at most of the normal estimation (with point_to_plane / generalized ICP)')
+    ap.add_argument('--icp_epsilon', type=float, default=1e-3,
+                    help='Covariance epsilon of generalized ICP, in (0, 1]')
+    ap.add_argument('--icp_loss', choices=('l2', 'huber', 'cauchy', 'gm', 'tukey'), default='l2',
+                    help='Robust kernel of point_to_plane / generalized ICP (needs --icp_loss_k unless l2)')
+    ap.add_argument('--icp_loss_k', type=float, metavar='K', help='The robust kernel\'s parameter k')
     ap.add_argument('--out', default='.', help='Output directory')
     return ap
 
@@ -83,7 +93,8 @@ def load_model(cfg, ckpt: str, device=None):
 
 def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: float = None,
              icp_radius: float = None, icp_iters: int = 30, icp_method: str = 'point_to_point',
-             normal_radius: float = None, normal_max_nn: int = 30) -> Dict:
+             normal_radius: float = None, normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
+             icp_loss_k: float = None) -> Dict:
     """Crop, forward and fit one pair.  src_xyz / tgt_xyz (N,3) float64 host arrays.
     -> dict of host arrays: src_xyz / tgt_xyz (cropped, float64), pose (L,3,4) fp32, src_kp, src_kp_warped (final
     layer), src_overlap (sigmoid of the final layer's logit, (n,)), the same for tgt, fit (4,) float64.
@@ -91,7 +102,8 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
     cropped clouds; fit is then that of the refined pose, and the dict gains pose_coarse (3,4) fp32 (the network's
     final pose), pose_icp (3,4) float64 and icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations.
     icp_method 'point_to_plane' refines against the cropped target's normals from `ops.estimate_normals` at
-    normal_radius (default 2 * icp_radius) and normal_max_nn."""
+    normal_radius (default 2 * icp_radius) and normal_max_nn; 'generalized' estimates the normals of both cropped
+    clouds in one call and refines with covariance epsilon icp_epsilon.  icp_loss / icp_loss_k: `ops.icp`'s loss."""
     from . import ops
     src_xyz = crop(cfg, np.asarray(src_xyz, dtype=np.float64))
     tgt_xyz = crop(cfg, np.asarray(tgt_xyz, dtype=np.float64))
@@ -105,12 +117,16 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
         status = ops.new_status(dev)
         final = pose[-1:]
         if icp_radius is not None:
-            normals = None
+            normals = src_normals = None
+            nr = 2.0 * icp_radius if normal_radius is None else normal_radius
             if icp_method == 'point_to_plane':
-                nr = 2.0 * icp_radius if normal_radius is None else normal_radius
                 normals = ops.estimate_normals([tgt_xyz], nr, normal_max_nn)
+            elif icp_method == 'generalized':
+                src_normals, normals = ops.estimate_normals([src_xyz, tgt_xyz], nr, normal_max_nn)
+                src_normals, normals = [src_normals], [normals]
             final, icp = ops.icp([src_xyz], [tgt_xyz], pose[-1:], icp_radius, icp_iters, method=icp_method,
-                                 tgt_normals=normals)
+                                 tgt_normals=normals, src_normals=src_normals, epsilon=icp_epsilon, loss=icp_loss,
+                                 loss_k=icp_loss_k)
         fit = ops.registration_fit([src_xyz], [tgt_xyz], final, radius, status)
         res = {'src_xyz': src_xyz, 'tgt_xyz': tgt_xyz, 'pose': pose.cpu().numpy()}
         if icp_radius is not None:
@@ -154,7 +170,10 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
 
 
 def main(argv=None):
-    opt = parser().parse_args(argv)
+    ap = parser()
+    opt = ap.parse_args(argv)
+    if opt.icp_loss != 'l2' and opt.icp_loss_k is None:
+        ap.error(f'--icp_loss {opt.icp_loss} needs --icp_loss_k')
     from .config import load_config
     from .pointio import load_point_cloud
     cfg_file = config_path(opt.ckpt, opt.config)
@@ -163,7 +182,8 @@ def main(argv=None):
     cfg = load_config(str(cfg_file))
     model = load_model(cfg, opt.ckpt)
     res = register(model, cfg, load_point_cloud(opt.src), load_point_cloud(opt.tgt), opt.fit_radius, opt.icp,
-                   opt.icp_iters, opt.icp_method, opt.normal_radius, opt.normal_max_nn)
+                   opt.icp_iters, opt.icp_method, opt.normal_radius, opt.normal_max_nn, opt.icp_epsilon,
+                   opt.icp_loss, opt.icp_loss_k)
     n_shown = write_outputs(res, opt.out, opt.threshold)
     f = [float(v) for v in res['fit']]
     line = {'pose': pose44(res['pose_icp'] if opt.icp is not None else res['pose'][-1]).tolist(),
@@ -176,6 +196,10 @@ def main(argv=None):
         icp = [float(v) for v in res['icp']]
         line.update(icp_fitness=icp[0], icp_rmse=icp[1], icp_iterations=int(icp[3]), icp_radius=float(opt.icp),
                     icp_method=opt.icp_method)
+        if opt.icp_loss != 'l2':
+            line.update(icp_loss=opt.icp_loss, icp_loss_k=float(opt.icp_loss_k))
+        if opt.icp_method == 'generalized':
+            line.update(icp_epsilon=float(opt.icp_epsilon))
     print(json.dumps(line))
     return res
 

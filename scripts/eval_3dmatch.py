@@ -2,10 +2,12 @@
 
     python scripts/eval_3dmatch.py --root <data/indoor> --info <test_3DMatch_info.pkl> \
         --gt <datasets/3dmatch/benchmarks/3DMatch> --ckpt <model.pth> --out logs/3DMatch [--icp R [--icp_iters N]
-        [--icp_method point_to_plane [--normal_radius NR] [--normal_max_nn 30]]]
+        [--icp_method point_to_plane|generalized [--normal_radius NR] [--normal_max_nn 30] [--icp_epsilon 1e-3]
+        [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
 
 --icp R refines every final pose by ICP on the full clouds (`ops.icp`, max correspondence distance R; point-to-point,
-or point-to-plane against target normals from `ops.estimate_normals` at NR, default 2 R): est.log then holds the
+or point-to-plane against target normals from `ops.estimate_normals` at NR, default 2 R, or generalized ICP on the
+normals of both clouds, optionally under a robust loss): est.log then holds the
 refined poses, and the metrics report both (`rot_err_deg` / `trans_err` refined, `*_coarse` the network's).
 Needs the dataset and trained weights (neither is available offline: SURVEY.md 8f N1)."""
 import argparse, os, sys
@@ -21,8 +23,11 @@ ap.add_argument('--ckpt', required=True); ap.add_argument('--out', default='logs
 ap.add_argument('--batch', type=int, default=1); ap.add_argument('--workers', type=int, default=4)
 ap.add_argument('--icp', type=float, help='Refine the poses by ICP with this max correspondence distance')
 ap.add_argument('--icp_iters', type=int, default=30)
-ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane'), default='point_to_point')
+ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane', 'generalized'), default='point_to_point')
 ap.add_argument('--normal_radius', type=float); ap.add_argument('--normal_max_nn', type=int, default=30)
+ap.add_argument('--icp_epsilon', type=float, default=1e-3)
+ap.add_argument('--icp_loss', choices=('l2', 'huber', 'cauchy', 'gm', 'tukey'), default='l2')
+ap.add_argument('--icp_loss_k', type=float)
 args = ap.parse_args()
 dev = torch.device('cuda:0')
 cfg = get_config('3dmatch')
@@ -34,7 +39,7 @@ ds = D.ThreeDMatchPairs(args.root, args.info, pin=True)
 batches = [list(range(i, min(i + args.batch, len(ds)))) for i in range(0, len(ds), args.batch)]
 forward = (lambda b: runner(b)) if args.icp is None else E.icp_forward(
     lambda b: runner(b), args.icp, args.icp_iters, method=args.icp_method, normal_radius=args.normal_radius,
-    normal_max_nn=args.normal_max_nn)
+    normal_max_nn=args.normal_max_nn, epsilon=args.icp_epsilon, loss=args.icp_loss, loss_k=args.icp_loss_k)
 res = E.run_3dmatch_benchmark(D.PairStream(ds, batches, workers=args.workers), forward, args.out,
                               args.benchmark, args.gt)
 print(res['summary']); print('registration recall', res['recall'])
