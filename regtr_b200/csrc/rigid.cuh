@@ -1,5 +1,5 @@
 // Internal to the library: float64 rigid-transform helpers shared by the pose solve (kabsch.cu), the training-data
-// preparation (traindata.cu), ICP (icp.cu, gicp.cu) and the pose-graph optimiser (posegraph.cu).
+// preparation (traindata.cu), ICP (icp.cu) and the pose-graph optimiser (posegraph.cu).
 #pragma once
 
 #include "common.cuh"

@@ -376,6 +376,69 @@ def summarize_modelnet_metrics(metrics: Dict[str, np.ndarray]) -> Dict[str, floa
 # ------------------------------------------------------------------- test loop (reference: test.py)
 
 
+def icp_refine(src_list, tgt_list, init, radius: float, max_iteration: int = 30, method: str = 'point_to_point',
+               normal_radius: float = None, normal_max_nn: int = 30, epsilon: float = 1e-3, loss: str = 'l2',
+               loss_k: float = None, normals=None, icp=None, estimate_normals=None):
+    """Refine B poses init (B,3,4) by ICP of src_list onto tgt_list: the normals each method needs, then one icp call.
+    -> icp's (pose (B,3,4), result).
+    icp(src_list, tgt_list, init, radius, max_iteration, ...) defaults to `ops.icp`; point-to-point passes nothing
+    more.  method='point_to_plane': the targets' normals come from estimate_normals(tgt_list, normal_radius (default
+    2 * radius), normal_max_nn) (default `ops.estimate_normals`), and icp gets method=method, tgt_normals=.
+    method='generalized': the normals of src_list + tgt_list come from one estimate_normals call, and icp also gets
+    src_normals=.  normals=(src_normals, tgt_normals) skips the estimation (only the ones the method needs are
+    passed on).  epsilon, loss and loss_k (see `ops.icp`) are passed on only when they differ from their defaults."""
+    if icp is None:
+        from .ops import icp
+    kw = {}
+    if method != 'point_to_point':
+        if normals is None:
+            if estimate_normals is None:
+                from .ops import estimate_normals
+            nr = 2.0 * radius if normal_radius is None else normal_radius
+            if method == 'generalized':
+                B = len(src_list)
+                est = estimate_normals(list(src_list) + list(tgt_list), nr, normal_max_nn)
+                normals = est[:B], est[B:]
+            else:
+                normals = None, estimate_normals(tgt_list, nr, normal_max_nn)
+        kw.update(method=method, tgt_normals=normals[1])
+        if method == 'generalized':
+            kw['src_normals'] = normals[0]
+    if epsilon != 1e-3:
+        kw['epsilon'] = epsilon
+    if loss != 'l2':
+        kw['loss'] = loss
+    if loss_k is not None:
+        kw['loss_k'] = loss_k
+    return icp(src_list, tgt_list, init, radius, max_iteration, **kw)
+
+
+def add_icp_arguments(ap, icp_help: str):
+    """The ICP refinement flags of a command line, for `icp_refine`: --icp R (help text icp_help), --icp_iters,
+    --icp_method, --normal_radius, --normal_max_nn, --icp_epsilon, --icp_loss and --icp_loss_k."""
+    from .ops import ICP_LOSSES, ICP_METHODS
+    ap.add_argument('--icp', type=float, metavar='R', help=icp_help)
+    ap.add_argument('--icp_iters', type=int, default=30, help='ICP iterations at most (with --icp)')
+    ap.add_argument('--icp_method', choices=ICP_METHODS, default='point_to_point',
+                    help='ICP error metric (with --icp); point_to_plane estimates the target normals first, '
+                         'generalized those of both clouds')
+    ap.add_argument('--normal_radius', type=float, metavar='NR',
+                    help='Normal estimation radius of point_to_plane / generalized ICP (default: 2 * the --icp radius)')
+    ap.add_argument('--normal_max_nn', type=int, default=30,
+                    help='Neighbours at most of the normal estimation (with point_to_plane / generalized ICP)')
+    ap.add_argument('--icp_epsilon', type=float, default=1e-3,
+                    help='Covariance epsilon of generalized ICP, in (0, 1]')
+    ap.add_argument('--icp_loss', choices=ICP_LOSSES, default='l2',
+                    help='Robust kernel of point_to_plane / generalized ICP (needs --icp_loss_k unless l2)')
+    ap.add_argument('--icp_loss_k', type=float, metavar='K', help='The robust kernel\'s parameter k')
+
+
+def check_icp_arguments(ap, opt):
+    """Reject, as a usage error, a robust --icp_loss without its --icp_loss_k, before any model is loaded."""
+    if opt.icp_loss != 'l2' and opt.icp_loss_k is None:
+        ap.error(f'--icp_loss {opt.icp_loss} needs --icp_loss_k')
+
+
 def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None, method: str = 'point_to_point',
                 normal_radius: float = None, normal_max_nn: int = 30, estimate_normals=None, epsilon: float = 1e-3,
                 loss: str = 'l2', loss_k: float = None):
@@ -383,40 +446,16 @@ def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None, me
     clouds: -> a NEW dict with pred's entries, pose (1,B,3,4) float64 the refined poses and pose_coarse
     (1,B,3,4) float64 the network's final poses (so that `compute_metrics` reports both, and EstLogWriter writes the
     refined ones).  pred's own tensors are not written to (a graphed forward owns them).
-    icp(src_list, tgt_list, init (B,3,4), radius, max_iteration) -> (pose (B,3,4), result): default `ops.icp`,
-    point-to-point.  method='point_to_plane': the targets' normals come from
-    estimate_normals(tgt_list, normal_radius (default 2 * radius), normal_max_nn) (default `ops.estimate_normals`) and
-    icp is called as icp(src_list, tgt_list, init, radius, max_iteration, method=method, tgt_normals=normals).
-    method='generalized': the normals of src_list + tgt_list come from one estimate_normals call, and icp also gets
-    src_normals=.  epsilon, loss and loss_k (see `ops.icp`) are passed on only when they differ from their defaults."""
-    if method not in ('point_to_point', 'point_to_plane', 'generalized'):
+    The refinement is `icp_refine` with these arguments, icp and estimate_normals included."""
+    from .ops import ICP_METHODS
+    if method not in ICP_METHODS:
         raise ValueError(f'icp_forward: unknown method {method!r}')
-    if icp is None:
-        from .ops import icp
-    if method != 'point_to_point' and estimate_normals is None:
-        from .ops import estimate_normals
-    nr = 2.0 * radius if normal_radius is None else normal_radius
-    extra = {}
-    if epsilon != 1e-3:
-        extra['epsilon'] = epsilon
-    if loss != 'l2':
-        extra['loss'] = loss
-    if loss_k is not None:
-        extra['loss_k'] = loss_k
     def run(batch):
         pred = forward_fn(batch)
         coarse = pred['pose'][-1].to(torch.float64)                     # (B,3,4), a new tensor
-        if method == 'point_to_point':
-            pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, **extra)
-        elif method == 'point_to_plane':
-            normals = estimate_normals(batch['tgt_xyz'], nr, normal_max_nn)
-            pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, method=method,
-                          tgt_normals=normals, **extra)
-        else:
-            B = len(batch['src_xyz'])
-            normals = estimate_normals(list(batch['src_xyz']) + list(batch['tgt_xyz']), nr, normal_max_nn)
-            pose, _ = icp(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, method=method,
-                          tgt_normals=normals[B:], src_normals=normals[:B], **extra)
+        pose, _ = icp_refine(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, method,
+                             normal_radius, normal_max_nn, epsilon, loss, loss_k, icp=icp,
+                             estimate_normals=estimate_normals)
         out = dict(pred)
         out['pose'] = torch.as_tensor(pose, dtype=torch.float64, device=coarse.device).reshape(coarse.shape)[None]
         out['pose_coarse'] = coarse[None]

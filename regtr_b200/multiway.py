@@ -38,6 +38,8 @@ from typing import Dict, List, Sequence
 import numpy as np
 import torch
 
+from .eval import add_icp_arguments, check_icp_arguments, icp_refine
+
 
 def parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(prog='python -m regtr_b200.multiway',
@@ -46,18 +48,7 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument('--ckpt', required=True, help='Checkpoint ({"state_dict": ...}), e.g. <logdir>/ckpt/model-best.pth')
     ap.add_argument('--config', help='Config file (default: config.yaml one level above the checkpoint directory)')
     ap.add_argument('--out', required=True, help='Output directory')
-    ap.add_argument('--icp', type=float, metavar='R', help='Refine every pair by ICP, max correspondence distance R')
-    ap.add_argument('--icp_iters', type=int, default=30, help='ICP iterations at most (with --icp)')
-    ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane', 'generalized'),
-                    default='point_to_point', help='ICP error metric (with --icp)')
-    ap.add_argument('--normal_radius', type=float, metavar='NR',
-                    help='Normal estimation radius of point_to_plane / generalized ICP (default: 2 * the --icp radius)')
-    ap.add_argument('--normal_max_nn', type=int, default=30, help='Neighbours at most of the normal estimation')
-    ap.add_argument('--icp_epsilon', type=float, default=1e-3,
-                    help='Covariance epsilon of generalized ICP, in (0, 1]')
-    ap.add_argument('--icp_loss', choices=('l2', 'huber', 'cauchy', 'gm', 'tukey'), default='l2',
-                    help='Robust kernel of point_to_plane / generalized ICP (needs --icp_loss_k unless l2)')
-    ap.add_argument('--icp_loss_k', type=float, metavar='K', help='The robust kernel\'s parameter k')
+    add_icp_arguments(ap, 'Refine every pair by ICP, max correspondence distance R')
     ap.add_argument('--info_radius', type=float, metavar='D',
                     help='Radius of the information matrices and the line process (default: overlap_radius)')
     ap.add_argument('--min_overlap', type=float, default=0.3,
@@ -78,7 +69,7 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
                    normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
                    icp_loss_k: float = None) -> np.ndarray:
     """RegTR's final-layer pose of every pair (i, j) of `all_pairs`, source j -> target i, optionally refined by ICP
-    (`ops.icp` with icp_method, epsilon=icp_epsilon, loss=icp_loss, loss_k=icp_loss_k; the point-to-plane and
+    (`eval.icp_refine` with icp_method, epsilon=icp_epsilon, loss=icp_loss, loss_k=icp_loss_k; the point-to-plane and
     generalized methods use every fragment's normals, estimated once).
     fragments: (n,3) float64 host arrays (already cropped).  -> (P,3,4) float64."""
     from . import ops
@@ -96,11 +87,10 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
             pred = model({'src_xyz': [dev_frags[j] for _, j in chunk], 'tgt_xyz': [dev_frags[i] for i, _ in chunk]})
             pose = pred['pose'][-1].double()
             if icp_radius is not None:
-                pose, _ = ops.icp([fragments[j] for _, j in chunk], [fragments[i] for i, _ in chunk], pose, icp_radius,
-                                  icp_iters, method=icp_method,
-                                  tgt_normals=None if normals is None else [normals[i] for i, _ in chunk],
-                                  src_normals=None if normals is None else [normals[j] for _, j in chunk],
-                                  epsilon=icp_epsilon, loss=icp_loss, loss_k=icp_loss_k)
+                pose, _ = icp_refine([fragments[j] for _, j in chunk], [fragments[i] for i, _ in chunk], pose,
+                                     icp_radius, icp_iters, icp_method, epsilon=icp_epsilon, loss=icp_loss,
+                                     loss_k=icp_loss_k, normals=None if normals is None else
+                                     ([normals[j] for _, j in chunk], [normals[i] for i, _ in chunk]))
             out.append(pose.cpu().numpy())
     return np.concatenate(out, 0)
 
@@ -197,7 +187,9 @@ def scene_name(path: str) -> str:
 
 
 def main(argv=None):
-    opt = parser().parse_args(argv)
+    ap = parser()
+    opt = ap.parse_args(argv)
+    check_icp_arguments(ap, opt)
     from .config import load_config
     from .pointio import load_point_cloud
     from .register import config_path, crop, load_model

@@ -38,6 +38,8 @@ from typing import Dict
 import numpy as np
 import torch
 
+from .eval import add_icp_arguments, check_icp_arguments, icp_refine
+
 
 def parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(prog='python -m regtr_b200.register',
@@ -49,22 +51,7 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument('--threshold', type=float, default=0.5,
                     help='Keypoints with predicted overlap above this go to src_kp.ply / src_kp_warped.ply')
     ap.add_argument('--fit_radius', type=float, help='Inlier radius of the fitness / RMSE (default: overlap_radius)')
-    ap.add_argument('--icp', type=float, metavar='R',
-                    help='Refine the pose with point-to-point ICP, max correspondence distance R (default: no ICP)')
-    ap.add_argument('--icp_iters', type=int, default=30, help='ICP iterations at most (with --icp)')
-    ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane', 'generalized'),
-                    default='point_to_point',
-                    help='ICP error metric (with --icp); point_to_plane estimates the target normals first, '
-                         'generalized those of both clouds')
-    ap.add_argument('--normal_radius', type=float, metavar='NR',
-                    help='Normal estimation radius of point_to_plane / generalized ICP (default: 2 * the --icp radius)')
-    ap.add_argument('--normal_max_nn', type=int, default=30,
-                    help='Neighbours at most of the normal estimation (with point_to_plane / generalized ICP)')
-    ap.add_argument('--icp_epsilon', type=float, default=1e-3,
-                    help='Covariance epsilon of generalized ICP, in (0, 1]')
-    ap.add_argument('--icp_loss', choices=('l2', 'huber', 'cauchy', 'gm', 'tukey'), default='l2',
-                    help='Robust kernel of point_to_plane / generalized ICP (needs --icp_loss_k unless l2)')
-    ap.add_argument('--icp_loss_k', type=float, metavar='K', help='The robust kernel\'s parameter k')
+    add_icp_arguments(ap, 'Refine the pose with point-to-point ICP, max correspondence distance R (default: no ICP)')
     ap.add_argument('--out', default='.', help='Output directory')
     return ap
 
@@ -98,12 +85,10 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
     """Crop, forward and fit one pair.  src_xyz / tgt_xyz (N,3) float64 host arrays.
     -> dict of host arrays: src_xyz / tgt_xyz (cropped, float64), pose (L,3,4) fp32, src_kp, src_kp_warped (final
     layer), src_overlap (sigmoid of the final layer's logit, (n,)), the same for tgt, fit (4,) float64.
-    icp_radius: refine the final layer's pose by ICP (`ops.icp` with icp_method, at most icp_iters iterations) on the
-    cropped clouds; fit is then that of the refined pose, and the dict gains pose_coarse (3,4) fp32 (the network's
-    final pose), pose_icp (3,4) float64 and icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations.
-    icp_method 'point_to_plane' refines against the cropped target's normals from `ops.estimate_normals` at
-    normal_radius (default 2 * icp_radius) and normal_max_nn; 'generalized' estimates the normals of both cropped
-    clouds in one call and refines with covariance epsilon icp_epsilon.  icp_loss / icp_loss_k: `ops.icp`'s loss."""
+    icp_radius: refine the final layer's pose by ICP on the cropped clouds (`eval.icp_refine` with icp_method, at most
+    icp_iters iterations, and normal_radius, normal_max_nn, icp_epsilon, icp_loss and icp_loss_k); fit is then that of
+    the refined pose, and the dict gains pose_coarse (3,4) fp32 (the network's final pose), pose_icp (3,4) float64 and
+    icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations."""
     from . import ops
     src_xyz = crop(cfg, np.asarray(src_xyz, dtype=np.float64))
     tgt_xyz = crop(cfg, np.asarray(tgt_xyz, dtype=np.float64))
@@ -117,16 +102,8 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
         status = ops.new_status(dev)
         final = pose[-1:]
         if icp_radius is not None:
-            normals = src_normals = None
-            nr = 2.0 * icp_radius if normal_radius is None else normal_radius
-            if icp_method == 'point_to_plane':
-                normals = ops.estimate_normals([tgt_xyz], nr, normal_max_nn)
-            elif icp_method == 'generalized':
-                src_normals, normals = ops.estimate_normals([src_xyz, tgt_xyz], nr, normal_max_nn)
-                src_normals, normals = [src_normals], [normals]
-            final, icp = ops.icp([src_xyz], [tgt_xyz], pose[-1:], icp_radius, icp_iters, method=icp_method,
-                                 tgt_normals=normals, src_normals=src_normals, epsilon=icp_epsilon, loss=icp_loss,
-                                 loss_k=icp_loss_k)
+            final, icp = icp_refine([src_xyz], [tgt_xyz], pose[-1:], icp_radius, icp_iters, icp_method, normal_radius,
+                                    normal_max_nn, icp_epsilon, icp_loss, icp_loss_k)
         fit = ops.registration_fit([src_xyz], [tgt_xyz], final, radius, status)
         res = {'src_xyz': src_xyz, 'tgt_xyz': tgt_xyz, 'pose': pose.cpu().numpy()}
         if icp_radius is not None:
@@ -172,8 +149,7 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
 def main(argv=None):
     ap = parser()
     opt = ap.parse_args(argv)
-    if opt.icp_loss != 'l2' and opt.icp_loss_k is None:
-        ap.error(f'--icp_loss {opt.icp_loss} needs --icp_loss_k')
+    check_icp_arguments(ap, opt)
     from .config import load_config
     from .pointio import load_point_cloud
     cfg_file = config_path(opt.ckpt, opt.config)

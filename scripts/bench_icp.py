@@ -126,11 +126,11 @@ def parser():
     ap.add_argument('--blocks', type=int, default=7)
     ap.add_argument('--reps', type=int, default=10)
     ap.add_argument('--cpu-reps', type=int, default=1)
-    ap.add_argument('--method', choices=('point_to_point', 'point_to_plane', 'generalized'), default='point_to_point')
+    ap.add_argument('--method', choices=ops.ICP_METHODS, default='point_to_point')
     ap.add_argument('--normal_radius', type=float, help='default: 2 * --radius')
     ap.add_argument('--normal_max_nn', type=int, default=30)
     ap.add_argument('--epsilon', type=float, default=1e-3, help='covariance epsilon of generalized ICP')
-    ap.add_argument('--loss', choices=('l2', 'huber', 'cauchy', 'gm', 'tukey'), default='l2')
+    ap.add_argument('--loss', choices=ops.ICP_LOSSES, default='l2')
     ap.add_argument('--loss_k', type=float)
     return ap
 

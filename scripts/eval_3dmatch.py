@@ -17,30 +17,36 @@ from regtr_b200 import data as D, eval as E
 from regtr_b200.config import get_config
 from regtr_b200.regtr import GraphedRegTR, RegTR
 
-ap = argparse.ArgumentParser()
-ap.add_argument('--root', required=True); ap.add_argument('--info', required=True); ap.add_argument('--gt', required=True)
-ap.add_argument('--ckpt', required=True); ap.add_argument('--out', default='logs'); ap.add_argument('--benchmark', default='3DMatch')
-ap.add_argument('--batch', type=int, default=1); ap.add_argument('--workers', type=int, default=4)
-ap.add_argument('--icp', type=float, help='Refine the poses by ICP with this max correspondence distance')
-ap.add_argument('--icp_iters', type=int, default=30)
-ap.add_argument('--icp_method', choices=('point_to_point', 'point_to_plane', 'generalized'), default='point_to_point')
-ap.add_argument('--normal_radius', type=float); ap.add_argument('--normal_max_nn', type=int, default=30)
-ap.add_argument('--icp_epsilon', type=float, default=1e-3)
-ap.add_argument('--icp_loss', choices=('l2', 'huber', 'cauchy', 'gm', 'tukey'), default='l2')
-ap.add_argument('--icp_loss_k', type=float)
-args = ap.parse_args()
-dev = torch.device('cuda:0')
-cfg = get_config('3dmatch')
-model = RegTR(cfg).to(dev).eval()
-state = torch.load(args.ckpt, map_location='cpu')
-model.load_state_dict(state.get('state_dict', state), strict=False)      # torch_helpers.py:222
-runner = GraphedRegTR(model)
-ds = D.ThreeDMatchPairs(args.root, args.info, pin=True)
-batches = [list(range(i, min(i + args.batch, len(ds)))) for i in range(0, len(ds), args.batch)]
-forward = (lambda b: runner(b)) if args.icp is None else E.icp_forward(
-    lambda b: runner(b), args.icp, args.icp_iters, method=args.icp_method, normal_radius=args.normal_radius,
-    normal_max_nn=args.normal_max_nn, epsilon=args.icp_epsilon, loss=args.icp_loss, loss_k=args.icp_loss_k)
-res = E.run_3dmatch_benchmark(D.PairStream(ds, batches, workers=args.workers), forward, args.out,
-                              args.benchmark, args.gt)
-print(res['summary']); print('registration recall', res['recall'])
-print({k: float(v) for k, v in res['metrics'].items() if not k.endswith('hist')})
+
+def parser():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--root', required=True); ap.add_argument('--info', required=True); ap.add_argument('--gt', required=True)
+    ap.add_argument('--ckpt', required=True); ap.add_argument('--out', default='logs'); ap.add_argument('--benchmark', default='3DMatch')
+    ap.add_argument('--batch', type=int, default=1); ap.add_argument('--workers', type=int, default=4)
+    E.add_icp_arguments(ap, 'Refine the poses by ICP with this max correspondence distance')
+    return ap
+
+
+def main(argv=None):
+    ap = parser()
+    args = ap.parse_args(argv)
+    E.check_icp_arguments(ap, args)
+    dev = torch.device('cuda:0')
+    cfg = get_config('3dmatch')
+    model = RegTR(cfg).to(dev).eval()
+    state = torch.load(args.ckpt, map_location='cpu')
+    model.load_state_dict(state.get('state_dict', state), strict=False)      # torch_helpers.py:222
+    runner = GraphedRegTR(model)
+    ds = D.ThreeDMatchPairs(args.root, args.info, pin=True)
+    batches = [list(range(i, min(i + args.batch, len(ds)))) for i in range(0, len(ds), args.batch)]
+    forward = (lambda b: runner(b)) if args.icp is None else E.icp_forward(
+        lambda b: runner(b), args.icp, args.icp_iters, method=args.icp_method, normal_radius=args.normal_radius,
+        normal_max_nn=args.normal_max_nn, epsilon=args.icp_epsilon, loss=args.icp_loss, loss_k=args.icp_loss_k)
+    res = E.run_3dmatch_benchmark(D.PairStream(ds, batches, workers=args.workers), forward, args.out,
+                                  args.benchmark, args.gt)
+    print(res['summary']); print('registration recall', res['recall'])
+    print({k: float(v) for k, v in res['metrics'].items() if not k.endswith('hist')})
+
+
+if __name__ == '__main__':
+    main()

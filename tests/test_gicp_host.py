@@ -1,7 +1,7 @@
 """Generalized ICP and robust kernels on the host: the float64 oracle (tests/gicp_oracle.py) against independent
 constructions of the covariance and the weights, recovery of a known transform, the robust kernels' resistance to an
-off-surface block, the CLI flags of register, multiway, eval_3dmatch and bench_icp, the 3DMatch benchmark wrapper's
-generalized layout, and that gicp.cu's kernels have no stack frame and do not spill."""
+off-surface block, the CLI flags of register, multiway, eval_3dmatch and bench_icp, and the 3DMatch benchmark
+wrapper's generalized layout.  (The ICP kernels' stack and spill check is in test_icp_host.py.)"""
 import os
 import re
 import subprocess
@@ -145,6 +145,33 @@ def test_bench_and_eval_scripts_accept_the_generalized_flags():
     assert 'generalized' in r.stdout
 
 
+def _eval_3dmatch():
+    sys.path.insert(0, os.path.join(ROOT, 'scripts'))
+    try:
+        import eval_3dmatch
+    finally:
+        sys.path.pop(0)
+    return eval_3dmatch
+
+
+@pytest.mark.parametrize('cli', ['register', 'multiway', 'eval_3dmatch'])
+def test_every_command_line_rejects_a_robust_loss_without_its_k(cli, capsys):
+    """At parse time, before any model or data is loaded: a usage error (exit status 2)."""
+    ap, main, args = {
+        'register': lambda: (R.parser(), R.main, ['a.ply', 'b.ply', '--ckpt', 'c/ckpt/m.pth']),
+        'multiway': lambda: (MW.parser(), MW.main, ['a.ply', 'b.ply', '--ckpt', 'c/ckpt/m.pth', '--out', 'o']),
+        'eval_3dmatch': lambda: (_eval_3dmatch().parser(), _eval_3dmatch().main,
+                                 ['--root', 'r', '--info', 'i.pkl', '--gt', 'g', '--ckpt', 'm.pth']),
+    }[cli]()
+    args += ['--icp', '0.03', '--icp_method', 'point_to_plane', '--icp_loss', 'huber']
+    with pytest.raises(SystemExit) as e:
+        main(args)
+    assert e.value.code == 2 and '--icp_loss huber needs --icp_loss_k' in capsys.readouterr().err
+    opt = ap.parse_args(args + ['--icp_loss_k', '0.02'])
+    E.check_icp_arguments(ap, opt)
+    assert (opt.icp_loss, opt.icp_loss_k) == ('huber', 0.02)
+
+
 def test_benchmark_wrapper_generalized_layout_on_cpu():
     rng = np.random.default_rng(11)
     B, L = 2, 3
@@ -189,20 +216,3 @@ def test_benchmark_wrapper_generalized_layout_on_cpu():
     assert seen == [['loss', 'loss_k', 'method', 'tgt_normals']]
     with pytest.raises(ValueError):
         E.icp_forward(lambda b: b, 0.05, method='gicp')
-
-
-def test_gicp_kernels_have_no_stack_frame_and_do_not_spill(tmp_path):
-    nvcc = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-    from regtr_b200 import build
-    r = subprocess.run([nvcc] + build.NVCC_FLAGS + ['-Xptxas', '-v', '-c', os.path.join(build.CSRC, 'gicp.cu'),
-                                                    '-o', str(tmp_path / 'gicp.o')],
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr
-    text = r.stdout + r.stderr
-    entries = re.findall(r"Compiling entry function '(\w+)'[^\n]*\n[^\n]*Function properties for \w+\n\s*(\d+) "
-                         r"bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", text)
-    names = sorted(e[0] for e in entries)
-    assert len(entries) == 2 and 'k_icp_robust_reduceILb0' in names[0] and 'k_icp_robust_reduceILb1' in names[1], names
-    for name, frame, st, ld in entries:
-        assert (frame, st, ld) == ('0', '0', '0'), (name, frame, st, ld)
-    assert set(re.findall(r'(\d+) bytes spill (?:stores|loads)', text)) == {'0'}

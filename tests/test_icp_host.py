@@ -1,8 +1,11 @@
 """Point-to-point ICP on the host: the float64 oracle (tests/icp_oracle.py) against brute force and known transforms,
-its edge cases, the CLI flags of `python -m regtr_b200.register`, and the 3DMatch benchmark's ICP wrapper."""
+its edge cases, the CLI flags of `python -m regtr_b200.register`, and the 3DMatch benchmark's ICP wrapper; and the
+spills and stack frames of every ICP kernel in icp.cu."""
+import functools
 import os
 import re
 import subprocess
+import tempfile
 
 import numpy as np
 import torch
@@ -121,15 +124,45 @@ def test_benchmark_wrapper_layout_on_cpu():
     assert 'rot_err_deg_final' in agg and 'rot_err_deg_coarse_final' in agg
 
 
-def test_icp_kernels_do_not_spill(tmp_path):
+ICP_KERNELS = ('k_icp_init', 'k_icp_nn', 'k_icp_reduce_point', 'k_icp_reduce_planeILNS_9PlaneModeE0',
+               'k_icp_reduce_planeILNS_9PlaneModeE1', 'k_icp_reduce_planeILNS_9PlaneModeE2', 'k_icp_updateILb0',
+               'k_icp_updateILb1')
+
+
+@functools.lru_cache(maxsize=None)
+def icp_ptxas():
+    """icp.cu compiled with -Xptxas -v: (ptxas output, {kernel of ICP_KERNELS: (stack, spill stores, spill loads)})."""
     nvcc = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
     from regtr_b200 import build
-    r = subprocess.run([nvcc] + build.NVCC_FLAGS + ['-Xptxas', '-v', '-c', os.path.join(build.CSRC, 'icp.cu'),
-                                                    '-o', str(tmp_path / 'icp.o')],
-                       capture_output=True, text=True, timeout=900)
+    with tempfile.TemporaryDirectory() as tmp:
+        r = subprocess.run([nvcc] + build.NVCC_FLAGS + ['-Xptxas', '-v', '-c', os.path.join(build.CSRC, 'icp.cu'),
+                                                        '-o', os.path.join(tmp, 'icp.o')],
+                           capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stderr
     text = r.stdout + r.stderr
-    for k in ('k_icp_init', 'k_icp_nn', 'k_icp_reduce', 'k_icp_update'):
-        block = text[text.index(k):]
-        stats = re.search(r'(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads', block)
-        assert stats and stats.groups()[1:] == ('0', '0'), (k, block[:400])
+    entries = re.findall(r"Compiling entry function '(\w+)'[^\n]*\n[^\n]*Function properties for \w+\n\s*(\d+) "
+                         r"bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", text)
+    assert len(entries) == len(ICP_KERNELS), [e[0] for e in entries]
+    stats = {}
+    for k in ICP_KERNELS:
+        hit = [e for e in entries if k + 'E' in e[0]]
+        assert len(hit) == 1, (k, [e[0] for e in entries])
+        stats[k] = hit[0][1:]
+    return text, stats
+
+
+def test_icp_kernels_do_not_spill():
+    """icp.cu's entry functions are exactly ICP_KERNELS; none spills, nor does any device function they call."""
+    text, stats = icp_ptxas()
+    for k, (_, st, ld) in stats.items():
+        assert (st, ld) == ('0', '0'), (k, st, ld)
+    assert set(re.findall(r'bytes spill (?:stores|loads)', text)) and \
+        set(re.findall(r'(\d+) bytes spill (?:stores|loads)', text)) == {'0'}
+
+
+def test_icp_kernels_have_no_stack_frame():
+    """Every ICP kernel but the two updates runs without a stack frame: in generalized ICP's reduction that means the
+    unsorted Jacobi sweeps keep M, A and V in registers."""
+    _, stats = icp_ptxas()
+    for k in ICP_KERNELS[:6]:
+        assert stats[k][0] == '0', (k, stats[k])
