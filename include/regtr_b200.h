@@ -631,6 +631,58 @@ int regtr_estimate_normals(const double* xyz, const int32_t* offs, int C, int n_
                            int max_nn, double* normals, int32_t* counts, uint32_t* status, void* ws, size_t ws_bytes,
                            void* state, size_t state_bytes, void* stream);
 
+/* RANSAC over correspondences of B pairs (Open3D's registration_ransac_based_on_correspondence with
+ * TransformationEstimationPointToPoint(false), CorrespondenceCheckerBasedOnEdgeLength(edge_length),
+ * CorrespondenceCheckerBasedOnDistance(distance) and RANSACConvergenceCriteria(max_iteration, confidence)), with one
+ * deterministic sequential rule in place of Open3D's OpenMP schedule.
+ * xyz (n_cap,3) float64 stacked src_0..src_{B-1}, tgt_0..tgt_{B-1} with offs (2B+1) i32 (the validation clouds);
+ * corr_src / corr_tgt (m_cap,3) float64, pair b's correspondences (a_i, c_i) in rows [coffs[b], coffs[b+1]) (coffs
+ * (B+1) i32); corr_mask (m_cap) u8, nullable: the correspondences with a non-zero byte take part.  The valid ones,
+ * in their original order, are 0..n-1.  Per pair:
+ *   n < ransac_n or max_iteration = 0: Open3D's empty result.  Otherwise hypotheses k = 0, 1, ... while k < est_k
+ *   (est_k = max_iteration at first).  Hypothesis k draws index j < ransac_n as mulhi32(w, n), w word j & 3 of
+ *   Philox4x32-10 at counter (k, pair_base + b, j >> 2, 0x52534143) with key (seed lo, seed hi), with replacement.
+ *   It is rejected by a repeated index; by the edge-length checker (edge_length > 0): for a pair i < j of the sample,
+ *   |a_i - a_j| < |c_i - c_j| edge_length or |c_i - c_j| < |a_i - a_j| edge_length; by Umeyama without scaling on
+ *   the sample (means, Sigma = sum (c - mc)(a - ma)^T / n, float64 Jacobi SVD, reflection fix, t = mc - R ma) having
+ *   S[1] <= 1e-12 S[0]; or by the distance checker (distance > 0): |T a_i - c_i| > distance for a sample point.
+ *   (Norms are sqrt((dx dx + dy dy) + dz dz) without contraction.)  Otherwise it is validated: the source moved by T
+ *   (((r0 x + r1 y) + r2 z) + t), the matches of regtr_overlap_nn (nearest target with d^2 < max_dist^2, ties to the
+ *   lowest index), fitness = k / n_src, rmse = sqrt(sum d^2 / k); sum d^2 in a fixed order (blocks of 1024 source
+ *   points summed as regtr_registration_fit sums a cloud, the blocks by 32 strided chains and a butterfly), so a cloud
+ *   of up to 1024 points gets regtr_registration_fit's bits.  It replaces the best (fitness 0, rmse 0, identity at
+ *   first) when its fitness is higher, or equal with a lower rmse; then d = log(1 - confidence) / log(1 - f^ransac_n)
+ *   (f^n as n - 1 products) sets est_k = ceil(d) when 0 <= d < est_k (d = -inf, a fitness too small for 1 - f^n to
+ *   differ from 1, leaves est_k alone).
+ * pose_out (B,3,4) float64 = the best T; result (B,5) float64 = (fitness, rmse, hypotheses walked, hypotheses
+ * validated, index of the best hypothesis or -1).  A moved source coordinate of a validated hypothesis, or a target
+ * coordinate, beyond regtr_overlap_coord_bound(max_dist, cell), or not finite, raises REGTR_STATUS_RANGE.
+ * Launches: 2 + 4 (the targets' cell list, cell = max_dist (1 + 1e-3) in fp32) + 3 per chunk, the chunks being
+ * first_chunk 2^c hypotheses, at most REGTR_RANSAC_CHUNK_MAX, the last cut at max_iteration; no host synchronisation.
+ * The result is bit-identical for every first_chunk, and for a pair alone or in a batch with the same pair_base + b.
+ * REGTR_ERR_ARG: ransac_n outside 3..REGTR_RANSAC_MAX_N, max_dist not > 0, confidence outside [0, 1], a negative or
+ * non-finite edge_length / distance, first_chunk outside 1..REGTR_RANSAC_CHUNK_MAX, a negative max_iteration or
+ * pair_base.  ws: regtr_ransac_ws_bytes(n_cap, m_cap, B, max_iteration, first_chunk); state: regtr_icp_state_bytes(n_cap)
+ * (ZERO before the first call; every call leaves it zero). */
+#define REGTR_RANSAC_MAX_N 16
+#define REGTR_RANSAC_CHUNK_MAX 8192
+typedef struct {
+    int max_iteration;                       /* hypotheses at most [100000] */
+    double confidence;                       /* in [0, 1] [0.999] */
+    int ransac_n;                            /* sample size, 3..REGTR_RANSAC_MAX_N [3] */
+    double edge_length;                      /* edge-length checker's similarity threshold, 0 = off [0.9] */
+    double distance;                         /* distance checker's threshold, 0 = off [0] */
+    unsigned long long seed;                 /* Philox key */
+    int pair_base;                           /* global index of pair 0 in the draws */
+    int first_chunk;                         /* hypotheses of the first chunk, 1..REGTR_RANSAC_CHUNK_MAX [256] */
+} regtr_ransac_options;
+
+size_t regtr_ransac_ws_bytes(int n_cap, int m_cap, int B, int max_iteration, int first_chunk);
+int regtr_ransac(const double* xyz, const int32_t* offs, int B, int n_cap, const double* corr_src,
+                 const double* corr_tgt, const int32_t* coffs, const uint8_t* corr_mask, int m_cap, double max_dist,
+                 float cell, const regtr_ransac_options* opt, double* pose_out, double* result, uint32_t* status,
+                 void* ws, size_t ws_bytes, void* state, size_t state_bytes, void* stream);
+
 /* ---- pose graph ------------------------------------------------------------------- */
 
 #define REGTR_POSE_GRAPH_MAX_NODES 256

@@ -463,6 +463,103 @@ def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None, me
     return run
 
 
+def ransac_refine(pred, src_list, tgt_list, radius: float, max_iteration: int = 100000, confidence: float = 0.999,
+                  ransac_n: int = 3, edge_length: float = 0.9, distance: float = None, overlap: float = 0.5,
+                  seed: int = 0, pair_base: int = 0, ransac=None, correspondences=None):
+    """A robust pose for every pair of a forward's output `pred`: RANSAC (`ops.ransac`, max correspondence distance
+    `radius`, validated on src_list / tgt_list) over RegTR's two-way correspondences with predicted overlap above
+    `overlap` (`ops.regtr_correspondences`).  -> ransac's (pose (B,3,4), result (B,5)).
+    ransac(src_list, tgt_list, corr_src, corr_tgt, radius, max_iteration, ...) and correspondences(pred, overlap)
+    default to the `ops` functions."""
+    if ransac is None:
+        from .ops import ransac
+    if correspondences is None:
+        from .ops import regtr_correspondences as correspondences
+    corr_src, corr_tgt, corr_mask = correspondences(pred, overlap)
+    return ransac(src_list, tgt_list, corr_src, corr_tgt, radius, max_iteration, confidence=confidence,
+                  ransac_n=ransac_n, edge_length=edge_length, distance=distance, corr_mask=corr_mask, seed=seed,
+                  pair_base=pair_base)
+
+
+def add_ransac_arguments(ap, ransac_help: str):
+    """The RANSAC flags of a command line, for `ransac_refine`: --ransac R (help text ransac_help), --ransac_iters,
+    --ransac_confidence, --ransac_n, --ransac_edge, --ransac_dist, --ransac_overlap and --ransac_seed."""
+    ap.add_argument('--ransac', type=float, metavar='R', help=ransac_help)
+    ap.add_argument('--ransac_iters', type=int, default=100000, help='RANSAC hypotheses at most (with --ransac)')
+    ap.add_argument('--ransac_confidence', type=float, default=0.999,
+                    help='RANSAC stops early once this confidence is reached, in [0, 1]')
+    ap.add_argument('--ransac_n', type=int, default=3, help='Correspondences per RANSAC sample, 3..16')
+    ap.add_argument('--ransac_edge', type=float, default=0.9,
+                    help='Edge-length checker\'s similarity threshold (0: off)')
+    ap.add_argument('--ransac_dist', type=float, metavar='D',
+                    help='Distance checker\'s threshold (default: off)')
+    ap.add_argument('--ransac_overlap', type=float, default=0.5,
+                    help='Correspondences whose predicted overlap is above this take part in RANSAC')
+    ap.add_argument('--ransac_seed', type=int, default=0, help='Seed of the RANSAC samples')
+
+
+def check_ransac_arguments(ap, opt):
+    """Reject, as a usage error, RANSAC options `ops.ransac` would refuse, before any model is loaded."""
+    from .ops import RANSAC_MAX_N
+    if opt.ransac is None:
+        return
+    if not opt.ransac > 0.0:
+        ap.error(f'--ransac {opt.ransac} must be > 0')
+    if not 3 <= opt.ransac_n <= RANSAC_MAX_N:
+        ap.error(f'--ransac_n {opt.ransac_n} must be in 3..{RANSAC_MAX_N}')
+    if not 0 <= opt.ransac_iters < 2 ** 31:
+        ap.error(f'--ransac_iters {opt.ransac_iters} must be >= 0')
+    if not 0.0 <= opt.ransac_confidence <= 1.0:
+        ap.error(f'--ransac_confidence {opt.ransac_confidence} must be in [0, 1]')
+    for flag, v in (('--ransac_edge', opt.ransac_edge), ('--ransac_dist', opt.ransac_dist)):
+        if v is not None and not (math.isfinite(v) and v >= 0.0):
+            ap.error(f'{flag} {v} must be a finite value >= 0')
+    if not 0 <= opt.ransac_seed < 2 ** 64:
+        ap.error(f'--ransac_seed {opt.ransac_seed} must be in [0, 2^64)')
+
+
+def ransac_kwargs(opt) -> Dict:
+    """`ransac_refine`'s keyword arguments from the parsed --ransac_* flags."""
+    return dict(max_iteration=opt.ransac_iters, confidence=opt.ransac_confidence, ransac_n=opt.ransac_n,
+                edge_length=opt.ransac_edge, distance=opt.ransac_dist, overlap=opt.ransac_overlap,
+                seed=opt.ransac_seed)
+
+
+def ransac_forward(forward_fn, radius: float, max_iteration: int = 100000, confidence: float = 0.999,
+                   ransac_n: int = 3, edge_length: float = 0.9, distance: float = None, overlap: float = 0.5,
+                   seed: int = 0, ransac=None, correspondences=None, icp_radius: float = None, icp_kwargs=None,
+                   icp=None, estimate_normals=None):
+    """Wrap `forward_fn(batch) -> pred` so that every pair's pose comes from RANSAC over the network's
+    correspondences (`ransac_refine` with these arguments, validated on the batch's full clouds): -> a NEW dict with
+    pred's entries, pose (1,B,3,4) float64 the RANSAC poses and pose_coarse (1,B,3,4) float64 the network's final
+    poses.  With icp_radius, ICP then starts from the RANSAC poses (Open3D's global-then-local pipeline:
+    `icp_refine` with icp_radius, icp_kwargs (its keyword arguments), icp and estimate_normals): pose is the refined
+    pose and pose_ransac the RANSAC one.  pred's own tensors are not written to."""
+    def run(batch):
+        pred = forward_fn(batch)
+        coarse = pred['pose'][-1].to(torch.float64)                     # (B,3,4), a new tensor
+        pose, _ = ransac_refine(pred, batch['src_xyz'], batch['tgt_xyz'], radius, max_iteration, confidence,
+                                ransac_n, edge_length, distance, overlap, seed, ransac=ransac,
+                                correspondences=correspondences)
+        pose = torch.as_tensor(pose, dtype=torch.float64, device=coarse.device).reshape(coarse.shape)
+        out = dict(pred)
+        out['pose_coarse'] = coarse[None]
+        if icp_radius is not None:
+            out['pose_ransac'] = pose[None]
+            pose, _ = icp_refine(batch['src_xyz'], batch['tgt_xyz'], pose, icp_radius, icp=icp,
+                                 estimate_normals=estimate_normals, **(icp_kwargs or {}))
+            pose = torch.as_tensor(pose, dtype=torch.float64, device=coarse.device).reshape(coarse.shape)
+        out['pose'] = pose[None]
+        return out
+    return run
+
+
+def icp_kwargs(opt) -> Dict:
+    """`icp_refine`'s keyword arguments from the parsed --icp_* / --normal_* flags (without the radius)."""
+    return dict(max_iteration=opt.icp_iters, method=opt.icp_method, normal_radius=opt.normal_radius,
+                normal_max_nn=opt.normal_max_nn, epsilon=opt.icp_epsilon, loss=opt.icp_loss, loss_k=opt.icp_loss_k)
+
+
 def run_3dmatch_benchmark(batches: Iterable[Dict], forward_fn, log_path: str, benchmark: str, gt_folder: str,
                           thresh_rot=10.0, thresh_trans=0.1):
     """`Trainer.test` + `GenericRegModel.test_step/test_epoch_end` for the 3DMatch benchmarks

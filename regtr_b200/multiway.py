@@ -4,6 +4,8 @@ registration after RegTR's pairwise poses).
     python -m regtr_b200.multiway FRAG_0 FRAG_1 ... --ckpt <logdir>/ckpt/model-best.pth [--config <yaml>] --out DIR
         [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized [--normal_radius NR]
          [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
+        [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
+         [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
         [--info_radius D] [--min_overlap 0.3] [--preference_loop_closure 1.0]
         [--voxel V] [--batch_pairs 8]
 
@@ -11,7 +13,9 @@ Fragments are given in sequence order, in any format `pointio` reads; fragment i
 scenes are numbered cloud_bin_0..N-1, so position is the benchmark index).  The config is found and the clouds are
 cropped as `register` does.  Every pair i < j is registered with source j and target i (the 3DMatch benchmark's
 direction) in eager forwards of --batch_pairs pairs, then refined by `ops.icp` with --icp as `register --icp` does
-(generalized ICP uses each fragment's normals as source and as target normals).
+(generalized ICP uses each fragment's normals as source and as target normals).  With --ransac R each pair's pose
+first comes from RANSAC over the network's correspondences (`ops.ransac`, as `register --ransac`), so that far loop
+closures with little overlap survive the network's outlier correspondences; ICP then starts from it.
 `ops.registration_information` at D (default: the config's overlap_radius) gives each pair its fit and information
 matrix.  Edge (source j, target i, X = the pair's pose): j = i + 1 is a certain odometry edge; any other pair is an
 uncertain loop-closure edge when Lambda[5,5] / min(n_j, n_i) >= --min_overlap (Open3D's reconstruction system's gate).
@@ -38,7 +42,8 @@ from typing import Dict, List, Sequence
 import numpy as np
 import torch
 
-from .eval import add_icp_arguments, check_icp_arguments, icp_refine
+from .eval import (add_icp_arguments, add_ransac_arguments, check_icp_arguments, check_ransac_arguments, icp_refine,
+                   ransac_kwargs, ransac_refine)
 
 
 def parser() -> argparse.ArgumentParser:
@@ -49,6 +54,8 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument('--config', help='Config file (default: config.yaml one level above the checkpoint directory)')
     ap.add_argument('--out', required=True, help='Output directory')
     add_icp_arguments(ap, 'Refine every pair by ICP, max correspondence distance R')
+    add_ransac_arguments(ap, 'Replace every pair\'s pose by RANSAC over the predicted correspondences, max '
+                             'correspondence distance R (before ICP with --icp)')
     ap.add_argument('--info_radius', type=float, metavar='D',
                     help='Radius of the information matrices and the line process (default: overlap_radius)')
     ap.add_argument('--min_overlap', type=float, default=0.3,
@@ -67,10 +74,13 @@ def all_pairs(n: int):
 def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8, icp_radius: float = None,
                    icp_iters: int = 30, icp_method: str = 'point_to_point', normal_radius: float = None,
                    normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
-                   icp_loss_k: float = None) -> np.ndarray:
+                   icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None) -> np.ndarray:
     """RegTR's final-layer pose of every pair (i, j) of `all_pairs`, source j -> target i, optionally refined by ICP
     (`eval.icp_refine` with icp_method, epsilon=icp_epsilon, loss=icp_loss, loss_k=icp_loss_k; the point-to-plane and
     generalized methods use every fragment's normals, estimated once).
+    With ransac_radius, the network's pose is first replaced by `eval.ransac_refine` at that radius (ransac_options:
+    its further keyword arguments), pair p of `all_pairs` drawing as pair p whatever batch_pairs; ICP then starts from
+    the RANSAC pose.
     fragments: (n,3) float64 host arrays (already cropped).  -> (P,3,4) float64."""
     from . import ops
     dev = model.device
@@ -86,6 +96,9 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
             chunk = pairs[a:a + batch_pairs]
             pred = model({'src_xyz': [dev_frags[j] for _, j in chunk], 'tgt_xyz': [dev_frags[i] for i, _ in chunk]})
             pose = pred['pose'][-1].double()
+            if ransac_radius is not None:
+                pose, _ = ransac_refine(pred, [fragments[j] for _, j in chunk], [fragments[i] for i, _ in chunk],
+                                        ransac_radius, pair_base=a, **(ransac_options or {}))
             if icp_radius is not None:
                 pose, _ = icp_refine([fragments[j] for _, j in chunk], [fragments[i] for i, _ in chunk], pose,
                                      icp_radius, icp_iters, icp_method, epsilon=icp_epsilon, loss=icp_loss,
@@ -190,6 +203,7 @@ def main(argv=None):
     ap = parser()
     opt = ap.parse_args(argv)
     check_icp_arguments(ap, opt)
+    check_ransac_arguments(ap, opt)
     from .config import load_config
     from .pointio import load_point_cloud
     from .register import config_path, crop, load_model
@@ -202,7 +216,8 @@ def main(argv=None):
     model = load_model(cfg, opt.ckpt)
     frags = [crop(cfg, np.asarray(load_point_cloud(f), dtype=np.float64)) for f in opt.fragments]
     T = register_pairs(model, frags, opt.batch_pairs, opt.icp, opt.icp_iters, opt.icp_method, opt.normal_radius,
-                       opt.normal_max_nn, opt.icp_epsilon, opt.icp_loss, opt.icp_loss_k)
+                       opt.normal_max_nn, opt.icp_epsilon, opt.icp_loss, opt.icp_loss_k, opt.ransac,
+                       ransac_kwargs(opt) if opt.ransac is not None else None)
     D = float(cfg['overlap_radius'] if opt.info_radius is None else opt.info_radius)
     res = optimize_scene(frags, T, D, opt.min_overlap, opt.preference_loop_closure)
     write_outputs(res, opt.out, scene_name(opt.fragments[0]), frags, opt.voxel)

@@ -1343,6 +1343,158 @@ def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iterat
     return pose, out
 
 
+RANSAC_MAX_N = 16                   # REGTR_RANSAC_MAX_N
+RANSAC_CHUNK_MAX = 8192             # REGTR_RANSAC_CHUNK_MAX
+
+
+class RansacOptions(ctypes.Structure):
+    """regtr_ransac_options (include/regtr_b200.h)."""
+    _fields_ = [('max_iteration', ctypes.c_int), ('confidence', ctypes.c_double), ('ransac_n', ctypes.c_int),
+                ('edge_length', ctypes.c_double), ('distance', ctypes.c_double), ('seed', ctypes.c_ulonglong),
+                ('pair_base', ctypes.c_int), ('first_chunk', ctypes.c_int)]
+
+
+def ransac_chunks(max_iteration: int, first_chunk: int = 256):
+    """The hypothesis chunks of one `ransac` call: [(first hypothesis, count)], first_chunk * 2^c hypotheses each, at
+    most RANSAC_CHUNK_MAX, the last one cut at max_iteration."""
+    out, start, c = [], 0, 0
+    while start < max_iteration:
+        size = min(int(first_chunk) << min(c, 20), RANSAC_CHUNK_MAX, max_iteration - start)
+        out.append((start, size))
+        start += size
+        c += 1
+    return out
+
+
+def _ransac_empty(max_correspondence_distance, ransac_n) -> bool:
+    """Open3D's early return of every pair: ransac_n < 3 or a radius that is not positive."""
+    return int(ransac_n) < 3 or not float(max_correspondence_distance) > 0.0
+
+
+def ransac_launches(max_iteration: int, first_chunk: int = 256, ransac_n: int = 3,
+                    max_correspondence_distance: float = 1.0) -> int:
+    """Kernel launches of one `ransac` call: the set-up (2), the targets' cell list (4), then 3 per chunk; none when
+    every pair returns Open3D's empty result for ransac_n < 3 or a radius that is not positive."""
+    if _ransac_empty(max_correspondence_distance, ransac_n):
+        return 0
+    return 6 + 3 * len(ransac_chunks(int(max_iteration), first_chunk))
+
+
+def _ransac_check(B, corr_src, corr_tgt, corr_mask, max_iteration, confidence, ransac_n, edge_length, distance, seed,
+                  pair_base, first_chunk):
+    """ValueError for every argument `ransac` rejects, before anything touches the device."""
+    def real(v):
+        return isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, bool)
+    if len(corr_src) != B or len(corr_tgt) != B:
+        raise ValueError(f'ransac: {len(corr_src)} / {len(corr_tgt)} correspondence arrays for {B} pairs')
+    if corr_mask is not None and len(corr_mask) != B:
+        raise ValueError(f'ransac: {len(corr_mask)} correspondence masks for {B} pairs')
+    for b in range(B):
+        a, c = corr_src[b], corr_tgt[b]
+        if len(a.shape) != 2 or a.shape[1] != 3 or tuple(a.shape) != tuple(c.shape):
+            raise ValueError(f'ransac: pair {b}: correspondences {tuple(a.shape)} and {tuple(c.shape)}, expected two '
+                             f'(m,3) arrays')
+        if corr_mask is not None and tuple(corr_mask[b].shape) != (a.shape[0],):
+            raise ValueError(f'ransac: pair {b}: mask {tuple(corr_mask[b].shape)} for {a.shape[0]} correspondences')
+    if not (real(max_iteration) and int(max_iteration) == max_iteration and 0 <= max_iteration < 2 ** 31):
+        raise ValueError(f'ransac: max_iteration {max_iteration!r} must be an integer in [0, 2^31)')
+    if not (real(confidence) and 0.0 <= float(confidence) <= 1.0):
+        raise ValueError(f'ransac: confidence {confidence!r} must be in [0, 1]')
+    if not (real(ransac_n) and int(ransac_n) == ransac_n and int(ransac_n) <= RANSAC_MAX_N):
+        raise ValueError(f'ransac: ransac_n {ransac_n!r} must be an integer <= {RANSAC_MAX_N}')
+    for name, v in (('edge_length', edge_length), ('distance', distance)):
+        if v is not None and not (real(v) and math.isfinite(float(v)) and float(v) >= 0.0):
+            raise ValueError(f'ransac: {name} {v!r} must be None or a finite value >= 0 (0 or None: checker off)')
+    if not (real(seed) and int(seed) == seed and 0 <= int(seed) < 2 ** 64):
+        raise ValueError(f'ransac: seed {seed!r} must be an integer in [0, 2^64)')
+    if not (real(pair_base) and int(pair_base) == pair_base and 0 <= int(pair_base) < 2 ** 31 - B):
+        raise ValueError(f'ransac: pair_base {pair_base!r} must be an integer >= 0')
+    if not (real(first_chunk) and int(first_chunk) == first_chunk and 1 <= int(first_chunk) <= RANSAC_CHUNK_MAX):
+        raise ValueError(f'ransac: first_chunk {first_chunk!r} must be an integer in 1..{RANSAC_CHUNK_MAX}')
+
+
+def ransac(src_list, tgt_list, corr_src, corr_tgt, max_correspondence_distance: float, max_iteration: int = 100000,
+           confidence: float = 0.999, ransac_n: int = 3, edge_length: float = 0.9, distance: float = None,
+           corr_mask=None, seed: int = 0, pair_base: int = 0, first_chunk: int = 256, status=None):
+    """RANSAC over correspondences of B pairs (regtr_ransac): Open3D's registration_ransac_based_on_correspondence
+    with TransformationEstimationPointToPoint(False), ransac_n, the checkers CorrespondenceCheckerBasedOnEdgeLength
+    (edge_length) and CorrespondenceCheckerBasedOnDistance(distance) (0 or None: that checker is off) and
+    RANSACConvergenceCriteria(max_iteration, confidence), with the library's deterministic sequential rule
+    (include/regtr_b200.h, tests/ransac_oracle.py).
+    src_list / tgt_list: B clouds (n,3) each, the validation clouds (numpy or torch, any float dtype; stacked in float64
+    on the device).  corr_src / corr_tgt: B (m,3) arrays each, correspondence i of pair b being corr_src[b][i] ->
+    corr_tgt[b][i] (Open3D's index form is src[corres[:,0]], tgt[corres[:,1]]); corr_mask: None or B (m,) boolean
+    arrays, the correspondences that take part.  seed and pair_base + b key the draws, so a pair gets the same result
+    alone or in a batch; first_chunk only sets the launch schedule, never the result.
+    -> (pose (B,3,4) float64, result (B,5) float64 = fitness, inlier_rmse, hypotheses walked, hypotheses validated,
+    index of the winning hypothesis or -1), both device tensors.  ransac_n < 3 or a radius that is not positive gives
+    every pair Open3D's empty result (identity, zeros, -1) without a launch.
+    No host sync unless status is None: then a word of this call is read and a coordinate of a moved source or of a
+    target beyond `overlap_coord_bound(max_correspondence_distance)` raises RegtrLibError; with the caller's word,
+    `check_fit_status` does that where the caller syncs."""
+    B = len(src_list)
+    if B == 0 or len(tgt_list) != B:
+        raise ValueError('ransac: expected as many source as target clouds, at least one pair')
+    corr_src = [torch.as_tensor(c) for c in corr_src]
+    corr_tgt = [torch.as_tensor(c) for c in corr_tgt]
+    corr_mask = None if corr_mask is None else [torch.as_tensor(m) for m in corr_mask]
+    _ransac_check(B, corr_src, corr_tgt, corr_mask, max_iteration, confidence, ransac_n, edge_length, distance, seed,
+                  pair_base, first_chunk)
+    r = float(max_correspondence_distance)
+    dev = next((c.device for c in corr_src if c.is_cuda), None)
+    xyz, offs, lens = _stack_pairs(src_list, tgt_list, 'ransac', dev)
+    dev = xyz.device
+    pose = torch.zeros((B, 3, 4), dtype=torch.float64, device=dev)
+    out = torch.zeros((B, 5), dtype=torch.float64, device=dev)
+    if _ransac_empty(r, ransac_n):
+        pose[:, 0, 0] = pose[:, 1, 1] = pose[:, 2, 2] = 1.0
+        out[:, 4] = -1.0
+        return pose, out
+    L = _lib.load()
+    ms = [int(c.shape[0]) for c in corr_src]
+    m = sum(ms)
+    ca = torch.empty((max(m, 1), 3), dtype=torch.float64, device=dev)
+    cc = torch.empty((max(m, 1), 3), dtype=torch.float64, device=dev)
+    mask = None if corr_mask is None else torch.empty(max(m, 1), dtype=torch.uint8, device=dev)
+    a = 0
+    for b, ln in enumerate(ms):
+        ca[a:a + ln].copy_(corr_src[b].to(dev, torch.float64))
+        cc[a:a + ln].copy_(corr_tgt[b].to(dev, torch.float64))
+        if mask is not None:
+            mask[a:a + ln].copy_(corr_mask[b].to(dev) != 0)
+        a += ln
+    coffs = make_offsets(ms, dev)
+    opt = RansacOptions(int(max_iteration), float(confidence), int(ransac_n), float(edge_length or 0.0),
+                        float(distance or 0.0), int(seed), int(pair_base), int(first_chunk))
+    n = sum(lens)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    ws = workspace(L.regtr_ransac_ws_bytes(n, m, B, int(max_iteration), int(first_chunk)), dev)
+    state = workspace(L.regtr_icp_state_bytes(n), dev, 'scan_state', zero=True)
+    _lib.check(L.regtr_ransac(_p(xyz), _p(offs), B, n, _p(ca), _p(cc), _p(coffs), _p(mask), m, r, overlap_cell(r),
+                              ctypes.addressof(opt), _p(pose), _p(out), _p(status), _p(ws), ws.numel(), _p(state),
+                              state.numel(), _stream()), 'regtr_ransac')
+    _count(ransac_launches(max_iteration, first_chunk))
+    if own:
+        check_fit_status(status, r, 'ransac')
+    return pose, out
+
+
+def regtr_correspondences(pred, threshold: float = 0.5):
+    """The two-way correspondence set of RegTR's weighted Kabsch, from a forward's output `pred`, per pair b:
+    the final decoder layer's src_kp -> src_kp_warped followed by tgt_kp_warped -> tgt_kp, and the mask
+    sigmoid(overlap) > threshold of the same rows.  -> (corr_src, corr_tgt, corr_mask), B device tensors each
+    ((m,3) float32, (m,3) float32, (m,) bool), for `ransac`.  No host sync."""
+    corr_src, corr_tgt, corr_mask = [], [], []
+    for b in range(len(pred['src_kp'])):
+        corr_src.append(torch.cat([pred['src_kp'][b], pred['tgt_kp_warped'][b][-1]], 0))
+        corr_tgt.append(torch.cat([pred['src_kp_warped'][b][-1], pred['tgt_kp'][b]], 0))
+        logit = torch.cat([pred['src_overlap'][b][-1][:, 0], pred['tgt_overlap'][b][-1][:, 0]], 0)
+        corr_mask.append(torch.sigmoid(logit) > threshold)
+    return corr_src, corr_tgt, corr_mask
+
+
 NORMALS_MAX_NN = 64
 
 

@@ -4,6 +4,8 @@
         [--threshold 0.5] [--fit_radius R] [--out DIR]
         [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized [--normal_radius NR]
          [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
+        [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
+         [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
 
 SRC / TGT: .ply, .pth, .bin or .npy (regtr_b200.pointio).  The config is the config.yaml one level above the
 checkpoint's directory, the layout `python -m regtr_b200.train` writes, unless --config names another.  Instead of the
@@ -24,8 +26,16 @@ generalized estimates the normals of both cropped clouds in one call and runs Op
 Open3D's robust kernel of that name;
 pose.txt, src_registered.ply and fit then use the refined pose, result.npz gains pose_coarse (the network's final
 pose), pose_icp (the refined one) and icp (4,) = fitness, inlier_rmse, correspondences, iterations.
+With --ransac R the final decoder layer's pose is replaced by RANSAC over the network's two-way correspondences with
+predicted overlap above --ransac_overlap (`ops.ransac`, Open3D's registration_ransac_based_on_correspondence with max
+correspondence distance R on the cropped full-resolution clouds, --ransac_iters hypotheses at most, confidence
+--ransac_confidence, --ransac_n correspondences per sample, the edge-length checker at --ransac_edge and the distance
+checker at --ransac_dist); with --icp as well, ICP starts from the RANSAC pose (Open3D's global-then-local pipeline).
+result.npz then gains pose_coarse, pose_ransac (3,4) float64 and ransac (5,) = fitness, inlier_rmse, hypotheses
+walked, hypotheses validated, winning hypothesis.
 One JSON line on stdout: the pose, the four fit numbers and the point counts (with --icp, also icp_fitness, icp_rmse,
-icp_iterations, icp_radius and icp_method, and icp_loss, icp_loss_k and icp_epsilon when they are given).
+icp_iterations, icp_radius and icp_method, and icp_loss, icp_loss_k and icp_epsilon when they are given; with --ransac,
+ransac_fitness, ransac_rmse, ransac_iterations, ransac_validations and ransac_radius).
 """
 from __future__ import annotations
 
@@ -38,7 +48,8 @@ from typing import Dict
 import numpy as np
 import torch
 
-from .eval import add_icp_arguments, check_icp_arguments, icp_refine
+from .eval import (add_icp_arguments, add_ransac_arguments, check_icp_arguments, check_ransac_arguments, icp_refine,
+                   ransac_kwargs, ransac_refine)
 
 
 def parser() -> argparse.ArgumentParser:
@@ -52,6 +63,8 @@ def parser() -> argparse.ArgumentParser:
                     help='Keypoints with predicted overlap above this go to src_kp.ply / src_kp_warped.ply')
     ap.add_argument('--fit_radius', type=float, help='Inlier radius of the fitness / RMSE (default: overlap_radius)')
     add_icp_arguments(ap, 'Refine the pose with point-to-point ICP, max correspondence distance R (default: no ICP)')
+    add_ransac_arguments(ap, 'Replace the pose by RANSAC over the predicted correspondences, max correspondence '
+                             'distance R (default: no RANSAC; before ICP with --icp)')
     ap.add_argument('--out', default='.', help='Output directory')
     return ap
 
@@ -81,14 +94,17 @@ def load_model(cfg, ckpt: str, device=None):
 def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: float = None,
              icp_radius: float = None, icp_iters: int = 30, icp_method: str = 'point_to_point',
              normal_radius: float = None, normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
-             icp_loss_k: float = None) -> Dict:
+             icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None) -> Dict:
     """Crop, forward and fit one pair.  src_xyz / tgt_xyz (N,3) float64 host arrays.
     -> dict of host arrays: src_xyz / tgt_xyz (cropped, float64), pose (L,3,4) fp32, src_kp, src_kp_warped (final
     layer), src_overlap (sigmoid of the final layer's logit, (n,)), the same for tgt, fit (4,) float64.
     icp_radius: refine the final layer's pose by ICP on the cropped clouds (`eval.icp_refine` with icp_method, at most
     icp_iters iterations, and normal_radius, normal_max_nn, icp_epsilon, icp_loss and icp_loss_k); fit is then that of
     the refined pose, and the dict gains pose_coarse (3,4) fp32 (the network's final pose), pose_icp (3,4) float64 and
-    icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations."""
+    icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations.
+    ransac_radius: first replace the final layer's pose by `eval.ransac_refine` at that radius on the cropped clouds,
+    with ransac_options its further keyword arguments (ICP then starts from it); the dict gains pose_coarse,
+    pose_ransac (3,4) float64 and ransac (5,) float64 = fitness, inlier_rmse, walked, validated, winner."""
     from . import ops
     src_xyz = crop(cfg, np.asarray(src_xyz, dtype=np.float64))
     tgt_xyz = crop(cfg, np.asarray(tgt_xyz, dtype=np.float64))
@@ -101,13 +117,19 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
         radius = float(cfg['overlap_radius'] if fit_radius is None else fit_radius)
         status = ops.new_status(dev)
         final = pose[-1:]
+        if ransac_radius is not None:
+            final, ransac = ransac_refine(out, [src_xyz], [tgt_xyz], ransac_radius, **(ransac_options or {}))
+            pose_ransac = final
         if icp_radius is not None:
-            final, icp = icp_refine([src_xyz], [tgt_xyz], pose[-1:], icp_radius, icp_iters, icp_method, normal_radius,
+            final, icp = icp_refine([src_xyz], [tgt_xyz], final, icp_radius, icp_iters, icp_method, normal_radius,
                                     normal_max_nn, icp_epsilon, icp_loss, icp_loss_k)
         fit = ops.registration_fit([src_xyz], [tgt_xyz], final, radius, status)
         res = {'src_xyz': src_xyz, 'tgt_xyz': tgt_xyz, 'pose': pose.cpu().numpy()}
         if icp_radius is not None:
             res.update(pose_coarse=res['pose'][-1], pose_icp=final[0].cpu().numpy(), icp=icp[0].cpu().numpy())
+        if ransac_radius is not None:
+            res.update(pose_coarse=res['pose'][-1], pose_ransac=pose_ransac[0].cpu().numpy(),
+                       ransac=ransac[0].cpu().numpy())
         for side in ('src', 'tgt'):
             res[f'{side}_kp'] = out[f'{side}_kp'][0].cpu().numpy()
             res[f'{side}_kp_warped'] = out[f'{side}_kp_warped'][0][-1].cpu().numpy()
@@ -128,15 +150,27 @@ def pose_text(pose34) -> str:
     return ''.join('\t'.join(map('{0:.12f}'.format, row)) + '\n' for row in pose44(pose34))
 
 
+def final_pose(res: Dict):
+    """The pose `register` settles on: ICP's, else RANSAC's, else the final decoder layer's."""
+    for k in ('pose_icp', 'pose_ransac'):
+        if k in res:
+            return res[k]
+    return res['pose'][-1]
+
+
 def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
     from .pointio import write_ply
     os.makedirs(out_dir, exist_ok=True)
-    final = res['pose_icp'] if 'pose_icp' in res else res['pose'][-1]
+    final = final_pose(res)
     with open(os.path.join(out_dir, 'pose.txt'), 'w') as fh:
         fh.write(pose_text(final))
     keys = ('pose', 'src_kp', 'src_kp_warped', 'src_overlap', 'tgt_kp', 'tgt_kp_warped', 'tgt_overlap', 'fit')
+    if 'pose_coarse' in res:
+        keys += ('pose_coarse',)
+    if 'pose_ransac' in res:
+        keys += ('pose_ransac', 'ransac')
     if 'pose_icp' in res:
-        keys += ('pose_coarse', 'pose_icp', 'icp')
+        keys += ('pose_icp', 'icp')
     np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
     p = final.astype(np.float64)
     write_ply(os.path.join(out_dir, 'src_registered.ply'), res['src_xyz'] @ p[:, :3].T + p[:, 3])
@@ -150,6 +184,7 @@ def main(argv=None):
     ap = parser()
     opt = ap.parse_args(argv)
     check_icp_arguments(ap, opt)
+    check_ransac_arguments(ap, opt)
     from .config import load_config
     from .pointio import load_point_cloud
     cfg_file = config_path(opt.ckpt, opt.config)
@@ -159,10 +194,10 @@ def main(argv=None):
     model = load_model(cfg, opt.ckpt)
     res = register(model, cfg, load_point_cloud(opt.src), load_point_cloud(opt.tgt), opt.fit_radius, opt.icp,
                    opt.icp_iters, opt.icp_method, opt.normal_radius, opt.normal_max_nn, opt.icp_epsilon,
-                   opt.icp_loss, opt.icp_loss_k)
+                   opt.icp_loss, opt.icp_loss_k, opt.ransac, ransac_kwargs(opt) if opt.ransac is not None else None)
     n_shown = write_outputs(res, opt.out, opt.threshold)
     f = [float(v) for v in res['fit']]
-    line = {'pose': pose44(res['pose_icp'] if opt.icp is not None else res['pose'][-1]).tolist(),
+    line = {'pose': pose44(final_pose(res)).tolist(),
             'fitness_src': f[0], 'rmse_src': f[1],
             'fitness_tgt': f[2], 'rmse_tgt': f[3], 'n_src': int(res['src_xyz'].shape[0]),
             'n_tgt': int(res['tgt_xyz'].shape[0]), 'n_src_kp': int(res['src_kp'].shape[0]),
@@ -176,6 +211,10 @@ def main(argv=None):
             line.update(icp_loss=opt.icp_loss, icp_loss_k=float(opt.icp_loss_k))
         if opt.icp_method == 'generalized':
             line.update(icp_epsilon=float(opt.icp_epsilon))
+    if opt.ransac is not None:
+        rs = [float(v) for v in res['ransac']]
+        line.update(ransac_fitness=rs[0], ransac_rmse=rs[1], ransac_iterations=int(rs[2]),
+                    ransac_validations=int(rs[3]), ransac_radius=float(opt.ransac))
     print(json.dumps(line))
     return res
 

@@ -4,11 +4,16 @@
         --gt <datasets/3dmatch/benchmarks/3DMatch> --ckpt <model.pth> --out logs/3DMatch [--icp R [--icp_iters N]
         [--icp_method point_to_plane|generalized [--normal_radius NR] [--normal_max_nn 30] [--icp_epsilon 1e-3]
         [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
+        [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
+         [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
 
 --icp R refines every final pose by ICP on the full clouds (`ops.icp`, max correspondence distance R; point-to-point,
 or point-to-plane against target normals from `ops.estimate_normals` at NR, default 2 R, or generalized ICP on the
 normals of both clouds, optionally under a robust loss): est.log then holds the
 refined poses, and the metrics report both (`rot_err_deg` / `trans_err` refined, `*_coarse` the network's).
+--ransac R replaces every network pose by RANSAC over the network's correspondences with predicted overlap above
+--ransac_overlap (`ops.ransac`, max correspondence distance R, validated on the full clouds); with --icp as well, ICP
+starts from the RANSAC pose, and the metrics also report `*_ransac`.
 Needs the dataset and trained weights (neither is available offline: SURVEY.md 8f N1)."""
 import argparse, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -24,6 +29,8 @@ def parser():
     ap.add_argument('--ckpt', required=True); ap.add_argument('--out', default='logs'); ap.add_argument('--benchmark', default='3DMatch')
     ap.add_argument('--batch', type=int, default=1); ap.add_argument('--workers', type=int, default=4)
     E.add_icp_arguments(ap, 'Refine the poses by ICP with this max correspondence distance')
+    E.add_ransac_arguments(ap, 'Replace the poses by RANSAC over the predicted correspondences, max correspondence '
+                               'distance R (before ICP with --icp)')
     return ap
 
 
@@ -31,6 +38,7 @@ def main(argv=None):
     ap = parser()
     args = ap.parse_args(argv)
     E.check_icp_arguments(ap, args)
+    E.check_ransac_arguments(ap, args)
     dev = torch.device('cuda:0')
     cfg = get_config('3dmatch')
     model = RegTR(cfg).to(dev).eval()
@@ -39,9 +47,13 @@ def main(argv=None):
     runner = GraphedRegTR(model)
     ds = D.ThreeDMatchPairs(args.root, args.info, pin=True)
     batches = [list(range(i, min(i + args.batch, len(ds)))) for i in range(0, len(ds), args.batch)]
-    forward = (lambda b: runner(b)) if args.icp is None else E.icp_forward(
-        lambda b: runner(b), args.icp, args.icp_iters, method=args.icp_method, normal_radius=args.normal_radius,
-        normal_max_nn=args.normal_max_nn, epsilon=args.icp_epsilon, loss=args.icp_loss, loss_k=args.icp_loss_k)
+    if args.ransac is not None:
+        forward = E.ransac_forward(lambda b: runner(b), args.ransac, **E.ransac_kwargs(args), icp_radius=args.icp,
+                                   icp_kwargs=E.icp_kwargs(args))
+    else:
+        forward = (lambda b: runner(b)) if args.icp is None else E.icp_forward(
+            lambda b: runner(b), args.icp, args.icp_iters, method=args.icp_method, normal_radius=args.normal_radius,
+            normal_max_nn=args.normal_max_nn, epsilon=args.icp_epsilon, loss=args.icp_loss, loss_k=args.icp_loss_k)
     res = E.run_3dmatch_benchmark(D.PairStream(ds, batches, workers=args.workers), forward, args.out,
                                   args.benchmark, args.gt)
     print(res['summary']); print('registration recall', res['recall'])
