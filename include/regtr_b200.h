@@ -631,6 +631,49 @@ int regtr_estimate_normals(const double* xyz, const int32_t* offs, int C, int n_
                            int max_nn, double* normals, int32_t* counts, uint32_t* status, void* ws, size_t ws_bytes,
                            void* state, size_t state_bytes, void* stream);
 
+/* FPFH features of C stacked clouds (Open3D's ComputeFPFHFeature(KDTreeSearchParamHybrid(radius, max_nn)), with this
+ * library's tie and order rules).  xyz / normals (n_cap,3) float64 with offs (C+1) i32, offs[0] = 0, C <= 32767 (the
+ * normals of regtr_estimate_normals; a zero normal is allowed); cell = radius * (1 + 1e-3) rounded to fp32
+ * (ops.overlap_cell); 1 <= max_nn <= REGTR_FPFH_MAX_NN (else REGTR_ERR_ARG).  feature (n_cap,33) float64, rows >= offs[C]
+ * untouched.
+ *   Neighbours of point i: regtr_estimate_normals' rule (own cloud, d^2 strictly below radius^2, i included, the max_nn
+ *   smallest by (d^2, index)), entry 0 first.  Fewer than 2 neighbours: a zero row.
+ *   Pair feature (p1, n1, p2, n2), products and sums rounded one by one, dot products (x x + y y) + z z: d = p2 - p1
+ *   (zero feature when |d| = 0); a1 = n1.d / |d|, a2 = n2.d / |d|; when |a1| < |a2|, n1 <-> n2, d -> -d, f2 = -a2,
+ *   else f2 = a1; v = d x n1 (zero feature when |v| = 0), v /= |v|; w = n1 x v; f1 = v.n2; f0 = atan2(w.n2, n1.n2).
+ *   SPFH of i (count >= 2): entries k >= 1, in order, add 100 / (count - 1) to bins floor(11 (f0 + pi) / 2pi),
+ *   11 + floor(11 (f1 + 1) 0.5) and 22 + floor(11 (f2 + 1) 0.5), each floor clamped to 0..10.
+ *   FPFH of i (count >= 2): entries k >= 1 with d^2 != 0, in order, add val = spfh[j][b] / d^2 to feature[b] and to
+ *   sum[b / 11]; then feature[b] = feature[b] * (sum != 0 ? 100 / sum : 0) + spfh[i][b].
+ * counts (n_cap) i32, nullable: the neighbour count per point.  A |coordinate| beyond
+ * regtr_overlap_coord_bound(radius, cell), or not finite, raises REGTR_STATUS_RANGE.  1 + 4 + 3 launches whatever C;
+ * no value atomics, no host synchronisation: the result is bit-identical whether a cloud is passed alone or in a stack.
+ * ws: regtr_fpfh_ws_bytes(n_cap, max_nn); state: regtr_fpfh_state_bytes(n_cap) (ZERO before the first call; every
+ * call leaves it zero). */
+#define REGTR_FPFH_DIM 33
+#define REGTR_FPFH_MAX_NN 128
+size_t regtr_fpfh_ws_bytes(int n_cap, int max_nn);
+size_t regtr_fpfh_state_bytes(int n_cap);
+int regtr_fpfh(const double* xyz, const double* normals, const int32_t* offs, int C, int n_cap, double radius,
+               float cell, int max_nn, double* feature, int32_t* counts, uint32_t* status, void* ws, size_t ws_bytes,
+               void* state, size_t state_bytes, void* stream);
+
+/* Feature-space correspondences of B pairs (the matching of Open3D's registration_ransac_based_on_feature_matching).
+ * src_feat (offs_s[B],33) float64 with soffs (B+1) i32; tgt_feat (nt_cap,33) float64 and tgt_xyz (nt_cap,3) float64
+ * with toffs (B+1) i32; every pair has at most ns_max sources and nt_max targets.  Per pair, with
+ * d^2(i, j) = sum over k = 0..32 of (a_k - b_k)^2 accumulated in that order without contraction:
+ *   nn[i] (local target index) = the lowest (d^2, j) over the targets (-1 without targets), corr_tgt[i] = its point;
+ *   the reverse match of target j = the lowest (d^2, i) over the sources; match i is mutual when the reverse match of
+ *   nn[i] is i; n_mutual[b] = their number; mask[i] = mutual, or 1 for every match when mutual_filter = 0 or
+ *   n_mutual[b] < min_mutual (Open3D's fallback below 3 ransac_n).
+ * Features must be finite.  3 launches; no atomics, no host synchronisation; the result is bit-identical for a pair
+ * alone or in a batch.  ws: regtr_feature_match_ws_bytes(B, ns_max, nt_max, nt_cap). */
+size_t regtr_feature_match_ws_bytes(int B, int ns_max, int nt_max, int nt_cap);
+int regtr_feature_match(const double* src_feat, const int32_t* soffs, const double* tgt_feat, const double* tgt_xyz,
+                        const int32_t* toffs, int B, int ns_max, int nt_max, int nt_cap, int mutual_filter,
+                        int min_mutual, int32_t* nn, double* corr_tgt, uint8_t* mask, int32_t* n_mutual, void* ws,
+                        size_t ws_bytes, void* stream);
+
 /* RANSAC over correspondences of B pairs (Open3D's registration_ransac_based_on_correspondence with
  * TransformationEstimationPointToPoint(false), CorrespondenceCheckerBasedOnEdgeLength(edge_length),
  * CorrespondenceCheckerBasedOnDistance(distance) and RANSACConvergenceCriteria(max_iteration, confidence)), with one

@@ -4,7 +4,7 @@
 //
 // One cell list over the fp32 copy of every cloud is built once, then one warp per point selects its neighbours and
 // solves the 3x3 eigenproblem: 1 + 4 + 1 launches whatever C, no host synchronisation, no value atomics.
-#include "cellgrid.cuh"
+#include "neighbours.cuh"
 #include "rigid.cuh"
 
 extern "C" int regtr_cellgrid_build(const float* xyz, const int32_t* offs, int n_clouds, int n_cap, float cell,
@@ -31,12 +31,10 @@ __global__ void k_normals_init(const double* __restrict__ xyz, const int32_t* __
     if (!(fabs(x) <= bound && fabs(y) <= bound && fabs(z) <= bound)) atomicOr(status, REGTR_STATUS_RANGE);
 }
 
-// One warp per point, in index order.  Lanes 0..26 look up one stencil cell each and the candidates are flattened 32
-// wide, as in k_icp_nn.  The neighbours are the candidates with d2 = (dx dx + dy dy) + dz dz (float64, no
-// contraction) strictly below r2, the point itself included; the warp extracts the next-smallest (d2, index) key
-// max_nn times, so nothing depends on how many candidates lie within the radius.  Then, in that order, the mean and
-// the centred covariance (float64, sequential sums, / count), its smallest eigenvector (the right singular vector of
-// the smallest singular value of svd3_jacobi), normalised and flipped when n . p > 0.  Fewer than 3 neighbours: 0.
+// One warp per point, in index order: the neighbours of warp_select_neighbours (neighbours.cuh).  Then, in that order,
+// the mean and the centred covariance (float64, sequential sums, / count), its smallest eigenvector (the right singular
+// vector of the smallest singular value of svd3_jacobi), normalised and flipped when n . p > 0.  Fewer than 3
+// neighbours: 0.
 __global__ void __launch_bounds__(NRM_WARPS * 32)
 k_normals(const double* __restrict__ xyz, const int32_t* __restrict__ offs, int C, int n_cap,
           const CellSlot* __restrict__ table, int log2t, const float4* __restrict__ sxyzi, float cell, double r2,
@@ -46,69 +44,20 @@ k_normals(const double* __restrict__ xyz, const int32_t* __restrict__ offs, int 
     for (int qi = blockIdx.x * NRM_WARPS + warp; qi < n_cap && qi < n; qi += gridDim.x * NRM_WARPS) {
         const int c = regtr_cloud_of(offs, C, qi);
         const double qx = xyz[3 * qi + 0], qy = xyz[3 * qi + 1], qz = xyz[3 * qi + 2];
-        const int cx = regtr_cell_of((float)qx, cell), cy = regtr_cell_of((float)qy, cell),
-                  cz = regtr_cell_of((float)qz, cell);
-        int c_start = 0, c_cnt = 0;
-        if (lane < 27) {
-            const int x = cx + lane / 9 - 1, y = cy + (lane / 3) % 3 - 1, z = cz + lane % 3 - 1;
-            if (x >= -32767 && x <= 32767 && y >= -32767 && y <= 32767 && z >= -32767 && z <= 32767)
-                cell_lookup(table, log2t, regtr_pack_key(c, x, y, z), c_start, c_cnt);
-        }
-        int pre = c_cnt;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int v = __shfl_up_sync(0xffffffffu, pre, o);
-            if (lane >= o) pre += v;
-        }
-        const int total = __shfl_sync(0xffffffffu, pre, 31);
-        // selection: key s is the smallest (d2, index) above key s - 1; lane s % 32 keeps its index
-        double pd = -1.0;
-        int pj = -1, cnt = 0, sel0 = -1, sel1 = -1;
-        for (int s = 0; s < max_nn; ++s) {
-            double best = r2;
-            int bi = -1;
-            for (int base = 0; base < total; base += 32) {
-                const int t = base + lane;
-                int cellid = 0;
-#pragma unroll
-                for (int step = 16; step > 0; step >>= 1) {
-                    const int pv = __shfl_sync(0xffffffffu, pre, cellid + step - 1);
-                    if (pv <= t) cellid += step;
-                }
-                const int cell_pre = __shfl_sync(0xffffffffu, pre, cellid);
-                const int cell_cnt = __shfl_sync(0xffffffffu, c_cnt, cellid);
-                const int cell_start = __shfl_sync(0xffffffffu, c_start, cellid);
-                if (t < total) {
-                    const int j = __float_as_int(sxyzi[cell_start + (t - (cell_pre - cell_cnt))].w);
-                    const double dx = __dsub_rn(qx, xyz[3 * j + 0]), dy = __dsub_rn(qy, xyz[3 * j + 1]),
-                                 dz = __dsub_rn(qz, xyz[3 * j + 2]);
-                    const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-                    const bool above = d2 > pd || (d2 == pd && j > pj);
-                    if (d2 < r2 && above && (bi < 0 || d2 < best || (d2 == best && j < bi))) { best = d2; bi = j; }
-                }
-            }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const double ob = __shfl_xor_sync(0xffffffffu, best, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                if (oi >= 0 && (bi < 0 || ob < best || (ob == best && oi < bi))) { best = ob; bi = oi; }
-            }
-            if (bi < 0) break;                               // warp-uniform: every lane holds the same key
-            if (lane == (s & 31)) { if (s < 32) sel0 = bi; else sel1 = bi; }
-            pd = best; pj = bi; cnt = s + 1;
-        }
+        int sel[NRM_MAX_NN / 32];
+        const int cnt = warp_select_neighbours(xyz, table, log2t, sxyzi, cell, c, qx, qy, qz, r2, max_nn, lane, sel);
         double nx = 0.0, ny = 0.0, nz = 0.0;
         if (cnt >= 3) {
             double m[3] = {0.0, 0.0, 0.0};
             for (int s = 0; s < cnt; ++s) {
-                const int j = __shfl_sync(0xffffffffu, s < 32 ? sel0 : sel1, s & 31);
+                const int j = sel_at(sel, s);
                 for (int a = 0; a < 3; ++a) m[a] += xyz[3 * j + a];
             }
             const double inv = 1.0 / (double)cnt;
             for (int a = 0; a < 3; ++a) m[a] *= inv;
             double cxx = 0.0, cxy = 0.0, cxz = 0.0, cyy = 0.0, cyz = 0.0, czz = 0.0;
             for (int s = 0; s < cnt; ++s) {
-                const int j = __shfl_sync(0xffffffffu, s < 32 ? sel0 : sel1, s & 31);
+                const int j = sel_at(sel, s);
                 const double dx = xyz[3 * j + 0] - m[0], dy = xyz[3 * j + 1] - m[1], dz = xyz[3 * j + 2] - m[2];
                 cxx += dx * dx; cxy += dx * dy; cxz += dx * dz;
                 cyy += dy * dy; cyz += dy * dz; czz += dz * dz;

@@ -554,6 +554,113 @@ def ransac_forward(forward_fn, radius: float, max_iteration: int = 100000, confi
     return run
 
 
+def fpfh_downsample(clouds, voxel: float):
+    """`ops.grid_subsample(dense=False)` of C clouds at `voxel` in one call: the mean of every occupied voxel of a grid
+    anchored at the origin (Open3D's voxel_down_sample anchors its grid at the bounding box's minimum corner).
+    -> list of C (m,3) float32 device tensors."""
+    from . import ops
+    dev = torch.device('cuda', torch.cuda.current_device())
+    ts = [torch.as_tensor(c).to(dev, torch.float32) for c in clouds]
+    xyz = torch.cat(ts, 0).contiguous()
+    status = ops.new_status(dev)
+    out, offs = ops.grid_subsample(xyz, ops.make_offsets([t.shape[0] for t in ts], dev), len(ts), voxel, status,
+                                   dense=False)
+    word = int(status.item())
+    if word:
+        raise RuntimeError(f'fpfh: grid sub-sampling at {voxel} failed (status {word:#x})')
+    o = offs.tolist()
+    return [out[o[k]:o[k + 1]] for k in range(len(ts))]
+
+
+def fpfh_register(src_list, tgt_list, voxel: float, normal_radius: float = None, normal_max_nn: int = 30,
+                  fpfh_radius: float = None, fpfh_max_nn: int = 100, mutual_filter: bool = True,
+                  ransac_radius: float = None, max_iteration: int = 100000, confidence: float = 0.999,
+                  ransac_n: int = 3, edge_length: float = 0.9, distance: float = None, seed: int = 0,
+                  pair_base: int = 0, icp_radius: float = None, icp_kwargs=None) -> Dict:
+    """Classical global registration of B pairs without a network, Open3D's tutorial pipeline on the device:
+    `fpfh_downsample` at voxel V, `ops.estimate_normals` (normal_radius, default 2 V, normal_max_nn), `ops.fpfh`
+    (fpfh_radius, default 5 V, fpfh_max_nn), then `ops.ransac_feature_matching` at ransac_radius (default 1.5 V) with the
+    distance checker at `distance` (default: ransac_radius; 0: off), validated on the downsampled clouds.  With
+    icp_radius, `icp_refine` (icp_kwargs) then starts from the RANSAC poses on the full clouds.
+    -> dict: pose (B,3,4) float64 (the final poses), pose_fpfh (B,3,4) the RANSAC poses, ransac (B,5), n_mutual (B,),
+    src_down / tgt_down (B downsampled clouds), and icp (B,4) with icp_radius; device tensors."""
+    from . import ops
+    B = len(src_list)
+    down = fpfh_downsample(list(src_list) + list(tgt_list), voxel)
+    normals = ops.estimate_normals(down, 2.0 * voxel if normal_radius is None else normal_radius, normal_max_nn)
+    feats = ops.fpfh(down, normals, 5.0 * voxel if fpfh_radius is None else fpfh_radius, fpfh_max_nn)
+    r = 1.5 * voxel if ransac_radius is None else ransac_radius
+    pose, res, n_mutual = ops.ransac_feature_matching(
+        down[:B], down[B:], feats[:B], feats[B:], mutual_filter, r, ransac_n, max_iteration=max_iteration,
+        confidence=confidence, edge_length=edge_length, distance=r if distance is None else distance, seed=seed,
+        pair_base=pair_base)
+    out = dict(pose=pose, pose_fpfh=pose, ransac=res, n_mutual=n_mutual, src_down=down[:B], tgt_down=down[B:])
+    if icp_radius is not None:
+        out['pose'], out['icp'] = icp_refine(src_list, tgt_list, pose, icp_radius, **(icp_kwargs or {}))
+    return out
+
+
+def fpfh_forward(voxel: float, icp_radius: float = None, icp_kwargs=None, **fpfh_kwargs):
+    """A network-free `forward_fn(batch) -> pred` for `run_3dmatch_benchmark`: `fpfh_register` of the batch's full
+    clouds (voxel, fpfh_kwargs, and ICP after it with icp_radius / icp_kwargs) -> dict with pose (1,B,3,4) float64,
+    and pose_fpfh (1,B,3,4) (the RANSAC poses) when ICP follows."""
+    def run(batch):
+        res = fpfh_register(batch['src_xyz'], batch['tgt_xyz'], voxel, icp_radius=icp_radius, icp_kwargs=icp_kwargs,
+                            **fpfh_kwargs)
+        out = {'pose': torch.as_tensor(res['pose'], dtype=torch.float64)[None]}
+        if icp_radius is not None:
+            out['pose_fpfh'] = res['pose_fpfh'][None]
+        return out
+    return run
+
+
+def add_fpfh_arguments(ap):
+    """The FPFH flags of a command line, for `fpfh_register`: --fpfh V, --fpfh_radius, --fpfh_max_nn and
+    --fpfh_no_mutual."""
+    ap.add_argument('--fpfh', type=float, metavar='V',
+                    help='Register without a network: FPFH features of the clouds downsampled at voxel V, matched in '
+                         'feature space, then RANSAC (Open3D\'s global registration); no --ckpt')
+    ap.add_argument('--fpfh_radius', type=float, metavar='FR', help='FPFH feature radius (default: 5 V)')
+    ap.add_argument('--fpfh_max_nn', type=int, default=100, help='Neighbours at most of the FPFH feature, 1..128')
+    ap.add_argument('--fpfh_no_mutual', action='store_true',
+                    help='Use every forward feature match, not only the mutual ones')
+
+
+def check_fpfh_arguments(ap, opt):
+    """With --fpfh: reject --ckpt and bad FPFH values as usage errors, and fill in the defaults that depend on V
+    (--fpfh_radius 5 V, --ransac 1.5 V, --ransac_dist the --ransac radius).  Without it,
+    --ckpt is required.  Call before `check_ransac_arguments`."""
+    from .ops import FPFH_MAX_NN
+    if opt.fpfh is None:
+        if opt.ckpt is None:
+            ap.error('the following arguments are required: --ckpt')
+        return
+    if opt.ckpt is not None:
+        ap.error('--fpfh registers without a network: --ckpt is not allowed')
+    if not opt.fpfh > 0.0:
+        ap.error(f'--fpfh {opt.fpfh} must be > 0')
+    if not 1 <= opt.fpfh_max_nn <= FPFH_MAX_NN:
+        ap.error(f'--fpfh_max_nn {opt.fpfh_max_nn} must be in 1..{FPFH_MAX_NN}')
+    if opt.fpfh_radius is None:
+        opt.fpfh_radius = 5.0 * opt.fpfh
+    if not opt.fpfh_radius > 0.0:
+        ap.error(f'--fpfh_radius {opt.fpfh_radius} must be > 0')
+    if opt.ransac is None:
+        opt.ransac = 1.5 * opt.fpfh
+    if opt.ransac_dist is None:
+        opt.ransac_dist = opt.ransac
+
+
+def fpfh_kwargs(opt) -> Dict:
+    """`fpfh_register`'s keyword arguments from the parsed --fpfh_* / --ransac_* flags (without V and ICP, and without
+    --ransac_overlap, which has no meaning without a network; the normals are always estimated at 2 V, 30, and
+    --normal_* stays ICP's)."""
+    return dict(fpfh_radius=opt.fpfh_radius,
+                fpfh_max_nn=opt.fpfh_max_nn, mutual_filter=not opt.fpfh_no_mutual, ransac_radius=opt.ransac,
+                max_iteration=opt.ransac_iters, confidence=opt.ransac_confidence, ransac_n=opt.ransac_n,
+                edge_length=opt.ransac_edge, distance=opt.ransac_dist, seed=opt.ransac_seed)
+
+
 def icp_kwargs(opt) -> Dict:
     """`icp_refine`'s keyword arguments from the parsed --icp_* / --normal_* flags (without the radius)."""
     return dict(max_iteration=opt.icp_iters, method=opt.icp_method, normal_radius=opt.normal_radius,

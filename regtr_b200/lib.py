@@ -109,6 +109,11 @@ SIGNATURES = {
     'regtr_estimate_normals_ws_bytes': (_Z, [_I]),
     'regtr_estimate_normals_state_bytes': (_Z, [_I]),
     'regtr_estimate_normals': (_I, [_P, _P, _I, _I, _c.c_double, _F, _I, _P, _P, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_fpfh_ws_bytes': (_Z, [_I, _I]),
+    'regtr_fpfh_state_bytes': (_Z, [_I]),
+    'regtr_fpfh': (_I, [_P, _P, _P, _I, _I, _c.c_double, _F, _I, _P, _P, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_feature_match_ws_bytes': (_Z, [_I, _I, _I, _I]),
+    'regtr_feature_match': (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _Z, _P]),
     'regtr_train_augment_ws_bytes': (_Z, [_I, _I]),
     'regtr_train_augment_state_bytes': (_Z, [_I]),
     'regtr_train_augment': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _c.c_ulonglong, _c.c_ulonglong, _I, _c.c_double,

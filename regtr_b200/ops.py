@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import contextlib
 import ctypes
+import inspect
 import itertools
 import math
 
@@ -1552,6 +1553,163 @@ def estimate_normals(clouds, radius: float, max_nn: int = 30, status=None, retur
     if return_counts:
         return out, [counts[bounds[k]:bounds[k + 1]] for k in range(C)]
     return out
+
+
+FPFH_DIM = 33                       # REGTR_FPFH_DIM
+FPFH_MAX_NN = 128                   # REGTR_FPFH_MAX_NN
+
+
+def fpfh_launches() -> int:
+    """Kernel launches of one `fpfh` call: the set-up, the cell list (4), neighbour lists, SPFH and FPFH."""
+    return 8
+
+
+def feature_match_launches() -> int:
+    """Kernel launches of one `feature_match` call: the distance sweep, the reduction of its partial minima and the
+    mutual filter."""
+    return 3
+
+
+def _stack_clouds(ts, dev, width, what):
+    """C (n,width) arrays stacked in float64 on the device -> (stacked (max(n,1),width), lens)."""
+    lens = [int(c.shape[0]) for c in ts]
+    out = torch.empty((max(sum(lens), 1), width), dtype=torch.float64, device=dev)
+    a = 0
+    for c, ln in zip(ts, lens):
+        out[a:a + ln].copy_(c.to(dev, torch.float64))
+        a += ln
+    return out, lens
+
+
+def _split(t, lens):
+    bounds = np.concatenate([[0], np.cumsum(lens)]).astype(int)
+    return [t[bounds[k]:bounds[k + 1]] for k in range(len(lens))]
+
+
+def fpfh(clouds, normals, radius: float, max_nn: int = 100, status=None, return_counts: bool = False):
+    """FPFH features of C clouds (regtr_fpfh): Open3D's compute_fpfh_feature(KDTreeSearchParamHybrid(radius, max_nn))
+    with the library's rules (include/regtr_b200.h, tests/fpfh_oracle.py).
+    clouds / normals: C (n,3) arrays each, normals aligned with their cloud (e.g. `estimate_normals`), numpy or torch,
+    any float dtype; stacked in float64 on the device.
+    -> list of C (n,33) float64 device tensors; with return_counts also the list of (n,) int32 neighbour counts.
+    No host sync unless status is None: then a word of this call is read and a coordinate beyond
+    `overlap_coord_bound(radius)`, or not finite, raises RegtrLibError; with the caller's word, `check_fit_status`
+    does that where the caller syncs."""
+    r = float(radius)
+    if not r > 0.0 or not 1 <= int(max_nn) <= FPFH_MAX_NN:
+        raise ValueError(f'fpfh: radius {r} must be > 0 and max_nn {max_nn} in 1..{FPFH_MAX_NN}')
+    C = len(clouds)
+    if C == 0 or len(normals) != C:
+        raise ValueError(f'fpfh: {C} clouds and {len(normals)} normal arrays; expected as many, at least one')
+    ts = [torch.as_tensor(c) for c in clouds]
+    ns = [torch.as_tensor(c) for c in normals]
+    for c, m in zip(ts, ns):
+        if c.dim() != 2 or c.shape[1] != 3 or tuple(m.shape) != tuple(c.shape):
+            raise ValueError(f'fpfh: cloud {tuple(c.shape)} and normals {tuple(m.shape)}, expected two (n,3) arrays')
+    L = _lib.load()
+    dev = next((c.device for c in ts + ns if c.is_cuda), torch.device('cuda', torch.cuda.current_device()))
+    xyz, lens = _stack_clouds(ts, dev, 3, 'fpfh')
+    nrm, _ = _stack_clouds(ns, dev, 3, 'fpfh')
+    n = sum(lens)
+    offs = make_offsets(lens, dev)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    feat = torch.empty((max(n, 1), FPFH_DIM), dtype=torch.float64, device=dev)
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev) if return_counts else None
+    ws = workspace(L.regtr_fpfh_ws_bytes(n, int(max_nn)), dev)
+    state = workspace(L.regtr_fpfh_state_bytes(n), dev, 'scan_state', zero=True)
+    _lib.check(L.regtr_fpfh(_p(xyz), _p(nrm), _p(offs), C, n, r, overlap_cell(r), int(max_nn), _p(feat), _p(counts),
+                            _p(status), _p(ws), ws.numel(), _p(state), state.numel(), _stream()), 'regtr_fpfh')
+    _count(fpfh_launches())
+    if own:
+        check_fit_status(status, r, 'fpfh')
+    if return_counts:
+        return _split(feat, lens), _split(counts, lens)
+    return _split(feat, lens)
+
+
+def feature_match(src_feat, tgt_feat, tgt_list, mutual_filter: bool = True, min_mutual: int = 9):
+    """Feature-space matches of B pairs (regtr_feature_match): src_feat / tgt_feat B (n_s,33) / (n_t,33) arrays,
+    tgt_list the B target clouds (n_t,3) (numpy or torch, any float dtype; stacked in float64 on the device).
+    -> (nn, corr_tgt, mask, n_mutual): B (n_s,) int32 (the nearest target by (d2, index)), B (n_s,3) float64 (its
+    point), B (n_s,) bool (mutual; every match without mutual_filter or below min_mutual mutual matches) and (B,)
+    int32 mutual counts, all device tensors.  No host sync."""
+    B = len(src_feat)
+    if B == 0 or len(tgt_feat) != B or len(tgt_list) != B:
+        raise ValueError(f'feature_match: {B} source, {len(tgt_feat)} target feature arrays and {len(tgt_list)} '
+                         f'target clouds; expected as many, at least one pair')
+    fs = [torch.as_tensor(f) for f in src_feat]
+    ft = [torch.as_tensor(f) for f in tgt_feat]
+    tx = [torch.as_tensor(c) for c in tgt_list]
+    for b in range(B):
+        for f in (fs[b], ft[b]):
+            if f.dim() != 2 or f.shape[1] != FPFH_DIM:
+                raise ValueError(f'feature_match: pair {b}: features {tuple(f.shape)}, expected (n,{FPFH_DIM})')
+        if tuple(tx[b].shape) != (ft[b].shape[0], 3):
+            raise ValueError(f'feature_match: pair {b}: target cloud {tuple(tx[b].shape)} for '
+                             f'{ft[b].shape[0]} target features')
+        if fs[b].shape[0] > 0 and ft[b].shape[0] == 0:
+            raise ValueError(f'feature_match: pair {b}: a target without points')
+    L = _lib.load()
+    dev = next((c.device for c in fs + ft + tx if c.is_cuda), torch.device('cuda', torch.cuda.current_device()))
+    sf, ls = _stack_clouds(fs, dev, FPFH_DIM, 'feature_match')
+    tf, lt = _stack_clouds(ft, dev, FPFH_DIM, 'feature_match')
+    txyz, _ = _stack_clouds(tx, dev, 3, 'feature_match')
+    ns, nt = sum(ls), sum(lt)
+    ns_max, nt_max = max(ls), max(lt)
+    nn = torch.empty(max(ns, 1), dtype=torch.int32, device=dev)
+    corr = torch.empty((max(ns, 1), 3), dtype=torch.float64, device=dev)
+    mask = torch.empty(max(ns, 1), dtype=torch.uint8, device=dev)
+    n_mutual = torch.empty(B, dtype=torch.int32, device=dev)
+    ws = workspace(L.regtr_feature_match_ws_bytes(B, ns_max, nt_max, nt), dev)
+    soffs, toffs = make_offsets(ls, dev), make_offsets(lt, dev)
+    _lib.check(L.regtr_feature_match(_p(sf), _p(soffs), _p(tf), _p(txyz), _p(toffs), B, ns_max, nt_max, nt,
+                                     int(bool(mutual_filter)), int(min_mutual), _p(nn), _p(corr), _p(mask), _p(n_mutual), _p(ws), ws.numel(), _stream()),
+               'regtr_feature_match')
+    _count(feature_match_launches())
+    return _split(nn, ls), _split(corr, ls), _split(mask.bool(), ls), n_mutual
+
+
+def feature_correspondences(src_list, tgt_list, src_feat, tgt_feat, mutual_filter: bool = True, ransac_n: int = 3):
+    """The correspondences of Open3D's registration_ransac_based_on_feature_matching, in `ransac`'s layout: source
+    point i -> its nearest target in feature space (`feature_match`); with mutual_filter only the mutual matches take
+    part, unless fewer than 3 ransac_n are mutual (then all do, as in Open3D).
+    -> (corr_src, corr_tgt, corr_mask, n_mutual): B (n_s,3) float64, B (n_s,3) float64, B (n_s,) bool device tensors
+    and the (B,) int32 device tensor of mutual counts.  No host sync."""
+    B = len(src_list)
+    if B == 0 or len(tgt_list) != B or len(src_feat) != B or len(tgt_feat) != B:
+        raise ValueError(f'feature_correspondences: {B} sources, {len(tgt_list)} targets, {len(src_feat)} / '
+                         f'{len(tgt_feat)} feature arrays; expected as many, at least one pair')
+    src = [torch.as_tensor(c) for c in src_list]
+    for b in range(B):
+        if src[b].dim() != 2 or src[b].shape[1] != 3 or src[b].shape[0] != torch.as_tensor(src_feat[b]).shape[0]:
+            raise ValueError(f'feature_correspondences: pair {b}: source cloud {tuple(src[b].shape)} for '
+                             f'{tuple(torch.as_tensor(src_feat[b]).shape)} source features')
+    _, corr_tgt, corr_mask, n_mutual = feature_match(src_feat, tgt_feat, tgt_list, mutual_filter, 3 * int(ransac_n))
+    dev = n_mutual.device
+    return [c.to(dev, torch.float64) for c in src], corr_tgt, corr_mask, n_mutual
+
+
+def ransac_feature_matching(src_list, tgt_list, src_feat, tgt_feat, mutual_filter: bool,
+                            max_correspondence_distance: float, ransac_n: int = 3, **ransac_kwargs):
+    """Open3D's registration_ransac_based_on_feature_matching for B pairs: `feature_correspondences`, then `ransac`
+    over them (validated on src_list / tgt_list, the clouds the features describe) with max_correspondence_distance,
+    ransac_n and ransac_kwargs (max_iteration, confidence, edge_length, distance, seed, ...).
+    -> (pose (B,3,4), result (B,5), n_mutual (B,)): `ransac`'s outputs and the mutual counts.  Arguments `ransac`
+    would reject raise ValueError before any launch."""
+    a = inspect.signature(ransac).bind(src_list, tgt_list, src_list, src_list, max_correspondence_distance,
+                                       ransac_n=ransac_n, **ransac_kwargs)
+    a.apply_defaults()
+    a = a.arguments
+    src = [torch.as_tensor(c) for c in src_list]
+    _ransac_check(len(src), src, src, None, a['max_iteration'], a['confidence'], a['ransac_n'], a['edge_length'],
+                  a['distance'], a['seed'], a['pair_base'], a['first_chunk'])
+    corr_src, corr_tgt, corr_mask, n_mutual = feature_correspondences(src_list, tgt_list, src_feat, tgt_feat,
+                                                                      mutual_filter, ransac_n)
+    pose, out = ransac(src_list, tgt_list, corr_src, corr_tgt, max_correspondence_distance, ransac_n=ransac_n,
+                       corr_mask=corr_mask, **ransac_kwargs)
+    return pose, out, n_mutual
 
 
 def registration_information(src_list, tgt_list, pose, radius: float, status=None):

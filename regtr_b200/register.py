@@ -6,6 +6,8 @@
          [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
         [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
+    python -m regtr_b200.register SRC TGT --fpfh V [--fpfh_radius FR] [--fpfh_max_nn 100] [--fpfh_no_mutual]
+        [--ransac R ...] [--icp R ...] [--fit_radius R] [--out DIR]
 
 SRC / TGT: .ply, .pth, .bin or .npy (regtr_b200.pointio).  The config is the config.yaml one level above the
 checkpoint's directory, the layout `python -m regtr_b200.train` writes, unless --config names another.  Instead of the
@@ -36,6 +38,16 @@ walked, hypotheses validated, winning hypothesis.
 One JSON line on stdout: the pose, the four fit numbers and the point counts (with --icp, also icp_fitness, icp_rmse,
 icp_iterations, icp_radius and icp_method, and icp_loss, icp_loss_k and icp_epsilon when they are given; with --ransac,
 ransac_fitness, ransac_rmse, ransac_iterations, ransac_validations and ransac_radius).
+With --fpfh V there is no network and no --ckpt: Open3D's classical global registration (`eval.fpfh_register`) on the
+device.  Both clouds are downsampled at voxel V (`ops.grid_subsample`, a grid anchored at the origin), their normals
+estimated at 2 V with 30 neighbours at most, their FPFH features computed at --fpfh_radius (default 5 V) with
+--fpfh_max_nn neighbours at most, and `ops.ransac_feature_matching` registers the downsampled clouds: mutual feature
+matches (every match with --fpfh_no_mutual, or when fewer than 3 --ransac_n are mutual), --ransac radius (default
+1.5 V), the distance checker at --ransac_dist (default: the --ransac radius); --ransac_overlap is ignored.  --icp then
+refines the pose on the full clouds as above, and fit is taken at --fit_radius (default: the --ransac radius).
+Written: pose.txt, src_registered.ply and result.npz with pose_fpfh (3,4) float64, ransac (5,), n_mutual, fit and,
+with --icp, pose_icp and icp; no keypoint files.  The JSON line has the pose, the fit numbers, the point counts,
+fpfh_voxel, n_src_down, n_tgt_down, n_mutual and the ransac_* (and icp_*) entries.
 """
 from __future__ import annotations
 
@@ -48,7 +60,8 @@ from typing import Dict
 import numpy as np
 import torch
 
-from .eval import (add_icp_arguments, add_ransac_arguments, check_icp_arguments, check_ransac_arguments, icp_refine,
+from .eval import (add_fpfh_arguments, add_icp_arguments, add_ransac_arguments, check_fpfh_arguments,
+                   check_icp_arguments, check_ransac_arguments, fpfh_kwargs, fpfh_register, icp_kwargs, icp_refine,
                    ransac_kwargs, ransac_refine)
 
 
@@ -57,16 +70,31 @@ def parser() -> argparse.ArgumentParser:
                                  description='Register a source point cloud to a target with a trained RegTR.')
     ap.add_argument('src', help='Source point cloud (.ply, .pth, .bin or .npy)')
     ap.add_argument('tgt', help='Target point cloud (.ply, .pth, .bin or .npy)')
-    ap.add_argument('--ckpt', required=True, help='Checkpoint ({"state_dict": ...}), e.g. <logdir>/ckpt/model-best.pth')
+    ap.add_argument('--ckpt', help='Checkpoint ({"state_dict": ...}), e.g. <logdir>/ckpt/model-best.pth (required '
+                                   'unless --fpfh)')
     ap.add_argument('--config', help='Config file (default: config.yaml one level above the checkpoint directory)')
     ap.add_argument('--threshold', type=float, default=0.5,
                     help='Keypoints with predicted overlap above this go to src_kp.ply / src_kp_warped.ply')
-    ap.add_argument('--fit_radius', type=float, help='Inlier radius of the fitness / RMSE (default: overlap_radius)')
+    ap.add_argument('--fit_radius', type=float,
+                    help='Inlier radius of the fitness / RMSE (default: overlap_radius; with --fpfh the RANSAC radius)')
     add_icp_arguments(ap, 'Refine the pose with point-to-point ICP, max correspondence distance R (default: no ICP)')
     add_ransac_arguments(ap, 'Replace the pose by RANSAC over the predicted correspondences, max correspondence '
-                             'distance R (default: no RANSAC; before ICP with --icp)')
+                             'distance R (default: no RANSAC; before ICP with --icp; with --fpfh 1.5 V)')
+    add_fpfh_arguments(ap)
     ap.add_argument('--out', default='.', help='Output directory')
     return ap
+
+
+def parse_args(argv=None):
+    """The parsed command line, its usage errors raised and the --fpfh defaults filled in."""
+    ap = parser()
+    opt = ap.parse_args(argv)
+    check_fpfh_arguments(ap, opt)
+    check_icp_arguments(ap, opt)
+    check_ransac_arguments(ap, opt)
+    if opt.fpfh is not None and opt.fit_radius is None:
+        opt.fit_radius = opt.ransac
+    return opt
 
 
 def config_path(ckpt: str, config: str = None) -> Path:
@@ -139,6 +167,27 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
     return res
 
 
+def register_fpfh(src_xyz: np.ndarray, tgt_xyz: np.ndarray, voxel: float, fit_radius: float,
+                  icp_radius: float = None, icp_options: Dict = None, fpfh_options: Dict = None) -> Dict:
+    """One pair without a network (`eval.fpfh_register` at voxel, fpfh_options its further keyword arguments, then ICP
+    on the full clouds with icp_radius and icp_options).  -> dict of host arrays: src_xyz / tgt_xyz (float64),
+    pose_fpfh (3,4) float64, ransac (5,), n_mutual, n_src_down, n_tgt_down, fit (4,) of the final pose at fit_radius,
+    and pose_icp / icp with icp_radius."""
+    from . import ops
+    src_xyz = np.asarray(src_xyz, dtype=np.float64)
+    tgt_xyz = np.asarray(tgt_xyz, dtype=np.float64)
+    out = fpfh_register([src_xyz], [tgt_xyz], voxel, icp_radius=icp_radius, icp_kwargs=icp_options,
+                        **(fpfh_options or {}))
+    fit = ops.registration_fit([src_xyz], [tgt_xyz], out['pose'], fit_radius)
+    res = {'src_xyz': src_xyz, 'tgt_xyz': tgt_xyz, 'pose_fpfh': out['pose_fpfh'][0].cpu().numpy(),
+           'ransac': out['ransac'][0].cpu().numpy(), 'n_mutual': int(out['n_mutual'][0]),
+           'n_src_down': int(out['src_down'][0].shape[0]), 'n_tgt_down': int(out['tgt_down'][0].shape[0]),
+           'fit': fit[0].cpu().numpy()}
+    if icp_radius is not None:
+        res.update(pose_icp=out['pose'][0].cpu().numpy(), icp=out['icp'][0].cpu().numpy())
+    return res
+
+
 def pose44(pose34) -> np.ndarray:
     p = np.eye(4)
     p[:3] = np.asarray(pose34, dtype=np.float64)
@@ -151,8 +200,9 @@ def pose_text(pose34) -> str:
 
 
 def final_pose(res: Dict):
-    """The pose `register` settles on: ICP's, else RANSAC's, else the final decoder layer's."""
-    for k in ('pose_icp', 'pose_ransac'):
+    """The pose `register` settles on: ICP's, else RANSAC's (over network or FPFH matches), else the final decoder
+    layer's."""
+    for k in ('pose_icp', 'pose_ransac', 'pose_fpfh'):
         if k in res:
             return res[k]
     return res['pose'][-1]
@@ -164,6 +214,12 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
     final = final_pose(res)
     with open(os.path.join(out_dir, 'pose.txt'), 'w') as fh:
         fh.write(pose_text(final))
+    p = final.astype(np.float64)
+    write_ply(os.path.join(out_dir, 'src_registered.ply'), res['src_xyz'] @ p[:, :3].T + p[:, 3])
+    if 'pose_fpfh' in res:
+        keys = ('pose_fpfh', 'ransac', 'n_mutual', 'fit') + (('pose_icp', 'icp') if 'pose_icp' in res else ())
+        np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
+        return 0
     keys = ('pose', 'src_kp', 'src_kp_warped', 'src_overlap', 'tgt_kp', 'tgt_kp_warped', 'tgt_overlap', 'fit')
     if 'pose_coarse' in res:
         keys += ('pose_coarse',)
@@ -172,8 +228,6 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
     if 'pose_icp' in res:
         keys += ('pose_icp', 'icp')
     np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
-    p = final.astype(np.float64)
-    write_ply(os.path.join(out_dir, 'src_registered.ply'), res['src_xyz'] @ p[:, :3].T + p[:, 3])
     m = res['src_overlap'] > threshold
     write_ply(os.path.join(out_dir, 'src_kp.ply'), res['src_kp'][m], {'overlap': res['src_overlap'][m]})
     write_ply(os.path.join(out_dir, 'src_kp_warped.ply'), res['src_kp_warped'][m], {'overlap': res['src_overlap'][m]})
@@ -181,12 +235,11 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
 
 
 def main(argv=None):
-    ap = parser()
-    opt = ap.parse_args(argv)
-    check_icp_arguments(ap, opt)
-    check_ransac_arguments(ap, opt)
-    from .config import load_config
+    opt = parse_args(argv)
     from .pointio import load_point_cloud
+    if opt.fpfh is not None:
+        return main_fpfh(opt, load_point_cloud(opt.src), load_point_cloud(opt.tgt))
+    from .config import load_config
     cfg_file = config_path(opt.ckpt, opt.config)
     if not cfg_file.exists():
         raise SystemExit(f'config not found: {cfg_file} (pass --config)')
@@ -204,17 +257,42 @@ def main(argv=None):
             'n_tgt_kp': int(res['tgt_kp'].shape[0]), 'n_src_kp_above_threshold': n_shown,
             'fit_radius': float(cfg['overlap_radius'] if opt.fit_radius is None else opt.fit_radius)}
     if opt.icp is not None:
-        icp = [float(v) for v in res['icp']]
-        line.update(icp_fitness=icp[0], icp_rmse=icp[1], icp_iterations=int(icp[3]), icp_radius=float(opt.icp),
-                    icp_method=opt.icp_method)
-        if opt.icp_loss != 'l2':
-            line.update(icp_loss=opt.icp_loss, icp_loss_k=float(opt.icp_loss_k))
-        if opt.icp_method == 'generalized':
-            line.update(icp_epsilon=float(opt.icp_epsilon))
+        line.update(icp_line(opt, res['icp']))
     if opt.ransac is not None:
         rs = [float(v) for v in res['ransac']]
         line.update(ransac_fitness=rs[0], ransac_rmse=rs[1], ransac_iterations=int(rs[2]),
                     ransac_validations=int(rs[3]), ransac_radius=float(opt.ransac))
+    print(json.dumps(line))
+    return res
+
+
+def icp_line(opt, icp) -> Dict:
+    """The JSON line's icp_* entries."""
+    icp = [float(v) for v in icp]
+    line = dict(icp_fitness=icp[0], icp_rmse=icp[1], icp_iterations=int(icp[3]), icp_radius=float(opt.icp),
+                icp_method=opt.icp_method)
+    if opt.icp_loss != 'l2':
+        line.update(icp_loss=opt.icp_loss, icp_loss_k=float(opt.icp_loss_k))
+    if opt.icp_method == 'generalized':
+        line.update(icp_epsilon=float(opt.icp_epsilon))
+    return line
+
+
+def main_fpfh(opt, src_xyz, tgt_xyz):
+    """`main` with --fpfh: `register_fpfh`, its files and its JSON line."""
+    res = register_fpfh(src_xyz, tgt_xyz, opt.fpfh, opt.fit_radius, opt.icp,
+                        icp_kwargs(opt) if opt.icp is not None else None, fpfh_kwargs(opt))
+    write_outputs(res, opt.out)
+    f = [float(v) for v in res['fit']]
+    rs = [float(v) for v in res['ransac']]
+    line = {'pose': pose44(final_pose(res)).tolist(), 'fitness_src': f[0], 'rmse_src': f[1], 'fitness_tgt': f[2],
+            'rmse_tgt': f[3], 'n_src': int(res['src_xyz'].shape[0]), 'n_tgt': int(res['tgt_xyz'].shape[0]),
+            'fit_radius': float(opt.fit_radius), 'fpfh_voxel': float(opt.fpfh), 'n_src_down': res['n_src_down'],
+            'n_tgt_down': res['n_tgt_down'], 'n_mutual': res['n_mutual'], 'ransac_fitness': rs[0],
+            'ransac_rmse': rs[1], 'ransac_iterations': int(rs[2]), 'ransac_validations': int(rs[3]),
+            'ransac_radius': float(opt.ransac)}
+    if opt.icp is not None:
+        line.update(icp_line(opt, res['icp']))
     print(json.dumps(line))
     return res
 
