@@ -726,6 +726,59 @@ int regtr_ransac(const double* xyz, const int32_t* offs, int B, int n_cap, const
                  float cell, const regtr_ransac_options* opt, double* pose_out, double* result, uint32_t* status,
                  void* ws, size_t ws_bytes, void* state, size_t state_bytes, void* stream);
 
+/* Fast Global Registration of B pairs (Open3D's registration_fgr_based_on_correspondence, and the solve of
+ * registration_fgr_based_on_feature_matching, with FastGlobalRegistrationOption; Zhou, Park and Koltun, ECCV 2016),
+ * with one deterministic rule in place of Open3D's rand() draws and OpenMP sums.
+ * xyz (n_cap,3) float64 stacked src_0..src_{B-1}, tgt_0..tgt_{B-1} with offs (2B+1) i32 (the clouds whose means and
+ * scale normalise the problem); corr_src / corr_tgt (m_cap,3) float64, pair b's correspondences (a_i, c_i) in rows
+ * [coffs[b], coffs[b+1]) (coffs (B+1) i32); corr_mask (m_cap) u8, nullable: the correspondences with a non-zero byte
+ * take part, in their original order (n of them).  Products, sums and norms are rounded one by one; norms are
+ * sqrt((dx dx + dy dy) + dz dz).  Per pair:
+ *   mu_s, mu_t: each cloud's mean (point i added to chain i % 512 in order; each warp's 32 chains by a halving tree,
+ *   then the 16 warp sums by a halving tree; / count, 0 for an empty cloud); sigma = the largest |p - mu| over both
+ *   clouds (1 when it is 0).  use_absolute_scale: sigma_g = 1, par0 = sigma; else sigma_g = sigma, par0 = 1.  Points
+ *   are used as (p - mu) / sigma_g.
+ *   tuple_test with n > 0: trials k = 0, 1, ... < 100 n; trial k draws indices mulhi32(w_e, n), e = 0..2, w the words
+ *   of Philox4x32-10 at counter (k, pair_base + b, 0, 0x46475254) with key (seed lo, seed hi); it passes when the
+ *   edges (0,1), (1,2), (2,0) of both sides have l_s tuple_scale < l_t < l_s / tuple_scale; a pass appends its three
+ *   correspondences in draw order, and the walk stops right after the pass that reaches maximum_tuple_count.  The
+ *   solve then runs on the 3 x tuples list; without the test on the n correspondences.
+ *   Fewer than 10 correspondences: the identity.  Otherwise T = I, par = par0, and iteration_number times: with q the
+ *   normalised target point moved by every earlier update, r = p - q, s = (par / (r.r + par))^2, the rows
+ *   J_x = (0, -q_z, q_y, -1, 0, 0), J_y = (q_z, 0, -q_x, 0, -1, 0), J_z = (-q_y, q_x, 0, 0, 0, -1) add (J_a J_b) s
+ *   to J^T J and (J_a r) s to J^T r (correspondence c to chain c % 256 in order, rows x, y, z; the chains reduced as
+ *   above with 8 warps); J^T J x = -J^T r by LDL^T (|det| < 1e-6 or not finite: T and the points stay as they are);
+ *   delta = Rz(x2) Ry(x1) Rx(x0) with t = (x3, x4, x5), T = delta T; then with decrease_mu, itr % 4 == 0 and
+ *   par > maximum_correspondence_distance, par /= division_factor.
+ * pose_out (B,3,4) float64 = R^T, -R^T (-R mu_t + sigma_g t + mu_s) (Open3D's GetInvTransformationOriginalScale);
+ * result (B,4) float64 = (correspondences of the solve, tuples kept, trials walked, final par).
+ * 2 launches whatever the data; no value atomics, no host synchronisation; the result is bit-identical for a pair
+ * alone or in a batch with the same pair_base + b.  Coordinates must be finite.
+ * REGTR_ERR_ARG: B < 1, m_cap above REGTR_FGR_MAX_CORR, division_factor or maximum_correspondence_distance not
+ * > 0 and finite, a negative iteration_number, tuple_scale outside (0, 1], maximum_tuple_count outside
+ * 1..REGTR_FGR_MAX_TUPLES, pair_base < 0 or pair_base + B beyond INT_MAX.
+ * ws: regtr_fgr_ws_bytes(m_cap, B, maximum_tuple_count). */
+#define REGTR_FGR_MAX_CORR 21474836                 /* 100 trials per correspondence stay below 2^31 */
+#define REGTR_FGR_MAX_TUPLES (1 << 20)
+typedef struct {
+    double division_factor;                  /* par divisor of the GNC schedule, > 0 [1.4] */
+    int use_absolute_scale;                  /* [0] */
+    int decrease_mu;                         /* [1] */
+    double maximum_correspondence_distance;  /* par's lower bound in the schedule, > 0 [0.025] */
+    int iteration_number;                    /* GNC iterations [64] */
+    double tuple_scale;                      /* in (0, 1] [0.95] */
+    int maximum_tuple_count;                 /* 1..REGTR_FGR_MAX_TUPLES [1000] */
+    int tuple_test;                          /* [0] */
+    unsigned long long seed;                 /* Philox key of the tuple draws */
+    int pair_base;                           /* global index of pair 0 in the draws */
+} regtr_fgr_options;
+
+size_t regtr_fgr_ws_bytes(int m_cap, int B, int maximum_tuple_count);
+int regtr_fgr(const double* xyz, const int32_t* offs, int B, int n_cap, const double* corr_src,
+              const double* corr_tgt, const int32_t* coffs, const uint8_t* corr_mask, int m_cap,
+              const regtr_fgr_options* opt, double* pose_out, double* result, void* ws, size_t ws_bytes,
+              void* stream);
+
 /* ---- pose graph ------------------------------------------------------------------- */
 
 #define REGTR_POSE_GRAPH_MAX_NODES 256

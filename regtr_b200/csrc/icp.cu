@@ -340,50 +340,6 @@ k_icp_reduce_plane(const double* __restrict__ xyz, const int32_t* __restrict__ o
     for (int e = 0; e < PART_PLANE; ++e) o[e] = out[e];
 }
 
-// Solve A x = -v for the symmetric 6x6 A given by its upper triangle H (row-major) by LDL^T without pivoting, in a
-// fixed order.  False, x untouched, when |det A| = |prod D| < 1e-6 or det is not finite (Open3D's
-// SolveLinearSystemPSD check).
-__device__ __forceinline__ bool solve6_ldlt(const double H[21], const double v[6], double x[6]) {
-    double A[6][6], L[6][6], D[6];
-#pragma unroll
-    for (int a = 0, e = 0; a < 6; ++a)
-#pragma unroll
-        for (int c = a; c < 6; ++c, ++e) { A[a][c] = H[e]; A[c][a] = H[e]; }
-    double det = 1.0;
-#pragma unroll
-    for (int j = 0; j < 6; ++j) {
-        double d = A[j][j];
-#pragma unroll
-        for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k] * D[k];
-        D[j] = d;
-        det *= d;
-#pragma unroll
-        for (int i = j + 1; i < 6; ++i) {
-            double a = A[i][j];
-#pragma unroll
-            for (int k = 0; k < j; ++k) a -= L[i][k] * L[j][k] * D[k];
-            L[i][j] = a / d;
-        }
-    }
-    if (!(fabs(det) >= 1e-6) || isinf(det)) return false;
-    double y[6];
-#pragma unroll
-    for (int i = 0; i < 6; ++i) {                      // L y = -v
-        double a = -v[i];
-#pragma unroll
-        for (int k = 0; k < i; ++k) a -= L[i][k] * y[k];
-        y[i] = a;
-    }
-#pragma unroll
-    for (int i = 5; i >= 0; --i) {                     // L^T x = D^-1 y
-        double a = y[i] / D[i];
-#pragma unroll
-        for (int k = i + 1; k < 6; ++k) a -= L[k][i] * x[k];
-        x[i] = a;
-    }
-    return true;
-}
-
 // One thread per pair.  The pair's chunks are combined in chunk order, giving k, fitness = k / n and inlier
 // RMSE = sqrt(sum d2 / k) of the current correspondences.  After round 0 the stop test |d fitness| < rel_fitness and
 // |d rmse| < rel_rmse ends the pair; so does round max_iter.  Otherwise the update, composed as T = update . T.

@@ -1,5 +1,6 @@
 // Internal to the library: float64 rigid-transform helpers shared by the pose solve (kabsch.cu), the training-data
-// preparation (traindata.cu), ICP (icp.cu) and the pose-graph optimiser (posegraph.cu).
+// preparation (traindata.cu), ICP (icp.cu), the pose-graph optimiser (posegraph.cu) and Fast Global Registration
+// (fgr.cu).
 #pragma once
 
 #include "common.cuh"
@@ -12,7 +13,7 @@ __device__ __forceinline__ double rt_row(const double* m, double x, double y, do
 }
 
 // x = (rx, ry, rz, tx, ty, tz) -> R = Rz(rz) Ry(ry) Rx(rx), t = (tx, ty, tz) (Open3D's TransformVector6dToMatrix4d):
-// the update of point-to-plane ICP (icp.cu) and of the pose-graph optimiser (posegraph.cu)
+// the update of point-to-plane ICP (icp.cu), of the pose-graph optimiser (posegraph.cu) and of FGR (fgr.cu)
 __device__ __forceinline__ void rigid_from_vec6(const double x[6], double R[3][3], double t[3]) {
     double sa, ca, sb, cb, sc, cc;
     sincos(x[0], &sa, &ca);
@@ -22,6 +23,50 @@ __device__ __forceinline__ void rigid_from_vec6(const double x[6], double R[3][3
     R[1][0] = sc * cb; R[1][1] = sc * sb * sa + cc * ca; R[1][2] = sc * sb * ca - cc * sa;
     R[2][0] = -sb;     R[2][1] = cb * sa;                R[2][2] = cb * ca;
     for (int r = 0; r < 3; ++r) t[r] = x[3 + r];
+}
+
+// Solve A x = -v for the symmetric 6x6 A given by its upper triangle H (row-major) by LDL^T without pivoting, in a
+// fixed order.  False, x untouched, when |det A| = |prod D| < 1e-6 or det is not finite (Open3D's
+// SolveLinearSystemPSD check).
+__device__ __forceinline__ bool solve6_ldlt(const double H[21], const double v[6], double x[6]) {
+    double A[6][6], L[6][6], D[6];
+#pragma unroll
+    for (int a = 0, e = 0; a < 6; ++a)
+#pragma unroll
+        for (int c = a; c < 6; ++c, ++e) { A[a][c] = H[e]; A[c][a] = H[e]; }
+    double det = 1.0;
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+        double d = A[j][j];
+#pragma unroll
+        for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k] * D[k];
+        D[j] = d;
+        det *= d;
+#pragma unroll
+        for (int i = j + 1; i < 6; ++i) {
+            double a = A[i][j];
+#pragma unroll
+            for (int k = 0; k < j; ++k) a -= L[i][k] * L[j][k] * D[k];
+            L[i][j] = a / d;
+        }
+    }
+    if (!(fabs(det) >= 1e-6) || isinf(det)) return false;
+    double y[6];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) {                      // L y = -v
+        double a = -v[i];
+#pragma unroll
+        for (int k = 0; k < i; ++k) a -= L[i][k] * y[k];
+        y[i] = a;
+    }
+#pragma unroll
+    for (int i = 5; i >= 0; --i) {                     // L^T x = D^-1 y
+        double a = y[i] / D[i];
+#pragma unroll
+        for (int k = i + 1; k < 6; ++k) a -= L[k][i] * x[k];
+        x[i] = a;
+    }
+    return true;
 }
 
 // The sweeps of svd3_jacobi: one-sided (Hestenes) Jacobi rotations of A's column pairs, accumulated in V, until the

@@ -554,6 +554,110 @@ def ransac_forward(forward_fn, radius: float, max_iteration: int = 100000, confi
     return run
 
 
+def fgr_refine(pred, src_list, tgt_list, overlap: float = 0.5, pair_base: int = 0, fgr=None, correspondences=None,
+               **fgr_kwargs):
+    """A global pose for every pair of a forward's output `pred`: Fast Global Registration (`ops.fgr`, normalised by
+    src_list / tgt_list, fgr_kwargs its options) over RegTR's two-way correspondences with predicted overlap above
+    `overlap` (`ops.regtr_correspondences`).  -> fgr's (pose (B,3,4), result (B,4)).
+    fgr(src_list, tgt_list, corr_src, corr_tgt, corr_mask, pair_base=, ...) and correspondences(pred, overlap) default
+    to the `ops` functions."""
+    if fgr is None:
+        from .ops import fgr
+    if correspondences is None:
+        from .ops import regtr_correspondences as correspondences
+    corr_src, corr_tgt, corr_mask = correspondences(pred, overlap)
+    return fgr(src_list, tgt_list, corr_src, corr_tgt, corr_mask, pair_base=pair_base, **fgr_kwargs)
+
+
+def add_fgr_arguments(ap, fgr_help: str):
+    """The FGR flags of a command line, for `fgr_refine` and `fpfh_register`: --fgr (help text fgr_help), --fgr_dist,
+    --fgr_iters, --fgr_division, --fgr_tuple_scale, --fgr_max_tuples, --fgr_tuple_test, --fgr_no_tuple_test,
+    --fgr_no_decrease_mu, --fgr_absolute_scale, --fgr_seed and --fgr_overlap."""
+    ap.add_argument('--fgr', action='store_true', help=fgr_help)
+    ap.add_argument('--fgr_dist', type=float, metavar='D',
+                    help='FGR maximum correspondence distance, the end of its GNC schedule (default: 0.025; with '
+                         '--fpfh 0.5 V)')
+    ap.add_argument('--fgr_iters', type=int, default=64, help='FGR iterations')
+    ap.add_argument('--fgr_division', type=float, default=1.4, help='FGR divisor of the GNC parameter, > 0')
+    ap.add_argument('--fgr_tuple_scale', type=float, default=0.95, help='FGR tuple test similarity, in (0, 1]')
+    ap.add_argument('--fgr_max_tuples', type=int, default=1000, help='FGR tuples kept at most by the tuple test')
+    ap.add_argument('--fgr_tuple_test', action='store_true',
+                    help='Run the tuple test on the predicted correspondences (the feature path always does, unless '
+                         '--fgr_no_tuple_test)')
+    ap.add_argument('--fgr_no_tuple_test', action='store_true', help='Skip the tuple test on FPFH matches (--fpfh)')
+    ap.add_argument('--fgr_no_decrease_mu', action='store_true', help='Keep FGR\'s GNC parameter fixed')
+    ap.add_argument('--fgr_absolute_scale', action='store_true',
+                    help='Do not rescale the clouds to unit size before the FGR solve')
+    ap.add_argument('--fgr_seed', type=int, default=0, help='Seed of the FGR tuple draws')
+    ap.add_argument('--fgr_overlap', type=float, default=0.5,
+                    help='Correspondences whose predicted overlap is above this take part in FGR')
+
+
+def check_fgr_arguments(ap, opt):
+    """Reject, as usage errors, FGR options `ops.fgr` would refuse and flag combinations that make no sense, before
+    any model is loaded, and fill in --fgr_dist (0.5 V with --fpfh V, else 0.025).  Call before
+    `check_fpfh_arguments`, which then leaves --ransac unset."""
+    from .ops import FGR_MAX_TUPLES
+    if not opt.fgr:
+        return
+    fpfh = getattr(opt, 'fpfh', None)
+    if opt.ransac is not None:
+        ap.error('--fgr and --ransac are exclusive: choose one global registration')
+    if fpfh is not None and opt.fpfh_no_mutual:
+        ap.error('--fpfh_no_mutual cannot be used with --fgr: FGR always keeps the mutual matches only')
+    if fpfh is None and opt.fgr_no_tuple_test:
+        ap.error('--fgr_no_tuple_test applies to --fpfh; on predicted correspondences the tuple test is off unless '
+                 '--fgr_tuple_test')
+    if opt.fgr_dist is None:
+        opt.fgr_dist = 0.5 * fpfh if fpfh is not None and fpfh > 0.0 else 0.025
+    for flag, v in (('--fgr_dist', opt.fgr_dist), ('--fgr_division', opt.fgr_division)):
+        if not (math.isfinite(v) and v > 0.0):
+            ap.error(f'{flag} {v} must be a finite value > 0')
+    if not 0 <= opt.fgr_iters < 2 ** 31:
+        ap.error(f'--fgr_iters {opt.fgr_iters} must be >= 0')
+    if not 0.0 < opt.fgr_tuple_scale <= 1.0:
+        ap.error(f'--fgr_tuple_scale {opt.fgr_tuple_scale} must be in (0, 1]')
+    if not 1 <= opt.fgr_max_tuples <= FGR_MAX_TUPLES:
+        ap.error(f'--fgr_max_tuples {opt.fgr_max_tuples} must be in 1..{FGR_MAX_TUPLES}')
+    if not 0 <= opt.fgr_seed < 2 ** 64:
+        ap.error(f'--fgr_seed {opt.fgr_seed} must be in [0, 2^64)')
+
+
+def fgr_kwargs(opt) -> Dict:
+    """`ops.fgr`'s keyword arguments from the parsed --fgr_* flags (without --fgr_overlap).  The tuple test runs on FPFH
+    matches (--fpfh) unless --fgr_no_tuple_test, and on predicted correspondences only with --fgr_tuple_test."""
+    tuple_test = not opt.fgr_no_tuple_test if getattr(opt, 'fpfh', None) is not None else opt.fgr_tuple_test
+    return dict(maximum_correspondence_distance=opt.fgr_dist, iteration_number=opt.fgr_iters,
+                division_factor=opt.fgr_division, decrease_mu=not opt.fgr_no_decrease_mu,
+                use_absolute_scale=opt.fgr_absolute_scale, tuple_test=tuple_test, tuple_scale=opt.fgr_tuple_scale,
+                maximum_tuple_count=opt.fgr_max_tuples, seed=opt.fgr_seed)
+
+
+def fgr_forward(forward_fn, overlap: float = 0.5, fgr=None, correspondences=None, icp_radius: float = None,
+                icp_kwargs=None, icp=None, estimate_normals=None, **fgr_kwargs):
+    """Wrap `forward_fn(batch) -> pred` so that every pair's pose comes from FGR over the network's correspondences
+    (`fgr_refine` with overlap and fgr_kwargs, normalised by the batch's full clouds): -> a NEW dict with pred's
+    entries, pose (1,B,3,4) float64 the FGR poses and pose_coarse (1,B,3,4) float64 the network's final poses.  With
+    icp_radius, ICP then starts from the FGR poses (`icp_refine` with icp_radius, icp_kwargs, icp and
+    estimate_normals): pose is the refined pose and pose_fgr the FGR one.  pred's own tensors are not written to."""
+    def run(batch):
+        pred = forward_fn(batch)
+        coarse = pred['pose'][-1].to(torch.float64)                     # (B,3,4), a new tensor
+        pose, _ = fgr_refine(pred, batch['src_xyz'], batch['tgt_xyz'], overlap, fgr=fgr,
+                             correspondences=correspondences, **fgr_kwargs)
+        pose = torch.as_tensor(pose, dtype=torch.float64, device=coarse.device).reshape(coarse.shape)
+        out = dict(pred)
+        out['pose_coarse'] = coarse[None]
+        if icp_radius is not None:
+            out['pose_fgr'] = pose[None]
+            pose, _ = icp_refine(batch['src_xyz'], batch['tgt_xyz'], pose, icp_radius, icp=icp,
+                                 estimate_normals=estimate_normals, **(icp_kwargs or {}))
+            pose = torch.as_tensor(pose, dtype=torch.float64, device=coarse.device).reshape(coarse.shape)
+        out['pose'] = pose[None]
+        return out
+    return run
+
+
 def fpfh_downsample(clouds, voxel: float):
     """`ops.grid_subsample(dense=False)` of C clouds at `voxel` in one call: the mean of every occupied voxel of a grid
     anchored at the origin (Open3D's voxel_down_sample anchors its grid at the bounding box's minimum corner).
@@ -576,19 +680,37 @@ def fpfh_register(src_list, tgt_list, voxel: float, normal_radius: float = None,
                   fpfh_radius: float = None, fpfh_max_nn: int = 100, mutual_filter: bool = True,
                   ransac_radius: float = None, max_iteration: int = 100000, confidence: float = 0.999,
                   ransac_n: int = 3, edge_length: float = 0.9, distance: float = None, seed: int = 0,
-                  pair_base: int = 0, icp_radius: float = None, icp_kwargs=None) -> Dict:
+                  pair_base: int = 0, icp_radius: float = None, icp_kwargs=None, method: str = 'ransac',
+                  fgr_kwargs=None) -> Dict:
     """Classical global registration of B pairs without a network, Open3D's tutorial pipeline on the device:
     `fpfh_downsample` at voxel V, `ops.estimate_normals` (normal_radius, default 2 V, normal_max_nn), `ops.fpfh`
     (fpfh_radius, default 5 V, fpfh_max_nn), then `ops.ransac_feature_matching` at ransac_radius (default 1.5 V) with the
-    distance checker at `distance` (default: ransac_radius; 0: off), validated on the downsampled clouds.  With
-    icp_radius, `icp_refine` (icp_kwargs) then starts from the RANSAC poses on the full clouds.
-    -> dict: pose (B,3,4) float64 (the final poses), pose_fpfh (B,3,4) the RANSAC poses, ransac (B,5), n_mutual (B,),
-    src_down / tgt_down (B downsampled clouds), and icp (B,4) with icp_radius; device tensors."""
+    distance checker at `distance` (default: ransac_radius; 0: off), validated on the downsampled clouds.
+    method='fgr' replaces RANSAC by `ops.fgr_feature_matching` on the downsampled clouds with fgr_kwargs (its options;
+    maximum_correspondence_distance defaults to 0.5 V as in Open3D's tutorial) and needs mutual_filter; the RANSAC
+    arguments are then unused.  With icp_radius, `icp_refine` (icp_kwargs) then starts from the global poses on the
+    full clouds.
+    -> dict: pose (B,3,4) float64 (the final poses), pose_fpfh (B,3,4) the RANSAC (or FGR) poses, ransac (B,5) (or
+    fgr (B,4)), n_mutual (B,), src_down / tgt_down (B downsampled clouds), and icp (B,4) with icp_radius; device
+    tensors."""
     from . import ops
+    if method not in ('ransac', 'fgr'):
+        raise ValueError(f'fpfh_register: unknown method {method!r}')
+    if method == 'fgr' and not mutual_filter:
+        raise ValueError('fpfh_register: FGR keeps the mutual matches only (mutual_filter=False is not supported)')
     B = len(src_list)
     down = fpfh_downsample(list(src_list) + list(tgt_list), voxel)
     normals = ops.estimate_normals(down, 2.0 * voxel if normal_radius is None else normal_radius, normal_max_nn)
     feats = ops.fpfh(down, normals, 5.0 * voxel if fpfh_radius is None else fpfh_radius, fpfh_max_nn)
+    if method == 'fgr':
+        kw = dict(fgr_kwargs or {})
+        kw.setdefault('maximum_correspondence_distance', 0.5 * voxel)
+        pose, res, n_mutual = ops.fgr_feature_matching(down[:B], down[B:], feats[:B], feats[B:], pair_base=pair_base,
+                                                       **kw)
+        out = dict(pose=pose, pose_fpfh=pose, fgr=res, n_mutual=n_mutual, src_down=down[:B], tgt_down=down[B:])
+        if icp_radius is not None:
+            out['pose'], out['icp'] = icp_refine(src_list, tgt_list, pose, icp_radius, **(icp_kwargs or {}))
+        return out
     r = 1.5 * voxel if ransac_radius is None else ransac_radius
     pose, res, n_mutual = ops.ransac_feature_matching(
         down[:B], down[B:], feats[:B], feats[B:], mutual_filter, r, ransac_n, max_iteration=max_iteration,
@@ -602,8 +724,8 @@ def fpfh_register(src_list, tgt_list, voxel: float, normal_radius: float = None,
 
 def fpfh_forward(voxel: float, icp_radius: float = None, icp_kwargs=None, **fpfh_kwargs):
     """A network-free `forward_fn(batch) -> pred` for `run_3dmatch_benchmark`: `fpfh_register` of the batch's full
-    clouds (voxel, fpfh_kwargs, and ICP after it with icp_radius / icp_kwargs) -> dict with pose (1,B,3,4) float64,
-    and pose_fpfh (1,B,3,4) (the RANSAC poses) when ICP follows."""
+    clouds (voxel, fpfh_kwargs (method='fgr' and fgr_kwargs included), and ICP after it with icp_radius / icp_kwargs)
+    -> dict with pose (1,B,3,4) float64, and pose_fpfh (1,B,3,4) (the RANSAC or FGR poses) when ICP follows."""
     def run(batch):
         res = fpfh_register(batch['src_xyz'], batch['tgt_xyz'], voxel, icp_radius=icp_radius, icp_kwargs=icp_kwargs,
                             **fpfh_kwargs)
@@ -619,7 +741,7 @@ def add_fpfh_arguments(ap):
     --fpfh_no_mutual."""
     ap.add_argument('--fpfh', type=float, metavar='V',
                     help='Register without a network: FPFH features of the clouds downsampled at voxel V, matched in '
-                         'feature space, then RANSAC (Open3D\'s global registration); no --ckpt')
+                         'feature space, then RANSAC, or FGR with --fgr (Open3D\'s global registration); no --ckpt')
     ap.add_argument('--fpfh_radius', type=float, metavar='FR', help='FPFH feature radius (default: 5 V)')
     ap.add_argument('--fpfh_max_nn', type=int, default=100, help='Neighbours at most of the FPFH feature, 1..128')
     ap.add_argument('--fpfh_no_mutual', action='store_true',
@@ -628,8 +750,8 @@ def add_fpfh_arguments(ap):
 
 def check_fpfh_arguments(ap, opt):
     """With --fpfh: reject --ckpt and bad FPFH values as usage errors, and fill in the defaults that depend on V
-    (--fpfh_radius 5 V, --ransac 1.5 V, --ransac_dist the --ransac radius).  Without it,
-    --ckpt is required.  Call before `check_ransac_arguments`."""
+    (--fpfh_radius 5 V, --ransac 1.5 V, --ransac_dist the --ransac radius; with --fgr, --ransac stays unset).
+    Without it, --ckpt is required.  Call before `check_ransac_arguments`."""
     from .ops import FPFH_MAX_NN
     if opt.fpfh is None:
         if opt.ckpt is None:
@@ -645,6 +767,8 @@ def check_fpfh_arguments(ap, opt):
         opt.fpfh_radius = 5.0 * opt.fpfh
     if not opt.fpfh_radius > 0.0:
         ap.error(f'--fpfh_radius {opt.fpfh_radius} must be > 0')
+    if getattr(opt, 'fgr', False):
+        return
     if opt.ransac is None:
         opt.ransac = 1.5 * opt.fpfh
     if opt.ransac_dist is None:
@@ -654,7 +778,9 @@ def check_fpfh_arguments(ap, opt):
 def fpfh_kwargs(opt) -> Dict:
     """`fpfh_register`'s keyword arguments from the parsed --fpfh_* / --ransac_* flags (without V and ICP, and without
     --ransac_overlap, which has no meaning without a network; the normals are always estimated at 2 V, 30, and
-    --normal_* stays ICP's)."""
+    --normal_* stays ICP's).  With --fgr: the features, method='fgr' and fgr_kwargs from the --fgr_* flags."""
+    if getattr(opt, 'fgr', False):
+        return dict(fpfh_radius=opt.fpfh_radius, fpfh_max_nn=opt.fpfh_max_nn, method='fgr', fgr_kwargs=fgr_kwargs(opt))
     return dict(fpfh_radius=opt.fpfh_radius,
                 fpfh_max_nn=opt.fpfh_max_nn, mutual_filter=not opt.fpfh_no_mutual, ransac_radius=opt.ransac,
                 max_iteration=opt.ransac_iters, confidence=opt.ransac_confidence, ransac_n=opt.ransac_n,

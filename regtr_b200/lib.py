@@ -106,6 +106,8 @@ SIGNATURES = {
                        _P, _Z, _P, _Z, _P]),
     'regtr_ransac_ws_bytes': (_Z, [_I, _I, _I, _I, _I]),
     'regtr_ransac': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _I, _c.c_double, _F, _P, _P, _P, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_fgr_ws_bytes': (_Z, [_I, _I, _I]),
+    'regtr_fgr': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _I, _P, _P, _P, _P, _Z, _P]),
     'regtr_estimate_normals_ws_bytes': (_Z, [_I]),
     'regtr_estimate_normals_state_bytes': (_Z, [_I]),
     'regtr_estimate_normals': (_I, [_P, _P, _I, _I, _c.c_double, _F, _I, _P, _P, _P, _P, _Z, _P, _Z, _P]),

@@ -6,6 +6,7 @@ registration after RegTR's pairwise poses).
          [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
         [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
+        [--fgr [--fgr_dist 0.025] [--fgr_iters 64] [--fgr_tuple_test] [--fgr_overlap 0.5] ...]
         [--info_radius D] [--min_overlap 0.3] [--preference_loop_closure 1.0]
         [--voxel V] [--batch_pairs 8]
 
@@ -15,7 +16,8 @@ cropped as `register` does.  Every pair i < j is registered with source j and ta
 direction) in eager forwards of --batch_pairs pairs, then refined by `ops.icp` with --icp as `register --icp` does
 (generalized ICP uses each fragment's normals as source and as target normals).  With --ransac R each pair's pose
 first comes from RANSAC over the network's correspondences (`ops.ransac`, as `register --ransac`), so that far loop
-closures with little overlap survive the network's outlier correspondences; ICP then starts from it.
+closures with little overlap survive the network's outlier correspondences; ICP then starts from it.  --fgr does the
+same with Fast Global Registration over those correspondences (`ops.fgr`, as `register --fgr`) instead of RANSAC.
 `ops.registration_information` at D (default: the config's overlap_radius) gives each pair its fit and information
 matrix.  Edge (source j, target i, X = the pair's pose): j = i + 1 is a certain odometry edge; any other pair is an
 uncertain loop-closure edge when Lambda[5,5] / min(n_j, n_i) >= --min_overlap (Open3D's reconstruction system's gate).
@@ -42,8 +44,9 @@ from typing import Dict, List, Sequence
 import numpy as np
 import torch
 
-from .eval import (add_icp_arguments, add_ransac_arguments, check_icp_arguments, check_ransac_arguments, icp_refine,
-                   ransac_kwargs, ransac_refine)
+from .eval import (add_fgr_arguments, add_icp_arguments, add_ransac_arguments, check_fgr_arguments,
+                   check_icp_arguments, check_ransac_arguments, fgr_kwargs, fgr_refine, icp_refine, ransac_kwargs,
+                   ransac_refine)
 
 
 def parser() -> argparse.ArgumentParser:
@@ -56,6 +59,8 @@ def parser() -> argparse.ArgumentParser:
     add_icp_arguments(ap, 'Refine every pair by ICP, max correspondence distance R')
     add_ransac_arguments(ap, 'Replace every pair\'s pose by RANSAC over the predicted correspondences, max '
                              'correspondence distance R (before ICP with --icp)')
+    add_fgr_arguments(ap, 'Replace every pair\'s pose by Fast Global Registration over the predicted correspondences '
+                          'instead of RANSAC (before ICP with --icp)')
     ap.add_argument('--info_radius', type=float, metavar='D',
                     help='Radius of the information matrices and the line process (default: overlap_radius)')
     ap.add_argument('--min_overlap', type=float, default=0.3,
@@ -74,13 +79,15 @@ def all_pairs(n: int):
 def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8, icp_radius: float = None,
                    icp_iters: int = 30, icp_method: str = 'point_to_point', normal_radius: float = None,
                    normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
-                   icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None) -> np.ndarray:
+                   icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None,
+                   fgr_options: Dict = None) -> np.ndarray:
     """RegTR's final-layer pose of every pair (i, j) of `all_pairs`, source j -> target i, optionally refined by ICP
     (`eval.icp_refine` with icp_method, epsilon=icp_epsilon, loss=icp_loss, loss_k=icp_loss_k; the point-to-plane and
     generalized methods use every fragment's normals, estimated once).
     With ransac_radius, the network's pose is first replaced by `eval.ransac_refine` at that radius (ransac_options:
     its further keyword arguments), pair p of `all_pairs` drawing as pair p whatever batch_pairs; ICP then starts from
-    the RANSAC pose.
+    the RANSAC pose.  fgr_options (a dict, possibly empty): the same with `eval.fgr_refine` and these keyword arguments
+    instead, pair p drawing its tuples as pair p.
     fragments: (n,3) float64 host arrays (already cropped).  -> (P,3,4) float64."""
     from . import ops
     dev = model.device
@@ -99,6 +106,9 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
             if ransac_radius is not None:
                 pose, _ = ransac_refine(pred, [fragments[j] for _, j in chunk], [fragments[i] for i, _ in chunk],
                                         ransac_radius, pair_base=a, **(ransac_options or {}))
+            if fgr_options is not None:
+                pose, _ = fgr_refine(pred, [fragments[j] for _, j in chunk], [fragments[i] for i, _ in chunk],
+                                     pair_base=a, **fgr_options)
             if icp_radius is not None:
                 pose, _ = icp_refine([fragments[j] for _, j in chunk], [fragments[i] for i, _ in chunk], pose,
                                      icp_radius, icp_iters, icp_method, epsilon=icp_epsilon, loss=icp_loss,
@@ -202,6 +212,7 @@ def scene_name(path: str) -> str:
 def main(argv=None):
     ap = parser()
     opt = ap.parse_args(argv)
+    check_fgr_arguments(ap, opt)
     check_icp_arguments(ap, opt)
     check_ransac_arguments(ap, opt)
     from .config import load_config
@@ -217,7 +228,8 @@ def main(argv=None):
     frags = [crop(cfg, np.asarray(load_point_cloud(f), dtype=np.float64)) for f in opt.fragments]
     T = register_pairs(model, frags, opt.batch_pairs, opt.icp, opt.icp_iters, opt.icp_method, opt.normal_radius,
                        opt.normal_max_nn, opt.icp_epsilon, opt.icp_loss, opt.icp_loss_k, opt.ransac,
-                       ransac_kwargs(opt) if opt.ransac is not None else None)
+                       ransac_kwargs(opt) if opt.ransac is not None else None,
+                       dict(fgr_kwargs(opt), overlap=opt.fgr_overlap) if opt.fgr else None)
     D = float(cfg['overlap_radius'] if opt.info_radius is None else opt.info_radius)
     res = optimize_scene(frags, T, D, opt.min_overlap, opt.preference_loop_closure)
     write_outputs(res, opt.out, scene_name(opt.fragments[0]), frags, opt.voxel)

@@ -1712,6 +1712,141 @@ def ransac_feature_matching(src_list, tgt_list, src_feat, tgt_feat, mutual_filte
     return pose, out, n_mutual
 
 
+FGR_MAX_CORR = 21474836             # REGTR_FGR_MAX_CORR
+FGR_MAX_TUPLES = 1 << 20            # REGTR_FGR_MAX_TUPLES
+
+
+class FgrOptions(ctypes.Structure):
+    """regtr_fgr_options (include/regtr_b200.h)."""
+    _fields_ = [('division_factor', ctypes.c_double), ('use_absolute_scale', ctypes.c_int),
+                ('decrease_mu', ctypes.c_int), ('maximum_correspondence_distance', ctypes.c_double),
+                ('iteration_number', ctypes.c_int), ('tuple_scale', ctypes.c_double),
+                ('maximum_tuple_count', ctypes.c_int), ('tuple_test', ctypes.c_int), ('seed', ctypes.c_ulonglong),
+                ('pair_base', ctypes.c_int)]
+
+
+def fgr_launches() -> int:
+    """Kernel launches of one `fgr` call: the preparation (means, scale, compaction, tuple test) and the solve."""
+    return 2
+
+
+def _fgr_check(B, corr_src, corr_tgt, corr_mask, maximum_correspondence_distance, iteration_number, division_factor,
+               tuple_scale, maximum_tuple_count, seed, pair_base):
+    """ValueError for every argument `fgr` rejects, before anything touches the device."""
+    def real(v):
+        return isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, bool)
+
+    def integer(v):
+        return real(v) and int(v) == v
+    if len(corr_src) != B or len(corr_tgt) != B:
+        raise ValueError(f'fgr: {len(corr_src)} / {len(corr_tgt)} correspondence arrays for {B} pairs')
+    if corr_mask is not None and len(corr_mask) != B:
+        raise ValueError(f'fgr: {len(corr_mask)} correspondence masks for {B} pairs')
+    m = 0
+    for b in range(B):
+        a, c = corr_src[b], corr_tgt[b]
+        if len(a.shape) != 2 or a.shape[1] != 3 or tuple(a.shape) != tuple(c.shape):
+            raise ValueError(f'fgr: pair {b}: correspondences {tuple(a.shape)} and {tuple(c.shape)}, expected two '
+                             f'(m,3) arrays')
+        if corr_mask is not None and tuple(corr_mask[b].shape) != (a.shape[0],):
+            raise ValueError(f'fgr: pair {b}: mask {tuple(corr_mask[b].shape)} for {a.shape[0]} correspondences')
+        m += int(a.shape[0])
+    if m > FGR_MAX_CORR:
+        raise ValueError(f'fgr: {m} correspondences in all, at most {FGR_MAX_CORR}')
+    for name, v in (('maximum_correspondence_distance', maximum_correspondence_distance),
+                    ('division_factor', division_factor)):
+        if not (real(v) and math.isfinite(float(v)) and float(v) > 0.0):
+            raise ValueError(f'fgr: {name} {v!r} must be a finite value > 0')
+    if not (integer(iteration_number) and 0 <= int(iteration_number) < 2 ** 31):
+        raise ValueError(f'fgr: iteration_number {iteration_number!r} must be an integer >= 0')
+    if not (real(tuple_scale) and 0.0 < float(tuple_scale) <= 1.0):
+        raise ValueError(f'fgr: tuple_scale {tuple_scale!r} must be in (0, 1]')
+    if not (integer(maximum_tuple_count) and 1 <= int(maximum_tuple_count) <= FGR_MAX_TUPLES):
+        raise ValueError(f'fgr: maximum_tuple_count {maximum_tuple_count!r} must be an integer in 1..{FGR_MAX_TUPLES}')
+    if not (integer(seed) and 0 <= int(seed) < 2 ** 64):
+        raise ValueError(f'fgr: seed {seed!r} must be an integer in [0, 2^64)')
+    if not (integer(pair_base) and 0 <= int(pair_base) <= 2 ** 31 - 1 - B):
+        raise ValueError(f'fgr: pair_base {pair_base!r} must be an integer in [0, 2^31 - 1 - B]')
+
+
+def fgr(src_list, tgt_list, corr_src, corr_tgt, corr_mask=None, *, maximum_correspondence_distance: float = 0.025,
+        iteration_number: int = 64, division_factor: float = 1.4, decrease_mu: bool = True,
+        use_absolute_scale: bool = False, tuple_test: bool = False, tuple_scale: float = 0.95,
+        maximum_tuple_count: int = 1000, seed: int = 0, pair_base: int = 0):
+    """Fast Global Registration of B pairs over correspondences (regtr_fgr): Open3D's
+    registration_fgr_based_on_correspondence with FastGlobalRegistrationOption, with the library's deterministic rule
+    (include/regtr_b200.h, tests/fgr_oracle.py).  Open3D runs no tuple test on given correspondences, hence
+    tuple_test=False by default here.
+    src_list / tgt_list: B clouds (n,3) each, whose means and scale normalise the problem (numpy or torch, any float
+    dtype; stacked in float64 on the device).  corr_src / corr_tgt: B (m,3) arrays each, correspondence i of pair b
+    being corr_src[b][i] -> corr_tgt[b][i]; corr_mask: None or B (m,) boolean arrays, the correspondences that take
+    part.  seed and pair_base + b key the tuple draws, so a pair gets the same result alone or in a batch.
+    -> (pose (B,3,4) float64 source -> target, result (B,4) float64 = correspondences entering the solve, tuples kept,
+    trials walked, final par), both device tensors.  Fewer than 10 correspondences give the identity.  No host sync.
+    Bad arguments raise ValueError before any launch."""
+    B = len(src_list)
+    if B == 0 or len(tgt_list) != B:
+        raise ValueError('fgr: expected as many source as target clouds, at least one pair')
+    corr_src = [torch.as_tensor(c) for c in corr_src]
+    corr_tgt = [torch.as_tensor(c) for c in corr_tgt]
+    corr_mask = None if corr_mask is None else [torch.as_tensor(m) for m in corr_mask]
+    _fgr_check(B, corr_src, corr_tgt, corr_mask, maximum_correspondence_distance, iteration_number, division_factor,
+               tuple_scale, maximum_tuple_count, seed, pair_base)
+    L = _lib.load()
+    dev = next((c.device for c in corr_src if c.is_cuda), None)
+    xyz, offs, lens = _stack_pairs(src_list, tgt_list, 'fgr', dev)
+    dev = xyz.device
+    ca, ms = _stack_clouds(corr_src, dev, 3, 'fgr')
+    cc, _ = _stack_clouds(corr_tgt, dev, 3, 'fgr')
+    m = sum(ms)
+    mask = None
+    if corr_mask is not None:
+        mask = torch.zeros(max(m, 1), dtype=torch.uint8, device=dev)
+        a = 0
+        for b, ln in enumerate(ms):
+            mask[a:a + ln].copy_(corr_mask[b].to(dev) != 0)
+            a += ln
+    coffs = make_offsets(ms, dev)
+    opt = FgrOptions(float(division_factor), int(bool(use_absolute_scale)), int(bool(decrease_mu)),
+                     float(maximum_correspondence_distance), int(iteration_number), float(tuple_scale),
+                     int(maximum_tuple_count), int(bool(tuple_test)), int(seed), int(pair_base))
+    pose = torch.empty((B, 3, 4), dtype=torch.float64, device=dev)
+    out = torch.empty((B, 4), dtype=torch.float64, device=dev)
+    ws = workspace(L.regtr_fgr_ws_bytes(m, B, int(maximum_tuple_count)), dev)
+    _lib.check(L.regtr_fgr(_p(xyz), _p(offs), B, sum(lens), _p(ca), _p(cc), _p(coffs), _p(mask), m,
+                           ctypes.addressof(opt), _p(pose), _p(out), _p(ws), ws.numel(), _stream()), 'regtr_fgr')
+    _count(fgr_launches())
+    return pose, out
+
+
+def fgr_feature_matching(src_list, tgt_list, src_feat, tgt_feat, **fgr_kwargs):
+    """Open3D's registration_fgr_based_on_feature_matching for B pairs: the mutual matches of `feature_match` (its
+    cross check; no fallback), source point i -> its nearest target in feature space, in source order, then `fgr` over
+    them with fgr_kwargs (tuple_test defaults to True here, as in Open3D).
+    -> (pose (B,3,4), result (B,4), n_mutual (B,)): `fgr`'s outputs and the mutual counts.  Arguments `fgr` would
+    reject raise ValueError before any launch."""
+    fgr_kwargs = dict(fgr_kwargs)
+    fgr_kwargs.setdefault('tuple_test', True)
+    B = len(src_list)
+    if B == 0 or len(tgt_list) != B or len(src_feat) != B or len(tgt_feat) != B:
+        raise ValueError(f'fgr_feature_matching: {B} sources, {len(tgt_list)} targets, {len(src_feat)} / '
+                         f'{len(tgt_feat)} feature arrays; expected as many, at least one pair')
+    a = inspect.signature(fgr).bind(src_list, tgt_list, src_list, src_list, **fgr_kwargs)
+    a.apply_defaults()
+    a = a.arguments
+    src = [torch.as_tensor(c) for c in src_list]
+    for b in range(B):
+        if src[b].dim() != 2 or src[b].shape[1] != 3 or src[b].shape[0] != torch.as_tensor(src_feat[b]).shape[0]:
+            raise ValueError(f'fgr_feature_matching: pair {b}: source cloud {tuple(src[b].shape)} for '
+                             f'{tuple(torch.as_tensor(src_feat[b]).shape)} source features')
+    _fgr_check(B, src, src, None, a['maximum_correspondence_distance'], a['iteration_number'],
+               a['division_factor'], a['tuple_scale'], a['maximum_tuple_count'], a['seed'], a['pair_base'])
+    _, corr_tgt, corr_mask, n_mutual = feature_match(src_feat, tgt_feat, tgt_list, True, 0)
+    dev = n_mutual.device
+    pose, out = fgr(src_list, tgt_list, [c.to(dev, torch.float64) for c in src], corr_tgt, corr_mask, **fgr_kwargs)
+    return pose, out, n_mutual
+
+
 def registration_information(src_list, tgt_list, pose, radius: float, status=None):
     """Fit and information matrices of B registered pairs from one `overlap_nn` (regtr_registration_fit and
     regtr_registration_information on the same matches): Open3D's evaluate_registration and

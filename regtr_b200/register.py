@@ -6,8 +6,10 @@
          [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
         [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
+        [--fgr [--fgr_dist 0.025] [--fgr_iters 64] [--fgr_division 1.4] [--fgr_tuple_test [--fgr_tuple_scale 0.95]
+         [--fgr_max_tuples 1000]] [--fgr_no_decrease_mu] [--fgr_absolute_scale] [--fgr_overlap 0.5] [--fgr_seed 0]]
     python -m regtr_b200.register SRC TGT --fpfh V [--fpfh_radius FR] [--fpfh_max_nn 100] [--fpfh_no_mutual]
-        [--ransac R ...] [--icp R ...] [--fit_radius R] [--out DIR]
+        [--ransac R ... | --fgr [--fgr_dist D] [--fgr_no_tuple_test] ...] [--icp R ...] [--fit_radius R] [--out DIR]
 
 SRC / TGT: .ply, .pth, .bin or .npy (regtr_b200.pointio).  The config is the config.yaml one level above the
 checkpoint's directory, the layout `python -m regtr_b200.train` writes, unless --config names another.  Instead of the
@@ -35,9 +37,16 @@ correspondence distance R on the cropped full-resolution clouds, --ransac_iters 
 checker at --ransac_dist); with --icp as well, ICP starts from the RANSAC pose (Open3D's global-then-local pipeline).
 result.npz then gains pose_coarse, pose_ransac (3,4) float64 and ransac (5,) = fitness, inlier_rmse, hypotheses
 walked, hypotheses validated, winning hypothesis.
+With --fgr (instead of --ransac) the final decoder layer's pose is replaced by Fast Global Registration over the same
+correspondences with predicted overlap above --fgr_overlap (`ops.fgr`, Open3D's registration_fgr_based_on_correspondence
+with FastGlobalRegistrationOption: --fgr_dist the maximum correspondence distance, --fgr_iters iterations, --fgr_division,
+--fgr_no_decrease_mu, --fgr_absolute_scale, and the tuple test only with --fgr_tuple_test); with --icp as well, ICP
+starts from the FGR pose.  result.npz then gains pose_coarse, pose_fgr (3,4) float64 and fgr (4,) = correspondences of
+the solve, tuples kept, trials walked, final GNC parameter.
 One JSON line on stdout: the pose, the four fit numbers and the point counts (with --icp, also icp_fitness, icp_rmse,
 icp_iterations, icp_radius and icp_method, and icp_loss, icp_loss_k and icp_epsilon when they are given; with --ransac,
-ransac_fitness, ransac_rmse, ransac_iterations, ransac_validations and ransac_radius).
+ransac_fitness, ransac_rmse, ransac_iterations, ransac_validations and ransac_radius; with --fgr, fgr_correspondences,
+fgr_tuples, fgr_trials, fgr_par and fgr_dist).
 With --fpfh V there is no network and no --ckpt: Open3D's classical global registration (`eval.fpfh_register`) on the
 device.  Both clouds are downsampled at voxel V (`ops.grid_subsample`, a grid anchored at the origin), their normals
 estimated at 2 V with 30 neighbours at most, their FPFH features computed at --fpfh_radius (default 5 V) with
@@ -48,6 +57,10 @@ refines the pose on the full clouds as above, and fit is taken at --fit_radius (
 Written: pose.txt, src_registered.ply and result.npz with pose_fpfh (3,4) float64, ransac (5,), n_mutual, fit and,
 with --icp, pose_icp and icp; no keypoint files.  The JSON line has the pose, the fit numbers, the point counts,
 fpfh_voxel, n_src_down, n_tgt_down, n_mutual and the ransac_* (and icp_*) entries.
+With --fpfh V --fgr the mutual FPFH matches go to FGR instead (`ops.fgr_feature_matching`, the tuple test on unless
+--fgr_no_tuple_test, --fgr_dist defaulting to 0.5 V as in Open3D's tutorial); --fpfh_no_mutual is then a usage error,
+and fit is taken at --fit_radius (default 1.5 V).  result.npz holds pose_fpfh (the FGR pose) and fgr (4,) in place of
+ransac, and the JSON line has the fgr_* entries in place of the ransac_* ones.
 """
 from __future__ import annotations
 
@@ -60,9 +73,9 @@ from typing import Dict
 import numpy as np
 import torch
 
-from .eval import (add_fpfh_arguments, add_icp_arguments, add_ransac_arguments, check_fpfh_arguments,
-                   check_icp_arguments, check_ransac_arguments, fpfh_kwargs, fpfh_register, icp_kwargs, icp_refine,
-                   ransac_kwargs, ransac_refine)
+from .eval import (add_fgr_arguments, add_fpfh_arguments, add_icp_arguments, add_ransac_arguments,
+                   check_fgr_arguments, check_fpfh_arguments, check_icp_arguments, check_ransac_arguments, fgr_kwargs,
+                   fgr_refine, fpfh_kwargs, fpfh_register, icp_kwargs, icp_refine, ransac_kwargs, ransac_refine)
 
 
 def parser() -> argparse.ArgumentParser:
@@ -80,6 +93,8 @@ def parser() -> argparse.ArgumentParser:
     add_icp_arguments(ap, 'Refine the pose with point-to-point ICP, max correspondence distance R (default: no ICP)')
     add_ransac_arguments(ap, 'Replace the pose by RANSAC over the predicted correspondences, max correspondence '
                              'distance R (default: no RANSAC; before ICP with --icp; with --fpfh 1.5 V)')
+    add_fgr_arguments(ap, 'Replace the pose by Fast Global Registration over the predicted correspondences (with '
+                          '--fpfh: over the FPFH matches) instead of RANSAC; before ICP with --icp')
     add_fpfh_arguments(ap)
     ap.add_argument('--out', default='.', help='Output directory')
     return ap
@@ -89,11 +104,12 @@ def parse_args(argv=None):
     """The parsed command line, its usage errors raised and the --fpfh defaults filled in."""
     ap = parser()
     opt = ap.parse_args(argv)
+    check_fgr_arguments(ap, opt)
     check_fpfh_arguments(ap, opt)
     check_icp_arguments(ap, opt)
     check_ransac_arguments(ap, opt)
     if opt.fpfh is not None and opt.fit_radius is None:
-        opt.fit_radius = opt.ransac
+        opt.fit_radius = 1.5 * opt.fpfh if opt.fgr else opt.ransac
     return opt
 
 
@@ -122,7 +138,8 @@ def load_model(cfg, ckpt: str, device=None):
 def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: float = None,
              icp_radius: float = None, icp_iters: int = 30, icp_method: str = 'point_to_point',
              normal_radius: float = None, normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
-             icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None) -> Dict:
+             icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None,
+             fgr_options: Dict = None) -> Dict:
     """Crop, forward and fit one pair.  src_xyz / tgt_xyz (N,3) float64 host arrays.
     -> dict of host arrays: src_xyz / tgt_xyz (cropped, float64), pose (L,3,4) fp32, src_kp, src_kp_warped (final
     layer), src_overlap (sigmoid of the final layer's logit, (n,)), the same for tgt, fit (4,) float64.
@@ -132,7 +149,9 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
     icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations.
     ransac_radius: first replace the final layer's pose by `eval.ransac_refine` at that radius on the cropped clouds,
     with ransac_options its further keyword arguments (ICP then starts from it); the dict gains pose_coarse,
-    pose_ransac (3,4) float64 and ransac (5,) float64 = fitness, inlier_rmse, walked, validated, winner."""
+    pose_ransac (3,4) float64 and ransac (5,) float64 = fitness, inlier_rmse, walked, validated, winner.
+    fgr_options: likewise, but `eval.fgr_refine` with these keyword arguments (overlap and `ops.fgr`'s options); the
+    dict gains pose_coarse, pose_fgr (3,4) float64 and fgr (4,) float64 = correspondences, tuples, trials, par."""
     from . import ops
     src_xyz = crop(cfg, np.asarray(src_xyz, dtype=np.float64))
     tgt_xyz = crop(cfg, np.asarray(tgt_xyz, dtype=np.float64))
@@ -148,6 +167,9 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
         if ransac_radius is not None:
             final, ransac = ransac_refine(out, [src_xyz], [tgt_xyz], ransac_radius, **(ransac_options or {}))
             pose_ransac = final
+        if fgr_options is not None:
+            final, fgr = fgr_refine(out, [src_xyz], [tgt_xyz], **fgr_options)
+            pose_fgr = final
         if icp_radius is not None:
             final, icp = icp_refine([src_xyz], [tgt_xyz], final, icp_radius, icp_iters, icp_method, normal_radius,
                                     normal_max_nn, icp_epsilon, icp_loss, icp_loss_k)
@@ -158,6 +180,8 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
         if ransac_radius is not None:
             res.update(pose_coarse=res['pose'][-1], pose_ransac=pose_ransac[0].cpu().numpy(),
                        ransac=ransac[0].cpu().numpy())
+        if fgr_options is not None:
+            res.update(pose_coarse=res['pose'][-1], pose_fgr=pose_fgr[0].cpu().numpy(), fgr=fgr[0].cpu().numpy())
         for side in ('src', 'tgt'):
             res[f'{side}_kp'] = out[f'{side}_kp'][0].cpu().numpy()
             res[f'{side}_kp_warped'] = out[f'{side}_kp_warped'][0][-1].cpu().numpy()
@@ -171,16 +195,17 @@ def register_fpfh(src_xyz: np.ndarray, tgt_xyz: np.ndarray, voxel: float, fit_ra
                   icp_radius: float = None, icp_options: Dict = None, fpfh_options: Dict = None) -> Dict:
     """One pair without a network (`eval.fpfh_register` at voxel, fpfh_options its further keyword arguments, then ICP
     on the full clouds with icp_radius and icp_options).  -> dict of host arrays: src_xyz / tgt_xyz (float64),
-    pose_fpfh (3,4) float64, ransac (5,), n_mutual, n_src_down, n_tgt_down, fit (4,) of the final pose at fit_radius,
-    and pose_icp / icp with icp_radius."""
+    pose_fpfh (3,4) float64, ransac (5,) (fgr (4,) with method='fgr' in fpfh_options), n_mutual, n_src_down,
+    n_tgt_down, fit (4,) of the final pose at fit_radius, and pose_icp / icp with icp_radius."""
     from . import ops
     src_xyz = np.asarray(src_xyz, dtype=np.float64)
     tgt_xyz = np.asarray(tgt_xyz, dtype=np.float64)
     out = fpfh_register([src_xyz], [tgt_xyz], voxel, icp_radius=icp_radius, icp_kwargs=icp_options,
                         **(fpfh_options or {}))
     fit = ops.registration_fit([src_xyz], [tgt_xyz], out['pose'], fit_radius)
+    glob = 'fgr' if 'fgr' in out else 'ransac'
     res = {'src_xyz': src_xyz, 'tgt_xyz': tgt_xyz, 'pose_fpfh': out['pose_fpfh'][0].cpu().numpy(),
-           'ransac': out['ransac'][0].cpu().numpy(), 'n_mutual': int(out['n_mutual'][0]),
+           glob: out[glob][0].cpu().numpy(), 'n_mutual': int(out['n_mutual'][0]),
            'n_src_down': int(out['src_down'][0].shape[0]), 'n_tgt_down': int(out['tgt_down'][0].shape[0]),
            'fit': fit[0].cpu().numpy()}
     if icp_radius is not None:
@@ -200,9 +225,9 @@ def pose_text(pose34) -> str:
 
 
 def final_pose(res: Dict):
-    """The pose `register` settles on: ICP's, else RANSAC's (over network or FPFH matches), else the final decoder
-    layer's."""
-    for k in ('pose_icp', 'pose_ransac', 'pose_fpfh'):
+    """The pose `register` settles on: ICP's, else RANSAC's or FGR's (over network or FPFH matches), else the final
+    decoder layer's."""
+    for k in ('pose_icp', 'pose_ransac', 'pose_fgr', 'pose_fpfh'):
         if k in res:
             return res[k]
     return res['pose'][-1]
@@ -217,7 +242,8 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
     p = final.astype(np.float64)
     write_ply(os.path.join(out_dir, 'src_registered.ply'), res['src_xyz'] @ p[:, :3].T + p[:, 3])
     if 'pose_fpfh' in res:
-        keys = ('pose_fpfh', 'ransac', 'n_mutual', 'fit') + (('pose_icp', 'icp') if 'pose_icp' in res else ())
+        keys = ('pose_fpfh', 'fgr' if 'fgr' in res else 'ransac', 'n_mutual', 'fit') + \
+            (('pose_icp', 'icp') if 'pose_icp' in res else ())
         np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
         return 0
     keys = ('pose', 'src_kp', 'src_kp_warped', 'src_overlap', 'tgt_kp', 'tgt_kp_warped', 'tgt_overlap', 'fit')
@@ -225,6 +251,8 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
         keys += ('pose_coarse',)
     if 'pose_ransac' in res:
         keys += ('pose_ransac', 'ransac')
+    if 'pose_fgr' in res:
+        keys += ('pose_fgr', 'fgr')
     if 'pose_icp' in res:
         keys += ('pose_icp', 'icp')
     np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
@@ -247,7 +275,8 @@ def main(argv=None):
     model = load_model(cfg, opt.ckpt)
     res = register(model, cfg, load_point_cloud(opt.src), load_point_cloud(opt.tgt), opt.fit_radius, opt.icp,
                    opt.icp_iters, opt.icp_method, opt.normal_radius, opt.normal_max_nn, opt.icp_epsilon,
-                   opt.icp_loss, opt.icp_loss_k, opt.ransac, ransac_kwargs(opt) if opt.ransac is not None else None)
+                   opt.icp_loss, opt.icp_loss_k, opt.ransac, ransac_kwargs(opt) if opt.ransac is not None else None,
+                   dict(fgr_kwargs(opt), overlap=opt.fgr_overlap) if opt.fgr else None)
     n_shown = write_outputs(res, opt.out, opt.threshold)
     f = [float(v) for v in res['fit']]
     line = {'pose': pose44(final_pose(res)).tolist(),
@@ -262,8 +291,17 @@ def main(argv=None):
         rs = [float(v) for v in res['ransac']]
         line.update(ransac_fitness=rs[0], ransac_rmse=rs[1], ransac_iterations=int(rs[2]),
                     ransac_validations=int(rs[3]), ransac_radius=float(opt.ransac))
+    if opt.fgr:
+        line.update(fgr_line(opt, res['fgr']))
     print(json.dumps(line))
     return res
+
+
+def fgr_line(opt, fgr) -> Dict:
+    """The JSON line's fgr_* entries."""
+    fgr = [float(v) for v in fgr]
+    return dict(fgr_correspondences=int(fgr[0]), fgr_tuples=int(fgr[1]), fgr_trials=int(fgr[2]), fgr_par=fgr[3],
+                fgr_dist=float(opt.fgr_dist))
 
 
 def icp_line(opt, icp) -> Dict:
@@ -284,13 +322,16 @@ def main_fpfh(opt, src_xyz, tgt_xyz):
                         icp_kwargs(opt) if opt.icp is not None else None, fpfh_kwargs(opt))
     write_outputs(res, opt.out)
     f = [float(v) for v in res['fit']]
-    rs = [float(v) for v in res['ransac']]
     line = {'pose': pose44(final_pose(res)).tolist(), 'fitness_src': f[0], 'rmse_src': f[1], 'fitness_tgt': f[2],
             'rmse_tgt': f[3], 'n_src': int(res['src_xyz'].shape[0]), 'n_tgt': int(res['tgt_xyz'].shape[0]),
             'fit_radius': float(opt.fit_radius), 'fpfh_voxel': float(opt.fpfh), 'n_src_down': res['n_src_down'],
-            'n_tgt_down': res['n_tgt_down'], 'n_mutual': res['n_mutual'], 'ransac_fitness': rs[0],
-            'ransac_rmse': rs[1], 'ransac_iterations': int(rs[2]), 'ransac_validations': int(rs[3]),
-            'ransac_radius': float(opt.ransac)}
+            'n_tgt_down': res['n_tgt_down'], 'n_mutual': res['n_mutual']}
+    if opt.fgr:
+        line.update(fgr_line(opt, res['fgr']))
+    else:
+        rs = [float(v) for v in res['ransac']]
+        line.update(ransac_fitness=rs[0], ransac_rmse=rs[1], ransac_iterations=int(rs[2]),
+                    ransac_validations=int(rs[3]), ransac_radius=float(opt.ransac))
     if opt.icp is not None:
         line.update(icp_line(opt, res['icp']))
     print(json.dumps(line))

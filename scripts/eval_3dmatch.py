@@ -6,9 +6,10 @@
         [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
         [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
+        [--fgr [--fgr_dist 0.025] [--fgr_iters 64] [--fgr_tuple_test] [--fgr_overlap 0.5] ...]
     python scripts/eval_3dmatch.py --root <data/indoor> --info <test_3DMatch_info.pkl> \
         --gt <datasets/3dmatch/benchmarks/3DMatch> --fpfh V [--fpfh_radius FR] [--fpfh_max_nn 100] [--fpfh_no_mutual]
-        [--ransac R ...] [--icp R ...] --out logs/3DMatch_fpfh
+        [--ransac R ... | --fgr [--fgr_dist D] [--fgr_no_tuple_test] ...] [--icp R ...] --out logs/3DMatch_fpfh
 
 --icp R refines every final pose by ICP on the full clouds (`ops.icp`, max correspondence distance R; point-to-point,
 or point-to-plane against target normals from `ops.estimate_normals` at NR, default 2 R, or generalized ICP on the
@@ -17,9 +18,12 @@ refined poses, and the metrics report both (`rot_err_deg` / `trans_err` refined,
 --ransac R replaces every network pose by RANSAC over the network's correspondences with predicted overlap above
 --ransac_overlap (`ops.ransac`, max correspondence distance R, validated on the full clouds); with --icp as well, ICP
 starts from the RANSAC pose, and the metrics also report `*_ransac`.
+--fgr replaces them by Fast Global Registration over the same correspondences instead (`ops.fgr`, --fgr_* options;
+`*_fgr` with --icp).
 --fpfh V (no --ckpt) scores the classical baseline instead of a network: `eval.fpfh_forward`, FPFH features of the
 clouds downsampled at V matched in feature space, then RANSAC (radius --ransac, default 1.5 V), and ICP after it with
---icp (the metrics then also report `*_fpfh`).
+--icp (the metrics then also report `*_fpfh`); with --fgr, FGR over the mutual feature matches replaces RANSAC
+(--fgr_dist defaulting to 0.5 V).
 Needs the dataset and trained weights (neither is available offline: SURVEY.md 8f N1)."""
 import argparse, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -37,12 +41,14 @@ def parser():
     E.add_icp_arguments(ap, 'Refine the poses by ICP with this max correspondence distance')
     E.add_ransac_arguments(ap, 'Replace the poses by RANSAC over the predicted correspondences, max correspondence '
                                'distance R (before ICP with --icp; with --fpfh 1.5 V)')
+    E.add_fgr_arguments(ap, 'Replace the poses by Fast Global Registration over the predicted correspondences (with '
+                            '--fpfh: over the FPFH matches) instead of RANSAC; before ICP with --icp')
     E.add_fpfh_arguments(ap)
     return ap
 
 
 def network_forward(args):
-    """The checkpoint's forward on the CUDA graph, with RANSAC and / or ICP after it as the flags ask."""
+    """The checkpoint's forward on the CUDA graph, with RANSAC or FGR and / or ICP after it as the flags ask."""
     dev = torch.device('cuda:0')
     cfg = get_config('3dmatch')
     model = RegTR(cfg).to(dev).eval()
@@ -52,6 +58,9 @@ def network_forward(args):
     if args.ransac is not None:
         return E.ransac_forward(lambda b: runner(b), args.ransac, **E.ransac_kwargs(args), icp_radius=args.icp,
                                 icp_kwargs=E.icp_kwargs(args))
+    if args.fgr:
+        return E.fgr_forward(lambda b: runner(b), args.fgr_overlap, icp_radius=args.icp, icp_kwargs=E.icp_kwargs(args),
+                             **E.fgr_kwargs(args))
     return (lambda b: runner(b)) if args.icp is None else E.icp_forward(
         lambda b: runner(b), args.icp, args.icp_iters, method=args.icp_method, normal_radius=args.normal_radius,
         normal_max_nn=args.normal_max_nn, epsilon=args.icp_epsilon, loss=args.icp_loss, loss_k=args.icp_loss_k)
@@ -60,6 +69,7 @@ def network_forward(args):
 def main(argv=None):
     ap = parser()
     args = ap.parse_args(argv)
+    E.check_fgr_arguments(ap, args)
     E.check_fpfh_arguments(ap, args)
     E.check_icp_arguments(ap, args)
     E.check_ransac_arguments(ap, args)
