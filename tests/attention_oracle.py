@@ -15,6 +15,7 @@ queries share), so these catch errors that zero-mean inputs hide.
 """
 import math
 
+import numpy as np
 import torch
 
 from grad_yardstick import FACTOR, FLOOR
@@ -215,6 +216,89 @@ def forward_reference(q, k, v, problems, n_heads, dtype):
         o[qs:qs + ql] = (torch.softmax(s, -1) @ _heads(v, ks, kl, n_heads)).transpose(0, 1).reshape(ql, E)
         lse[qs:qs + ql] = (torch.logsumexp(s, -1) / math.log(2)).transpose(0, 1)
     return o, lse
+
+
+LOG2E = 1.4426950408889634
+
+
+def round_bf16(x):
+    """x rounded to the nearest bfloat16 value, ties to even, kept in x's dtype.  float32 goes through
+    gemm_oracle.bf16_rne, the rounding of the kernels' fp32 -> bf16 conversions.  float64 is rounded once, from the
+    float64 value itself: x / ulp is exact, so torch.round (half to even) rounds it.  bf16 has fp32's exponent range,
+    so below 2^-126 the ulp stays 2^-133 (subnormals)."""
+    if x.dtype == torch.float32:
+        import gemm_oracle as go
+        u = torch.from_numpy(go.bf16_rne(x.detach().contiguous().numpy()).astype(np.int32)) << 16
+        return u.view(torch.float32).view(x.shape)
+    _, e = torch.frexp(x)                                                   # |x| in [2^(e-1), 2^e)
+    ulp = torch.pow(2.0, (e.clamp_min(-125) - 8).to(x.dtype))
+    return torch.round(x / ulp) * ulp
+
+
+def bf16_forward_reference(qk, vt, problems, n_heads, dtype, round_p=True):
+    """The bf16 wgmma core's operation (csrc/attention_tc.cu) in `dtype` on the CPU, on the bf16 tensors it reads:
+    qk [n, >= 2E] (q | k columns) and vt [E, >= n] (v transposed).  Per problem with queries and keys, and head:
+    s = q k^T, m = max_j s over the problem's keys, p = bf16(exp2((s - m) * scale * log2 e)), l = sum_j p of the rounded
+    p, O = (sum_j p_j v_j) / l.  round_p=False leaves p unrounded (then this is softmax(q k^T * scale) v).
+    -> dict: o [n, E] (0 on rows outside every problem, as on the rows of a problem without keys), l [n, n_heads] (sum
+    of the p used), l_exact [n, n_heads] (sum of the unrounded p), p: per such problem the p used, [n_heads, q_len,
+    k_len] bfloat16 when rounded (every value is a bf16 one), and in float64 with rounding the near ties (`ties`)."""
+    E = n_heads * HD
+    n = qk.shape[0]
+    q, k = qk[:, :E].to(dtype), qk[:, E:2 * E].to(dtype)
+    v = vt[:, :n].t().to(dtype)
+    c = SCALE * LOG2E
+    o = torch.zeros(n, E, dtype=dtype)
+    l, l_exact = torch.zeros(n, n_heads, dtype=dtype), torch.zeros(n, n_heads, dtype=dtype)
+    tie = dtype == torch.float64 and round_p
+    allow, n_ties, tie_masks = torch.zeros(n, E, dtype=dtype), 0, []
+    ps = []
+    for qs, ql, ks, kl in problems:
+        if ql == 0 or kl == 0:
+            continue
+        Q, K, V = _heads(q, qs, ql, n_heads), _heads(k, ks, kl, n_heads), _heads(v, ks, kl, n_heads)
+        s = Q @ K.transpose(1, 2)
+        pe = torch.exp2((s - s.amax(-1, keepdim=True)) * c)
+        p = round_bf16(pe) if round_p else pe
+        l_exact[qs:qs + ql] = pe.sum(-1).t()
+        lp = p.sum(-1, keepdim=True)
+        l[qs:qs + ql] = lp[..., 0].t()
+        out = p @ V / lp
+        o[qs:qs + ql] = out.transpose(0, 1).reshape(ql, E)
+        if tie:
+            # the p an fp32 computation may round to the other neighbour: within its error of a rounding midpoint.
+            # Error of the exponent: s and m summed from 32 products in fp32 (at most 2^-19 sum_d |q_d k_d| each),
+            # the products with c and their difference (2^-22 (|s| + |m|) c); exp2 and the rest: 2^-21 of p.
+            a = Q.abs() @ K.abs().transpose(1, 2)
+            m_abs = s.abs().amax(-1, keepdim=True)
+            tau = (2.0 ** -19 * (a + a.amax(-1, keepdim=True)) + 2.0 ** -22 * (s.abs() + m_abs)) * c * math.log(2) \
+                + 2.0 ** -21
+            del a
+            _, e = torch.frexp(pe)
+            ulp = torch.pow(2.0, (e.clamp_min(-125) - 8).to(dtype))
+            near = (ulp / 2 - (pe - p).abs()) <= tau * pe
+            w = torch.where(near, ulp, torch.zeros_like(ulp)) / lp                # one flip moves O_i by w_ij (v_j - O_i)
+            allow[qs:qs + ql] = (w @ V.abs() + w.sum(-1, keepdim=True) * out.abs()).transpose(0, 1).reshape(ql, E)
+            n_ties += int(near.sum())
+            tie_masks.append(near)
+        del s, pe
+        ps.append(p.to(torch.bfloat16) if round_p else p)
+    r = dict(o=o, l=l, l_exact=l_exact, p=ps)
+    if tie:
+        r['ties'] = dict(allow=allow, count=n_ties, masks=tie_masks)
+    return r
+
+
+def beyond_ties(got, ref, allow):
+    """got with its deviation from ref shrunk by `allow` (bf16_forward_reference's ties['allow']): what is left is the
+    part no set of near-tie roundings can explain."""
+    d = got.detach().double() - ref.double()
+    return ref.double() + d.sign() * (d.abs() - allow.double()).clamp_min(0)
+
+
+def p_flips(a, b):
+    """(entries of p that differ, entries) between two runs of bf16_forward_reference."""
+    return sum(int((x != y).sum()) for x, y in zip(a['p'], b['p'])), sum(x.numel() for x in a['p'])
 
 
 def per_problem(name, problems, n_heads, hd, got, fp32, ref):
