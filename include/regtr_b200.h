@@ -342,7 +342,7 @@ int regtr_mha_varlen_bwd(const float* Q, int ldq, const float* K, int ldk, const
 /* Backward of regtr_layernorm_pos: dy and dy_pos (either may be NULL; they add) are the gradients of y and y_pos,
  * dres (optional) a gradient of x arriving through a residual connection, added to dx.  Mean and rstd are
  * recomputed from x.  dgamma / dbeta (E) from per-block column partials summed in a fixed order.  E % 32 == 0,
- * E <= 256.  ws: regtr_layernorm_bwd_ws_bytes(n, E) bytes.
+ * E <= 256.  ws: regtr_layernorm_bwd_ws_bytes(n, E) bytes.  n = 0 writes dgamma = dbeta = 0 (x and dx may be NULL).
  * drop (optional; offs, dz and drop are all NULL or all set): the backward of the residual dropout, with x = the
  * forward's x_out: dx is the gradient of x' (dres included), plus dz = dx m scale. */
 size_t regtr_layernorm_bwd_ws_bytes(int n, int E);

@@ -496,7 +496,8 @@ int regtr_layernorm_bwd(const float* x, const float* gamma, const float* dy, con
     if (drop && drop_key_of(drop, dk) != REGTR_OK) return REGTR_ERR_ARG;
     if (n < 0 || E <= 0 || E % 32 != 0) return REGTR_ERR_ARG;
     if (E > 32 * LN_PER) return REGTR_ERR_UNSUPPORTED;
-    if (!x || !gamma || !dx || !dgamma || !dbeta) return REGTR_ERR_ARG;
+    // n = 0 (empty tensors, null pointers) still writes dgamma = dbeta = 0
+    if (!gamma || !dgamma || !dbeta || (n > 0 && (!x || !dx))) return REGTR_ERR_ARG;
     if (!ws || ws_bytes < regtr_layernorm_bwd_ws_bytes(n, E)) return REGTR_ERR_WORKSPACE;
     float* part = (float*)ws;
     const int nb = n > 0 ? regtr_cdiv(n, LNB_ROWS) : 0;

@@ -1,6 +1,7 @@
-"""GPU tests of the backward kernels (attention core, LayerNorm, dense layers) and of RegTR.forward_train: op by op
-against float64 torch autograd of the same math, bit-for-bit determinism, and the model's parameter gradients
-against the unmodified reference's own backward (tests/golden/grad.npz) and against the CPU oracle's autograd."""
+"""GPU tests of the attention-core backward and of RegTR.forward_train: the op against float64 torch autograd of the
+same math, bit-for-bit determinism, and the model's parameter gradients against the unmodified reference's own
+backward (tests/golden/grad.npz) and against the CPU oracle's autograd.  The LayerNorm and dense-layer backward are
+in tests/test_gpu_train_ops.py."""
 import math
 import os
 import sys
@@ -117,75 +118,6 @@ def test_attention_backward_matches_float64(kind):
     d2 = torch.zeros_like(qkv)
     ops.mha_varlen_bwd(q, k, v, o, lse, d_o, d2[:, :E], d2[:, E:2 * E], d2[:, 2 * E:], qs, ql, ks, kl, max_q, max_k, H)
     assert torch.equal(d, d2)
-
-
-# ---------------------------------------------------------------------------------------------------- LayerNorm
-
-@pytest.mark.parametrize('with_dres', [False, True])
-@pytest.mark.parametrize('grads', ['dy', 'dy_pos', 'both'])
-def test_layernorm_backward_matches_float64(grads, with_dres):
-    from regtr_b200 import ops
-    g = torch.Generator().manual_seed(3)
-    n, E = 301, 256
-    x = (torch.randn(n, E, generator=g) * 2 + 0.5)
-    gamma, beta = torch.randn(E, generator=g), torch.randn(E, generator=g)
-    pos = torch.randn(n, E, generator=g)
-    dy = torch.randn(n, E, generator=g) if grads in ('dy', 'both') else None
-    dyp = torch.randn(n, E, generator=g) if grads in ('dy_pos', 'both') else None
-    dres = torch.randn(n, E, generator=g) if with_dres else None
-    G = lambda t: None if t is None else t.to(DEV).contiguous()
-    dx, dg, db = ops.layernorm_bwd(G(x), G(gamma), G(dy), G(dyp), G(dres), 1e-5)
-    dx2, dg2, db2 = ops.layernorm_bwd(G(x), G(gamma), G(dy), G(dyp), G(dres), 1e-5)
-    assert torch.equal(dx, dx2) and torch.equal(dg, dg2) and torch.equal(db, db2)
-    xr, gr, br = (t.double().requires_grad_(True) for t in (x, gamma, beta))
-    y = torch.nn.functional.layer_norm(xr, (E,), gr, br, 1e-5)
-    loss = 0
-    if dy is not None:
-        loss = loss + (y * dy.double()).sum()
-    if dyp is not None:
-        loss = loss + ((y + pos.double()) * dyp.double()).sum()
-    loss.backward()
-    want_dx = xr.grad + (dres.double() if dres is not None else 0)
-    errs = dict(dx=_rel(dx.cpu(), want_dx), dgamma=_rel(dg.cpu(), gr.grad), dbeta=_rel(db.cpu(), br.grad))
-    assert max(errs.values()) <= 1e-5, errs
-
-
-# ------------------------------------------------------------------------------------------------- dense layers
-
-@pytest.mark.parametrize('K,N,relu,residual', [(256, 768, False, False), (256, 1024, True, False),
-                                               (1024, 256, False, True), (256, 256, True, False),
-                                               (256, 3, False, False), (256, 1, False, False)])
-@pytest.mark.parametrize('M', [1, 37, 1503])
-def test_linear_backward_matches_float64(M, K, N, relu, residual):
-    from regtr_b200 import ops
-    g = torch.Generator().manual_seed(M * 7 + N)
-    x = torch.randn(M, K, generator=g)
-    w = torch.randn(N, K, generator=g) / math.sqrt(K)
-    b = torch.randn(N, generator=g)
-    r = torch.randn(M, N, generator=g) if residual else None
-    gy = torch.randn(M, N, generator=g)
-
-    def run():
-        xs, ws, bs = (t.to(DEV).requires_grad_(True) for t in (x, w, b))
-        rs = r.to(DEV).requires_grad_(True) if residual else None
-        y = ops.linear(xs, ws, bs, residual=rs, relu=relu)
-        y.backward(gy.to(DEV))
-        return y.detach(), xs.grad, ws.grad, bs.grad, (rs.grad if residual else None)
-
-    y, dx, dw, db, dr = run()
-    y2, dx2, dw2, db2, dr2 = run()
-    assert torch.equal(dx, dx2) and torch.equal(dw, dw2) and torch.equal(db, db2)
-    xr, wr, br = (t.double().requires_grad_(True) for t in (x, w, b))
-    rr = r.double().requires_grad_(True) if residual else None
-    yr = xr @ wr.t() + br + (rr if residual else 0)
-    if relu:
-        yr = torch.relu(yr)
-    yr.backward(gy.double())
-    errs = dict(y=_rel(y.cpu(), yr.detach()), dx=_rel(dx.cpu(), xr.grad), dw=_rel(dw.cpu(), wr.grad),
-                db=_rel(db.cpu(), br.grad))
-    if residual:
-        errs['dres'] = _rel(dr.cpu(), rr.grad)
-    assert max(errs.values()) <= 1e-5, errs
 
 
 # ------------------------------------------------------------------------------------------------ whole model
