@@ -589,7 +589,19 @@ int regtr_transform_clouds(const double* xyz, const int32_t* offs, int C, int n_
  * residual row of point-to-plane (r = (p - q) . n) or generalized ICP by Open3D's RobustKernel::Weight(r):
  * huber 1 if |r| <= k else k / |r|; cauchy 1 / (1 + (r/k)^2); gm k / (k + r^2)^2; tukey (1 - (r/k)^2)^2 if |r| <= k
  * else 0.  REGTR_ERR_ARG: src_normals without tgt_normals, a loss other than L2 without tgt_normals, an unknown loss,
- * loss_k not > 0 or not finite with a loss other than L2, epsilon outside (0, 1].  Same launches in every mode. */
+ * loss_k not > 0 or not finite with a loss other than L2, epsilon outside (0, 1].  Same launches in every mode.
+ * opt->src_colors non-NULL (needs tgt_normals, opt->tgt_colors and opt->tgt_color_gradients, and no src_normals):
+ * colored ICP (Open3D's registration_colored_icp with TransformationEstimationForColoredICP(lambda_geometric, kernel)),
+ * with the correspondences, fitness, RMSE (point distances), stop test and update of point-to-plane.  src_colors
+ * (offs[B], 3) and tgt_colors (offs[2B] - offs[B], 3) float64 rgb stacked like their clouds, intensity
+ * ((r + g) + b) / 3; tgt_color_gradients (offs[2B] - offs[B], 3) float64 (regtr_color_gradients).  Per correspondence
+ * (p moved source, q target, n its normal, d its gradient, l = lambda_geometric), two residual rows, each into J^T J
+ * and J^T r with weight loss(r) of its own r: geometric r = sqrt(l) (p - q) . n, J = [p x sqrt(l) n ; sqrt(l) n];
+ * photometric, with p' = p - ((p - q) . n) n, is0 = d . (p' - q) + it_q and m = (d . n) n - d (= -(I - n n^T) d):
+ * r = sqrt(1 - l) (is_p - is0), J = [p x sqrt(1 - l) m ; sqrt(1 - l) m].  A zero target normal drops its
+ * correspondence out of the update, not out of k.  REGTR_ERR_ARG: lambda_geometric outside [0, 1], tgt_colors or
+ * tgt_color_gradients without src_colors, or src_colors without tgt_normals, tgt_colors or tgt_color_gradients, or
+ * with src_normals. */
 #define REGTR_ICP_LOSS_L2 0
 #define REGTR_ICP_LOSS_HUBER 1
 #define REGTR_ICP_LOSS_CAUCHY 2
@@ -599,6 +611,10 @@ typedef struct {
     int loss;                                /* REGTR_ICP_LOSS_* [L2] */
     double loss_k;                           /* the loss's parameter k, > 0 (ignored by L2) */
     double epsilon;                          /* generalized ICP's covariance epsilon, 0 < epsilon <= 1 [1e-3] */
+    const double* src_colors;                /* colored ICP's device inputs (see above) [NULL: not colored] */
+    const double* tgt_colors;
+    const double* tgt_color_gradients;
+    double lambda_geometric;                 /* colored ICP's weight of the geometric residual, 0 <= l <= 1 */
 } regtr_icp_options;
 
 size_t regtr_icp_ws_bytes(int n_cap, int B);
@@ -630,6 +646,27 @@ size_t regtr_estimate_normals_state_bytes(int n_cap);
 int regtr_estimate_normals(const double* xyz, const int32_t* offs, int C, int n_cap, double radius, float cell,
                            int max_nn, double* normals, int32_t* counts, uint32_t* status, void* ws, size_t ws_bytes,
                            void* state, size_t state_bytes, void* stream);
+
+/* Intensity gradients of C stacked coloured clouds for colored ICP (Open3D's InitializePointCloudForColoredICP with
+ * KDTreeSearchParamHybrid(radius, max_nn), with this library's tie and order rules).  xyz / normals / colors
+ * (n_cap,3) float64 with offs (C+1) i32, offs[0] = 0, C <= 32767 (normals from regtr_estimate_normals, a zero normal
+ * allowed; colors rgb); cell = radius * (1 + 1e-3) rounded to fp32 (ops.overlap_cell); 1 <= max_nn <= 64 (else
+ * REGTR_ERR_ARG).  grad (n_cap,3) float64, rows >= offs[C] untouched.
+ *   Neighbours of point p: regtr_estimate_normals' rule (own cloud, d^2 strictly below radius^2, p included, the
+ *   max_nn smallest by (d^2, index)), nn of them.  Intensity it = ((r + g) + b) / 3.
+ *   Gradient 0 when nn < 4 or the normal n of p is zero.  Otherwise rows of A and b: for every entry i >= 1 in
+ *   ascending (d^2, index) order, with q_i - ((q_i - p) . n) n = v_i, the row v_i - p and b = it_i - it_p; then the row
+ *   (nn - 1) n with b = 0.  (A^T A) x = A^T b, both summed row by row in that order in float64, solved by LDL^T; the
+ *   gradient is x, or 0 when |det A^T A| < 1e-6 or det is not finite (Open3D's SolveLinearSystemPSD, as regtr_icp).
+ * A |coordinate| beyond regtr_overlap_coord_bound(radius, cell), or not finite, raises REGTR_STATUS_RANGE.
+ * 1 + 4 + 1 launches whatever C; no value atomics, no host synchronisation: the result is bit-identical whether a cloud
+ * is passed alone or in a stack.  ws / state: the *_bytes functions below (state ZERO before the first call; every
+ * call leaves it zero). */
+size_t regtr_color_gradients_ws_bytes(int n_cap);
+size_t regtr_color_gradients_state_bytes(int n_cap);
+int regtr_color_gradients(const double* xyz, const double* normals, const double* colors, const int32_t* offs, int C,
+                          int n_cap, double radius, float cell, int max_nn, double* grad, uint32_t* status, void* ws,
+                          size_t ws_bytes, void* state, size_t state_bytes, void* stream);
 
 /* FPFH features of C stacked clouds (Open3D's ComputeFPFHFeature(KDTreeSearchParamHybrid(radius, max_nn)), with this
  * library's tie and order rules).  xyz / normals (n_cap,3) float64 with offs (C+1) i32, offs[0] = 0, C <= 32767 (the

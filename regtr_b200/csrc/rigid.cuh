@@ -25,25 +25,26 @@ __device__ __forceinline__ void rigid_from_vec6(const double x[6], double R[3][3
     for (int r = 0; r < 3; ++r) t[r] = x[3 + r];
 }
 
-// Solve A x = -v for the symmetric 6x6 A given by its upper triangle H (row-major) by LDL^T without pivoting, in a
+// Solve A x = -v for the symmetric NxN A given by its upper triangle H (row-major) by LDL^T without pivoting, in a
 // fixed order.  False, x untouched, when |det A| = |prod D| < 1e-6 or det is not finite (Open3D's
 // SolveLinearSystemPSD check).
-__device__ __forceinline__ bool solve6_ldlt(const double H[21], const double v[6], double x[6]) {
-    double A[6][6], L[6][6], D[6];
+template <int N>
+__device__ __forceinline__ bool solve_ldlt(const double* H, const double* v, double* x) {
+    double A[N][N], L[N][N], D[N];
 #pragma unroll
-    for (int a = 0, e = 0; a < 6; ++a)
+    for (int a = 0, e = 0; a < N; ++a)
 #pragma unroll
-        for (int c = a; c < 6; ++c, ++e) { A[a][c] = H[e]; A[c][a] = H[e]; }
+        for (int c = a; c < N; ++c, ++e) { A[a][c] = H[e]; A[c][a] = H[e]; }
     double det = 1.0;
 #pragma unroll
-    for (int j = 0; j < 6; ++j) {
+    for (int j = 0; j < N; ++j) {
         double d = A[j][j];
 #pragma unroll
         for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k] * D[k];
         D[j] = d;
         det *= d;
 #pragma unroll
-        for (int i = j + 1; i < 6; ++i) {
+        for (int i = j + 1; i < N; ++i) {
             double a = A[i][j];
 #pragma unroll
             for (int k = 0; k < j; ++k) a -= L[i][k] * L[j][k] * D[k];
@@ -51,22 +52,26 @@ __device__ __forceinline__ bool solve6_ldlt(const double H[21], const double v[6
         }
     }
     if (!(fabs(det) >= 1e-6) || isinf(det)) return false;
-    double y[6];
+    double y[N];
 #pragma unroll
-    for (int i = 0; i < 6; ++i) {                      // L y = -v
+    for (int i = 0; i < N; ++i) {                      // L y = -v
         double a = -v[i];
 #pragma unroll
         for (int k = 0; k < i; ++k) a -= L[i][k] * y[k];
         y[i] = a;
     }
 #pragma unroll
-    for (int i = 5; i >= 0; --i) {                     // L^T x = D^-1 y
+    for (int i = N - 1; i >= 0; --i) {                 // L^T x = D^-1 y
         double a = y[i] / D[i];
 #pragma unroll
-        for (int k = i + 1; k < 6; ++k) a -= L[k][i] * x[k];
+        for (int k = i + 1; k < N; ++k) a -= L[k][i] * x[k];
         x[i] = a;
     }
     return true;
+}
+
+__device__ __forceinline__ bool solve6_ldlt(const double H[21], const double v[6], double x[6]) {
+    return solve_ldlt<6>(H, v, x);
 }
 
 // The sweeps of svd3_jacobi: one-sided (Hestenes) Jacobi rotations of A's column pairs, accumulated in V, until the

@@ -378,7 +378,8 @@ def summarize_modelnet_metrics(metrics: Dict[str, np.ndarray]) -> Dict[str, floa
 
 def icp_refine(src_list, tgt_list, init, radius: float, max_iteration: int = 30, method: str = 'point_to_point',
                normal_radius: float = None, normal_max_nn: int = 30, epsilon: float = 1e-3, loss: str = 'l2',
-               loss_k: float = None, normals=None, icp=None, estimate_normals=None):
+               loss_k: float = None, normals=None, icp=None, estimate_normals=None, colors=None,
+               lambda_geometric: float = 0.968, color_gradients=None):
     """Refine B poses init (B,3,4) by ICP of src_list onto tgt_list: the normals each method needs, then one icp call.
     -> icp's (pose (B,3,4), result).
     icp(src_list, tgt_list, init, radius, max_iteration, ...) defaults to `ops.icp`; point-to-point passes nothing
@@ -386,9 +387,15 @@ def icp_refine(src_list, tgt_list, init, radius: float, max_iteration: int = 30,
     2 * radius), normal_max_nn) (default `ops.estimate_normals`), and icp gets method=method, tgt_normals=.
     method='generalized': the normals of src_list + tgt_list come from one estimate_normals call, and icp also gets
     src_normals=.  normals=(src_normals, tgt_normals) skips the estimation (only the ones the method needs are
-    passed on).  epsilon, loss and loss_k (see `ops.icp`) are passed on only when they differ from their defaults."""
+    passed on).  epsilon, loss and loss_k (see `ops.icp`) are passed on only when they differ from their defaults.
+    method='colored' (Open3D's registration_colored_icp): colors=(src_colors, tgt_colors), B (n,3) rgb arrays each;
+    the targets' normals are estimated as for point_to_plane, then their intensity gradients by
+    color_gradients(tgt_list, normals, tgt_colors, 2 * radius, 30) (default `ops.color_gradients`; Open3D's own
+    parameters), and icp also gets src_colors=, tgt_colors=, tgt_color_gradients= and lambda_geometric=."""
     if icp is None:
         from .ops import icp
+    if method == 'colored' and colors is None:
+        raise ValueError('icp_refine: colored ICP needs colors=(src_colors, tgt_colors)')
     kw = {}
     if method != 'point_to_point':
         if normals is None:
@@ -404,6 +411,12 @@ def icp_refine(src_list, tgt_list, init, radius: float, max_iteration: int = 30,
         kw.update(method=method, tgt_normals=normals[1])
         if method == 'generalized':
             kw['src_normals'] = normals[0]
+    if method == 'colored':
+        if color_gradients is None:
+            from .ops import color_gradients
+        grads = color_gradients(tgt_list, normals[1], colors[1], 2.0 * radius, 30)
+        kw.update(src_colors=colors[0], tgt_colors=colors[1], tgt_color_gradients=grads,
+                  lambda_geometric=lambda_geometric)
     if epsilon != 1e-3:
         kw['epsilon'] = epsilon
     if loss != 'l2':
@@ -415,13 +428,15 @@ def icp_refine(src_list, tgt_list, init, radius: float, max_iteration: int = 30,
 
 def add_icp_arguments(ap, icp_help: str):
     """The ICP refinement flags of a command line, for `icp_refine`: --icp R (help text icp_help), --icp_iters,
-    --icp_method, --normal_radius, --normal_max_nn, --icp_epsilon, --icp_loss and --icp_loss_k."""
+    --icp_method, --normal_radius, --normal_max_nn, --icp_epsilon, --icp_loss, --icp_loss_k and
+    --icp_lambda_geometric."""
     from .ops import ICP_LOSSES, ICP_METHODS
     ap.add_argument('--icp', type=float, metavar='R', help=icp_help)
     ap.add_argument('--icp_iters', type=int, default=30, help='ICP iterations at most (with --icp)')
     ap.add_argument('--icp_method', choices=ICP_METHODS, default='point_to_point',
                     help='ICP error metric (with --icp); point_to_plane estimates the target normals first, '
-                         'generalized those of both clouds')
+                         'generalized those of both clouds, colored the target normals and colour gradients '
+                         '(needs .ply inputs with red, green and blue)')
     ap.add_argument('--normal_radius', type=float, metavar='NR',
                     help='Normal estimation radius of point_to_plane / generalized ICP (default: 2 * the --icp radius)')
     ap.add_argument('--normal_max_nn', type=int, default=30,
@@ -431,31 +446,61 @@ def add_icp_arguments(ap, icp_help: str):
     ap.add_argument('--icp_loss', choices=ICP_LOSSES, default='l2',
                     help='Robust kernel of point_to_plane / generalized ICP (needs --icp_loss_k unless l2)')
     ap.add_argument('--icp_loss_k', type=float, metavar='K', help='The robust kernel\'s parameter k')
+    ap.add_argument('--icp_lambda_geometric', type=float, default=0.968, metavar='L',
+                    help='Weight of the geometric residual of colored ICP, in [0, 1]')
 
 
-def check_icp_arguments(ap, opt):
-    """Reject, as a usage error, a robust --icp_loss without its --icp_loss_k, before any model is loaded."""
+def check_icp_arguments(ap, opt, colors: bool = False):
+    """Reject, as usage errors and before any model is loaded, a robust --icp_loss without its --icp_loss_k, an
+    --icp_lambda_geometric outside [0, 1], and --icp_method colored on a command line whose inputs carry no colour
+    (colors=False)."""
     if opt.icp_loss != 'l2' and opt.icp_loss_k is None:
         ap.error(f'--icp_loss {opt.icp_loss} needs --icp_loss_k')
+    if not 0.0 <= opt.icp_lambda_geometric <= 1.0:
+        ap.error(f'--icp_lambda_geometric {opt.icp_lambda_geometric} must be in [0, 1]')
+    if opt.icp_method == 'colored' and not colors:
+        ap.error('--icp_method colored needs coloured clouds, and this command line reads none')
+
+
+def load_icp_colors(ap, opt, paths):
+    """With --icp and --icp_method colored: the rgb (N,3) of every file of `paths` (`pointio.load_point_cloud_colors`),
+    a file without colours being a usage error that names it; else None."""
+    if opt.icp is None or opt.icp_method != 'colored':
+        return None
+    from .pointio import load_point_cloud_colors
+    out = []
+    for path in paths:
+        try:
+            out.append(load_point_cloud_colors(path)[1])
+        except ValueError as e:
+            ap.error(f'--icp_method colored: {e}')
+    return out
 
 
 def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None, method: str = 'point_to_point',
                 normal_radius: float = None, normal_max_nn: int = 30, estimate_normals=None, epsilon: float = 1e-3,
-                loss: str = 'l2', loss_k: float = None):
+                loss: str = 'l2', loss_k: float = None, lambda_geometric: float = 0.968, color_gradients=None):
     """Wrap `forward_fn(batch) -> pred` so that the final pose of every pair is refined by ICP on the batch's full
     clouds: -> a NEW dict with pred's entries, pose (1,B,3,4) float64 the refined poses and pose_coarse
     (1,B,3,4) float64 the network's final poses (so that `compute_metrics` reports both, and EstLogWriter writes the
     refined ones).  pred's own tensors are not written to (a graphed forward owns them).
-    The refinement is `icp_refine` with these arguments, icp and estimate_normals included."""
+    The refinement is `icp_refine` with these arguments, icp, estimate_normals and color_gradients included; with
+    method='colored' the colours are the batch's src_colors / tgt_colors (a batch without them raises ValueError)."""
     from .ops import ICP_METHODS
     if method not in ICP_METHODS:
         raise ValueError(f'icp_forward: unknown method {method!r}')
     def run(batch):
         pred = forward_fn(batch)
         coarse = pred['pose'][-1].to(torch.float64)                     # (B,3,4), a new tensor
+        kw = {}
+        if method == 'colored':
+            if 'src_colors' not in batch or 'tgt_colors' not in batch:
+                raise ValueError('icp_forward: colored ICP needs the batch\'s src_colors and tgt_colors')
+            kw = dict(colors=(batch['src_colors'], batch['tgt_colors']), lambda_geometric=lambda_geometric,
+                      color_gradients=color_gradients)
         pose, _ = icp_refine(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, method,
                              normal_radius, normal_max_nn, epsilon, loss, loss_k, icp=icp,
-                             estimate_normals=estimate_normals)
+                             estimate_normals=estimate_normals, **kw)
         out = dict(pred)
         out['pose'] = torch.as_tensor(pose, dtype=torch.float64, device=coarse.device).reshape(coarse.shape)[None]
         out['pose_coarse'] = coarse[None]
@@ -789,8 +834,11 @@ def fpfh_kwargs(opt) -> Dict:
 
 def icp_kwargs(opt) -> Dict:
     """`icp_refine`'s keyword arguments from the parsed --icp_* / --normal_* flags (without the radius)."""
-    return dict(max_iteration=opt.icp_iters, method=opt.icp_method, normal_radius=opt.normal_radius,
-                normal_max_nn=opt.normal_max_nn, epsilon=opt.icp_epsilon, loss=opt.icp_loss, loss_k=opt.icp_loss_k)
+    kw = dict(max_iteration=opt.icp_iters, method=opt.icp_method, normal_radius=opt.normal_radius,
+              normal_max_nn=opt.normal_max_nn, epsilon=opt.icp_epsilon, loss=opt.icp_loss, loss_k=opt.icp_loss_k)
+    if opt.icp_method == 'colored':
+        kw['lambda_geometric'] = opt.icp_lambda_geometric
+    return kw
 
 
 def run_3dmatch_benchmark(batches: Iterable[Dict], forward_fn, log_path: str, benchmark: str, gt_folder: str,

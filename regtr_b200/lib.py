@@ -111,6 +111,9 @@ SIGNATURES = {
     'regtr_estimate_normals_ws_bytes': (_Z, [_I]),
     'regtr_estimate_normals_state_bytes': (_Z, [_I]),
     'regtr_estimate_normals': (_I, [_P, _P, _I, _I, _c.c_double, _F, _I, _P, _P, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_color_gradients_ws_bytes': (_Z, [_I]),
+    'regtr_color_gradients_state_bytes': (_Z, [_I]),
+    'regtr_color_gradients': (_I, [_P, _P, _P, _P, _I, _I, _c.c_double, _F, _I, _P, _P, _P, _Z, _P, _Z, _P]),
     'regtr_fpfh_ws_bytes': (_Z, [_I, _I]),
     'regtr_fpfh_state_bytes': (_Z, [_I]),
     'regtr_fpfh': (_I, [_P, _P, _P, _I, _I, _c.c_double, _F, _I, _P, _P, _P, _P, _Z, _P, _Z, _P]),

@@ -2,8 +2,9 @@
 registration after RegTR's pairwise poses).
 
     python -m regtr_b200.multiway FRAG_0 FRAG_1 ... --ckpt <logdir>/ckpt/model-best.pth [--config <yaml>] --out DIR
-        [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized [--normal_radius NR]
-         [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
+        [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized|colored
+         [--normal_radius NR] [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_lambda_geometric 0.968]
+         [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
         [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
         [--fgr [--fgr_dist 0.025] [--fgr_iters 64] [--fgr_tuple_test] [--fgr_overlap 0.5] ...]
@@ -14,7 +15,8 @@ Fragments are given in sequence order, in any format `pointio` reads; fragment i
 scenes are numbered cloud_bin_0..N-1, so position is the benchmark index).  The config is found and the clouds are
 cropped as `register` does.  Every pair i < j is registered with source j and target i (the 3DMatch benchmark's
 direction) in eager forwards of --batch_pairs pairs, then refined by `ops.icp` with --icp as `register --icp` does
-(generalized ICP uses each fragment's normals as source and as target normals).  With --ransac R each pair's pose
+(generalized ICP uses each fragment's normals as source and as target normals; colored ICP reads every fragment's PLY
+colours, a fragment without them being a usage error, and takes its target's gradients at radius 2 R, 30 neighbours).  With --ransac R each pair's pose
 first comes from RANSAC over the network's correspondences (`ops.ransac`, as `register --ransac`), so that far loop
 closures with little overlap survive the network's outlier correspondences; ICP then starts from it.  --fgr does the
 same with Fast Global Registration over those correspondences (`ops.fgr`, as `register --fgr`) instead of RANSAC.
@@ -80,14 +82,16 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
                    icp_iters: int = 30, icp_method: str = 'point_to_point', normal_radius: float = None,
                    normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
                    icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None,
-                   fgr_options: Dict = None) -> np.ndarray:
+                   fgr_options: Dict = None, colors: Sequence[np.ndarray] = None,
+                   icp_lambda_geometric: float = 0.968) -> np.ndarray:
     """RegTR's final-layer pose of every pair (i, j) of `all_pairs`, source j -> target i, optionally refined by ICP
     (`eval.icp_refine` with icp_method, epsilon=icp_epsilon, loss=icp_loss, loss_k=icp_loss_k; the point-to-plane and
     generalized methods use every fragment's normals, estimated once).
     With ransac_radius, the network's pose is first replaced by `eval.ransac_refine` at that radius (ransac_options:
     its further keyword arguments), pair p of `all_pairs` drawing as pair p whatever batch_pairs; ICP then starts from
     the RANSAC pose.  fgr_options (a dict, possibly empty): the same with `eval.fgr_refine` and these keyword arguments
-    instead, pair p drawing its tuples as pair p.
+    instead, pair p drawing its tuples as pair p.  colors: every fragment's (n,3) rgb, for icp_method='colored' (with
+    icp_lambda_geometric).
     fragments: (n,3) float64 host arrays (already cropped).  -> (P,3,4) float64."""
     from . import ops
     dev = model.device
@@ -113,7 +117,10 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
                 pose, _ = icp_refine([fragments[j] for _, j in chunk], [fragments[i] for i, _ in chunk], pose,
                                      icp_radius, icp_iters, icp_method, epsilon=icp_epsilon, loss=icp_loss,
                                      loss_k=icp_loss_k, normals=None if normals is None else
-                                     ([normals[j] for _, j in chunk], [normals[i] for i, _ in chunk]))
+                                     ([normals[j] for _, j in chunk], [normals[i] for i, _ in chunk]),
+                                     colors=None if colors is None else
+                                     ([colors[j] for _, j in chunk], [colors[i] for i, _ in chunk]),
+                                     lambda_geometric=icp_lambda_geometric)
             out.append(pose.cpu().numpy())
     return np.concatenate(out, 0)
 
@@ -213,23 +220,29 @@ def main(argv=None):
     ap = parser()
     opt = ap.parse_args(argv)
     check_fgr_arguments(ap, opt)
-    check_icp_arguments(ap, opt)
+    check_icp_arguments(ap, opt, colors=True)
     check_ransac_arguments(ap, opt)
     from .config import load_config
+    from .eval import load_icp_colors
     from .pointio import load_point_cloud
-    from .register import config_path, crop, load_model
+    from .register import config_path, crop, crop_colors, load_model
     if len(opt.fragments) < 2:
         raise SystemExit('expected at least two fragments')
+    colors = load_icp_colors(ap, opt, opt.fragments)
     cfg_file = config_path(opt.ckpt, opt.config)
     if not cfg_file.exists():
         raise SystemExit(f'config not found: {cfg_file} (pass --config)')
     cfg = load_config(str(cfg_file))
     model = load_model(cfg, opt.ckpt)
-    frags = [crop(cfg, np.asarray(load_point_cloud(f), dtype=np.float64)) for f in opt.fragments]
+    raw = [np.asarray(load_point_cloud(f), dtype=np.float64) for f in opt.fragments]
+    frags = [crop(cfg, x) for x in raw]
+    if colors is not None:
+        colors = [crop_colors(cfg, x, c) for x, c in zip(raw, colors)]
     T = register_pairs(model, frags, opt.batch_pairs, opt.icp, opt.icp_iters, opt.icp_method, opt.normal_radius,
                        opt.normal_max_nn, opt.icp_epsilon, opt.icp_loss, opt.icp_loss_k, opt.ransac,
                        ransac_kwargs(opt) if opt.ransac is not None else None,
-                       dict(fgr_kwargs(opt), overlap=opt.fgr_overlap) if opt.fgr else None)
+                       dict(fgr_kwargs(opt), overlap=opt.fgr_overlap) if opt.fgr else None, colors,
+                       opt.icp_lambda_geometric)
     D = float(cfg['overlap_radius'] if opt.info_radius is None else opt.info_radius)
     res = optimize_scene(frags, T, D, opt.min_overlap, opt.preference_loop_closure)
     write_outputs(res, opt.out, scene_name(opt.fragments[0]), frags, opt.voxel)

@@ -1254,25 +1254,28 @@ def icp_launches(max_iteration: int) -> int:
     return 5 + 3 * (int(max_iteration) + 1)
 
 
-ICP_METHODS = ('point_to_point', 'point_to_plane', 'generalized')
+ICP_METHODS = ('point_to_point', 'point_to_plane', 'generalized', 'colored')
 ICP_LOSSES = ('l2', 'huber', 'cauchy', 'gm', 'tukey')      # REGTR_ICP_LOSS_L2 .. REGTR_ICP_LOSS_TUKEY
 
 
 class IcpOptions(ctypes.Structure):
     """regtr_icp_options (include/regtr_b200.h)."""
-    _fields_ = [('loss', ctypes.c_int), ('loss_k', ctypes.c_double), ('epsilon', ctypes.c_double)]
+    _fields_ = [('loss', ctypes.c_int), ('loss_k', ctypes.c_double), ('epsilon', ctypes.c_double),
+                ('src_colors', ctypes.c_void_p), ('tgt_colors', ctypes.c_void_p),
+                ('tgt_color_gradients', ctypes.c_void_p), ('lambda_geometric', ctypes.c_double)]
 
 
-def _stack_normals(normals, lens, what, dev):
-    """B (n,3) normal arrays aligned with clouds of `lens` points -> one (max(sum, 1), 3) float64 device tensor."""
-    if len(normals) != len(lens):
-        raise ValueError(f'icp: {len(normals)} {what} normal arrays for {len(lens)} pairs')
+def _stack_normals(normals, lens, what, dev, kind='normals'):
+    """B (n,3) normal (or `kind`) arrays aligned with clouds of `lens` points -> one (max(sum, 1), 3) float64 device
+    tensor."""
+    if normals is None or len(normals) != len(lens):
+        raise ValueError(f'icp: {0 if normals is None else len(normals)} {what} {kind} arrays for {len(lens)} pairs')
     out = torch.empty((max(sum(lens), 1), 3), dtype=torch.float64, device=dev)
     a = 0
     for c, ln in zip(normals, lens):
         c = torch.as_tensor(c)
         if tuple(c.shape) != (ln, 3):
-            raise ValueError(f'icp: {what} normals {tuple(c.shape)} for a {what} of {ln} points')
+            raise ValueError(f'icp: {what} {kind} {tuple(c.shape)} for a {what} of {ln} points')
         out[a:a + ln].copy_(c.to(dev, torch.float64))
         a += ln
     return out
@@ -1280,18 +1283,22 @@ def _stack_normals(normals, lens, what, dev):
 
 def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iteration: int = 30,
         relative_fitness: float = 1e-6, relative_rmse: float = 1e-6, status=None, method: str = 'point_to_point',
-        tgt_normals=None, src_normals=None, epsilon: float = 1e-3, loss: str = 'l2', loss_k: float = None):
+        tgt_normals=None, src_normals=None, epsilon: float = 1e-3, loss: str = 'l2', loss_k: float = None,
+        src_colors=None, tgt_colors=None, tgt_color_gradients=None, lambda_geometric: float = 0.968):
     """ICP of B pairs (regtr_icp): Open3D's registration_icp with TransformationEstimationPointToPoint (no scaling) or,
     with method='point_to_plane', TransformationEstimationPointToPlane, or with method='generalized',
-    registration_generalized_icp with TransformationEstimationForGeneralizedICP(epsilon), and
+    registration_generalized_icp with TransformationEstimationForGeneralizedICP(epsilon), or with method='colored',
+    registration_colored_icp with TransformationEstimationForColoredICP(lambda_geometric), and
     ICPConvergenceCriteria(relative_fitness, relative_rmse, max_iteration), on the device.
     src_list / tgt_list: B clouds (n,3) each (numpy or torch, any float dtype; stacked in float64 on the device);
     init (B,3,4) source -> target.  tgt_normals: with 'point_to_plane' and 'generalized', B (n,3) normals aligned with
     tgt_list (e.g. `estimate_normals(tgt_list, ...)`); a zero normal drops its correspondence out of the point-to-plane
     update.  src_normals: with 'generalized', B (n,3) normals aligned with src_list (a zero normal gives the identity
-    covariance); epsilon in (0, 1] the covariances' epsilon.  loss: one of ICP_LOSSES, Open3D's robust kernel of the
-    point-to-plane and generalized estimations, with loss_k its parameter k > 0 ('l2', the default, takes none; the
-    point-to-point estimation has no kernel).
+    covariance); epsilon in (0, 1] the covariances' epsilon.  'colored' takes tgt_normals, B (n,3) rgb arrays
+    src_colors / tgt_colors aligned with the clouds, the targets' tgt_color_gradients (`color_gradients`) and
+    lambda_geometric in [0, 1], the weight of the geometric residual.  loss: one of ICP_LOSSES, Open3D's robust kernel
+    of the point-to-plane, generalized and colored estimations, with loss_k its parameter k > 0 ('l2', the default,
+    takes none; the point-to-point estimation has no kernel).
     -> (pose (B,3,4) float64, result (B,4) float64 = fitness, inlier_rmse, n_corr, iterations), both device tensors.
     No host sync unless status is None: then a word of this call is read and a coordinate of a moved source or of a
     target beyond `overlap_coord_bound(max_correspondence_distance)` raises RegtrLibError; with the caller's word,
@@ -1316,6 +1323,14 @@ def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iterat
         raise ValueError(f'icp: {method} needs the target normals (tgt_normals), e.g. from estimate_normals')
     if gicp and src_normals is None:
         raise ValueError('icp: generalized needs the source normals (src_normals), e.g. from estimate_normals')
+    colored = method == 'colored'
+    if colored:
+        if not 0.0 <= float(lambda_geometric) <= 1.0:
+            raise ValueError(f'icp: lambda_geometric {lambda_geometric!r} must be in [0, 1]')
+        for name, v in (('src_colors', src_colors), ('tgt_colors', tgt_colors),
+                        ('tgt_color_gradients', tgt_color_gradients)):
+            if v is None:
+                raise ValueError(f'icp: colored needs {name}')
     B = len(src_list)
     dev = init.device if torch.is_tensor(init) and init.is_cuda else None
     xyz, offs, lens = _stack_pairs(src_list, tgt_list, 'icp', dev)
@@ -1323,8 +1338,14 @@ def icp(src_list, tgt_list, init, max_correspondence_distance: float, max_iterat
     nrm = None if method == 'point_to_point' else _stack_normals(tgt_normals, lens[B:], 'target', dev)
     snrm = _stack_normals(src_normals, lens[:B], 'source', dev) if gicp else None
     opt = None
-    if gicp or loss != 'l2':
+    if gicp or colored or loss != 'l2':
         opt = IcpOptions(ICP_LOSSES.index(loss), float(loss_k) if loss != 'l2' else 1.0, float(epsilon))
+    if colored:
+        scol = _stack_normals(src_colors, lens[:B], 'source', dev, 'colors')
+        tcol = _stack_normals(tgt_colors, lens[B:], 'target', dev, 'colors')
+        tgrd = _stack_normals(tgt_color_gradients, lens[B:], 'target', dev, 'color gradients')
+        opt.src_colors, opt.tgt_colors, opt.tgt_color_gradients = _p(scol), _p(tcol), _p(tgrd)
+        opt.lambda_geometric = float(lambda_geometric)
     init64 = torch.as_tensor(init).to(dev, torch.float64).reshape(B, 3, 4).contiguous()
     n = sum(lens)
     own = status is None
@@ -1553,6 +1574,51 @@ def estimate_normals(clouds, radius: float, max_nn: int = 30, status=None, retur
     if return_counts:
         return out, [counts[bounds[k]:bounds[k + 1]] for k in range(C)]
     return out
+
+
+def color_gradients(clouds, normals, colors, radius: float, max_nn: int = 30, status=None):
+    """Intensity gradients of C coloured clouds for colored ICP (regtr_color_gradients): Open3D's
+    InitializePointCloudForColoredICP(KDTreeSearchParamHybrid(radius, max_nn)) with the library's rules (the
+    neighbours of `estimate_normals`; a zero gradient with fewer than 4 neighbours, a zero normal or a failed solve).
+    clouds / normals / colors: C (n,3) arrays each, normals from `estimate_normals`, colors rgb; numpy or torch, any
+    float dtype, stacked in float64 on the device.  -> list of C (n,3) float64 device tensors.
+    No host sync unless status is None: then a word of this call is read and a coordinate beyond
+    `overlap_coord_bound(radius)`, or not finite, raises RegtrLibError; with the caller's word, `check_fit_status`
+    does that where the caller syncs."""
+    r = float(radius)
+    if not r > 0.0 or not 1 <= int(max_nn) <= NORMALS_MAX_NN:
+        raise ValueError(f'color_gradients: radius {r} must be > 0 and max_nn {max_nn} in 1..{NORMALS_MAX_NN}')
+    C = len(clouds)
+    if C == 0 or len(normals) != C or len(colors) != C:
+        raise ValueError(f'color_gradients: {C} clouds, {len(normals)} normal and {len(colors)} colour arrays; '
+                         f'expected as many, at least one')
+    ts = [torch.as_tensor(c) for c in clouds]
+    ns = [torch.as_tensor(c) for c in normals]
+    cs = [torch.as_tensor(c) for c in colors]
+    for c, m, k in zip(ts, ns, cs):
+        if c.dim() != 2 or c.shape[1] != 3 or tuple(m.shape) != tuple(c.shape) or tuple(k.shape) != tuple(c.shape):
+            raise ValueError(f'color_gradients: cloud {tuple(c.shape)}, normals {tuple(m.shape)} and colors '
+                             f'{tuple(k.shape)}, expected three (n,3) arrays')
+    L = _lib.load()
+    dev = next((c.device for c in ts + ns + cs if c.is_cuda), torch.device('cuda', torch.cuda.current_device()))
+    xyz, lens = _stack_clouds(ts, dev, 3, 'color_gradients')
+    nrm, _ = _stack_clouds(ns, dev, 3, 'color_gradients')
+    rgb, _ = _stack_clouds(cs, dev, 3, 'color_gradients')
+    n = sum(lens)
+    offs = make_offsets(lens, dev)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    grad = torch.empty((max(n, 1), 3), dtype=torch.float64, device=dev)
+    ws = workspace(L.regtr_color_gradients_ws_bytes(n), dev)
+    state = workspace(L.regtr_color_gradients_state_bytes(n), dev, 'scan_state', zero=True)
+    _lib.check(L.regtr_color_gradients(_p(xyz), _p(nrm), _p(rgb), _p(offs), C, n, r, overlap_cell(r), int(max_nn),
+                                       _p(grad), _p(status), _p(ws), ws.numel(), _p(state), state.numel(), _stream()),
+               'regtr_color_gradients')
+    _count(normals_launches())
+    if own:
+        check_fit_status(status, r, 'color_gradients')
+    return _split(grad, lens)
 
 
 FPFH_DIM = 33                       # REGTR_FPFH_DIM

@@ -7,6 +7,7 @@
 * `.bin`: KITTI velodyne scans, float32 x, y, z, reflectance.
 * `.npy`: a plain numpy array (no pickles).
 Every loader keeps the first three columns, as the reference does, and returns (N, 3) float64.
+`load_point_cloud_colors` also reads a PLY file's red / green / blue vertex properties, for colored ICP.
 """
 from __future__ import annotations
 
@@ -62,9 +63,10 @@ def _ply_header(fh, path):
     return fmt, elements
 
 
-def read_ply(path) -> np.ndarray:
-    """x, y, z of the `vertex` element -> (N, 3) float64.  Other scalar vertex properties are skipped; list
-    properties on the vertex element or on an element stored before it raise ValueError."""
+def _ply_vertex(path, wanted, optional=()):
+    """The `vertex` element's scalar properties `wanted` (all required) and those of `optional` that exist ->
+    ({name: (N,) float64}, {name: PLY numpy type code}).  List properties on the vertex element or on an element stored
+    before it raise ValueError."""
     with open(path, 'rb') as fh:
         fmt, elements = _ply_header(fh, path)
         names = [e[0] for e in elements]
@@ -78,10 +80,11 @@ def read_ply(path) -> np.ndarray:
                                  f'on or before the vertex element)')
         _, n, props = elements[vi]
         pnames = [p for p, _ in props]
-        missing = [a for a in 'xyz' if a not in pnames]
+        missing = [a for a in wanted if a not in pnames]
         if missing:
             raise ValueError(f'{path}: PLY vertex element lacks {missing}')
-        cols = [pnames.index(a) for a in 'xyz']
+        keys = list(wanted) + [a for a in optional if a in pnames]
+        types = {a: props[pnames.index(a)][1] for a in keys}
         order = _PLY_FORMATS[fmt]
         if order is None:                                       # ascii: one element per line
             lines = fh.read().decode('ascii', 'replace').splitlines()
@@ -93,8 +96,9 @@ def read_ply(path) -> np.ndarray:
             vals = [r.split() for r in rows]
             if any(len(v) != len(props) for v in vals):
                 raise ValueError(f'{path}: a PLY vertex line does not have {len(props)} values')
-            arr = np.array([[float(v[c]) for c in cols] for v in vals], dtype=np.float64).reshape(n, 3)
-            return arr
+            cols = [pnames.index(a) for a in keys]
+            arr = np.array([[float(v[c]) for c in cols] for v in vals], dtype=np.float64).reshape(n, len(keys))
+            return {a: arr[:, k] for k, a in enumerate(keys)}, types
         skip = sum(cnt * np.dtype([(p, order + t) for p, t in pr]).itemsize for _, cnt, pr in elements[:vi])
         dt = np.dtype([(p, order + t) for p, t in props])
         fh.seek(skip, os.SEEK_CUR)
@@ -102,7 +106,35 @@ def read_ply(path) -> np.ndarray:
         if len(buf) < n * dt.itemsize:
             raise ValueError(f'{path}: PLY data ends after {len(buf) // max(dt.itemsize, 1)} of {n} vertices')
         rec = np.frombuffer(buf, dtype=dt, count=n)
-        return np.stack([rec[a].astype(np.float64) for a in 'xyz'], axis=1).reshape(n, 3)
+        return {a: rec[a].astype(np.float64) for a in keys}, types
+
+
+def read_ply(path) -> np.ndarray:
+    """x, y, z of the `vertex` element -> (N, 3) float64.  Other scalar vertex properties are skipped; list
+    properties on the vertex element or on an element stored before it raise ValueError."""
+    cols, _ = _ply_vertex(path, 'xyz')
+    return np.stack([cols[a] for a in 'xyz'], axis=1).reshape(-1, 3)
+
+
+# Open3D's scaling of PLY colour channels to [0, 1]: uchar / 255, ushort / 65535, float and double as stored
+_PLY_COLOR_SCALE = {'u1': 255.0, 'u2': 65535.0, 'f4': 1.0, 'f8': 1.0}
+
+
+def read_ply_colors(path):
+    """x, y, z and red, green, blue of the `vertex` element -> (xyz (N,3) float64, rgb (N,3) float64), each channel
+    scaled as Open3D does (uchar / 255, ushort / 65535, float or double as stored).  A missing channel or one of
+    another type raises ValueError."""
+    cols, types = _ply_vertex(path, 'xyz', ('red', 'green', 'blue'))
+    rgb = []
+    for ch in ('red', 'green', 'blue'):
+        if ch not in cols:
+            raise ValueError(f'{path}: PLY vertex element has no {ch!r} colour property')
+        if types[ch] not in _PLY_COLOR_SCALE:
+            raise ValueError(f'{path}: PLY colour property {ch!r} has an unsupported type (expected uchar, ushort, '
+                             f'float or double)')
+        rgb.append(cols[ch] / _PLY_COLOR_SCALE[types[ch]])
+    xyz = np.stack([cols[a] for a in 'xyz'], axis=1).reshape(-1, 3)
+    return xyz, np.stack(rgb, axis=1).reshape(-1, 3)
 
 
 def _numpy_globals():
@@ -147,16 +179,36 @@ def load_point_cloud(path) -> np.ndarray:
     return np.ascontiguousarray(data[:, :3], dtype=np.float64)
 
 
-def write_ply(path, xyz, scalars: Optional[Dict[str, np.ndarray]] = None):
-    """Binary little-endian PLY with double x, y, z (the layout Open3D writes) and one float property per entry of
-    `scalars` (per-vertex arrays)."""
+def load_point_cloud_colors(path):
+    """A coloured point cloud -> (xyz (N,3) float64, rgb (N,3) float64 in [0, 1]): `.ply` files with red, green and
+    blue vertex properties (`read_ply_colors`).  `.pth`, `.bin` and `.npy` files carry no colour and raise ValueError,
+    as does a PLY file without all three channels."""
+    path = str(path)
+    ext = os.path.splitext(path)[1].lower()
+    if ext != '.ply':
+        raise ValueError(f'{path}: {ext or "this"} files carry no colour (colours are read from .ply files with red, '
+                         f'green and blue vertex properties)')
+    return read_ply_colors(path)
+
+
+def write_ply(path, xyz, scalars: Optional[Dict[str, np.ndarray]] = None, colors=None):
+    """Binary little-endian PLY with double x, y, z (the layout Open3D writes), with `colors` (N,3) in [0, 1] uchar
+    red, green, blue (round(255 c), clipped to [0, 1] first), and one float property per entry of `scalars` (per-vertex
+    arrays)."""
     xyz = np.asarray(xyz, dtype=np.float64).reshape(-1, 3)
     n = xyz.shape[0]
     scalars = dict(scalars or {})
-    fields = [('x', '<f8'), ('y', '<f8'), ('z', '<f8')] + [(k, '<f4') for k in scalars]
+    rgb = ('red', 'green', 'blue') if colors is not None else ()
+    fields = [('x', '<f8'), ('y', '<f8'), ('z', '<f8')] + [(k, 'u1') for k in rgb] + [(k, '<f4') for k in scalars]
     rec = np.empty(n, dtype=np.dtype(fields))
     for a, k in enumerate('xyz'):
         rec[k] = xyz[:, a]
+    if colors is not None:
+        c = np.asarray(colors, dtype=np.float64)
+        if c.shape != (n, 3):
+            raise ValueError(f'write_ply: colors {c.shape} for {n} points')
+        for a, k in enumerate(rgb):
+            rec[k] = np.round(np.clip(c[:, a], 0.0, 1.0) * 255.0).astype(np.uint8)
     for k, v in scalars.items():
         v = np.asarray(v).reshape(-1)
         if v.shape[0] != n:
@@ -164,7 +216,7 @@ def write_ply(path, xyz, scalars: Optional[Dict[str, np.ndarray]] = None):
         rec[k] = v
     head = ['ply', 'format binary_little_endian 1.0', 'comment Created by regtr_b200', f'element vertex {n}',
             'property double x', 'property double y', 'property double z']
-    head += [f'property float {k}' for k in scalars] + ['end_header']
+    head += [f'property uchar {k}' for k in rgb] + [f'property float {k}' for k in scalars] + ['end_header']
     with open(path, 'wb') as fh:
         fh.write(('\n'.join(head) + '\n').encode('ascii'))
         fh.write(rec.tobytes())

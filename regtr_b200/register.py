@@ -2,8 +2,9 @@
 
     python -m regtr_b200.register SRC TGT --ckpt <logdir>/ckpt/model-best.pth [--config <yaml>] \\
         [--threshold 0.5] [--fit_radius R] [--out DIR]
-        [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized [--normal_radius NR]
-         [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
+        [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized|colored
+         [--normal_radius NR] [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_lambda_geometric 0.968]
+         [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
         [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
         [--fgr [--fgr_dist 0.025] [--fgr_iters 64] [--fgr_division 1.4] [--fgr_tuple_test [--fgr_tuple_scale 0.95]
@@ -26,8 +27,11 @@ Open3D's registration_icp with max_correspondence_distance R and --icp_iters ite
 default; --icp_method point_to_plane first estimates the cropped target's normals (`ops.estimate_normals`, Open3D's
 estimate_normals with KDTreeSearchParamHybrid(--normal_radius, default 2 R, --normal_max_nn)); --icp_method
 generalized estimates the normals of both cropped clouds in one call and runs Open3D's registration_generalized_icp
-(covariance epsilon --icp_epsilon); --icp_loss with --icp_loss_k weights the point-to-plane or generalized residuals by
-Open3D's robust kernel of that name;
+(covariance epsilon --icp_epsilon); --icp_method colored reads both files' colours (PLY red / green / blue, a file
+without them is a usage error), estimates the cropped target's normals as point_to_plane does and its intensity
+gradients (`ops.color_gradients`, radius 2 R, 30 neighbours at most, Open3D's parameters), and runs Open3D's
+registration_colored_icp (geometric weight --icp_lambda_geometric); --icp_loss with --icp_loss_k weights the
+point-to-plane, generalized or colored residuals by Open3D's robust kernel of that name;
 pose.txt, src_registered.ply and fit then use the refined pose, result.npz gains pose_coarse (the network's final
 pose), pose_icp (the refined one) and icp (4,) = fitness, inlier_rmse, correspondences, iterations.
 With --ransac R the final decoder layer's pose is replaced by RANSAC over the network's two-way correspondences with
@@ -44,7 +48,8 @@ with FastGlobalRegistrationOption: --fgr_dist the maximum correspondence distanc
 starts from the FGR pose.  result.npz then gains pose_coarse, pose_fgr (3,4) float64 and fgr (4,) = correspondences of
 the solve, tuples kept, trials walked, final GNC parameter.
 One JSON line on stdout: the pose, the four fit numbers and the point counts (with --icp, also icp_fitness, icp_rmse,
-icp_iterations, icp_radius and icp_method, and icp_loss, icp_loss_k and icp_epsilon when they are given; with --ransac,
+icp_iterations, icp_radius and icp_method, and icp_loss, icp_loss_k, icp_epsilon and icp_lambda_geometric when they
+are given; with --ransac,
 ransac_fitness, ransac_rmse, ransac_iterations, ransac_validations and ransac_radius; with --fgr, fgr_correspondences,
 fgr_tuples, fgr_trials, fgr_par and fgr_dist).
 With --fpfh V there is no network and no --ckpt: Open3D's classical global registration (`eval.fpfh_register`) on the
@@ -106,7 +111,7 @@ def parse_args(argv=None):
     opt = ap.parse_args(argv)
     check_fgr_arguments(ap, opt)
     check_fpfh_arguments(ap, opt)
-    check_icp_arguments(ap, opt)
+    check_icp_arguments(ap, opt, colors=True)
     check_ransac_arguments(ap, opt)
     if opt.fpfh is not None and opt.fit_radius is None:
         opt.fit_radius = 1.5 * opt.fpfh if opt.fgr else opt.ransac
@@ -125,6 +130,13 @@ def crop(cfg, xyz: np.ndarray) -> np.ndarray:
     return xyz
 
 
+def crop_colors(cfg, xyz: np.ndarray, rgb: np.ndarray) -> np.ndarray:
+    """The rows of rgb (N,3) that `crop(cfg, xyz)` keeps of xyz (N,3) float64."""
+    if 'crop_radius' in cfg:
+        return rgb[np.linalg.norm(xyz, axis=1) < cfg['crop_radius'], :]
+    return rgb
+
+
 def load_model(cfg, ckpt: str, device=None):
     """RegTR(cfg) on the device in eval mode with the checkpoint's state_dict loaded strictly (as the demo does)."""
     from .regtr import RegTR
@@ -139,8 +151,9 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
              icp_radius: float = None, icp_iters: int = 30, icp_method: str = 'point_to_point',
              normal_radius: float = None, normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
              icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None,
-             fgr_options: Dict = None) -> Dict:
-    """Crop, forward and fit one pair.  src_xyz / tgt_xyz (N,3) float64 host arrays.
+             fgr_options: Dict = None, colors=None, icp_lambda_geometric: float = 0.968) -> Dict:
+    """Crop, forward and fit one pair.  src_xyz / tgt_xyz (N,3) float64 host arrays; colors (src_rgb, tgt_rgb) (N,3)
+    host arrays aligned with them, cropped alike, for icp_method='colored' (with icp_lambda_geometric).
     -> dict of host arrays: src_xyz / tgt_xyz (cropped, float64), pose (L,3,4) fp32, src_kp, src_kp_warped (final
     layer), src_overlap (sigmoid of the final layer's logit, (n,)), the same for tgt, fit (4,) float64.
     icp_radius: refine the final layer's pose by ICP on the cropped clouds (`eval.icp_refine` with icp_method, at most
@@ -153,8 +166,10 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
     fgr_options: likewise, but `eval.fgr_refine` with these keyword arguments (overlap and `ops.fgr`'s options); the
     dict gains pose_coarse, pose_fgr (3,4) float64 and fgr (4,) float64 = correspondences, tuples, trials, par."""
     from . import ops
-    src_xyz = crop(cfg, np.asarray(src_xyz, dtype=np.float64))
-    tgt_xyz = crop(cfg, np.asarray(tgt_xyz, dtype=np.float64))
+    src_xyz, tgt_xyz = np.asarray(src_xyz, dtype=np.float64), np.asarray(tgt_xyz, dtype=np.float64)
+    if colors is not None:
+        colors = [crop_colors(cfg, src_xyz, colors[0])], [crop_colors(cfg, tgt_xyz, colors[1])]
+    src_xyz, tgt_xyz = crop(cfg, src_xyz), crop(cfg, tgt_xyz)
     dev = model.device
     batch = {'src_xyz': [torch.from_numpy(src_xyz).float().to(dev)],
              'tgt_xyz': [torch.from_numpy(tgt_xyz).float().to(dev)]}
@@ -172,7 +187,8 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
             pose_fgr = final
         if icp_radius is not None:
             final, icp = icp_refine([src_xyz], [tgt_xyz], final, icp_radius, icp_iters, icp_method, normal_radius,
-                                    normal_max_nn, icp_epsilon, icp_loss, icp_loss_k)
+                                    normal_max_nn, icp_epsilon, icp_loss, icp_loss_k, colors=colors,
+                                    lambda_geometric=icp_lambda_geometric)
         fit = ops.registration_fit([src_xyz], [tgt_xyz], final, radius, status)
         res = {'src_xyz': src_xyz, 'tgt_xyz': tgt_xyz, 'pose': pose.cpu().numpy()}
         if icp_radius is not None:
@@ -264,9 +280,11 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
 
 def main(argv=None):
     opt = parse_args(argv)
+    from .eval import load_icp_colors
     from .pointio import load_point_cloud
+    colors = load_icp_colors(parser(), opt, [opt.src, opt.tgt])
     if opt.fpfh is not None:
-        return main_fpfh(opt, load_point_cloud(opt.src), load_point_cloud(opt.tgt))
+        return main_fpfh(opt, load_point_cloud(opt.src), load_point_cloud(opt.tgt), colors)
     from .config import load_config
     cfg_file = config_path(opt.ckpt, opt.config)
     if not cfg_file.exists():
@@ -276,7 +294,8 @@ def main(argv=None):
     res = register(model, cfg, load_point_cloud(opt.src), load_point_cloud(opt.tgt), opt.fit_radius, opt.icp,
                    opt.icp_iters, opt.icp_method, opt.normal_radius, opt.normal_max_nn, opt.icp_epsilon,
                    opt.icp_loss, opt.icp_loss_k, opt.ransac, ransac_kwargs(opt) if opt.ransac is not None else None,
-                   dict(fgr_kwargs(opt), overlap=opt.fgr_overlap) if opt.fgr else None)
+                   dict(fgr_kwargs(opt), overlap=opt.fgr_overlap) if opt.fgr else None, colors,
+                   opt.icp_lambda_geometric)
     n_shown = write_outputs(res, opt.out, opt.threshold)
     f = [float(v) for v in res['fit']]
     line = {'pose': pose44(final_pose(res)).tolist(),
@@ -313,13 +332,17 @@ def icp_line(opt, icp) -> Dict:
         line.update(icp_loss=opt.icp_loss, icp_loss_k=float(opt.icp_loss_k))
     if opt.icp_method == 'generalized':
         line.update(icp_epsilon=float(opt.icp_epsilon))
+    if opt.icp_method == 'colored':
+        line.update(icp_lambda_geometric=float(opt.icp_lambda_geometric))
     return line
 
 
-def main_fpfh(opt, src_xyz, tgt_xyz):
-    """`main` with --fpfh: `register_fpfh`, its files and its JSON line."""
-    res = register_fpfh(src_xyz, tgt_xyz, opt.fpfh, opt.fit_radius, opt.icp,
-                        icp_kwargs(opt) if opt.icp is not None else None, fpfh_kwargs(opt))
+def main_fpfh(opt, src_xyz, tgt_xyz, colors=None):
+    """`main` with --fpfh: `register_fpfh`, its files and its JSON line (colors: the files' rgb for colored ICP)."""
+    icp_options = None
+    if opt.icp is not None:
+        icp_options = dict(icp_kwargs(opt), **({} if colors is None else {'colors': ([colors[0]], [colors[1]])}))
+    res = register_fpfh(src_xyz, tgt_xyz, opt.fpfh, opt.fit_radius, opt.icp, icp_options, fpfh_kwargs(opt))
     write_outputs(res, opt.out)
     f = [float(v) for v in res['fit']]
     line = {'pose': pose44(final_pose(res)).tolist(), 'fitness_src': f[0], 'rmse_src': f[1], 'fitness_tgt': f[2],
