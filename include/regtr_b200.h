@@ -70,6 +70,23 @@ int regtr_grid_subsample_sorted(const float* xyz, const int32_t* offs, int n_clo
                                 float* out_xyz, int out_cap, int32_t* out_offs, uint32_t* status,
                                 void* ws, size_t ws_bytes, void* stream);
 
+/* Float64 voxel down-sampling with attributes (Open3D's PointCloud::VoxelDownSample), the multi-scale ICP pyramid's
+ * per-level step.  xyz (n_cap,3) float64 with offs (C+1) i32, offs[0] = 0, 1 <= C <= 32767; voxel V > 0 and finite
+ * (else REGTR_ERR_ARG).  attr (n_cap,3) float64, nullable (colours); out_attr is then required.
+ *   Per cloud: lo = the exact per-axis minimum of its points, origin = lo - 0.5 V, and point p falls in voxel
+ *   v = floor((p - origin) / V) per axis, the subtraction and the division each rounded to nearest (no contraction).
+ *   One output row per occupied voxel, rows in ascending (cloud, vx, vy, vz); a row is the float64 sum of its member
+ *   points in ascending point index divided by their count, and out_attr's row the same of their attributes.
+ * out_xyz / out_attr (n_cap,3) float64 capacity buffers (always sufficient); out_offs (C+1) i32 the rows of each
+ * cloud (an empty cloud has none).  An index above 65535 on any axis, or a non-finite coordinate, raises
+ * REGTR_STATUS_KEY_RANGE (Open3D allows up to INT_MAX); the rows are then not meaningful.  5 launches plus the
+ * library radix sort and scan whatever C and the data; no value atomics and no host synchronisation: a cloud's rows
+ * are the same bits alone or in a stack.  ws: regtr_voxel_down_sample_ws_bytes(n_cap, C). */
+size_t regtr_voxel_down_sample_ws_bytes(int n_cap, int C);
+int regtr_voxel_down_sample(const double* xyz, const double* attr, const int32_t* offs, int C, int n_cap,
+                            double voxel, double* out_xyz, double* out_attr, int32_t* out_offs, uint32_t* status,
+                            void* ws, size_t ws_bytes, void* stream);
+
 /* Uniform cell list over a stacked point set (search structure for regtr_ball_query).
  * `grid` is an opaque caller-owned buffer of regtr_cellgrid_bytes(n_cap) bytes; `order`
  * (n_cap) i32, optional, receives the cell-sorted permutation of the points (a spatially

@@ -14,6 +14,7 @@ on the GPU hot path.  Pinned against the reference's own functions by tests/gold
 """
 from __future__ import annotations
 
+import argparse
 import math
 import os
 from typing import Dict, Iterable, List
@@ -376,10 +377,42 @@ def summarize_modelnet_metrics(metrics: Dict[str, np.ndarray]) -> Dict[str, floa
 # ------------------------------------------------------------------- test loop (reference: test.py)
 
 
+def icp_levels(voxels, radii=None, level_iters=None, radius: float = None, max_iteration: int = 30):
+    """The multi-scale ICP pyramid as [(V_l, R_l, I_l)], or ValueError naming what is wrong.  voxels: L > 0 values,
+    strictly decreasing, all > 0 except that the last may be 0 (the full clouds, not down-sampled).  radii: the
+    levels' max correspondence distances, each finite and > 0 (default: V_l, Open3D's colored-ICP tutorial's rule; the
+    positional radius at V = 0).  level_iters: iterations at most per level, each >= 0 (default: max_iteration)."""
+    vox = [float(v) for v in voxels]
+    L = len(vox)
+    if L == 0:
+        raise ValueError('icp voxels: expected at least one level')
+    for name, vals in (('radii', radii), ('level_iters', level_iters)):
+        if vals is not None and len(vals) != L:
+            raise ValueError(f'icp {name}: {len(vals)} values for {L} voxels')
+    if not all(math.isfinite(v) for v in vox) or any(b >= a for a, b in zip(vox, vox[1:])) or \
+            any(v <= 0.0 for v in vox[:-1]) or vox[-1] < 0.0:
+        raise ValueError(f'icp voxels {vox}: must be finite and strictly decreasing, all > 0 except a last 0')
+    rad = [float(r) for r in radii] if radii is not None else [v if v > 0.0 else radius for v in vox]
+    if not all(r is not None and math.isfinite(r) and r > 0.0 for r in rad):
+        raise ValueError(f'icp radii {rad}: must be finite and > 0')
+    its = [int(i) for i in level_iters] if level_iters is not None else [int(max_iteration)] * L
+    if any(i < 0 for i in its):
+        raise ValueError(f'icp level_iters {its}: must be >= 0')
+    return list(zip(vox, rad, its))
+
+
+def _stack_levels(results):
+    """Per-level (B,4) results -> (B,L,4), torch or numpy as they come."""
+    if torch.is_tensor(results[0]):
+        return torch.stack(results, 1)
+    return np.stack([np.asarray(r) for r in results], 1)
+
+
 def icp_refine(src_list, tgt_list, init, radius: float, max_iteration: int = 30, method: str = 'point_to_point',
                normal_radius: float = None, normal_max_nn: int = 30, epsilon: float = 1e-3, loss: str = 'l2',
                loss_k: float = None, normals=None, icp=None, estimate_normals=None, colors=None,
-               lambda_geometric: float = 0.968, color_gradients=None):
+               lambda_geometric: float = 0.968, color_gradients=None, voxels=None, radii=None, level_iters=None,
+               return_levels: bool = False, voxel_down_sample=None):
     """Refine B poses init (B,3,4) by ICP of src_list onto tgt_list: the normals each method needs, then one icp call.
     -> icp's (pose (B,3,4), result).
     icp(src_list, tgt_list, init, radius, max_iteration, ...) defaults to `ops.icp`; point-to-point passes nothing
@@ -391,7 +424,46 @@ def icp_refine(src_list, tgt_list, init, radius: float, max_iteration: int = 30,
     method='colored' (Open3D's registration_colored_icp): colors=(src_colors, tgt_colors), B (n,3) rgb arrays each;
     the targets' normals are estimated as for point_to_plane, then their intensity gradients by
     color_gradients(tgt_list, normals, tgt_colors, 2 * radius, 30) (default `ops.color_gradients`; Open3D's own
-    parameters), and icp also gets src_colors=, tgt_colors=, tgt_color_gradients= and lambda_geometric=."""
+    parameters), and icp also gets src_colors=, tgt_colors=, tgt_color_gradients= and lambda_geometric=.
+    Multi-scale ICP (Open3D's colored-ICP tutorial, the tensor API's multi_scale_icp): voxels, radii and level_iters as
+    `icp_levels` takes them.  Level l down-samples src_list + tgt_list (and their colours, for 'colored') in one
+    voxel_down_sample(clouds, V_l, colors=) call (default `ops.voxel_down_sample`; none at V = 0), then runs the
+    single-level refinement above at R_l for at most I_l iterations from the previous level's pose (level 0 from
+    init): normals at 2 R_l with normal_max_nn, gradients at 2 R_l with 30.  normals= and normal_radius= are refused
+    with voxels.  -> the last level's (pose, result); return_levels adds the (B,L,4) results of every level (L = 1
+    without voxels)."""
+    if voxels is None:
+        pose, res = _icp_level(src_list, tgt_list, init, radius, max_iteration, method, normal_radius, normal_max_nn,
+                               epsilon, loss, loss_k, normals, icp, estimate_normals, colors, lambda_geometric,
+                               color_gradients)
+        return (pose, res, _stack_levels([res])) if return_levels else (pose, res)
+    if normals is not None or normal_radius is not None:
+        raise ValueError('icp_refine: normals= and normal_radius= do not go with voxels (each level estimates its own '
+                         'normals at 2 R_l)')
+    plan = icp_levels(voxels, radii, level_iters, radius, max_iteration)
+    if method == 'colored' and colors is None:
+        raise ValueError('icp_refine: colored ICP needs colors=(src_colors, tgt_colors)')
+    if voxel_down_sample is None:
+        from .ops import voxel_down_sample
+    B = len(src_list)
+    colors = colors if method == 'colored' else None
+    pose, results = init, []
+    for v, r, it in plan:
+        src, tgt, col = src_list, tgt_list, colors
+        if v > 0.0:
+            down, dc = voxel_down_sample(list(src_list) + list(tgt_list), v,
+                                         colors=None if colors is None else list(colors[0]) + list(colors[1]))
+            src, tgt = down[:B], down[B:]
+            col = None if dc is None else (dc[:B], dc[B:])
+        pose, res = _icp_level(src, tgt, pose, r, it, method, None, normal_max_nn, epsilon, loss, loss_k, None, icp,
+                               estimate_normals, col, lambda_geometric, color_gradients)
+        results.append(res)
+    return (pose, res, _stack_levels(results)) if return_levels else (pose, res)
+
+
+def _icp_level(src_list, tgt_list, init, radius, max_iteration, method, normal_radius, normal_max_nn, epsilon, loss,
+               loss_k, normals, icp, estimate_normals, colors, lambda_geometric, color_gradients):
+    """`icp_refine` at one scale: the normals and gradients the method needs, then one icp call."""
     if icp is None:
         from .ops import icp
     if method == 'colored' and colors is None:
@@ -426,10 +498,11 @@ def icp_refine(src_list, tgt_list, init, radius: float, max_iteration: int = 30,
     return icp(src_list, tgt_list, init, radius, max_iteration, **kw)
 
 
+
 def add_icp_arguments(ap, icp_help: str):
     """The ICP refinement flags of a command line, for `icp_refine`: --icp R (help text icp_help), --icp_iters,
-    --icp_method, --normal_radius, --normal_max_nn, --icp_epsilon, --icp_loss, --icp_loss_k and
-    --icp_lambda_geometric."""
+    --icp_method, --normal_radius, --normal_max_nn, --icp_epsilon, --icp_loss, --icp_loss_k,
+    --icp_lambda_geometric, and the multi-scale pyramid's --icp_voxels, --icp_radii and --icp_level_iters."""
     from .ops import ICP_LOSSES, ICP_METHODS
     ap.add_argument('--icp', type=float, metavar='R', help=icp_help)
     ap.add_argument('--icp_iters', type=int, default=30, help='ICP iterations at most (with --icp)')
@@ -448,18 +521,50 @@ def add_icp_arguments(ap, icp_help: str):
     ap.add_argument('--icp_loss_k', type=float, metavar='K', help='The robust kernel\'s parameter k')
     ap.add_argument('--icp_lambda_geometric', type=float, default=0.968, metavar='L',
                     help='Weight of the geometric residual of colored ICP, in [0, 1]')
+    ap.add_argument('--icp_voxels', type=_number_list(float), metavar='V1,V2,...',
+                    help='Multi-scale ICP (with --icp): voxel sizes, strictly decreasing, a last 0 meaning the full '
+                         'clouds; every level down-samples both clouds, estimates its own normals at 2 R_l and starts '
+                         'from the previous level\'s pose')
+    ap.add_argument('--icp_radii', type=_number_list(float), metavar='R1,...',
+                    help='Max correspondence distance per level (with --icp_voxels; default: the voxel sizes, the '
+                         '--icp radius at a 0 voxel)')
+    ap.add_argument('--icp_level_iters', type=_number_list(int), metavar='I1,...',
+                    help='ICP iterations at most per level (with --icp_voxels; default: --icp_iters at every level)')
+
+
+def _number_list(kind):
+    """argparse type: 'a,b,c' -> [kind(a), kind(b), kind(c)]."""
+    def parse(text):
+        try:
+            return [kind(v) for v in text.split(',')]
+        except ValueError:
+            raise argparse.ArgumentTypeError(f'expected comma-separated {kind.__name__} values, got {text!r}')
+    return parse
 
 
 def check_icp_arguments(ap, opt, colors: bool = False):
     """Reject, as usage errors and before any model is loaded, a robust --icp_loss without its --icp_loss_k, an
-    --icp_lambda_geometric outside [0, 1], and --icp_method colored on a command line whose inputs carry no colour
-    (colors=False)."""
+    --icp_lambda_geometric outside [0, 1], --icp_method colored on a command line whose inputs carry no colour
+    (colors=False), and a pyramid that `icp_levels` refuses, --icp_voxels / --icp_radii / --icp_level_iters without
+    --icp, the last two without --icp_voxels, or --normal_radius with --icp_voxels."""
     if opt.icp_loss != 'l2' and opt.icp_loss_k is None:
         ap.error(f'--icp_loss {opt.icp_loss} needs --icp_loss_k')
     if not 0.0 <= opt.icp_lambda_geometric <= 1.0:
         ap.error(f'--icp_lambda_geometric {opt.icp_lambda_geometric} must be in [0, 1]')
     if opt.icp_method == 'colored' and not colors:
         ap.error('--icp_method colored needs coloured clouds, and this command line reads none')
+    given = [f for f in ('icp_voxels', 'icp_radii', 'icp_level_iters') if getattr(opt, f) is not None]
+    if given and opt.icp is None:
+        ap.error(f'--{given[0]} needs --icp')
+    if given and opt.icp_voxels is None:
+        ap.error(f'--{given[0]} needs --icp_voxels')
+    if opt.icp_voxels is not None:
+        if opt.normal_radius is not None:
+            ap.error('--normal_radius does not go with --icp_voxels: every level estimates its normals at 2 R_l')
+        try:
+            icp_levels(opt.icp_voxels, opt.icp_radii, opt.icp_level_iters, opt.icp, opt.icp_iters)
+        except ValueError as e:
+            ap.error(f'--icp_voxels / --icp_radii / --icp_level_iters: {e}')
 
 
 def load_icp_colors(ap, opt, paths):
@@ -479,12 +584,14 @@ def load_icp_colors(ap, opt, paths):
 
 def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None, method: str = 'point_to_point',
                 normal_radius: float = None, normal_max_nn: int = 30, estimate_normals=None, epsilon: float = 1e-3,
-                loss: str = 'l2', loss_k: float = None, lambda_geometric: float = 0.968, color_gradients=None):
+                loss: str = 'l2', loss_k: float = None, lambda_geometric: float = 0.968, color_gradients=None,
+                voxels=None, radii=None, level_iters=None):
     """Wrap `forward_fn(batch) -> pred` so that the final pose of every pair is refined by ICP on the batch's full
     clouds: -> a NEW dict with pred's entries, pose (1,B,3,4) float64 the refined poses and pose_coarse
     (1,B,3,4) float64 the network's final poses (so that `compute_metrics` reports both, and EstLogWriter writes the
     refined ones).  pred's own tensors are not written to (a graphed forward owns them).
-    The refinement is `icp_refine` with these arguments, icp, estimate_normals and color_gradients included; with
+    The refinement is `icp_refine` with these arguments, icp, estimate_normals, color_gradients and the pyramid's
+    voxels, radii and level_iters included; with
     method='colored' the colours are the batch's src_colors / tgt_colors (a batch without them raises ValueError)."""
     from .ops import ICP_METHODS
     if method not in ICP_METHODS:
@@ -492,11 +599,11 @@ def icp_forward(forward_fn, radius: float, max_iteration: int = 30, icp=None, me
     def run(batch):
         pred = forward_fn(batch)
         coarse = pred['pose'][-1].to(torch.float64)                     # (B,3,4), a new tensor
-        kw = {}
+        kw = {} if voxels is None else dict(voxels=voxels, radii=radii, level_iters=level_iters)
         if method == 'colored':
             if 'src_colors' not in batch or 'tgt_colors' not in batch:
                 raise ValueError('icp_forward: colored ICP needs the batch\'s src_colors and tgt_colors')
-            kw = dict(colors=(batch['src_colors'], batch['tgt_colors']), lambda_geometric=lambda_geometric,
+            kw.update(colors=(batch['src_colors'], batch['tgt_colors']), lambda_geometric=lambda_geometric,
                       color_gradients=color_gradients)
         pose, _ = icp_refine(batch['src_xyz'], batch['tgt_xyz'], coarse, radius, max_iteration, method,
                              normal_radius, normal_max_nn, epsilon, loss, loss_k, icp=icp,
@@ -736,8 +843,8 @@ def fpfh_register(src_list, tgt_list, voxel: float, normal_radius: float = None,
     arguments are then unused.  With icp_radius, `icp_refine` (icp_kwargs) then starts from the global poses on the
     full clouds.
     -> dict: pose (B,3,4) float64 (the final poses), pose_fpfh (B,3,4) the RANSAC (or FGR) poses, ransac (B,5) (or
-    fgr (B,4)), n_mutual (B,), src_down / tgt_down (B downsampled clouds), and icp (B,4) with icp_radius; device
-    tensors."""
+    fgr (B,4)), n_mutual (B,), src_down / tgt_down (B downsampled clouds), and icp (B,4) with icp_radius (and
+    icp_levels (B,L,4) with voxels in icp_kwargs); device tensors."""
     from . import ops
     if method not in ('ransac', 'fgr'):
         raise ValueError(f'fpfh_register: unknown method {method!r}')
@@ -753,8 +860,7 @@ def fpfh_register(src_list, tgt_list, voxel: float, normal_radius: float = None,
         pose, res, n_mutual = ops.fgr_feature_matching(down[:B], down[B:], feats[:B], feats[B:], pair_base=pair_base,
                                                        **kw)
         out = dict(pose=pose, pose_fpfh=pose, fgr=res, n_mutual=n_mutual, src_down=down[:B], tgt_down=down[B:])
-        if icp_radius is not None:
-            out['pose'], out['icp'] = icp_refine(src_list, tgt_list, pose, icp_radius, **(icp_kwargs or {}))
+        _fpfh_icp(out, src_list, tgt_list, icp_radius, icp_kwargs)
         return out
     r = 1.5 * voxel if ransac_radius is None else ransac_radius
     pose, res, n_mutual = ops.ransac_feature_matching(
@@ -762,9 +868,20 @@ def fpfh_register(src_list, tgt_list, voxel: float, normal_radius: float = None,
         confidence=confidence, edge_length=edge_length, distance=r if distance is None else distance, seed=seed,
         pair_base=pair_base)
     out = dict(pose=pose, pose_fpfh=pose, ransac=res, n_mutual=n_mutual, src_down=down[:B], tgt_down=down[B:])
-    if icp_radius is not None:
-        out['pose'], out['icp'] = icp_refine(src_list, tgt_list, pose, icp_radius, **(icp_kwargs or {}))
+    _fpfh_icp(out, src_list, tgt_list, icp_radius, icp_kwargs)
     return out
+
+
+def _fpfh_icp(out, src_list, tgt_list, icp_radius, icp_kwargs):
+    """`fpfh_register`'s ICP from out['pose'] (with icp_radius): sets pose and icp, and icp_levels (B,L,4) when
+    icp_kwargs has voxels."""
+    if icp_radius is None:
+        return
+    kw = dict(icp_kwargs or {})
+    levels = kw.get('voxels') is not None
+    out['pose'], out['icp'], *lv = icp_refine(src_list, tgt_list, out['pose'], icp_radius, return_levels=levels, **kw)
+    if levels:
+        out['icp_levels'] = lv[0]
 
 
 def fpfh_forward(voxel: float, icp_radius: float = None, icp_kwargs=None, **fpfh_kwargs):
@@ -833,11 +950,14 @@ def fpfh_kwargs(opt) -> Dict:
 
 
 def icp_kwargs(opt) -> Dict:
-    """`icp_refine`'s keyword arguments from the parsed --icp_* / --normal_* flags (without the radius)."""
+    """`icp_refine`'s keyword arguments from the parsed --icp_* / --normal_* flags (without the radius); voxels, radii
+    and level_iters only with --icp_voxels."""
     kw = dict(max_iteration=opt.icp_iters, method=opt.icp_method, normal_radius=opt.normal_radius,
               normal_max_nn=opt.normal_max_nn, epsilon=opt.icp_epsilon, loss=opt.icp_loss, loss_k=opt.icp_loss_k)
     if opt.icp_method == 'colored':
         kw['lambda_geometric'] = opt.icp_lambda_geometric
+    if opt.icp_voxels is not None:
+        kw.update(voxels=opt.icp_voxels, radii=opt.icp_radii, level_iters=opt.icp_level_iters)
     return kw
 
 

@@ -4,7 +4,8 @@ registration after RegTR's pairwise poses).
     python -m regtr_b200.multiway FRAG_0 FRAG_1 ... --ckpt <logdir>/ckpt/model-best.pth [--config <yaml>] --out DIR
         [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized|colored
          [--normal_radius NR] [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_lambda_geometric 0.968]
-         [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
+         [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]
+         [--icp_voxels V1,V2,... [--icp_radii R1,...] [--icp_level_iters I1,...]]]]
         [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
         [--fgr [--fgr_dist 0.025] [--fgr_iters 64] [--fgr_tuple_test] [--fgr_overlap 0.5] ...]
@@ -16,7 +17,8 @@ scenes are numbered cloud_bin_0..N-1, so position is the benchmark index).  The 
 cropped as `register` does.  Every pair i < j is registered with source j and target i (the 3DMatch benchmark's
 direction) in eager forwards of --batch_pairs pairs, then refined by `ops.icp` with --icp as `register --icp` does
 (generalized ICP uses each fragment's normals as source and as target normals; colored ICP reads every fragment's PLY
-colours, a fragment without them being a usage error, and takes its target's gradients at radius 2 R, 30 neighbours).  With --ransac R each pair's pose
+colours, a fragment without them being a usage error, and takes its target's gradients at radius 2 R, 30 neighbours;
+--icp_voxels runs multi-scale ICP, each level down-sampling the pair and its colours).  With --ransac R each pair's pose
 first comes from RANSAC over the network's correspondences (`ops.ransac`, as `register --ransac`), so that far loop
 closures with little overlap survive the network's outlier correspondences; ICP then starts from it.  --fgr does the
 same with Fast Global Registration over those correspondences (`ops.fgr`, as `register --fgr`) instead of RANSAC.
@@ -83,7 +85,8 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
                    normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
                    icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None,
                    fgr_options: Dict = None, colors: Sequence[np.ndarray] = None,
-                   icp_lambda_geometric: float = 0.968) -> np.ndarray:
+                   icp_lambda_geometric: float = 0.968, icp_voxels=None, icp_radii=None,
+                   icp_level_iters=None) -> np.ndarray:
     """RegTR's final-layer pose of every pair (i, j) of `all_pairs`, source j -> target i, optionally refined by ICP
     (`eval.icp_refine` with icp_method, epsilon=icp_epsilon, loss=icp_loss, loss_k=icp_loss_k; the point-to-plane and
     generalized methods use every fragment's normals, estimated once).
@@ -91,16 +94,20 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
     its further keyword arguments), pair p of `all_pairs` drawing as pair p whatever batch_pairs; ICP then starts from
     the RANSAC pose.  fgr_options (a dict, possibly empty): the same with `eval.fgr_refine` and these keyword arguments
     instead, pair p drawing its tuples as pair p.  colors: every fragment's (n,3) rgb, for icp_method='colored' (with
-    icp_lambda_geometric).
+    icp_lambda_geometric).  icp_voxels, icp_radii, icp_level_iters: multi-scale ICP (`eval.icp_refine`'s voxels, radii
+    and level_iters); every level estimates its own normals (with normal_max_nn) on the down-sampled pair, so the
+    once-per-fragment normals are skipped, and the colours are down-sampled with the fragments.
     fragments: (n,3) float64 host arrays (already cropped).  -> (P,3,4) float64."""
     from . import ops
     dev = model.device
     pairs = all_pairs(len(fragments))
     dev_frags = [torch.from_numpy(np.ascontiguousarray(f)).float().to(dev) for f in fragments]
     normals = None
-    if icp_radius is not None and icp_method != 'point_to_point':
+    if icp_radius is not None and icp_method != 'point_to_point' and icp_voxels is None:
         nr = 2.0 * icp_radius if normal_radius is None else normal_radius
         normals = ops.estimate_normals(fragments, nr, normal_max_nn)
+    pyramid = {} if icp_voxels is None else dict(voxels=icp_voxels, radii=icp_radii, level_iters=icp_level_iters,
+                                                  normal_max_nn=normal_max_nn)
     out = []
     with torch.no_grad():
         for a in range(0, len(pairs), batch_pairs):
@@ -120,7 +127,7 @@ def register_pairs(model, fragments: Sequence[np.ndarray], batch_pairs: int = 8,
                                      ([normals[j] for _, j in chunk], [normals[i] for i, _ in chunk]),
                                      colors=None if colors is None else
                                      ([colors[j] for _, j in chunk], [colors[i] for i, _ in chunk]),
-                                     lambda_geometric=icp_lambda_geometric)
+                                     lambda_geometric=icp_lambda_geometric, **pyramid)
             out.append(pose.cpu().numpy())
     return np.concatenate(out, 0)
 
@@ -242,7 +249,7 @@ def main(argv=None):
                        opt.normal_max_nn, opt.icp_epsilon, opt.icp_loss, opt.icp_loss_k, opt.ransac,
                        ransac_kwargs(opt) if opt.ransac is not None else None,
                        dict(fgr_kwargs(opt), overlap=opt.fgr_overlap) if opt.fgr else None, colors,
-                       opt.icp_lambda_geometric)
+                       opt.icp_lambda_geometric, opt.icp_voxels, opt.icp_radii, opt.icp_level_iters)
     D = float(cfg['overlap_radius'] if opt.info_radius is None else opt.info_radius)
     res = optimize_scene(frags, T, D, opt.min_overlap, opt.preference_loop_closure)
     write_outputs(res, opt.out, scene_name(opt.fragments[0]), frags, opt.voxel)

@@ -1517,6 +1517,61 @@ def regtr_correspondences(pred, threshold: float = 0.5):
     return corr_src, corr_tgt, corr_mask
 
 
+STATUS_KEY_RANGE = 1                                                     # REGTR_STATUS_KEY_RANGE
+
+
+def voxel_down_sample_launches() -> int:
+    """Kernel launches of one `voxel_down_sample` call (the library radix sort and scan aside): the per-cloud minima,
+    the keys, the head flags, the means and the offsets."""
+    return 5
+
+
+def voxel_down_sample(clouds, voxel: float, colors=None, status=None):
+    """Open3D's voxel_down_sample of C clouds in one call (regtr_voxel_down_sample): a grid of voxel V anchored at each
+    cloud's bounding-box minimum minus V / 2, one point per occupied voxel, the float64 mean of its members in ascending
+    index order, rows in ascending (vx, vy, vz).  colors: C (n,3) arrays aligned with the clouds, averaged alike.
+    clouds / colors: numpy or torch, any float dtype; stacked in float64 on the device.
+    -> (list of C (m,3) float64 device tensors, list of C (m,3) colour tensors or None).  The row counts are read once
+    to split the output.  With status=None a voxel index above 65535 or a non-finite coordinate raises RegtrLibError;
+    with the caller's word, REGTR_STATUS_KEY_RANGE (STATUS_KEY_RANGE) is OR-ed into it and nothing is raised."""
+    v = float(voxel)
+    if not (v > 0.0 and math.isfinite(v)):
+        raise ValueError(f'voxel_down_sample: voxel {v} must be finite and > 0')
+    C = len(clouds)
+    if C == 0 or (colors is not None and len(colors) != C):
+        raise ValueError(f'voxel_down_sample: {C} clouds and {None if colors is None else len(colors)} colour arrays; '
+                         f'expected at least one cloud, and as many colour arrays when given')
+    ts = [torch.as_tensor(c) for c in clouds]
+    cs = None if colors is None else [torch.as_tensor(c) for c in colors]
+    for b, c in enumerate(ts):
+        if c.dim() != 2 or c.shape[1] != 3 or (cs is not None and tuple(cs[b].shape) != tuple(c.shape)):
+            raise ValueError(f'voxel_down_sample: cloud {tuple(c.shape)} and colors '
+                             f'{None if cs is None else tuple(cs[b].shape)}, expected (n,3) arrays')
+    L = _lib.load()
+    dev = next((c.device for c in ts + (cs or []) if c.is_cuda), torch.device('cuda', torch.cuda.current_device()))
+    xyz, lens = _stack_clouds(ts, dev, 3, 'voxel_down_sample')
+    rgb = None if cs is None else _stack_clouds(cs, dev, 3, 'voxel_down_sample')[0]
+    n_cap = xyz.shape[0]
+    offs = make_offsets(lens, dev)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    out = torch.empty((n_cap, 3), dtype=torch.float64, device=dev)
+    out_rgb = None if rgb is None else torch.empty((n_cap, 3), dtype=torch.float64, device=dev)
+    out_offs = torch.empty(C + 1, dtype=torch.int32, device=dev)
+    ws = workspace(L.regtr_voxel_down_sample_ws_bytes(n_cap, C), dev)
+    _lib.check(L.regtr_voxel_down_sample(_p(xyz), _p(rgb), _p(offs), C, n_cap, v, _p(out), _p(out_rgb), _p(out_offs),
+                                         _p(status), _p(ws), ws.numel(), _stream()), 'regtr_voxel_down_sample')
+    _count(voxel_down_sample_launches())
+    if own:
+        word = int(status.item())
+        if word:
+            raise _lib.RegtrLibError(f'voxel_down_sample at voxel {v}: a voxel index above 65535 or a coordinate that '
+                                     f'is not finite (status {word:#x})')
+    counts = np.diff(out_offs.cpu().numpy())
+    return _split(out, counts), None if out_rgb is None else _split(out_rgb, counts)
+
+
 NORMALS_MAX_NN = 64
 
 

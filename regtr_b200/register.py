@@ -4,7 +4,8 @@
         [--threshold 0.5] [--fit_radius R] [--out DIR]
         [--icp R [--icp_iters 30] [--icp_method point_to_point|point_to_plane|generalized|colored
          [--normal_radius NR] [--normal_max_nn 30] [--icp_epsilon 1e-3] [--icp_lambda_geometric 0.968]
-         [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
+         [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]
+         [--icp_voxels V1,V2,... [--icp_radii R1,...] [--icp_level_iters I1,...]]]]
         [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
         [--fgr [--fgr_dist 0.025] [--fgr_iters 64] [--fgr_division 1.4] [--fgr_tuple_test [--fgr_tuple_scale 0.95]
@@ -33,7 +34,12 @@ gradients (`ops.color_gradients`, radius 2 R, 30 neighbours at most, Open3D's pa
 registration_colored_icp (geometric weight --icp_lambda_geometric); --icp_loss with --icp_loss_k weights the
 point-to-plane, generalized or colored residuals by Open3D's robust kernel of that name;
 pose.txt, src_registered.ply and fit then use the refined pose, result.npz gains pose_coarse (the network's final
-pose), pose_icp (the refined one) and icp (4,) = fitness, inlier_rmse, correspondences, iterations.
+pose), pose_icp (the refined one) and icp (4,) = fitness, inlier_rmse, correspondences, iterations.  --icp_voxels
+V1,V2,... runs multi-scale ICP (Open3D's colored-ICP tutorial): level l down-samples both clouds at V_l
+(`ops.voxel_down_sample`, a grid anchored at each cloud's bounding box; a last 0 keeps the full clouds), estimates its
+normals at 2 R_l and runs ICP at R_l (--icp_radii, default V_l, or R at a 0 voxel) for at most I_l iterations
+(--icp_level_iters, default --icp_iters) from the previous level's pose; icp is then the last level's, and result.npz
+and the JSON line gain icp_levels (L,4), the JSON line also icp_voxels, icp_radii and icp_level_iters.
 With --ransac R the final decoder layer's pose is replaced by RANSAC over the network's two-way correspondences with
 predicted overlap above --ransac_overlap (`ops.ransac`, Open3D's registration_ransac_based_on_correspondence with max
 correspondence distance R on the cropped full-resolution clouds, --ransac_iters hypotheses at most, confidence
@@ -80,7 +86,8 @@ import torch
 
 from .eval import (add_fgr_arguments, add_fpfh_arguments, add_icp_arguments, add_ransac_arguments,
                    check_fgr_arguments, check_fpfh_arguments, check_icp_arguments, check_ransac_arguments, fgr_kwargs,
-                   fgr_refine, fpfh_kwargs, fpfh_register, icp_kwargs, icp_refine, ransac_kwargs, ransac_refine)
+                   fgr_refine, fpfh_kwargs, fpfh_register, icp_kwargs, icp_levels, icp_refine, ransac_kwargs,
+                   ransac_refine)
 
 
 def parser() -> argparse.ArgumentParser:
@@ -151,7 +158,8 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
              icp_radius: float = None, icp_iters: int = 30, icp_method: str = 'point_to_point',
              normal_radius: float = None, normal_max_nn: int = 30, icp_epsilon: float = 1e-3, icp_loss: str = 'l2',
              icp_loss_k: float = None, ransac_radius: float = None, ransac_options: Dict = None,
-             fgr_options: Dict = None, colors=None, icp_lambda_geometric: float = 0.968) -> Dict:
+             fgr_options: Dict = None, colors=None, icp_lambda_geometric: float = 0.968, icp_voxels=None,
+             icp_radii=None, icp_level_iters=None) -> Dict:
     """Crop, forward and fit one pair.  src_xyz / tgt_xyz (N,3) float64 host arrays; colors (src_rgb, tgt_rgb) (N,3)
     host arrays aligned with them, cropped alike, for icp_method='colored' (with icp_lambda_geometric).
     -> dict of host arrays: src_xyz / tgt_xyz (cropped, float64), pose (L,3,4) fp32, src_kp, src_kp_warped (final
@@ -159,7 +167,9 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
     icp_radius: refine the final layer's pose by ICP on the cropped clouds (`eval.icp_refine` with icp_method, at most
     icp_iters iterations, and normal_radius, normal_max_nn, icp_epsilon, icp_loss and icp_loss_k); fit is then that of
     the refined pose, and the dict gains pose_coarse (3,4) fp32 (the network's final pose), pose_icp (3,4) float64 and
-    icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations.
+    icp (4,) float64 = fitness, inlier_rmse, correspondences, iterations.  icp_voxels (with icp_radii and
+    icp_level_iters): multi-scale ICP (`eval.icp_refine`'s voxels, radii and level_iters); icp is then the last
+    level's, and the dict gains icp_levels (L,4) float64, the four numbers of every level.
     ransac_radius: first replace the final layer's pose by `eval.ransac_refine` at that radius on the cropped clouds,
     with ransac_options its further keyword arguments (ICP then starts from it); the dict gains pose_coarse,
     pose_ransac (3,4) float64 and ransac (5,) float64 = fitness, inlier_rmse, walked, validated, winner.
@@ -186,13 +196,17 @@ def register(model, cfg, src_xyz: np.ndarray, tgt_xyz: np.ndarray, fit_radius: f
             final, fgr = fgr_refine(out, [src_xyz], [tgt_xyz], **fgr_options)
             pose_fgr = final
         if icp_radius is not None:
-            final, icp = icp_refine([src_xyz], [tgt_xyz], final, icp_radius, icp_iters, icp_method, normal_radius,
-                                    normal_max_nn, icp_epsilon, icp_loss, icp_loss_k, colors=colors,
-                                    lambda_geometric=icp_lambda_geometric)
+            pyramid = {} if icp_voxels is None else dict(voxels=icp_voxels, radii=icp_radii,
+                                                          level_iters=icp_level_iters, return_levels=True)
+            final, icp, *levels = icp_refine([src_xyz], [tgt_xyz], final, icp_radius, icp_iters, icp_method,
+                                             normal_radius, normal_max_nn, icp_epsilon, icp_loss, icp_loss_k,
+                                             colors=colors, lambda_geometric=icp_lambda_geometric, **pyramid)
         fit = ops.registration_fit([src_xyz], [tgt_xyz], final, radius, status)
         res = {'src_xyz': src_xyz, 'tgt_xyz': tgt_xyz, 'pose': pose.cpu().numpy()}
         if icp_radius is not None:
             res.update(pose_coarse=res['pose'][-1], pose_icp=final[0].cpu().numpy(), icp=icp[0].cpu().numpy())
+            if levels:
+                res['icp_levels'] = levels[0][0].cpu().numpy()
         if ransac_radius is not None:
             res.update(pose_coarse=res['pose'][-1], pose_ransac=pose_ransac[0].cpu().numpy(),
                        ransac=ransac[0].cpu().numpy())
@@ -212,7 +226,8 @@ def register_fpfh(src_xyz: np.ndarray, tgt_xyz: np.ndarray, voxel: float, fit_ra
     """One pair without a network (`eval.fpfh_register` at voxel, fpfh_options its further keyword arguments, then ICP
     on the full clouds with icp_radius and icp_options).  -> dict of host arrays: src_xyz / tgt_xyz (float64),
     pose_fpfh (3,4) float64, ransac (5,) (fgr (4,) with method='fgr' in fpfh_options), n_mutual, n_src_down,
-    n_tgt_down, fit (4,) of the final pose at fit_radius, and pose_icp / icp with icp_radius."""
+    n_tgt_down, fit (4,) of the final pose at fit_radius, and pose_icp / icp with icp_radius (and icp_levels with
+    voxels in icp_options)."""
     from . import ops
     src_xyz = np.asarray(src_xyz, dtype=np.float64)
     tgt_xyz = np.asarray(tgt_xyz, dtype=np.float64)
@@ -226,6 +241,8 @@ def register_fpfh(src_xyz: np.ndarray, tgt_xyz: np.ndarray, voxel: float, fit_ra
            'fit': fit[0].cpu().numpy()}
     if icp_radius is not None:
         res.update(pose_icp=out['pose'][0].cpu().numpy(), icp=out['icp'][0].cpu().numpy())
+    if 'icp_levels' in out:
+        res['icp_levels'] = out['icp_levels'][0].cpu().numpy()
     return res
 
 
@@ -259,7 +276,7 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
     write_ply(os.path.join(out_dir, 'src_registered.ply'), res['src_xyz'] @ p[:, :3].T + p[:, 3])
     if 'pose_fpfh' in res:
         keys = ('pose_fpfh', 'fgr' if 'fgr' in res else 'ransac', 'n_mutual', 'fit') + \
-            (('pose_icp', 'icp') if 'pose_icp' in res else ())
+            (('pose_icp', 'icp') if 'pose_icp' in res else ()) + (('icp_levels',) if 'icp_levels' in res else ())
         np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
         return 0
     keys = ('pose', 'src_kp', 'src_kp_warped', 'src_overlap', 'tgt_kp', 'tgt_kp_warped', 'tgt_overlap', 'fit')
@@ -271,6 +288,8 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
         keys += ('pose_fgr', 'fgr')
     if 'pose_icp' in res:
         keys += ('pose_icp', 'icp')
+    if 'icp_levels' in res:
+        keys += ('icp_levels',)
     np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
     m = res['src_overlap'] > threshold
     write_ply(os.path.join(out_dir, 'src_kp.ply'), res['src_kp'][m], {'overlap': res['src_overlap'][m]})
@@ -295,7 +314,7 @@ def main(argv=None):
                    opt.icp_iters, opt.icp_method, opt.normal_radius, opt.normal_max_nn, opt.icp_epsilon,
                    opt.icp_loss, opt.icp_loss_k, opt.ransac, ransac_kwargs(opt) if opt.ransac is not None else None,
                    dict(fgr_kwargs(opt), overlap=opt.fgr_overlap) if opt.fgr else None, colors,
-                   opt.icp_lambda_geometric)
+                   opt.icp_lambda_geometric, opt.icp_voxels, opt.icp_radii, opt.icp_level_iters)
     n_shown = write_outputs(res, opt.out, opt.threshold)
     f = [float(v) for v in res['fit']]
     line = {'pose': pose44(final_pose(res)).tolist(),
@@ -305,7 +324,7 @@ def main(argv=None):
             'n_tgt_kp': int(res['tgt_kp'].shape[0]), 'n_src_kp_above_threshold': n_shown,
             'fit_radius': float(cfg['overlap_radius'] if opt.fit_radius is None else opt.fit_radius)}
     if opt.icp is not None:
-        line.update(icp_line(opt, res['icp']))
+        line.update(icp_line(opt, res))
     if opt.ransac is not None:
         rs = [float(v) for v in res['ransac']]
         line.update(ransac_fitness=rs[0], ransac_rmse=rs[1], ransac_iterations=int(rs[2]),
@@ -323,9 +342,10 @@ def fgr_line(opt, fgr) -> Dict:
                 fgr_dist=float(opt.fgr_dist))
 
 
-def icp_line(opt, icp) -> Dict:
-    """The JSON line's icp_* entries."""
-    icp = [float(v) for v in icp]
+def icp_line(opt, res: Dict) -> Dict:
+    """The JSON line's icp_* entries from `register`'s dict (those of the last level with --icp_voxels, which adds
+    icp_voxels, icp_radii and icp_level_iters as resolved and icp_levels, the four numbers of every level)."""
+    icp = [float(v) for v in res['icp']]
     line = dict(icp_fitness=icp[0], icp_rmse=icp[1], icp_iterations=int(icp[3]), icp_radius=float(opt.icp),
                 icp_method=opt.icp_method)
     if opt.icp_loss != 'l2':
@@ -334,6 +354,10 @@ def icp_line(opt, icp) -> Dict:
         line.update(icp_epsilon=float(opt.icp_epsilon))
     if opt.icp_method == 'colored':
         line.update(icp_lambda_geometric=float(opt.icp_lambda_geometric))
+    if opt.icp_voxels is not None:
+        plan = icp_levels(opt.icp_voxels, opt.icp_radii, opt.icp_level_iters, opt.icp, opt.icp_iters)
+        line.update(icp_voxels=[v for v, _, _ in plan], icp_radii=[r for _, r, _ in plan],
+                    icp_level_iters=[i for _, _, i in plan], icp_levels=res['icp_levels'].tolist())
     return line
 
 
@@ -356,7 +380,7 @@ def main_fpfh(opt, src_xyz, tgt_xyz, colors=None):
         line.update(ransac_fitness=rs[0], ransac_rmse=rs[1], ransac_iterations=int(rs[2]),
                     ransac_validations=int(rs[3]), ransac_radius=float(opt.ransac))
     if opt.icp is not None:
-        line.update(icp_line(opt, res['icp']))
+        line.update(icp_line(opt, res))
     print(json.dumps(line))
     return res
 

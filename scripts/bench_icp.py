@@ -16,7 +16,16 @@ oracle.  With colored, the synthetic pairs (which have no colour) are coloured b
 targets' normal estimation, their colour gradients (`ops.color_gradients`, radius 2 R, 30 neighbours, as
 `eval.icp_refine` uses) and the colored ICP are timed separately, L2 point-to-plane ICP on the same target normals is
 timed too, and the iterations are reported under both and for the oracle.  --loss applies to every method but
-point_to_point.  Prints one JSON line with the card name and power limit read in the same run."""
+point_to_point.  Prints one JSON line with the card name and power limit read in the same run.
+
+    python scripts/bench_icp.py --voxels V1,V2,... [--radii R1,...] [--level_iters I1,...] [--method ...]
+        [--deg 4 --metres 0.04]
+
+times multi-scale ICP (`eval.icp_refine` with voxels=) instead, on pairs perturbed by --deg / --metres: per level the
+down-sampling of all 2B clouds (`ops.voxel_down_sample`), the normals, the colour gradients (colored) and the ICP from
+that level's starting pose; the whole pyramid; and single-level ICP at the finest radius (--radius) with --iters
+iterations.  It reports the iterations of every level and the rotation (degrees) and translation (metres) errors of
+both results against the ground truth."""
 import argparse
 import json
 import os
@@ -144,6 +153,89 @@ def time_device(pairs, iters, radius, blocks, reps, method='point_to_point', nor
     return out, host(normals), host(src_normals), host(colour_kw.get('tgt_color_gradients'))
 
 
+def pose_errors(pose, pairs, seed0=7000):
+    """-> (rotation errors in degrees, translation errors in metres) of B poses against the pairs' ground truths."""
+    rot, trans = [], []
+    for b, p in enumerate(np.asarray(pose)):
+        gt = make_3dmatch_pair(seed0 + b)['pose']
+        c = (np.trace(p[:, :3] @ gt[:, :3].T) - 1.0) / 2.0
+        rot.append(round(float(np.degrees(np.arccos(np.clip(c, -1.0, 1.0)))), 4))
+        trans.append(round(float(np.linalg.norm(p[:, 3] - gt[:, 3])), 5))
+    return rot, trans
+
+
+def time_pyramid(pairs, opt, colours=None):
+    """Multi-scale ICP of one batch: -> dict of per-level and total timings, iterations and pose errors."""
+    from regtr_b200 import eval as E
+    dev = torch.device('cuda:0')
+    B = len(pairs)
+    src = [torch.from_numpy(s).to(dev) for s, _, _ in pairs]
+    tgt = [torch.from_numpy(t).to(dev) for _, t, _ in pairs]
+    init = torch.from_numpy(np.stack([p for _, _, p in pairs])).to(dev)
+    cols = None
+    if colours is not None:
+        cols = ([torch.from_numpy(s).to(dev) for s, _ in colours], [torch.from_numpy(t).to(dev) for _, t in colours])
+    plan = E.icp_levels(opt.voxels, opt.radii, opt.level_iters, opt.radius, opt.iters)
+    kw = dict(voxels=opt.voxels, radii=opt.radii, level_iters=opt.level_iters, normal_max_nn=opt.normal_max_nn,
+              loss=opt.loss, loss_k=opt.loss_k, epsilon=opt.epsilon, colors=cols, lambda_geometric=opt.lambda_geometric)
+    starts = []
+
+    def record(s, t, x, r, it, **k):
+        starts.append(x.clone())
+        return ops.icp(s, t, x, r, it, **k)
+    E.icp_refine(src, tgt, init, opt.radius, opt.iters, opt.method, icp=record, **kw)
+
+    def stat(ms):
+        return dict(ms_median=float(np.median(ms)), ms_min=float(min(ms)), ms_max=float(max(ms)))
+    levels = []
+    for (v, r, it), x in zip(plan, starts):
+        row = {'voxel': v, 'radius': r, 'level_iters': it}
+        s_l, t_l, c_l = src, tgt, cols
+        if v > 0:
+            flat = None if cols is None or opt.method != 'colored' else cols[0] + cols[1]
+            ms, _, (down, dc) = time_calls(lambda st: ops.voxel_down_sample(src + tgt, v, colors=flat, status=st), r,
+                                           'voxel_down_sample', opt.blocks, opt.reps)
+            row['down_sample'] = stat(ms)
+            s_l, t_l = down[:B], down[B:]
+            c_l = None if dc is None else (dc[:B], dc[B:])
+        row['points_per_cloud'] = int(np.mean([len(c) for c in s_l + t_l]))
+        normals = src_normals = None
+        icp_kw = {}
+        if opt.method != 'point_to_point':
+            clouds = s_l + t_l if opt.method == 'generalized' else t_l
+            ms, _, normals = time_calls(lambda st: ops.estimate_normals(clouds, 2.0 * r, opt.normal_max_nn, st),
+                                        2.0 * r, 'estimate_normals', opt.blocks, opt.reps)
+            row['normals'] = stat(ms)
+            if opt.method == 'generalized':
+                src_normals, normals = normals[:B], normals[B:]
+            icp_kw = dict(method=opt.method, tgt_normals=normals, src_normals=src_normals, epsilon=opt.epsilon,
+                          loss=opt.loss, loss_k=opt.loss_k)
+        if opt.method == 'colored':
+            ms, _, grads = time_calls(lambda st: ops.color_gradients(t_l, normals, c_l[1], 2.0 * r, 30, st), 2.0 * r,
+                                      'color_gradients', opt.blocks, opt.reps)
+            row['gradients'] = stat(ms)
+            icp_kw.update(src_colors=c_l[0], tgt_colors=c_l[1], tgt_color_gradients=grads,
+                          lambda_geometric=opt.lambda_geometric)
+        ms, _, (_, res) = time_calls(lambda st: ops.icp(s_l, t_l, x, r, it, status=st, **icp_kw), r, 'icp',
+                                     opt.blocks, opt.reps)
+        row['icp'] = stat(ms)
+        row['iterations'] = [int(i) for i in res[:, 3].cpu().numpy()]
+        levels.append(row)
+    ms, _, (pose, _) = time_calls(lambda st: E.icp_refine(src, tgt, init, opt.radius, opt.iters, opt.method, **kw),
+                                  opt.radius, 'icp_refine', opt.blocks, opt.reps)
+    one_kw = dict(kw, voxels=None, radii=None, level_iters=None)
+    ms1, _, (pose1, res1) = time_calls(
+        lambda st: E.icp_refine(src, tgt, init, opt.radius, opt.iters, opt.method, **one_kw), opt.radius,
+        'icp_refine', opt.blocks, opt.reps)
+    rot, trans = pose_errors(pose.cpu().numpy(), pairs)
+    rot1, trans1 = pose_errors(pose1.cpu().numpy(), pairs)
+    rot0, trans0 = pose_errors(init.cpu().numpy(), pairs)
+    return dict(levels=levels, pyramid=dict(stat(ms), rot_err_deg=rot, trans_err_m=trans),
+                single_level=dict(stat(ms1), iterations=[int(i) for i in res1[:, 3].cpu().numpy()], rot_err_deg=rot1,
+                                  trans_err_m=trans1),
+                init_rot_err_deg=rot0, init_trans_err_m=trans0)
+
+
 def parser():
     ap = argparse.ArgumentParser()
     ap.add_argument('--iters', type=int, default=30)
@@ -158,6 +250,12 @@ def parser():
     ap.add_argument('--lambda_geometric', type=float, default=0.968, help='geometric weight of colored ICP')
     ap.add_argument('--loss', choices=ops.ICP_LOSSES, default='l2')
     ap.add_argument('--loss_k', type=float)
+    num = lambda kind: lambda text: [kind(v) for v in text.split(',')]          # noqa: E731
+    ap.add_argument('--voxels', type=num(float), help='multi-scale ICP: voxel sizes V1,V2,... (a last 0: full clouds)')
+    ap.add_argument('--radii', type=num(float), help='per-level radii (default: the voxels)')
+    ap.add_argument('--level_iters', type=num(int), help='per-level iterations (default: --iters)')
+    ap.add_argument('--deg', type=float, default=4.0, help='perturbation of the ground truth, degrees')
+    ap.add_argument('--metres', type=float, default=0.04, help='perturbation of the ground truth, metres')
     return ap
 
 
@@ -176,6 +274,13 @@ def main():
         out['epsilon'] = opt.epsilon
     if opt.method == 'colored':
         out.update(lambda_geometric=opt.lambda_geometric, gradient_radius=2.0 * opt.radius, gradient_max_nn=30)
+    if opt.voxels is not None:
+        out.update(voxels=opt.voxels, radii=opt.radii, level_iters=opt.level_iters, deg=opt.deg, metres=opt.metres)
+        for B in (1, 8):
+            pairs = perturbed_pairs(B, deg=opt.deg, metres=opt.metres)
+            out[f'B{B}'] = time_pyramid(pairs, opt, pair_colours(B) if opt.method == 'colored' else None)
+        print(json.dumps(out))
+        return
     for B in (1, 8):
         pairs = perturbed_pairs(B)
         colours = pair_colours(B) if opt.method == 'colored' else None

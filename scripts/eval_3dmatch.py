@@ -3,7 +3,8 @@
     python scripts/eval_3dmatch.py --root <data/indoor> --info <test_3DMatch_info.pkl> \
         --gt <datasets/3dmatch/benchmarks/3DMatch> --ckpt <model.pth> --out logs/3DMatch [--icp R [--icp_iters N]
         [--icp_method point_to_plane|generalized [--normal_radius NR] [--normal_max_nn 30] [--icp_epsilon 1e-3]
-        [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]]]
+        [--icp_loss l2|huber|cauchy|gm|tukey --icp_loss_k K]
+        [--icp_voxels V1,V2,... [--icp_radii R1,...] [--icp_level_iters I1,...]]]]
         [--ransac R [--ransac_iters 100000] [--ransac_confidence 0.999] [--ransac_n 3] [--ransac_edge 0.9]
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
         [--fgr [--fgr_dist 0.025] [--fgr_iters 64] [--fgr_tuple_test] [--fgr_overlap 0.5] ...]
@@ -13,7 +14,8 @@
 
 --icp R refines every final pose by ICP on the full clouds (`ops.icp`, max correspondence distance R; point-to-point,
 or point-to-plane against target normals from `ops.estimate_normals` at NR, default 2 R, or generalized ICP on the
-normals of both clouds, optionally under a robust loss): est.log then holds the
+normals of both clouds, optionally under a robust loss; --icp_voxels runs multi-scale ICP over a voxel pyramid of the
+clouds, `eval.icp_refine`'s voxels / radii / level_iters): est.log then holds the
 refined poses, and the metrics report both (`rot_err_deg` / `trans_err` refined, `*_coarse` the network's).
 --ransac R replaces every network pose by RANSAC over the network's correspondences with predicted overlap above
 --ransac_overlap (`ops.ransac`, max correspondence distance R, validated on the full clouds); with --icp as well, ICP
@@ -63,7 +65,8 @@ def network_forward(args):
                              **E.fgr_kwargs(args))
     return (lambda b: runner(b)) if args.icp is None else E.icp_forward(
         lambda b: runner(b), args.icp, args.icp_iters, method=args.icp_method, normal_radius=args.normal_radius,
-        normal_max_nn=args.normal_max_nn, epsilon=args.icp_epsilon, loss=args.icp_loss, loss_k=args.icp_loss_k)
+        normal_max_nn=args.normal_max_nn, epsilon=args.icp_epsilon, loss=args.icp_loss, loss_k=args.icp_loss_k,
+        voxels=args.icp_voxels, radii=args.icp_radii, level_iters=args.icp_level_iters)
 
 
 def main(argv=None):
