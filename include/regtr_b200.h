@@ -87,6 +87,71 @@ int regtr_voxel_down_sample(const double* xyz, const double* attr, const int32_t
                             double voxel, double* out_xyz, double* out_attr, int32_t* out_offs, uint32_t* status,
                             void* ws, size_t ws_bytes, void* stream);
 
+/* Outlier removal (Open3D's PointCloud::RemoveStatisticalOutliers and RemoveRadiusOutliers) for C stacked clouds:
+ * xyz (n_cap,3) float64 with offs (C+1) i32, offs[0] = 0, 1 <= C <= 32767.  Each filter writes per-point keep flags
+ * (n_cap) i32, 1 = kept, rows >= offs[C] untouched; regtr_select_points then gathers the kept rows.  No value atomics
+ * and no host synchronisation: a cloud's results are the same bits alone or in a stack, and the launch counts
+ * depend on neither the data nor C.  ws: regtr_outlier_ws_bytes(n_cap, C); state: regtr_outlier_state_bytes(n_cap),
+ * ZERO before the first call, every call leaves it zero.
+ *
+ * k nearest neighbours (both in the statistical filter): the neighbours of point i are the k points of i's own cloud
+ * with the smallest (d^2, index) keys, d^2 = (dx dx + dy dy) + dz dz in float64, each operation rounded on its own
+ * (no contraction), i itself included, ties to the lower index, all m = min(k, n) points of a cloud of n < k points;
+ * no radius.  The result is defined by this rule, not by the search (one warp per point walks rings of cells of a
+ * cell list of size `cell` around the point and sweeps its whole cloud past 4 rings), so it is the same bits for any
+ * cell size.
+ *
+ * regtr_statistical_outlier, RemoveStatisticalOutliers(nb_neighbors, std_ratio) restated:
+ *   1. for each point i, its k = nb_neighbors nearest neighbours by the rule above, m = min(k, n) of them;
+ *   2. avg_i = (sum of sqrt(d^2)) / m, the sum sequential in ascending (d^2, index) order (nanoflann's result order);
+ *   3. valid = the number of points with m > 0, i.e. n for a non-empty cloud;
+ *   4. cloud_mean = (sum of avg_i over the points with avg_i > 0) / valid: points with avg 0 are left out of the sum
+ *      but counted in valid (Open3D's rule, kept);
+ *   5. sq_sum = sum over the points with avg_i > 0 of (avg_i - cloud_mean)^2;
+ *   6. std_dev = sqrt(sq_sum / (valid - 1)), threshold = cloud_mean + std_ratio * std_dev;
+ *   7. point i is kept iff avg_i > 0 and avg_i < threshold.
+ *   So exact duplicates of k or more points are dropped, a one-point cloud keeps nothing (valid - 1 = 0 makes the
+ *   threshold NaN) and an empty cloud yields nothing (its statistics are NaN).
+ *   Summation order (the departure from Open3D, which sums 4. and 5. sequentially over the cloud): each sum runs over
+ *   chunks of 256 points anchored at the cloud's first point, past-the-end entries 0 and excluded points 0; a chunk
+ *   is reduced by the fixed tree e[i] = e[i] + e[i + h] for h = 128, 64, ..., 1, and the chunk partials are added in
+ *   ascending chunk order starting from 0.  Every operation is rounded on its own, including (avg_i - cloud_mean)^2,
+ *   std_ratio * std_dev and its addition.  The result then differs from Open3D's sequential sums in the last bits of
+ *   cloud_mean and std_dev at most.
+ *   nb_neighbors in 1..64, std_ratio > 0 and finite, cell > 0 and finite (else REGTR_ERR_ARG).  avg (n_cap) f64;
+ *   stats (C,3) f64: (cloud_mean, std_dev, threshold) per cloud.  A |coordinate| above 1e30 (the cell list holds fp32
+ *   copies) or not finite raises REGTR_STATUS_RANGE; a cell index of floor(fp32(p) / cell) outside +-32766 raises
+ *   REGTR_STATUS_KEY_RANGE, so a caller picks cell >= max |coordinate| / 32000 (ops.knn_cell does).  1 + 4 + 7
+ *   launches.
+ *
+ * regtr_radius_outlier, RemoveRadiusOutliers(nb_points, radius): counts[i] = the number of points of i's own cloud
+ *   with d^2 (as above) strictly below radius^2, i included (the library's radius rule and nanoflann's strict test),
+ *   always the full count; point i is kept iff counts[i] >= nb_points.  nb_points >= 1, radius > 0 and finite, cell
+ *   = radius * (1 + 1e-3) rounded to fp32 (ops.overlap_cell), cell > radius (else REGTR_ERR_ARG).  counts (n_cap)
+ *   i32.  A |coordinate| beyond regtr_overlap_coord_bound(radius, cell), or not finite, raises REGTR_STATUS_RANGE,
+ *   as in regtr_estimate_normals.  1 + 4 + 1 launches.
+ *
+ * regtr_select_points: the stable compaction of either filter's output.  keep (n_cap) i32, nonzero = kept; attr
+ * (n_cap,3) f64 nullable (colours), out_attr then required.  Kept rows go to out_xyz / out_attr (n_cap,3) in their
+ * original order; out_index (n_cap) i32, nullable, receives the index of each kept row inside its own cloud;
+ * out_offs (C+1) i32 the kept rows of each cloud.  3 launches (flags, the single-pass scan, the scatter).
+ * ws: regtr_select_points_ws_bytes(n_cap); state: regtr_select_points_state_bytes(n_cap), ZERO before the first call,
+ * every call leaves it zero. */
+size_t regtr_outlier_ws_bytes(int n_cap, int C);
+size_t regtr_outlier_state_bytes(int n_cap);
+int regtr_statistical_outlier(const double* xyz, const int32_t* offs, int C, int n_cap, int nb_neighbors,
+                              double std_ratio, float cell, double* avg, int32_t* keep, double* stats,
+                              uint32_t* status, void* ws, size_t ws_bytes, void* state, size_t state_bytes,
+                              void* stream);
+int regtr_radius_outlier(const double* xyz, const int32_t* offs, int C, int n_cap, int nb_points, double radius,
+                         float cell, int32_t* counts, int32_t* keep, uint32_t* status, void* ws, size_t ws_bytes,
+                         void* state, size_t state_bytes, void* stream);
+size_t regtr_select_points_ws_bytes(int n_cap);
+size_t regtr_select_points_state_bytes(int n_cap);
+int regtr_select_points(const double* xyz, const double* attr, const int32_t* keep, const int32_t* offs, int C,
+                        int n_cap, double* out_xyz, double* out_attr, int32_t* out_index, int32_t* out_offs, void* ws,
+                        size_t ws_bytes, void* state, size_t state_bytes, void* stream);
+
 /* Uniform cell list over a stacked point set (search structure for regtr_ball_query).
  * `grid` is an opaque caller-owned buffer of regtr_cellgrid_bytes(n_cap) bytes; `order`
  * (n_cap) i32, optional, receives the cell-sorted permutation of the points (a spatially

@@ -567,6 +567,60 @@ def check_icp_arguments(ap, opt, colors: bool = False):
             ap.error(f'--icp_voxels / --icp_radii / --icp_level_iters: {e}')
 
 
+def add_outlier_arguments(ap):
+    """The outlier-removal flags of a command line, for `remove_outliers`: --remove_statistical_outlier K S and
+    --remove_radius_outlier N R."""
+    ap.add_argument('--remove_statistical_outlier', nargs=2, metavar=('K', 'S'),
+                    help='Drop the points whose mean distance to their K nearest neighbours is at least S standard '
+                         'deviations above their cloud\'s mean (Open3D\'s remove_statistical_outlier), on the clouds as '
+                         'read, before the crop')
+    ap.add_argument('--remove_radius_outlier', nargs=2, metavar=('N', 'R'),
+                    help='Drop the points with fewer than N points within radius R (Open3D\'s remove_radius_outlier), '
+                         'on the clouds as read, after --remove_statistical_outlier and before the crop')
+
+
+def check_outlier_arguments(ap, opt):
+    """Reject, as usage errors, outlier options the filters would refuse, before any model is loaded, and turn the
+    flags' values into (nb_neighbors int, std_ratio float) and (nb_points int, radius float)."""
+    from .ops import OUTLIER_MAX_NEIGHBORS
+    for flag, first, second in (('statistical', 'K', 'S'), ('radius', 'N', 'R')):
+        name = f'remove_{flag}_outlier'
+        vals = getattr(opt, name)
+        if vals is None:
+            continue
+        try:
+            n, v = int(vals[0]), float(vals[1])
+        except ValueError:
+            ap.error(f'--{name} {" ".join(vals)}: expected an integer {first} and a number {second}')
+        if flag == 'statistical' and not (1 <= n <= OUTLIER_MAX_NEIGHBORS and math.isfinite(v) and v > 0.0):
+            ap.error(f'--{name} {n} {v}: K must be in 1..{OUTLIER_MAX_NEIGHBORS} and S finite and > 0')
+        if flag == 'radius' and not (n >= 1 and math.isfinite(v) and v > 0.0):
+            ap.error(f'--{name} {n} {v}: N must be >= 1 and R finite and > 0')
+        setattr(opt, name, (n, v))
+
+
+def remove_outliers(clouds, colors=None, statistical=None, radius=None, remove_statistical_outlier=None,
+                    remove_radius_outlier=None):
+    """The clouds (and colours) of a command line filtered as its outlier flags ask: `ops.remove_statistical_outlier`
+    with statistical = (nb_neighbors, std_ratio), then `ops.remove_radius_outlier` with radius = (nb_points, radius)
+    on what is left, every cloud in one call each (either function injectable).
+    clouds / colors: lists of (n,3) host arrays.  -> (clouds, colours or None, indices): lists of host float64 arrays
+    and of int64 arrays, the rows of each input cloud that survive, ascending."""
+    if remove_statistical_outlier is None or remove_radius_outlier is None:
+        from . import ops
+        remove_statistical_outlier = remove_statistical_outlier or ops.remove_statistical_outlier
+        remove_radius_outlier = remove_radius_outlier or ops.remove_radius_outlier
+    index = [np.arange(np.asarray(c).shape[0], dtype=np.int64) for c in clouds]
+    for fn, args in ((remove_statistical_outlier, statistical), (remove_radius_outlier, radius)):
+        if args is None:
+            continue
+        kept, kc, ki = fn(clouds, args[0], args[1], colors=colors)
+        clouds = [np.asarray(torch.as_tensor(c).cpu(), dtype=np.float64) for c in kept]
+        colors = None if kc is None else [np.asarray(torch.as_tensor(c).cpu(), dtype=np.float64) for c in kc]
+        index = [ix[np.asarray(torch.as_tensor(k).cpu(), dtype=np.int64)] for ix, k in zip(index, ki)]
+    return clouds, colors, index
+
+
 def load_icp_colors(ap, opt, paths):
     """With --icp and --icp_method colored: the rgb (N,3) of every file of `paths` (`pointio.load_point_cloud_colors`),
     a file without colours being a usage error that names it; else None."""

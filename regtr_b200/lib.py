@@ -38,6 +38,13 @@ SIGNATURES = {
     'regtr_grid_subsample_sorted': (_I, [_P, _P, _I, _I, _F, _P, _I, _P, _P, _P, _Z, _P]),
     'regtr_voxel_down_sample_ws_bytes': (_Z, [_I, _I]),
     'regtr_voxel_down_sample': (_I, [_P, _P, _P, _I, _I, _c.c_double, _P, _P, _P, _P, _P, _Z, _P]),
+    'regtr_outlier_ws_bytes': (_Z, [_I, _I]),
+    'regtr_outlier_state_bytes': (_Z, [_I]),
+    'regtr_statistical_outlier': (_I, [_P, _P, _I, _I, _I, _c.c_double, _F, _P, _P, _P, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_radius_outlier': (_I, [_P, _P, _I, _I, _I, _c.c_double, _F, _P, _P, _P, _P, _Z, _P, _Z, _P]),
+    'regtr_select_points_ws_bytes': (_Z, [_I]),
+    'regtr_select_points_state_bytes': (_Z, [_I]),
+    'regtr_select_points': (_I, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _Z, _P, _Z, _P]),
     'regtr_cellgrid_bytes': (_Z, [_I]),
     'regtr_cellgrid_ws_bytes': (_Z, [_I]),
     'regtr_cellgrid_state_bytes': (_Z, [_I]),

@@ -10,7 +10,7 @@ registration after RegTR's pairwise poses).
          [--ransac_dist D] [--ransac_overlap 0.5] [--ransac_seed 0]]
         [--fgr [--fgr_dist 0.025] [--fgr_iters 64] [--fgr_tuple_test] [--fgr_overlap 0.5] ...]
         [--info_radius D] [--min_overlap 0.3] [--preference_loop_closure 1.0]
-        [--voxel V] [--batch_pairs 8]
+        [--voxel V] [--batch_pairs 8] [--remove_statistical_outlier K S] [--remove_radius_outlier N R]
 
 Fragments are given in sequence order, in any format `pointio` reads; fragment index = position in the list (3DMatch
 scenes are numbered cloud_bin_0..N-1, so position is the benchmark index).  The config is found and the clouds are
@@ -35,6 +35,10 @@ Outputs in DIR:
                        `scripts/evaluate_3dmatch.py --results_dir logs`;
   scene.ply            with --voxel V: every fragment moved by its pose, concatenated and grid-subsampled at V
                        (a barycentre per voxel).
+With --remove_statistical_outlier K S and / or --remove_radius_outlier N R every fragment is filtered once, as read and
+before the crop and the pairing, as `register` filters its clouds (all fragments in one call per filter, colours
+alike); the filtered fragments are the ones registered and written to scene.ply, and result.npz gains point_index (M,)
+and point_offsets (N+1,): fragment f's surviving rows are point_index[point_offsets[f]:point_offsets[f+1]].
 One JSON line on stdout: fragments, pairs, edges (odometry, loop, kept), iterations of both passes, final objective.
 """
 from __future__ import annotations
@@ -48,9 +52,9 @@ from typing import Dict, List, Sequence
 import numpy as np
 import torch
 
-from .eval import (add_fgr_arguments, add_icp_arguments, add_ransac_arguments, check_fgr_arguments,
-                   check_icp_arguments, check_ransac_arguments, fgr_kwargs, fgr_refine, icp_refine, ransac_kwargs,
-                   ransac_refine)
+from .eval import (add_fgr_arguments, add_icp_arguments, add_outlier_arguments, add_ransac_arguments,
+                   check_fgr_arguments, check_icp_arguments, check_outlier_arguments, check_ransac_arguments, fgr_kwargs,
+                   fgr_refine, icp_refine, ransac_kwargs, ransac_refine, remove_outliers)
 
 
 def parser() -> argparse.ArgumentParser:
@@ -72,6 +76,7 @@ def parser() -> argparse.ArgumentParser:
     ap.add_argument('--preference_loop_closure', type=float, default=1.0, help='Line-process preference')
     ap.add_argument('--voxel', type=float, metavar='V', help='Write scene.ply, grid-subsampled at V')
     ap.add_argument('--batch_pairs', type=int, default=8, help='Pairs per forward')
+    add_outlier_arguments(ap)
     return ap
 
 
@@ -200,9 +205,10 @@ def write_outputs(res: Dict, out_dir: str, scene: str, fragments: Sequence[np.nd
     from .eval import EstLogWriter
     from .pointio import write_ply
     os.makedirs(out_dir, exist_ok=True)
-    np.savez(os.path.join(out_dir, 'result.npz'),
-             **{k: res[k] for k in ('poses', 'edges', 'transformation', 'information', 'uncertain', 'confidence',
-                                    'kept', 'pairs', 'fit')})
+    keys = ('poses', 'edges', 'transformation', 'information', 'uncertain', 'confidence', 'kept', 'pairs', 'fit')
+    if 'point_index' in res:
+        keys += ('point_index', 'point_offsets')
+    np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
     log = os.path.join(out_dir, scene, 'est.log')
     if os.path.exists(log):
         os.remove(log)
@@ -229,6 +235,7 @@ def main(argv=None):
     check_fgr_arguments(ap, opt)
     check_icp_arguments(ap, opt, colors=True)
     check_ransac_arguments(ap, opt)
+    check_outlier_arguments(ap, opt)
     from .config import load_config
     from .eval import load_icp_colors
     from .pointio import load_point_cloud
@@ -242,6 +249,9 @@ def main(argv=None):
     cfg = load_config(str(cfg_file))
     model = load_model(cfg, opt.ckpt)
     raw = [np.asarray(load_point_cloud(f), dtype=np.float64) for f in opt.fragments]
+    index = None
+    if opt.remove_statistical_outlier is not None or opt.remove_radius_outlier is not None:
+        raw, colors, index = remove_outliers(raw, colors, opt.remove_statistical_outlier, opt.remove_radius_outlier)
     frags = [crop(cfg, x) for x in raw]
     if colors is not None:
         colors = [crop_colors(cfg, x, c) for x, c in zip(raw, colors)]
@@ -252,6 +262,9 @@ def main(argv=None):
                        opt.icp_lambda_geometric, opt.icp_voxels, opt.icp_radii, opt.icp_level_iters)
     D = float(cfg['overlap_radius'] if opt.info_radius is None else opt.info_radius)
     res = optimize_scene(frags, T, D, opt.min_overlap, opt.preference_loop_closure)
+    if index is not None:
+        res['point_index'] = np.concatenate(index)
+        res['point_offsets'] = np.concatenate([[0], np.cumsum([ix.shape[0] for ix in index])]).astype(np.int64)
     write_outputs(res, opt.out, scene_name(opt.fragments[0]), frags, opt.voxel)
     r = res['result']
     line = {'n_fragments': len(frags), 'pairs': int(len(res['pairs'])), 'edges_odometry': res['n_odometry'],

@@ -1572,6 +1572,170 @@ def voxel_down_sample(clouds, voxel: float, colors=None, status=None):
     return _split(out, counts), None if out_rgb is None else _split(out_rgb, counts)
 
 
+OUTLIER_MAX_NEIGHBORS = 64
+
+
+def statistical_outlier_launches() -> int:
+    """Kernel launches of `regtr_statistical_outlier`: the fp32 copy, the cell list (4), the kNN averages, the chunk
+    offsets, two chunk sums and two per-cloud steps, the keep flags."""
+    return 12
+
+
+def radius_outlier_launches() -> int:
+    """Kernel launches of `regtr_radius_outlier`: the fp32 copy, the cell list (4), the counts."""
+    return 6
+
+
+def select_points_launches() -> int:
+    """Kernel launches of `regtr_select_points`: the flags, the scan, the scatter."""
+    return 3
+
+
+def knn_cell(xyz, n_max: int, k: int) -> float:
+    """Cell size of the kNN search's cell list for stacked float64 clouds `xyz` (the largest with n_max points): about
+    the k-th neighbour distance of a surface scan spread over the clouds' extent L, L / sqrt(n_max) * sqrt(k / pi),
+    and never below max |coordinate| / 32000, so that every cell index fits the cell list's key.  The search's result
+    does not depend on it (include/regtr_b200.h).  One host read."""
+    if xyz.shape[0] == 0 or n_max == 0:
+        return 1.0
+    m, ext = torch.stack([xyz.abs().amax(), (xyz.amax(0) - xyz.amin(0)).amax()]).tolist()
+    if not (math.isfinite(m) and m <= 1e30):
+        return 1.0                             # the device raises REGTR_STATUS_RANGE
+    cell = ext / math.sqrt(n_max) * math.sqrt(k / math.pi)
+    return _knn_cell_floor(m, cell)
+
+
+def _knn_cell_floor(m: float, cell: float) -> float:
+    return float(np.float32(max(cell, m / 32000.0 * 1.001, 1e-30)))
+
+
+def _outlier_inputs(what, clouds, colors):
+    C = len(clouds)
+    if not 1 <= C <= 32767 or (colors is not None and len(colors) != C):
+        raise ValueError(f'{what}: {C} clouds and {None if colors is None else len(colors)} colour arrays; expected '
+                         f'1..32767 clouds, and as many colour arrays when given')
+    ts = [torch.as_tensor(c) for c in clouds]
+    cs = None if colors is None else [torch.as_tensor(c) for c in colors]
+    for b, c in enumerate(ts):
+        if c.dim() != 2 or c.shape[1] != 3 or (cs is not None and tuple(cs[b].shape) != tuple(c.shape)):
+            raise ValueError(f'{what}: cloud {tuple(c.shape)} and colors {None if cs is None else tuple(cs[b].shape)}, '
+                             f'expected (n,3) arrays')
+    dev = next((c.device for c in ts + (cs or []) if c.is_cuda), torch.device('cuda', torch.cuda.current_device()))
+    xyz, lens = _stack_clouds(ts, dev, 3, what)
+    rgb = None if cs is None else _stack_clouds(cs, dev, 3, what)[0]
+    return C, dev, xyz, rgb, lens
+
+
+def _select_points(xyz, rgb, keep, offs, C, n, dev):
+    """regtr_select_points -> (kept clouds, kept colours or None, in-cloud indices), lists of C device tensors."""
+    L = _lib.load()
+    rows = max(n, 1)
+    out = torch.empty((rows, 3), dtype=torch.float64, device=dev)
+    out_rgb = None if rgb is None else torch.empty((rows, 3), dtype=torch.float64, device=dev)
+    index = torch.empty(rows, dtype=torch.int32, device=dev)
+    out_offs = torch.empty(C + 1, dtype=torch.int32, device=dev)
+    ws = workspace(L.regtr_select_points_ws_bytes(n), dev)
+    state = workspace(L.regtr_select_points_state_bytes(n), dev, 'scan_state', zero=True)
+    _lib.check(L.regtr_select_points(_p(xyz), _p(rgb), _p(keep), _p(offs), C, n, _p(out), _p(out_rgb), _p(index),
+                                     _p(out_offs), _p(ws), ws.numel(), _p(state), state.numel(), _stream()),
+               'regtr_select_points')
+    _count(select_points_launches())
+    counts = np.diff(out_offs.cpu().numpy())
+    return _split(out, counts), None if out_rgb is None else _split(out_rgb, counts), _split(index, counts)
+
+
+def _outlier_status(status, own, what):
+    if own:
+        word = int(status.item())
+        if word & (STATUS_RANGE | STATUS_KEY_RANGE):
+            raise _lib.RegtrLibError(f'{what}: a coordinate beyond the search range or not finite (status {word:#x})')
+
+
+def remove_statistical_outlier(clouds, nb_neighbors: int, std_ratio: float, colors=None, status=None,
+                               return_details: bool = False, knn_cell_size=None):
+    """Open3D's remove_statistical_outlier(nb_neighbors, std_ratio) for C clouds in one call
+    (regtr_statistical_outlier, then regtr_select_points): a point is kept when the mean distance to its nb_neighbors
+    nearest neighbours (itself included) is positive and below cloud_mean + std_ratio * std_dev of its cloud.  The
+    exact rules and summation order are in include/regtr_b200.h.
+    clouds / colors: C (n,3) arrays (numpy or torch, any float dtype; stacked in float64 on the device), colours
+    selected with their points.  knn_cell_size: the kNN cell list's cell (default `knn_cell`); the result is the same
+    for any cell, which is raised to max |coordinate| / 32000 when smaller.
+    -> (kept clouds, kept colours or None, kept indices): lists of C device tensors, (m,3) float64 and (m,) int32
+    indices into each input cloud, ascending.  With return_details also a dict: 'avg' (list of C (n,) float64),
+    'keep' (list of C (n,) int32) and 'stats' ((C,3) float64: cloud_mean, std_dev, threshold).
+    The kept row counts are read to split the output.  With status=None a coordinate above 1e30 or not finite raises
+    RegtrLibError; with the caller's word REGTR_STATUS_RANGE is OR-ed into it and nothing is raised.
+    Departure from Open3D: nb_neighbors is at most 64."""
+    what = 'remove_statistical_outlier'
+    k, s = int(nb_neighbors), float(std_ratio)
+    if not (1 <= k <= OUTLIER_MAX_NEIGHBORS and s > 0.0 and math.isfinite(s)):
+        raise ValueError(f'{what}: nb_neighbors {nb_neighbors} must be in 1..{OUTLIER_MAX_NEIGHBORS} and std_ratio '
+                         f'{std_ratio} finite and > 0')
+    if knn_cell_size is not None and not (float(knn_cell_size) > 0.0 and math.isfinite(float(knn_cell_size))):
+        raise ValueError(f'{what}: knn_cell_size {knn_cell_size} must be finite and > 0')
+    C, dev, xyz, rgb, lens = _outlier_inputs(what, clouds, colors)
+    n = sum(lens)
+    if knn_cell_size is None:
+        cell = knn_cell(xyz[:n], max(lens), k)
+    else:
+        m = float(xyz[:n].abs().amax()) if n else 0.0
+        cell = _knn_cell_floor(m if math.isfinite(m) and m <= 1e30 else 0.0, float(knn_cell_size))
+    L = _lib.load()
+    offs = make_offsets(lens, dev)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    avg = torch.empty(max(n, 1), dtype=torch.float64, device=dev)
+    keep = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    stats = torch.empty((C, 3), dtype=torch.float64, device=dev)
+    ws = workspace(L.regtr_outlier_ws_bytes(n, C), dev)
+    state = workspace(L.regtr_outlier_state_bytes(n), dev, 'scan_state', zero=True)
+    _lib.check(L.regtr_statistical_outlier(_p(xyz), _p(offs), C, n, k, s, cell, _p(avg), _p(keep), _p(stats),
+                                           _p(status), _p(ws), ws.numel(), _p(state), state.numel(), _stream()),
+               'regtr_statistical_outlier')
+    _count(statistical_outlier_launches())
+    _outlier_status(status, own, what)
+    out = _select_points(xyz, rgb, keep, offs, C, n, dev)
+    if return_details:
+        return out + ({'avg': _split(avg, lens), 'keep': _split(keep, lens), 'stats': stats},)
+    return out
+
+
+def remove_radius_outlier(clouds, nb_points: int, radius: float, colors=None, status=None,
+                          return_details: bool = False):
+    """Open3D's remove_radius_outlier(nb_points, radius) for C clouds in one call (regtr_radius_outlier, then
+    regtr_select_points): a point is kept when at least nb_points points of its own cloud, itself included, lie
+    strictly within `radius` (float64 d^2 < radius^2).  clouds / colors as in `remove_statistical_outlier`.
+    -> (kept clouds, kept colours or None, kept indices) as there; with return_details also a dict: 'counts' (list of
+    C (n,) int32 full neighbour counts) and 'keep' (list of C (n,) int32).  With status=None a coordinate beyond
+    `overlap_coord_bound(radius)`, or not finite, raises RegtrLibError; with the caller's word REGTR_STATUS_RANGE is
+    OR-ed into it and nothing is raised."""
+    what = 'remove_radius_outlier'
+    k, r = int(nb_points), float(radius)
+    if not (k >= 1 and r > 0.0 and math.isfinite(r)):
+        raise ValueError(f'{what}: nb_points {nb_points} must be >= 1 and radius {radius} finite and > 0')
+    C, dev, xyz, rgb, lens = _outlier_inputs(what, clouds, colors)
+    n = sum(lens)
+    L = _lib.load()
+    offs = make_offsets(lens, dev)
+    own = status is None
+    if own:
+        status = new_status(dev)
+    counts = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    keep = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    ws = workspace(L.regtr_outlier_ws_bytes(n, C), dev)
+    state = workspace(L.regtr_outlier_state_bytes(n), dev, 'scan_state', zero=True)
+    _lib.check(L.regtr_radius_outlier(_p(xyz), _p(offs), C, n, k, r, overlap_cell(r), _p(counts), _p(keep),
+                                      _p(status), _p(ws), ws.numel(), _p(state), state.numel(), _stream()),
+               'regtr_radius_outlier')
+    _count(radius_outlier_launches())
+    _outlier_status(status, own, what)
+    out = _select_points(xyz, rgb, keep, offs, C, n, dev)
+    if return_details:
+        return out + ({'counts': _split(counts, lens), 'keep': _split(keep, lens)},)
+    return out
+
+
 NORMALS_MAX_NN = 64
 
 

@@ -12,6 +12,7 @@
          [--fgr_max_tuples 1000]] [--fgr_no_decrease_mu] [--fgr_absolute_scale] [--fgr_overlap 0.5] [--fgr_seed 0]]
     python -m regtr_b200.register SRC TGT --fpfh V [--fpfh_radius FR] [--fpfh_max_nn 100] [--fpfh_no_mutual]
         [--ransac R ... | --fgr [--fgr_dist D] [--fgr_no_tuple_test] ...] [--icp R ...] [--fit_radius R] [--out DIR]
+    either form also takes [--remove_statistical_outlier K S] [--remove_radius_outlier N R]
 
 SRC / TGT: .ply, .pth, .bin or .npy (regtr_b200.pointio).  The config is the config.yaml one level above the
 checkpoint's directory, the layout `python -m regtr_b200.train` writes, unless --config names another.  Instead of the
@@ -68,6 +69,12 @@ refines the pose on the full clouds as above, and fit is taken at --fit_radius (
 Written: pose.txt, src_registered.ply and result.npz with pose_fpfh (3,4) float64, ransac (5,), n_mutual, fit and,
 with --icp, pose_icp and icp; no keypoint files.  The JSON line has the pose, the fit numbers, the point counts,
 fpfh_voxel, n_src_down, n_tgt_down, n_mutual and the ransac_* (and icp_*) entries.
+With --remove_statistical_outlier K S and / or --remove_radius_outlier N R, both clouds are first filtered as read
+from the files, before the config's crop (`eval.remove_outliers`: Open3D's remove_statistical_outlier(K, S), then
+remove_radius_outlier(N, R) on what is left, with the colours read for colored ICP filtered alike), which equals
+reading the files in Open3D, filtering, saving and registering the saved clouds.  result.npz then gains src_index and
+tgt_index (the surviving rows of each file) and the JSON line n_src_read, n_tgt_read, n_src_filtered and
+n_tgt_filtered, on both paths.
 With --fpfh V --fgr the mutual FPFH matches go to FGR instead (`ops.fgr_feature_matching`, the tuple test on unless
 --fgr_no_tuple_test, --fgr_dist defaulting to 0.5 V as in Open3D's tutorial); --fpfh_no_mutual is then a usage error,
 and fit is taken at --fit_radius (default 1.5 V).  result.npz holds pose_fpfh (the FGR pose) and fgr (4,) in place of
@@ -84,10 +91,10 @@ from typing import Dict
 import numpy as np
 import torch
 
-from .eval import (add_fgr_arguments, add_fpfh_arguments, add_icp_arguments, add_ransac_arguments,
-                   check_fgr_arguments, check_fpfh_arguments, check_icp_arguments, check_ransac_arguments, fgr_kwargs,
-                   fgr_refine, fpfh_kwargs, fpfh_register, icp_kwargs, icp_levels, icp_refine, ransac_kwargs,
-                   ransac_refine)
+from .eval import (add_fgr_arguments, add_fpfh_arguments, add_icp_arguments, add_outlier_arguments,
+                   add_ransac_arguments, check_fgr_arguments, check_fpfh_arguments, check_icp_arguments,
+                   check_outlier_arguments, check_ransac_arguments, fgr_kwargs, fgr_refine, fpfh_kwargs, fpfh_register,
+                   icp_kwargs, icp_levels, icp_refine, ransac_kwargs, ransac_refine, remove_outliers)
 
 
 def parser() -> argparse.ArgumentParser:
@@ -108,6 +115,7 @@ def parser() -> argparse.ArgumentParser:
     add_fgr_arguments(ap, 'Replace the pose by Fast Global Registration over the predicted correspondences (with '
                           '--fpfh: over the FPFH matches) instead of RANSAC; before ICP with --icp')
     add_fpfh_arguments(ap)
+    add_outlier_arguments(ap)
     ap.add_argument('--out', default='.', help='Output directory')
     return ap
 
@@ -120,6 +128,7 @@ def parse_args(argv=None):
     check_fpfh_arguments(ap, opt)
     check_icp_arguments(ap, opt, colors=True)
     check_ransac_arguments(ap, opt)
+    check_outlier_arguments(ap, opt)
     if opt.fpfh is not None and opt.fit_radius is None:
         opt.fit_radius = 1.5 * opt.fpfh if opt.fgr else opt.ransac
     return opt
@@ -276,7 +285,8 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
     write_ply(os.path.join(out_dir, 'src_registered.ply'), res['src_xyz'] @ p[:, :3].T + p[:, 3])
     if 'pose_fpfh' in res:
         keys = ('pose_fpfh', 'fgr' if 'fgr' in res else 'ransac', 'n_mutual', 'fit') + \
-            (('pose_icp', 'icp') if 'pose_icp' in res else ()) + (('icp_levels',) if 'icp_levels' in res else ())
+            (('pose_icp', 'icp') if 'pose_icp' in res else ()) + (('icp_levels',) if 'icp_levels' in res else ()) + \
+            (('src_index', 'tgt_index') if 'src_index' in res else ())
         np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
         return 0
     keys = ('pose', 'src_kp', 'src_kp_warped', 'src_overlap', 'tgt_kp', 'tgt_kp_warped', 'tgt_overlap', 'fit')
@@ -290,6 +300,8 @@ def write_outputs(res: Dict, out_dir: str, threshold: float = 0.5):
         keys += ('pose_icp', 'icp')
     if 'icp_levels' in res:
         keys += ('icp_levels',)
+    if 'src_index' in res:
+        keys += ('src_index', 'tgt_index')
     np.savez(os.path.join(out_dir, 'result.npz'), **{k: res[k] for k in keys})
     m = res['src_overlap'] > threshold
     write_ply(os.path.join(out_dir, 'src_kp.ply'), res['src_kp'][m], {'overlap': res['src_overlap'][m]})
@@ -303,18 +315,20 @@ def main(argv=None):
     from .pointio import load_point_cloud
     colors = load_icp_colors(parser(), opt, [opt.src, opt.tgt])
     if opt.fpfh is not None:
-        return main_fpfh(opt, load_point_cloud(opt.src), load_point_cloud(opt.tgt), colors)
+        return main_fpfh(opt, *read_clouds(opt, load_point_cloud(opt.src), load_point_cloud(opt.tgt), colors))
     from .config import load_config
     cfg_file = config_path(opt.ckpt, opt.config)
     if not cfg_file.exists():
         raise SystemExit(f'config not found: {cfg_file} (pass --config)')
     cfg = load_config(str(cfg_file))
     model = load_model(cfg, opt.ckpt)
-    res = register(model, cfg, load_point_cloud(opt.src), load_point_cloud(opt.tgt), opt.fit_radius, opt.icp,
+    src_xyz, tgt_xyz, colors, filtered = read_clouds(opt, load_point_cloud(opt.src), load_point_cloud(opt.tgt), colors)
+    res = register(model, cfg, src_xyz, tgt_xyz, opt.fit_radius, opt.icp,
                    opt.icp_iters, opt.icp_method, opt.normal_radius, opt.normal_max_nn, opt.icp_epsilon,
                    opt.icp_loss, opt.icp_loss_k, opt.ransac, ransac_kwargs(opt) if opt.ransac is not None else None,
                    dict(fgr_kwargs(opt), overlap=opt.fgr_overlap) if opt.fgr else None, colors,
                    opt.icp_lambda_geometric, opt.icp_voxels, opt.icp_radii, opt.icp_level_iters)
+    n_outlier = outlier_line(res, filtered)
     n_shown = write_outputs(res, opt.out, opt.threshold)
     f = [float(v) for v in res['fit']]
     line = {'pose': pose44(final_pose(res)).tolist(),
@@ -331,8 +345,33 @@ def main(argv=None):
                     ransac_validations=int(rs[3]), ransac_radius=float(opt.ransac))
     if opt.fgr:
         line.update(fgr_line(opt, res['fgr']))
+    line.update(n_outlier)
     print(json.dumps(line))
     return res
+
+
+def read_clouds(opt, src_xyz, tgt_xyz, colors):
+    """The clouds as read, filtered by the outlier flags when given (`eval.remove_outliers`, colours alike).
+    -> (src_xyz, tgt_xyz, colors, filtered): filtered None without the flags, else ((n_src_read, n_tgt_read),
+    [src_index, tgt_index])."""
+    if opt.remove_statistical_outlier is None and opt.remove_radius_outlier is None:
+        return src_xyz, tgt_xyz, colors, None
+    read = (int(src_xyz.shape[0]), int(tgt_xyz.shape[0]))
+    (src_xyz, tgt_xyz), colors, index = remove_outliers([src_xyz, tgt_xyz], colors, opt.remove_statistical_outlier,
+                                                        opt.remove_radius_outlier)
+    return src_xyz, tgt_xyz, colors, (read, index)
+
+
+def outlier_line(res: Dict, filtered) -> Dict:
+    """With the outlier flags (filtered = ((n_src_read, n_tgt_read), [src_index, tgt_index])): the surviving rows of
+    each file into `register`'s dict as src_index / tgt_index, and -> the JSON line's point counts before and after
+    the filters; else {}."""
+    if filtered is None:
+        return {}
+    read, index = filtered
+    res['src_index'], res['tgt_index'] = index
+    return {'n_src_read': read[0], 'n_tgt_read': read[1], 'n_src_filtered': int(index[0].shape[0]),
+            'n_tgt_filtered': int(index[1].shape[0])}
 
 
 def fgr_line(opt, fgr) -> Dict:
@@ -361,12 +400,14 @@ def icp_line(opt, res: Dict) -> Dict:
     return line
 
 
-def main_fpfh(opt, src_xyz, tgt_xyz, colors=None):
-    """`main` with --fpfh: `register_fpfh`, its files and its JSON line (colors: the files' rgb for colored ICP)."""
+def main_fpfh(opt, src_xyz, tgt_xyz, colors=None, filtered=None):
+    """`main` with --fpfh: `register_fpfh`, its files and its JSON line (colors: the files' rgb for colored ICP;
+    filtered: what the outlier filters kept, as `outlier_line` takes it)."""
     icp_options = None
     if opt.icp is not None:
         icp_options = dict(icp_kwargs(opt), **({} if colors is None else {'colors': ([colors[0]], [colors[1]])}))
     res = register_fpfh(src_xyz, tgt_xyz, opt.fpfh, opt.fit_radius, opt.icp, icp_options, fpfh_kwargs(opt))
+    n_outlier = outlier_line(res, filtered)
     write_outputs(res, opt.out)
     f = [float(v) for v in res['fit']]
     line = {'pose': pose44(final_pose(res)).tolist(), 'fitness_src': f[0], 'rmse_src': f[1], 'fitness_tgt': f[2],
@@ -381,6 +422,7 @@ def main_fpfh(opt, src_xyz, tgt_xyz, colors=None):
                     ransac_validations=int(rs[3]), ransac_radius=float(opt.ransac))
     if opt.icp is not None:
         line.update(icp_line(opt, res))
+    line.update(n_outlier)
     print(json.dumps(line))
     return res
 
