@@ -707,8 +707,14 @@ int regtr_kpconv_aggregate(const float* q, const float* s, const int32_t* idx, c
         REGTR_CHECK_LAUNCH();
     }
     if (Cin <= 16) {
-        const size_t smem = agg_smem_bytes(K);
-        if (smem > 48 * 1024) return REGTR_ERR_UNSUPPORTED;
+        const size_t smem = agg_smem_bytes(K);      // 84 KB at K = 128: above K = 73 it needs the opt-in
+        static size_t attr_smem = 0;
+        if (smem > 48 * 1024 && smem > attr_smem) {
+            if (cudaFuncSetAttribute(k_kpconv_agg_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
+                cudaSuccess)
+                return REGTR_ERR_UNSUPPORTED;
+            attr_smem = smem;
+        }
         k_kpconv_agg_small<<<regtr_cdiv(Nq, AGG_WARPS), AGG_WARPS * 32, smem, st>>>(q, s, idx, x, rowflag_ws, kp, Nq,
                                                                                    Ns, nq_dev, ns_dev, K, Cin, extent, wf);
         REGTR_CHECK_LAUNCH();

@@ -274,12 +274,18 @@ def kpconv_aggregate(q_pts, s_pts, idx32, x, kernel_points, extent: float, wf=No
     return wf
 
 
+MAX_POOL_BWD_K = 255       # regtr_max_pool_bwd's limit (uint8 winner slot)
+
+
 def max_pool(x, idx32, ns_dev=None):
     """max over the K gathered rows with a zero shadow row.  Differentiable (_MaxPoolFn) when grad mode is on and x
     requires grad (exact shapes only)."""
     if _wants_grad(x):
         if ns_dev is not None:
             raise ValueError('max_pool: the backward needs exact shapes (no ns_dev)')
+        if idx32.shape[1] > MAX_POOL_BWD_K:          # the backward keeps each winner's slot in one byte
+            raise ValueError(f'max_pool: the backward takes at most {MAX_POOL_BWD_K} neighbours per query, got '
+                             f'{idx32.shape[1]}')
         return _MaxPoolFn.apply(x, idx32)
     return _max_pool_fwd(x, idx32, ns_dev)
 
